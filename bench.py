@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""bench.py — events/sec aggregated by the B200 streaming-sketch engine (BASELINE.json metric).
+"""bench.py — events/sec aggregated by the H100 streaming-sketch engine (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # product arm
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path on this box's host cores
+    python bench.py ... --dump-outputs DIR                   # also write what the last timed step left in the engine, DIR/*.npy
 
 One STEP = one pass of the hot path over one batch of synthetic events: ingest_kernel (count-min / HLL / process histograms; a
 response sample of a hot service updates its dense row of value bins, any other becomes a sort key), 4 one-sweep radix passes,
 runs_mark / runs_sum (per-(service, bin) counts and sums of the keys), bins_merge (histogram cells + t-digest merge from rows and runs). N > 1 adds ONE sketch merge (gysk_merge_global: fold + one NCCL group + merge-compress) per timed
 window, as a deployment merges once per query window. Workload = BASELINE.json configs[2] ("100 M mixed TCP/syscall events,
-100 K services, t-digest p50/p95/p99 on 1xB200"), the largest single-GPU configuration: per rank EVENTS_PER_STEP
+100 K services, t-digest p50/p95/p99 on one GPU"), the largest single-GPU configuration: per rank EVENTS_PER_STEP
 events of the 70/20/10 RESP/TCP/TASK mix over 100 K services (weak scaling: each rank ingests its own host shard).
 
 `value`  : whole-job events/s with the batch already resident in HBM (device timed, CUDA events, max over ranks).
@@ -17,7 +18,7 @@ events of the 70/20/10 RESP/TCP/TASK mix over 100 K services (weak scaling: each
            (18.4 B/event); `e2e_event32` = 32-byte canonical records; `e2e_wire` = 16 host threads calling gysk_ingest_msg /
            gysk_ingest_raw with TCP_CONN_NOTIFY / AGGR_TASK_STATE_NOTIFY messages and raw tcp_ipv4_resp_event_t arrays.
 `roofline`: dominant kernel, algorithmic bytes (SURVEY.md §8d; 54.8 B/event + 32 B per event that took the hot-row way, `hot_rows`)
-           / CUDA-event time, against MEASURED_PEAKS.json.
+           / CUDA-event time, against MEASURED_PEAKS.json when present, else the H100 SXM data-sheet HBM3 bandwidth.
 `cpu_baseline`: the CPU oracle port (all host cores, events pre-sharded by host) on a bounded sample of the same stream.
 """
 import argparse
@@ -64,6 +65,7 @@ def parse():
     ap.add_argument("--cpu-sample", type=int, default=20_000_000)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step left in the engine as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -236,6 +238,40 @@ def wire_leg(ge, local, nthreads=16, rounds_per_thread=8, total_events=32_000_00
 
 
 # ---------------------------------------------------------------------------------------------------------------
+# outputs of the timed path, for comparing two builds
+# ---------------------------------------------------------------------------------------------------------------
+DUMP_SVCS = 4096
+DUMP_CMS_CELLS = 1 << 20
+
+
+def dump_outputs(out_dir, eng, rank):
+    """what a caller reads back after the last timed step, as float64 arrays: the per-service summaries (gysk_query_svcs, every
+    field but the id) and current-window response histograms of a fixed, seeded sample of the rank's services, the engine's
+    counters and a fixed, seeded sample of the count-min cells split into {count, kbytes}. About 19 MB. Counts and sums are below
+    2^53 and exact; sentinels such as INT64_MAX round to the nearest float64."""
+    from gyeeta_b200 import engine as ge
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(20261015)
+    ids = np.sort(rng.choice(rank_service_ids(rank), DUMP_SVCS, replace=False))
+    fields = [f for f, _ in ge.SvcSummary._fields_ if f != "glob_id"]
+    summ = eng.query_svcs(ids)
+    hist = np.full((len(ids), 32), np.nan)
+    for i, id_ in enumerate(ids):
+        h = eng.export_hist(int(id_), ge.HIST_RESP_CUR)
+        if h is not None:
+            hist[i] = np.concatenate([h[0]["count"], h[0]["sum"], [h[1], h[2]]])
+    cms = eng.export_cms()
+    cells = np.sort(rng.choice(len(cms), DUMP_CMS_CELLS, replace=False))
+    st = eng.stats()
+    out = {"svc_summary": np.array([[float(s[f]) for f in fields] for s in summ]),
+           "resp_hist_cur": hist,
+           "cms_sample": np.stack([(cms[cells] & np.uint64(0xFFFFFFFF)).astype(np.float64), (cms[cells] >> np.uint64(32)).astype(np.float64)], axis=1),
+           "stats": np.array([float(st[k]) for k in sorted(st)])}
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64))
+
+
+# ---------------------------------------------------------------------------------------------------------------
 # clocks
 # ---------------------------------------------------------------------------------------------------------------
 class ClockSampler:
@@ -288,15 +324,6 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "samples_inside_timed_region": len(inside)}
 
 
-def ncu_traffic_per_event():
-    """DRAM bytes per event of each kernel group from the committed `ncu --set full` captures (profiles/ncu_traffic.json)"""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return {}
-
-
 def measured_peak_gbs():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -304,7 +331,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -533,6 +560,8 @@ def main():
     dev_ms = t0.elapsed_time(t1)
     launches = eng.stats()["kernel_launches"] - launches0           # kernels of libgysketch.so launched inside the timed region
     ms_ing, ms_td, nb = eng.profile_read()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, rank)        # the state the last timed step left, before anything else is ingested
     # share of the events that took the hot-row way (two REDs into the service's dense value bins inside ingest_kernel instead of a
     # sort key): read from the engine after the timed region — response samples of the last batch minus its sort keys
     resp0 = eng.stats()["events_resp"]
@@ -657,21 +686,18 @@ def main():
     peak, peak_src = measured_peak_gbs()
     nev_total = n * args.steps
     roof = []
-    traffic = ncu_traffic_per_event()
     # a hot response sample's histogram-cell read-modify-write (32 of its 98 B, SURVEY.md §8d) happens in ingest_kernel — the two
     # 64-bit REDs into its value bin — not in the chain: those bytes move from one kernel group to the other, the sum stays 101 B
     moved = 32.0 * hot_share
-    for name, key, ms, bpe in (("ingest_kernel", "ingest_kernel", ms_ing, BYTES_INGEST + moved),
-                               ("sort + runs + bins-merge chain (os_pass x4, runs_mark, runs_sum, bins_merge)" + (" with side_drain_kernel beside it" if SIDE_DRAIN else ""), "chain", ms_td, BYTES_TDIGEST - moved)):
+    for name, ms, bpe in (("ingest_kernel", ms_ing, BYTES_INGEST + moved),
+                          ("sort + runs + bins-merge chain (os_pass x4, runs_mark, runs_sum, bins_merge)" + (" with side_drain_kernel beside it" if SIDE_DRAIN else ""), ms_td, BYTES_TDIGEST - moved)):
         if ms > 0:
             ach = nev_total * bpe / (ms * 1e-3) / 1e9
-            tr = traffic.get(key, {}).get("dram_bytes_per_event")
             roof.append({"kernel": name, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                         "traffic": (tr * n if tr else None), "traffic_note": traffic.get(key, {}).get("source"),
                          "algorithmic_bytes_per_launch": bpe * n, "ms_per_launch": ms / max(nb, 1),
                          "ms_total": ms, "launch_groups": nb, "algorithmic_bytes_per_event": bpe, "peak_source": peak_src})
     # `roofline` = the dominant SINGLE kernel: ingest_kernel is one launch per device batch and holds the largest share of any
-    # individual kernel (profiles/r02_launches_*.csv); the chain is 7 launches of 4 kernels
+    # individual kernel; the chain is 7 launches of 4 kernels
     roof.sort(key=lambda r: 0 if r["kernel"] == "ingest_kernel" else 1)
     whole = nev_total * BYTES_EVENT / (max_ms * 1e-3) / 1e9
 

@@ -1,4 +1,4 @@
-"""Builds gyeeta_b200/libgysketch.so (in-tree, so it travels to the GPU box) with nvcc for sm_100a only, and libgysynth.so, the
+"""Builds gyeeta_b200/libgysketch.so (in-tree, next to the package) with nvcc for sm_90a only, and libgysynth.so, the
 on-device synthetic event source the sustained-stream run uses (a bench utility, not linked into the product library)."""
 import os
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgysketch.so")
 SYNTH_LIB = os.path.join(HERE, "libgysynth.so")
 SOURCES = ["gysk_kernels.cu", "gysk_engine.cu", "gysk_merge.cu", "gysk_groupby.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function", "-Xptxas", "-v"]
 
 
@@ -42,7 +42,7 @@ def build(force=False, verbose=False):
         if r.returncode:
             raise RuntimeError("nvcc failed for " + src)
         objs.append(obj)
-    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC"]
+    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode:
         sys.stderr.write(r.stdout + r.stderr)

@@ -1,4 +1,4 @@
-// gysk_device.cuh — device-side building blocks shared by the kernels of libgysketch.so (sm_100a only).
+// gysk_device.cuh — device-side building blocks shared by the kernels of libgysketch.so (sm_90a only).
 //
 // Everything here is a from-scratch CUDA formulation of behaviour defined by the reference (citations are
 // relative to the reference tree) or by the sketch definitions stated in DESIGN.md.
@@ -41,7 +41,7 @@ static constexpr unsigned long long BIN_CNT_MASK = (1ull << BIN_CNT_BITS) - 1;
 // A hot service's row: HOT_ROW_BINS words {samples | remainders} followed by HOT_ROW_BINS words of usec sums (the two REDs of a
 // sample go to different lines), bin b at word hot_word(b) — the 32 x 32 transpose of the index, so that neighbouring bins, which
 // fill up together around the mode of a service's response times, lie two 128-byte lines apart: same-line atomics are serialised
-// in L2 and the fullest line of the busiest service is what the ingest kernel ends up waiting for (profiles/r02_hot_rows_ab.json).
+// in L2 and the fullest line of the busiest service is what the ingest kernel ends up waiting for.
 static constexpr int HOT_ROW_BINS = 1024, HOT_ROW_WORDS = 2 * HOT_ROW_BINS;
 static_assert(NBINS <= HOT_ROW_BINS, "a row holds every bin");
 __host__ __device__ __forceinline__ uint32_t hot_word(uint32_t bin) { return ((bin & 31u) << 5) | (bin >> 5); }

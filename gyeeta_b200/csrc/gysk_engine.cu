@@ -495,7 +495,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 
 	cudaDeviceProp prop;
 	if ((ce = cudaGetDeviceProperties(&prop, cfg.device)) != cudaSuccess) return fail(nullptr, GYSK_ERR_NODEV, "cudaGetDeviceProperties", ce);
-	if (prop.major != 10) return fail(nullptr, GYSK_ERR_NODEV, "device is not sm_100 (kernels are built for sm_100a only)");
+	if (prop.major != 9 || prop.minor != 0) return fail(nullptr, GYSK_ERR_NODEV, "device is not sm_90 (kernels are built for sm_90a only)");
 
 	gysk_engine *e = new (std::nothrow) gysk_engine;
 	if (!e) return fail(nullptr, GYSK_ERR_NOMEM, "new gysk_engine");

@@ -1,4 +1,4 @@
-// gysk_kernels.cu — hand-written sm_100a kernels of the streaming-sketch engine.
+// gysk_kernels.cu — hand-written sm_90a kernels of the streaming-sketch engine.
 //
 //   ingest_kernel        one pass over a batch of 32-byte events: id -> slot, then per event type
 //                          RESP : one 64-bit sort key {slot | value bin | usec}; CONN_BITMAP bit, batch min / max when they change
@@ -98,7 +98,7 @@ __device__ __forceinline__ void cell_add_global(const DevState &st, uint32_t cel
 		HistCell *c = st.task_hist + (cell & ~CELL_TASK);
 		red_add_u64(&c->count, cnt); red_add_u64((unsigned long long *)&c->sum, sum);
 		// max_val_seen_ of the histogram: a fire-and-forget RED.MAX — looking first (to skip the atomic) made every process record wait
-		// for an L2 round trip (7.7 % of the kernel's stall samples, profiles/r02_ncu_full_raw_final.csv); the busy processes' cells
+		// for an L2 round trip; the busy processes' cells
 		// live in the CTA's hot table and reach this point once per CTA
 		red_max_s64(&st.task_hist[(cell & ~CELL_TASK) | 15u].sum, (long long)vmax);
 	}
@@ -521,7 +521,7 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState s
 // ---------------------------------------------------------------------------------------------------
 // EXPERIMENT (GYSK_SIDE_DRAIN=1, off by default): the connection and process records ingest_kernel queued, applied next to the sort
 // chain on the engine's side stream. Idea: the radix passes are bound by instruction issue and leave the L2 atomic units idle, the ~85 M
-// REDs of the two drains (ablation: 0.8 + 0.75 ms inside ingest_kernel, profiles/r02_ablation.json) are bound by exactly those units.
+// REDs of the two drains are bound by exactly those units.
 // Outcome: correct (the whole GPU suite passes with it on) but slower, see side_drain_enabled(). Persistent grid; a warp takes 32
 // records at a time; hot cells are privatised per CTA as in ingest_kernel.
 // ---------------------------------------------------------------------------------------------------
@@ -701,7 +701,7 @@ __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned l
 	}
 
 	// Lanes holding the same digit form a group. match.any finds the groups in one instruction, but the hardware walks the
-	// distinct values of the warp one by one (ADU pipe: 73 % busy on a pass whose digits are uniform, ncu r01); one ballot per
+	// distinct values of the warp one by one (the address-divergence unit stays busy on a pass whose digits are uniform); one ballot per
 	// digit bit costs the same whatever the data. The CTA picks per pass: expected number of distinct digits among 32 keys,
 	// from the global histogram of the pass.
 	bool use_ballot;
@@ -1051,7 +1051,7 @@ static constexpr int TD_WARPS = 3;		// warps (= services in flight) per CTA; wor
 // pass cuts the list to at most TD_CAP clusters (warp_merge_compress). Lists of up to 2 x TD_CAP entries work in shared memory;
 // longer ones (a first batch can fill several hundred bins) in the warp's L2-resident scratch — same code, same result.
 // SMEM_N = longest merged list (old centroids + batch items) that works in shared memory: the smaller the work area, the more
-// services a SM has in flight (the kernel is latency-bound: ~2 600 dependent warp instructions per service, ncu profiles/).
+// services a SM has in flight (the kernel is latency-bound: a long chain of dependent warp instructions per service).
 template <int SMEM_N>
 __global__ void __launch_bounds__(TD_WARPS * 32) bins_merge_kernel(DevState st, const uint32_t *__restrict__ touched, const unsigned long long *__restrict__ ntouched_p,
 		const RunRec *__restrict__ pool, const uint16_t *__restrict__ run_bin, const BatchSeg *__restrict__ segs,
@@ -1511,7 +1511,7 @@ static inline uint32_t div_up(uint64_t a, uint64_t b) { return (uint32_t)((a + b
 // cudaFuncSetAttribute is per DEVICE: one process may own an engine on every GPU of the box (INTEGRATION.md §2)
 static constexpr int MAX_DEVICES = 64;
 static int current_device() { int dev = 0; cudaGetDevice(&dev); return dev < 0 || dev >= MAX_DEVICES ? 0 : dev; }
-static int sm_count(int dev) { int nsm = 148; cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev); return nsm; }
+static int sm_count(int dev) { int nsm = 132; cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev); return nsm; }
 
 int launch_init_state(const DevState &st, uint32_t max_svcs, uint32_t max_tasks, cudaStream_t s)
 {
@@ -1535,9 +1535,8 @@ static int ingest_variant()
 }
 
 // the radix passes of the RESP keys sort on {slot | bin} = key bits [30, 40 + slot bits): TD_CODE_BITS + slot bits significant
-// bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible (27 bits -> 7 7 7 6). 8-bit passes run
-// at 0.39-0.49 ms per 70 M keys, a 9-bit pass (two look-back rows per thread, nine ballots per key) at 0.76 ms (profiles/): four
-// of the former beat three of the latter.
+// bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible (27 bits -> 7 7 7 6). A 9-bit pass
+// has two look-back rows per thread and nine ballots per key; GYSK_KEY_DIGIT_MAX=9 selects such digits (one pass fewer) for A/B runs.
 static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
 {
 	int slot_bits = 1;
@@ -1555,9 +1554,9 @@ static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
 }
 
 // GYSK_SIDE_DRAIN=1: the connection / process records are queued by ingest_kernel and applied by side_drain_kernel on a second
-// stream next to the sort chain. Measured and NOT the default (profiles/r02_side_drain_ab.json): ingest_kernel gets 0.4 ms faster,
-// but the block scheduler does not interleave the side kernel with the radix passes (they fill every SM's register file), so its
-// 1.5 - 2.5 ms land behind the chain: 8.1 ms per batch against 6.9 ms with the drains inside ingest_kernel.
+// stream next to the sort chain. NOT the default: ingest_kernel gets faster, but the block scheduler does not interleave the side
+// kernel with the radix passes (they fill every SM's register file), so its work lands behind the chain and the batch takes longer
+// than with the drains inside ingest_kernel.
 bool side_drain_enabled()
 {
 	static const bool on = []{ const char *e = getenv("GYSK_SIDE_DRAIN"); return e && atoi(e) != 0; }();

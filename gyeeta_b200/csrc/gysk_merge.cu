@@ -367,7 +367,7 @@ int gysk_merge_prepare(gysk_engine *e)
 				mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax);
 		fold_hll_kernel<<<div_up((uint64_t)nl << (e->cfg.hll_p - 2), 256), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, nl, null_slot,
 				reinterpret_cast<uint32_t *>(mg.l_hll));
-		fold_td_kernel<<<std::min<uint32_t>(div_up(nl, MG_WARPS), 148 * 8), MG_WARPS * 32, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, nl, null_slot,
+		fold_td_kernel<<<std::min<uint32_t>(div_up(nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, nl, null_slot,
 				reinterpret_cast<SlabEntry *>(mg.slab));
 		e->kernel_launches += 3;
 	}
@@ -412,7 +412,7 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 	const SlabEntry *src = d_gathered ? static_cast<const SlabEntry *>(d_gathered) : reinterpret_cast<const SlabEntry *>(mg.slab);
 	if (!d_gathered) world = 1;
 	if (mg.nlogical) {
-		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.nlogical, MG_WARPS), 148 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.nlogical,
+		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.nlogical, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.nlogical,
 				reinterpret_cast<SlabEntry *>(mg.final_slab), e->st.td);
 		e->kernel_launches++;
 	}

@@ -61,7 +61,7 @@ __device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid 
 		double av = i < na ? am[i] : 0.0, bv = k < nb ? bm[k] : 0.0;
 		// the two-finger walk touches shared memory only: it notes where every output comes from (S.nxt is free until the cell
 		// search) and the weights — which the walk does not need — are fetched afterwards, all loads of a lane in flight together
-		// (a weight load inside the walk put an L2 round trip into every step: 8.7 % of the kernel's stall samples)
+		// (a weight load inside the walk put an L2 round trip into every step)
 		for (uint32_t pos = d0; pos < d1; ++pos) {
 			const bool ta = i < na && (k >= nb || av <= bv);
 			S.mean[pos] = ta ? av : bv;

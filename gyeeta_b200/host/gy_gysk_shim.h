@@ -5,7 +5,7 @@
 //     MCONN_HANDLER::partha_aggr_task_state   server/gy_mconnhdlr.h:2098   (definition gy_mconnhdlr.cc:9959)
 //     MCONN_HANDLER::partha_listener_state    server/gy_mconnhdlr.h:2129   (definition gy_mconnhdlr.cc:10993)
 //     MCONN_HANDLER::handle_partha_active_conns server/gy_mconnhdlr.h:2155 (definition gy_mconnhdlr.cc:7705)
-// and forward the record batch to the B200 engine through the C ABI of include/gysketch.h. The template parameters
+// and forward the record batch to the GPU engine through the C ABI of include/gysketch.h. The template parameters
 // stand for the reference's own types (std::shared_ptr<PARTHA_INFO>, comm::TCP_CONN_NOTIFY, POOL_ALLOC_ARRAY, PGConnPool) so
 // that this header compiles both inside gy_mconnhdlr.cc (with the real types) and stand-alone in this repository's tests (with
 // the POD mirrors of gyeeta_b200/csrc/gysk_wire.h). See INTEGRATION.md for the call-site patch.

@@ -1,5 +1,5 @@
 /*
- * gysketch.h — C ABI of libgysketch.so, the B200-native streaming-sketch aggregation engine that sits
+ * gysketch.h — C ABI of libgysketch.so, the H100-native streaming-sketch aggregation engine that sits
  * behind Gyeeta's madhava ingest path.
  *
  * Every entry point replaces (or is what a cgo/ctypes/C++ shim would bind for) a named piece of the
@@ -30,7 +30,7 @@
  * Conventions: plain pointers and sizes, no exceptions cross the boundary, 0 = ok, negative = -errno style
  * (mirrors the reference handlers' bool/int returns wrapped in GY_CATCH_EXCEPTION, gy_mconnhdlr.cc:4763-4774).
  * CUDA errors are sticky: once a call fails with GYSK_ERR_CUDA every later call fails too; gysk_last_error()
- * returns the text. There is NO CPU fallback: gysk_create() fails when no sm_100 device is usable.
+ * returns the text. There is NO CPU fallback: gysk_create() fails when no sm_90 device is usable.
  */
 #ifndef GYSKETCH_H
 #define GYSKETCH_H

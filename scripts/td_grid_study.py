@@ -1,6 +1,6 @@
 """CPU-only study (numpy restatement of the batched t-digest update of DESIGN.md §2; not used by the product or the tests): how
 far is the digest's p50 / p95 / p99 from the EXACT sample quantile on log-normal streams (sigma 1.2 / 1.5, n = 10 K .. 1 M, 1 or 8
-batches), for the shipped K_1 unit grid and for tail-weighted grids with the same number of cells? Results: profiles/r02_td_grid_study.md.
+batches), for the shipped K_1 unit grid and for tail-weighted grids with the same number of cells?
 
     python scripts/td_grid_study.py
 """

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

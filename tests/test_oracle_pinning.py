@@ -1,12 +1,11 @@
 """Pins the CPU oracle (oracle/gysk_oracle.c) before anything trusts it:
   1. the reference's own asserted fixture, test/test_histogram.cc:29-147 (bucket ids + 4 percentiles);
   2. golden vectors produced by RUNNING the reference here (tests/golden/*.npz, made by make_golden.py);
-  3. live comparison with the compiled reference (oracle/_ref/libgyref.so) on random streams, when present.
+  3. what the compiled reference (oracle/_ref/libgyref.so) returned on seeded random streams (tests/golden/ref_random_golden.npz).
 """
 import os
 
 import numpy as np
-import pytest
 
 from oracle import pyoracle as po
 
@@ -108,13 +107,15 @@ def test_jhash_golden(golden_dir):
     assert [L.gyo_jhash2(po._p(words), n, 0xceedfead) for n in range(13)] == g["hwords"].tolist()
 
 
-# ---- 3. live against the compiled reference ------------------------------------------------------------
-@pytest.mark.skipif(po.ref() is None, reason="oracle/_ref/libgyref.so not built (no reference tree)")
-def test_oracle_vs_compiled_reference_random():
-    R = po.ref()
-    assert R.gyref_sizeof_hist_resp() == 280
+# ---- 3. random streams against the compiled reference's stored answers ----------------------------------
+def test_oracle_vs_compiled_reference_random(golden_dir):
+    """the oracle on seeded random streams of every class, type and scale against what the reference's own code
+    (oracle/_ref/libgyref.so) returned for the same streams, stored by make_golden.py"""
+    import hashlib
+    g = np.load(os.path.join(golden_dir, "ref_random_golden.npz"))
     rng = np.random.default_rng(7)
     pcts = [25, 50, 95, 99, 99.9]
+    i = 0
     for name, cls in po.CLS.items():
         if name.startswith("FD_"):
             continue
@@ -122,12 +123,13 @@ def test_oracle_vs_compiled_reference_random():
             for scale in (50, 5000, 2 ** 20, 2 ** 34):
                 vals = rng.integers(-scale // 10, scale, 5000, dtype=np.int64)
                 a = run(cls, tk, vals, pcts)
-                b = po.hist_run(R, "gyref_hist_run", cls, tk, vals, pcts)
-                for k in ("nb", "total", "max"):
-                    assert a[k] == b[k], (name, tk, scale, k)
-                assert np.array_equal(a["buckets"], b["buckets"]), (name, tk, scale)
-                assert np.array_equal(a["stats"], b["stats"]), (name, tk, scale)
-                assert np.array_equal(a["pct"], b["pct"]), (name, tk, scale)
-                assert np.float32(a["avg"]) == np.float32(b["avg"])
+                nb, total, mx = g["nb_total_max"][i].tolist()
+                assert [a["nb"], a["total"], a["max"]] == [nb, total, mx], (name, tk, scale)
+                assert hashlib.sha256(a["buckets"].astype(np.int64).tobytes()).digest() == g["buckets_sha256"][i].tobytes(), (name, tk, scale)
+                assert np.array_equal(a["stats"], g["stats"][i, :nb]), (name, tk, scale)
+                assert np.array_equal(a["pct"], g["pct"][i]), (name, tk, scale)
+                assert np.float32(a["avg"]) == g["avg"][i]
+                i += 1
+    assert i == len(g["nb_total_max"])
     keys = rng.integers(0, 2 ** 64, 2000, dtype=np.uint64)
-    assert [L.gyo_uint64_hash(int(k)) for k in keys] == [R.gyref_uint64_hash(int(k)) for k in keys]
+    assert [L.gyo_uint64_hash(int(k)) for k in keys] == g["h64"].tolist()
