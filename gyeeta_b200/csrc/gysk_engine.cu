@@ -46,7 +46,8 @@ namespace {
 
 uint32_t pow2_at_least(uint64_t v) { uint32_t p = 16; while (p < v) p <<= 1; return p; }
 
-// one device batch: ingest kernel, then the sort + t-digest chain over the keys it emitted
+// one device batch: ingest kernel, the TCP and TASK drain passes over the records it queued, then the sort + t-digest chain over
+// the keys it emitted
 template <typename AfterIngest>
 int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, AfterIngest after_ingest)
 {
@@ -66,21 +67,13 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, Aft
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	e->kernel_launches += launch_ingest(e->st, e->tmp, d_ev, n, e->cfg.max_svcs, e->stream);
-	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
-	const bool side = side_drain_enabled();
-	if (side) {
-		// the queued connection / process records are applied on the side stream, next to the sort chain of the main stream
-		CU(e, cudaEventRecord(e->ev_ingested, e->stream));
-		CU(e, cudaStreamWaitEvent(e->side_stream, e->ev_ingested, 0));
-		e->kernel_launches += launch_side_drain(e->st, e->tmp, n, e->side_stream);
-		CU(e, cudaEventRecord(e->ev_side_done, e->side_stream));
-	}
 	// the events of this batch are consumed once the ingest kernel has run: callers release / refill the event buffer here,
-	// so that the next H2D copy overlaps the merge kernels
+	// so that the next H2D copy overlaps the drain and merge kernels
 	{ int rc_ai = after_ingest(); if (rc_ai) return rc_ai; }
+	e->kernel_launches += launch_drains(e->st, e->tmp, n, e->stream);
+	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, e->cfg.max_svcs, e->stream);
-	if (side) CU(e, cudaStreamWaitEvent(e->stream, e->ev_side_done, 0));		// the batch is complete on the main stream only with its side work
 	if (pe) CU(e, cudaEventRecord(pe[2], e->stream));
 	e->batches++;
 	return post_launch(e, "ingest batch");
@@ -446,7 +439,6 @@ void gysk_destroy(gysk_engine *e)
 	cudaSetDevice(e->dev);
 	if (e->stream) cudaStreamSynchronize(e->stream);
 	if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
-	if (e->side_stream) cudaStreamSynchronize(e->side_stream);
 	merge_release(e);
 	for (int k = 0; k < NBUF; ++k) {
 		if (e->ev_copied[k]) cudaEventDestroy(e->ev_copied[k]);
@@ -463,9 +455,6 @@ void gysk_destroy(gysk_engine *e)
 	for (void *p : e->hallocs) cudaFreeHost(p);
 	if (e->stream) cudaStreamDestroy(e->stream);
 	if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-	if (e->side_stream) cudaStreamDestroy(e->side_stream);
-	if (e->ev_ingested) cudaEventDestroy(e->ev_ingested);
-	if (e->ev_side_done) cudaEventDestroy(e->ev_side_done);
 	delete e;
 }
 
@@ -508,10 +497,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 
 	if ((ce = cudaSetDevice(e->dev)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaSetDevice", ce); return bail(GYSK_ERR_CUDA); }
 	if ((ce = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking)) != cudaSuccess ||
-			(ce = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess ||
-			(ce = cudaStreamCreateWithFlags(&e->side_stream, cudaStreamNonBlocking)) != cudaSuccess ||
-			(ce = cudaEventCreateWithFlags(&e->ev_ingested, cudaEventDisableTiming)) != cudaSuccess ||
-			(ce = cudaEventCreateWithFlags(&e->ev_side_done, cudaEventDisableTiming)) != cudaSuccess) {
+			(ce = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) {
 		fail(e, GYSK_ERR_CUDA, "cudaStreamCreate", ce); return bail(GYSK_ERR_CUDA);
 	}
 
@@ -590,9 +576,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.pool, pool_cap, false)); A(dalloc(e, &tmp.run_bin, pool_cap, false));
 		A(dalloc(e, &tmp.chunk_run, ((size_t)cfg.max_batch >> 7) + 16, false)); A(dalloc(e, &tmp.segs, ns));
 		A(dalloc(e, &tmp.items_scratch, nmw * NBINS, false)); A(dalloc(e, &tmp.big_scratch, nmw, false));
-		if (side_drain_enabled()) {		// the experiment's record queue: one buffer, filled from both ends
-			A(dalloc(e, &tmp.tcpq, (size_t)cfg.max_batch + 64, false)); tmp.taskq = tmp.tcpq + ((size_t)cfg.max_batch + 63);
-		}
+		// the batch's connection / process record queue: one buffer, filled from both ends
+		A(dalloc(e, &tmp.tcpq, (size_t)cfg.max_batch + 64, false)); tmp.taskq = tmp.tcpq + ((size_t)cfg.max_batch + 63);
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
 

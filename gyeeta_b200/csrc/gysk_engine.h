@@ -124,8 +124,7 @@ struct gysk_engine
 {
 	gysk_config		cfg {};
 	int			dev {0};
-	cudaStream_t		stream {nullptr}, copy_stream {nullptr}, side_stream {nullptr};
-	cudaEvent_t		ev_ingested {nullptr}, ev_side_done {nullptr};	// main -> side after ingest_kernel, side -> main at the end of the batch
+	cudaStream_t		stream {nullptr}, copy_stream {nullptr};
 	gysk::DevState		st {};
 	gysk::SortTemp		tmp {};
 	std::vector<void *>	dallocs;
@@ -155,7 +154,7 @@ struct gysk_engine
 
 	// optional per-kernel timing
 	bool			profiling {false};
-	std::vector<cudaEvent_t> prof_events;		// triples: before ingest, after ingest, after t-digest chain
+	std::vector<cudaEvent_t> prof_events;		// triples: before ingest, after the drain passes, after t-digest chain
 	size_t			prof_used {0};
 
 	// rolling levels: epoch held by each ring slot (~0 = never written) and the time of the last flush

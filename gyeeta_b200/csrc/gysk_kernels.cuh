@@ -61,7 +61,7 @@ struct SortTemp
 	TdWorkBig		*big_scratch;		// [merge warps] work arrays for merged lists beyond 2 x TD_CAP entries
 	uint4			*tcpq, *taskq;		// ONE buffer of max_batch records {slot, value, flow key}: connection records from the front
 							// (tcpq), process records from the back (taskq = last entry, growing down); ingest_kernel
-							// resolves the ids and queues them, side_drain_kernel applies them next to the sort chain
+							// resolves the ids and queues them, the drain passes (launch_drains) apply them
 	uint32_t		max_tiles;
 };
 
@@ -104,8 +104,7 @@ int launch_init_state(const DevState &st, uint32_t max_svcs, uint32_t max_tasks,
 int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_t n, int is_task, cudaStream_t s);
 int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
-bool side_drain_enabled();
-int launch_side_drain(const DevState &st, const SortTemp &tmp, uint64_t n_events, cudaStream_t s);
+int launch_drains(const DevState &st, const SortTemp &tmp, uint64_t n_events, cudaStream_t s);
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo1, int hi1, int lo2, int hi2, int *which, cudaStream_t s);
 int radix_sort_plan(int lo1, int hi1, int lo2, int hi2, int out[][4], int cap);
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int metric, int host_filter, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
