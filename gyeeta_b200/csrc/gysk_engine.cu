@@ -66,11 +66,14 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, Aft
 		e->prof_used += 3;
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
-	e->kernel_launches += launch_ingest(e->st, e->tmp, d_ev, n, e->cfg.max_svcs, e->stream);
+	RecRegions rr;
+	const int li = launch_ingest(e->st, e->tmp, d_ev, n, e->cfg.max_svcs, rr, e->stream);
+	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
+	e->kernel_launches += li;
 	// the events of this batch are consumed once the ingest kernel has run: callers release / refill the event buffer here,
 	// so that the next H2D copy overlaps the drain and merge kernels
 	{ int rc_ai = after_ingest(); if (rc_ai) return rc_ai; }
-	e->kernel_launches += launch_drains(e->st, e->tmp, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, e->cfg.max_svcs, e->stream);
@@ -576,8 +579,11 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.pool, pool_cap, false)); A(dalloc(e, &tmp.run_bin, pool_cap, false));
 		A(dalloc(e, &tmp.chunk_run, ((size_t)cfg.max_batch >> 7) + 16, false)); A(dalloc(e, &tmp.segs, ns));
 		A(dalloc(e, &tmp.items_scratch, nmw * NBINS, false)); A(dalloc(e, &tmp.big_scratch, nmw, false));
-		// the batch's connection / process record queue: one buffer, filled from both ends
-		A(dalloc(e, &tmp.tcpq, (size_t)cfg.max_batch + 64, false)); tmp.taskq = tmp.tcpq + ((size_t)cfg.max_batch + 63);
+		// the batch's connection / process record queue: one region per ingest warp (SortTemp::recq)
+		const uint32_t nsm = (uint32_t)prop.multiProcessorCount;
+		tmp.recq_cap = (uint64_t)cfg.max_batch + (uint64_t)nsm * INGEST_MAX_CHUNK_EVENTS_PER_SM;
+		tmp.rec_cnt_cap = nsm * INGEST_MAX_WARPS_PER_SM;
+		A(dalloc(e, &tmp.recq, (size_t)tmp.recq_cap, false)); A(dalloc(e, &tmp.rec_cnt, (size_t)tmp.rec_cnt_cap, false));
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
 

@@ -203,17 +203,26 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t pari
 //       histograms on the way out); beside it only what would change state: the batch extremes of the slot and the CONN_BITMAP bit,
 //       each behind a load so that the atomic is issued only while the value still moves;
 //   (3) TCP / TASK events join one of the warp's two private shared-memory queues (ballot + popc, no atomics: the queue
-//       lengths are warp-uniform registers); a queue leaves for the batch's global record queue only in whole multiples of 32
-//       entries (one cursor atomic per warp and hand-over, coalesced 16-byte stores), the < 32 left-over entries move to the
-//       front. drain_kernel applies the records after this kernel: TCP = two lookup2 hashes per flow key -> four count-min REDs +
-//       HLL register + the service's exact {count, kbytes} cell; TASK = the three histograms of MAGGR_TASK::set_local_task_state
-//       with one (record, histogram) pair per lane.
+//       lengths are warp-uniform registers); a queue leaves for the warp's own region of the batch's record queue only in whole
+//       multiples of 32 entries (coalesced 16-byte stores at the warp's running offset, no atomic), the < 32 left-over entries
+//       move to the front. drain_kernel applies the records after this kernel: TCP = two lookup2 hashes per flow key -> four
+//       count-min REDs + HLL register + the service's exact {count, kbytes} cell; TASK = the three histograms of
+//       MAGGR_TASK::set_local_task_state with one (record, histogram) pair per lane.
 // The histogram cells and the t-digest of a service are produced from its bins by bins_merge_kernel after the batch.
 struct alignas(16) IngestRec { uint32_t slot; uint32_t value; unsigned long long flow_key; };		// moved as one 128-bit word
 static_assert(sizeof(IngestRec) == 16, "IngestRec travels as one uint4");
 
-// m queued connection records (all 32 lanes call; q in shared or global memory): two lookup2 hashes per flow key -> four count-min
-// REDs + the HLL register + the service's exact {count, kbytes} cell
+// a queued record is read exactly once: evict-first, like the __stcs that wrote it, so that it does not push the drain pass's
+// count-min / histogram lines out of L2
+__device__ __forceinline__ IngestRec ld_rec(const IngestRec *p)
+{
+	const uint4 v = __ldcs(reinterpret_cast<const uint4 *>(p));
+	IngestRec r; r.slot = v.x; r.value = v.y; r.flow_key = ((unsigned long long)v.w << 32) | v.z;
+	return r;
+}
+
+// m queued connection records (all 32 lanes call): two lookup2 hashes per flow key -> four count-min REDs + the HLL register + the
+// service's exact {count, kbytes} cell
 template <typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, HotTable &hot, const IngestRec *q, uint32_t m, int lane)
 {
@@ -221,7 +230,7 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, HotTable &hot
 		const bool act = i < m;
 		uint32_t cell = 0, idx = 0, rank = 0, hw = 0; int kb = 0;
 		if (act) {
-			const IngestRec r = q[i];
+			const IngestRec r = ld_rec(q + i);
 			uint32_t h1, h2;
 			flow_hashes(r.flow_key, h1, h2);
 			// the HLL register word is asked for first and looked at last: the count-min REDs and the cell update hide its latency
@@ -248,7 +257,7 @@ __device__ __forceinline__ void drain_task_recs(const DevState &st, HotTable &ho
 		uint32_t cell = 0; int d = 0;
 		if (act) {
 			const uint32_t e = p / 3u, h = p - e * 3u;
-			const IngestRec r = BACKWARDS ? *(q - (long long)e) : q[e];
+			const IngestRec r = ld_rec(BACKWARDS ? q - (long long)e : q + e);
 			// GY_HISTOGRAM<int, ...>::add_data(int): the three values narrow to int (server/gy_msocket.h:1014-1016)
 			d = h == 0 ? (int)r.value : (h == 1 ? (int)(uint32_t)r.flow_key : (int)(uint32_t)(r.flow_key >> 32));
 			const uint32_t b = h == 0 ? (uint32_t)bucket_hash_1_3000(d) : (uint32_t)bucket_duration(d);
@@ -275,7 +284,7 @@ struct IngestSharedT
 
 template <int WARPS, int MIN_CTAS, int EPT, bool TMA, int DH>
 __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
-		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ tcpq, uint4 *__restrict__ taskq)
+		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt)
 {
 	using Shared = IngestSharedT<WARPS, EPT, TMA, DH>;
 	constexpr int CHUNK = Shared::CHUNK;
@@ -307,21 +316,20 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState s
 	};
 	if (TMA && lane == 0 && gwarp < nchunks) tma_issue(gwarp);
 
-	// ---- queue drains (all 32 lanes, m = multiple of 32 except in the final drain): handed as one coalesced run to the batch's
-	//      record queues, which the two drain_kernel passes apply after this kernel ----
-	// one buffer holds both queues: connection records grow from its front, process records from its back (taskq points at the last
-	// entry; together they never exceed the batch's event count)
-	auto hand_over = [&](const IngestRec *q, uint32_t m, uint4 *gq, int ctr, bool backwards) {
-		unsigned long long base = 0;
-		if (lane == 0) base = atomicAdd(st.counters + ctr, (unsigned long long)m);
-		base = __shfl_sync(0xffffffffu, base, 0);
+	// ---- queue drains (all 32 lanes, m = multiple of 32 except in the final drain): handed as one coalesced run to the warp's
+	//      region of the batch's record queue, which the two drain_kernel passes apply after this kernel ----
+	// the region holds what the warp's chunks can bring (rcap = its number of chunks x CHUNK): connection records grow from its front,
+	// process records from its back (taskq = its last entry); the offsets are the warp's totals so far, no atomic
+	const uint64_t rcap = (nchunks + nwarps - 1) / nwarps * CHUNK;
+	uint4 *const tcpq = recq + gwarp * rcap, *const taskq = tcpq + (rcap - 1);
+	auto hand_over = [&](const IngestRec *q, uint32_t m, uint4 *gq, unsigned long long base, bool backwards) {
 		for (uint32_t i = lane; i < m; i += 32) {
 			const uint4 v = *reinterpret_cast<const uint4 *>(q + i);
 			if (backwards) __stcs(gq - (long long)(base + i), v); else __stcs(gq + base + i, v);
 		}
 	};
-	auto drain_tcp = [&](uint32_t m) { hand_over(W.tcp, m, tcpq, CTR_NTCPQ, false); };
-	auto drain_task = [&](uint32_t m) { hand_over(W.task, m, taskq, CTR_NTASKQ, true); };
+	auto drain_tcp = [&](uint32_t m) { hand_over(W.tcp, m, tcpq, t_tcp, false); };
+	auto drain_task = [&](uint32_t m) { hand_over(W.task, m, taskq, t_task, true); };
 	auto keep_rest = [&](IngestRec *q, uint32_t m, uint32_t total) {		// entries [m, total) move to the front (total - m < 32)
 		IngestRec r;
 		const bool mv = m + lane < total;
@@ -482,6 +490,7 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState s
 	if (ntcp) { drain_tcp(ntcp); t_tcp += ntcp; }
 	if (ntask) { drain_task(ntask); t_task += ntask; }
 	if (nk) flush_keys();
+	if (lane == 0) rec_cnt[gwarp] = make_uint2((uint32_t)t_tcp, (uint32_t)t_task);	// every warp of the launch: no memset needed
 
 	__syncthreads();
 	// retire: one RED per digit this CTA saw
@@ -519,22 +528,53 @@ static constexpr int DR_WARPS = 8;
 static constexpr int DR_HOT_BITS = 12;		// 4096 entries, 80 KB: on the bench workload faster than 2^11 and 2^9 (DESIGN.md §7)
 using DrainHot = HotTableT<DR_HOT_BITS>;
 
+// The records sit in the ingest launch's per-warp regions (RecRegions). Each CTA scans the regions' counts into a table of where
+// each region's groups of 32 records start, and every warp takes an equal, contiguous share of all groups: the regions' sizes
+// differ, the drain warps' work does not.
 template <bool TASK>
-__global__ void __launch_bounds__(DR_WARPS * 32) drain_kernel(DevState st, const uint4 *__restrict__ q)
+__global__ void __launch_bounds__(DR_WARPS * 32) drain_kernel(DevState st, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt, RecRegions rr)
 {
 	extern __shared__ __align__(16) unsigned char drain_smem[];
 	DrainHot &hot = *reinterpret_cast<DrainHot *>(drain_smem);
+	// [nwarps + 1] per region: first group << 5 | (records & 31); the last entry holds the number of groups << 5
+	uint32_t *rstart = reinterpret_cast<uint32_t *>(drain_smem + sizeof(DrainHot));
+	__shared__ uint32_t wsum[DR_WARPS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 	for (int i = threadIdx.x; i < DrainHot::N; i += DR_WARPS * 32) { hot.tag[i] = 0; hot.count[i] = 0; hot.sum[i] = 0; hot.vmax[i] = INT_MIN; }
-	__syncthreads();
-	const unsigned long long nq = st.counters[TASK ? CTR_NTASKQ : CTR_NTCPQ];
-	const unsigned long long gw = (unsigned long long)blockIdx.x * DR_WARPS + wid, nw = (unsigned long long)gridDim.x * DR_WARPS;
-	const IngestRec *recs = reinterpret_cast<const IngestRec *>(q);
 
-	for (unsigned long long base = gw * 32; base < nq; base += nw * 32) {
-		const uint32_t m = (uint32_t)(nq - base < 32 ? nq - base : 32);
-		if (TASK) drain_task_recs<DrainHot, true>(st, hot, recs - (long long)base, m, lane);
-		else drain_tcp_recs(st, hot, recs + base, m, lane);
+	// exclusive scan of the regions' group counts: thread t takes a contiguous run of regions
+	const uint32_t nreg = rr.nwarps, per = (nreg + DR_WARPS * 32 - 1) / (DR_WARPS * 32), r0 = threadIdx.x * per;
+	const uint32_t r1 = min(r0 + per, nreg);
+	uint32_t s = 0;
+	for (uint32_t r = r0; r < r1; ++r) {
+		const uint32_t c = TASK ? cnt[r].y : cnt[r].x;
+		rstart[r] = c; s += (c + 31u) >> 5;
+	}
+	uint32_t incl = s;
+#pragma unroll
+	for (int off = 1; off < 32; off <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, off); if (lane >= off) incl += t; }
+	if (lane == 31) wsum[wid] = incl;
+	__syncthreads();
+	uint32_t g0 = incl - s, ngroups = 0;
+#pragma unroll
+	for (int w = 0; w < DR_WARPS; ++w) { if (w < wid) g0 += wsum[w]; ngroups += wsum[w]; }
+	for (uint32_t r = r0; r < r1; ++r) { const uint32_t c = rstart[r]; rstart[r] = (g0 << 5) | (c & 31u); g0 += (c + 31u) >> 5; }
+	if (threadIdx.x == 0) rstart[nreg] = ngroups << 5;
+	__syncthreads();
+
+	const uint32_t gw = blockIdx.x * DR_WARPS + wid, nw = gridDim.x * DR_WARPS;
+	const uint32_t gbeg = (uint32_t)((unsigned long long)ngroups * gw / nw), gend = (uint32_t)((unsigned long long)ngroups * (gw + 1) / nw);
+	const IngestRec *recs = reinterpret_cast<const IngestRec *>(q);
+	// region of group gbeg: the last one that starts at or before it
+	uint32_t r = 0;
+	for (uint32_t hi = nreg; r < hi; ) { const uint32_t mid = (r + hi + 1) >> 1; if ((rstart[mid] >> 5) <= gbeg) r = mid; else hi = mid - 1; }
+	for (uint32_t g = gbeg; g < gend; ++g) {
+		while ((rstart[r + 1] >> 5) <= g) ++r;			// empty regions start where the next one does
+		const uint32_t first = rstart[r] >> 5, tail = rstart[r] & 31u, off = (g - first) * 32u;
+		const uint32_t m = (g + 1 == rstart[r + 1] >> 5 && tail) ? tail : 32u;
+		const IngestRec *region = recs + (unsigned long long)r * rr.cap;
+		if (TASK) drain_task_recs<DrainHot, true>(st, hot, region + (rr.cap - 1 - off), m, lane);
+		else drain_tcp_recs(st, hot, region + off, m, lane);
 	}
 
 	__syncthreads();
@@ -1555,10 +1595,12 @@ static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
 }
 
 template <int WARPS, int MIN_CTAS, int EPT, bool TMA, int DH>
-static void launch_ingest_variant(const DevState &st, const gysk_event *d_ev, uint64_t n, unsigned long long *d_keys, uint32_t *ghist, const SortPlan &plan,
-		uint4 *tcpq, uint4 *taskq, int dev, cudaStream_t s)
+static int launch_ingest_variant(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, const SortPlan &plan, RecRegions &rr,
+		int dev, cudaStream_t s)
 {
 	using Shared = IngestSharedT<WARPS, EPT, TMA, DH>;
+	static_assert(WARPS * MIN_CTAS <= INGEST_MAX_WARPS_PER_SM && WARPS * MIN_CTAS * Shared::CHUNK <= INGEST_MAX_CHUNK_EVENTS_PER_SM,
+			"the record queue is sized for a smaller grid");
 	static bool attr_set[MAX_DEVICES] = {};
 	if (!attr_set[dev]) {
 		cudaFuncSetAttribute(ingest_kernel<WARPS, MIN_CTAS, EPT, TMA, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Shared));
@@ -1566,10 +1608,17 @@ static void launch_ingest_variant(const DevState &st, const gysk_event *d_ev, ui
 	}
 	const uint64_t want = (n + (uint64_t)Shared::CHUNK * WARPS - 1) / ((uint64_t)Shared::CHUNK * WARPS);
 	const uint64_t full = (uint64_t)sm_count(dev) * MIN_CTAS;
-	ingest_kernel<WARPS, MIN_CTAS, EPT, TMA, DH><<<(uint32_t)(want < full ? want : full), WARPS * 32, sizeof(Shared), s>>>(st, d_ev, n, d_keys, ghist, plan, tcpq, taskq);
+	const uint32_t grid = (uint32_t)(want < full ? want : full);
+	// the kernel computes the same regions from its grid
+	const uint64_t nchunks = (n + Shared::CHUNK - 1) / Shared::CHUNK;
+	rr.nwarps = grid * WARPS;
+	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * Shared::CHUNK;
+	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
+	ingest_kernel<WARPS, MIN_CTAS, EPT, TMA, DH><<<grid, WARPS * 32, sizeof(Shared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt);
+	return 1;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, cudaStream_t s)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
 	const int dev = current_device();
@@ -1582,8 +1631,8 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	cudaMemsetAsync(tmp.os_ghist, 0, (OS_MAX_PASSES * RADIX_MAX + OS_MAX_PASSES) * sizeof(uint32_t), s);
 	bool wide = false;
 	for (int p = 0; p < plan.np; ++p) wide |= plan.bits[p] > 8;
-	cudaMemsetAsync(st.counters + CTR_NTCPQ, 0, (CTR_NTASKQ - CTR_NTCPQ + 1) * sizeof(unsigned long long), s);	// record queue cursors
-#define GYSK_LI2(W, C, E, T, D) launch_ingest_variant<W, C, E, T, D>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.tcpq, tmp.taskq, dev, s)
+	int rc;
+#define GYSK_LI2(W, C, E, T, D) rc = launch_ingest_variant<W, C, E, T, D>(st, tmp, d_ev, n, plan, rr, dev, s)
 #define GYSK_LI(W, C, E, T) do { if (wide) GYSK_LI2(W, C, E, T, 512); else GYSK_LI2(W, C, E, T, 256); } while (0)
 	switch (ingest_variant()) {
 	case 842 : GYSK_LI(8, 4, 2, false); break;
@@ -1598,33 +1647,36 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	}
 #undef GYSK_LI
 #undef GYSK_LI2
-	return 1;
+	return rc;
 }
 
-// one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x DR_WARPS events of the batch)
+// one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x DR_WARPS events of the batch); shared memory = the hot
+// table + the region start table, whose largest size sets the occupancy
 template <bool TASK>
-static void launch_drain_pass(const DevState &st, const uint4 *q, uint64_t n_events, int dev, cudaStream_t s)
+static void launch_drain_pass(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev, cudaStream_t s)
 {
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
-		cudaFuncSetAttribute(drain_kernel<TASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DrainHot));
+		const size_t smem_max = sizeof(DrainHot) + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
+		cudaFuncSetAttribute(drain_kernel<TASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK>, DR_WARPS * 32, sizeof(DrainHot));
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK>, DR_WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + DR_WARPS * 32 - 1) / (DR_WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
-	drain_kernel<TASK><<<(uint32_t)(want < full ? want : full), DR_WARPS * 32, sizeof(DrainHot), s>>>(st, q);
+	const size_t smem = sizeof(DrainHot) + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
+	drain_kernel<TASK><<<(uint32_t)(want < full ? want : full), DR_WARPS * 32, smem, s>>>(st, tmp.recq, tmp.rec_cnt, rr);
 }
 
 // the batch's queued connection records -> count-min, HLL, exact cells; then its process records -> process histograms
-int launch_drains(const DevState &st, const SortTemp &tmp, uint64_t n_events, cudaStream_t s)
+int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
 	int launches = 0;
-	if (!(exp_ablate() & 4)) { launch_drain_pass<false>(st, tmp.tcpq, n_events, dev, s); launches++; }
-	if (!(exp_ablate() & 8)) { launch_drain_pass<true>(st, tmp.taskq, n_events, dev, s); launches++; }
+	if (!(exp_ablate() & 4)) { launch_drain_pass<false>(st, tmp, rr, n_events, dev, s); launches++; }
+	if (!(exp_ablate() & 8)) { launch_drain_pass<true>(st, tmp, rr, n_events, dev, s); launches++; }
 	return launches;
 }
 

@@ -59,11 +59,23 @@ struct SortTemp
 	uint4			*segs;			// [max_svcs] BatchSeg of each touched service
 	Centroid		*items_scratch;		// [merge warps][NBINS] a warp's list of batch items
 	TdWorkBig		*big_scratch;		// [merge warps] work arrays for merged lists beyond 2 x TD_CAP entries
-	uint4			*tcpq, *taskq;		// ONE buffer of max_batch records {slot, value, flow key}: connection records from the front
-							// (tcpq), process records from the back (taskq = last entry, growing down); ingest_kernel
-							// resolves the ids and queues them, the drain passes (launch_drains) apply them
+	uint4			*recq;			// [recq_cap] records {slot, value, flow key}: ingest_kernel resolves the ids of connection and
+							// process events and queues them, the drain passes (launch_drains) apply them. Warp w of the
+							// ingest launch owns region [w * cap, (w + 1) * cap) (RecRegions): its connection records from
+							// the front, its process records from the back, stored at warp-local offsets without any atomic
+	uint2			*rec_cnt;		// [rec_cnt_cap] {connection, process} records of each region, written by every warp of the launch
+	uint64_t		recq_cap;		// max_batch + the regions' rounding (INGEST_MAX_CHUNK_EVENTS_PER_SM per SM)
+	uint32_t		rec_cnt_cap;		// INGEST_MAX_WARPS_PER_SM per SM
 	uint32_t		max_tiles;
 };
+
+// the record queue regions of one ingest launch: one per warp, cap = ceil(chunks / warps) x events per chunk, the most records a
+// warp can queue (chunks are dealt to the warps round-robin)
+struct RecRegions { uint32_t nwarps; uint64_t cap; };
+
+// the largest grid of any ingest_kernel launch shape (GYSK_INGEST_VARIANT), per SM: warps, and warps x events per chunk. They size
+// the record queue beyond max_batch; launch_ingest checks every launch against the buffers.
+static constexpr uint32_t INGEST_MAX_WARPS_PER_SM = 40, INGEST_MAX_CHUNK_EVENTS_PER_SM = 4096;
 
 // raw per-id record gathered for queries / exports
 struct SvcRaw
@@ -102,9 +114,10 @@ static constexpr int TD_MERGE_CTAS_PER_SM = 7, TD_MERGE_MAX_SMS = 192;	// bins_m
 // every launcher returns the number of kernel launches it issued
 int launch_init_state(const DevState &st, uint32_t max_svcs, uint32_t max_tasks, cudaStream_t s);
 int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_t n, int is_task, cudaStream_t s);
-int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, cudaStream_t s);
+// -1: no sort plan for max_svcs, or the launch's record regions do not fit the buffers
+int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
-int launch_drains(const DevState &st, const SortTemp &tmp, uint64_t n_events, cudaStream_t s);
+int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo1, int hi1, int lo2, int hi2, int *which, cudaStream_t s);
 int radix_sort_plan(int lo1, int hi1, int lo2, int hi2, int out[][4], int cap);
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int metric, int host_filter, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
