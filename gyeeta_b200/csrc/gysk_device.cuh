@@ -223,6 +223,42 @@ __device__ __forceinline__ void red_max_s64(long long *p, long long v)
 	asm volatile("red.global.max.s64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
 }
 
+// L2 eviction priorities. A policy (createpolicy, a 64-bit register) travels with each access through .L2::cache_hint: ptxas for
+// sm_90a accepts a priority written directly on ld only for 256-bit loads, so the policy operand is the form open to 32- and
+// 64-bit accesses. atom.cas takes no hint at all.
+__device__ __forceinline__ unsigned long long l2_policy_evict_first()
+{
+	unsigned long long pol;
+	asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+	return pol;
+}
+
+__device__ __forceinline__ unsigned long long l2_policy_evict_last()
+{
+	unsigned long long pol;
+	asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+	return pol;
+}
+
+__device__ __forceinline__ void red_add_u64_hint(unsigned long long *p, unsigned long long v, unsigned long long pol)
+{
+	asm volatile("red.global.add.L2::cache_hint.u64 [%0], %1, %2;" :: "l"(p), "l"(v), "l"(pol) : "memory");
+}
+
+// 32-bit load that does not allocate in L1 and allocates in L2 with the policy's priority
+__device__ __forceinline__ uint32_t ld_na_hint_u32(const uint32_t *p, unsigned long long pol)
+{
+	uint32_t v;
+	asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+	return v;
+}
+
+// a line's L2 priority back to normal (a line brought in with evict_last keeps that priority after the kernel ends)
+__device__ __forceinline__ void l2_evict_normal_line(const void *p)
+{
+	asm volatile("applypriority.global.L2::evict_normal [%0], 128;" :: "l"(p) : "memory");
+}
+
 __device__ __forceinline__ uint4 ld_cg_v4(const void *p)
 {
 	uint4 v;

@@ -39,7 +39,8 @@ __device__ __forceinline__ uint32_t key_bin(unsigned long long k) { return (uint
 
 struct SortPlan { int np; int shift[OS_MAX_PASSES_VK]; int bits[OS_MAX_PASSES_VK]; int exp; };	// digit p = (key >> shift[p]) & ((1 << bits[p]) - 1)
 // exp: ABLATION switches for timing runs only (GYSK_EXP_ABLATE; results are wrong when set): 1 = no batch-extreme / CONN_BITMAP loads and
-// atomics, 2 = no digit histograms, 4 = no TCP drain pass, 8 = no TASK drain pass
+// atomics, 2 = no digit histograms, 4 = no TCP drain pass, 8 = no TASK drain pass, 16 = TCP drain pass without the count-min REDs,
+// 32 = TCP drain pass without the HLL register peek / raise
 
 // ---------------------------------------------------------------------------------------------------
 // state init / registration
@@ -222,9 +223,15 @@ __device__ __forceinline__ IngestRec ld_rec(const IngestRec *p)
 }
 
 // m queued connection records (all 32 lanes call): two lookup2 hashes per flow key -> four count-min REDs + the HLL register + the
-// service's exact {count, kbytes} cell
+// service's exact {count, kbytes} cell.
+// L2 priorities (DESIGN.md §7): the count-min lines are taken evict_last, the HLL register sectors evict_first, the records are read
+// evict-first (ld_rec). The table is 32 MB and takes 80 M REDs per 100 M-event batch; at normal priority the 20 M HLL sectors, spread
+// over hundreds of MB by the services' Zipf tail, pushed its lines out of the 50 MB L2 and many REDs became DRAM read-modify-writes.
+// The drain_kernel TASK pass sets the table's lines back to evict_normal. pol_hll / pol_cms: l2_policy_evict_first / _last.
+// exp (timing runs only): 16 = no count-min REDs, 32 = no HLL peek / raise
 template <typename HotTable>
-__device__ __forceinline__ void drain_tcp_recs(const DevState &st, HotTable &hot, const IngestRec *q, uint32_t m, int lane)
+__device__ __forceinline__ void drain_tcp_recs(const DevState &st, HotTable &hot, const IngestRec *q, uint32_t m, int lane,
+		unsigned long long pol_hll, unsigned long long pol_cms, int exp)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
@@ -234,16 +241,20 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, HotTable &hot
 			uint32_t h1, h2;
 			flow_hashes(r.flow_key, h1, h2);
 			// the HLL register word is asked for first and looked at last: the count-min REDs and the cell update hide its latency
-			hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
-			hw = hll_peek(st.hll + ((size_t)r.slot << st.hll_p), idx);
+			// (stale is harmless: the CAS re-validates)
+			if (!(exp & 32)) {
+				hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
+				hw = ld_na_hint_u32(reinterpret_cast<const uint32_t *>(st.hll + ((size_t)r.slot << st.hll_p)) + (idx >> 2), pol_hll);
+			}
 			const unsigned long long inc = cms_increment(r.value);
-			for (uint32_t row = 0; row < st.cms_depth; ++row)
-				red_add_u64(st.cms_cur + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
+			if (!(exp & 16))
+				for (uint32_t row = 0; row < st.cms_depth; ++row)
+					red_add_u64_hint(st.cms_cur + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc, pol_cms);
 			cell = r.slot;
 			kb = (int)(r.value >> 10);
 		}
 		cell_add(st, hot, act, cell, kb);
-		if (act) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
+		if (act && !(exp & 32)) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
 	}
 }
 
@@ -522,7 +533,8 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState s
 // histograms, about 19 MB), and each fits in the H100's 50 MB L2 on its own; inside ingest_kernel they competed with each other and
 // with the RESP path's tables, bitmaps and hot rows for it (DESIGN.md §7). Two launches, not two phases of one kernel: CTAs would
 // reach the second phase at different times and mix the two working sets again. Persistent grid; a warp takes 32 records at a time;
-// hot cells are privatised per CTA (cell_add).
+// hot cells are privatised per CTA (cell_add). Inside the TCP pass, L2 priorities keep the count-min table resident against the HLL
+// sectors (drain_tcp_recs).
 // ---------------------------------------------------------------------------------------------------
 static constexpr int DR_WARPS = 8;
 static constexpr int DR_HOT_BITS = 12;		// 4096 entries, 80 KB: on the bench workload faster than 2^11 and 2^9 (DESIGN.md §7)
@@ -532,8 +544,16 @@ using DrainHot = HotTableT<DR_HOT_BITS>;
 // each region's groups of 32 records start, and every warp takes an equal, contiguous share of all groups: the regions' sizes
 // differ, the drain warps' work does not.
 template <bool TASK>
-__global__ void __launch_bounds__(DR_WARPS * 32) drain_kernel(DevState st, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt, RecRegions rr)
+__global__ void __launch_bounds__(DR_WARPS * 32) drain_kernel(DevState st, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt, RecRegions rr, int exp)
 {
+	if (TASK) {
+		// the TCP pass left the count-min lines evict_last, a priority they keep after it ends: back to normal, so that they do not
+		// hold L2 against the next batch's ingest_kernel and chain
+		const size_t lines = ((size_t)st.cms_depth << st.cms_log2w) * sizeof(unsigned long long) / 128u;
+		for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < lines; i += (size_t)gridDim.x * blockDim.x)
+			l2_evict_normal_line(reinterpret_cast<const char *>(st.cms_cur) + i * 128u);
+	}
+	const unsigned long long pol_hll = TASK ? 0 : l2_policy_evict_first(), pol_cms = TASK ? 0 : l2_policy_evict_last();
 	extern __shared__ __align__(16) unsigned char drain_smem[];
 	DrainHot &hot = *reinterpret_cast<DrainHot *>(drain_smem);
 	// [nwarps + 1] per region: first group << 5 | (records & 31); the last entry holds the number of groups << 5
@@ -574,7 +594,7 @@ __global__ void __launch_bounds__(DR_WARPS * 32) drain_kernel(DevState st, const
 		const uint32_t m = (g + 1 == rstart[r + 1] >> 5 && tail) ? tail : 32u;
 		const IngestRec *region = recs + (unsigned long long)r * rr.cap;
 		if (TASK) drain_task_recs<DrainHot, true>(st, hot, region + (rr.cap - 1 - off), m, lane);
-		else drain_tcp_recs(st, hot, region + off, m, lane);
+		else drain_tcp_recs(st, hot, region + off, m, lane, pol_hll, pol_cms, exp);
 	}
 
 	__syncthreads();
@@ -1653,7 +1673,7 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x DR_WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
 template <bool TASK>
-static void launch_drain_pass(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev, cudaStream_t s)
+static void launch_drain_pass(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int exp, int dev, cudaStream_t s)
 {
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
@@ -1666,7 +1686,7 @@ static void launch_drain_pass(const DevState &st, const SortTemp &tmp, const Rec
 	const uint64_t want = (n_events + DR_WARPS * 32 - 1) / (DR_WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = sizeof(DrainHot) + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK><<<(uint32_t)(want < full ? want : full), DR_WARPS * 32, smem, s>>>(st, tmp.recq, tmp.rec_cnt, rr);
+	drain_kernel<TASK><<<(uint32_t)(want < full ? want : full), DR_WARPS * 32, smem, s>>>(st, tmp.recq, tmp.rec_cnt, rr, exp);
 }
 
 // the batch's queued connection records -> count-min, HLL, exact cells; then its process records -> process histograms
@@ -1674,9 +1694,10 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr,
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
+	const int exp = exp_ablate();
 	int launches = 0;
-	if (!(exp_ablate() & 4)) { launch_drain_pass<false>(st, tmp, rr, n_events, dev, s); launches++; }
-	if (!(exp_ablate() & 8)) { launch_drain_pass<true>(st, tmp, rr, n_events, dev, s); launches++; }
+	if (!(exp & 4)) { launch_drain_pass<false>(st, tmp, rr, n_events, exp, dev, s); launches++; }
+	if (!(exp & 8)) { launch_drain_pass<true>(st, tmp, rr, n_events, exp, dev, s); launches++; }
 	return launches;
 }
 
