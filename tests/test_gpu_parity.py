@@ -73,7 +73,8 @@ def test_table_full_and_no_auto_register():
     assert tot == s2["events_resp"]
 
 
-@pytest.mark.parametrize("nsvc,n,batch", [(50, 20_000, 8192), (3000, 300_000, 1 << 17)])
+@pytest.mark.parametrize("nsvc,n,batch", [(50, 20_000, 8192), (3000, 300_000, 1 << 17),
+                                          (3000, 1_500_000, 700_000)])       # batches beyond one full ingest grid (~200 K events)
 def test_mixed_stream_bit_exact(nsvc, n, batch):
     rng = np.random.default_rng(11)
     ev = synth.gen_mixed(rng, n, nsvc, ntask=max(nsvc // 4, 4), nhosts=64, nclients=20_000)
