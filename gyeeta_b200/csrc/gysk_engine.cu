@@ -581,8 +581,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.items_scratch, nmw * NBINS, false)); A(dalloc(e, &tmp.big_scratch, nmw, false));
 		// the batch's connection / process record queue: one region per ingest warp (SortTemp::recq)
 		const uint32_t nsm = (uint32_t)prop.multiProcessorCount;
-		tmp.recq_cap = (uint64_t)cfg.max_batch + (uint64_t)nsm * INGEST_MAX_CHUNK_EVENTS_PER_SM;
-		tmp.rec_cnt_cap = nsm * INGEST_MAX_WARPS_PER_SM;
+		tmp.rec_cnt_cap = nsm * IngestShape::WARPS * IngestShape::MIN_CTAS;
+		tmp.recq_cap = (uint64_t)cfg.max_batch + (uint64_t)tmp.rec_cnt_cap * IngestShape::CHUNK;
 		A(dalloc(e, &tmp.recq, (size_t)tmp.recq_cap, false)); A(dalloc(e, &tmp.rec_cnt, (size_t)tmp.rec_cnt_cap, false));
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;

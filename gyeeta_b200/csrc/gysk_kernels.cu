@@ -37,6 +37,7 @@ __device__ __forceinline__ uint32_t key_usec(unsigned long long k) { return (uin
 __device__ __forceinline__ uint32_t key_slot(unsigned long long k) { return (uint32_t)(k >> KEY_SLOT_SHIFT); }
 __device__ __forceinline__ uint32_t key_bin(unsigned long long k) { return (uint32_t)(k >> KEY_GROUP_SHIFT) & ((1u << TD_CODE_BITS) - 1u); }
 
+static constexpr int KEY_DIGIT_MAX = 8;				// widest digit of the RESP-key passes (key_sort_plan)
 struct SortPlan { int np; int shift[OS_MAX_PASSES_VK]; int bits[OS_MAX_PASSES_VK]; int exp; };	// digit p = (key >> shift[p]) & ((1 << bits[p]) - 1)
 // exp: ABLATION switches for timing runs only (GYSK_EXP_ABLATE; results are wrong when set): 1 = no batch-extreme / CONN_BITMAP loads and
 // atomics, 2 = no digit histograms, 4 = no TCP drain pass, 8 = no TASK drain pass, 16 = TCP drain pass without the count-min REDs,
@@ -179,27 +180,6 @@ __device__ __forceinline__ void hll_update(uint8_t *regs, uint32_t idx, uint32_t
 	hll_raise(regs, idx, rank, hll_peek(regs, idx));
 }
 
-// ---- TMA (bulk async copy) of a warp's next event chunk into shared memory, completion on the warp's own mbarrier ----
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, uint32_t count)
-{
-	asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
-}
-
-__device__ __forceinline__ void tma_load_1d(void *dst_smem, const void *src_gmem, uint32_t bytes, unsigned long long *bar)
-{
-	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-			:: "r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t parity)
-{
-	asm volatile("{\n\t.reg .pred p;\n\tWAIT_LOOP:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra WAIT_DONE;\n\tbra WAIT_LOOP;\n\tWAIT_DONE:\n\t}"
-			:: "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
 // The kernel is WARP-AUTONOMOUS: no block barrier anywhere in the event loop. A warp takes a chunk of 32 x EPT events and
 //   (1) decodes them fully converged: 2 x 128-bit load per event, shard filter, id -> slot lookup with the first table probe
 //       of all EPT events in flight together;
@@ -286,53 +266,35 @@ __device__ __forceinline__ void drain_task_group(const DevState &st, HotTable &h
 }
 
 
-template <int WARPS, int EPT, bool TMA, int DH>
-struct IngestSharedT
+struct IngestShared
 {
-	static constexpr int CHUNK = 32 * EPT;			// events per warp and round
-	static constexpr int KQ_CAP = EPT <= 2 ? 192 : 256, KQ_FLUSH = KQ_CAP - CHUNK;	// a flush leaves room for a whole chunk of RESP events
-	static constexpr int RQ_CAP = 32 + CHUNK;			// < 32 left over + one chunk
-	static_assert(CHUNK <= 128, "key queue sized for chunks of at most 128 events");
+	static constexpr int KQ_CAP = 192, KQ_FLUSH = KQ_CAP - IngestShape::CHUNK;	// a flush leaves room for a whole chunk of RESP events
+	static constexpr int RQ_CAP = 32 + IngestShape::CHUNK;		// < 32 left over + one chunk
+	static constexpr int DH = 1 << KEY_DIGIT_MAX;			// digit values of a RESP-key radix pass
 	struct Warp { unsigned long long kq[KQ_CAP]; IngestRec tcp[RQ_CAP], task[RQ_CAP]; };
-	alignas(128) uint4	evbuf[TMA ? WARPS * CHUNK * 2 : 1];	// per warp: its next chunk of 32-byte events, filled by cp.async.bulk
-	unsigned long long	mbar[TMA ? WARPS : 1];
-	Warp		w[WARPS];
-	uint32_t	dhist[OS_MAX_PASSES_VK][DH];			// digit histograms of this CTA's keys, one per radix pass (DH = 256 unless a pass has 9-bit digits)
+	Warp		w[IngestShape::WARPS];
+	uint32_t	dhist[OS_MAX_PASSES_VK][DH];			// digit histograms of this CTA's keys, one per radix pass
 };
 
-template <int WARPS, int MIN_CTAS, int EPT, bool TMA, int DH>
-__global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
+__global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
 		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt)
 {
-	using Shared = IngestSharedT<WARPS, EPT, TMA, DH>;
-	constexpr int CHUNK = Shared::CHUNK;
+	constexpr int WARPS = IngestShape::WARPS, EPT = IngestShape::EPT, CHUNK = IngestShape::CHUNK, DH = IngestShared::DH;
 	extern __shared__ __align__(128) unsigned char smem_raw[];
-	Shared &S = *reinterpret_cast<Shared *>(smem_raw);
+	IngestShared &S = *reinterpret_cast<IngestShared *>(smem_raw);
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	typename Shared::Warp &W = S.w[wid];
+	IngestShared::Warp &W = S.w[wid];
 	const uint32_t lt = (1u << lane) - 1u;
 	uint32_t c_in = 0, c_foreign = 0, n_resp = 0, n_active = 0;	// per thread: < 2^32 events per launch
 	uint32_t nk = 0, ntcp = 0, ntask = 0;				// queue lengths (warp-uniform)
 	unsigned long long t_tcp = 0, t_task = 0;			// queued in total (warp-uniform)
 
 	for (int i = threadIdx.x; i < OS_MAX_PASSES_VK * DH; i += WARPS * 32) (&S.dhist[0][0])[i] = 0;
-	if (TMA && lane == 0) mbar_init(&S.mbar[wid], 1);
 	__syncthreads();						// the only block barriers: here and before the retire step
-	if (TMA) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");	// mbarrier init visible to the async proxy
 
 	const uint64_t nchunks = (n + CHUNK - 1) / CHUNK;
 	const uint64_t nwarps = (uint64_t)gridDim.x * WARPS;
 	const uint64_t gwarp = (uint64_t)blockIdx.x * WARPS + wid;
-	uint4 *evw = S.evbuf + (TMA ? wid * CHUNK * 2 : 0);
-	uint32_t tma_phase = 0;
-	auto tma_issue = [&](uint64_t chunk) {
-		const uint64_t b0 = chunk * CHUNK;
-		const uint64_t cnt = n - b0 < (uint64_t)CHUNK ? n - b0 : (uint64_t)CHUNK;
-		// every lane's generic-proxy reads of the buffer happened before the __syncwarp that precedes this call
-		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-		tma_load_1d(evw, ev + b0, (uint32_t)cnt * 32u, &S.mbar[wid]);
-	};
-	if (TMA && lane == 0 && gwarp < nchunks) tma_issue(gwarp);
 
 	// ---- queue drains (all 32 lanes, m = multiple of 32 except in the final drain): handed as one coalesced run to the warp's
 	//      region of the batch's record queue, which the two drain_kernel passes apply after this kernel ----
@@ -374,22 +336,14 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState s
 	for (uint64_t chunk = gwarp; chunk < nchunks; chunk += nwarps) {
 		const uint64_t cbase = chunk * CHUNK;
 		uint4 ra[EPT], rb[EPT];
-		if (TMA) mbar_wait(&S.mbar[wid], tma_phase), tma_phase ^= 1u;
 #pragma unroll
 		for (int k = 0; k < EPT; ++k) {
 			const uint64_t i = cbase + (uint64_t)k * 32 + lane;
 			if (i < n) {
-				if (TMA) { ra[k] = evw[2 * (k * 32 + lane)]; rb[k] = evw[2 * (k * 32 + lane) + 1]; }
-				else {
-					ra[k] = __ldcs(reinterpret_cast<const uint4 *>(ev + i));		// streamed once: evict-first, keep L2 for
-					rb[k] = __ldcs(reinterpret_cast<const uint4 *>(ev + i) + 1);	// the id table / histogram / count-min lines
-				}
+				ra[k] = __ldcs(reinterpret_cast<const uint4 *>(ev + i));		// streamed once: evict-first, keep L2 for
+				rb[k] = __ldcs(reinterpret_cast<const uint4 *>(ev + i) + 1);	// the id table / histogram / count-min lines
 			}
 			else { ra[k] = make_uint4(0, 0, 0, 0); rb[k] = make_uint4(0, 0, 0, 0xFFFFu); }	// type 0xFFFF: padding, not counted
-		}
-		if (TMA) {
-			__syncwarp();								// the whole warp has copied its events out of the buffer
-			if (lane == 0 && chunk + nwarps < nchunks) tma_issue(chunk + nwarps);	// next chunk flies in while this one is processed
 		}
 
 		// decode; put the first id-table probe of all EPT events in flight before any of them is resolved
@@ -502,7 +456,7 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) ingest_kernel(DevState s
 
 		if (ntcp >= 32) { const uint32_t m = ntcp & ~31u; drain_tcp(m); keep_rest(W.tcp, m, ntcp); t_tcp += m; ntcp -= m; }
 		if (ntask >= 32) { const uint32_t m = ntask & ~31u; drain_task(m); keep_rest(W.task, m, ntask); t_task += m; ntask -= m; }
-		if (nk > (uint32_t)Shared::KQ_FLUSH) flush_keys();
+		if (nk > (uint32_t)IngestShared::KQ_FLUSH) flush_keys();
 	}
 	// what is left in the queues
 	if (ntcp) { drain_tcp(ntcp); t_tcp += ntcp; }
@@ -764,8 +718,7 @@ struct OneSweepSharedT
 template <int RBITS>
 __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned long long *__restrict__ in, unsigned long long *__restrict__ out,
 		const unsigned long long *__restrict__ d_n, DigitSpec D, const uint32_t *__restrict__ ghist /* [RADIX] of this pass */,
-		unsigned long long *__restrict__ status /* [ntiles][RADIX] */, uint32_t *__restrict__ ticket, uint32_t epoch,
-		int rank_mode /* 0 auto, 1 match.any, 2 ballots */)
+		unsigned long long *__restrict__ status /* [ntiles][RADIX] */, uint32_t *__restrict__ ticket, uint32_t epoch)
 {
 	constexpr int RADIX = 1 << RBITS;
 	constexpr int DPT = RADIX >= OS_THREADS ? RADIX / OS_THREADS : 1;	// digits per thread in the per-digit steps (threads >= RADIX idle there)
@@ -816,7 +769,9 @@ __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned l
 		float tot = 0.f;
 #pragma unroll
 		for (int w = 0; w < OS_WARPS; ++w) tot += S.fscan[w];
-		use_ballot = rank_mode == 2 || (rank_mode == 0 && tot > 10.f);
+		// every thread has the same tot; taking lane 0's choice costs one shuffle and cuts the kernel's local-memory spills by a
+		// third (ptxas -v)
+		use_ballot = __shfl_sync(0xffffffffu, (int)(tot > 10.f), 0);
 	}
 	const bool partial = (tile + 1) * (uint32_t)SORT_TILE > n;
 
@@ -930,9 +885,9 @@ __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned l
 struct RunRec { unsigned long long cw; unsigned long long us; };		// {samples : 27 | remainders : 37}, usec sum — as Bin
 struct BatchSeg { uint32_t run0, nruns; uint32_t key0, nkeys; };		// a touched service's runs in the pool / keys in the sorted array
 
+static constexpr int RM_THREADS = 256;
 static constexpr int RM_V = 8;	// keys per thread: positions wbase + t * 32 + lane; a CTA of RM_THREADS threads covers RM_THREADS * RM_V keys
 
-template <int RM_THREADS>
 __global__ void __launch_bounds__(RM_THREADS) runs_mark_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *__restrict__ d_n,
 		unsigned long long *__restrict__ status, uint32_t epoch, RunRec *__restrict__ pool, uint16_t *__restrict__ run_bin,
 		uint32_t *__restrict__ chunk_run, BatchSeg *__restrict__ segs /* [slot] */, uint32_t *__restrict__ touched, unsigned long long *ntouched,
@@ -1137,7 +1092,10 @@ __global__ void __launch_bounds__(256) runs_sum_kernel(const unsigned long long 
 	}
 }
 
-static constexpr int TD_WARPS = 3;		// warps (= services in flight) per CTA; work area per warp: 10.4 KB at 384 entries, 13.8 KB at 512
+static constexpr int TD_WARPS = 3;		// warps (= services in flight) per CTA
+// longest merged list (old centroids + batch items) that works in shared memory, 10.4 KB per warp: the smaller the work area, the
+// more services a SM has in flight (the kernel is latency-bound: a long chain of dependent warp instructions per service)
+static constexpr int TD_SMEM_N = 384;
 
 // One warp per touched service. Its runs become the batch's items {mean = exact usec sum / samples, weight = samples} — in value
 // order, because the bin index is monotone — and every run adds {samples, exact msec sum} to its bucket of the window histogram:
@@ -1145,14 +1103,11 @@ static constexpr int TD_WARPS = 3;		// warps (= services in flight) per CTA; wor
 // the batch's exact extremes. The items are then merged with the old centroids (old first on equal means) and the greedy K_1
 // pass cuts the list to at most TD_CAP clusters (warp_merge_compress). Lists of up to 2 x TD_CAP entries work in shared memory;
 // longer ones (a first batch can fill several hundred bins) in the warp's L2-resident scratch — same code, same result.
-// SMEM_N = longest merged list (old centroids + batch items) that works in shared memory: the smaller the work area, the more
-// services a SM has in flight (the kernel is latency-bound: a long chain of dependent warp instructions per service).
-template <int SMEM_N>
 __global__ void __launch_bounds__(TD_WARPS * 32) bins_merge_kernel(DevState st, const uint32_t *__restrict__ touched, const unsigned long long *__restrict__ ntouched_p,
 		const RunRec *__restrict__ pool, const uint16_t *__restrict__ run_bin, const BatchSeg *__restrict__ segs,
 		Centroid *__restrict__ items_scratch /* [nwarps][NBINS] */, TdWorkBig *__restrict__ big_scratch /* [nwarps] */)
 {
-	__shared__ TdWorkT<SMEM_N> work[TD_WARPS];
+	__shared__ TdWorkT<TD_SMEM_N> work[TD_WARPS];
 	// window histogram of the service's batch: 32-bit shared-memory atomics (native; a 64-bit shared atomicAdd is a CAS loop). A bucket's
 	// sample count of one batch fits 32 bits (max_batch < 2^27); the msec sum is kept as {low word, carries + high words}
 	__shared__ uint32_t hcnt[TD_WARPS][16], hsum_lo[TD_WARPS][16], hsum_hi[TD_WARPS][16];
@@ -1263,7 +1218,7 @@ __global__ void __launch_bounds__(TD_WARPS * 32) bins_merge_kernel(DevState st, 
 		TdHead head = st.td_head[slot];
 		Centroid *cent = st.td_cent + (size_t)slot * TD_CAP;
 		uint32_t nout;
-		if (head.n + nitems <= (uint32_t)SMEM_N) nout = warp_merge_compress(work[wid], cent, head.n, items, nitems, cent, st.td);
+		if (head.n + nitems <= (uint32_t)TD_SMEM_N) nout = warp_merge_compress(work[wid], cent, head.n, items, nitems, cent, st.td);
 		else nout = warp_merge_compress(big_scratch[gw], cent, head.n, items, nitems, cent, st.td);
 		if (lane == 0) {
 			head.n = nout;
@@ -1622,13 +1577,6 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 	return 1;
 }
 
-// GYSK_INGEST_VARIANT selects a shape of the warp-autonomous ingest kernel for A/B runs
-static int ingest_variant()
-{
-	static const int v = []{ const char *e = getenv("GYSK_INGEST_VARIANT"); return e ? atoi(e) : 0; }();
-	return v;
-}
-
 // GYSK_EXP_ABLATE: the SortPlan::exp bits, for timing runs only
 static int exp_ablate()
 {
@@ -1637,45 +1585,20 @@ static int exp_ablate()
 }
 
 // the radix passes of the RESP keys sort on {slot | bin} = key bits [30, 40 + slot bits): TD_CODE_BITS + slot bits significant
-// bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible (27 bits -> 7 7 7 6). A 9-bit pass
-// has two look-back rows per thread and nine ballots per key; GYSK_KEY_DIGIT_MAX=9 selects such digits (one pass fewer) for A/B runs.
+// bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible (27 bits -> 7 7 7 6). Not 9 bits, even
+// where that would save a pass: a 9-bit pass has two look-back rows per thread and nine ballots per key.
 static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
 {
 	int slot_bits = 1;
 	while (slot_bits < 24 && (1ull << slot_bits) < max_svcs) slot_bits++;
 	const int T = TD_CODE_BITS + slot_bits;
-	static const int dmax = []{ const char *e = getenv("GYSK_KEY_DIGIT_MAX"); const int v = e ? atoi(e) : 8; return v == 9 ? 9 : 8; }();
-	const int np = (T + dmax - 1) / dmax;
+	const int np = (T + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
 	if (np > OS_MAX_PASSES_VK) return -1;
 	int at = KEY_GROUP_SHIFT;
 	for (int p = 0; p < np; ++p) { P.bits[p] = T / np + (p < T % np ? 1 : 0); P.shift[p] = at; at += P.bits[p]; }
 	P.np = np;
 	P.exp = exp_ablate();
 	return np;
-}
-
-template <int WARPS, int MIN_CTAS, int EPT, bool TMA, int DH>
-static int launch_ingest_variant(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, const SortPlan &plan, RecRegions &rr,
-		int dev, cudaStream_t s)
-{
-	using Shared = IngestSharedT<WARPS, EPT, TMA, DH>;
-	static_assert(WARPS * MIN_CTAS <= INGEST_MAX_WARPS_PER_SM && WARPS * MIN_CTAS * Shared::CHUNK <= INGEST_MAX_CHUNK_EVENTS_PER_SM,
-			"the record queue is sized for a smaller grid");
-	static bool attr_set[MAX_DEVICES] = {};
-	if (!attr_set[dev]) {
-		cudaFuncSetAttribute(ingest_kernel<WARPS, MIN_CTAS, EPT, TMA, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Shared));
-		attr_set[dev] = true;
-	}
-	const uint64_t want = (n + (uint64_t)Shared::CHUNK * WARPS - 1) / ((uint64_t)Shared::CHUNK * WARPS);
-	const uint64_t full = (uint64_t)sm_count(dev) * MIN_CTAS;
-	const uint32_t grid = (uint32_t)(want < full ? want : full);
-	// the kernel computes the same regions from its grid
-	const uint64_t nchunks = (n + Shared::CHUNK - 1) / Shared::CHUNK;
-	rr.nwarps = grid * WARPS;
-	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * Shared::CHUNK;
-	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
-	ingest_kernel<WARPS, MIN_CTAS, EPT, TMA, DH><<<grid, WARPS * 32, sizeof(Shared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt);
-	return 1;
 }
 
 int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s)
@@ -1689,25 +1612,22 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	// key cursor, digit histograms and tile tickets of this batch's sort
 	cudaMemsetAsync(st.counters + CTR_NKEYS, 0, sizeof(unsigned long long), s);
 	cudaMemsetAsync(tmp.os_ghist, 0, (OS_MAX_PASSES * RADIX_MAX + OS_MAX_PASSES) * sizeof(uint32_t), s);
-	bool wide = false;
-	for (int p = 0; p < plan.np; ++p) wide |= plan.bits[p] > 8;
-	int rc;
-#define GYSK_LI2(W, C, E, T, D) rc = launch_ingest_variant<W, C, E, T, D>(st, tmp, d_ev, n, plan, rr, dev, s)
-#define GYSK_LI(W, C, E, T) do { if (wide) GYSK_LI2(W, C, E, T, 512); else GYSK_LI2(W, C, E, T, 256); } while (0)
-	switch (ingest_variant()) {
-	case 842 : GYSK_LI(8, 4, 2, false); break;
-	case 852 : GYSK_LI(8, 5, 2, false); break;
-	case 834 : GYSK_LI(8, 3, 4, false); break;
-	case 844 : GYSK_LI(8, 4, 4, false); break;
-	case 832 : GYSK_LI(8, 3, 2, false); break;
-	case 482 : GYSK_LI(4, 8, 2, false); break;
-	case 1832 : GYSK_LI(8, 3, 2, true); break;	// TMA-staged chunks
-	case 1834 : GYSK_LI(8, 3, 4, true); break;
-	default : GYSK_LI(8, 3, 2, false); break;
+	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
+	static bool attr_set[MAX_DEVICES] = {};
+	if (!attr_set[dev]) {
+		cudaFuncSetAttribute(ingest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		attr_set[dev] = true;
 	}
-#undef GYSK_LI
-#undef GYSK_LI2
-	return rc;
+	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
+	const uint64_t full = (uint64_t)sm_count(dev) * IngestShape::MIN_CTAS;
+	const uint32_t grid = (uint32_t)(want < full ? want : full);
+	// the kernel computes the same regions from its grid
+	const uint64_t nchunks = (n + CHUNK - 1) / CHUNK;
+	rr.nwarps = grid * WARPS;
+	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
+	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
+	ingest_kernel<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt);
+	return 1;
 }
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
@@ -1769,15 +1689,6 @@ static int build_digit_specs(int lo1, int hi1, int lo2, int hi2, DigitSpecs &P)
 	return (p1 < hi1 || p2 < hi2) ? -1 : 0;		// more than 64 significant bits cannot happen
 }
 
-// host-side view of the pass plan (C ABI: gysk_sort_plan): per pass {shift1, bits1, shift2, bits2}
-int radix_sort_plan(int lo1, int hi1, int lo2, int hi2, int out[][4], int cap)
-{
-	DigitSpecs P;
-	if (build_digit_specs(lo1, hi1, lo2, hi2, P)) return -1;
-	for (int p = 0; p < P.np && p < cap; ++p) { out[p][0] = P.d[p].s1; out[p][1] = P.d[p].b1; out[p][2] = P.d[p].s2; out[p][3] = P.d[p].b2; }
-	return P.np;
-}
-
 static void os_set_attrs(int dev)
 {
 	static bool attr_set[MAX_DEVICES] = {};
@@ -1801,21 +1712,17 @@ static uint32_t next_epoch(const SortTemp &tmp, uint32_t max_tiles, cudaStream_t
 	return e;
 }
 
-static const int g_rank_mode = []{ const char *e = getenv("GYSK_OS_RANK"); return e ? atoi(e) : 0; }();
-
 // one radix pass with the kernel instantiation of the digit's width: a 7-bit digit has half the per-digit work (per-warp counters to
-// clear and prefix, status words to publish and look back through, ballots per key) of an 8-bit one
+// clear and prefix, status words to publish and look back through, ballots per key) of an 8-bit one. The grid is persistent
+// (os_pass_kernel): at most as many CTAs as the SMs hold at once, whatever the number of possible tiles.
 static void launch_os_pass(int bits, uint32_t ntiles, const unsigned long long *in, unsigned long long *out, const unsigned long long *d_n, const DigitSpec &D,
 		const uint32_t *ghist, unsigned long long *status, uint32_t *ticket, uint32_t epoch, cudaStream_t s)
 {
-	static const bool narrow = []{ const char *e = getenv("GYSK_OS_NARROW"); return !e || atoi(e) != 0; }();
-	// GYSK_OS_PERSIST=0: one CTA per possible tile (A/B runs)
-	static const bool persist = []{ const char *e = getenv("GYSK_OS_PERSIST"); return !e || atoi(e) != 0; }();
-	if (persist) ntiles = std::min<uint32_t>(ntiles, (uint32_t)sm_count(current_device()) * 4u);		// __launch_bounds__(OS_THREADS, 4)
-	if (bits > 8) os_pass_kernel<9><<<ntiles, OS_THREADS, sizeof(OneSweepSharedT<9>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch, g_rank_mode);
-	else if (bits == 8 || !narrow) os_pass_kernel<8><<<ntiles, OS_THREADS, sizeof(OneSweepSharedT<8>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch, g_rank_mode);
-	else if (bits == 7) os_pass_kernel<7><<<ntiles, OS_THREADS, sizeof(OneSweepSharedT<7>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch, g_rank_mode);
-	else os_pass_kernel<6><<<ntiles, OS_THREADS, sizeof(OneSweepSharedT<6>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch, g_rank_mode);
+	const uint32_t grid = std::min<uint32_t>(ntiles, (uint32_t)sm_count(current_device()) * 4u);		// __launch_bounds__(OS_THREADS, 4)
+	if (bits > 8) os_pass_kernel<9><<<grid, OS_THREADS, sizeof(OneSweepSharedT<9>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
+	else if (bits == 8) os_pass_kernel<8><<<grid, OS_THREADS, sizeof(OneSweepSharedT<8>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
+	else if (bits == 7) os_pass_kernel<7><<<grid, OS_THREADS, sizeof(OneSweepSharedT<7>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
+	else os_pass_kernel<6><<<grid, OS_THREADS, sizeof(OneSweepSharedT<6>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
 }
 
 // stable LSD radix sort of the *d_n keys in keys_a on their own bits (plain mode, the top-N sorts): n_max >= *d_n sizes the grids
@@ -1843,9 +1750,7 @@ int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64
 	else os_hist_kernel<8, 257><<<hgrid, 512, (size_t)P.np * copies * stride * sizeof(uint32_t), s>>>(bufs[w], d_n, P, ghist);
 	launches++;
 	for (int p = 0; p < P.np; ++p) {
-		const bool nine = P.d[p].b1 + P.d[p].b2 > 8;
 		const uint32_t epoch = next_epoch(tmp, tmp.max_tiles, s);
-		(void)nine;
 		launch_os_pass(P.d[p].b1 + P.d[p].b2, ntiles, bufs[w], bufs[w ^ 1], d_n, P.d[p], ghist + p * RADIX_MAX, tmp.tile_status, tickets + p, epoch, s);
 		launches++;
 		w ^= 1;
@@ -1884,20 +1789,11 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 
 	cudaMemsetAsync(d_ntouched, 0, sizeof(unsigned long long), s);
 	const uint32_t epoch = next_epoch(tmp, tmp.max_tiles, s);
-	// GYSK_RM_THREADS=512: tiles of 4096 keys (half the look-back steps) — A/B runs
-	static const int rm_threads = []{ const char *e = getenv("GYSK_RM_THREADS"); return e && atoi(e) == 512 ? 512 : 256; }();
-#define RM_ARGS src, d_nkeys, tmp.tile_status, epoch, reinterpret_cast<RunRec *>(tmp.pool), tmp.run_bin, tmp.chunk_run, \
-		reinterpret_cast<BatchSeg *>(tmp.segs), tmp.touched, d_ntouched, st.counters + CTR_NRUNS
-	if (rm_threads == 256) runs_mark_kernel<256><<<div_up(n_events, 256 * RM_V), 256, 0, s>>>(RM_ARGS);
-	else runs_mark_kernel<512><<<div_up(n_events, 512 * RM_V), 512, 0, s>>>(RM_ARGS);
-#undef RM_ARGS
+	runs_mark_kernel<<<div_up(n_events, RM_THREADS * RM_V), RM_THREADS, 0, s>>>(src, d_nkeys, tmp.tile_status, epoch, reinterpret_cast<RunRec *>(tmp.pool),
+			tmp.run_bin, tmp.chunk_run, reinterpret_cast<BatchSeg *>(tmp.segs), tmp.touched, d_ntouched, st.counters + CTR_NRUNS);
 	runs_sum_kernel<<<nsm * 8, 256, 0, s>>>(src, d_nkeys, tmp.chunk_run, reinterpret_cast<RunRec *>(tmp.pool));
-	// GYSK_MERGE_SMEM_N=512 selects the larger work area (A/B runs)
-	static const int merge_smem_n = []{ const char *e = getenv("GYSK_MERGE_SMEM_N"); return e && atoi(e) == 512 ? 512 : 384; }();
-	const int merge_ctas = std::min(nsm, TD_MERGE_MAX_SMS) * (merge_smem_n == 512 ? 5 : TD_MERGE_CTAS_PER_SM);
-	if (merge_smem_n == 512) bins_merge_kernel<512><<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, tmp.touched, d_ntouched,
-			reinterpret_cast<const RunRec *>(tmp.pool), tmp.run_bin, reinterpret_cast<const BatchSeg *>(tmp.segs), tmp.items_scratch, tmp.big_scratch);
-	else bins_merge_kernel<384><<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, tmp.touched, d_ntouched,
+	const int merge_ctas = std::min(nsm, TD_MERGE_MAX_SMS) * TD_MERGE_CTAS_PER_SM;
+	bins_merge_kernel<<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, tmp.touched, d_ntouched,
 			reinterpret_cast<const RunRec *>(tmp.pool), tmp.run_bin, reinterpret_cast<const BatchSeg *>(tmp.segs), tmp.items_scratch, tmp.big_scratch);
 	return launches + 3;
 }

@@ -64,8 +64,8 @@ struct SortTemp
 							// ingest launch owns region [w * cap, (w + 1) * cap) (RecRegions): its connection records from
 							// the front, its process records from the back, stored at warp-local offsets without any atomic
 	uint2			*rec_cnt;		// [rec_cnt_cap] {connection, process} records of each region, written by every warp of the launch
-	uint64_t		recq_cap;		// max_batch + the regions' rounding (INGEST_MAX_CHUNK_EVENTS_PER_SM per SM)
-	uint32_t		rec_cnt_cap;		// INGEST_MAX_WARPS_PER_SM per SM
+	uint64_t		recq_cap;		// max_batch + the regions' rounding (one chunk per warp of a full ingest grid)
+	uint32_t		rec_cnt_cap;		// warps of a full ingest grid
 	uint32_t		max_tiles;
 };
 
@@ -73,9 +73,10 @@ struct SortTemp
 // warp can queue (chunks are dealt to the warps round-robin)
 struct RecRegions { uint32_t nwarps; uint64_t cap; };
 
-// the largest grid of any ingest_kernel launch shape (GYSK_INGEST_VARIANT), per SM: warps, and warps x events per chunk. They size
-// the record queue beyond max_batch; launch_ingest checks every launch against the buffers.
-static constexpr uint32_t INGEST_MAX_WARPS_PER_SM = 40, INGEST_MAX_CHUNK_EVENTS_PER_SM = 4096;
+// launch shape of ingest_kernel: warps per CTA, CTAs per SM (the full grid, and __launch_bounds__), events per lane and chunk
+// (DESIGN.md §7 has the measurements). It also sizes the record queue beyond max_batch; launch_ingest checks every launch against
+// the buffers.
+struct IngestShape { static constexpr int WARPS = 8, MIN_CTAS = 3, EPT = 2, CHUNK = 32 * EPT; };
 
 // raw per-id record gathered for queries / exports
 struct SvcRaw
@@ -119,7 +120,6 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
 int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo1, int hi1, int lo2, int hi2, int *which, cudaStream_t s);
-int radix_sort_plan(int lo1, int hi1, int lo2, int hi2, int out[][4], int cap);
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int metric, int host_filter, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
 int launch_topn_tasks(const DevState &st, const SortTemp &tmp, uint32_t ntasks, int metric, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
 int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s);

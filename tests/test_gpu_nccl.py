@@ -92,9 +92,10 @@ def test_nccl_two_gpu_merge():
 
 def test_two_engines_on_two_devices_in_one_process():
     """the deployment INTEGRATION.md describes: ONE process owns an engine per GPU. cudaFuncSetAttribute is per device, so the
-    second engine must get its own opt-in for the large dynamic shared memory of ingest_kernel / os_pass_kernel<9> — drive a
-    9-bit-digit sort (max_svcs 2^17 -> 9 + 9 + 9) and a plain top-N sort on BOTH devices and compare with the oracle; then merge
-    the two engines with a caller-made communicator (ncclCommInitAll equivalent: two comms from one unique id, one per thread)."""
+    second engine must get its own opt-in for the large dynamic shared memory of ingest_kernel / os_pass_kernel<9> — drive the
+    batch's key sort (max_svcs 2^17 -> 7 + 7 + 7 + 6-bit digits) and a plain top-N sort on BOTH devices and compare with the
+    oracle; then merge the two engines with a caller-made communicator (ncclCommInitAll equivalent: two comms from one unique id,
+    one per thread); last, a group-by of more than 2^16 samples on both devices (17 group bits: a 9-bit and an 8-bit pass)."""
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
@@ -156,3 +157,10 @@ def test_two_engines_on_two_devices_in_one_process():
             members = sids[logical == lid]
             tot = sum(h[1] for h in (one.export_hist(int(m), 1) for m in members) if h is not None)
             assert o["nqrys_5s"] == tot
+    from gyeeta_b200 import wire
+    from tests.test_gpu_boundary import _proc_samples
+    s = _proc_samples(rng, 100_000, 20_000)                    # n <= max_batch (2^18)
+    want = po.task_groupby(s, wire.TASK)
+    for e_ in engs:
+        got, ng = e_.task_groupby(s)
+        assert ng == len(want) and got.tobytes() == want.tobytes()

@@ -1,18 +1,13 @@
-"""The connection / process record queue of ingest_kernel at batch sizes where every warp takes several chunks, and every launch
-shape and sort switch of the library, against the CPU oracle.
+"""The connection / process record queue of ingest_kernel at batch sizes where every warp takes several chunks, against the CPU
+oracle.
 
 ingest_kernel deals its chunks of 32 x EPT events to the warps round-robin. Each warp owns one region of the batch's record queue,
 rcap = ceil(chunks / warps) x CHUNK entries: connection (TCP) records grow from its front, process (TASK) records from its back, and
 the drain_kernel passes find each region's groups of 32 records through a table built from the per-warp counts (DESIGN.md §4). Below
-one full grid of chunks (nsm x MIN_CTAS x WARPS of them, about 200 000 events for the default shape on an H100) every region holds
-at most one chunk, so the batches here are sized in chunks relative to that grid, from the device's SM count and the active shape.
-
-The shape and the sort switches are read once per process, so test_every_shape_and_switch re-runs these tests and a set of parity
-tests in a child process per setting; test_switch_list_is_complete (no GPU) keeps that list in step with the sources."""
+one full grid of chunks (nsm x MIN_CTAS x WARPS of them, about 200 000 events on an H100) every region holds at most one chunk, so
+the batches here are sized in chunks relative to that grid, from the device's SM count and the launch shape (IngestShape)."""
 import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -24,19 +19,10 @@ from tests.util import assert_hist_equal, make_pair
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "gyeeta_b200", "csrc")
 
-# GYSK_INGEST_VARIANT -> (WARPS, MIN_CTAS, EPT, TMA): the `switch (ingest_variant())` of launch_ingest; unset or unknown = 832
-SHAPES = {832: (8, 3, 2, False), 842: (8, 4, 2, False), 852: (8, 5, 2, False), 834: (8, 3, 4, False), 844: (8, 4, 4, False),
-          482: (4, 8, 2, False), 1832: (8, 3, 2, True), 1834: (8, 3, 4, True)}
-DEFAULT_VARIANT = 832
+# ingest_kernel's launch shape, IngestShape in gysk_kernels.cuh (test_ingest_shape_matches_the_sources keeps the two equal)
+WARPS, MIN_CTAS, EPT = 8, 3, 2
 
-# every launch shape and sort switch; test_every_shape_and_switch runs the tests below once per entry
-SETTINGS = [{"GYSK_INGEST_VARIANT": str(v)} for v in (832, 842, 852, 834, 844, 482, 1832, 1834)] + [
-    {"GYSK_KEY_DIGIT_MAX": "9"},                                   # 9-bit digits: os_pass_kernel<9>, ingest_kernel with DH = 512
-    {"GYSK_KEY_DIGIT_MAX": "9", "GYSK_INGEST_VARIANT": "1834"},    # ... in ingest_kernel's largest shared-memory layout
-    {"GYSK_OS_RANK": "1"}, {"GYSK_OS_RANK": "2"},                  # one ranking code in every radix tile (the default picks per tile)
-    {"GYSK_OS_NARROW": "0"}, {"GYSK_OS_PERSIST": "0"}, {"GYSK_RM_THREADS": "512"}, {"GYSK_MERGE_SMEM_N": "512"},
-]
-# switches that are not in SETTINGS, and why
+# every GYSK_ string the library reads from the environment, and why no test here sets it
 NOT_RUN = {
     "GYSK_EXP_ABLATE": "timing runs only: each bit skips part of the work, so the results are wrong by definition",
     "GYSK_HOT_ROWS": "read per engine, so a test can set it: tests/test_gpu_hot_rows.py",
@@ -44,11 +30,6 @@ NOT_RUN = {
     "GYSK_HOT_MAX": "read per engine, so a test can set it: tests/test_gpu_hot_rows.py",
     "GYSK_HOT_BIN_MAX": "read per engine, so a test can set it: tests/test_gpu_hot_rows.py",
 }
-# what each child process runs besides this file's region tests
-PARITY_TESTS = ["tests/test_gpu_parity.py::test_mixed_stream_bit_exact", "tests/test_gpu_parity.py::test_full_value_range_keys",
-                "tests/test_gpu_parity.py::test_topn_services_last_window",
-                "tests/test_gpu_hot_rows.py::test_hot_rows_are_taken_and_every_batch_is_bit_exact"]
-CHILD_TIMEOUT_S = 1800
 
 NSVC, NTASK = 2000, 500
 TIDS = synth.task_ids(NTASK)
@@ -59,18 +40,13 @@ COUNTERS = (("events_in", "in"), ("events_dropped", "dropped"), ("events_resp", 
 TASK_HISTS = (ge.HIST_TASK_CPU_PCT, ge.HIST_TASK_CPU_DELAY, ge.HIST_TASK_BLKIO_DELAY)
 
 
-def _setting_id(s):
-    return ",".join(f"{k}={v}" for k, v in s.items())
-
-
 # ---------------------------------------------------------------------------------------------------------------------------
-# geometry of the record regions, as launch_ingest_variant and ingest_kernel compute it
+# geometry of the record regions, as launch_ingest and ingest_kernel compute it
 # ---------------------------------------------------------------------------------------------------------------------------
 class Geometry:
-    def __init__(self, nsm, variant):
+    def __init__(self, nsm):
         self.nsm = nsm
-        self.warps, self.min_ctas, self.ept, self.tma = SHAPES.get(variant, SHAPES[DEFAULT_VARIANT])
-        self.chunk = 32 * self.ept
+        self.warps, self.min_ctas, self.chunk = WARPS, MIN_CTAS, 32 * EPT
         self.full = nsm * self.min_ctas * self.warps           # warps of a full grid (N)
 
     def regions(self, n):
@@ -91,17 +67,10 @@ class Geometry:
         return n1, n2, n3
 
 
-def _variant():
-    try:
-        return int(os.environ.get("GYSK_INGEST_VARIANT", "0"))
-    except ValueError:
-        return 0
-
-
 @pytest.fixture(scope="module")
 def geo():
     import torch
-    return Geometry(torch.cuda.get_device_properties(0).multi_processor_count, _variant())
+    return Geometry(torch.cuda.get_device_properties(0).multi_processor_count)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -258,7 +227,7 @@ class Pair:
 @pytest.mark.gpu
 def test_mixed_stream_several_chunks_per_warp(geo):
     """(a) the mixed stream in batches of N + 1, 2 N and 3.5 N chunks, flushed between windows. 65 536 services: 26 sort-key bits,
-    so GYSK_KEY_DIGIT_MAX=9 sorts in 9/9/8-bit passes (8-bit digits: 7/7/6/6)."""
+    sorted in 7/7/6/6-bit passes."""
     n1, n2, n3 = geo.sizes()
     rng = np.random.default_rng(101)
     p = Pair(max_batch=n3, max_svcs=1 << 16)
@@ -345,23 +314,8 @@ def test_sharded_mixed_stream_skips_empty_regions(geo):
     assert sum(p.eng.stats()["events_in"] for p in pairs) == sum(len(b) for b in batches)
 
 
+# the sources
 # ---------------------------------------------------------------------------------------------------------------------------
-# every launch shape and sort switch
-# ---------------------------------------------------------------------------------------------------------------------------
-@pytest.mark.gpu
-@pytest.mark.parametrize("setting", SETTINGS, ids=[_setting_id(s) for s in SETTINGS])
-def test_every_shape_and_switch(setting):
-    """the region tests above and the parity tests of PARITY_TESTS in a child process with the setting in its environment (the
-    library reads these switches once per process); one run, the child's output in the failure message"""
-    env = {k: v for k, v in os.environ.items() if not k.startswith("GYSK_")}
-    env.update(setting)
-    env["PYTHONDONTWRITEBYTECODE"] = "1"
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \
-        ["-m", "pytest", "-q", "-x", "-m", "gpu", "-p", "no:cacheprovider", "tests/test_gpu_record_regions.py", "-k", "not every_shape"] + PARITY_TESTS
-    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=CHILD_TIMEOUT_S)
-    assert r.returncode == 0, f"{_setting_id(setting)}: the child exited with {r.returncode}\n{r.stdout[-12000:]}\n{r.stderr[-4000:]}"
-
-
 def _sources():
     out = {}
     for f in sorted(os.listdir(CSRC)):
@@ -371,60 +325,20 @@ def _sources():
     return out
 
 
-def _variant_cases(src):
-    """{label: (WARPS, MIN_CTAS, EPT, TMA)} of the case lines of `switch (ingest_variant())`, and the default's shape"""
-    i = src.index("switch (ingest_variant())")
-    body = src[i: src.index("default", i)]
-    line = r"\s*:\s*GYSK_LI\(\s*(\d+)\s*,\s*(\d+)\s*,\s*(\d+)\s*,\s*(true|false)\s*\)"
-    cases = {int(c): (int(w), int(m), int(e), t == "true") for c, w, m, e, t in re.findall(r"case\s+(\d+)" + line, body)}
-    assert len(cases) == body.count("case "), "a case line of the switch does not have the expected form"
-    w, m, e, t = re.search(r"default" + line, src[i:]).groups()
-    return cases, (int(w), int(m), int(e), t == "true")
+def test_ingest_shape_matches_the_sources():
+    """the shape Geometry sizes the batches with is IngestShape, so they still hit N + 1, 2 N and 3.5 N chunks"""
+    m = re.search(r"struct IngestShape\s*\{([^}]*)\}", _sources()["gysk_kernels.cuh"])
+    assert m, "IngestShape not found in gysk_kernels.cuh"
+    shape = {k: int(v) for k, v in re.findall(r"\b(WARPS|MIN_CTAS|EPT)\s*=\s*(\d+)", m.group(1))}
+    assert shape == {"WARPS": WARPS, "MIN_CTAS": MIN_CTAS, "EPT": EPT}, shape
+    assert re.search(r"\bCHUNK\s*=\s*32\s*\*\s*EPT\b", m.group(1))
+    Geometry(132).sizes()                # the batch sizes of an H100 land where the region tests want them
 
 
-def _selecting_values(src):
-    """switch -> the values that select its other code path, read off the line that reads it (`== 9` selects 9, `!= 0` is
-    switched off by 0); for GYSK_OS_RANK the modes other than 0 (auto) that the radix pass's rank_mode parameter documents"""
-    out = {}
-    for ln in src.splitlines():
-        m = re.search(r'getenv\("(GYSK_\w+)"\)', ln)
-        if m and re.findall(r"[!=]= (\d+)", ln[m.end():]):
-            out[m.group(1)] = set(re.findall(r"[!=]= (\d+)", ln[m.end():]))
-    modes = re.search(r"int rank_mode\s*/\*([^*]*)\*/", src)
-    assert modes and "GYSK_OS_RANK" in src
-    out["GYSK_OS_RANK"] = set(re.findall(r"(\d+) ", modes.group(1))) - {"0"}
-    return out
-
-
-def test_switch_list_is_complete():
-    """every ingest shape (case label) and every GYSK_ switch the library reads is in SETTINGS or, with its reason, in NOT_RUN;
-    SHAPES equals the template arguments of the case lines"""
-    srcs = _sources()
-    allsrc = "\n".join(srcs.values())
-    run = {}
-    for s in SETTINGS:
-        for k, v in s.items():
-            run.setdefault(k, set()).add(v)
-    # launch shapes
-    cases, default = _variant_cases(srcs["gysk_kernels.cu"])
-    assert cases == SHAPES, (cases, SHAPES)
-    assert default == SHAPES[DEFAULT_VARIANT]
-    missing = [v for v in cases if {"GYSK_INGEST_VARIANT": str(v)} not in SETTINGS]
-    assert not missing, f"ingest shapes not run on their own: {sorted(missing)}"
-    assert {int(v) for v in run["GYSK_INGEST_VARIANT"]} <= set(cases)
-    # switches: every name in a string literal of the sources is an environment switch (getenv and the engine's envl helper)
-    names = set(re.findall(r'"(GYSK_[A-Z0-9_]+)"', allsrc))
-    assert "GYSK_INGEST_VARIANT" in names and len(names) >= 10
-    unlisted = names - set(run) - set(NOT_RUN)
-    assert not unlisted, f"switches neither run nor excluded: {sorted(unlisted)}"
-    assert not set(run) & set(NOT_RUN)
-    assert set(run) | set(NOT_RUN) <= names, f"listed switches the library does not read: {sorted(set(run) | set(NOT_RUN) - names)}"
-    # each switch is run with every value that changes what the library does
-    for name, vals in _selecting_values(allsrc).items():
-        if name in NOT_RUN:
-            continue
-        assert vals <= run.get(name, set()), f"{name}: values {sorted(vals - run.get(name, set()))} never run"
-        assert all({name: v} in SETTINGS for v in vals), f"{name} is not run on its own"
-    # 9-bit digits also with the TMA-staged shape of the widest chunks: ingest_kernel's largest shared-memory layout
-    widest_tma = max((v for v, s in SHAPES.items() if s[3]), key=lambda v: SHAPES[v][2])
-    assert {"GYSK_KEY_DIGIT_MAX": "9", "GYSK_INGEST_VARIANT": str(widest_tma)} in SETTINGS, "9-bit digits with the largest ingest layout"
+def test_every_switch_is_listed_with_its_reason():
+    """every GYSK_ string literal of the sources (getenv and the engine's envl helper) is in NOT_RUN with its reason: a new
+    process-wide switch fails here until it comes with one"""
+    names = set(re.findall(r'"(GYSK_[A-Z0-9_]+)"', "\n".join(_sources().values())))
+    assert names, "no GYSK_ switch found in the sources"
+    assert names == set(NOT_RUN), f"unlisted: {sorted(names - set(NOT_RUN))}, no longer read: {sorted(set(NOT_RUN) - names)}"
+    assert all(NOT_RUN.values())

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from gyeeta_b200 import engine as ge
-from tests.test_gpu_record_regions import TIDS, Geometry, Pair, _tcp, _variant
+from tests.test_gpu_record_regions import TIDS, Geometry, Pair, _tcp
 
 BIG = 1 << 31
 
@@ -17,7 +17,7 @@ BIG = 1 << 31
 @pytest.fixture(scope="module")
 def geo():
     import torch
-    return Geometry(torch.cuda.get_device_properties(0).multi_processor_count, _variant())
+    return Geometry(torch.cuda.get_device_properties(0).multi_processor_count)
 
 
 def _task_events(n, ids, value, cpu_delay, blkio, rng):
