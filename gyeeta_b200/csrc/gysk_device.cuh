@@ -301,10 +301,16 @@ __device__ __forceinline__ int table_resolve_slow(const IdTable &t, unsigned lon
 		if (k == 0) {
 			if (!insert) return -1;
 			// no slot left (nothing on the free stack, every fresh one handed out): give up BEFORE claiming the entry, so a
-			// full engine does not fill its table with dead keys (unknown ids keep arriving: one per netns/ip/port on the raw path)
-			if ((!t.free_n || *((volatile int32_t *)t.free_n) <= 0) && *((volatile uint32_t *)t.count) >= t.max_slots) return -1;
-			k = atomicCAS(&e->key, 0ull, key);
-			if (k == 0) {
+			// full engine does not fill its table with dead keys (unknown ids keep arriving: one per netns/ip/port on the raw path).
+			// The entry was empty when probed, but another event of this same id may have claimed it since and taken the last
+			// slot — the one that filled the table: look again before dropping the event (every successful claim precedes the
+			// slot-count add that made the table full, so its key is visible by now)
+			if ((!t.free_n || *((volatile int32_t *)t.free_n) <= 0) && *((volatile uint32_t *)t.count) >= t.max_slots) {
+				__threadfence();
+				k = *((volatile unsigned long long *)&e->key);
+				if (k == 0) return -1;
+			}
+			else if ((k = atomicCAS(&e->key, 0ull, key)) == 0) {
 				// a slot recycled by an eviction first, else the next fresh one
 				uint32_t s = SLOT_INVALID;
 				if (t.free_n) {

@@ -96,7 +96,7 @@ __global__ void fold_hll_kernel(DevState st, const uint32_t *__restrict__ offs, 
 
 static constexpr int MG_WARPS = 2;		// 2 x 17.8 KB of scratch: static shared memory
 
-// one warp per logical service: fold member digests one after the other (member order = slot order of the map call)
+// one warp per logical service: fold member digests one after the other (member order = the order of the map call's list)
 __global__ void __launch_bounds__(MG_WARPS * 32) fold_td_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members,
 		uint32_t nl, uint32_t null_slot, SlabEntry *__restrict__ slab)
 {

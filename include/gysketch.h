@@ -198,7 +198,7 @@ typedef struct gysk_config
 	uint32_t	cms_depth;		/* rows, 1..8 (default 4) */
 	uint32_t	cms_log2_width;		/* columns = 1 << this (default 20) */
 	uint32_t	hll_p;			/* registers per service = 1 << p, 4..16 (default 12) */
-	uint32_t	td_compression;		/* t-digest delta, 10..220 (default 200: up to 256 centroids kept; exports for Postgres are
+	uint32_t	td_compression;		/* t-digest delta, 10..256 (default 200: up to 256 centroids kept; exports for Postgres are
 						   recompressed to public.tdigest(x, 100), gy_query_common.cc:1855) */
 	uint32_t	max_batch;		/* max events per device batch = one ingest + merge pass, < 2^27 (default 1 << 22) */
 	uint32_t	flags;			/* GYSK_FLAG_* */

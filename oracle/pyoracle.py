@@ -80,6 +80,8 @@ def lib():
         L.gyo_hll_estimate.restype = C.c_double
         L.gyo_hll_estimate.argtypes = [C.c_void_p, C.c_uint32]
         L.gyo_td_init.argtypes = [C.c_void_p]
+        L.gyo_td_compress.restype = C.c_uint32
+        L.gyo_td_compress.argtypes = [C.c_void_p, C.c_uint32, C.c_double, C.c_void_p, C.c_uint32]
         L.gyo_td_add_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_double]
         L.gyo_td_add_classic.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_double]
         L.gyo_td_quantile.restype = C.c_double
@@ -272,6 +274,14 @@ def td_new():
     td = TDigest()
     lib().gyo_td_init(C.byref(td))
     return td
+
+
+def td_compress(cent, delta, cap=TD_CAP):
+    """gyo_td_compress: one K_1 pass over a mean-sorted CENTROID_DTYPE list -> at most cap centroids"""
+    cent = np.ascontiguousarray(cent, dtype=CENTROID_DTYPE)
+    out = np.zeros(cap, dtype=CENTROID_DTYPE)
+    n = lib().gyo_td_compress(_p(cent), len(cent), float(delta), _p(out), cap)
+    return out[: min(n, cap)].copy()
 
 
 def td_add(td, vals, delta=200.0, classic=False):
