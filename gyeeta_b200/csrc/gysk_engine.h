@@ -21,6 +21,7 @@ namespace gysk {
 
 constexpr int NBUF = 2;
 constexpr uint32_t QCHUNK = 1024;		// ids per query kernel launch
+constexpr uint32_t WIN_ROWS = 8192;		// rows per pass of a window read (the page-locked stage holds WIN_ROWS service rows)
 constexpr uint32_t THREAD_STAGE_EVENTS = 1u << 16;	// events per per-thread staging chunk (2 MB page-locked, two chunks per thread)
 constexpr uint32_t RAW_BULK_MIN = 16384;		// raw fixed-stride batches from this size on are expanded on the device: below it the
 							// per-call copy / launch / event calls under the engine mutex cost more than the
@@ -151,6 +152,9 @@ struct gysk_engine
 	int32_t			*d_found {nullptr}, *h_found {nullptr};
 	gysk_flow_est		*d_flowout {nullptr}, *h_flowout {nullptr};
 	unsigned long long	*h_counters {nullptr};
+	uint8_t			*d_wstage {nullptr}, *h_wstage {nullptr};	// window reads / gysk_query_tasks: WIN_ROWS rows per pass
+	std::vector<uint64_t>	win_keys, win_ids;			// a window read's {host | slot} keys and their ids on the host
+	std::vector<std::pair<uint64_t, uint64_t>> win_rows;		// ... as {id, slot}, ordered within each host
 
 	// optional per-kernel timing
 	bool			profiling {false};

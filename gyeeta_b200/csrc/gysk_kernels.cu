@@ -15,8 +15,10 @@
 //   state_kernel         listener state of the closed window (get_curr_state)          common/gy_socket_stat.cc:2020-2875
 //   evict_kernel         idle listeners leave, slots recycled                          common/gy_socket_stat.cc:3968-4037
 //   gather_* / query_* / topn_*   read side
+//   window_* / task_summary_kernel  window reads: every live id, summarised on the device (gysk_summary.cuh)
 #include "gysk_kernels.cuh"
 #include "gysk_state.cuh"
+#include "gysk_summary.cuh"
 
 #include <cfloat>
 #include <climits>
@@ -1459,22 +1461,11 @@ __global__ void rebuild_table_kernel(DevState st, uint32_t max_svcs)
 // ---------------------------------------------------------------------------------------------------
 // read side: one warp per queried id
 // ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, uint32_t max_svcs,
-		uint32_t live0, uint32_t live1, SvcRaw *__restrict__ out)
+
+// the warp's copy of one slot's state (all but id / found / slot); hh: 64 words of scratch for the HLL register histogram
+__device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32_t max_svcs, uint32_t live0, uint32_t live1, SvcRaw &o,
+		uint32_t *hh, int lane)
 {
-	__shared__ uint32_t hh[4][64];
-	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	const uint32_t q = blockIdx.x * 4 + wid;
-
-	if (q >= n) return;
-	SvcRaw &o = out[q];
-	const unsigned long long id = ids[q];
-	int slot = -1;
-	if (lane == 0 && id) slot = table_lookup(st.svc_tbl, id, false);
-	slot = __shfl_sync(0xffffffffu, slot, 0);
-	if (lane == 0) { o.id = id; o.found = slot >= 0; o.slot = (uint32_t)slot; }
-	if (slot < 0) return;
-
 	if (lane < HIST_CELLS) {
 		o.cur[lane] = st.hist_cur[(size_t)slot * HIST_CELLS + lane];
 		o.last[lane] = st.hist_last[(size_t)slot * HIST_CELLS + lane];
@@ -1504,12 +1495,169 @@ __global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const uns
 	if (lane < HIST_CELLS) { o.qps[lane] = st.qps_hist[(size_t)slot * HIST_CELLS + lane]; o.act[lane] = st.act_hist[(size_t)slot * HIST_CELLS + lane]; }
 	for (int i = lane; i < TD_CAP; i += 32) o.cent[i] = st.td_cent[(size_t)slot * TD_CAP + i];
 
-	hh[wid][lane] = 0; hh[wid][lane + 32] = 0;
+	hh[lane] = 0; hh[lane + 32] = 0;
 	__syncwarp();
 	const uint8_t *regs = st.hll + ((size_t)slot << st.hll_p);
-	for (uint32_t i = lane; i < (1u << st.hll_p); i += 32) atomicAdd(&hh[wid][regs[i] > 63 ? 63 : regs[i]], 1u);
+	for (uint32_t i = lane; i < (1u << st.hll_p); i += 32) atomicAdd(&hh[regs[i] > 63 ? 63 : regs[i]], 1u);
 	__syncwarp();
-	o.hll_hist[lane] = hh[wid][lane]; o.hll_hist[lane + 32] = hh[wid][lane + 32];
+	o.hll_hist[lane] = hh[lane]; o.hll_hist[lane + 32] = hh[lane + 32];
+}
+
+__global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, uint32_t max_svcs,
+		uint32_t live0, uint32_t live1, SvcRaw *__restrict__ out)
+{
+	__shared__ uint32_t hh[4][64];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t q = blockIdx.x * 4 + wid;
+
+	if (q >= n) return;
+	SvcRaw &o = out[q];
+	const unsigned long long id = ids[q];
+	int slot = -1;
+	if (lane == 0 && id) slot = table_lookup(st.svc_tbl, id, false);
+	slot = __shfl_sync(0xffffffffu, slot, 0);
+	if (lane == 0) { o.id = id; o.found = slot >= 0; o.slot = (uint32_t)slot; }
+	if (slot < 0) return;
+	gather_slot(st, slot, max_svcs, live0, live1, o, hh[wid], lane);
+}
+
+// ---- window reads (gysk_query_window / gysk_query_task_window) ----
+
+// live slots below nslots (host filter, closed-window filter) -> keys {host : 32 | slot : 32} in any order, *d_n of them. A service is
+// active when its last window with events is the one the last flush closed (active_mark, the rule of state_kernel); a process when
+// one of its histograms took samples in that window.
+__global__ void window_select_kernel(DevState st, uint32_t nslots, int is_task, int host_filter, uint32_t active_only, uint32_t active_mark,
+		unsigned long long *__restrict__ keys, unsigned long long *d_n)
+{
+	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
+	bool take = false;
+	uint32_t host = 0;
+	if (slot < nslots) {
+		host = is_task ? st.task_slot_host[slot] : st.slot_host[slot];
+		take = (is_task ? st.task_slot_id[slot] : st.slot_id[slot]) != 0 && (host_filter < 0 || host == (uint32_t)host_filter);
+		if (take && active_only) {
+			if (is_task) {
+				const HistCell *l = st.task_last + (size_t)slot * 3;
+				take = (l[0].count | l[1].count | l[2].count) != 0;
+			}
+			else take = st.slot_last_active[slot] == active_mark;
+		}
+	}
+	const unsigned mask = __ballot_sync(0xffffffffu, take);
+	if (!mask) return;
+	const int lane = threadIdx.x & 31;
+	unsigned long long base = 0;
+	if (lane == __ffs(mask) - 1) base = atomicAdd(d_n, (unsigned long long)__popc(mask));
+	base = __shfl_sync(0xffffffffu, base, __ffs(mask) - 1);
+	if (take) keys[base + __popc(mask & ((1u << lane) - 1u))] = ((unsigned long long)host << 32) | slot;
+}
+
+// ids of the slots of the (sorted) keys
+__global__ void window_ids_kernel(DevState st, int is_task, const unsigned long long *__restrict__ keys, const unsigned long long *d_n,
+		unsigned long long *__restrict__ ids)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= *d_n) return;
+	const uint32_t slot = (uint32_t)keys[i];
+	ids[i] = is_task ? st.task_slot_id[slot] : st.slot_id[slot];
+}
+
+// td_quantile (gysk_summary.cuh) of the digest in shared memory, by one warp: each lane takes a run of centroids, a uint64 prefix over
+// the warp gives every centroid the cumulative weight the host loop reaches, a ballot finds the first centre above the target
+__device__ double td_quantile_warp(const Centroid *c, uint32_t n, double minv, double maxv, double q, int lane)
+{
+	const uint32_t per = (n + 31) >> 5, b = min(n, lane * per), e = min(n, b + per);
+	unsigned long long s = 0;
+	for (uint32_t i = b; i < e; ++i) s += c[i].weight;
+	unsigned long long incl = s;
+	for (int o = 1; o < 32; o <<= 1) {
+		const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+		if (lane >= o) incl += t;
+	}
+	const unsigned long long total = __shfl_sync(0xffffffffu, incl, 31);
+	if (q <= 0) return minv;
+	if (q >= 1) return maxv;
+	const double target = __dmul_rn(q, (double)total);
+	unsigned long long cum = incl - s;
+	int hit = -1;
+	for (uint32_t i = b; i < e; ++i) {
+		if (target < td_center((double)cum, c[i].weight)) { hit = (int)i; break; }
+		cum += c[i].weight;
+	}
+	const unsigned mask = __ballot_sync(0xffffffffu, hit >= 0);
+	if (!mask) {
+		const Centroid l = c[n - 1];
+		return td_interp(l.mean, maxv, target, td_center((double)(total - l.weight), l.weight), (double)total);
+	}
+	const int src = __ffs(mask) - 1;
+	const int i = __shfl_sync(0xffffffffu, hit, src);
+	const unsigned long long cb = __shfl_sync(0xffffffffu, cum, src);
+	const double center = td_center((double)cb, c[i].weight);
+	if (i == 0) return td_interp(minv, c[0].mean, target, 0.0, center);
+	const Centroid p = c[i - 1];
+	return td_interp(p.mean, c[i].mean, target, td_center((double)(cb - p.weight), p.weight), center);
+}
+
+// one warp per listed slot: the slot's state into shared memory (the words gather_svcs_kernel reads), then the summary of
+// summarize_raw. distinct_clients may come out as -(zero registers): the host finishes it with hll_finish.
+static constexpr int WIN_WARPS = 4;
+__global__ void __launch_bounds__(WIN_WARPS * 32) window_svcs_kernel(DevState st, const unsigned long long *__restrict__ slots, uint32_t n,
+		uint32_t max_svcs, uint32_t live0, uint32_t live1, gysk_svc_summary *__restrict__ out)
+{
+	__shared__ SvcRaw raw[WIN_WARPS];
+	__shared__ unsigned long long summ[WIN_WARPS][sizeof(gysk_svc_summary) / 8];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t q = blockIdx.x * WIN_WARPS + wid;
+
+	if (q >= n) return;
+	SvcRaw &r = raw[wid];
+	gysk_svc_summary &o = *reinterpret_cast<gysk_svc_summary *>(summ[wid]);
+	const uint32_t slot = (uint32_t)slots[q];
+	if (lane == 0) { r.id = st.slot_id[slot]; r.found = 1; r.slot = slot; }
+	gather_slot(st, (int)slot, max_svcs, live0, live1, r, r.hll_hist, lane);
+	__syncwarp();
+	if (lane == 0) {
+		summarize_fields(r, r.id, o);
+		o.distinct_clients = hll_pending(r.hll_hist, st.hll_p);
+	}
+	const uint32_t nc = min(r.td.n, (uint32_t)TD_CAP);
+	if (nc) {
+		const double p50 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.50, lane);
+		const double p95 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.95, lane);
+		const double p99 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.99, lane);
+		if (lane == 0) { o.td_p50_us = p50; o.td_p95_us = p95; o.td_p99_us = p99; }
+	}
+	__syncwarp();
+	unsigned long long *dst = reinterpret_cast<unsigned long long *>(out + q);
+	if (lane < (int)(sizeof(gysk_svc_summary) / 8)) dst[lane] = summ[wid][lane];
+}
+
+// one warp per process: by id (ids != nullptr: looked up, unknown ids give found = 0) or by slot (the window read)
+__global__ void __launch_bounds__(128) task_summary_kernel(DevState st, const unsigned long long *__restrict__ ids,
+		const unsigned long long *__restrict__ slots, uint32_t n, gysk_task_summary *__restrict__ out)
+{
+	__shared__ HistCell h[4][3 * HIST_CELLS + 3];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t q = blockIdx.x * 4 + wid;
+
+	if (q >= n) return;
+	int slot;
+	unsigned long long id;
+	if (ids) {
+		id = ids[q];
+		slot = -1;
+		if (lane == 0 && id) slot = table_lookup(st.task_tbl, id, false);
+		slot = __shfl_sync(0xffffffffu, slot, 0);
+	}
+	else { slot = (int)(uint32_t)slots[q]; id = st.task_slot_id[slot]; }
+	if (slot < 0) {
+		if (lane == 0) { gysk_task_summary z; memset(&z, 0, sizeof(z)); z.aggr_task_id = id; out[q] = z; }
+		return;
+	}
+	for (int i = lane; i < 3 * HIST_CELLS; i += 32) h[wid][i] = st.task_hist[(size_t)slot * 3 * HIST_CELLS + i];
+	if (lane < 3) h[wid][3 * HIST_CELLS + lane] = st.task_last[(size_t)slot * 3 + lane];
+	__syncwarp();
+	if (lane == 0) summarize_task(h[wid], h[wid] + 3 * HIST_CELLS, id, st.task_slot_host[slot], out[q]);
 }
 
 __global__ void gather_tasks_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, TaskRaw *__restrict__ out)
@@ -1955,6 +2103,38 @@ int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uin
 {
 	if (!n) return 0;
 	query_flows_kernel<<<div_up(n, 256), 256, 0, s>>>(st, d_keys, n, last_window, d_out);
+	return 1;
+}
+
+int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int host_filter, uint32_t active_only,
+		uint32_t active_mark, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids, cudaStream_t s)
+{
+	cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s);
+	*keys = tmp.keys_a; *ids = tmp.keys_b;
+	if (!nslots) return 0;
+	window_select_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, is_task, host_filter, active_only, active_mark, tmp.keys_a, d_n);
+	if (!order) return 1;
+	int which = 0;
+	const int sorted = launch_radix_sort(tmp, d_n, nslots, 32, 64, 64, 64, &which, s);
+	if (sorted < 0) return sorted;
+	*keys = which ? tmp.keys_b : tmp.keys_a; *ids = which ? tmp.keys_a : tmp.keys_b;
+	window_ids_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, is_task, *keys, d_n, const_cast<unsigned long long *>(*ids));
+	return 2 + sorted;
+}
+
+int launch_window_svcs(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask0, uint32_t live_mask1,
+		gysk_svc_summary *d_out, cudaStream_t s)
+{
+	if (!n) return 0;
+	window_svcs_kernel<<<div_up(n, WIN_WARPS), WIN_WARPS * 32, 0, s>>>(st, d_slots, n, max_svcs, live_mask0, live_mask1, d_out);
+	return 1;
+}
+
+int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, gysk_task_summary *d_out,
+		cudaStream_t s)
+{
+	if (!n) return 0;
+	task_summary_kernel<<<div_up(n, 4), 128, 0, s>>>(st, d_ids, d_slots, n, d_out);
 	return 1;
 }
 

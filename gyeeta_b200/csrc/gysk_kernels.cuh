@@ -130,6 +130,15 @@ int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint
 		SvcRaw *d_out, cudaStream_t s);
 int launch_gather_tasks(const DevState &st, const unsigned long long *d_ids, uint32_t n, TaskRaw *d_out, cudaStream_t s);
 int launch_gather_hll(const DevState &st, unsigned long long id, uint8_t *d_out, int32_t *d_found, cudaStream_t s);
+// window reads: the live slots (host filter, closed-window filter) as keys {host : 32 | slot : 32}, *d_n of them; with `order` sorted
+// by host (stable) and the ids of the sorted keys in *ids. *keys / *ids point into the sort buffers of tmp.
+int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int host_filter, uint32_t active_only,
+		uint32_t active_mark, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids, cudaStream_t s);
+int launch_window_svcs(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask0, uint32_t live_mask1,
+		gysk_svc_summary *d_out, cudaStream_t s);
+// by id (d_ids) or, with d_ids == nullptr, by slot (d_slots)
+int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, gysk_task_summary *d_out,
+		cudaStream_t s);
 int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uint32_t n, int last_window, gysk_flow_est *d_out, cudaStream_t s);
 
 } // namespace gysk

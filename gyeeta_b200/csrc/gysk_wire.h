@@ -127,6 +127,21 @@ struct alignas(8) LISTENER_STATE_NOTIFY					// common/gy_comm_proto.h:2183-2254
 };
 static_assert(sizeof(LISTENER_STATE_NOTIFY) == 88 && offsetof(LISTENER_STATE_NOTIFY, padding_len_) == 86, "LISTENER_STATE_NOTIFY");
 
+// the per-process p95 records madhava fills in handle_aggr_task_hist_stats (server/gy_mconnhdlr.cc:14648-14706)
+struct alignas(8) AGGR_TASK_HIST_STATS					// common/gy_comm_proto.h:2966-2977
+{
+	uint64_t	aggr_task_id_;
+	uint64_t	starttimeusec_;
+	uint32_t	p95_cpu_pct_, p95_cpu_delay_ms_, p95_blkio_delay_ms_;
+	uint32_t	nprocs_, nthreads_;
+	uint16_t	max_cores_allowed_;
+	uint8_t		cpu_cg_pct_limit_, max_mem_cg_pct_rss_;
+
+	static constexpr size_t MAX_NUM_TASKS = 1200;
+};
+static_assert(sizeof(AGGR_TASK_HIST_STATS) == 40 && offsetof(AGGR_TASK_HIST_STATS, p95_cpu_pct_) == 16 &&
+		offsetof(AGGR_TASK_HIST_STATS, max_cores_allowed_) == 36, "AGGR_TASK_HIST_STATS");
+
 // raw eBPF records, common/gy_ebpf_kernel.h:37-52,106-111 ; common/gy_ebpf_bpf_common.h:23-30
 struct tcp_ipv4_event_t
 {

@@ -66,6 +66,20 @@ class SvcSummary(C.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+WINDOW_ACTIVE_ONLY = 1
+
+
+class TaskSummary(C.Structure):
+    _fields_ = [("aggr_task_id", C.c_uint64), ("found", C.c_int32), ("host_idx", C.c_uint32), ("p95_cpu_pct", C.c_int32),
+                ("p95_cpu_delay_ms", C.c_int32), ("p95_blkio_delay_ms", C.c_int32), ("pad", C.c_uint32), ("nsamples", C.c_uint64),
+                ("last_count", C.c_uint64 * 3), ("last_sum", C.c_int64 * 3)]
+
+    def asdict(self):
+        d = {f: getattr(self, f) for f, _ in self._fields_ if f != "pad"}
+        d["last_count"], d["last_sum"] = list(self.last_count), list(self.last_sum)
+        return d
+
+
 class ListenerStateIn(C.Structure):
     """gysk_listener_state_in: the inputs of TCP_LISTENER::get_curr_state (include/gysketch.h)"""
     _fields_ = [(n, C.c_int64) for n in ("r5p95", "r5p99", "r300p95", "r300p99", "r5dp95", "r5dp99", "r5dp25", "rallp95", "rallp99")] + \
@@ -147,6 +161,10 @@ def load_library(path=None):
         "gysk_evicted_ids": (i32, [vp, vp, u32, vp]),
         "gysk_query_svcs": (i32, [vp, vp, u32, vp]),
         "gysk_query_flows": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_window": (i32, [vp, C.c_int32, u32, vp, u32, vp]),
+        "gysk_query_window_hosts": (i32, [vp, C.c_int32, u32, vp, vp, u32, vp]),
+        "gysk_query_tasks": (i32, [vp, vp, u32, vp]),
+        "gysk_query_task_window": (i32, [vp, C.c_int32, u32, vp, u32, vp]),
         "gysk_query_host_summary": (i32, [vp, u32, vp]),
         "gysk_topn_svcs": (i32, [vp, i32, C.c_int32, u32, vp, vp]),
         "gysk_topn_tasks": (i32, [vp, i32, u32, vp, vp]),
@@ -327,6 +345,44 @@ class Engine:
         nrecs, nbytes = C.c_uint32(), C.c_uint32()
         self._chk(self.L.gysk_encode_listener_state(out, len(ids), buf, len(buf), C.byref(nrecs), C.byref(nbytes)))
         return nrecs.value, buf.raw[: nbytes.value]
+
+    def _window(self, fn, row_type, host_idx, active_only, cap):
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(fn(self.h, host_idx, flags, None, 0, C.byref(n)))
+            cap = n.value
+        out = (row_type * max(cap, 1))()
+        self._chk(fn(self.h, host_idx, flags, out if cap else None, cap, C.byref(n)))
+        return out[: min(cap, n.value)], n.value
+
+    def query_window(self, host_idx=-1, active_only=False, cap=None):
+        """gysk_query_window: (SvcSummary rows grouped by host, ids ascending within a host; number of matching rows).
+        cap None = all rows (a count call first); 0 = the count only"""
+        return self._window(self.L.gysk_query_window, SvcSummary, host_idx, active_only, cap)
+
+    def query_window_hosts(self, host_idx=-1, active_only=False, cap=None):
+        """gysk_query_window_hosts: (rows, host_idx of each row as a uint32 array, number of matching rows)"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_window_hosts(self.h, host_idx, flags, None, None, 0, C.byref(n)))
+            cap = n.value
+        out = (SvcSummary * max(cap, 1))()
+        hosts = np.zeros(max(cap, 1), dtype=np.uint32)
+        self._chk(self.L.gysk_query_window_hosts(self.h, host_idx, flags, out if cap else None, _p(hosts) if cap else None, cap, C.byref(n)))
+        k = min(cap, n.value)
+        return out[:k], hosts[:k].copy(), n.value
+
+    def query_tasks(self, ids):
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (TaskSummary * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_tasks(self.h, _p(ids), len(ids), out))
+        return out[: len(ids)]
+
+    def query_task_window(self, host_idx=-1, active_only=False, cap=None):
+        """gysk_query_task_window: (TaskSummary rows in the order of query_window, number of matching rows)"""
+        return self._window(self.L.gysk_query_task_window, TaskSummary, host_idx, active_only, cap)
 
     def query_flows(self, keys, last_window=False):
         keys = np.ascontiguousarray(keys, dtype=np.uint64)

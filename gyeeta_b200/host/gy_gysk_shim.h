@@ -1,10 +1,11 @@
 // gy_gysk_shim.h — the host-side mirror of the reference's ingest interface for this path (C++17, header only).
 //
-// The three handlers below keep the names, argument meaning and bool return of the reference's member functions
+// The handlers below keep the names, argument meaning and bool return of the reference's member functions
 //     MCONN_HANDLER::partha_tcp_conn_info     server/gy_mconnhdlr.h:2091   (definition gy_mconnhdlr.cc:9052)
 //     MCONN_HANDLER::partha_aggr_task_state   server/gy_mconnhdlr.h:2098   (definition gy_mconnhdlr.cc:9959)
 //     MCONN_HANDLER::partha_listener_state    server/gy_mconnhdlr.h:2129   (definition gy_mconnhdlr.cc:10993)
 //     MCONN_HANDLER::handle_partha_active_conns server/gy_mconnhdlr.h:2155 (definition gy_mconnhdlr.cc:7705)
+//     MCONN_HANDLER::handle_aggr_task_hist_stats server/gy_mconnhdlr.h:2109 (definition gy_mconnhdlr.cc:14648; reads the engine)
 // and forward the record batch to the GPU engine through the C ABI of include/gysketch.h. The template parameters
 // stand for the reference's own types (std::shared_ptr<PARTHA_INFO>, comm::TCP_CONN_NOTIFY, POOL_ALLOC_ARRAY, PGConnPool) so
 // that this header compiles both inside gy_mconnhdlr.cc (with the real types) and stand-alone in this repository's tests (with
@@ -130,6 +131,69 @@ public :
 		catch (...) { return -1; }
 	}
 
+	// The 5-s tick's read side in raw-forward mode: every listener the engine holds, as LISTENER_STATE_NOTIFY batches of at most 512
+	// records (MAX_NUM_LISTENERS, common/gy_comm_proto.h:2222), host by host in ascending host index, ids ascending within a host,
+	// from one gysk_query_window_hosts snapshot. Call after flush_window. on_batch(uint32_t host_idx, const void *recs, uint32_t nrecs,
+	// uint32_t nbytes) is where madhava calls its unchanged partha_listener_state; handing the same buffer to
+	// gysk_ingest(GYSK_NOTIFY_LISTENER_STATE) fills the engine's per-host summaries, top-N lists and cluster state. Returns false on
+	// failure. Its scratch is local: safe to call while other threads use this handler.
+	template <typename OnBatch>
+	bool window_listener_states(OnBatch && on_batch) noexcept
+	{
+		try {
+			std::vector<gysk_svc_summary> rows;
+			std::vector<uint32_t> hosts;
+			uint32_t n = 0, cap = 0;
+			// count, then read; listeners created in between make the read report more rows than room: read again, larger
+			for (int tries = 0; ; ++tries) {
+				rows.resize(cap); hosts.resize(cap);
+				if (0 != gysk_query_window_hosts(engine_, -1, 0, cap ? rows.data() : nullptr, cap ? hosts.data() : nullptr, cap, &n)) return false;
+				if (n <= cap) break;
+				if (tries == 3) return false;
+				cap = n + n / 8 + 64;
+			}
+			std::vector<uint8_t> recs(MAX_BATCH * RECORD_BYTES);
+			for (uint32_t a = 0; a < n; ) {
+				uint32_t b = a + 1;
+				while (b < n && b - a < MAX_BATCH && hosts[b] == hosts[a]) ++b;
+				uint32_t nrecs = 0, nbytes = 0;
+				if (0 != gysk_encode_listener_state(rows.data() + a, b - a, recs.data(), (uint32_t)recs.size(), &nrecs, &nbytes)) return false;
+				on_batch(hosts[a], (const void *)recs.data(), nrecs, nbytes);
+				a = b;
+			}
+			return true;
+		}
+		catch (...) { return false; }
+	}
+
+	// bool handle_aggr_task_hist_stats(const std::shared_ptr<MCONNTRACK> &, AGGR_TASK_HIST_STATS *, int nevents, POOL_ALLOC_ARRAY *, PGConnPool &)
+	// (server/gy_mconnhdlr.cc:14648-14706) when the process histograms live in the engine: fills p95_cpu_pct_, p95_cpu_delay_ms_ and
+	// p95_blkio_delay_ms_ of the records whose aggregated process the engine holds for this partha (the reference looks each id up in
+	// the partha's own task_aggr_tbl_, :14693; here the process's host_idx must be the partha's host index), with get_percentiles({95})
+	// of the three MTASK_HIST histograms, the int result stored into the uint32 fields like the reference's assignment. Other records
+	// stay as they are. madhava keeps the rest of its handler (pmtask->histstats_ = *pone). Its scratch is local: L2 threads may call
+	// it concurrently.
+	template <typename ParthaInfo, typename AggrTaskHistStats>
+	bool handle_aggr_task_hist_stats(const std::shared_ptr<ParthaInfo> & partha_shr, AggrTaskHistStats *ptask, int n) noexcept
+	{
+		if (!partha_shr || !ptask || n < 0) return false;
+		try {
+			const uint32_t host = partha_traits<ParthaInfo>::host_index(*partha_shr);
+			std::vector<uint64_t> ids(n);
+			std::vector<gysk_task_summary> tasks(n);
+			for (int i = 0; i < n; ++i) ids[i] = ptask[i].aggr_task_id_;
+			if (0 != gysk_query_tasks(engine_, ids.data(), (uint32_t)n, tasks.data())) return false;
+			for (int i = 0; i < n; ++i) {
+				if (!tasks[i].found || tasks[i].host_idx != host) continue;
+				ptask[i].p95_cpu_pct_ = tasks[i].p95_cpu_pct;
+				ptask[i].p95_cpu_delay_ms_ = tasks[i].p95_cpu_delay_ms;
+				ptask[i].p95_blkio_delay_ms_ = tasks[i].p95_blkio_delay_ms;
+			}
+		}
+		catch (...) { return false; }
+		return true;
+	}
+
 	gysk_engine * engine() const noexcept { return engine_; }
 
 private :
@@ -142,8 +206,10 @@ private :
 				subtype, recs, (uint32_t)nevents, pendptr);
 	}
 
+	static constexpr uint32_t MAX_BATCH = 512, RECORD_BYTES = 88;		// records per NOTIFY_LISTENER_STATE message, sizeof(LISTENER_STATE_NOTIFY)
+
 	gysk_engine		*engine_;
-	std::vector<uint64_t>	evicted_;
+	std::vector<uint64_t>	evicted_;		// scratch of flush_window(tsec, on_delete) and listener_state_records: one caller at a time
 	std::vector<gysk_svc_summary> summ_;
 };
 

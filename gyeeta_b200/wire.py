@@ -17,6 +17,11 @@ TASK = np.dtype([("aggr_task_id", "<u8"), ("onecomm", "S16"), ("pid_arr", "<i4",
                  ("total_cpu_pct", "<f4"), ("rss_mb", "<u4"), ("cpu_delay_msec", "<u4"), ("vm_delay_msec", "<u4"), ("blkio_delay_msec", "<u4"),
                  ("ntasks_total", "<u2"), ("ntasks_issue", "<u2"), ("curr_state", "u1"), ("curr_issue", "u1"), ("issue_bit_hist", "u1"),
                  ("severe_issue_bit_hist", "u1"), ("issue_string_len", "u1"), ("padding_len", "u1"), ("pad", "u1", 2)])
+# AGGR_TASK_HIST_STATS, common/gy_comm_proto.h:2966-2977 (the records of handle_aggr_task_hist_stats)
+AGGR_TASK_HIST_STATS = np.dtype([("aggr_task_id", "<u8"), ("starttimeusec", "<u8"), ("p95_cpu_pct", "<u4"), ("p95_cpu_delay_ms", "<u4"),
+                                 ("p95_blkio_delay_ms", "<u4"), ("nprocs", "<u4"), ("nthreads", "<u4"), ("max_cores_allowed", "<u2"),
+                                 ("cpu_cg_pct_limit", "u1"), ("max_mem_cg_pct_rss", "u1")])
+assert AGGR_TASK_HIST_STATS.itemsize == 40
 RESP4 = np.dtype([("saddr", "<u4"), ("daddr", "<u4"), ("netns", "<u4"), ("sport", "<u2"), ("dport", "<u2"), ("lsndtime", "<u4"), ("lrcvtime", "<u4")])
 assert TCP_CONN.itemsize == 280 and TASK.itemsize == 72 and HDR.itemsize == 24 and RESP4.itemsize == 24
 PM_MAGIC, COMM_EVENT_NOTIFY = 0x05666605, 14

@@ -372,6 +372,39 @@ int		gysk_evicted_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n);
 
 /* ---- queries ---- */
 int		gysk_query_svcs(gysk_engine *e, const uint64_t *glob_ids, uint32_t n, gysk_svc_summary *out);
+
+/* ---- window reads: every live id of the engine in one device pass, summarised on the device ----
+ * Rows are grouped by ascending host_idx and, within a host, ordered by ascending id. The host_idx of an id is the host of the
+ * event that created its slot (what gysk_topn_svcs reports); ids created by gysk_register_ids have host 0.
+ * host_idx < 0 reads every host. *n = number of matching rows; at most cap rows are written (out may be NULL when cap is 0). */
+#define GYSK_WINDOW_ACTIVE_ONLY		0x1u	/* only ids whose closed window held events (the last gysk_flush) */
+/* A service row equals the gysk_query_svcs row of its id, byte for byte: what madhava's 5-s tick reads for every listener
+ * (partha_listener_state, server/gy_mconnhdlr.cc:10993-11410) once the reduction runs in the engine */
+int		gysk_query_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_summary *out, uint32_t cap, uint32_t *n);
+/* the same read with the host_idx of every written row in hosts[] (cap entries, or NULL): rows and hosts come from one
+ * snapshot, so a caller that splits the rows by host (the shim's window_listener_states) needs one call, not one per host */
+int		gysk_query_window_hosts(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_summary *out, uint32_t *hosts, uint32_t cap,
+				uint32_t *n);
+
+/* per aggregated process: the p95 fields of AGGR_TASK_HIST_STATS (common/gy_comm_proto.h:2966-2977) as
+ * handle_aggr_task_hist_stats fills them (server/gy_mconnhdlr.cc:14648-14706: get_percentiles({95}) of the three MTASK_HIST
+ * histograms, T = int, -1 for an empty histogram) and the last closed window of each histogram, the window the top-N lists rank */
+typedef struct gysk_task_summary
+{
+	uint64_t	aggr_task_id;
+	int32_t		found;			/* 0 if the id is unknown (the other fields are then zero) */
+	uint32_t	host_idx;		/* host of the event that created the slot */
+	int32_t		p95_cpu_pct;		/* cpu_pct_histogram_		(HASH_1_3000) */
+	int32_t		p95_cpu_delay_ms;	/* cpu_delay_histogram_		(DURATION_HASH) */
+	int32_t		p95_blkio_delay_ms;	/* blkio_delay_histogram_	(DURATION_HASH) */
+	uint32_t	pad;
+	uint64_t	nsamples;		/* samples since start (count of the cpu % histogram) */
+	uint64_t	last_count[3];		/* last closed window per histogram {cpu %, cpu delay, blkio delay}: samples */
+	int64_t		last_sum[3];		/* ... and their sum */
+} gysk_task_summary;
+int		gysk_query_tasks(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_task_summary *out);
+/* the task rows of every live aggregated process, in the order and with the count / capacity rules of gysk_query_window */
+int		gysk_query_task_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_task_summary *out, uint32_t cap, uint32_t *n);
 int		gysk_query_flows(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_est *out);
 /* LISTEN_SUMM_STATS of the last NOTIFY_LISTENER_STATE message of a host (partha_listener_state, gy_mconnhdlr.cc:11251) */
 /* host_idx < 0: over all hosts of this engine; n <= 64 */
