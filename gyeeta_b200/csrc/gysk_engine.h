@@ -146,13 +146,13 @@ struct gysk_engine
 
 	// query scratch
 	unsigned long long	*d_qids {nullptr}, *h_qids {nullptr};
-	gysk::SvcRaw		*d_svcraw {nullptr}, *h_svcraw {nullptr};
+	gysk::SvcRaw		*d_svcraw {nullptr}, *h_svcraw {nullptr};	// the single-id exports: one entry each
 	gysk::TaskRaw		*d_taskraw {nullptr}, *h_taskraw {nullptr};
 	uint8_t			*d_hllout {nullptr}, *h_hllout {nullptr};
 	int32_t			*d_found {nullptr}, *h_found {nullptr};
 	gysk_flow_est		*d_flowout {nullptr}, *h_flowout {nullptr};
 	unsigned long long	*h_counters {nullptr};
-	uint8_t			*d_wstage {nullptr}, *h_wstage {nullptr};	// window reads / gysk_query_tasks: WIN_ROWS rows per pass
+	uint8_t			*d_wstage {nullptr}, *h_wstage {nullptr};	// summary rows: WIN_ROWS per window-read pass, QCHUNK per by-id pass
 	std::vector<uint64_t>	win_keys, win_ids;			// a window read's {host | slot} keys and their ids on the host
 	std::vector<std::pair<uint64_t, uint64_t>> win_rows;		// ... as {id, slot}, ordered within each host
 
@@ -199,7 +199,8 @@ int drain_all(gysk_engine *e);
 int sync_locked(gysk_engine *e);
 int collect_evicted(gysk_engine *e, bool wait);
 void merge_release(gysk_engine *e);
-void summarize_raw(const gysk_engine *e, const SvcRaw &r, uint64_t id, gysk_svc_summary &o);
+// the first k service rows of the window stage -> out (synchronises the stream), distinct_clients finished with hll_finish
+int copy_svc_rows(gysk_engine *e, uint32_t k, gysk_svc_summary *out, const char *what);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 // readers: hand every thread's partial chunk to the device, then take the engine

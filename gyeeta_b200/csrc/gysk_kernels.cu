@@ -1462,9 +1462,8 @@ __global__ void rebuild_table_kernel(DevState st, uint32_t max_svcs)
 // read side: one warp per queried id
 // ---------------------------------------------------------------------------------------------------
 
-// the warp's copy of one slot's state (all but id / found / slot); hh: 64 words of scratch for the HLL register histogram
-__device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32_t max_svcs, uint32_t live0, uint32_t live1, SvcRaw &o,
-		uint32_t *hh, int lane)
+// the warp's copy of one slot's state (all but id / found / slot and the HLL register histogram)
+__device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32_t max_svcs, uint32_t live0, uint32_t live1, SvcRaw &o, int lane)
 {
 	if (lane < HIST_CELLS) {
 		o.cur[lane] = st.hist_cur[(size_t)slot * HIST_CELLS + lane];
@@ -1494,19 +1493,12 @@ __device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32
 	}
 	if (lane < HIST_CELLS) { o.qps[lane] = st.qps_hist[(size_t)slot * HIST_CELLS + lane]; o.act[lane] = st.act_hist[(size_t)slot * HIST_CELLS + lane]; }
 	for (int i = lane; i < TD_CAP; i += 32) o.cent[i] = st.td_cent[(size_t)slot * TD_CAP + i];
-
-	hh[lane] = 0; hh[lane + 32] = 0;
-	__syncwarp();
-	const uint8_t *regs = st.hll + ((size_t)slot << st.hll_p);
-	for (uint32_t i = lane; i < (1u << st.hll_p); i += 32) atomicAdd(&hh[regs[i] > 63 ? 63 : regs[i]], 1u);
-	__syncwarp();
-	o.hll_hist[lane] = hh[lane]; o.hll_hist[lane + 32] = hh[lane + 32];
 }
 
+// the single-id exports (gysk_export_hist / _conn_bitmap / _tdigest): the raw state of the id
 __global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, uint32_t max_svcs,
 		uint32_t live0, uint32_t live1, SvcRaw *__restrict__ out)
 {
-	__shared__ uint32_t hh[4][64];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 	const uint32_t q = blockIdx.x * 4 + wid;
 
@@ -1518,7 +1510,7 @@ __global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const uns
 	slot = __shfl_sync(0xffffffffu, slot, 0);
 	if (lane == 0) { o.id = id; o.found = slot >= 0; o.slot = (uint32_t)slot; }
 	if (slot < 0) return;
-	gather_slot(st, slot, max_svcs, live0, live1, o, hh[wid], lane);
+	gather_slot(st, slot, max_svcs, live0, live1, o, lane);
 }
 
 // ---- window reads (gysk_query_window / gysk_query_task_window) ----
@@ -1562,74 +1554,35 @@ __global__ void window_ids_kernel(DevState st, int is_task, const unsigned long 
 	ids[i] = is_task ? st.task_slot_id[slot] : st.slot_id[slot];
 }
 
-// td_quantile (gysk_summary.cuh) of the digest in shared memory, by one warp: each lane takes a run of centroids, a uint64 prefix over
-// the warp gives every centroid the cumulative weight the host loop reaches, a ballot finds the first centre above the target
-__device__ double td_quantile_warp(const Centroid *c, uint32_t n, double minv, double maxv, double q, int lane)
+// one warp per service: by id (ids != nullptr: looked up, id 0 and unknown ids give found = 0) or by slot (the window read). The
+// slot's state goes into shared memory, then summarize_warp makes the row.
+static constexpr int SUMM_WARPS = 4;
+__global__ void __launch_bounds__(SUMM_WARPS * 32) svc_summary_kernel(DevState st, const unsigned long long *__restrict__ ids,
+		const unsigned long long *__restrict__ slots, uint32_t n, uint32_t max_svcs, uint32_t live0, uint32_t live1,
+		gysk_svc_summary *__restrict__ out)
 {
-	const uint32_t per = (n + 31) >> 5, b = min(n, lane * per), e = min(n, b + per);
-	unsigned long long s = 0;
-	for (uint32_t i = b; i < e; ++i) s += c[i].weight;
-	unsigned long long incl = s;
-	for (int o = 1; o < 32; o <<= 1) {
-		const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
-		if (lane >= o) incl += t;
-	}
-	const unsigned long long total = __shfl_sync(0xffffffffu, incl, 31);
-	if (q <= 0) return minv;
-	if (q >= 1) return maxv;
-	const double target = __dmul_rn(q, (double)total);
-	unsigned long long cum = incl - s;
-	int hit = -1;
-	for (uint32_t i = b; i < e; ++i) {
-		if (target < td_center((double)cum, c[i].weight)) { hit = (int)i; break; }
-		cum += c[i].weight;
-	}
-	const unsigned mask = __ballot_sync(0xffffffffu, hit >= 0);
-	if (!mask) {
-		const Centroid l = c[n - 1];
-		return td_interp(l.mean, maxv, target, td_center((double)(total - l.weight), l.weight), (double)total);
-	}
-	const int src = __ffs(mask) - 1;
-	const int i = __shfl_sync(0xffffffffu, hit, src);
-	const unsigned long long cb = __shfl_sync(0xffffffffu, cum, src);
-	const double center = td_center((double)cb, c[i].weight);
-	if (i == 0) return td_interp(minv, c[0].mean, target, 0.0, center);
-	const Centroid p = c[i - 1];
-	return td_interp(p.mean, c[i].mean, target, td_center((double)(cb - p.weight), p.weight), center);
-}
-
-// one warp per listed slot: the slot's state into shared memory (the words gather_svcs_kernel reads), then the summary of
-// summarize_raw. distinct_clients may come out as -(zero registers): the host finishes it with hll_finish.
-static constexpr int WIN_WARPS = 4;
-__global__ void __launch_bounds__(WIN_WARPS * 32) window_svcs_kernel(DevState st, const unsigned long long *__restrict__ slots, uint32_t n,
-		uint32_t max_svcs, uint32_t live0, uint32_t live1, gysk_svc_summary *__restrict__ out)
-{
-	__shared__ SvcRaw raw[WIN_WARPS];
-	__shared__ unsigned long long summ[WIN_WARPS][sizeof(gysk_svc_summary) / 8];
+	__shared__ SvcRaw raw[SUMM_WARPS];
+	__shared__ unsigned long long summ[SUMM_WARPS][sizeof(gysk_svc_summary) / 8];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	const uint32_t q = blockIdx.x * WIN_WARPS + wid;
+	const uint32_t q = blockIdx.x * SUMM_WARPS + wid;
 
 	if (q >= n) return;
 	SvcRaw &r = raw[wid];
-	gysk_svc_summary &o = *reinterpret_cast<gysk_svc_summary *>(summ[wid]);
-	const uint32_t slot = (uint32_t)slots[q];
-	if (lane == 0) { r.id = st.slot_id[slot]; r.found = 1; r.slot = slot; }
-	gather_slot(st, (int)slot, max_svcs, live0, live1, r, r.hll_hist, lane);
-	__syncwarp();
-	if (lane == 0) {
-		summarize_fields(r, r.id, o);
-		o.distinct_clients = hll_pending(r.hll_hist, st.hll_p);
+	int slot;
+	unsigned long long id;
+	if (ids) {
+		id = ids[q];
+		slot = -1;
+		if (lane == 0 && id) slot = table_lookup(st.svc_tbl, id, false);
+		slot = __shfl_sync(0xffffffffu, slot, 0);
 	}
-	const uint32_t nc = min(r.td.n, (uint32_t)TD_CAP);
-	if (nc) {
-		const double p50 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.50, lane);
-		const double p95 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.95, lane);
-		const double p99 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.99, lane);
-		if (lane == 0) { o.td_p50_us = p50; o.td_p95_us = p95; o.td_p99_us = p99; }
+	else { slot = (int)(uint32_t)slots[q]; id = st.slot_id[slot]; }
+	if (lane == 0) { r.id = id; r.found = slot >= 0; r.slot = (uint32_t)slot; }
+	if (slot >= 0) {
+		gather_slot(st, slot, max_svcs, live0, live1, r, lane);
+		hll_hist_warp(st.hll + ((size_t)slot << st.hll_p), st.hll_p, r.hll_hist, lane);
 	}
-	__syncwarp();
-	unsigned long long *dst = reinterpret_cast<unsigned long long *>(out + q);
-	if (lane < (int)(sizeof(gysk_svc_summary) / 8)) dst[lane] = summ[wid][lane];
+	summarize_warp(r, id, st.hll_p, summ[wid], out + q, lane);
 }
 
 // one warp per process: by id (ids != nullptr: looked up, unknown ids give found = 0) or by slot (the window read)
@@ -2122,11 +2075,11 @@ int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots,
 	return 2 + sorted;
 }
 
-int launch_window_svcs(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask0, uint32_t live_mask1,
-		gysk_svc_summary *d_out, cudaStream_t s)
+int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs,
+		uint32_t live_mask0, uint32_t live_mask1, gysk_svc_summary *d_out, cudaStream_t s)
 {
 	if (!n) return 0;
-	window_svcs_kernel<<<div_up(n, WIN_WARPS), WIN_WARPS * 32, 0, s>>>(st, d_slots, n, max_svcs, live_mask0, live_mask1, d_out);
+	svc_summary_kernel<<<div_up(n, SUMM_WARPS), SUMM_WARPS * 32, 0, s>>>(st, d_ids, d_slots, n, max_svcs, live_mask0, live_mask1, d_out);
 	return 1;
 }
 

@@ -78,7 +78,7 @@ struct RecRegions { uint32_t nwarps; uint64_t cap; };
 // the buffers.
 struct IngestShape { static constexpr int WARPS = 8, MIN_CTAS = 3, EPT = 2, CHUNK = 32 * EPT; };
 
-// raw per-id record gathered for queries / exports
+// one service's state: what a summary warp reads (in shared memory), and what the single-id exports copy to the host
 struct SvcRaw
 {
 	unsigned long long	id;
@@ -134,9 +134,9 @@ int launch_gather_hll(const DevState &st, unsigned long long id, uint8_t *d_out,
 // by host (stable) and the ids of the sorted keys in *ids. *keys / *ids point into the sort buffers of tmp.
 int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int host_filter, uint32_t active_only,
 		uint32_t active_mark, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids, cudaStream_t s);
-int launch_window_svcs(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask0, uint32_t live_mask1,
-		gysk_svc_summary *d_out, cudaStream_t s);
-// by id (d_ids) or, with d_ids == nullptr, by slot (d_slots)
+// service / process rows by id (d_ids) or, with d_ids == nullptr, by slot (d_slots)
+int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs,
+		uint32_t live_mask0, uint32_t live_mask1, gysk_svc_summary *d_out, cudaStream_t s);
 int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, gysk_task_summary *d_out,
 		cudaStream_t s);
 int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uint32_t n, int last_window, gysk_flow_est *d_out, cudaStream_t s);

@@ -17,6 +17,7 @@
 // SHCONN_HANDLER::aggregate_cluster_state (server/gy_shconnhdlr.cc:4583) and of GY_HISTOGRAM::update_from_serialized
 // (common/gy_statistics.h:625-650): integer sums are order independent => bit-exact at any GPU count.
 #include "gysk_engine.h"
+#include "gysk_summary.cuh"
 
 #include <climits>
 #include <dlfcn.h>
@@ -148,42 +149,45 @@ __global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntr
 	}
 }
 
-// read side: logical arrays -> SvcRaw (so the host summary code is shared with gysk_query_svcs)
-__global__ void __launch_bounds__(128) gather_logical_kernel(const int32_t *__restrict__ lidx, uint32_t n, uint32_t hll_p,
+// read side: one warp per logical service, its merged arrays into a shared-memory SvcRaw, then the row of summarize_warp (the
+// summary of gysk_query_svcs). The merge folds neither the current window, the rolling levels, the connection bitmaps nor the
+// per-slot aux / state / qps / active-connection words: they are zero. glob_id is left 0 for the host to fill in.
+static constexpr int LG_WARPS = 4;
+__global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const int32_t *__restrict__ lidx, uint32_t n, uint32_t hll_p,
 		const HistCell *__restrict__ l_last, const HistCell *__restrict__ l_all, const unsigned long long *__restrict__ l_conn,
-		const long long *__restrict__ l_hmax, const uint8_t *__restrict__ l_hll, const SlabEntry *__restrict__ slab, SvcRaw *__restrict__ out)
+		const long long *__restrict__ l_hmax, const uint8_t *__restrict__ l_hll, const SlabEntry *__restrict__ slab,
+		gysk_svc_summary *__restrict__ out)
 {
-	__shared__ uint32_t hh[4][64];
+	__shared__ SvcRaw raw[LG_WARPS];
+	__shared__ unsigned long long summ[LG_WARPS][sizeof(gysk_svc_summary) / 8];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	const uint32_t q = blockIdx.x * 4 + wid;
+	const uint32_t q = blockIdx.x * LG_WARPS + wid;
 
 	if (q >= n) return;
-	SvcRaw &o = out[q];
+	SvcRaw &r = raw[wid];
 	const int32_t l = lidx[q];
-	if (lane == 0) { o.id = 0; o.found = l >= 0; o.slot = (uint32_t)l; }
-	if (l < 0) return;
-
-	if (lane < HIST_CELLS) {
-		HistCell a = l_last[(size_t)l * HIST_CELLS + lane], b = l_all[(size_t)l * HIST_CELLS + lane];
-		if (lane == HIST_MAX_CELL) { a.sum = l_hmax[2 * l]; b.sum = l_hmax[2 * l + 1]; }
-		o.last[lane] = a; o.all[lane] = b; o.cur[lane] = HistCell {0, 0};
-		o.lvl[0][lane] = HistCell {0, 0}; o.lvl[1][lane] = HistCell {0, 0};
-		o.bm_cur[lane] = 0; o.bm_last[lane] = 0;
+	if (lane == 0) { r.id = 0; r.found = l >= 0; r.slot = (uint32_t)l; }
+	if (l >= 0) {
+		if (lane < HIST_CELLS) {
+			HistCell a = l_last[(size_t)l * HIST_CELLS + lane], b = l_all[(size_t)l * HIST_CELLS + lane];
+			if (lane == HIST_MAX_CELL) { a.sum = l_hmax[2 * l]; b.sum = l_hmax[2 * l + 1]; }
+			r.last[lane] = a; r.all[lane] = b; r.cur[lane] = HistCell {0, 0};
+			r.lvl[0][lane] = HistCell {0, 0}; r.lvl[1][lane] = HistCell {0, 0};
+			r.bm_cur[lane] = 0; r.bm_last[lane] = 0;
+			r.qps[lane] = HistCell {0, 0}; r.act[lane] = HistCell {0, 0};
+		}
+		if (lane == 0) {
+			r.conn_cur = 0;
+			r.conn_last = (l_conn[4 * l] & 0xFFFFFFFFull) | (l_conn[4 * l + 1] << 32);
+			r.conn_all_cnt = l_conn[4 * l + 2]; r.conn_all_kb = l_conn[4 * l + 3];
+			r.td = slab[l].head;
+			r.aux = SlotAux {0, 0, 0, 0, 0, 0};
+			r.sst = SlotState {0, 0, 0, 0, 0};
+		}
+		for (int i = lane; i < TD_CAP; i += 32) r.cent[i] = slab[l].cent[i];
+		hll_hist_warp(l_hll + ((size_t)l << hll_p), hll_p, r.hll_hist, lane);
 	}
-	if (lane == 0) {
-		o.conn_cur = 0;
-		o.conn_last = (l_conn[4 * l] & 0xFFFFFFFFull) | (l_conn[4 * l + 1] << 32);
-		o.conn_all_cnt = l_conn[4 * l + 2]; o.conn_all_kb = l_conn[4 * l + 3];
-		o.td = slab[l].head;
-	}
-	for (int i = lane; i < TD_CAP; i += 32) o.cent[i] = slab[l].cent[i];
-
-	hh[wid][lane] = 0; hh[wid][lane + 32] = 0;
-	__syncwarp();
-	const uint8_t *regs = l_hll + ((size_t)l << hll_p);
-	for (uint32_t i = lane; i < (1u << hll_p); i += 32) atomicAdd(&hh[wid][regs[i] > 63 ? 63 : regs[i]], 1u);
-	__syncwarp();
-	o.hll_hist[lane] = hh[wid][lane]; o.hll_hist[lane + 32] = hh[wid][lane + 32];
+	summarize_warp(r, 0, hll_p, summ[wid], out + q, lane);
 }
 
 } // namespace gysk
@@ -430,6 +434,7 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical: no finished merge");
 
 	int32_t *h_l = reinterpret_cast<int32_t *>(e->h_qids), *d_l = reinterpret_cast<int32_t *>(e->d_qids);
+	gysk_svc_summary *d_rows = reinterpret_cast<gysk_svc_summary *>(e->d_wstage);
 	for (uint32_t off = 0; off < n; off += QCHUNK) {
 		const uint32_t m = std::min(QCHUNK, n - off);
 		for (uint32_t i = 0; i < m; ++i) {
@@ -437,14 +442,14 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 			h_l[i] = it == mg.index.end() ? -1 : (int32_t)it->second;
 		}
 		CU(e, cudaMemcpyAsync(d_l, h_l, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
-		gather_logical_kernel<<<div_up(m, 4), 128, 0, e->stream>>>(d_l, m, e->cfg.hll_p, mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax,
-				mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab), e->d_svcraw);
+		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(d_l, m, e->cfg.hll_p, mg.l_hist_last, mg.l_hist_all,
+				mg.l_conn, mg.l_hmax, mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab), d_rows);
 		e->kernel_launches++;
-		CU(e, cudaMemcpyAsync(e->h_svcraw, e->d_svcraw, (size_t)m * sizeof(SvcRaw), cudaMemcpyDeviceToHost, e->stream));
-		CU(e, cudaStreamSynchronize(e->stream));
-		for (uint32_t i = 0; i < m; ++i) summarize_raw(e, e->h_svcraw[i], logical_ids[off + i], out[off + i]);
+		int rc = copy_svc_rows(e, m, out + off, "query_logical");
+		if (rc) return rc;
+		for (uint32_t i = 0; i < m; ++i) out[off + i].glob_id = logical_ids[off + i];
 	}
-	return post_launch(e, "query_logical");
+	return GYSK_OK;
 }
 
 // global count-min point query on the merged table

@@ -1,12 +1,14 @@
 // gysk_summary.cuh — the arithmetic of one service's / one process's summary, host + device.
 //
-// gysk_query_svcs / gysk_query_logical gather an SvcRaw to the host and summarise it there (summarize_raw); the window reads of
-// gysk_query_window / gysk_query_task_window summarise on the device. Both sides call the functions below, so the two give the same
-// bytes. What keeps them equal:
+// Every service row (gysk_query_svcs, gysk_query_window, gysk_query_logical) is summarised on the device, one warp per row
+// (summarize_warp); every process row too (summarize_task). The host keeps td_quantile and hll_estimate_from_hist for the public
+// gysk_tdigest_quantile / gysk_hll_estimate / gysk_query_quantiles, which answer from a service's exported sketches what its row
+// holds. What keeps the two sides equal:
 //   * the percentile rule is GY_HISTOGRAM::get_percentiles (common/gy_statistics.h:707-791) through hist_pct_bucket (gysk_state.cuh);
-//   * t-digest quantiles: the cumulative weights are sums of integer weights below 2^53, exact in any order, so the device's uint64
-//     warp prefix gives the doubles of the host's running sum; the interpolation is written with explicit round-to-nearest
-//     operations on the device so that nvcc does not contract it into a fused multiply-add;
+//   * t-digest quantiles: while the cumulative weights stay below 2^53 they are exact in any order, so the device's uint64 warp
+//     prefix gives the doubles of the host's running sum; a heavier digest runs the host's loop on the device (td_quantile_warp).
+//     The arithmetic is written with explicit round-to-nearest operations on the device so that nvcc does not contract it into a
+//     fused multiply-add;
 //   * HLL: the raw sum keeps the host's order (r = 63 down to 0). The linear-counting branch needs log(), which neither CUDA nor
 //     glibc rounds correctly, so the device hands back -(zero registers) and the host finishes with hll_finish().
 #pragma once
@@ -95,24 +97,44 @@ GYSK_HD double td_interp(double prev_mean, double next, double target, double pr
 	return GYSK_DADD(prev_mean, GYSK_DMUL(GYSK_DADD(next, -prev_mean), GYSK_DDIV(GYSK_DADD(target, -prev_center), span)));
 }
 
-inline double td_quantile(const double *means, const uint64_t *weights, uint32_t n, double minv, double maxv, double q)
+// the centroids td_quantile_seq reads: separate mean / weight arrays (the public API) or an array of Centroid (a row's digest)
+struct TdArrays
+{
+	const double *means; const uint64_t *weights;
+	GYSK_HD double mean(uint32_t i) const { return means[i]; }
+	GYSK_HD uint64_t weight(uint32_t i) const { return weights[i]; }
+};
+struct TdCentroids
+{
+	const Centroid *c;
+	GYSK_HD double mean(uint32_t i) const { return c[i].mean; }
+	GYSK_HD uint64_t weight(uint32_t i) const { return c[i].weight; }
+};
+
+template <typename D>
+GYSK_HD double td_quantile_seq(const D &d, uint32_t n, double minv, double maxv, double q)
 {
 	if (!n) return NAN;
 	double total = 0;
-	for (uint32_t i = 0; i < n; ++i) total += (double)weights[i];
+	for (uint32_t i = 0; i < n; ++i) total = GYSK_DADD(total, (double)d.weight(i));
 	if (q <= 0) return minv;
 	if (q >= 1) return maxv;
 
-	const double target = q * total;
+	const double target = GYSK_DMUL(q, total);
 	double cum = 0, prev_center = 0, prev_mean = minv;
 
 	for (uint32_t i = 0; i < n; ++i) {
-		const double center = td_center(cum, weights[i]);
-		if (target < center) return td_interp(prev_mean, means[i], target, prev_center, center);
-		prev_center = center; prev_mean = means[i];
-		cum += (double)weights[i];
+		const double center = td_center(cum, d.weight(i));
+		if (target < center) return td_interp(prev_mean, d.mean(i), target, prev_center, center);
+		prev_center = center; prev_mean = d.mean(i);
+		cum = GYSK_DADD(cum, (double)d.weight(i));
 	}
 	return td_interp(prev_mean, maxv, target, prev_center, total);
+}
+
+inline double td_quantile(const double *means, const uint64_t *weights, uint32_t n, double minv, double maxv, double q)
+{
+	return td_quantile_seq(TdArrays {means, weights}, n, minv, maxv, q);
 }
 
 // ---- HLL estimate from the register histogram (hist64[r] = registers holding r, r clamped to 63) ----
@@ -148,7 +170,7 @@ GYSK_HD uint64_t cells_total(const HistCell *c, int nb, uint64_t *counts)
 	return t;
 }
 
-// everything but distinct_clients and the three t-digest quantiles (left NaN), which each side computes its own way
+// everything but distinct_clients and the three t-digest quantiles (left NaN), which summarize_warp adds
 GYSK_HD void summarize_fields(const SvcRaw &r, uint64_t id, gysk_svc_summary &o)
 {
 	memset(&o, 0, sizeof(o));
@@ -187,6 +209,91 @@ GYSK_HD void summarize_fields(const SvcRaw &r, uint64_t id, gysk_svc_summary &o)
 	o.curr_state = r.sst.state; o.curr_issue = r.sst.issue; o.issue_bit_hist = r.sst.issue_bits; o.high_resp_bit_hist = r.sst.high_bits;
 	o.td_count = r.td.total;
 }
+
+#ifdef __CUDACC__
+// the heavy digests' case of td_quantile_warp, one out-of-line copy instead of three inlined ones: no real stream reaches it
+static __device__ __noinline__ double td_quantile_heavy(const Centroid *c, uint32_t n, double minv, double maxv, double q)
+{
+	return td_quantile_seq(TdCentroids {c}, n, minv, maxv, q);
+}
+
+// td_quantile of the digest in shared memory (n <= TD_CAP centroids), by one warp: each lane takes a run of centroids, a uint64 prefix
+// over the warp gives every centroid the cumulative weight the host loop reaches, a ballot finds the first centre above the target.
+// That holds while the weights stay below 2^45: no sum of TD_CAP of them reaches 2^53. A heavier digest takes the host's loop itself,
+// whose running double sum rounds.
+__device__ inline double td_quantile_warp(const Centroid *c, uint32_t n, double minv, double maxv, double q, int lane)
+{
+	const uint32_t per = (n + 31) >> 5, b = min(n, lane * per), e = min(n, b + per);
+	unsigned long long s = 0, bits = 0;
+	for (uint32_t i = b; i < e; ++i) { s += c[i].weight; bits |= c[i].weight; }
+	static_assert(TD_CAP <= 256, "TD_CAP weights below 2^45 sum below 2^53");
+	if (__any_sync(0xffffffffu, bits >> 45)) return td_quantile_heavy(c, n, minv, maxv, q);
+	unsigned long long incl = s;
+	for (int o = 1; o < 32; o <<= 1) {
+		const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+		if (lane >= o) incl += t;
+	}
+	const unsigned long long total = __shfl_sync(0xffffffffu, incl, 31);
+	if (q <= 0) return minv;
+	if (q >= 1) return maxv;
+	const double target = __dmul_rn(q, (double)total);
+	unsigned long long cum = incl - s;
+	int hit = -1;
+	for (uint32_t i = b; i < e; ++i) {
+		if (target < td_center((double)cum, c[i].weight)) { hit = (int)i; break; }
+		cum += c[i].weight;
+	}
+	const unsigned mask = __ballot_sync(0xffffffffu, hit >= 0);
+	if (!mask) {
+		const Centroid l = c[n - 1];
+		return td_interp(l.mean, maxv, target, td_center((double)(total - l.weight), l.weight), (double)total);
+	}
+	const int src = __ffs(mask) - 1;
+	const int i = __shfl_sync(0xffffffffu, hit, src);
+	const unsigned long long cb = __shfl_sync(0xffffffffu, cum, src);
+	const double center = td_center((double)cb, c[i].weight);
+	if (i == 0) return td_interp(minv, c[0].mean, target, 0.0, center);
+	const Centroid p = c[i - 1];
+	return td_interp(p.mean, c[i].mean, target, td_center((double)(cb - p.weight), p.weight), center);
+}
+
+// the HLL register histogram of 2^p registers (p >= 4, 16-byte aligned) by one warp, into hist64 in shared memory; four registers per
+// load, as each lane's loads are serialised by the atomics behind them
+__device__ inline void hll_hist_warp(const uint8_t *regs, uint32_t p, uint32_t *hist64, int lane)
+{
+	hist64[lane] = 0; hist64[lane + 32] = 0;
+	__syncwarp();
+	const uint32_t *words = reinterpret_cast<const uint32_t *>(regs);
+	for (uint32_t i = lane; i < (1u << p) / 4u; i += 32) {
+		const uint32_t w = words[i];
+		for (int k = 0; k < 32; k += 8) atomicAdd(&hist64[min((w >> k) & 0xFFu, 63u)], 1u);
+	}
+	__syncwarp();
+}
+
+// the row of r by one warp: r in shared memory (hll_hist included when found), summ the warp's sizeof(gysk_svc_summary) bytes of
+// shared scratch, out the row in global memory. distinct_clients may come out as -(zero registers): the host finishes it with
+// hll_finish.
+__device__ inline void summarize_warp(const SvcRaw &r, uint64_t id, uint32_t hll_p, unsigned long long *summ, gysk_svc_summary *out, int lane)
+{
+	gysk_svc_summary &o = *reinterpret_cast<gysk_svc_summary *>(summ);
+	__syncwarp();
+	if (lane == 0) {
+		summarize_fields(r, id, o);
+		if (r.found) o.distinct_clients = hll_pending(r.hll_hist, hll_p);
+	}
+	const uint32_t nc = r.found ? min(r.td.n, (uint32_t)TD_CAP) : 0u;
+	if (nc) {
+		const double p50 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.50, lane);
+		const double p95 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.95, lane);
+		const double p99 = td_quantile_warp(r.cent, nc, r.td.minv, r.td.maxv, 0.99, lane);
+		if (lane == 0) { o.td_p50_us = p50; o.td_p95_us = p95; o.td_p99_us = p99; }
+	}
+	__syncwarp();
+	unsigned long long *dst = reinterpret_cast<unsigned long long *>(out);
+	if (lane < (int)(sizeof(gysk_svc_summary) / 8)) dst[lane] = summ[lane];
+}
+#endif
 
 // ---- per-process summary: the three MTASK_HIST p95 of AGGR_TASK_HIST_STATS (server/gy_mconnhdlr.cc:14648-14706) ----
 

@@ -491,6 +491,11 @@ int		gysk_merge_finish(gysk_engine *e, const void *d_gathered_slabs, uint32_t wo
 int		gysk_nccl_unique_id(uint8_t out[GYSK_NCCL_UNIQUE_ID_BYTES]);
 int		gysk_nccl_comm_init(gysk_engine *e, const uint8_t uid[GYSK_NCCL_UNIQUE_ID_BYTES], uint32_t nranks, uint32_t rank);
 int		gysk_merge_global(gysk_engine *e, void *nccl_comm);
+/* One gysk_svc_summary per logical id from the last finished merge: glob_id = the logical id, found = 0 for an id not in the map.
+ * The merge folds the last closed window, the all-time histogram, the connection counters, the HLL registers and the t-digest,
+ * and only those: nqrys_5min, nqrys_5day, nconns_active, active_kbytes, max_rtt_msec, cli_errors, ser_errors, curr_state,
+ * curr_issue, issue_bit_hist and high_resp_bit_hist are always 0, and p95_5min_resp_ms, p99_5min_resp_ms and p95_5day_resp_ms
+ * -1 (the percentiles of an empty histogram). */
 int		gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_svc_summary *out);
 int		gysk_query_flows_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_est *out);
 

@@ -1,5 +1,5 @@
 """Times the window read of every service (gysk_query_window) against the by-id read of the same ids (gysk_query_svcs), at
-100 K and 1 M services: ms per call, bytes copied device to host, and window_svcs_kernel's bytes read over its time (torch.profiler)
+100 K and 1 M services: ms per call, bytes copied device to host, and svc_summary_kernel's bytes read over its time (torch.profiler)
 against the 3.35 TB/s HBM3 data-sheet figure of the H100 SXM. Also the tick's whole read path, the steps of the shim's
 window_listener_states: one gysk_query_window_hosts call, then every host's rows encoded into LISTENER_STATE_NOTIFY batches of at
 most 512 records. Prints one JSON line per size, with the card's name and power limit.
@@ -19,13 +19,12 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gyeeta_b200 import engine as ge  # noqa: E402
 
-SVCRAW_BYTES = 6400          # sizeof(SvcRaw) (gysk_kernels.cuh): what gysk_query_svcs copies to the host per id
 ROW_BYTES = C.sizeof(ge.SvcSummary)
 HBM_TBS = 3.35
 
 
 def kernel_bytes_per_slot(hll_p, live0=1, live1=1):
-    """words window_svcs_kernel reads per slot (those of gather_svcs_kernel): cur / last / all histograms, both CONN_BITMAPs, the live
+    """words svc_summary_kernel reads per listed slot: cur / last / all histograms, both CONN_BITMAPs, the live
     ring slots of both levels, the qps / active-conn histograms (16 cells of 16 B each), conn counters, t-digest head, aux, state,
     all TD_CAP centroids, the HLL registers, the slot's id and its list entry; plus the 208-byte row it writes"""
     hist = 16 * 16
@@ -112,13 +111,13 @@ def probe(n, name):
         torch.cuda.synchronize()
     kus = 0.0
     for e in prof.key_averages():
-        if "window_svcs_kernel" in e.key:
+        if "svc_summary_kernel" in e.key:
             kus += getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0)
     kb = kernel_bytes_per_slot(eng.cfg.hll_p) * n
     eng.close()
     return dict(services=n, card=name, window_ms=round(ms_win, 3), window_runs_ms=t_win, tick_read_ms=round(ms_tick, 3), tick_runs_ms=t_tick,
                 tick_batches=batches[0], by_id_ms=round(ms_ids, 3), by_id_runs_ms=t_ids,
-                rows_equal=same, window_d2h_bytes=n * (ROW_BYTES + 16) + 8, by_id_d2h_bytes=n * SVCRAW_BYTES,
+                rows_equal=same, window_d2h_bytes=n * (ROW_BYTES + 16) + 8, by_id_d2h_bytes=n * ROW_BYTES,
                 by_id_launches=-(-n // 1024), window_kernel_ms=round(kus / 1e3, 3), window_kernel_bytes=kb,
                 window_kernel_tbs=round(kb / (kus * 1e-6) / 1e12, 3) if kus else None,
                 window_kernel_share_of_3_35_tbs=round(kb / (kus * 1e-6) / 1e12 / HBM_TBS, 3) if kus else None)

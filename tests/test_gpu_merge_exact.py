@@ -19,9 +19,8 @@ TD_HEAD_DTYPE = np.dtype([("total", "<u8"), ("minv", "<f8"), ("maxv", "<f8"), ("
 SLAB_DTYPE = np.dtype([("head", TD_HEAD_DTYPE), ("cent", po.CENTROID_DTYPE, (po.TD_CAP,))])
 assert TD_HEAD_DTYPE.itemsize == 32 and SLAB_DTYPE.itemsize == 4128          # SlabEntry: TdHead + TD_CAP centroids
 
-INT_FIELDS = ["found", "nqrys_5s", "total_resp_5sec", "p95_5s_resp_ms", "p99_5s_resp_ms", "p25_5s_resp_ms", "p95_all_resp_ms",
-              "p99_all_resp_ms", "nqrys_all", "max_resp_ms", "nconns_5s", "kbytes_5s", "nconns_all", "kbytes_all", "td_count"]
 DOUBLE_FIELDS = ["distinct_clients", "td_p50_us", "td_p95_us", "td_p99_us"]
+INT_FIELDS = [f for f, _ in ge.SvcSummary._fields_ if f not in DOUBLE_FIELDS]      # every other field, glob_id included
 
 NSVC, NHOSTS = 400, 40
 LATE = range(300, 340)                  # services whose first events arrive in the second window, after the map was set
@@ -66,10 +65,17 @@ def conn_only_events(rng, conn_ids, n, tsec):
 
 
 def window_events(rng, w, n, ids, conn_ids):
+    """the mixed stream; 2 % of its connection events are ACTIVE_CONN_STATS records, so the services' own rows carry active
+    connections and a max rtt"""
     ev = synth.gen_mixed(rng, n, NSVC, ntask=32, nhosts=NHOSTS, nclients=5000)
     if w == 0:
         late = ids[list(LATE)]
         ev = ev[(ev["type"] == ge.EV_TASK) | ~np.isin(ev["svc_id"], late)]
+    act = (ev["type"] >= ge.EV_CONNECT) & (ev["type"] <= ge.EV_CLOSE_SER) & (rng.random(len(ev)) < 0.02)
+    k = int(act.sum())
+    ev["type"][act] = ge.EV_ACTIVE
+    ev["flags"][act] = rng.integers(1, 200, k)                                       # active connections
+    ev["tsec"][act] = (rng.random(k) * 500).astype(np.float32).view(np.uint32)       # max rtt, msec
     return np.concatenate([ev, conn_only_events(rng, conn_ids, 200, 1)])
 
 
@@ -136,7 +142,9 @@ class Shards:
             for k, g in zip(np.asarray(flow_keys).tolist(), got):
                 cells = [int(tbl[r, L.gyo_cms_index(k, r, self.log2w)]) for r in range(self.depth)]
                 assert (g["count"], g["kbytes"]) == (min(c & M32 for c in cells), min(c >> 32 for c in cells)), hex(k)
-        # every logical service's answers, on every rank
+        # every logical service's answers, on every rank, each engine having just read its own services by id: a logical row
+        # carries none of their values
+        self.svc_rows = [s for e in self.engines for s in e.query_svcs([r.glob_id for r in e.query_window()[0]])]
         lib = ge.load_library()
         want = {lid: rs.summary(lid, lib) for lid in lids}
         for r, e in enumerate(self.engines):
@@ -180,6 +188,8 @@ def test_merged_answers_equal_the_restatement(world):
         sh.flush(5 * (w + 1))
         keys = np.unique(ev["flow_key"][(ev["type"] >= ge.EV_CONNECT) & (ev["type"] <= ge.EV_CLOSE_SER)])[:300]
         want = sh.check_merge(torch, keys)
+        # the by-id reads before the logical ones returned active connections and listener states
+        assert any(s["nconns_active"] for s in sh.svc_rows) and any(s["curr_state"] for s in sh.svc_rows)
         # the map covers what it should: every rank holds members of 9000 and 9001, the late services count from window 2 on
         assert want[9000]["td_count"] > 10_000 and want[9001]["td_count"] > 1000
         assert want[9003]["found"] == 1 and want[9003]["td_count"] == 0 and want[9003]["nconns_all"] > 0

@@ -1,7 +1,7 @@
 """gysk_query_window / gysk_query_tasks / gysk_query_task_window against the CPU oracle (make_pair / feed_both), over several
 flushes with idle eviction on: the rows are exactly the oracle's live ids, grouped by host and ordered by id; each service row is
-byte-equal to gysk_query_svcs of its id and equals a restatement of summarize_raw from the oracle's exports; each process row equals
-the reference's percentile rule on the exported task histograms."""
+byte-equal to gysk_query_svcs of its id and equals a restatement of the summary from the oracle's exports; each process row equals
+the reference's percentile rule on the exported task histograms. gysk_query_svcs over several chunks of live, unknown and zero ids."""
 import ctypes as C
 
 import numpy as np
@@ -76,8 +76,8 @@ def _pct(cls, t_is_int, hist, pcts):
 
 
 def _restate(eng, orc, id_, row):
-    """summarize_raw restated from the oracle's exports and its get_percentiles (gyo_hist_percentiles), and from the engine's
-    sketch exports (HLL registers, centroids) through the host estimators"""
+    """the service summary restated from the oracle's exports and its get_percentiles (gyo_hist_percentiles), and from the
+    engine's sketch exports (HLL registers, centroids) through the host estimators"""
     L = eng.L
     last = orc.export_hist(id_, ge.HIST_RESP_LAST)
     assert row.nqrys_5s == last[1] and row.total_resp_5sec == int(last[0]["sum"].sum())
@@ -263,6 +263,29 @@ def test_read_in_three_passes_and_recycled_slots():
     assert len(rows) == 1500 and {r.glob_id for r in rows} == set(int(i) for i in ids[:1000]) | set(int(i) for i in new)
     for r in rows[:: 50]:
         _restate(eng, orc, r.glob_id, r)
+
+
+def test_by_id_read_across_chunks():
+    """gysk_query_svcs of more than two 1024-id chunks, live ids shuffled among unknown ids and id 0: a live row is byte-equal to the
+    window row of its id, every other row to the not-found row (the id, found = 0, every other byte zero, NaN quantiles)"""
+    rng = np.random.default_rng(7)
+    eng = ge.Engine(max_svcs=1 << 12)
+    ids = (rng.choice(1 << 40, 1500, replace=False) + 1).astype(np.uint64)
+    ev = _stream(rng, ids, np.zeros(0, dtype=np.uint64), 30000)
+    eng.ingest_events(ev)
+    eng.sync()
+    eng.flush(5)
+    rows, n = eng.query_window()
+    win = {r.glob_id: bytes(r) for r in rows}
+    assert n > 1000
+    unknown = (rng.choice(1 << 40, 1200, replace=False) + (1 << 42)).astype(np.uint64)
+    q = np.concatenate([np.array(list(win), dtype=np.uint64), unknown, np.zeros(300, dtype=np.uint64)])[rng.permutation(n + 1500)]
+    assert len(q) > 2 * 1024
+    nan = float("nan")
+    for id_, r in zip(q.tolist(), _svcs_rows(eng, q)):
+        want = win.get(id_) or bytes(ge.SvcSummary(glob_id=id_, td_p50_us=nan, td_p95_us=nan, td_p99_us=nan))
+        assert bytes(r) == want, hex(id_)
+    eng.close()
 
 
 def test_same_stream_different_slots_gives_identical_bytes():

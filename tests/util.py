@@ -203,8 +203,9 @@ class MergeRestatement:
         return dict(last=last, all=all_, max_last=mx_last, max_all=mx_all, conn=conn, regs=regs)
 
     def summary(self, lid, eng_lib):
-        """the integer fields of gysk_query_logical, the HLL estimate and the t-digest answers of one logical service; the
-        percentiles of the summed cells go through the library's gysk_hist_percentiles, the host code both paths share"""
+        """every field of the gysk_query_logical row of one logical service; the percentiles of the summed cells go through the
+        library's gysk_hist_percentiles. The merge folds no rolling levels, active connections, errors or listener state: those
+        fields are 0, and the percentiles of the empty 5-min / 5-day histograms -1."""
         import ctypes as C
         c = self.cells(lid)
         pcts = np.array([95.0, 99.0, 25.0], dtype=np.float32)
@@ -218,7 +219,9 @@ class MergeRestatement:
 
         p5, pa = pct(c["last"], 3), pct(c["all"], 2)
         d = self.digest(lid)
-        return dict(found=1, nqrys_5s=int(c["last"]["count"].sum()) & M32, total_resp_5sec=int(c["last"]["sum"].sum()),
+        return dict(glob_id=int(lid), found=1, p95_5min_resp_ms=-1, p99_5min_resp_ms=-1, nqrys_5min=0, p95_5day_resp_ms=-1, nqrys_5day=0,
+                    nconns_active=0, active_kbytes=0, max_rtt_msec=0.0, cli_errors=0, ser_errors=0, curr_state=0, curr_issue=0,
+                    issue_bit_hist=0, high_resp_bit_hist=0, nqrys_5s=int(c["last"]["count"].sum()) & M32, total_resp_5sec=int(c["last"]["sum"].sum()),
                     p95_5s_resp_ms=p5[0], p99_5s_resp_ms=p5[1], p25_5s_resp_ms=p5[2], p95_all_resp_ms=pa[0], p99_all_resp_ms=pa[1],
                     nqrys_all=int(c["all"]["count"].sum()), max_resp_ms=c["max_all"], nconns_5s=c["conn"][0] & M32,
                     kbytes_5s=c["conn"][1] & M32, nconns_all=c["conn"][2], kbytes_all=c["conn"][3],
