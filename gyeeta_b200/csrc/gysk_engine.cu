@@ -280,31 +280,53 @@ uint32_t live_mask(const gysk_engine *e, int l)
 	return m;
 }
 
-int gather_svc(gysk_engine *e, uint64_t id)		// the single-id exports; result in e->h_svcraw[0]
+// the unit grid of the K_1 scale: q_j = (sin(pi (j/delta - 1/2)) + 1)/2 — libm on the host, the same expression as the oracle. The
+// device's grid and the pgtext export's compress both come from here.
+std::vector<double> k1_grid(uint32_t delta)
 {
-	e->h_qids[0] = id;
-	CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-	e->kernel_launches += launch_gather_svcs(e->st, e->d_qids, 1, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1), e->d_svcraw, e->stream);
-	CU(e, cudaMemcpyAsync(e->h_svcraw, e->d_svcraw, sizeof(SvcRaw), cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaStreamSynchronize(e->stream));
-	return post_launch(e, "gather_svcs");
+	std::vector<double> q(delta + 1);
+	for (uint32_t j = 0; j <= delta; ++j) q[j] = 0.5 * (sin(M_PI * ((double)j / (double)delta - 0.5)) + 1.0);
+	q[0] = 0.0; q[delta] = 1.0;
+	return q;
 }
+
+// the single-id reads: one piece of one id, whose raw state (`bytes` of it) the caller reads from the head of h_wstage
+template <typename Launch>
+int stage_one(gysk_engine *e, uint64_t id, size_t bytes, const char *what, Launch launch)
+{
+	return staged_read(e, &id, 1, 1, bytes, what, launch, RowsStay {});
+}
+
+int stage_svc_raw(gysk_engine *e, uint64_t id)
+{
+	return stage_one(e, id, sizeof(SvcRaw), "gather_svcs", [&](const unsigned long long *d_ids, uint32_t, uint32_t m) {
+		return launch_gather_svcs(e->st, d_ids, m, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1), reinterpret_cast<SvcRaw *>(e->d_wstage), e->stream);
+	});
+}
+
+// the two summary rows, by id (d_ids) or by slot (d_slots), into the stage
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_summary *)
+{
+	return launch_svc_summaries(e->st, d_ids, d_slots, m, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1),
+			reinterpret_cast<gysk_svc_summary *>(e->d_wstage), e->stream);
+}
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_task_summary *)
+{
+	return launch_task_summaries(e->st, d_ids, d_slots, m, reinterpret_cast<gysk_task_summary *>(e->d_wstage), e->stream);
+}
+SvcRows finish_rows(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
+CopyRows<gysk_task_summary> finish_rows(const gysk_engine *, gysk_task_summary *out) { return CopyRows<gysk_task_summary> {out}; }
 
 } // namespace
 
 // the linear-counting branch of the HLL estimate needs log(), which neither CUDA nor glibc rounds correctly: the host takes it
-int gysk::copy_svc_rows(gysk_engine *e, uint32_t k, gysk_svc_summary *out, const char *what)
+void gysk::SvcRows::operator()(const uint8_t *rows, uint32_t off, uint32_t m) const
 {
-	const gysk_svc_summary *rows = reinterpret_cast<const gysk_svc_summary *>(e->h_wstage);
-	CU(e, cudaMemcpyAsync(e->h_wstage, e->d_wstage, (size_t)k * sizeof(gysk_svc_summary), cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaStreamSynchronize(e->stream));
-	int rc = post_launch(e, what);
-	if (rc) return rc;
-	for (uint32_t i = 0; i < k; ++i) {
-		out[i] = rows[i];
-		out[i].distinct_clients = hll_finish(rows[i].distinct_clients, e->cfg.hll_p);
+	const gysk_svc_summary *r = reinterpret_cast<const gysk_svc_summary *>(rows);
+	for (uint32_t i = 0; i < m; ++i) {
+		out[off + i] = r[i];
+		out[off + i].distinct_clients = hll_finish(r[i].distinct_clients, hll_p);
 	}
-	return 0;
 }
 
 // ============================================================================================================
@@ -439,10 +461,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
 	st.td_delta = (double)cfg.td_compression;
 	{
-		// the unit grid of the K_1 scale: q_j = (sin(pi (j/delta - 1/2)) + 1)/2 — libm on the host, the same expression as the oracle
-		std::vector<double> qtab(cfg.td_compression + 1);
-		for (uint32_t j = 0; j <= cfg.td_compression; ++j) qtab[j] = 0.5 * (sin(M_PI * ((double)j / (double)cfg.td_compression - 0.5)) + 1.0);
-		qtab[0] = 0.0; qtab[cfg.td_compression] = 1.0;
+		const std::vector<double> qtab = k1_grid(cfg.td_compression);
 		double *d_q = nullptr;
 		A(dalloc(e, &d_q, qtab.size(), false));
 		if ((ce = cudaMemcpy(d_q, qtab.data(), qtab.size() * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "qtab", ce); return bail(GYSK_ERR_CUDA); }
@@ -501,14 +520,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		}
 	}
 	A(dalloc(e, &e->d_qids, (size_t)QCHUNK)); A(halloc(e, &e->h_qids, (size_t)QCHUNK));
-	A(dalloc(e, &e->d_svcraw, (size_t)1)); A(halloc(e, &e->h_svcraw, (size_t)1));
-	A(dalloc(e, &e->d_taskraw, (size_t)1)); A(halloc(e, &e->h_taskraw, (size_t)1));
-	A(dalloc(e, &e->d_hllout, (size_t)1 << cfg.hll_p)); A(halloc(e, &e->h_hllout, (size_t)1 << cfg.hll_p));
-	A(dalloc(e, &e->d_found, (size_t)1)); A(halloc(e, &e->h_found, (size_t)1));
-	A(dalloc(e, &e->d_flowout, (size_t)QCHUNK)); A(halloc(e, &e->h_flowout, (size_t)QCHUNK));
 	A(halloc(e, &e->h_counters, (size_t)CTR_MAX + 2));
-	A(dalloc(e, &e->d_wstage, (size_t)WIN_ROWS * sizeof(gysk_svc_summary), false));
-	A(halloc(e, &e->h_wstage, (size_t)WIN_ROWS * sizeof(gysk_svc_summary)));
+	A(dalloc(e, &e->d_wstage, STAGE_BYTES, false)); A(halloc(e, &e->h_wstage, STAGE_BYTES));
 #undef A
 
 	e->kernel_launches += launch_init_state(st, cfg.max_svcs + 1, cfg.max_tasks, e->stream);
@@ -620,14 +633,8 @@ int gysk_register_ids(gysk_engine *e, const uint64_t *ids, uint32_t n, int is_ta
 	if (!ids && n) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e);
 	CU(e, cudaSetDevice(e->dev));
-	for (uint32_t off = 0; off < n; off += QCHUNK) {
-		const uint32_t m = std::min(QCHUNK, n - off);
-		memcpy(e->h_qids, ids + off, (size_t)m * sizeof(uint64_t));
-		CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-		e->kernel_launches += launch_register(e->st, e->d_qids, m, is_task, e->stream);
-		CU(e, cudaStreamSynchronize(e->stream));
-	}
-	return post_launch(e, "register");
+	return staged_read(e, ids, n, QCHUNK, 0, "register",
+			[&](const unsigned long long *d_ids, uint32_t, uint32_t m) { return launch_register(e->st, d_ids, m, is_task, e->stream); }, RowsStay {});
 }
 
 // ---- ingest -----------------------------------------------------------------------------------------------
@@ -1110,32 +1117,11 @@ int gysk_evicted_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n)
 	return GYSK_OK;
 }
 
-// ---- queries ------------------------------------------------------------------------------------------------
-
-int gysk_query_svcs(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_svc_summary *out)
-{
-	CHECK_ENGINE(e);
-	if ((!ids || !out) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = submit_stage(e);
-	if (rc) return rc;
-	gysk_svc_summary *d_rows = reinterpret_cast<gysk_svc_summary *>(e->d_wstage);
-	for (uint32_t off = 0; off < n; off += QCHUNK) {
-		const uint32_t m = std::min(QCHUNK, n - off);
-		memcpy(e->h_qids, ids + off, (size_t)m * sizeof(uint64_t));
-		CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-		e->kernel_launches += launch_svc_summaries(e->st, e->d_qids, nullptr, m, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1), d_rows, e->stream);
-		if ((rc = copy_svc_rows(e, m, out + off, "svc_summaries"))) return rc;
-	}
-	return GYSK_OK;
-}
-
 } // extern "C"
 
-namespace {
+// ---- queries ------------------------------------------------------------------------------------------------
 
-static_assert(sizeof(gysk_task_summary) <= sizeof(gysk_svc_summary) && QCHUNK <= WIN_ROWS, "window stage holds a chunk of rows");
+namespace {
 
 // The slots a window read returns, in its order, at tmp.keys_a[0 .. want): the live slots of the selection grouped by host (a stable
 // radix sort of {host | slot} keys on the device), then by id inside each host (on the host: slot numbers depend on insertion races,
@@ -1181,9 +1167,76 @@ int window_list(gysk_engine *e, int is_task, int32_t host_idx, uint32_t flags, u
 	return 0;
 }
 
+// gysk_query_svcs / gysk_query_tasks: the rows of n ids, in QCHUNK pieces
+template <typename Row>
+int query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out, const char *what)
+{
+	CHECK_ENGINE(e);
+	if ((!ids || !out) && n) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e);
+	CU(e, cudaSetDevice(e->dev));
+	int rc = submit_stage(e);
+	if (rc) return rc;
+	return staged_read(e, ids, n, QCHUNK, sizeof(Row), what,
+			[&](const unsigned long long *d_ids, uint32_t, uint32_t m) { return launch_rows(e, d_ids, nullptr, m, out); }, finish_rows(e, out));
+}
+
+// gysk_query_window_hosts / gysk_query_task_window: the slots of window_list, summarised in WIN_ROWS pieces; hosts (optional) from
+// the same snapshot
+template <typename Row>
+int window_rows(gysk_engine *e, int32_t host_idx, uint32_t flags, Row *out, uint32_t *hosts, uint32_t cap, uint32_t *n, const char *what)
+{
+	CHECK_ENGINE(e);
+	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e);
+	CU(e, cudaSetDevice(e->dev));
+	int rc = sync_locked(e);
+	if (rc) return rc;
+	uint32_t total = 0;
+	if ((rc = window_list(e, std::is_same<Row, gysk_task_summary>::value, host_idx, flags, cap, &total))) return rc;
+	const uint32_t m = std::min(cap, total);
+	rc = staged_read<uint64_t>(e, nullptr, m, WIN_ROWS, sizeof(Row), what,
+			[&](const unsigned long long *, uint32_t off, uint32_t k) { return launch_rows(e, nullptr, e->tmp.keys_a + off, k, out); }, finish_rows(e, out));
+	if (rc) return rc;
+	// the within-host reorder of window_list leaves every position in its host's run
+	if (hosts) for (uint32_t i = 0; i < m; ++i) hosts[i] = (uint32_t)(e->win_keys[i] >> 32);
+	*n = total;
+	return GYSK_OK;
+}
+
+// gysk_topn_svcs / gysk_topn_tasks: the n best of nslots by one metric, the non-zero entries kept
+int topn_rows(gysk_engine *e, int is_task, int metric, int32_t host_idx, uint32_t n, gysk_topn_entry *out, uint32_t *nout, const char *what)
+{
+	GYSK_ENTER(e);
+	CU(e, cudaSetDevice(e->dev));
+	int rc = sync_locked(e);
+	if (rc) return rc;
+	uint32_t nslots = 0;
+	CU(e, cudaMemcpy(&nslots, is_task ? e->st.task_tbl.count : e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	nslots = std::min(nslots, is_task ? e->cfg.max_tasks : e->cfg.max_svcs);
+	gysk_topn_entry *d_out = reinterpret_cast<gysk_topn_entry *>(e->d_wstage);
+	const gysk_topn_entry *h_out = reinterpret_cast<const gysk_topn_entry *>(e->h_wstage);
+	CU(e, cudaMemsetAsync(d_out, 0, sizeof(gysk_topn_entry) * n, e->stream));
+	const int nl = launch_topn(e->st, e->tmp, nslots, is_task, metric, host_idx, n, d_out, e->stream);
+	if (nl < 0) return fail(e, GYSK_ERR_INVAL, (std::string(what) + ": sort failed").c_str());
+	e->kernel_launches += nl;
+	CU(e, cudaMemcpyAsync(e->h_wstage, d_out, sizeof(gysk_topn_entry) * n, cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	if ((rc = post_launch(e, what))) return rc;
+	uint32_t k = 0;
+	for (uint32_t i = 0; i < n; ++i) if (h_out[i].glob_id && h_out[i].score) out[k++] = h_out[i];
+	*nout = k;
+	return GYSK_OK;
+}
+
 } // namespace
 
 extern "C" {
+
+int gysk_query_svcs(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_svc_summary *out)
+{
+	return query_rows(e, ids, n, out, "svc_summaries");
+}
 
 int gysk_query_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_summary *out, uint32_t cap, uint32_t *n)
 {
@@ -1192,71 +1245,17 @@ int gysk_query_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc
 
 int gysk_query_window_hosts(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_summary *out, uint32_t *hosts, uint32_t cap, uint32_t *n)
 {
-	CHECK_ENGINE(e);
-	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = sync_locked(e);
-	if (rc) return rc;
-	uint32_t total = 0;
-	if ((rc = window_list(e, 0, host_idx, flags, cap, &total))) return rc;
-	const uint32_t m = std::min(cap, total);
-	gysk_svc_summary *d_rows = reinterpret_cast<gysk_svc_summary *>(e->d_wstage);
-	for (uint32_t off = 0; off < m; off += WIN_ROWS) {
-		const uint32_t k = std::min(WIN_ROWS, m - off);
-		e->kernel_launches += launch_svc_summaries(e->st, nullptr, e->tmp.keys_a + off, k, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1), d_rows, e->stream);
-		if ((rc = copy_svc_rows(e, k, out + off, "query_window"))) return rc;
-	}
-	// the within-host reorder of window_list leaves every position in its host's run
-	if (hosts) for (uint32_t i = 0; i < m; ++i) hosts[i] = (uint32_t)(e->win_keys[i] >> 32);
-	*n = total;
-	return GYSK_OK;
+	return window_rows(e, host_idx, flags, out, hosts, cap, n, "query_window");
 }
 
 int gysk_query_tasks(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_task_summary *out)
 {
-	CHECK_ENGINE(e);
-	if ((!ids || !out) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = submit_stage(e);
-	if (rc) return rc;
-	gysk_task_summary *d_rows = reinterpret_cast<gysk_task_summary *>(e->d_wstage), *h_rows = reinterpret_cast<gysk_task_summary *>(e->h_wstage);
-	for (uint32_t off = 0; off < n; off += QCHUNK) {
-		const uint32_t m = std::min(QCHUNK, n - off);
-		memcpy(e->h_qids, ids + off, (size_t)m * sizeof(uint64_t));
-		CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-		e->kernel_launches += launch_task_summaries(e->st, e->d_qids, nullptr, m, d_rows, e->stream);
-		CU(e, cudaMemcpyAsync(h_rows, d_rows, (size_t)m * sizeof(gysk_task_summary), cudaMemcpyDeviceToHost, e->stream));
-		CU(e, cudaStreamSynchronize(e->stream));
-		if ((rc = post_launch(e, "task_summaries"))) return rc;
-		memcpy(out + off, h_rows, (size_t)m * sizeof(gysk_task_summary));
-	}
-	return GYSK_OK;
+	return query_rows(e, ids, n, out, "task_summaries");
 }
 
 int gysk_query_task_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_task_summary *out, uint32_t cap, uint32_t *n)
 {
-	CHECK_ENGINE(e);
-	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = sync_locked(e);
-	if (rc) return rc;
-	uint32_t total = 0;
-	if ((rc = window_list(e, 1, host_idx, flags, cap, &total))) return rc;
-	const uint32_t m = std::min(cap, total);
-	gysk_task_summary *d_rows = reinterpret_cast<gysk_task_summary *>(e->d_wstage), *h_rows = reinterpret_cast<gysk_task_summary *>(e->h_wstage);
-	for (uint32_t off = 0; off < m; off += WIN_ROWS) {
-		const uint32_t k = std::min(WIN_ROWS, m - off);
-		e->kernel_launches += launch_task_summaries(e->st, nullptr, e->tmp.keys_a + off, k, d_rows, e->stream);
-		CU(e, cudaMemcpyAsync(h_rows, d_rows, (size_t)k * sizeof(gysk_task_summary), cudaMemcpyDeviceToHost, e->stream));
-		CU(e, cudaStreamSynchronize(e->stream));
-		if ((rc = post_launch(e, "task_window"))) return rc;
-		memcpy(out + off, h_rows, (size_t)k * sizeof(gysk_task_summary));
-	}
-	*n = total;
-	return GYSK_OK;
+	return window_rows(e, host_idx, flags, out, nullptr, cap, n, "task_window");
 }
 
 int gysk_export_hist(gysk_engine *e, uint64_t id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS], uint64_t *total, int64_t *maxv)
@@ -1270,8 +1269,8 @@ int gysk_export_hist(gysk_engine *e, uint64_t id, int which, gysk_hist_serial ou
 	CU(e, cudaSetDevice(e->dev));
 	int rc = submit_stage(e);
 	if (rc) return rc;
-	if ((rc = gather_svc(e, id))) return rc;
-	const SvcRaw &r = e->h_svcraw[0];
+	if ((rc = stage_svc_raw(e, id))) return rc;
+	const SvcRaw &r = *reinterpret_cast<const SvcRaw *>(e->h_wstage);
 	if (!r.found) return GYSK_ERR_NOENT;
 	if (which == GYSK_HIST_RESP_5MIN || which == GYSK_HIST_RESP_5DAY) {
 		hist_from_cells(r.lvl[which - GYSK_HIST_RESP_5MIN], 15, out, total, maxv, false);
@@ -1292,15 +1291,14 @@ int gysk_export_task_hist(gysk_engine *e, uint64_t id, int which, gysk_hist_seri
 	CU(e, cudaSetDevice(e->dev));
 	int rc = submit_stage(e);
 	if (rc) return rc;
-	e->h_qids[0] = id;
-	CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-	e->kernel_launches += launch_gather_tasks(e->st, e->d_qids, 1, e->d_taskraw, e->stream);
-	CU(e, cudaMemcpyAsync(e->h_taskraw, e->d_taskraw, sizeof(TaskRaw), cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaStreamSynchronize(e->stream));
-	if ((rc = post_launch(e, "gather_tasks"))) return rc;
-	if (!e->h_taskraw[0].found) return GYSK_ERR_NOENT;
+	rc = stage_one(e, id, sizeof(TaskRaw), "gather_tasks", [&](const unsigned long long *d_ids, uint32_t, uint32_t m) {
+		return launch_gather_tasks(e->st, d_ids, m, reinterpret_cast<TaskRaw *>(e->d_wstage), e->stream);
+	});
+	if (rc) return rc;
+	const TaskRaw &r = *reinterpret_cast<const TaskRaw *>(e->h_wstage);
+	if (!r.found) return GYSK_ERR_NOENT;
 	const int h = which - GYSK_HIST_TASK_CPU_PCT;
-	hist_from_cells(e->h_taskraw[0].h[h], h == 0 ? 14 : 15, out, total, maxv, true);
+	hist_from_cells(r.h[h], h == 0 ? 14 : 15, out, total, maxv, true);
 	return GYSK_OK;
 }
 
@@ -1313,8 +1311,8 @@ int gysk_export_conn_bitmap(gysk_engine *e, uint64_t id, int last_window, uint32
 	CU(e, cudaSetDevice(e->dev));
 	int rc = submit_stage(e);
 	if (rc) return rc;
-	if ((rc = gather_svc(e, id))) return rc;
-	const SvcRaw &r = e->h_svcraw[0];
+	if ((rc = stage_svc_raw(e, id))) return rc;
+	const SvcRaw &r = *reinterpret_cast<const SvcRaw *>(e->h_wstage);
 	if (!r.found) return GYSK_ERR_NOENT;
 	const uint32_t *bm = last_window ? r.bm_last : r.bm_cur;
 	for (int j = 0; j < GYSK_HIST_MAX_BUCKETS; ++j) { masks[j] = bm[j]; nconn_arr[j] = (uint8_t)__builtin_popcount(bm[j]); }
@@ -1329,13 +1327,12 @@ int gysk_export_hll(gysk_engine *e, uint64_t id, uint8_t *regs)
 	CU(e, cudaSetDevice(e->dev));
 	int rc = submit_stage(e);
 	if (rc) return rc;
-	e->kernel_launches += launch_gather_hll(e->st, id, e->d_hllout, e->d_found, e->stream);
-	CU(e, cudaMemcpyAsync(e->h_hllout, e->d_hllout, (size_t)1 << e->cfg.hll_p, cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaMemcpyAsync(e->h_found, e->d_found, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaStreamSynchronize(e->stream));
-	if ((rc = post_launch(e, "gather_hll"))) return rc;
-	if (!*e->h_found) return GYSK_ERR_NOENT;
-	memcpy(regs, e->h_hllout, (size_t)1 << e->cfg.hll_p);
+	rc = stage_one(e, id, HLL_STAGE_REGS + ((size_t)1 << e->cfg.hll_p), "gather_hll", [&](const unsigned long long *d_ids, uint32_t, uint32_t) {
+		return launch_gather_hll(e->st, d_ids, reinterpret_cast<int32_t *>(e->d_wstage), e->d_wstage + HLL_STAGE_REGS, e->stream);
+	});
+	if (rc) return rc;
+	if (!*reinterpret_cast<const int32_t *>(e->h_wstage)) return GYSK_ERR_NOENT;
+	memcpy(regs, e->h_wstage + HLL_STAGE_REGS, (size_t)1 << e->cfg.hll_p);
 	return GYSK_OK;
 }
 
@@ -1347,8 +1344,8 @@ int gysk_export_tdigest(gysk_engine *e, uint64_t id, double *means, uint64_t *we
 	CU(e, cudaSetDevice(e->dev));
 	int rc = submit_stage(e);
 	if (rc) return rc;
-	if ((rc = gather_svc(e, id))) return rc;
-	const SvcRaw &r = e->h_svcraw[0];
+	if ((rc = stage_svc_raw(e, id))) return rc;
+	const SvcRaw &r = *reinterpret_cast<const SvcRaw *>(e->h_wstage);
 	if (!r.found) return GYSK_ERR_NOENT;
 	const uint32_t nc = std::min<uint32_t>(std::min<uint32_t>(r.td.n, TD_CAP), cap);
 	for (uint32_t c = 0; c < nc; ++c) { means[c] = r.cent[c].mean; weights[c] = r.cent[c].weight; }
@@ -1424,9 +1421,7 @@ int gysk_tdigest_to_pgtext(const double *means, const uint64_t *weights, uint32_
 static uint32_t host_td_compress(const double *means, const uint64_t *w, uint32_t n, uint32_t delta, double *om, uint64_t *ow)
 {
 	if (!n) return 0;
-	std::vector<double> qtab(delta + 1);
-	for (uint32_t j = 0; j <= delta; ++j) qtab[j] = 0.5 * (sin(M_PI * ((double)j / (double)delta - 0.5)) + 1.0);
-	qtab[0] = 0.0; qtab[delta] = 1.0;
+	const std::vector<double> qtab = k1_grid(delta);
 	uint64_t W = 0, pref = 0, cw = 0;
 	for (uint32_t i = 0; i < n; ++i) W += w[i];
 	uint32_t nout = 0, cur = 0;
@@ -1474,72 +1469,23 @@ int gysk_query_flows(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_
 	CU(e, cudaSetDevice(e->dev));
 	int rc = submit_stage(e);
 	if (rc) return rc;
-	for (uint32_t off = 0; off < n; off += QCHUNK) {
-		const uint32_t m = std::min(QCHUNK, n - off);
-		memcpy(e->h_qids, keys + off, (size_t)m * sizeof(uint64_t));
-		CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-		e->kernel_launches += launch_query_flows(e->st, e->d_qids, m, last_window, e->d_flowout, e->stream);
-		CU(e, cudaMemcpyAsync(e->h_flowout, e->d_flowout, (size_t)m * sizeof(gysk_flow_est), cudaMemcpyDeviceToHost, e->stream));
-		CU(e, cudaStreamSynchronize(e->stream));
-		memcpy(out + off, e->h_flowout, (size_t)m * sizeof(gysk_flow_est));
-	}
-	return post_launch(e, "query_flows");
+	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_est), "query_flows", [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
+		return launch_query_flows(e->st, d_keys, m, last_window, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
+	}, CopyRows<gysk_flow_est> {out});
 }
 
 int gysk_topn_svcs(gysk_engine *e, int metric, int32_t host_idx, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
 {
 	CHECK_ENGINE(e);
 	if (!out || !nout || n == 0 || n > 64 || metric < GYSK_TOPN_QPS || metric > GYSK_TOPN_ISSUE) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = sync_locked(e);
-	if (rc) return rc;
-	uint32_t nslots = 0;
-	CU(e, cudaMemcpy(&nslots, e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-	nslots = std::min(nslots, e->cfg.max_svcs);
-	gysk_topn_entry *d_out = reinterpret_cast<gysk_topn_entry *>(e->d_flowout);		// QCHUNK * 16 B >= 64 * 24 B
-	CU(e, cudaMemsetAsync(d_out, 0, sizeof(gysk_topn_entry) * n, e->stream));
-	{
-		const int nl = launch_topn(e->st, e->tmp, nslots, metric, host_idx, n, d_out, e->stream);
-		if (nl < 0) return fail(e, GYSK_ERR_INVAL, "gysk_topn_svcs: sort failed");
-		e->kernel_launches += nl;
-	}
-	gysk_topn_entry *h_out = reinterpret_cast<gysk_topn_entry *>(e->h_flowout);
-	CU(e, cudaMemcpyAsync(h_out, d_out, sizeof(gysk_topn_entry) * n, cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaStreamSynchronize(e->stream));
-	if ((rc = post_launch(e, "topn"))) return rc;
-	uint32_t k = 0;
-	for (uint32_t i = 0; i < n; ++i) if (h_out[i].glob_id && h_out[i].score) out[k++] = h_out[i];
-	*nout = k;
-	return GYSK_OK;
+	return topn_rows(e, 0, metric, host_idx, n, out, nout, "gysk_topn_svcs");
 }
 
 int gysk_topn_tasks(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
 {
 	CHECK_ENGINE(e);
 	if (!out || !nout || n == 0 || n > 64 || metric < GYSK_TOPN_TASK_CPU || metric > GYSK_TOPN_TASK_BLKIO_DELAY) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = sync_locked(e);
-	if (rc) return rc;
-	uint32_t ntasks = 0;
-	CU(e, cudaMemcpy(&ntasks, e->st.task_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-	ntasks = std::min(ntasks, e->cfg.max_tasks);
-	gysk_topn_entry *d_out = reinterpret_cast<gysk_topn_entry *>(e->d_flowout);		// QCHUNK * 16 B >= 64 * 24 B
-	CU(e, cudaMemsetAsync(d_out, 0, sizeof(gysk_topn_entry) * n, e->stream));
-	{
-		const int nl = launch_topn_tasks(e->st, e->tmp, ntasks, metric, n, d_out, e->stream);
-		if (nl < 0) return fail(e, GYSK_ERR_INVAL, "gysk_topn_tasks: sort failed");
-		e->kernel_launches += nl;
-	}
-	gysk_topn_entry *h_out = reinterpret_cast<gysk_topn_entry *>(e->h_flowout);
-	CU(e, cudaMemcpyAsync(h_out, d_out, sizeof(gysk_topn_entry) * n, cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaStreamSynchronize(e->stream));
-	if ((rc = post_launch(e, "topn_tasks"))) return rc;
-	uint32_t k = 0;
-	for (uint32_t i = 0; i < n; ++i) if (h_out[i].glob_id && h_out[i].score) out[k++] = h_out[i];
-	*nout = k;
-	return GYSK_OK;
+	return topn_rows(e, 1, metric, -1, n, out, nout, "gysk_topn_tasks");
 }
 
 int gysk_query_host_summary(gysk_engine *e, uint32_t host_idx, gysk_host_summary *out)

@@ -144,15 +144,11 @@ struct gysk_engine
 	cudaEvent_t		ev_raw_copied[gysk::NBUF] {}, ev_raw_done[gysk::NBUF] {};
 	int			raw_cur {0};
 
-	// query scratch
-	unsigned long long	*d_qids {nullptr}, *h_qids {nullptr};
-	gysk::SvcRaw		*d_svcraw {nullptr}, *h_svcraw {nullptr};	// the single-id exports: one entry each
-	gysk::TaskRaw		*d_taskraw {nullptr}, *h_taskraw {nullptr};
-	uint8_t			*d_hllout {nullptr}, *h_hllout {nullptr};
-	int32_t			*d_found {nullptr}, *h_found {nullptr};
-	gysk_flow_est		*d_flowout {nullptr}, *h_flowout {nullptr};
+	// query scratch (staged_read). The stage is only valid under mtx: every read copies its result out of it before it returns.
+	unsigned long long	*d_qids {nullptr}, *h_qids {nullptr};		// a piece of a read's input: QCHUNK ids, keys or logical indices
 	unsigned long long	*h_counters {nullptr};
-	uint8_t			*d_wstage {nullptr}, *h_wstage {nullptr};	// summary rows: WIN_ROWS per window-read pass, QCHUNK per by-id pass
+	uint8_t			*d_wstage {nullptr}, *h_wstage {nullptr};	// every read's output: WIN_ROWS summary rows per window-read pass,
+										// QCHUNK rows per by-id pass, one id's raw state, the top-N entries
 	std::vector<uint64_t>	win_keys, win_ids;			// a window read's {host | slot} keys and their ids on the host
 	std::vector<std::pair<uint64_t, uint64_t>> win_rows;		// ... as {id, slot}, ordered within each host
 
@@ -199,8 +195,6 @@ int drain_all(gysk_engine *e);
 int sync_locked(gysk_engine *e);
 int collect_evicted(gysk_engine *e, bool wait);
 void merge_release(gysk_engine *e);
-// the first k service rows of the window stage -> out (synchronises the stream), distinct_clients finished with hll_finish
-int copy_svc_rows(gysk_engine *e, uint32_t k, gysk_svc_summary *out, const char *what);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 // readers: hand every thread's partial chunk to the device, then take the engine
@@ -234,5 +228,53 @@ int halloc(gysk_engine *e, T **p, size_t n)
 	*p = static_cast<T *>(q);
 	return 0;
 }
+
+// ---- the read path: one stage for every read -------------------------------------------------------------------
+
+constexpr size_t STAGE_BYTES = (size_t)WIN_ROWS * sizeof(gysk_svc_summary);
+constexpr size_t HLL_STAGE_REGS = 16;		// gysk_export_hll: the found word at the head of the stage, the registers from here on
+static_assert(sizeof(gysk_task_summary) <= sizeof(gysk_svc_summary) && QCHUNK <= WIN_ROWS, "the stage holds a chunk of rows");
+static_assert(sizeof(SvcRaw) <= STAGE_BYTES && sizeof(TaskRaw) <= STAGE_BYTES, "the stage holds one id's raw state");
+static_assert(HLL_STAGE_REGS + (1u << 16) <= STAGE_BYTES, "the stage holds the found word and 2^16 HLL registers");
+static_assert(QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES && 64 * sizeof(gysk_topn_entry) <= STAGE_BYTES, "the stage holds the flow and top-N rows");
+
+// A staged read, engine mutex held. The optional input (ids, flow keys or logical indices) travels through h_qids / d_qids in pieces
+// of `piece` entries; without one (the window reads) the pieces only cut the n rows. For each piece, launch(d_in, off, m) writes m
+// rows of row_bytes into d_wstage and returns its kernel launches; the rows come back into h_wstage, the stream is synchronised, and
+// finish(h_wstage, off, m) copies them out.
+template <typename In, typename Launch, typename Finish>
+int staged_read(gysk_engine *e, const In *in, uint32_t n, uint32_t piece, size_t row_bytes, const char *what, Launch launch, Finish finish)
+{
+	static_assert(sizeof(In) <= sizeof(unsigned long long), "h_qids holds a piece of the input");
+	for (uint32_t off = 0; off < n; off += piece) {
+		const uint32_t m = std::min(piece, n - off);
+		if (in) {
+			memcpy(e->h_qids, in + off, (size_t)m * sizeof(In));
+			CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, (size_t)m * sizeof(In), cudaMemcpyHostToDevice, e->stream));
+		}
+		e->kernel_launches += launch(in ? e->d_qids : nullptr, off, m);
+		if (row_bytes) CU(e, cudaMemcpyAsync(e->h_wstage, e->d_wstage, m * row_bytes, cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaStreamSynchronize(e->stream));
+		int rc = post_launch(e, what);
+		if (rc) return rc;
+		finish(e->h_wstage, off, m);
+	}
+	return 0;
+}
+
+// finish callbacks: the rows as they are; service rows, whose HLL estimate the host finishes (hll_finish); or nothing, when the
+// read has no rows (gysk_register_ids) or its caller reads them from the stage itself (the single-id exports)
+template <typename T> struct CopyRows
+{
+	T *out;
+	void operator()(const uint8_t *rows, uint32_t off, uint32_t m) const { memcpy(out + off, rows, (size_t)m * sizeof(T)); }
+};
+struct SvcRows
+{
+	uint32_t hll_p;
+	gysk_svc_summary *out;
+	void operator()(const uint8_t *rows, uint32_t off, uint32_t m) const;
+};
+struct RowsStay { void operator()(const uint8_t *, uint32_t, uint32_t) const {} };
 
 } // namespace gysk

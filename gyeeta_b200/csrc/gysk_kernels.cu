@@ -1462,6 +1462,23 @@ __global__ void rebuild_table_kernel(DevState st, uint32_t max_svcs)
 // read side: one warp per queried id
 // ---------------------------------------------------------------------------------------------------
 
+// row q of a warp's read: by id (ids != nullptr: lane 0 looks it up, id 0 and unknown ids give slot -1) or by slot (the window reads:
+// the id from the table's slot -> id array)
+struct Resolved { int slot; unsigned long long id; };
+__device__ __forceinline__ Resolved resolve_warp(const IdTable &t, const unsigned long long *__restrict__ ids, const unsigned long long *__restrict__ slots,
+		uint32_t q, int lane)
+{
+	Resolved r;
+	if (ids) {
+		r.id = ids[q];
+		r.slot = -1;
+		if (lane == 0 && r.id) r.slot = table_lookup(t, r.id, false);
+		r.slot = __shfl_sync(0xffffffffu, r.slot, 0);
+	}
+	else { r.slot = (int)(uint32_t)slots[q]; r.id = t.slot_id[r.slot]; }
+	return r;
+}
+
 // the warp's copy of one slot's state (all but id / found / slot and the HLL register histogram)
 __device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32_t max_svcs, uint32_t live0, uint32_t live1, SvcRaw &o, int lane)
 {
@@ -1504,13 +1521,10 @@ __global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const uns
 
 	if (q >= n) return;
 	SvcRaw &o = out[q];
-	const unsigned long long id = ids[q];
-	int slot = -1;
-	if (lane == 0 && id) slot = table_lookup(st.svc_tbl, id, false);
-	slot = __shfl_sync(0xffffffffu, slot, 0);
-	if (lane == 0) { o.id = id; o.found = slot >= 0; o.slot = (uint32_t)slot; }
-	if (slot < 0) return;
-	gather_slot(st, slot, max_svcs, live0, live1, o, lane);
+	const Resolved r = resolve_warp(st.svc_tbl, ids, nullptr, q, lane);
+	if (lane == 0) { o.id = r.id; o.found = r.slot >= 0; o.slot = (uint32_t)r.slot; }
+	if (r.slot < 0) return;
+	gather_slot(st, r.slot, max_svcs, live0, live1, o, lane);
 }
 
 // ---- window reads (gysk_query_window / gysk_query_task_window) ----
@@ -1568,21 +1582,13 @@ __global__ void __launch_bounds__(SUMM_WARPS * 32) svc_summary_kernel(DevState s
 
 	if (q >= n) return;
 	SvcRaw &r = raw[wid];
-	int slot;
-	unsigned long long id;
-	if (ids) {
-		id = ids[q];
-		slot = -1;
-		if (lane == 0 && id) slot = table_lookup(st.svc_tbl, id, false);
-		slot = __shfl_sync(0xffffffffu, slot, 0);
+	const Resolved s = resolve_warp(st.svc_tbl, ids, slots, q, lane);
+	if (lane == 0) { r.id = s.id; r.found = s.slot >= 0; r.slot = (uint32_t)s.slot; }
+	if (s.slot >= 0) {
+		gather_slot(st, s.slot, max_svcs, live0, live1, r, lane);
+		hll_hist_warp(st.hll + ((size_t)s.slot << st.hll_p), st.hll_p, r.hll_hist, lane);
 	}
-	else { slot = (int)(uint32_t)slots[q]; id = st.slot_id[slot]; }
-	if (lane == 0) { r.id = id; r.found = slot >= 0; r.slot = (uint32_t)slot; }
-	if (slot >= 0) {
-		gather_slot(st, slot, max_svcs, live0, live1, r, lane);
-		hll_hist_warp(st.hll + ((size_t)slot << st.hll_p), st.hll_p, r.hll_hist, lane);
-	}
-	summarize_warp(r, id, st.hll_p, summ[wid], out + q, lane);
+	summarize_warp(r, s.id, st.hll_p, summ[wid], out + q, lane);
 }
 
 // one warp per process: by id (ids != nullptr: looked up, unknown ids give found = 0) or by slot (the window read)
@@ -1594,47 +1600,37 @@ __global__ void __launch_bounds__(128) task_summary_kernel(DevState st, const un
 	const uint32_t q = blockIdx.x * 4 + wid;
 
 	if (q >= n) return;
-	int slot;
-	unsigned long long id;
-	if (ids) {
-		id = ids[q];
-		slot = -1;
-		if (lane == 0 && id) slot = table_lookup(st.task_tbl, id, false);
-		slot = __shfl_sync(0xffffffffu, slot, 0);
-	}
-	else { slot = (int)(uint32_t)slots[q]; id = st.task_slot_id[slot]; }
-	if (slot < 0) {
-		if (lane == 0) { gysk_task_summary z; memset(&z, 0, sizeof(z)); z.aggr_task_id = id; out[q] = z; }
+	const Resolved s = resolve_warp(st.task_tbl, ids, slots, q, lane);
+	if (s.slot < 0) {
+		if (lane == 0) { gysk_task_summary z; memset(&z, 0, sizeof(z)); z.aggr_task_id = s.id; out[q] = z; }
 		return;
 	}
-	for (int i = lane; i < 3 * HIST_CELLS; i += 32) h[wid][i] = st.task_hist[(size_t)slot * 3 * HIST_CELLS + i];
-	if (lane < 3) h[wid][3 * HIST_CELLS + lane] = st.task_last[(size_t)slot * 3 + lane];
+	for (int i = lane; i < 3 * HIST_CELLS; i += 32) h[wid][i] = st.task_hist[(size_t)s.slot * 3 * HIST_CELLS + i];
+	if (lane < 3) h[wid][3 * HIST_CELLS + lane] = st.task_last[(size_t)s.slot * 3 + lane];
 	__syncwarp();
-	if (lane == 0) summarize_task(h[wid], h[wid] + 3 * HIST_CELLS, id, st.task_slot_host[slot], out[q]);
+	if (lane == 0) summarize_task(h[wid], h[wid] + 3 * HIST_CELLS, s.id, st.task_slot_host[s.slot], out[q]);
 }
 
-__global__ void gather_tasks_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, TaskRaw *__restrict__ out)
+// the single-id export gysk_export_task_hist: one warp per id, the id's three histograms
+__global__ void __launch_bounds__(128) gather_tasks_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, TaskRaw *__restrict__ out)
 {
-	const uint32_t q = blockIdx.x;
+	const int lane = threadIdx.x & 31;
+	const uint32_t q = blockIdx.x * 4 + (threadIdx.x >> 5);
+
 	if (q >= n) return;
-	__shared__ int sslot;
-	if (threadIdx.x == 0) {
-		const unsigned long long id = ids[q];
-		sslot = id ? table_lookup(st.task_tbl, id, false) : -1;
-		out[q].id = id; out[q].found = sslot >= 0; out[q].slot = (uint32_t)sslot;
-	}
-	__syncthreads();
-	if (sslot < 0) return;
-	if (threadIdx.x < 3 * HIST_CELLS) (&out[q].h[0][0])[threadIdx.x] = st.task_hist[(size_t)sslot * 3 * HIST_CELLS + threadIdx.x];
+	const Resolved r = resolve_warp(st.task_tbl, ids, nullptr, q, lane);
+	if (lane == 0) { out[q].id = r.id; out[q].found = r.slot >= 0; out[q].slot = (uint32_t)r.slot; }
+	if (r.slot < 0) return;
+	for (int i = lane; i < 3 * HIST_CELLS; i += 32) (&out[q].h[0][0])[i] = st.task_hist[(size_t)r.slot * 3 * HIST_CELLS + i];
 }
 
-__global__ void gather_hll_kernel(DevState st, unsigned long long id, uint8_t *__restrict__ out, int32_t *found)
+// gysk_export_hll: the registers of one id (ids[0]); every warp resolves the id itself
+__global__ void gather_hll_kernel(DevState st, const unsigned long long *__restrict__ ids, int32_t *found, uint8_t *__restrict__ out)
 {
-	__shared__ int sslot;
-	if (threadIdx.x == 0) { sslot = id ? table_lookup(st.svc_tbl, id, false) : -1; *found = sslot >= 0; }
-	__syncthreads();
-	if (sslot < 0) return;
-	const uint8_t *regs = st.hll + ((size_t)sslot << st.hll_p);
+	const int slot = resolve_warp(st.svc_tbl, ids, nullptr, 0, threadIdx.x & 31).slot;
+	if (threadIdx.x == 0) *found = slot >= 0;
+	if (slot < 0) return;
+	const uint8_t *regs = st.hll + ((size_t)slot << st.hll_p);
 	for (uint32_t i = threadIdx.x; i < (1u << st.hll_p); i += blockDim.x) out[i] = regs[i];
 }
 
@@ -1928,7 +1924,22 @@ __global__ void topn_score_kernel(DevState st, uint32_t nslots, int metric, int 
 	keys[slot] = (score << 32) | slot;
 }
 
-__global__ void topn_pick_kernel(DevState st, const unsigned long long *__restrict__ sorted, uint32_t nslots, uint32_t want, gysk_topn_entry *__restrict__ out)
+// top-N aggregated processes of the last closed window by cpu / cpu delay / blkio delay: the atask_top_cpu_ / _cpu_delay_ /
+// _io_delay_ queues of partha_aggr_task_state (server/gy_mconnhdlr.cc:10020-10065; entries with a zero metric never enter)
+__global__ void topn_task_score_kernel(DevState st, uint32_t ntasks, int metric, unsigned long long *__restrict__ keys, unsigned long long *d_n)
+{
+	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
+	if (slot == 0) *d_n = ntasks;
+	if (slot >= ntasks) return;
+	unsigned long long score = st.task_slot_id[slot] ? (unsigned long long)st.task_last[(size_t)slot * 3 + metric].sum : 0ull;
+	if ((long long)score < 0) score = 0;
+	if (score > 0xFFFFFFFFull) score = 0xFFFFFFFFull;
+	keys[slot] = (score << 32) | slot;
+}
+
+// the want best of the sorted keys, with the id and host of their slots (services' or processes')
+__global__ void topn_pick_kernel(const unsigned long long *__restrict__ slot_id, const uint32_t *__restrict__ slot_host,
+		const unsigned long long *__restrict__ sorted, uint32_t nslots, uint32_t want, gysk_topn_entry *__restrict__ out)
 {
 	const uint32_t i = threadIdx.x;
 	if (i >= want) return;
@@ -1936,21 +1947,24 @@ __global__ void topn_pick_kernel(DevState st, const unsigned long long *__restri
 	if (i < nslots) {
 		const unsigned long long k = sorted[nslots - 1 - i];		// descending
 		const uint32_t slot = (uint32_t)k;
-		o.glob_id = st.slot_id[slot]; o.score = k >> 32; o.host_idx = st.slot_host[slot];
+		o.glob_id = slot_id[slot]; o.score = k >> 32; o.host_idx = slot_host[slot];
 	}
 	out[i] = o;
 }
 
-int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int metric, int host_filter, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s)
+int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
+		gysk_topn_entry *d_out, cudaStream_t s)
 {
 	if (!nslots) return 0;
 	unsigned long long *d_n = st.counters + CTR_NKEYS;
 	int which = 0, launches = 2;
-	topn_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, host_filter, tmp.keys_a, d_n);
+	if (is_task) topn_task_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, tmp.keys_a, d_n);
+	else topn_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, host_filter, tmp.keys_a, d_n);
 	const int sorted = launch_radix_sort(tmp, d_n, nslots, 32, 64, 64, 64, &which, s);
 	if (sorted < 0) return sorted;
 	launches += sorted;
-	topn_pick_kernel<<<1, 64, 0, s>>>(st, which ? tmp.keys_b : tmp.keys_a, nslots, want, d_out);
+	topn_pick_kernel<<<1, 64, 0, s>>>(is_task ? st.task_slot_id : st.slot_id, is_task ? st.task_slot_host : st.slot_host,
+			which ? tmp.keys_b : tmp.keys_a, nslots, want, d_out);
 	return launches;
 }
 
@@ -1971,45 +1985,6 @@ int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s)
 {
 	task_flush_kernel<<<div_up((uint64_t)max_tasks * 3, 256), 256, 0, s>>>(st, max_tasks);
 	return 1;
-}
-
-// top-N aggregated processes of the last closed window by cpu / cpu delay / blkio delay: the atask_top_cpu_ / _cpu_delay_ /
-// _io_delay_ queues of partha_aggr_task_state (server/gy_mconnhdlr.cc:10020-10065; entries with a zero metric never enter)
-__global__ void topn_task_score_kernel(DevState st, uint32_t ntasks, int metric, unsigned long long *__restrict__ keys, unsigned long long *d_n)
-{
-	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
-	if (slot == 0) *d_n = ntasks;
-	if (slot >= ntasks) return;
-	unsigned long long score = st.task_slot_id[slot] ? (unsigned long long)st.task_last[(size_t)slot * 3 + metric].sum : 0ull;
-	if ((long long)score < 0) score = 0;
-	if (score > 0xFFFFFFFFull) score = 0xFFFFFFFFull;
-	keys[slot] = (score << 32) | slot;
-}
-
-__global__ void topn_task_pick_kernel(DevState st, const unsigned long long *__restrict__ sorted, uint32_t ntasks, uint32_t want, gysk_topn_entry *__restrict__ out)
-{
-	const uint32_t i = threadIdx.x;
-	if (i >= want) return;
-	gysk_topn_entry o; o.glob_id = 0; o.score = 0; o.host_idx = 0; o.pad = 0;
-	if (i < ntasks) {
-		const unsigned long long k = sorted[ntasks - 1 - i];		// descending
-		const uint32_t slot = (uint32_t)k;
-		o.glob_id = st.task_slot_id[slot]; o.score = k >> 32; o.host_idx = st.task_slot_host[slot];
-	}
-	out[i] = o;
-}
-
-int launch_topn_tasks(const DevState &st, const SortTemp &tmp, uint32_t ntasks, int metric, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s)
-{
-	if (!ntasks) return 0;
-	int which = 0, launches = 2;
-	unsigned long long *d_n = st.counters + CTR_NKEYS;
-	topn_task_score_kernel<<<div_up(ntasks, 256), 256, 0, s>>>(st, ntasks, metric, tmp.keys_a, d_n);
-	const int sorted = launch_radix_sort(tmp, d_n, ntasks, 32, 64, 64, 64, &which, s);
-	if (sorted < 0) return sorted;
-	launches += sorted;
-	topn_task_pick_kernel<<<1, 64, 0, s>>>(st, which ? tmp.keys_b : tmp.keys_a, ntasks, want, d_out);
-	return launches;
 }
 
 int launch_flush(const DevState &st, uint32_t nslots, HistCell *ring_plane0, HistCell *ring_plane1, uint32_t tsec, uint32_t idle_secs,
@@ -2042,13 +2017,13 @@ int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint
 int launch_gather_tasks(const DevState &st, const unsigned long long *d_ids, uint32_t n, TaskRaw *d_out, cudaStream_t s)
 {
 	if (!n) return 0;
-	gather_tasks_kernel<<<n, 64, 0, s>>>(st, d_ids, n, d_out);
+	gather_tasks_kernel<<<div_up(n, 4), 128, 0, s>>>(st, d_ids, n, d_out);
 	return 1;
 }
 
-int launch_gather_hll(const DevState &st, unsigned long long id, uint8_t *d_out, int32_t *d_found, cudaStream_t s)
+int launch_gather_hll(const DevState &st, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s)
 {
-	gather_hll_kernel<<<1, 256, 0, s>>>(st, id, d_out, d_found);
+	gather_hll_kernel<<<1, 256, 0, s>>>(st, d_ids, found, d_out);
 	return 1;
 }
 

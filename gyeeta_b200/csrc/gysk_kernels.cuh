@@ -120,16 +120,18 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
 int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo1, int hi1, int lo2, int hi2, int *which, cudaStream_t s);
-int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int metric, int host_filter, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
-int launch_topn_tasks(const DevState &st, const SortTemp &tmp, uint32_t ntasks, int metric, uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
+// the want best services (host_filter < 0: of every host) or processes (is_task) of nslots by one metric; -1: sort failed
+int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
+		gysk_topn_entry *d_out, cudaStream_t s);
 int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s);
 int launch_flush(const DevState &st, uint32_t max_svcs, HistCell *ring_plane0, HistCell *ring_plane1, uint32_t tsec, uint32_t idle_secs,
 		uint32_t live_mask0, uint32_t live_mask1, cudaStream_t s);
 int launch_rebuild_table(const DevState &st, uint32_t max_svcs, cudaStream_t s);
+// the single-id exports: the raw state of n ids (id 0 and unknown ids: found = 0); the HLL registers of the id d_ids[0]
 int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint32_t n, uint32_t max_svcs, uint32_t live_mask0, uint32_t live_mask1,
 		SvcRaw *d_out, cudaStream_t s);
 int launch_gather_tasks(const DevState &st, const unsigned long long *d_ids, uint32_t n, TaskRaw *d_out, cudaStream_t s);
-int launch_gather_hll(const DevState &st, unsigned long long id, uint8_t *d_out, int32_t *d_found, cudaStream_t s);
+int launch_gather_hll(const DevState &st, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s);
 // window reads: the live slots (host filter, closed-window filter) as keys {host : 32 | slot : 32}, *d_n of them; with `order` sorted
 // by host (stable) and the ids of the sorted keys in *ids. *keys / *ids point into the sort buffers of tmp.
 int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int host_filter, uint32_t active_only,

@@ -433,23 +433,21 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical: no finished merge");
 
-	int32_t *h_l = reinterpret_cast<int32_t *>(e->h_qids), *d_l = reinterpret_cast<int32_t *>(e->d_qids);
-	gysk_svc_summary *d_rows = reinterpret_cast<gysk_svc_summary *>(e->d_wstage);
-	for (uint32_t off = 0; off < n; off += QCHUNK) {
-		const uint32_t m = std::min(QCHUNK, n - off);
-		for (uint32_t i = 0; i < m; ++i) {
-			auto it = mg.index.find(logical_ids[off + i]);
-			h_l[i] = it == mg.index.end() ? -1 : (int32_t)it->second;
-		}
-		CU(e, cudaMemcpyAsync(d_l, h_l, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
-		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(d_l, m, e->cfg.hll_p, mg.l_hist_last, mg.l_hist_all,
-				mg.l_conn, mg.l_hmax, mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab), d_rows);
-		e->kernel_launches++;
-		int rc = copy_svc_rows(e, m, out + off, "query_logical");
-		if (rc) return rc;
-		for (uint32_t i = 0; i < m; ++i) out[off + i].glob_id = logical_ids[off + i];
+	std::vector<int32_t> lidx(n);		// dense logical index, -1 for an id the map does not have
+	for (uint32_t i = 0; i < n; ++i) {
+		auto it = mg.index.find(logical_ids[i]);
+		lidx[i] = it == mg.index.end() ? -1 : (int32_t)it->second;
 	}
-	return GYSK_OK;
+	const SvcRows rows {e->cfg.hll_p, out};
+	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(gysk_svc_summary), "query_logical", [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
+		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(reinterpret_cast<const int32_t *>(d_l), m, e->cfg.hll_p,
+				mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax, mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab),
+				reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
+		return 1;
+	}, [&](const uint8_t *h_rows, uint32_t off, uint32_t m) {
+		rows(h_rows, off, m);
+		for (uint32_t i = 0; i < m; ++i) out[off + i].glob_id = logical_ids[off + i];
+	});
 }
 
 // global count-min point query on the merged table
@@ -463,16 +461,9 @@ int gysk_query_flows_global(gysk_engine *e, const uint64_t *keys, uint32_t n, in
 	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global: no merge");
 	DevState st = e->st;
 	st.cms_cur = mg.g_cms_cur; st.cms_last = mg.g_cms_last;
-	for (uint32_t off = 0; off < n; off += QCHUNK) {
-		const uint32_t m = std::min(QCHUNK, n - off);
-		memcpy(e->h_qids, keys + off, (size_t)m * sizeof(uint64_t));
-		CU(e, cudaMemcpyAsync(e->d_qids, e->h_qids, (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-		e->kernel_launches += launch_query_flows(st, e->d_qids, m, last_window, e->d_flowout, e->stream);
-		CU(e, cudaMemcpyAsync(e->h_flowout, e->d_flowout, (size_t)m * sizeof(gysk_flow_est), cudaMemcpyDeviceToHost, e->stream));
-		CU(e, cudaStreamSynchronize(e->stream));
-		memcpy(out + off, e->h_flowout, (size_t)m * sizeof(gysk_flow_est));
-	}
-	return post_launch(e, "query_flows_global");
+	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_est), "query_flows_global", [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
+		return launch_query_flows(st, d_keys, m, last_window, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
+	}, CopyRows<gysk_flow_est> {out});
 }
 
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)

@@ -1,7 +1,8 @@
 """gysk_query_window / gysk_query_tasks / gysk_query_task_window against the CPU oracle (make_pair / feed_both), over several
 flushes with idle eviction on: the rows are exactly the oracle's live ids, grouped by host and ordered by id; each service row is
 byte-equal to gysk_query_svcs of its id and equals a restatement of the summary from the oracle's exports; each process row equals
-the reference's percentile rule on the exported task histograms. gysk_query_svcs over several chunks of live, unknown and zero ids."""
+the reference's percentile rule on the exported task histograms. gysk_query_svcs and gysk_query_tasks over several chunks of live,
+unknown and zero ids; gysk_query_flows and gysk_register_ids over several chunks."""
 import ctypes as C
 
 import numpy as np
@@ -285,6 +286,57 @@ def test_by_id_read_across_chunks():
     for id_, r in zip(q.tolist(), _svcs_rows(eng, q)):
         want = win.get(id_) or bytes(ge.SvcSummary(glob_id=id_, td_p50_us=nan, td_p95_us=nan, td_p99_us=nan))
         assert bytes(r) == want, hex(id_)
+    eng.close()
+
+
+def test_task_flow_and_register_reads_across_chunks():
+    """gysk_query_tasks, gysk_query_flows and gysk_register_ids over more than two 1024-entry chunks. Live process ids shuffled among
+    unknown ids and id 0: a live row is byte-equal to the window row of its id, every other row to the zero row with only
+    aggr_task_id set. Flow keys of the stream among random keys: each estimate is the min over the rows of the exported count-min
+    table, in the current and in the last window. Registered ids are counted and read back as found."""
+    from oracle import pyoracle as po
+    rng = np.random.default_rng(8)
+    eng = ge.Engine(max_svcs=1 << 12, max_tasks=1 << 12)
+    svc_ids = (rng.choice(1 << 40, 300, replace=False) + 1).astype(np.uint64)
+    task_ids = (rng.choice(1 << 40, 1500, replace=False) + (1 << 41)).astype(np.uint64)
+    ev = _stream(rng, svc_ids, task_ids, 60000)
+    eng.ingest_events(ev)
+    eng.sync()
+    eng.flush(5)
+    ev2 = _stream(rng, svc_ids, task_ids, 20000)
+    eng.ingest_events(ev2)
+    eng.sync()
+
+    rows, n = eng.query_task_window()
+    win = {r.aggr_task_id: bytes(r) for r in rows}
+    assert n > 1000
+    unknown = (rng.choice(1 << 40, 1200, replace=False) + (1 << 42)).astype(np.uint64)
+    q = np.concatenate([np.array(list(win), dtype=np.uint64), unknown, np.zeros(300, dtype=np.uint64)])[rng.permutation(n + 1500)]
+    assert len(q) > 2 * 1024
+    for id_, r in zip(q.tolist(), eng.query_tasks(q)):
+        assert bytes(r) == (win.get(id_) or bytes(ge.TaskSummary(aggr_task_id=id_))), hex(id_)
+
+    tcp = np.concatenate([ev, ev2])
+    tcp = tcp[(tcp["type"] == ge.EV_ACCEPT)]
+    keys = np.concatenate([np.unique(tcp["flow_key"])[:1500], rng.integers(0, 1 << 62, 1000, dtype=np.uint64)])[rng.permutation(2500)]
+    O = po.lib()
+    depth, log2w = eng.cfg.cms_depth, eng.cfg.cms_log2_width
+    for lw in (False, True):
+        tbl = eng.export_cms(last_window=lw).reshape(depth, -1)
+        est = eng.query_flows(keys, last_window=lw)
+        assert est["flow_key"].tolist() == keys.tolist()
+        for k, e_ in zip(keys.tolist(), est):
+            cells = [int(tbl[r, O.gyo_cms_index(k, r, log2w)]) for r in range(depth)]
+            assert (e_["count"], e_["kbytes"]) == (min(c & M32 for c in cells), min(c >> 32 for c in cells)), (hex(k), lw)
+    eng.close()
+
+    eng = ge.Engine(max_svcs=1 << 12, max_tasks=1 << 12)
+    for is_task, count in ((False, 2500), (True, 2100)):
+        ids = (rng.choice(1 << 40, count, replace=False) + 1).astype(np.uint64)
+        eng.register_ids(ids, is_task=is_task)
+        assert eng.stats()["ntasks" if is_task else "nsvcs"] == count
+        found = [r.found for r in eng.query_tasks(ids)] if is_task else [r.found for r in _svcs_rows(eng, ids)]
+        assert found == [1] * count
     eng.close()
 
 
