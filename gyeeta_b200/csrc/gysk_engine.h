@@ -141,7 +141,7 @@ struct gysk_engine
 	int			stage_cur {0};
 	uint8_t			*d_raw[gysk::NBUF] {};		// raw records on their way to decode_raw_kernel
 	size_t			raw_bytes {0};
-	cudaEvent_t		ev_raw_copied[gysk::NBUF] {}, ev_raw_done[gysk::NBUF] {};
+	cudaEvent_t		ev_raw_done[gysk::NBUF] {};
 	int			raw_cur {0};
 
 	// query scratch (staged_read). The stage is only valid under mtx: every read copies its result out of it before it returns.
@@ -190,16 +190,35 @@ namespace gysk {
 int fail(gysk_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess);
 int post_launch(gysk_engine *e, const char *what);
 int submit_stage(gysk_engine *e);
-int append_chunk(gysk_engine *e, const gysk_event *src_pinned, uint64_t n);
 int drain_all(gysk_engine *e);
 int sync_locked(gysk_engine *e);
-int collect_evicted(gysk_engine *e, bool wait);
 void merge_release(gysk_engine *e);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
-// readers: hand every thread's partial chunk to the device, then take the engine
-#define GYSK_ENTER(e) { int rc_d__ = gysk::drain_all(e); if (rc_d__) return rc_d__; } std::lock_guard<std::mutex> lk((e)->mtx)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)
+
+// What an ABI call does with the events of the current device buffer when it enters: leave them (Drain: only every thread's
+// partial chunk is handed over), run their batch (Submit: the call sees every event handed in before it), or run it and wait for
+// both streams (Sync: the call reads results on the host).
+enum class Pending { Drain, Submit, Sync };
+
+// One ABI call's hold on the engine: every thread's partial chunk goes to the device, then the engine mutex is taken, the device
+// selected and the pending events handled as `mode` says. A non-zero rc is the call's error; the mutex is held only when rc is 0.
+struct Entry
+{
+	std::unique_lock<std::mutex> lk;
+	int rc;
+	Entry(gysk_engine *e, Pending mode) : rc(drain_all(e))
+	{
+		if (rc) return;
+		lk = std::unique_lock<std::mutex>(e->mtx);
+		const cudaError_t ce = cudaSetDevice(e->dev);
+		if (ce != cudaSuccess) rc = fail(e, GYSK_ERR_CUDA, "cudaSetDevice(e->dev)", ce);
+		else if (mode == Pending::Submit) rc = submit_stage(e);
+		else if (mode == Pending::Sync) rc = sync_locked(e);
+	}
+};
+#define GYSK_ENTER(e, mode) gysk::Entry entry__((e), gysk::Pending::mode); if (entry__.rc) return entry__.rc
 
 template <typename T>
 int dalloc(gysk_engine *e, T **p, size_t n, bool zero = true)

@@ -114,10 +114,7 @@ extern "C" int gysk_task_groupby(gysk_engine *e, const gysk_proc_sample *samples
 	*ngroups = 0;
 	if (!n) return GYSK_OK;
 	if (n > e->cfg.max_batch) return fail(e, GYSK_ERR_INVAL, "gysk_task_groupby: more samples than max_batch (the sort buffers' size)");
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = sync_locked(e);					// the sort buffers are shared with the batch kernels
-	if (rc) return rc;
+	GYSK_ENTER(e, Sync);					// the sort buffers are shared with the batch kernels
 
 	uint32_t tcap = 1024;
 	while (tcap < 2ull * n) tcap <<= 1;

@@ -269,10 +269,7 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 {
 	CHECK_ENGINE(e);
 	if ((!glob_ids || !logical_ids) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
-	int rc = sync_locked(e);
-	if (rc) return rc;
+	GYSK_ENTER(e, Sync);
 
 	MergeState &mg = e->mg;
 
@@ -324,7 +321,8 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	mg.off_maxu8 = off; const size_t o_hll = off; off += align256((size_t)nl << e->cfg.hll_p); mg.bytes_maxu8 = off - mg.off_maxu8;
 	mg.arena_bytes = off;
 
-	if ((rc = dalloc(e, &mg.arena, mg.arena_bytes))) return rc;
+	int rc = dalloc(e, &mg.arena, mg.arena_bytes);
+	if (rc) return rc;
 	mg.g_cms_cur = reinterpret_cast<unsigned long long *>(mg.arena + o_cms_cur);
 	mg.g_cms_last = reinterpret_cast<unsigned long long *>(mg.arena + o_cms_last);
 	mg.l_hist_last = reinterpret_cast<HistCell *>(mg.arena + o_hl);
@@ -349,12 +347,9 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 int gysk_merge_prepare(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
+	GYSK_ENTER(e, Submit);
 	MergeState &mg = e->mg;
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_prepare: call gysk_set_logical_map first");
-	int rc = submit_stage(e);
-	if (rc) return rc;
 
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8;
 	const uint32_t nl = mg.nlogical;
@@ -384,7 +379,7 @@ int gysk_merge_buffers(gysk_engine *e, gysk_buffer_desc *out, uint32_t cap, uint
 {
 	CHECK_ENGINE(e);
 	if (!out || !n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
+	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_buffers: call gysk_set_logical_map first");
 	if (cap < 3) return GYSK_ERR_NOSPC;
@@ -399,7 +394,7 @@ int gysk_merge_tdigest_slab(gysk_engine *e, void **dptr, uint64_t *nbytes)
 {
 	CHECK_ENGINE(e);
 	if (!dptr || !nbytes) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
+	GYSK_ENTER(e, Drain);
 	if (!e->mg.slab) return fail(e, GYSK_ERR_INVAL, "gysk_merge_tdigest_slab: call gysk_set_logical_map first");
 	*dptr = e->mg.slab; *nbytes = (uint64_t)e->mg.nlogical * sizeof(SlabEntry);
 	return GYSK_OK;
@@ -408,8 +403,7 @@ int gysk_merge_tdigest_slab(gysk_engine *e, void **dptr, uint64_t *nbytes)
 int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 {
 	CHECK_ENGINE(e);
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
+	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: call gysk_merge_prepare first");
 	if (!world) world = 1;
@@ -428,8 +422,7 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 {
 	CHECK_ENGINE(e);
 	if ((!logical_ids || !out) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
+	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical: no finished merge");
 
@@ -455,8 +448,7 @@ int gysk_query_flows_global(gysk_engine *e, const uint64_t *keys, uint32_t n, in
 {
 	CHECK_ENGINE(e);
 	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
+	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global: no merge");
 	DevState st = e->st;
@@ -486,8 +478,7 @@ int gysk_nccl_comm_init(gysk_engine *e, const uint8_t uid[GYSK_NCCL_UNIQUE_ID_BY
 	if (!uid || !nranks || rank >= nranks) return GYSK_ERR_INVAL;
 	NcclApi *a = nccl_api();
 	if (!a) return fail(e, GYSK_ERR_NOTSUP, "libnccl.so.2 could not be loaded");
-	GYSK_ENTER(e);
-	CU(e, cudaSetDevice(e->dev));
+	GYSK_ENTER(e, Drain);
 	if (e->mg.comm) { a->CommDestroy((ncclComm_t)e->mg.comm); e->mg.comm = nullptr; }
 	ncclUniqueId id;
 	memcpy(&id, uid, sizeof(id));
@@ -510,8 +501,7 @@ int gysk_merge_global(gysk_engine *e, void *comm)
 	if (rc) return rc;
 	int world = 0;
 	{
-		GYSK_ENTER(e);
-		CU(e, cudaSetDevice(e->dev));
+		GYSK_ENTER(e, Drain);
 		MergeState &mg = e->mg;
 		NC(e, a->CommCount(c, &world));
 		if (world < 1) return fail(e, GYSK_ERR_INVAL, "gysk_merge_global: empty communicator");

@@ -202,6 +202,7 @@ struct alignas(8) ACTIVE_CONN_STATS					// common/gy_comm_proto.h:2766-2810 (fix
 	uint8_t		pad_;
 
 	static constexpr size_t MAX_NUM_CONNS = 2048;			// :2786
+	size_t get_elem_size() const noexcept { return sizeof(*this); }
 };
 static_assert(sizeof(ACTIVE_CONN_STATS) == 104 && offsetof(ACTIVE_CONN_STATS, bytes_sent_) == 72 && offsetof(ACTIVE_CONN_STATS, active_conns_) == 100, "ACTIVE_CONN_STATS");
 
