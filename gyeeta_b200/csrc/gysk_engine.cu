@@ -321,8 +321,13 @@ int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned 
 {
 	return launch_task_summaries(e->st, d_ids, d_slots, m, reinterpret_cast<gysk_task_summary *>(e->d_wstage), e->stream);
 }
+int launch_rows(gysk_engine *e, const unsigned long long *, const unsigned long long *d_slots, uint32_t m, gysk_listener_day_stats *)
+{
+	return launch_day_stats(e->st, d_slots, m, e->cfg.max_svcs, live_mask(e, 1), reinterpret_cast<gysk_listener_day_stats *>(e->d_wstage), e->stream);
+}
 SvcRows finish_rows(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
 CopyRows<gysk_task_summary> finish_rows(const gysk_engine *, gysk_task_summary *out) { return CopyRows<gysk_task_summary> {out}; }
+CopyRows<gysk_listener_day_stats> finish_rows(const gysk_engine *, gysk_listener_day_stats *out) { return CopyRows<gysk_listener_day_stats> {out}; }
 
 } // namespace
 
@@ -1113,28 +1118,38 @@ int gysk_evicted_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n)
 
 namespace {
 
-// The slots a window read returns, in its order, at tmp.keys_a[0 .. want): the live slots of the selection grouped by host (a stable
-// radix sort of {host | slot} keys on the device), then by id inside each host (on the host: slot numbers depend on insertion races,
-// the order must not). *n = rows that match. Stream synchronised by the caller.
-int window_list(gysk_engine *e, int is_task, int32_t host_idx, uint32_t flags, uint32_t want, uint32_t *n)
+uint32_t active_mark(const gysk_engine *e) { return e->last_flush_tsec ? e->last_flush_tsec : 1u; }	// slot_last_active of the closed window (state_kernel)
+
+// the device half of a window read: the listed keys {host | slot} of the selection (seen_before: see launch_window_list), host-sorted
+// with `order`, at *d_keys (their ids at *d_ids); *n of them
+int list_slots(gysk_engine *e, int is_task, int32_t host_idx, uint32_t flags, uint32_t seen_before, bool order, const unsigned long long **d_keys,
+		const unsigned long long **d_ids, uint32_t *n)
 {
 	uint32_t nslots = 0;
 	CU(e, cudaMemcpyAsync(&nslots, is_task ? e->st.task_tbl.count : e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
 	nslots = std::min(nslots, is_task ? e->cfg.max_tasks : e->cfg.max_svcs);
-	const uint32_t active_mark = e->last_flush_tsec ? e->last_flush_tsec : 1u;		// slot_last_active of the closed window (state_kernel)
 	unsigned long long *d_n = e->st.counters + CTR_NWINDOW;
-	const unsigned long long *d_keys = nullptr, *d_ids = nullptr;
-	const int nl = launch_window_list(e->st, e->tmp, nslots, is_task, host_idx, flags & GYSK_WINDOW_ACTIVE_ONLY, active_mark, d_n, want > 0,
-			&d_keys, &d_ids, e->stream);
+	const int nl = launch_window_list(e->st, e->tmp, nslots, is_task, host_idx, flags & GYSK_WINDOW_ACTIVE_ONLY, active_mark(e), seen_before, d_n, order,
+			d_keys, d_ids, e->stream);
 	if (nl < 0) return fail(e, GYSK_ERR_INVAL, "window read: sort failed");
 	e->kernel_launches += nl;
 	unsigned long long cnt = 0;
 	CU(e, cudaMemcpyAsync(&cnt, d_n, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
-	int rc = post_launch(e, "window list");
-	if (rc) return rc;
 	*n = (uint32_t)cnt;
+	return post_launch(e, "window list");
+}
+
+// The slots a window read returns, in its order, at tmp.keys_a[0 .. want): the live slots of the selection grouped by host (a stable
+// radix sort of {host | slot} keys on the device), then by id inside each host (on the host: slot numbers depend on insertion races,
+// the order must not). *n = rows that match. Stream synchronised by the caller.
+int window_list(gysk_engine *e, int is_task, int32_t host_idx, uint32_t flags, uint32_t seen_before, uint32_t want, uint32_t *n)
+{
+	const unsigned long long *d_keys = nullptr, *d_ids = nullptr;
+	int rc = list_slots(e, is_task, host_idx, flags, seen_before, want > 0, &d_keys, &d_ids, n);
+	if (rc) return rc;
+	const uint32_t cnt = *n;
 	if (!want || !cnt) return 0;
 
 	std::vector<uint64_t> &keys = e->win_keys, &ids = e->win_ids;
@@ -1176,8 +1191,10 @@ int window_rows(gysk_engine *e, int32_t host_idx, uint32_t flags, Row *out, uint
 	CHECK_ENGINE(e);
 	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Sync);
+	// day stats: only services first seen more than 15 minutes before the last flush (tcur > tstart + 15 * 60, gy_socket_stat.cc:2102)
+	const uint32_t seen_before = !std::is_same<Row, gysk_listener_day_stats>::value ? ~0u : e->last_flush_tsec > 900u ? e->last_flush_tsec - 900u : 0u;
 	uint32_t total = 0;
-	int rc = window_list(e, std::is_same<Row, gysk_task_summary>::value, host_idx, flags, cap, &total);
+	int rc = window_list(e, std::is_same<Row, gysk_task_summary>::value, host_idx, flags, seen_before, cap, &total);
 	if (rc) return rc;
 	const uint32_t m = std::min(cap, total);
 	rc = staged_read<uint64_t>(e, nullptr, m, WIN_ROWS, sizeof(Row), what,
@@ -1228,6 +1245,41 @@ int gysk_query_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc
 int gysk_query_window_hosts(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_summary *out, uint32_t *hosts, uint32_t cap, uint32_t *n)
 {
 	return window_rows(e, host_idx, flags, out, hosts, cap, n, "query_window");
+}
+
+int gysk_query_day_stats(gysk_engine *e, int32_t host_idx, gysk_listener_day_stats *out, uint32_t *hosts, uint32_t cap, uint32_t *n)
+{
+	return window_rows(e, host_idx, 0, out, hosts, cap, n, "day_stats");
+}
+
+// the host-sorted keys of every live service, the per-run counts beside them in the other sort buffer, then the host rows in stage-sized
+// pieces by rank
+int gysk_query_host_listen(gysk_engine *e, gysk_host_listen *out, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!n || (!out && cap)) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Sync);
+	const unsigned long long *d_keys = nullptr, *d_ids = nullptr;
+	uint32_t nkeys = 0;
+	int rc = list_slots(e, 0, -1, 0, ~0u, true, &d_keys, &d_ids, &nkeys);
+	if (rc) return rc;
+	if (!nkeys) { *n = 0; return GYSK_OK; }
+	unsigned long long *acc = const_cast<unsigned long long *>(d_ids), *d_rows = e->st.counters + CTR_NHOSTS;
+	const unsigned long long *d_n = e->st.counters + CTR_NWINDOW;
+	gysk_host_listen *d_out = reinterpret_cast<gysk_host_listen *>(e->d_wstage);
+	constexpr uint32_t piece = (uint32_t)(STAGE_BYTES / sizeof(gysk_host_listen));
+	e->kernel_launches += launch_host_listen_count(e->st, d_keys, d_n, nkeys, active_mark(e), acc, e->stream);
+	e->kernel_launches += launch_host_listen_rows(d_keys, d_n, acc, 0, std::min(cap, piece), d_out, d_rows, e->stream);
+	unsigned long long nrows = 0;
+	CU(e, cudaMemcpyAsync(&nrows, d_rows, sizeof(nrows), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	if ((rc = post_launch(e, "host_listen"))) return rc;
+	*n = (uint32_t)nrows;
+	// the first piece is in the stage already; more than `piece` hosts take one more pass over the keys per piece
+	return staged_read<uint64_t>(e, nullptr, std::min(cap, *n), piece, sizeof(gysk_host_listen), "host_listen",
+			[&](const unsigned long long *, uint32_t off, uint32_t m) {
+				return off ? launch_host_listen_rows(d_keys, d_n, acc, off, m, d_out, d_rows, e->stream) : 0;
+			}, CopyRows<gysk_host_listen> {out});
 }
 
 int gysk_query_tasks(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_task_summary *out)
@@ -1556,6 +1608,13 @@ int gysk_classify_listener(const gysk_listener_state_in *in, uint8_t *high_resp_
 {
 	if (!in || !high_resp_bit_hist || !state || !issue) return GYSK_ERR_INVAL;
 	classify_listener(*in, *high_resp_bit_hist, *state, *issue);
+	return GYSK_OK;
+}
+
+int gysk_classify_host(const gysk_host_state_in *in, uint8_t *state)
+{
+	if (!in || !state) return GYSK_ERR_INVAL;
+	*state = classify_host(*in);
 	return GYSK_OK;
 }
 

@@ -1326,6 +1326,23 @@ __device__ __forceinline__ LevelStat level_stat(const uint64_t *counts, uint64_t
 	return r;
 }
 
+// p95 / p25 of qps_hist_ and active_conn_hist_ from their bucket counts (cnt is scratch). The active-connection histogram is read over
+// its 14 buckets (HASH_1_3000).
+struct QpsActPct { int64_t qps_p95, qps_p25, act_p95, act_p25; };
+__device__ __forceinline__ QpsActPct qps_act_pct(const HistCell *q, const HistCell *a, uint64_t *cnt)
+{
+	QpsActPct r;
+	uint64_t tot = 0;
+	for (int b = 0; b < HIST_MAX_CELL; ++b) { cnt[b] = q[b].count; tot += cnt[b]; }
+	r.qps_p95 = qps_bucket_value(hist_pct_bucket(cnt, HIST_MAX_CELL, tot, 95.0f), tot);
+	r.qps_p25 = qps_bucket_value(hist_pct_bucket(cnt, HIST_MAX_CELL, tot, 25.0f), tot);
+	tot = 0;
+	for (int b = 0; b < HIST_MAX_CELL; ++b) { cnt[b] = b < 14 ? a[b].count : 0; tot += cnt[b]; }
+	r.act_p95 = act_bucket_value(hist_pct_bucket(cnt, 14, tot, 95.0f), tot);
+	r.act_p25 = act_bucket_value(hist_pct_bucket(cnt, 14, tot, 25.0f), tot);
+	return r;
+}
+
 __global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots, uint32_t tsec, uint32_t live0, uint32_t live1)
 {
 	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1374,14 +1391,8 @@ __global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots
 		const int qb = bucket_semi_log_lo(qv), ab = bucket_hash_1_3000(av);
 		q[qb].count += 1; q[qb].sum += qv; if ((long long)qv > q[HIST_MAX_CELL].sum) q[HIST_MAX_CELL].sum = qv;
 		a[ab].count += 1; a[ab].sum += av; if ((long long)av > a[HIST_MAX_CELL].sum) a[HIST_MAX_CELL].sum = av;
-		uint64_t tot = 0;
-		for (int b = 0; b < HIST_MAX_CELL; ++b) { cnt[b] = q[b].count; tot += cnt[b]; }
-		in.qps_p95 = qps_bucket_value(hist_pct_bucket(cnt, HIST_MAX_CELL, tot, 95.0f), tot);
-		in.qps_p25 = qps_bucket_value(hist_pct_bucket(cnt, HIST_MAX_CELL, tot, 25.0f), tot);
-		tot = 0;
-		for (int b = 0; b < HIST_MAX_CELL; ++b) { cnt[b] = b < 14 ? a[b].count : 0; tot += cnt[b]; }
-		in.act_p95 = act_bucket_value(hist_pct_bucket(cnt, 14, tot, 95.0f), tot);
-		in.act_p25 = act_bucket_value(hist_pct_bucket(cnt, 14, tot, 25.0f), tot);
+		const QpsActPct p = qps_act_pct(q, a, cnt);
+		in.qps_p95 = p.qps_p95; in.qps_p25 = p.qps_p25; in.act_p95 = p.act_p95; in.act_p25 = p.act_p25;
 	}
 
 	in.nconn = (int32_t)ss.nconn_active;
@@ -1399,6 +1410,45 @@ __global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots
 	classify_listener(in, ss.high_bits, ss.state, ss.issue);
 	apply_issue_history(age, in.ser_errors, ss.state, ss.issue, ss.issue_bits);
 	st.slot_state[slot] = ss;
+}
+
+// The LISTENER_DAY_STATS record of a listener (get_curr_state, common/gy_socket_stat.cc:2101-2117), one warp per listed slot: lanes
+// 0..15 gather one cell each of the 5-day level's live ring slots and of qps_hist_ / active_conn_hist_, lane 0 takes the percentiles
+// with state_kernel's helpers. The int64 values go into the uint32 fields by plain conversion, as the reference's assignments do.
+static constexpr int DAY_WARPS = 4;
+__global__ void __launch_bounds__(DAY_WARPS * 32) day_stats_kernel(DevState st, const unsigned long long *__restrict__ slots, uint32_t n,
+		uint32_t max_svcs, uint32_t live1, gysk_listener_day_stats *__restrict__ out)
+{
+	__shared__ HistCell lvl[DAY_WARPS][HIST_CELLS], qa[DAY_WARPS][2][HIST_CELLS];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t q = blockIdx.x * DAY_WARPS + wid;
+
+	if (q >= n) return;
+	const uint32_t slot = (uint32_t)slots[q];
+	if (lane < HIST_CELLS) {
+		HistCell a {0, 0};
+		for (int k = 0; k < NSLOTS; ++k) {
+			if (!((live1 >> k) & 1u)) continue;
+			const HistCell x = st.hist_ring[(((size_t)NSLOTS + k) * max_svcs + slot) * HIST_CELLS + lane];
+			a.count += x.count; a.sum += x.sum;
+		}
+		lvl[wid][lane] = a;
+		qa[wid][0][lane] = st.qps_hist[(size_t)slot * HIST_CELLS + lane];
+		qa[wid][1][lane] = st.act_hist[(size_t)slot * HIST_CELLS + lane];
+	}
+	__syncwarp();
+	if (lane) return;
+	uint64_t cnt[HIST_MAX_CELL], sum = 0;
+	for (int b = 0; b < HIST_MAX_CELL; ++b) { cnt[b] = lvl[wid][b].count; sum += (uint64_t)lvl[wid][b].sum; }
+	const LevelStat d = level_stat(cnt, sum);
+	const QpsActPct p = qps_act_pct(qa[wid][0], qa[wid][1], cnt);
+	gysk_listener_day_stats r;
+	r.glob_id = st.slot_id[slot];
+	r.tcount_5d = (int64_t)d.cnt; r.tsum_5d = (int64_t)d.sum;
+	r.p95_5d_respms = (uint32_t)d.p95; r.p25_5d_respms = (uint32_t)d.p25;
+	r.p95_qps = (uint32_t)p.qps_p95; r.p25_qps = (uint32_t)p.qps_p25;
+	r.p95_nactive = (uint32_t)p.act_p95; r.p25_nactive = (uint32_t)p.act_p25;
+	out[q] = r;
 }
 
 // one CTA per evicted slot (grid-stride): the id's table entry becomes a tombstone, every per-slot array returns to its
@@ -1531,9 +1581,10 @@ __global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const uns
 
 // live slots below nslots (host filter, closed-window filter) -> keys {host : 32 | slot : 32} in any order, *d_n of them. A service is
 // active when its last window with events is the one the last flush closed (active_mark, the rule of state_kernel); a process when
-// one of its histograms took samples in that window.
+// one of its histograms took samples in that window. seen_before != ~0u keeps only services whose slot a flush before that tsec saw
+// (the day-stats read).
 __global__ void window_select_kernel(DevState st, uint32_t nslots, int is_task, int host_filter, uint32_t active_only, uint32_t active_mark,
-		unsigned long long *__restrict__ keys, unsigned long long *d_n)
+		uint32_t seen_before, unsigned long long *__restrict__ keys, unsigned long long *d_n)
 {
 	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
 	bool take = false;
@@ -1547,6 +1598,10 @@ __global__ void window_select_kernel(DevState st, uint32_t nslots, int is_task, 
 				take = (l[0].count | l[1].count | l[2].count) != 0;
 			}
 			else take = st.slot_last_active[slot] == active_mark;
+		}
+		if (take && seen_before != ~0u) {
+			const uint32_t first = st.slot_first_seen[slot];
+			take = first && first < seen_before;
 		}
 	}
 	const unsigned mask = __ballot_sync(0xffffffffu, take);
@@ -1566,6 +1621,70 @@ __global__ void window_ids_kernel(DevState st, int is_task, const unsigned long 
 	if (i >= *d_n) return;
 	const uint32_t slot = (uint32_t)keys[i];
 	ids[i] = is_task ? st.task_slot_id[slot] : st.slot_id[slot];
+}
+
+// ---- per-host listener counts (gysk_query_host_listen) over the host-sorted keys of the window list ----
+
+// first position in [lo, hi) whose key's host is > h (above = true) or >= h
+__device__ __forceinline__ uint32_t host_bound(const unsigned long long *keys, uint32_t lo, uint32_t hi, uint32_t h, bool above)
+{
+	while (lo < hi) {
+		const uint32_t mid = lo + ((hi - lo) >> 1);
+		const uint32_t hm = (uint32_t)(keys[mid] >> 32);
+		if (hm < h || (above && hm == h)) lo = mid + 1; else hi = mid;
+	}
+	return lo;
+}
+
+// Every listed service adds {issue : 32 | severe : 32} to acc[head of its host's run] (acc zeroed): issue = evaluated at the last flush
+// (slot_last_active == active_mark) with issue bit 0 set there, severe = issue and state >= SEVERE (listener_stats_update's nissue /
+// nsevere, common/gy_socket_stat.cc:4242-4252). Lanes of one run add once per warp.
+__global__ void host_listen_count_kernel(DevState st, const unsigned long long *__restrict__ keys, const unsigned long long *d_n, uint32_t active_mark,
+		unsigned long long *__restrict__ acc)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, n = (uint32_t)*d_n;
+	const unsigned live = __ballot_sync(0xffffffffu, i < n);
+	if (i >= n) return;
+	const unsigned long long key = keys[i];
+	const uint32_t slot = (uint32_t)key, head = host_bound(keys, 0, i, (uint32_t)(key >> 32), false);
+	const SlotState ss = st.slot_state[slot];
+	const bool issue = st.slot_last_active[slot] == active_mark && (ss.issue_bits & 1u), severe = issue && ss.state >= GYSK_STATE_SEVERE;
+	const unsigned run = __match_any_sync(live, head);
+	const unsigned bi = __ballot_sync(run, issue), bs = __ballot_sync(run, severe);
+	if ((threadIdx.x & 31) == __ffs(run) - 1 && bi)
+		atomicAdd(acc + head, ((unsigned long long)__popc(bi) << 32) | (unsigned long long)__popc(bs));
+}
+
+// One CTA walks the keys in order and writes the row of every host run whose rank lies in [rlo, rlo + cap): {host, run length, issue,
+// severe}; *d_rows = number of runs. A block-wide ballot scan ranks the run heads of each 1024-key tile.
+__global__ void __launch_bounds__(1024) host_listen_rows_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *d_n,
+		const unsigned long long *__restrict__ acc, uint32_t rlo, uint32_t cap, gysk_host_listen *__restrict__ out, unsigned long long *d_rows)
+{
+	__shared__ uint32_t wcnt[32];
+	const uint32_t n = (uint32_t)*d_n;
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	uint32_t running = 0;
+
+	for (uint32_t t = 0; t < n; t += 1024) {
+		const uint32_t i = t + threadIdx.x;
+		const uint32_t h = i < n ? (uint32_t)(keys[i] >> 32) : 0;
+		const bool head = i < n && (i == 0 || (uint32_t)(keys[i - 1] >> 32) != h);
+		const unsigned b = __ballot_sync(0xffffffffu, head);
+		if (lane == 0) wcnt[wid] = __popc(b);
+		__syncthreads();
+		uint32_t before = 0, total = 0;
+		for (int w = 0; w < 32; ++w) { const uint32_t c = wcnt[w]; before += w < wid ? c : 0; total += c; }
+		if (head) {
+			const uint32_t r = running + before + __popc(b & ((1u << lane) - 1u));
+			if (r >= rlo && r - rlo < cap) {
+				const unsigned long long a = acc[i];
+				out[r - rlo] = gysk_host_listen {h, host_bound(keys, i + 1, n, h, true) - i, (uint32_t)(a >> 32), (uint32_t)a};
+			}
+		}
+		running += total;
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) *d_rows = running;
 }
 
 // one warp per service: by id (ids != nullptr: looked up, id 0 and unknown ids give found = 0) or by slot (the window read). The
@@ -2035,12 +2154,13 @@ int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uin
 }
 
 int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int host_filter, uint32_t active_only,
-		uint32_t active_mark, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids, cudaStream_t s)
+		uint32_t active_mark, uint32_t seen_before, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids,
+		cudaStream_t s)
 {
 	cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s);
 	*keys = tmp.keys_a; *ids = tmp.keys_b;
 	if (!nslots) return 0;
-	window_select_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, is_task, host_filter, active_only, active_mark, tmp.keys_a, d_n);
+	window_select_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, is_task, host_filter, active_only, active_mark, seen_before, tmp.keys_a, d_n);
 	if (!order) return 1;
 	int which = 0;
 	const int sorted = launch_radix_sort(tmp, d_n, nslots, 32, 64, 64, 64, &which, s);
@@ -2063,6 +2183,30 @@ int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, c
 {
 	if (!n) return 0;
 	task_summary_kernel<<<div_up(n, 4), 128, 0, s>>>(st, d_ids, d_slots, n, d_out);
+	return 1;
+}
+
+int launch_day_stats(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask1,
+		gysk_listener_day_stats *d_out, cudaStream_t s)
+{
+	if (!n) return 0;
+	day_stats_kernel<<<div_up(n, DAY_WARPS), DAY_WARPS * 32, 0, s>>>(st, d_slots, n, max_svcs, live_mask1, d_out);
+	return 1;
+}
+
+int launch_host_listen_count(const DevState &st, const unsigned long long *keys, const unsigned long long *d_n, uint32_t n, uint32_t active_mark,
+		unsigned long long *acc, cudaStream_t s)
+{
+	if (!n) return 0;
+	cudaMemsetAsync(acc, 0, (size_t)n * sizeof(unsigned long long), s);
+	host_listen_count_kernel<<<div_up(n, 256), 256, 0, s>>>(st, keys, d_n, active_mark, acc);
+	return 1;
+}
+
+int launch_host_listen_rows(const unsigned long long *keys, const unsigned long long *d_n, const unsigned long long *acc, uint32_t rlo, uint32_t cap,
+		gysk_host_listen *d_out, unsigned long long *d_rows, cudaStream_t s)
+{
+	host_listen_rows_kernel<<<1, 1024, 0, s>>>(keys, d_n, acc, rlo, cap, d_out, d_rows);
 	return 1;
 }
 

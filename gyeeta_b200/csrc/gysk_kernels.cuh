@@ -132,10 +132,21 @@ int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint
 		SvcRaw *d_out, cudaStream_t s);
 int launch_gather_tasks(const DevState &st, const unsigned long long *d_ids, uint32_t n, TaskRaw *d_out, cudaStream_t s);
 int launch_gather_hll(const DevState &st, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s);
-// window reads: the live slots (host filter, closed-window filter) as keys {host : 32 | slot : 32}, *d_n of them; with `order` sorted
-// by host (stable) and the ids of the sorted keys in *ids. *keys / *ids point into the sort buffers of tmp.
+// window reads: the live slots (host filter, closed-window filter, with seen_before != ~0u only services first seen by a flush before
+// that tsec) as keys {host : 32 | slot : 32}, *d_n of them; with `order` sorted by host (stable) and the ids of the sorted keys in *ids.
+// *keys / *ids point into the sort buffers of tmp.
 int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int host_filter, uint32_t active_only,
-		uint32_t active_mark, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids, cudaStream_t s);
+		uint32_t active_mark, uint32_t seen_before, unsigned long long *d_n, bool order, const unsigned long long **keys, const unsigned long long **ids,
+		cudaStream_t s);
+// LISTENER_DAY_STATS rows of n slots
+int launch_day_stats(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask1,
+		gysk_listener_day_stats *d_out, cudaStream_t s);
+// per-host listener counts over the n host-sorted keys of launch_window_list (*d_n on the device): the issue / severe counts of each
+// host's run at acc[run head] (acc: n entries of scratch), then the rows of the runs ranked [rlo, rlo + cap) and *d_rows = runs
+int launch_host_listen_count(const DevState &st, const unsigned long long *keys, const unsigned long long *d_n, uint32_t n, uint32_t active_mark,
+		unsigned long long *acc, cudaStream_t s);
+int launch_host_listen_rows(const unsigned long long *keys, const unsigned long long *d_n, const unsigned long long *acc, uint32_t rlo, uint32_t cap,
+		gysk_host_listen *d_out, unsigned long long *d_rows, cudaStream_t s);
 // service / process rows by id (d_ids) or, with d_ids == nullptr, by slot (d_slots)
 int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs,
 		uint32_t live_mask0, uint32_t live_mask1, gysk_svc_summary *d_out, cudaStream_t s);

@@ -224,4 +224,22 @@ GYSK_HD void apply_issue_history(uint32_t age_secs, uint32_t ser_errors, uint8_t
 	else { issue_bit_hist = 0; issue = GYSK_ISSUE_NONE; state = GYSK_STATE_OK; }
 }
 
+// TCP_SOCK_HANDLER::host_status_update's state rule, common/gy_socket_stat.cc:4455-4528, in its statement order
+inline uint8_t classify_host(const gysk_host_state_in &in)
+{
+	const bool cpu = !!in.cpu_issue, mem = !!in.mem_issue, scpu = !!in.severe_cpu_issue, smem = !!in.severe_mem_issue;
+	const uint32_t nti = in.ntasks_issue, nts = in.ntasks_severe, nli = in.nlisten_issue, nls = in.nlisten_severe;
+
+	if ((nts || nls) && (scpu || smem)) return GYSK_STATE_SEVERE;					// :4462
+	if (!cpu && !mem && !nti && !nli) return in.cpu_idle ? GYSK_STATE_IDLE : GYSK_STATE_GOOD;		// :4467
+	if ((nti || nli) && (cpu || mem)) return (nti > 5 || nli > 5) ? GYSK_STATE_SEVERE : GYSK_STATE_BAD;	// :4479
+	if (cpu || mem) return (scpu || smem) ? GYSK_STATE_BAD : GYSK_STATE_OK;				// :4488
+	if (nli) {												// :4498
+		if (nls || nti) return nli > 5 ? GYSK_STATE_SEVERE : GYSK_STATE_BAD;
+		return nli > 2 ? GYSK_STATE_BAD : GYSK_STATE_OK;
+	}
+	if (nti && (nts || nti > 5)) return GYSK_STATE_BAD;						// :4518
+	return GYSK_STATE_OK;
+}
+
 } // namespace gysk

@@ -206,6 +206,53 @@ struct alignas(8) ACTIVE_CONN_STATS					// common/gy_comm_proto.h:2766-2810 (fix
 };
 static_assert(sizeof(ACTIVE_CONN_STATS) == 104 && offsetof(ACTIVE_CONN_STATS, bytes_sent_) == 72 && offsetof(ACTIVE_CONN_STATS, active_conns_) == 100, "ACTIVE_CONN_STATS");
 
+struct alignas(8) LISTENER_DAY_STATS					// common/gy_comm_proto.h:1620-1653 (fixed stride)
+{
+	uint64_t	glob_id_;
+	int64_t		tcount_5d_;
+	int64_t		tsum_5d_;
+	uint32_t	p95_5d_respms_;
+	uint32_t	p25_5d_respms_;
+	uint32_t	p95_qps_;
+	uint32_t	p25_qps_;
+	uint32_t	p95_nactive_;
+	uint32_t	p25_nactive_;
+
+	static constexpr size_t MAX_NUM_LISTENERS = 2048;			// :1632, records per NOTIFY_LISTENER_DAY_STATS message
+};
+static_assert(sizeof(LISTENER_DAY_STATS) == 48 && sizeof(gysk_listener_day_stats) == 48, "LISTENER_DAY_STATS");
+static_assert(offsetof(LISTENER_DAY_STATS, tcount_5d_) == offsetof(gysk_listener_day_stats, tcount_5d) &&
+		offsetof(LISTENER_DAY_STATS, tsum_5d_) == offsetof(gysk_listener_day_stats, tsum_5d) &&
+		offsetof(LISTENER_DAY_STATS, p95_5d_respms_) == offsetof(gysk_listener_day_stats, p95_5d_respms) &&
+		offsetof(LISTENER_DAY_STATS, p25_5d_respms_) == offsetof(gysk_listener_day_stats, p25_5d_respms) &&
+		offsetof(LISTENER_DAY_STATS, p95_qps_) == offsetof(gysk_listener_day_stats, p95_qps) &&
+		offsetof(LISTENER_DAY_STATS, p25_qps_) == offsetof(gysk_listener_day_stats, p25_qps) &&
+		offsetof(LISTENER_DAY_STATS, p95_nactive_) == offsetof(gysk_listener_day_stats, p95_nactive) &&
+		offsetof(LISTENER_DAY_STATS, p25_nactive_) == offsetof(gysk_listener_day_stats, p25_nactive), "gysk_listener_day_stats = LISTENER_DAY_STATS");
+
+struct alignas(8) HOST_STATE_NOTIFY					// common/gy_comm_proto.h:2289-2330 (one record per message)
+{
+	uint64_t	curr_time_usec_;
+	uint32_t	ntasks_issue_;
+	uint32_t	ntasks_severe_;
+	uint32_t	ntasks_;
+	uint32_t	nlisten_issue_;
+	uint32_t	nlisten_severe_;
+	uint32_t	nlisten_;
+	uint8_t		curr_state_;
+	uint8_t		issue_bit_hist_;
+	bool		cpu_issue_;
+	bool		mem_issue_;
+	bool		severe_cpu_issue_;
+	bool		severe_mem_issue_;
+	alignas(8) uint32_t total_cpu_delayms_;
+	uint32_t	total_vm_delayms_;
+	uint32_t	total_io_delayms_;
+};
+static_assert(sizeof(HOST_STATE_NOTIFY) == 56 && offsetof(HOST_STATE_NOTIFY, nlisten_issue_) == 20 && offsetof(HOST_STATE_NOTIFY, nlisten_) == 28 &&
+		offsetof(HOST_STATE_NOTIFY, curr_state_) == 32 && offsetof(HOST_STATE_NOTIFY, severe_mem_issue_) == 37 &&
+		offsetof(HOST_STATE_NOTIFY, total_cpu_delayms_) == 40, "HOST_STATE_NOTIFY");
+
 // The shape shared by TCP_CONN_NOTIFY::validate / AGGR_TASK_STATE_NOTIFY::validate / LISTENER_STATE_NOTIFY::validate
 // (common/gy_comm_proto.cc:840-881, :912-953, :955-996): nevents <= MAX, every element size a multiple of 8 and
 // inside the remaining length, trailing string NUL-forced in place, success iff all nevents were walked.

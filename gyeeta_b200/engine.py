@@ -102,6 +102,35 @@ def classify_listener(inp, high_resp_bit_hist=0):
     return st.value, iss.value, hb.value
 
 
+class ListenerDayStats(C.Structure):
+    """gysk_listener_day_stats: byte-compatible with LISTENER_DAY_STATS (48 bytes)"""
+    _fields_ = [("glob_id", C.c_uint64), ("tcount_5d", C.c_int64), ("tsum_5d", C.c_int64)] + \
+               [(n, C.c_uint32) for n in ("p95_5d_respms", "p25_5d_respms", "p95_qps", "p25_qps", "p95_nactive", "p25_nactive")]
+
+    def astuple(self):
+        return tuple(getattr(self, f) for f, _ in self._fields_)
+
+
+class HostListen(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("host_idx", "nlisten", "nlisten_issue", "nlisten_severe")]
+
+
+class HostStateIn(C.Structure):
+    """gysk_host_state_in: the inputs of host_status_update's state rule"""
+    _fields_ = [(n, C.c_uint8) for n in ("cpu_issue", "mem_issue", "severe_cpu_issue", "severe_mem_issue", "cpu_idle")] + \
+               [("pad", C.c_uint8 * 3)] + [(n, C.c_uint32) for n in ("ntasks_issue", "ntasks_severe", "nlisten_issue", "nlisten_severe")]
+
+
+def classify_host(**kw):
+    """gysk_classify_host on the named fields of HostStateIn (missing ones 0) -> GYSK_STATE_*"""
+    L = load_library()
+    st = C.c_uint8()
+    rc = L.gysk_classify_host(C.byref(HostStateIn(**kw)), C.byref(st))
+    if rc:
+        raise GyskError(rc, "gysk_classify_host")
+    return st.value
+
+
 class HostSummary(C.Structure):
     _fields_ = [("nstates", C.c_int32 * 8)] + [(n, C.c_int32) for n in ("tot_qps", "tot_act_conn", "tot_kb_inbound", "tot_kb_outbound",
                                                                          "tot_ser_errors", "nlisteners", "nactive", "pad")]
@@ -184,6 +213,9 @@ def load_library(path=None):
         "gysk_hist_bucket": (i32, [i32, C.c_int64]),
         "gysk_hist_percentiles": (i32, [i32, i32, vp, u64, vp, u32, vp]),
         "gysk_classify_listener": (i32, [vp, vp, vp, vp]),
+        "gysk_query_day_stats": (i32, [vp, C.c_int32, vp, vp, u32, vp]),
+        "gysk_query_host_listen": (i32, [vp, vp, u32, vp]),
+        "gysk_classify_host": (i32, [vp, vp]),
         "gysk_task_groupby": (i32, [vp, vp, u32, vp, u32, vp]),
         "gysk_hll_estimate": (C.c_double, [vp, u32]),
         "gysk_tdigest_quantile": (C.c_double, [vp, vp, u32, C.c_double, C.c_double, C.c_double]),
@@ -373,6 +405,29 @@ class Engine:
         self._chk(self.L.gysk_query_window_hosts(self.h, host_idx, flags, out if cap else None, _p(hosts) if cap else None, cap, C.byref(n)))
         k = min(cap, n.value)
         return out[:k], hosts[:k].copy(), n.value
+
+    def query_day_stats(self, host_idx=-1, cap=None):
+        """gysk_query_day_stats: (ListenerDayStats rows in the order of query_window_hosts, host_idx of each row, number of rows).
+        cap None = all rows (a count call first); 0 = the count only"""
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_day_stats(self.h, host_idx, None, None, 0, C.byref(n)))
+            cap = n.value
+        out = (ListenerDayStats * max(cap, 1))()
+        hosts = np.zeros(max(cap, 1), dtype=np.uint32)
+        self._chk(self.L.gysk_query_day_stats(self.h, host_idx, out if cap else None, _p(hosts) if cap else None, cap, C.byref(n)))
+        k = min(cap, n.value)
+        return out[:k], hosts[:k].copy(), n.value
+
+    def query_host_listen(self, cap=None):
+        """gysk_query_host_listen: (HostListen rows by ascending host, number of hosts). cap None = all rows; 0 = the count only"""
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_host_listen(self.h, None, 0, C.byref(n)))
+            cap = n.value
+        out = (HostListen * max(cap, 1))()
+        self._chk(self.L.gysk_query_host_listen(self.h, out if cap else None, cap, C.byref(n)))
+        return out[: min(cap, n.value)], n.value
 
     def query_tasks(self, ids):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)

@@ -6,14 +6,21 @@
 //     MCONN_HANDLER::partha_listener_state    server/gy_mconnhdlr.h:2129   (definition gy_mconnhdlr.cc:10993)
 //     MCONN_HANDLER::handle_partha_active_conns server/gy_mconnhdlr.h:2155 (definition gy_mconnhdlr.cc:7705)
 //     MCONN_HANDLER::handle_aggr_task_hist_stats server/gy_mconnhdlr.h:2109 (definition gy_mconnhdlr.cc:14648; reads the engine)
-// and forward the record batch to the GPU engine through the C ABI of include/gysketch.h. The template parameters
+// and forward the record batch to the GPU engine through the C ABI of include/gysketch.h. window_listener_day_stats and host_state
+// produce from the engine what a raw-forward partha no longer sends for MCONN_HANDLER::handle_listener_day_stats (gy_mconnhdlr.cc:12805)
+// and handle_host_state (gy_mconnhdlr.cc:12971). The template parameters
 // stand for the reference's own types (std::shared_ptr<PARTHA_INFO>, comm::TCP_CONN_NOTIFY, POOL_ALLOC_ARRAY, PGConnPool) so
 // that this header compiles both inside gy_mconnhdlr.cc (with the real types) and stand-alone in this repository's tests (with
 // the POD mirrors of gyeeta_b200/csrc/gysk_wire.h). See INTEGRATION.md for the call-site patch.
 #pragma once
 
+#include <algorithm>
+#include <atomic>
 #include <cstdint>
 #include <memory>
+#include <mutex>
+#include <new>
+#include <utility>
 #include <vector>
 
 #include "../../include/gysketch.h"
@@ -33,6 +40,11 @@ class GYSK_HANDLER
 {
 public :
 	explicit GYSK_HANDLER(gysk_engine *engine) noexcept : engine_(engine) {}
+	// a copy starts with host_state's rows unread
+	GYSK_HANDLER(const GYSK_HANDLER & o) : engine_(o.engine_), evicted_(o.evicted_), summ_(o.summ_) {}
+	GYSK_HANDLER & operator=(const GYSK_HANDLER & o) { if (this != &o) { GYSK_HANDLER t(o); *this = std::move(t); } return *this; }
+	GYSK_HANDLER(GYSK_HANDLER &&) noexcept = default;
+	GYSK_HANDLER & operator=(GYSK_HANDLER &&) noexcept = default;
 
 	// bool partha_tcp_conn_info(const std::shared_ptr<PARTHA_INFO> &, comm::TCP_CONN_NOTIFY *, int nconns, uint8_t *pendptr, POOL_ALLOC_ARRAY *)
 	template <typename ParthaInfo, typename TcpConnNotify, typename PoolArr>
@@ -93,7 +105,12 @@ public :
 	}
 
 	// the 5-s reducer tick (TCP_SOCK_HANDLER::listener_stats_update cadence, common/gy_socket_stat.cc:3898)
-	bool flush_window(uint32_t tsec) noexcept { return 0 == gysk_flush(engine_, tsec); }
+	bool flush_window(uint32_t tsec) noexcept
+	{
+		if (0 != gysk_flush(engine_, tsec)) return false;
+		if (hl_) hl_->flushes.fetch_add(1);
+		return true;
+	}
 
 	// The tick plus what the reference does when a partha reports a deleted listener (LISTENER_STATE_NOTIFY with
 	// query_flags_ == LISTEN_FLAG_DELETE, common/gy_socket_stat.cc:4023-4033): with gysk_config.idle_evict_secs set, the ids the
@@ -101,7 +118,7 @@ public :
 	template <typename OnDelete>
 	bool flush_window(uint32_t tsec, OnDelete && on_delete) noexcept
 	{
-		if (0 != gysk_flush(engine_, tsec)) return false;
+		if (!flush_window(tsec)) return false;
 		try {
 			uint32_t n = 0;
 			evicted_.resize(evicted_.size() < 1024 ? 1024 : evicted_.size());
@@ -166,6 +183,88 @@ public :
 		catch (...) { return false; }
 	}
 
+	// The 5-minute half of the listener walk in raw-forward mode (listener_stats_update sends it when tcurr > next_listen_stat_tsec_,
+	// common/gy_socket_stat.cc:3916-3919, :4417-4421): every listener older than 15 minutes as LISTENER_DAY_STATS records (48 bytes) in
+	// batches of at most 2048 (MAX_NUM_LISTENERS, common/gy_comm_proto.h:1632), host by host in ascending host index, ids ascending
+	// within a host, from one gysk_query_day_stats snapshot. Call after flush_window, every 5 minutes. on_batch(uint32_t host_idx,
+	// const void *recs, uint32_t nrecs) is where madhava calls its unchanged handle_listener_day_stats. Returns false on failure. Its
+	// scratch is local: safe to call while other threads use this handler.
+	template <typename OnBatch>
+	bool window_listener_day_stats(OnBatch && on_batch) noexcept
+	{
+		try {
+			std::vector<gysk_listener_day_stats> rows;
+			std::vector<uint32_t> hosts;
+			uint32_t n = 0, cap = 0;
+			for (int tries = 0; ; ++tries) {
+				rows.resize(cap); hosts.resize(cap);
+				if (0 != gysk_query_day_stats(engine_, -1, cap ? rows.data() : nullptr, cap ? hosts.data() : nullptr, cap, &n)) return false;
+				if (n <= cap) break;
+				if (tries == 3) return false;
+				cap = n + n / 8 + 64;
+			}
+			for (uint32_t a = 0; a < n; ) {
+				uint32_t b = a + 1;
+				while (b < n && b - a < MAX_DAY_BATCH && hosts[b] == hosts[a]) ++b;
+				on_batch(hosts[a], (const void *)(rows.data() + a), b - a);
+				a = b;
+			}
+			return true;
+		}
+		catch (...) { return false; }
+	}
+
+	// Before madhava's handle_host_state (server/gy_mconnhdlr.cc:12971-13026) when the listeners live in the engine: a raw-forward partha
+	// has no listener walk, so its HOST_STATE_NOTIFY (common/gy_comm_proto.h:2289-2330) reports no listeners. This fills nlisten_,
+	// nlisten_issue_ and nlisten_severe_ from gysk_query_host_listen for the partha's host, recomputes curr_state_ with
+	// host_status_update's rule (gysk_classify_host, common/gy_socket_stat.cc:4455-4528) from the message's own cpu, memory and task
+	// fields, and rewrites bit 0 of issue_bit_hist_ (:4540-4541). cpu_idle is not on the wire: it is taken as curr_state_ == IDLE. The
+	// rule reads cpu_idle only when nothing has an issue, and then partha's own evaluation, with zero listeners, took that same branch.
+	// A host without live services keeps zero counts. Returns false on failure (the message is then unchanged).
+	// Every partha sends one HOST_STATE_NOTIFY per 5 s, and the counts change only at a flush: the first call after each flush_window of
+	// this handler reads the rows of every host with one gysk_query_host_listen call, and every other call answers from those rows
+	// without entering the engine. Safe to call from any number of threads.
+	template <typename ParthaInfo, typename HostStateNotify>
+	bool host_state(const std::shared_ptr<ParthaInfo> & partha_shr, HostStateNotify *p) noexcept
+	{
+		if (!partha_shr || !p || !hl_) return false;
+		try {
+			const uint32_t host = partha_traits<ParthaInfo>::host_index(*partha_shr);
+			gysk_host_listen hl {host, 0, 0, 0};
+			{
+				std::lock_guard<std::mutex> g(hl_->m);
+				const uint64_t gen = hl_->flushes.load();
+				if (hl_->read_at != gen) {
+					if (hl_->rows.size() < HOST_ROWS) hl_->rows.resize(HOST_ROWS);
+					uint32_t n = 0;
+					if (0 != gysk_query_host_listen(engine_, hl_->rows.data(), (uint32_t)hl_->rows.size(), &n)) return false;
+					if (n > hl_->rows.size()) {			// more hosts than ever before: once more, with room
+						hl_->rows.resize(n + n / 8 + 64);
+						if (0 != gysk_query_host_listen(engine_, hl_->rows.data(), (uint32_t)hl_->rows.size(), &n)) return false;
+					}
+					hl_->n = n < hl_->rows.size() ? n : (uint32_t)hl_->rows.size();
+					hl_->read_at = gen;
+				}
+				const auto end = hl_->rows.begin() + hl_->n;		// ascending host_idx
+				const auto it = std::lower_bound(hl_->rows.begin(), end, host, [](const gysk_host_listen &r, uint32_t h) { return r.host_idx < h; });
+				if (it != end && it->host_idx == host) hl = *it;
+			}
+			gysk_host_state_in in {};
+			in.cpu_issue = p->cpu_issue_; in.mem_issue = p->mem_issue_;
+			in.severe_cpu_issue = p->severe_cpu_issue_; in.severe_mem_issue = p->severe_mem_issue_;
+			in.cpu_idle = p->curr_state_ == GYSK_STATE_IDLE;
+			in.ntasks_issue = p->ntasks_issue_; in.ntasks_severe = p->ntasks_severe_;
+			in.nlisten_issue = hl.nlisten_issue; in.nlisten_severe = hl.nlisten_severe;
+			uint8_t state = 0;
+			if (0 != gysk_classify_host(&in, &state)) return false;
+			p->nlisten_ = hl.nlisten; p->nlisten_issue_ = hl.nlisten_issue; p->nlisten_severe_ = hl.nlisten_severe;
+			p->curr_state_ = state;
+			p->issue_bit_hist_ = (uint8_t)((p->issue_bit_hist_ & ~1u) | (state >= GYSK_STATE_BAD ? 1u : 0u));
+			return true;
+		}
+		catch (...) { return false; }
+	}
+
 	// bool handle_aggr_task_hist_stats(const std::shared_ptr<MCONNTRACK> &, AGGR_TASK_HIST_STATS *, int nevents, POOL_ALLOC_ARRAY *, PGConnPool &)
 	// (server/gy_mconnhdlr.cc:14648-14706) when the process histograms live in the engine: fills p95_cpu_pct_, p95_cpu_delay_ms_ and
 	// p95_blkio_delay_ms_ of the records whose aggregated process the engine holds for this partha (the reference looks each id up in
@@ -207,8 +306,22 @@ private :
 	}
 
 	static constexpr uint32_t MAX_BATCH = 512, RECORD_BYTES = 88;		// records per NOTIFY_LISTENER_STATE message, sizeof(LISTENER_STATE_NOTIFY)
+	static constexpr uint32_t MAX_DAY_BATCH = 2048;				// records per NOTIFY_LISTENER_DAY_STATS message
+
+	static constexpr uint32_t HOST_ROWS = 1024;				// host_state's first read: MAX_PARTHA_PER_MADHAVA (512) hosts fit
+
+	// host_state's per-host rows, read once per flush_window (a separate object: the handler stays movable and copyable)
+	struct HostListenCache
+	{
+		std::mutex			m;
+		std::atomic<uint64_t>		flushes {1};		// flush_window calls so far + 1
+		uint64_t			read_at {0};		// ... when the rows were read
+		std::vector<gysk_host_listen>	rows;
+		uint32_t			n {0};
+	};
 
 	gysk_engine		*engine_;
+	std::unique_ptr<HostListenCache> hl_ {new (std::nothrow) HostListenCache};
 	std::vector<uint64_t>	evicted_;		// scratch of flush_window(tsec, on_delete) and listener_state_records: one caller at a time
 	std::vector<gysk_svc_summary> summ_;
 };

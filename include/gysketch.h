@@ -386,6 +386,61 @@ int		gysk_query_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_sv
 int		gysk_query_window_hosts(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_summary *out, uint32_t *hosts, uint32_t cap,
 				uint32_t *n);
 
+/* ---- the rest of the 5-s listener walk (TCP_SOCK_HANDLER::listener_stats_update, common/gy_socket_stat.cc:3898-4445) ---- */
+
+/* byte-compatible with LISTENER_DAY_STATS, common/gy_comm_proto.h:1620-1653 (48 bytes, at most 2048 per NOTIFY_LISTENER_DAY_STATS
+ * message): what madhava's handle_listener_day_stats (server/gy_mconnhdlr.cc:12805-12836) turns into the svcinfo fields p95resp5d,
+ * avgresp5d, p95qps and p95aconn */
+typedef struct gysk_listener_day_stats
+{
+	uint64_t	glob_id;
+	int64_t		tcount_5d;		/* histstat_[n5days].tcount_ */
+	int64_t		tsum_5d;		/* histstat_[n5days].tsum_ (msec) */
+	uint32_t	p95_5d_respms, p25_5d_respms;	/* r5daysp95 / r5daysp25 */
+	uint32_t	p95_qps, p25_qps;	/* qps_hist_ percentiles */
+	uint32_t	p95_nactive, p25_nactive;	/* active_conn_hist_ percentiles */
+} gysk_listener_day_stats;
+
+/* The LISTENER_DAY_STATS records of get_curr_state (common/gy_socket_stat.cc:2101-2117), as of the last gysk_flush:
+ *  - rows, their order (grouped by ascending host_idx, ascending id within a host), hosts[] and the count / capacity rules are those of
+ *    gysk_query_window_hosts (cap 0 counts; *n may exceed cap), restricted to the services old enough for a row;
+ *  - a service has a row only when last flush tsec > tsec of the first flush that saw its slot + 900: the reference's
+ *    tcur > tstart + 15 * 60 (:2102), under which a young listener sends nothing (statn.glob_id_ == 0, :4367). A slot recycled after an
+ *    eviction starts over. A stale service (no events in the closed window) has a row: the reference evaluates it too;
+ *  - tcount_5d / tsum_5d / p95_5d_respms / p25_5d_respms: the 5-day level (GYSK_HIST_RESP_5DAY) with the GY_HISTOGRAM percentile rule,
+ *    the values gysk_flush hands the state classifier; p95_qps / p25_qps / p95_nactive / p25_nactive: the percentiles of qps_hist_ and
+ *    active_conn_hist_ (GYSK_HIST_QPS / GYSK_HIST_ACTIVE_CONN) as they stand after the flush: for a service evaluated at that flush the
+ *    classifier's values, for a stale one what the reference computes without an add_data (:4099-4112). Every value is stored into its
+ *    field by the reference's int64 -> uint32 conversion (an empty qps histogram's -1 becomes 0xFFFFFFFF);
+ *  - the reference sends these every 5 minutes (next_listen_stat_tsec_, :4420): the cadence is the caller's, the engine keeps no timer. */
+int		gysk_query_day_stats(gysk_engine *e, int32_t host_idx, gysk_listener_day_stats *out, uint32_t *hosts, uint32_t cap, uint32_t *n);
+
+/* the listener half of the tuple listener_stats_update returns to host_status_update (common/gy_socket_stat.cc:173-175) */
+typedef struct gysk_host_listen
+{
+	uint32_t	host_idx;
+	uint32_t	nlisten;		/* nlist++ (:4277): the host's rows of gysk_query_window_hosts(-1, 0) */
+	uint32_t	nlisten_issue;		/* nissue++ (:4242-4249): services evaluated at the last flush whose issue bit 0 was set there */
+	uint32_t	nlisten_severe;		/* nsevere++ (:4250-4252): ... of those, the ones in GYSK_STATE_SEVERE or worse */
+} gysk_host_listen;
+/* One row per host with live services, ascending host_idx; *n = number of such hosts, at most cap rows are written (out may be NULL
+ * when cap is 0). Only these rows travel to the host, not one per service. nlisten_issue / nlisten_severe are those of the last
+ * gysk_flush; nlisten is the row count of gysk_query_window_hosts(-1, 0) at the time of the call, so it also counts services whose first
+ * events arrived after the last flush (and a host with only such services has a row). The reference's walk skips a listener younger
+ * than 1 s (:4040-4062); here arrival granularity is the window. Every call lists and sorts every live service: a caller with one
+ * message per host and window (HOST_STATE_NOTIFY) reads all hosts once per flush and answers the messages from those rows, as the
+ * shim's host_state does. */
+int		gysk_query_host_listen(gysk_engine *e, gysk_host_listen *out, uint32_t cap, uint32_t *n);
+
+/* inputs of host_status_update's state rule (common/gy_socket_stat.cc:4455-4528) */
+typedef struct gysk_host_state_in
+{
+	uint8_t		cpu_issue, mem_issue, severe_cpu_issue, severe_mem_issue, cpu_idle, pad[3];
+	uint32_t	ntasks_issue, ntasks_severe, nlisten_issue, nlisten_severe;
+} gysk_host_state_in;
+/* host_status_update's state rule: writes the GYSK_STATE_* of HOST_STATE_NOTIFY::curr_state_. Pure, no engine, like gysk_classify_listener */
+int		gysk_classify_host(const gysk_host_state_in *in, uint8_t *state);
+
 /* per aggregated process: the p95 fields of AGGR_TASK_HIST_STATS (common/gy_comm_proto.h:2966-2977) as
  * handle_aggr_task_hist_stats fills them (server/gy_mconnhdlr.cc:14648-14706: get_percentiles({95}) of the three MTASK_HIST
  * histograms, T = int, -1 for an empty histogram) and the last closed window of each histogram, the window the top-N lists rank */
