@@ -31,7 +31,7 @@ static constexpr int TD_CAP = 256;		// delta = 200 yields 200 ... 1.3 x 200 cent
 // so that the bin's exact msec sum (GY_HISTOGRAM::add_data adds usec / 1000 per sample) is (us - remainders) / 1000 and its mean
 // us / samples. Bin index = td_code(usec) + RESP_TIME_HASH bucket of its msec value: both terms are monotone in usec, so the
 // index is too and no bin straddles a histogram bucket. Two ways lead to the same numbers: the samples of most services travel as
-// sort keys and are summed per run of equal {slot, bin} (RunRec, gysk_kernels.cu); a HOT service — one that brought at least
+// sort keys and are summed per run of equal {slot, bin} (bins_merge_kernel, gysk_kernels.cu); a HOT service — one that brought at least
 // hot_min samples in an earlier batch — owns a dense row of such bins (DevState::hot_rows, L2-resident; layout below) and
 // every one of its samples is two 64-bit REDs into it, no key, no sort. The batch's merge kernel reads a row in order and zeroes it.
 struct alignas(16) Bin { unsigned long long cw; unsigned long long us; };
@@ -76,7 +76,8 @@ static constexpr unsigned long long KEY_TOMBSTONE = ~0ull;	// table entry of an 
 
 // device counters (index into Engine::d_counters). CTR_NKEYS is the sort-key cursor, which ingest_kernel bumps once per warp and
 // key flush (about 160 K returning atomics per 100 M-event batch); the connection / process records need no cursor (SortTemp::recq).
-enum { CTR_IN = 0, CTR_DROPPED, CTR_RESP, CTR_TCP, CTR_TASK, CTR_FOREIGN, CTR_NKEYS, CTR_INSERT_FAIL, CTR_NTOUCHED, CTR_NRUNS, CTR_NEVICT, CTR_EVICTED_TOTAL,
+enum { CTR_IN = 0, CTR_DROPPED, CTR_RESP, CTR_TCP, CTR_TASK, CTR_FOREIGN, CTR_NKEYS, CTR_INSERT_FAIL, CTR_NTOUCHED /* short key segments */,
+	CTR_NLONG /* long key segments (batch rows) */, CTR_NEVICT, CTR_EVICTED_TOTAL,
 	CTR_NHOT /* hot rows in use by the batch in flight */, CTR_NHOT_NEXT /* rows handed out so far */, CTR_NWINDOW /* rows of the last window read */,
 	CTR_NHOSTS /* host rows of the last gysk_query_host_listen */, CTR_MAX };
 
@@ -222,6 +223,12 @@ __device__ __forceinline__ void red_add_u64(unsigned long long *p, unsigned long
 __device__ __forceinline__ void red_max_s64(long long *p, long long v)
 {
 	asm volatile("red.global.max.s64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+}
+
+// bring the 128-byte line holding p into L2 (no register waits for it)
+__device__ __forceinline__ void prefetch_l2(const void *p)
+{
+	asm volatile("prefetch.global.L2 [%0];" :: "l"(p));
 }
 
 // L2 eviction priorities. A policy (createpolicy, a 64-bit register) travels with each access through .L2::cache_hint: ptxas for

@@ -506,10 +506,10 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &tmp.touched, ns));
 	{
 		const size_t nmw = (size_t)TD_MERGE_MAX_SMS * TD_MERGE_CTAS_PER_SM * 4;		// warps of bins_merge_kernel
-		// a batch cannot have more runs than keys, nor than the engine has bins
-		const size_t pool_cap = std::min<size_t>((size_t)cfg.max_batch, (size_t)cfg.max_svcs * NBINS) + 8;
-		A(dalloc(e, &tmp.pool, pool_cap, false)); A(dalloc(e, &tmp.run_bin, pool_cap, false));
-		A(dalloc(e, &tmp.chunk_run, ((size_t)cfg.max_batch >> 7) + 16, false)); A(dalloc(e, &tmp.segs, ns));
+		// a batch has fewer than max_batch / LONG_SEG segments of more than LONG_SEG keys, and no more than one per service. The
+		// rows start at zero and bins_merge_kernel leaves them so.
+		const size_t nbrows = std::min<size_t>(ns, ((size_t)cfg.max_batch + LONG_SEG - 1) / LONG_SEG);
+		A(dalloc(e, &tmp.segs, ns)); A(dalloc(e, &tmp.long_slot, nbrows, false)); A(dalloc(e, &tmp.batch_rows, nbrows * HOT_ROW_WORDS));
 		A(dalloc(e, &tmp.items_scratch, nmw * NBINS, false)); A(dalloc(e, &tmp.big_scratch, nmw, false));
 		// the batch's connection / process record queue: one region per ingest warp (SortTemp::recq)
 		const uint32_t nsm = (uint32_t)prop.multiProcessorCount;

@@ -53,10 +53,10 @@ struct SortTemp
 	uint32_t		*epoch;			// HOST counter of radix passes launched (tags the status words)
 	uint32_t		*os_ghist;		// [8][512] global digit histograms of the one-sweep passes + [8] tile tickets
 	uint32_t		*touched;		// [max_svcs] services with RESP samples in the batch
-	ulonglong2		*pool;			// [pool_cap] RunRec: one record per run (non-empty bin of a service) of the batch
-	uint16_t		*run_bin;		// [pool_cap] bin index of each run
-	uint32_t		*chunk_run;		// [max_batch / 128] run of the first key of every 128-key chunk
-	uint4			*segs;			// [max_svcs] BatchSeg of each touched service
+	uint4			*segs;			// [max_svcs] BatchSeg of each touched service: its keys in the sorted array, its batch row
+	uint32_t		*long_slot;		// [batch rows] slot of each long segment (more than LONG_SEG keys) of the batch
+	unsigned long long	*batch_rows;		// [batch rows][HOT_ROW_WORDS] dense value bins of the long segments, hot-row layout; zero
+							// between batches (bins_merge_kernel zeroes what it reads)
 	Centroid		*items_scratch;		// [merge warps][NBINS] a warp's list of batch items
 	TdWorkBig		*big_scratch;		// [merge warps] work arrays for merged lists beyond 2 x TD_CAP entries
 	uint4			*recq;			// [recq_cap] records {slot, value, flow key}: ingest_kernel resolves the ids of connection and
@@ -111,6 +111,9 @@ static constexpr int RADIX_MAX_BITS = 9;
 static constexpr int RADIX_MAX = 1 << RADIX_MAX_BITS;
 static constexpr int OS_MAX_PASSES_VK = 5;		// {slot : <= 24 | bin : 10} = <= 34 bits in digits of <= 8 bits
 static constexpr int TD_MERGE_CTAS_PER_SM = 7, TD_MERGE_MAX_SMS = 192;	// bins_merge_kernel grid (<= 4 warps per CTA)
+// a service segment of more than LONG_SEG sorted keys is summed into a batch row by long_sum_kernel; a shorter one is read by one warp
+// of bins_merge_kernel (DESIGN.md §4). Batch rows: min(max_svcs, ceil(max_batch / LONG_SEG)).
+static constexpr int LONG_SEG = 8192;
 
 // every launcher returns the number of kernel launches it issued
 int launch_init_state(const DevState &st, uint32_t max_svcs, uint32_t max_tasks, cudaStream_t s);

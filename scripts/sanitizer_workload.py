@@ -3,7 +3,7 @@
     compute-sanitizer --tool racecheck python scripts/sanitizer_workload.py
 
 ingest_kernel (all five event kinds, auto-registration), the one-sweep radix passes with 6- to 8-bit digits (the batches' key
-sorts, the top-N sorts) and 9-bit digits (a group-by of 100 000 samples), runs_mark / runs_sum / bins_merge (small and > 512-entry
+sorts, the top-N sorts) and 9-bit digits (a group-by of 100 000 samples), segs_mark / long_sum / bins_merge (small and > 512-entry
 merged lists), flush + eviction + table rebuild, the raw decode kernel, the merge step's fold / finish kernels, the read-side
 gathers. Sizes keep a racecheck run within a few minutes."""
 import os
