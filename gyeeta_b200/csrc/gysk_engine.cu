@@ -254,7 +254,7 @@ int gysk::drain_all(gysk_engine *e)
 	return 0;
 }
 
-namespace {
+namespace gysk {
 
 // ---- pure host helpers: the reference's percentile rule and the estimators -------------------------------
 
@@ -286,6 +286,10 @@ uint32_t live_mask(const gysk_engine *e, int l)
 	}
 	return m;
 }
+
+} // namespace gysk
+
+namespace {
 
 // the unit grid of the K_1 scale: q_j = (sin(pi (j/delta - 1/2)) + 1)/2 — libm on the host, the same expression as the oracle. The
 // device's grid and the pgtext export's compress both come from here.

@@ -99,14 +99,20 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn
-	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux]
+	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt, flush tsec]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
 	HistCell		*l_hist_last {nullptr}, *l_hist_all {nullptr};
 	unsigned long long	*l_conn {nullptr};			// [nl][4]: last cnt, last kb, all cnt, all kb
 	long long		*l_hmax {nullptr};			// [nl][2]: last, all
 	uint8_t			*l_hll {nullptr};
+	// GYSK_FLAG_MERGE_LEVELS only (nullptr without it): appended to the ends of the SUM and i64 MAX regions
+	HistCell		*l_lvl {nullptr};			// SUM [2][nl][16]: the live ring slots of the 300-s / 5-day levels, cells 0..14
+	unsigned long long	*l_aux {nullptr};			// SUM [nl][4]: active conns, active kbytes, client errors, server errors
+	long long		*l_lvl_max {nullptr};			// MAX [nl][2]: max_val_seen_ of the 300-s / 5-day levels
+	long long		*l_rtt {nullptr};			// MAX [nl]: the largest rtt_last bit pattern (a non-negative float's order)
+	long long		*l_flush {nullptr};			// MAX [2]: {last_flush_tsec, -last_flush_tsec} of this engine
 	// t-digest slab: fixed [nl] x {TdHead, Centroid[TD_CAP]}
 	uint8_t			*slab {nullptr};
 	size_t			slab_bytes {0};
@@ -193,6 +199,10 @@ int submit_stage(gysk_engine *e);
 int drain_all(gysk_engine *e);
 int sync_locked(gysk_engine *e);
 void merge_release(gysk_engine *e);
+// HIST_SERIAL of 16 cells (cell HIST_MAX_CELL holds max_val_seen_ in .sum); total = the sum of the first nb counts
+void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint64_t *total, int64_t *maxv, bool t_is_int);
+// ring slots of rolling level l (0: 300 s, 1: 5 days) still inside the level's span at the last flush
+uint32_t live_mask(const gysk_engine *e, int l);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)

@@ -8,10 +8,12 @@
 //   gysk_merge_prepare     fold this GPU's member services into per-logical arrays laid out in ONE arena:
 //                            [u64 SUM region : global CMS cur/last | histogram last/all | conn cells]
 //                            [i64 MAX region : max_val_seen_ last/all]   [u8 MAX region : HLL registers]
-//                          and a fixed t-digest slab (not element-wise mergeable)
+//                          and a fixed t-digest slab (not element-wise mergeable); GYSK_FLAG_MERGE_LEVELS appends the rolling
+//                          levels and aux sums to the SUM region, their maxima, the rtt and the flush tsec pair to the i64 MAX one
 //   (caller)               all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
+//   gysk_export_logical_hist / gysk_merge_flush_range   one merged histogram / the ranks' flush tsec range
 //
 // It is the additive roll-up of MS_CLUSTER_STATE::STATE_ONE::add_stats (common/gy_comm_proto.h:3199-3214) /
 // SHCONN_HANDLER::aggregate_cluster_state (server/gy_shconnhdlr.cc:4583) and of GY_HISTOGRAM::update_from_serialized
@@ -75,6 +77,64 @@ __global__ void fold_hist_kernel(DevState st, const uint32_t *__restrict__ offs,
 		l_last[i] = HistCell {0, 0}; l_all[i] = HistCell {0, 0};
 		l_hmax[2 * l] = ml; l_hmax[2 * l + 1] = ma;
 		l_conn[4 * l] = lc; l_conn[4 * l + 1] = lk; l_conn[4 * l + 2] = ac; l_conn[4 * l + 3] = ak;
+	}
+}
+
+// GYSK_FLAG_MERGE_LEVELS, one thread per (logical, cell): cells 0..14 sum the live ring slots of both rolling levels over the members
+// (live0 / live1: the masks gather_slot applies, so a member adds exactly the lvl[] of its own gysk_query_svcs row); the cell-15
+// thread takes the level maxima, the aux words of the last closed window and the largest rtt. Thread 0 also writes this engine's
+// {last flush tsec, -last flush tsec}, whose i64 max over the ranks gives their latest and earliest flush.
+__global__ void fold_levels_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t nl, uint32_t null_slot,
+		uint32_t live0, uint32_t live1, long long flush_tsec, HistCell *__restrict__ l_lvl, unsigned long long *__restrict__ l_aux,
+		long long *__restrict__ l_lvl_max, long long *__restrict__ l_rtt, long long *__restrict__ l_flush)
+{
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i == 0) { l_flush[0] = flush_tsec; l_flush[1] = -flush_tsec; }
+	if (i >= (uint64_t)nl * HIST_CELLS) return;
+	const uint32_t l = (uint32_t)(i >> 4);
+	const int cell = (int)(i & 15);
+	const uint32_t b = offs[l], e = offs[l + 1];
+	const size_t max_svcs = null_slot;		// the null slot is the index past the last one: the ring planes hold max_svcs slots
+	auto ring = [&](int lv, int k, uint32_t s) -> const HistCell & {
+		return st.hist_ring[(((size_t)lv * NSLOTS + k) * max_svcs + s) * HIST_CELLS + cell];
+	};
+
+	if (cell < HIST_MAX_CELL) {
+		HistCell a[NLEVELS] {};
+		for (uint32_t m = b; m < e; ++m) {
+			const uint32_t s = members[m];
+			if (s == null_slot) continue;
+#pragma unroll
+			for (int lv = 0; lv < NLEVELS; ++lv) {
+				const uint32_t live = lv ? live1 : live0;
+#pragma unroll
+				for (int k = 0; k < NSLOTS; ++k) {
+					if (!((live >> k) & 1u)) continue;
+					const HistCell x = ring(lv, k, s);
+					a[lv].count += x.count; a[lv].sum += x.sum;
+				}
+			}
+		}
+		for (int lv = 0; lv < NLEVELS; ++lv) l_lvl[((size_t)lv * nl + l) * HIST_CELLS + cell] = a[lv];
+	}
+	else {
+		long long mx[NLEVELS] = {LLONG_MIN, LLONG_MIN};
+		unsigned long long ac = 0, ak = 0, ce = 0, se = 0;
+		uint32_t rtt = 0;
+		for (uint32_t m = b; m < e; ++m) {
+			const uint32_t s = members[m];
+			if (s == null_slot) continue;
+			for (int lv = 0; lv < NLEVELS; ++lv) {
+				const uint32_t live = lv ? live1 : live0;
+				for (int k = 0; k < NSLOTS; ++k) if ((live >> k) & 1u) mx[lv] = max(mx[lv], ring(lv, k, s).sum);
+			}
+			const SlotAux x = st.slot_aux[s];
+			ac += (uint32_t)x.act_last; ak += x.act_last >> 32; ce += (uint32_t)x.err_last; se += x.err_last >> 32;
+			rtt = max(rtt, x.rtt_last);
+		}
+		for (int lv = 0; lv < NLEVELS; ++lv) { l_lvl[((size_t)lv * nl + l) * HIST_CELLS + cell] = HistCell {0, 0}; l_lvl_max[2 * l + lv] = mx[lv]; }
+		l_aux[4 * l] = ac; l_aux[4 * l + 1] = ak; l_aux[4 * l + 2] = ce; l_aux[4 * l + 3] = se;
+		l_rtt[l] = rtt;
 	}
 }
 
@@ -149,13 +209,17 @@ __global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntr
 	}
 }
 
+// the merged rolling levels and aux words (GYSK_FLAG_MERGE_LEVELS; lvl == nullptr without it)
+struct LevelArrays { const HistCell *lvl; const unsigned long long *aux; const long long *lvl_max, *rtt; uint32_t nl; };
+
 // read side: one warp per logical service, its merged arrays into a shared-memory SvcRaw, then the row of summarize_warp (the
-// summary of gysk_query_svcs). The merge folds neither the current window, the rolling levels, the connection bitmaps nor the
-// per-slot aux / state / qps / active-connection words: they are zero. glob_id is left 0 for the host to fill in.
+// summary of gysk_query_svcs). The merge folds neither the current window, the connection bitmaps nor the per-slot state / qps /
+// active-connection words: they are zero; so are the rolling levels and the aux words unless the engine merges them (lv.lvl).
+// glob_id is left 0 for the host to fill in.
 static constexpr int LG_WARPS = 4;
 __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const int32_t *__restrict__ lidx, uint32_t n, uint32_t hll_p,
 		const HistCell *__restrict__ l_last, const HistCell *__restrict__ l_all, const unsigned long long *__restrict__ l_conn,
-		const long long *__restrict__ l_hmax, const uint8_t *__restrict__ l_hll, const SlabEntry *__restrict__ slab,
+		const long long *__restrict__ l_hmax, const uint8_t *__restrict__ l_hll, const SlabEntry *__restrict__ slab, LevelArrays lv,
 		gysk_svc_summary *__restrict__ out)
 {
 	__shared__ SvcRaw raw[LG_WARPS];
@@ -172,7 +236,14 @@ __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const in
 			HistCell a = l_last[(size_t)l * HIST_CELLS + lane], b = l_all[(size_t)l * HIST_CELLS + lane];
 			if (lane == HIST_MAX_CELL) { a.sum = l_hmax[2 * l]; b.sum = l_hmax[2 * l + 1]; }
 			r.last[lane] = a; r.all[lane] = b; r.cur[lane] = HistCell {0, 0};
-			r.lvl[0][lane] = HistCell {0, 0}; r.lvl[1][lane] = HistCell {0, 0};
+			for (int k = 0; k < NLEVELS; ++k) {
+				HistCell c {0, 0};
+				if (lv.lvl) {
+					c = lv.lvl[((size_t)k * lv.nl + l) * HIST_CELLS + lane];
+					if (lane == HIST_MAX_CELL) c.sum = lv.lvl_max[2 * l + k];
+				}
+				r.lvl[k][lane] = c;
+			}
 			r.bm_cur[lane] = 0; r.bm_last[lane] = 0;
 			r.qps[lane] = HistCell {0, 0}; r.act[lane] = HistCell {0, 0};
 		}
@@ -182,6 +253,12 @@ __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const in
 			r.conn_all_cnt = l_conn[4 * l + 2]; r.conn_all_kb = l_conn[4 * l + 3];
 			r.td = slab[l].head;
 			r.aux = SlotAux {0, 0, 0, 0, 0, 0};
+			if (lv.lvl) {
+				const unsigned long long *a = lv.aux + 4 * (size_t)l;
+				r.aux.act_last = (a[0] & 0xFFFFFFFFull) | (a[1] << 32);
+				r.aux.err_last = (a[2] & 0xFFFFFFFFull) | (a[3] << 32);
+				r.aux.rtt_last = (uint32_t)lv.rtt[l];
+			}
 			r.sst = SlotState {0, 0, 0, 0, 0};
 		}
 		for (int i = lane; i < TD_CAP; i += 32) r.cent[i] = slab[l].cent[i];
@@ -316,8 +393,21 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	const size_t o_hl = off; off += align256(b_hist);
 	const size_t o_ha = off; off += align256(b_hist);
 	const size_t o_conn = off; off += align256(b_conn);
+	// GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX regions: still three regions, three collectives
+	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS;
+	size_t o_lvl = 0, o_aux = 0, o_lmax = 0, o_rtt = 0, o_flush = 0;
+	if (levels) {
+		o_lvl = off; off += align256((size_t)NLEVELS * b_hist);
+		o_aux = off; off += align256((size_t)nl * 4 * 8);
+	}
 	mg.bytes_sum = off - mg.off_sum;
-	mg.off_maxi64 = off; const size_t o_hmax = off; off += align256((size_t)nl * 2 * 8); mg.bytes_maxi64 = off - mg.off_maxi64;
+	mg.off_maxi64 = off; const size_t o_hmax = off; off += align256((size_t)nl * 2 * 8);
+	if (levels) {
+		o_lmax = off; off += align256((size_t)nl * NLEVELS * 8);
+		o_rtt = off; off += align256((size_t)nl * 8);
+		o_flush = off; off += align256(2 * 8);
+	}
+	mg.bytes_maxi64 = off - mg.off_maxi64;
 	mg.off_maxu8 = off; const size_t o_hll = off; off += align256((size_t)nl << e->cfg.hll_p); mg.bytes_maxu8 = off - mg.off_maxu8;
 	mg.arena_bytes = off;
 
@@ -330,6 +420,13 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	mg.l_conn = reinterpret_cast<unsigned long long *>(mg.arena + o_conn);
 	mg.l_hmax = reinterpret_cast<long long *>(mg.arena + o_hmax);
 	mg.l_hll = mg.arena + o_hll;
+	if (levels) {
+		mg.l_lvl = reinterpret_cast<HistCell *>(mg.arena + o_lvl);
+		mg.l_aux = reinterpret_cast<unsigned long long *>(mg.arena + o_aux);
+		mg.l_lvl_max = reinterpret_cast<long long *>(mg.arena + o_lmax);
+		mg.l_rtt = reinterpret_cast<long long *>(mg.arena + o_rtt);
+		mg.l_flush = reinterpret_cast<long long *>(mg.arena + o_flush);
+	}
 	mg.slab_bytes = (size_t)(nl ? nl : 1) * sizeof(SlabEntry);
 	if ((rc = dalloc(e, &mg.slab, mg.slab_bytes))) return rc;
 	if ((rc = dalloc(e, &mg.final_slab, mg.slab_bytes))) return rc;
@@ -370,6 +467,12 @@ int gysk_merge_prepare(gysk_engine *e)
 				reinterpret_cast<SlabEntry *>(mg.slab));
 		e->kernel_launches += 3;
 	}
+	if (mg.l_lvl) {		// GYSK_FLAG_MERGE_LEVELS: also with no logical service, for the flush tsec pair
+		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members,
+				nl, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1), (long long)e->last_flush_tsec, mg.l_lvl, mg.l_aux, mg.l_lvl_max, mg.l_rtt,
+				mg.l_flush);
+		e->kernel_launches++;
+	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
 	return post_launch(e, "merge_prepare");
@@ -383,8 +486,11 @@ int gysk_merge_buffers(gysk_engine *e, gysk_buffer_desc *out, uint32_t cap, uint
 	MergeState &mg = e->mg;
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_buffers: call gysk_set_logical_map first");
 	if (cap < 3) return GYSK_ERR_NOSPC;
-	out[0] = gysk_buffer_desc {"sum_u64: cms_cur|cms_last|hist_last|hist_all|conn", mg.arena + mg.off_sum, mg.bytes_sum, GYSK_RED_SUM_U64, 0};
-	out[1] = gysk_buffer_desc {"max_i64: hist max_val_seen", mg.arena + mg.off_maxi64, mg.bytes_maxi64, GYSK_RED_MAX_I64, 0};
+	const bool lv = mg.l_lvl != nullptr;
+	out[0] = gysk_buffer_desc {lv ? "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn|levels|aux" : "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn",
+			mg.arena + mg.off_sum, mg.bytes_sum, GYSK_RED_SUM_U64, 0};
+	out[1] = gysk_buffer_desc {lv ? "max_i64: hist max_val_seen|level max_val_seen|rtt|flush tsec" : "max_i64: hist max_val_seen",
+			mg.arena + mg.off_maxi64, mg.bytes_maxi64, GYSK_RED_MAX_I64, 0};
 	out[2] = gysk_buffer_desc {"max_u8: hll registers", mg.arena + mg.off_maxu8, mg.bytes_maxu8, GYSK_RED_MAX_U8, 0};
 	*n = 3;
 	return GYSK_OK;
@@ -432,15 +538,65 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 		lidx[i] = it == mg.index.end() ? -1 : (int32_t)it->second;
 	}
 	const SvcRows rows {e->cfg.hll_p, out};
+	const LevelArrays lv {mg.l_lvl, mg.l_aux, mg.l_lvl_max, mg.l_rtt, mg.nlogical};
 	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(gysk_svc_summary), "query_logical", [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
 		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(reinterpret_cast<const int32_t *>(d_l), m, e->cfg.hll_p,
-				mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax, mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab),
+				mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax, mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab), lv,
 				reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
 		return 1;
 	}, [&](const uint8_t *h_rows, uint32_t off, uint32_t m) {
 		rows(h_rows, off, m);
 		for (uint32_t i = 0; i < m; ++i) out[off + i].glob_id = logical_ids[off + i];
 	});
+}
+
+int gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS], uint64_t *total,
+		int64_t *maxv)
+{
+	CHECK_ENGINE(e);
+	if (!out || !total || !maxv) return GYSK_ERR_INVAL;
+	const bool level = which == GYSK_HIST_RESP_5MIN || which == GYSK_HIST_RESP_5DAY;
+	if (!level && which != GYSK_HIST_RESP_LAST && which != GYSK_HIST_RESP_ALL) return GYSK_ERR_INVAL;
+	if (level && !(e->cfg.flags & GYSK_FLAG_MERGE_LEVELS)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_export_logical_hist: no finished merge");
+	const auto it = mg.index.find(logical_id);
+	if (it == mg.index.end()) return GYSK_ERR_NOENT;
+	const uint32_t l = it->second;
+	const HistCell *cells;
+	const long long *mx;
+	if (level) {
+		const int k = which - GYSK_HIST_RESP_5MIN;
+		cells = mg.l_lvl + ((size_t)k * mg.nlogical + l) * HIST_CELLS; mx = mg.l_lvl_max + 2 * (size_t)l + k;
+	}
+	else {
+		const int k = which == GYSK_HIST_RESP_ALL;
+		cells = (k ? mg.l_hist_all : mg.l_hist_last) + (size_t)l * HIST_CELLS; mx = mg.l_hmax + 2 * (size_t)l + k;
+	}
+	// the 15 cells, then max_val_seen_ into cell 15 (stream order: behind the merge that wrote them)
+	HistCell *h = reinterpret_cast<HistCell *>(e->h_wstage);
+	CU(e, cudaMemcpyAsync(h, cells, HIST_CELLS * sizeof(HistCell), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaMemcpyAsync(&h[HIST_MAX_CELL].sum, mx, sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	hist_from_cells(h, 15, out, total, maxv, false);
+	if (level && *total == 0) *maxv = INT64_MIN;		// as gysk_export_hist answers an empty level
+	return GYSK_OK;
+}
+
+int gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tsec)
+{
+	CHECK_ENGINE(e);
+	if (!min_tsec || !max_tsec) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_MERGE_LEVELS)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_merge_flush_range: no finished merge");
+	long long *h = reinterpret_cast<long long *>(e->h_wstage);
+	CU(e, cudaMemcpyAsync(h, mg.l_flush, 2 * sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	*max_tsec = (uint32_t)h[0]; *min_tsec = (uint32_t)-h[1];
+	return GYSK_OK;
 }
 
 // global count-min point query on the merged table

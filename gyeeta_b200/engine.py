@@ -32,7 +32,7 @@ assert RESP16_DTYPE.itemsize == 16 and TCP24_DTYPE.itemsize == 24 and TASK24_DTY
 NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CONN_STATS = 0x309, 0x30C, 0x310, 0x312
 (HOSTTOP_SVC_ISSUE, HOSTTOP_SVC_QPS, HOSTTOP_SVC_CONNS, HOSTTOP_SVC_NET, HOSTTOP_TASK_ISSUE, HOSTTOP_TASK_NET, HOSTTOP_TASK_CPU, HOSTTOP_TASK_RSS,
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
-FLAG_AUTO_REGISTER = 1
+FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS = 1, 2
 TD_CAP = 256
 
 
@@ -226,6 +226,8 @@ def load_library(path=None):
         "gysk_merge_tdigest_slab": (i32, [vp, vp, vp]),
         "gysk_merge_finish": (i32, [vp, vp, u32]),
         "gysk_query_logical": (i32, [vp, vp, u32, vp]),
+        "gysk_export_logical_hist": (i32, [vp, u64, i32, vp, vp, vp]),
+        "gysk_merge_flush_range": (i32, [vp, vp, vp]),
         "gysk_query_flows_global": (i32, [vp, vp, u32, i32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
@@ -251,7 +253,8 @@ class Engine:
     """One engine = one GPU. Mirrors the C ABI one to one."""
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
-                 td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0):
+                 td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
+                 merge_levels=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -260,7 +263,7 @@ class Engine:
         cfg.max_batch = max_batch
         cfg.stage_batch = stage_batch
         cfg.idle_evict_secs = idle_evict_secs
-        cfg.flags = FLAG_AUTO_REGISTER if auto_register else 0
+        cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -585,6 +588,23 @@ class Engine:
         out = (SvcSummary * len(ids))()
         self._chk(self.L.gysk_query_logical(self.h, _p(ids), len(ids), out))
         return [o.asdict() for o in out]
+
+    def export_logical_hist(self, logical_id, which):
+        """gysk_export_logical_hist: (SERIAL_DTYPE[15], total, max) of a logical service from the last merge; None for an id
+        the map does not have"""
+        out = np.zeros(15, dtype=SERIAL_DTYPE)
+        total, mx = C.c_uint64(), C.c_int64()
+        rc = self.L.gysk_export_logical_hist(self.h, int(logical_id), which, _p(out), C.byref(total), C.byref(mx))
+        if rc == -2:
+            return None
+        self._chk(rc)
+        return out, total.value, mx.value
+
+    def merge_flush_range(self):
+        """gysk_merge_flush_range: (earliest, latest) tsec of the ranks' last flush, as the last merge all-reduced them"""
+        lo, hi = C.c_uint32(), C.c_uint32()
+        self._chk(self.L.gysk_merge_flush_range(self.h, C.byref(lo), C.byref(hi)))
+        return lo.value, hi.value
 
     def query_flows_global(self, keys, last_window=False):
         keys = np.ascontiguousarray(keys, dtype=np.uint64)

@@ -188,6 +188,9 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 #define GYSK_FLAG_AUTO_REGISTER		0x1u	/* unknown svc/task ids are inserted on first sight (device side);
 						   without it unknown ids are skipped like a failed
 						   listen_tbl_.lookup_single_elem_locked, gy_mconnhdlr.cc:11183 */
+#define GYSK_FLAG_MERGE_LEVELS		0x2u	/* the merge step also folds the 300-s / 5-day levels, active connections, errors
+						   and max rtt of the member services into each logical service (see
+						   gysk_query_logical); without it the merge arena and its collectives are as before */
 
 typedef struct gysk_config
 {
@@ -547,11 +550,28 @@ int		gysk_nccl_unique_id(uint8_t out[GYSK_NCCL_UNIQUE_ID_BYTES]);
 int		gysk_nccl_comm_init(gysk_engine *e, const uint8_t uid[GYSK_NCCL_UNIQUE_ID_BYTES], uint32_t nranks, uint32_t rank);
 int		gysk_merge_global(gysk_engine *e, void *nccl_comm);
 /* One gysk_svc_summary per logical id from the last finished merge: glob_id = the logical id, found = 0 for an id not in the map.
- * The merge folds the last closed window, the all-time histogram, the connection counters, the HLL registers and the t-digest,
- * and only those: nqrys_5min, nqrys_5day, nconns_active, active_kbytes, max_rtt_msec, cli_errors, ser_errors, curr_state,
- * curr_issue, issue_bit_hist and high_resp_bit_hist are always 0, and p95_5min_resp_ms, p99_5min_resp_ms and p95_5day_resp_ms
- * -1 (the percentiles of an empty histogram). */
+ * The merge always folds the last closed window, the all-time histogram, the connection counters, the HLL registers and the
+ * t-digest. curr_state, curr_issue, issue_bit_hist and high_resp_bit_hist are always 0: listener states are not merged.
+ * Without GYSK_FLAG_MERGE_LEVELS nqrys_5min, nqrys_5day, nconns_active, active_kbytes, max_rtt_msec, cli_errors and ser_errors
+ * are 0, and p95_5min_resp_ms, p99_5min_resp_ms and p95_5day_resp_ms -1 (the percentiles of an empty histogram).
+ * With it those fields are the member services' own, merged exactly at any GPU count:
+ *   nqrys_5min / nqrys_5day and the three level percentiles: the live ring slots of every member (the lvl its gysk_query_svcs row
+ *     shows) summed cell by cell over members and ranks, through the GY_HISTOGRAM percentile rule;
+ *   nconns_active, active_kbytes, cli_errors, ser_errors: sums over the members' last closed window, truncated to 32 bits;
+ *   max_rtt_msec: the largest of the members' values.
+ * A rank's levels are relative to its own last gysk_flush: see gysk_merge_flush_range. */
 int		gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_svc_summary *out);
+/* The merged histogram of one logical service from the last finished merge, with the contract of gysk_export_hist (HIST_SERIAL
+ * byte-compatible, for GY_HISTOGRAM::update_from_serialized): which = GYSK_HIST_RESP_LAST, _RESP_ALL, _RESP_5MIN or _RESP_5DAY.
+ * GYSK_ERR_NOENT for an id the map does not have, GYSK_ERR_NOTSUP for the two levels without GYSK_FLAG_MERGE_LEVELS,
+ * GYSK_ERR_INVAL before a finished merge or for another `which`. */
+int		gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS],
+				uint64_t *total_count, int64_t *max_val);
+/* The earliest and latest tsec of the ranks' last gysk_flush, as all-reduced by the last finished merge (GYSK_FLAG_MERGE_LEVELS;
+ * GYSK_ERR_NOTSUP without it, GYSK_ERR_INVAL before a finished merge). Each rank's level slots are relative to its own last
+ * flush, so *min_tsec != *max_tsec means the ranks had closed different windows and the merged levels mix them. That is not an
+ * error: the collectives cannot fail on one rank alone, so the caller decides what to do with such an answer. */
+int		gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tsec);
 int		gysk_query_flows_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_est *out);
 
 /* per-kernel device timing (CUDA events on the launching stream around the ingest kernel and around the sort +
