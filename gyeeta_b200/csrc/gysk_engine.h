@@ -87,10 +87,51 @@ struct HostTaskTopn
 	}
 };
 
+// one logical service's t-digest in the merge step: fixed size, so that the slabs all-gather as bytes
+struct SlabEntry { TdHead head; Centroid cent[TD_CAP]; };
+
+// The merged arrays of the nl logical services: the merge arena's per-logical arrays and the t-digest slabs, passed by value to the
+// merge kernels. lvl .. flush exist with GYSK_FLAG_MERGE_LEVELS only (nullptr without it).
+struct LogicalArrays
+{
+	uint32_t		nl {0};
+	HistCell		*last {nullptr}, *all {nullptr};	// SUM [nl][16]: last-window / all-time histograms, cells 0..14
+	unsigned long long	*conn {nullptr};			// SUM [nl][4]: last cnt, last kb, all cnt, all kb
+	HistCell		*lvl {nullptr};				// SUM [2][nl][16]: the live ring slots of the 300-s / 5-day levels, cells 0..14
+	unsigned long long	*aux {nullptr};				// SUM [nl][4]: active conns, active kbytes, client errors, server errors
+	long long		*hmax {nullptr};			// MAX [nl][2]: max_val_seen_ of last, all
+	long long		*lvl_max {nullptr};			// MAX [nl][2]: max_val_seen_ of the 300-s / 5-day levels
+	long long		*rtt {nullptr};				// MAX [nl]: the largest rtt_last bit pattern (a non-negative float's order)
+	long long		*flush {nullptr};			// MAX [2]: {last_flush_tsec, -last_flush_tsec} of this engine
+	uint8_t			*hll {nullptr};				// MAX [nl][1 << hll_p]
+	SlabEntry		*slab {nullptr};			// [nl] this engine's folded digests
+	SlabEntry		*final_slab {nullptr};			// [nl] merged over ranks
+
+	// histogram `which` (GYSK_HIST_RESP_LAST, _ALL, _5MIN or _5DAY) of logical service l: its cells 0..14 and its max_val_seen_
+	struct Hist { HistCell *cells; long long *max; };
+	__host__ __device__ __forceinline__ Hist hist(int which, uint32_t l) const
+	{
+		if (which == GYSK_HIST_RESP_LAST) return Hist {last + (size_t)l * HIST_CELLS, hmax + 2 * (size_t)l};
+		if (which == GYSK_HIST_RESP_ALL) return Hist {all + (size_t)l * HIST_CELLS, hmax + 2 * (size_t)l + 1};
+		const int k = which - GYSK_HIST_RESP_5MIN;
+		return Hist {lvl + ((size_t)k * nl + l) * HIST_CELLS, lvl_max + 2 * (size_t)l + k};
+	}
+	// cell c of that histogram as a row shows it: cell 15 holds max_val_seen_
+	__device__ __forceinline__ HistCell cell(int which, uint32_t l, int c) const
+	{
+		const Hist h = hist(which, l);
+		HistCell x = h.cells[c];
+		if (c == HIST_MAX_CELL) x.sum = *h.max;
+		return x;
+	}
+	__host__ __device__ __forceinline__ unsigned long long *conn_of(uint32_t l) const { return conn + 4 * (size_t)l; }
+	__host__ __device__ __forceinline__ unsigned long long *aux_of(uint32_t l) const { return aux + 4 * (size_t)l; }
+	__host__ __device__ __forceinline__ uint8_t *hll_of(uint32_t l, uint32_t hll_p) const { return hll + ((size_t)l << hll_p); }
+};
+
 // per-logical-service state of the merge step (SURVEY.md §8e)
 struct MergeState
 {
-	uint32_t		nlogical {0};
 	std::vector<uint64_t>	logical_ids;		// dense index -> logical id
 	std::unordered_map<uint64_t, uint32_t> index;	// logical id -> dense index
 	uint32_t		*d_offsets {nullptr}, *d_members {nullptr};	// CSR: logical -> member slots on this GPU
@@ -103,25 +144,12 @@ struct MergeState
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt, flush tsec]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
-	HistCell		*l_hist_last {nullptr}, *l_hist_all {nullptr};
-	unsigned long long	*l_conn {nullptr};			// [nl][4]: last cnt, last kb, all cnt, all kb
-	long long		*l_hmax {nullptr};			// [nl][2]: last, all
-	uint8_t			*l_hll {nullptr};
-	// GYSK_FLAG_MERGE_LEVELS only (nullptr without it): appended to the ends of the SUM and i64 MAX regions
-	HistCell		*l_lvl {nullptr};			// SUM [2][nl][16]: the live ring slots of the 300-s / 5-day levels, cells 0..14
-	unsigned long long	*l_aux {nullptr};			// SUM [nl][4]: active conns, active kbytes, client errors, server errors
-	long long		*l_lvl_max {nullptr};			// MAX [nl][2]: max_val_seen_ of the 300-s / 5-day levels
-	long long		*l_rtt {nullptr};			// MAX [nl]: the largest rtt_last bit pattern (a non-negative float's order)
-	long long		*l_flush {nullptr};			// MAX [2]: {last_flush_tsec, -last_flush_tsec} of this engine
-	// t-digest slab: fixed [nl] x {TdHead, Centroid[TD_CAP]}
-	uint8_t			*slab {nullptr};
-	size_t			slab_bytes {0};
-	uint8_t			*final_slab {nullptr};			// merged over ranks
+	LogicalArrays		lg;
 	bool			prepared {false}, finished {false};
 	void			*comm {nullptr};			// ncclComm_t of gysk_nccl_comm_init
 	uint32_t		comm_world {0};
 	bool			comm_owned {false};
-	uint8_t			*gathered {nullptr};			// [world] slabs, target of the all-gather
+	SlabEntry		*gathered {nullptr};			// [world] slabs, target of the all-gather
 	uint32_t		gathered_world {0};
 };
 
@@ -163,7 +191,7 @@ struct gysk_engine
 	std::vector<cudaEvent_t> prof_events;		// triples: before ingest, after the drain passes, after t-digest chain
 	size_t			prof_used {0};
 
-	// rolling levels: epoch held by each ring slot (~0 = never written) and the time of the last flush
+	// rolling levels: epoch held by each ring slot (~0 = never written; roll_levels) and the time of the last flush
 	uint64_t		ring_epoch[gysk::NLEVELS][gysk::NSLOTS];
 	uint32_t		last_flush_tsec {0};
 
@@ -201,8 +229,6 @@ int sync_locked(gysk_engine *e);
 void merge_release(gysk_engine *e);
 // HIST_SERIAL of 16 cells (cell HIST_MAX_CELL holds max_val_seen_ in .sum); total = the sum of the first nb counts
 void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint64_t *total, int64_t *maxv, bool t_is_int);
-// ring slots of rolling level l (0: 300 s, 1: 5 days) still inside the level's span at the last flush
-uint32_t live_mask(const gysk_engine *e, int l);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)
@@ -244,6 +270,16 @@ int dalloc(gysk_engine *e, T **p, size_t n, bool zero = true)
 	}
 	*p = static_cast<T *>(q);
 	return 0;
+}
+
+// frees a buffer of dalloc (nullptr: nothing to free) and clears the pointer
+template <typename T>
+void dfree(gysk_engine *e, T *&p)
+{
+	if (!p) return;
+	cudaFree(p);
+	e->dallocs.erase(std::remove(e->dallocs.begin(), e->dallocs.end(), (void *)p), e->dallocs.end());
+	p = nullptr;
 }
 
 template <typename T>

@@ -1289,7 +1289,7 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 // (300 s, common/gy_socket_stat.h:997) once it is older than twice that (common/gy_socket_stat.cc:3968-3982: tclock != 0,
 // tclock + 300 s < now, tstart + 600 s < now) and tells madhava with LISTEN_FLAG_DELETE (:4023-4033). Here the flush records,
 // per slot, the first flush that saw it and the last window that held events, and lists the slots that meet the rule.
-__global__ void flush_kernel(DevState st, uint32_t nslots, HistCell *__restrict__ ring0, HistCell *__restrict__ ring1, uint32_t tsec, uint32_t idle_secs)
+__global__ void flush_kernel(DevState st, uint32_t nslots, uint32_t tsec, uint32_t idle_secs)
 {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	const bool valid = i < (uint64_t)nslots * HIST_CELLS;		// nslots * 16: whole half-warps are valid or not
@@ -1313,13 +1313,14 @@ __global__ void flush_kernel(DevState st, uint32_t nslots, HistCell *__restrict_
 	st.hist_last[i] = c;
 	// rolling levels: the window is added to the current slot of each level (cleared by the host when its epoch changed).
 	// A cleared slot's max cell reads 0, which is below any recorded response time or equal to it: harmless for max().
+	HistCell &r0 = st.levels.row(0, st.levels.cur[0], slot)[cell], &r1 = st.levels.row(1, st.levels.cur[1], slot)[cell];
 	if (cell == HIST_MAX_CELL) {
-		if (c.sum > ring0[i].sum) ring0[i].sum = c.sum;
-		if (c.sum > ring1[i].sum) ring1[i].sum = c.sum;
+		if (c.sum > r0.sum) r0.sum = c.sum;
+		if (c.sum > r1.sum) r1.sum = c.sum;
 	}
 	else {
-		ring0[i].count += c.count; ring0[i].sum += c.sum;
-		ring1[i].count += c.count; ring1[i].sum += c.sum;
+		r0.count += c.count; r0.sum += c.sum;
+		r1.count += c.count; r1.sum += c.sum;
 	}
 	if (cell == HIST_MAX_CELL) {
 		if (c.sum > st.hist_all[i].sum) st.hist_all[i].sum = c.sum;
@@ -1391,7 +1392,7 @@ __device__ __forceinline__ QpsActPct qps_act_pct(const HistCell *q, const HistCe
 	return r;
 }
 
-__global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots, uint32_t tsec, uint32_t live0, uint32_t live1)
+__global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots, uint32_t tsec)
 {
 	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
 	if (slot >= nslots || !st.slot_id[slot]) return;
@@ -1408,14 +1409,12 @@ __global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots
 	const LevelStat s5 = level_stat(cnt, sum);
 	LevelStat lv[NLEVELS];
 	for (int l = 0; l < NLEVELS; ++l) {
-		const uint32_t live = l ? live1 : live0;
 		for (int b = 0; b < HIST_MAX_CELL; ++b) cnt[b] = 0;
 		sum = 0;
-		for (int k = 0; k < NSLOTS; ++k) {
-			if (!((live >> k) & 1u)) continue;
-			const HistCell *ring = st.hist_ring + (((size_t)l * NSLOTS + k) * nslots + slot) * HIST_CELLS;
+		// LevelRing::cell's sums, a ring row at a time: each thread reads its rows front to back
+		st.levels.each_live(l, slot, [&](const HistCell *ring) {
 			for (int b = 0; b < HIST_MAX_CELL; ++b) { const HistCell c = ring[b]; cnt[b] += c.count; sum += (uint64_t)c.sum; }
-		}
+		});
 		lv[l] = level_stat(cnt, sum);
 	}
 	sum = 0;
@@ -1465,7 +1464,7 @@ __global__ void __launch_bounds__(128) state_kernel(DevState st, uint32_t nslots
 // with state_kernel's helpers. The int64 values go into the uint32 fields by plain conversion, as the reference's assignments do.
 static constexpr int DAY_WARPS = 4;
 __global__ void __launch_bounds__(DAY_WARPS * 32) day_stats_kernel(DevState st, const unsigned long long *__restrict__ slots, uint32_t n,
-		uint32_t max_svcs, uint32_t live1, gysk_listener_day_stats *__restrict__ out)
+		gysk_listener_day_stats *__restrict__ out)
 {
 	__shared__ HistCell lvl[DAY_WARPS][HIST_CELLS], qa[DAY_WARPS][2][HIST_CELLS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -1474,13 +1473,7 @@ __global__ void __launch_bounds__(DAY_WARPS * 32) day_stats_kernel(DevState st, 
 	if (q >= n) return;
 	const uint32_t slot = (uint32_t)slots[q];
 	if (lane < HIST_CELLS) {
-		HistCell a {0, 0};
-		for (int k = 0; k < NSLOTS; ++k) {
-			if (!((live1 >> k) & 1u)) continue;
-			const HistCell x = st.hist_ring[(((size_t)NSLOTS + k) * max_svcs + slot) * HIST_CELLS + lane];
-			a.count += x.count; a.sum += x.sum;
-		}
-		lvl[wid][lane] = a;
+		if (lane < HIST_MAX_CELL) lvl[wid][lane] = st.levels.cell(1, slot, lane);		// level_stat reads cells 0..14 only
 		qa[wid][0][lane] = st.qps_hist[(size_t)slot * HIST_CELLS + lane];
 		qa[wid][1][lane] = st.act_hist[(size_t)slot * HIST_CELLS + lane];
 	}
@@ -1501,7 +1494,7 @@ __global__ void __launch_bounds__(DAY_WARPS * 32) day_stats_kernel(DevState st, 
 
 // one CTA per evicted slot (grid-stride): the id's table entry becomes a tombstone, every per-slot array returns to its
 // just-created state and the slot number goes on the free stack for the next unknown id
-__global__ void __launch_bounds__(256) evict_kernel(DevState st, uint32_t max_svcs)
+__global__ void __launch_bounds__(256) evict_kernel(DevState st)
 {
 	const uint32_t nev = (uint32_t)st.counters[CTR_NEVICT];
 
@@ -1533,7 +1526,8 @@ __global__ void __launch_bounds__(256) evict_kernel(DevState st, uint32_t max_sv
 			st.bm_cur[c] = 0; st.bm_last[c] = 0;
 			const HistCell zi {0, threadIdx.x == HIST_MAX_CELL ? (long long)INT_MIN : 0};
 			st.qps_hist[c] = zi; st.act_hist[c] = zi;
-			for (int pl = 0; pl < NLEVELS * NSLOTS; ++pl) st.hist_ring[((size_t)pl * max_svcs + slot) * HIST_CELLS + threadIdx.x] = HistCell {0, 0};
+			for (int l = 0; l < NLEVELS; ++l)
+				for (int k = 0; k < NSLOTS; ++k) st.levels.row(l, k, slot)[threadIdx.x] = HistCell {0, 0};
 		}
 		uint32_t *hw = reinterpret_cast<uint32_t *>(st.hll + ((size_t)slot << st.hll_p));
 		for (uint32_t w = threadIdx.x; w < (1u << st.hll_p) / 4u; w += blockDim.x) hw[w] = 0;
@@ -1578,26 +1572,14 @@ __device__ __forceinline__ Resolved resolve_warp(const IdTable &t, const unsigne
 }
 
 // the warp's copy of one slot's state (all but id / found / slot and the HLL register histogram)
-__device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32_t max_svcs, uint32_t live0, uint32_t live1, SvcRaw &o, int lane)
+__device__ __forceinline__ void gather_slot(const DevState &st, int slot, SvcRaw &o, int lane)
 {
 	if (lane < HIST_CELLS) {
 		o.cur[lane] = st.hist_cur[(size_t)slot * HIST_CELLS + lane];
 		o.last[lane] = st.hist_last[(size_t)slot * HIST_CELLS + lane];
 		o.all[lane] = st.hist_all[(size_t)slot * HIST_CELLS + lane];
 		o.bm_cur[lane] = st.bm_cur[(size_t)slot * HIST_CELLS + lane]; o.bm_last[lane] = st.bm_last[(size_t)slot * HIST_CELLS + lane];
-		// rolling levels: sum of the slots still inside the level's span
-		for (int l = 0; l < NLEVELS; ++l) {
-			const uint32_t live = l ? live1 : live0;
-			HistCell a {0, 0};
-			if (lane == HIST_MAX_CELL) a.sum = LLONG_MIN;
-			for (int k = 0; k < NSLOTS; ++k) {
-				if (!((live >> k) & 1u)) continue;
-				const HistCell x = st.hist_ring[(((size_t)l * NSLOTS + k) * max_svcs + slot) * HIST_CELLS + lane];
-				if (lane == HIST_MAX_CELL) a.sum = max(a.sum, x.sum);
-				else { a.count += x.count; a.sum += x.sum; }
-			}
-			o.lvl[l][lane] = a;
-		}
+		for (int l = 0; l < NLEVELS; ++l) o.lvl[l][lane] = st.levels.cell(l, slot, lane);
 	}
 	if (lane == 0) {
 		o.conn_cur = st.conn_cur[slot]; o.conn_last = st.conn_last[slot];
@@ -1611,8 +1593,7 @@ __device__ __forceinline__ void gather_slot(const DevState &st, int slot, uint32
 }
 
 // the single-id exports (gysk_export_hist / _conn_bitmap / _tdigest): the raw state of the id
-__global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, uint32_t max_svcs,
-		uint32_t live0, uint32_t live1, SvcRaw *__restrict__ out)
+__global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const unsigned long long *__restrict__ ids, uint32_t n, SvcRaw *__restrict__ out)
 {
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 	const uint32_t q = blockIdx.x * 4 + wid;
@@ -1622,7 +1603,7 @@ __global__ void __launch_bounds__(128) gather_svcs_kernel(DevState st, const uns
 	const Resolved r = resolve_warp(st.svc_tbl, ids, nullptr, q, lane);
 	if (lane == 0) { o.id = r.id; o.found = r.slot >= 0; o.slot = (uint32_t)r.slot; }
 	if (r.slot < 0) return;
-	gather_slot(st, r.slot, max_svcs, live0, live1, o, lane);
+	gather_slot(st, r.slot, o, lane);
 }
 
 // ---- window reads (gysk_query_window / gysk_query_task_window) ----
@@ -1739,8 +1720,7 @@ __global__ void __launch_bounds__(1024) host_listen_rows_kernel(const unsigned l
 // slot's state goes into shared memory, then summarize_warp makes the row.
 static constexpr int SUMM_WARPS = 4;
 __global__ void __launch_bounds__(SUMM_WARPS * 32) svc_summary_kernel(DevState st, const unsigned long long *__restrict__ ids,
-		const unsigned long long *__restrict__ slots, uint32_t n, uint32_t max_svcs, uint32_t live0, uint32_t live1,
-		gysk_svc_summary *__restrict__ out)
+		const unsigned long long *__restrict__ slots, uint32_t n, gysk_svc_summary *__restrict__ out)
 {
 	__shared__ SvcRaw raw[SUMM_WARPS];
 	__shared__ unsigned long long summ[SUMM_WARPS][sizeof(gysk_svc_summary) / 8];
@@ -1752,7 +1732,7 @@ __global__ void __launch_bounds__(SUMM_WARPS * 32) svc_summary_kernel(DevState s
 	const Resolved s = resolve_warp(st.svc_tbl, ids, slots, q, lane);
 	if (lane == 0) { r.id = s.id; r.found = s.slot >= 0; r.slot = (uint32_t)s.slot; }
 	if (s.slot >= 0) {
-		gather_slot(st, s.slot, max_svcs, live0, live1, r, lane);
+		gather_slot(st, s.slot, r, lane);
 		hll_hist_warp(st.hll + ((size_t)s.slot << st.hll_p), st.hll_p, r.hll_hist, lane);
 	}
 	summarize_warp(r, s.id, st.hll_p, summ[wid], out + q, lane);
@@ -2155,15 +2135,14 @@ int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s)
 	return 1;
 }
 
-int launch_flush(const DevState &st, uint32_t nslots, HistCell *ring_plane0, HistCell *ring_plane1, uint32_t tsec, uint32_t idle_secs,
-		uint32_t live_mask0, uint32_t live_mask1, cudaStream_t s)
+int launch_flush(const DevState &st, uint32_t nslots, uint32_t tsec, uint32_t idle_secs, cudaStream_t s)
 {
 	if (!nslots) return 0;
 	cudaMemsetAsync(st.counters + CTR_NEVICT, 0, sizeof(unsigned long long), s);
-	flush_kernel<<<div_up((uint64_t)nslots * HIST_CELLS, 256), 256, 0, s>>>(st, nslots, ring_plane0, ring_plane1, tsec, idle_secs);
-	state_kernel<<<div_up(nslots, 128), 128, 0, s>>>(st, nslots, tsec, live_mask0, live_mask1);
+	flush_kernel<<<div_up((uint64_t)nslots * HIST_CELLS, 256), 256, 0, s>>>(st, nslots, tsec, idle_secs);
+	state_kernel<<<div_up(nslots, 128), 128, 0, s>>>(st, nslots, tsec);
 	if (!idle_secs) return 2;
-	evict_kernel<<<296, 256, 0, s>>>(st, nslots);		// grid-stride over the (device-side) eviction list
+	evict_kernel<<<296, 256, 0, s>>>(st);		// grid-stride over the (device-side) eviction list
 	return 3;
 }
 
@@ -2174,11 +2153,10 @@ int launch_rebuild_table(const DevState &st, uint32_t max_svcs, cudaStream_t s)
 	return 1;
 }
 
-int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint32_t n, uint32_t max_svcs, uint32_t live_mask0, uint32_t live_mask1,
-		SvcRaw *d_out, cudaStream_t s)
+int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint32_t n, SvcRaw *d_out, cudaStream_t s)
 {
 	if (!n) return 0;
-	gather_svcs_kernel<<<div_up(n, 4), 128, 0, s>>>(st, d_ids, n, max_svcs, live_mask0, live_mask1, d_out);
+	gather_svcs_kernel<<<div_up(n, 4), 128, 0, s>>>(st, d_ids, n, d_out);
 	return 1;
 }
 
@@ -2219,11 +2197,11 @@ int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots,
 	return 2 + sorted;
 }
 
-int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs,
-		uint32_t live_mask0, uint32_t live_mask1, gysk_svc_summary *d_out, cudaStream_t s)
+int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, gysk_svc_summary *d_out,
+		cudaStream_t s)
 {
 	if (!n) return 0;
-	svc_summary_kernel<<<div_up(n, SUMM_WARPS), SUMM_WARPS * 32, 0, s>>>(st, d_ids, d_slots, n, max_svcs, live_mask0, live_mask1, d_out);
+	svc_summary_kernel<<<div_up(n, SUMM_WARPS), SUMM_WARPS * 32, 0, s>>>(st, d_ids, d_slots, n, d_out);
 	return 1;
 }
 
@@ -2235,11 +2213,10 @@ int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, c
 	return 1;
 }
 
-int launch_day_stats(const DevState &st, const unsigned long long *d_slots, uint32_t n, uint32_t max_svcs, uint32_t live_mask1,
-		gysk_listener_day_stats *d_out, cudaStream_t s)
+int launch_day_stats(const DevState &st, const unsigned long long *d_slots, uint32_t n, gysk_listener_day_stats *d_out, cudaStream_t s)
 {
 	if (!n) return 0;
-	day_stats_kernel<<<div_up(n, DAY_WARPS), DAY_WARPS * 32, 0, s>>>(st, d_slots, n, max_svcs, live_mask1, d_out);
+	day_stats_kernel<<<div_up(n, DAY_WARPS), DAY_WARPS * 32, 0, s>>>(st, d_slots, n, d_out);
 	return 1;
 }
 

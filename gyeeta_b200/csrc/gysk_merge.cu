@@ -29,8 +29,6 @@ using namespace gysk;
 
 namespace gysk {
 
-struct SlabEntry { TdHead head; Centroid cent[TD_CAP]; };
-
 // The map keeps every {glob_id, logical} pair it was given; which of them live on this GPU, and in which slot, is looked up at
 // every merge: a service that registers after gysk_set_logical_map takes part from its first window on, one that was evicted (or whose
 // slot now belongs to another id) drops out. An id without a slot maps to the engine's null slot (index max_svcs: always in its
@@ -45,14 +43,15 @@ __global__ void resolve_members_kernel(DevState st, const unsigned long long *__
 }
 
 // one thread per (logical, cell)
-__global__ void fold_hist_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t nl, uint32_t null_slot,
-		HistCell *__restrict__ l_last, HistCell *__restrict__ l_all, unsigned long long *__restrict__ l_conn, long long *__restrict__ l_hmax)
+__global__ void fold_hist_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t null_slot,
+		LogicalArrays lg)
 {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= (uint64_t)nl * HIST_CELLS) return;
+	if (i >= (uint64_t)lg.nl * HIST_CELLS) return;
 	const uint32_t l = (uint32_t)(i >> 4);
 	const int cell = (int)(i & 15);
 	const uint32_t b = offs[l], e = offs[l + 1];
+	const LogicalArrays::Hist hl = lg.hist(GYSK_HIST_RESP_LAST, l), ha = lg.hist(GYSK_HIST_RESP_ALL, l);
 
 	if (cell < HIST_MAX_CELL) {
 		HistCell a {0, 0}, c {0, 0};
@@ -61,7 +60,7 @@ __global__ void fold_hist_kernel(DevState st, const uint32_t *__restrict__ offs,
 			const HistCell x = st.hist_last[(size_t)members[m] * HIST_CELLS + cell], y = st.hist_all[(size_t)members[m] * HIST_CELLS + cell];
 			a.count += x.count; a.sum += x.sum; c.count += y.count; c.sum += y.sum;
 		}
-		l_last[i] = a; l_all[i] = c;
+		hl.cells[cell] = a; ha.cells[cell] = c;
 	}
 	else {
 		long long ml = LLONG_MIN, ma = LLONG_MIN;
@@ -74,30 +73,26 @@ __global__ void fold_hist_kernel(DevState st, const uint32_t *__restrict__ offs,
 			const unsigned long long cl = st.conn_last[s];
 			lc += (uint32_t)cl; lk += cl >> 32; ac += st.conn_all_cnt[s]; ak += st.conn_all_kb[s];
 		}
-		l_last[i] = HistCell {0, 0}; l_all[i] = HistCell {0, 0};
-		l_hmax[2 * l] = ml; l_hmax[2 * l + 1] = ma;
-		l_conn[4 * l] = lc; l_conn[4 * l + 1] = lk; l_conn[4 * l + 2] = ac; l_conn[4 * l + 3] = ak;
+		hl.cells[cell] = HistCell {0, 0}; ha.cells[cell] = HistCell {0, 0};
+		*hl.max = ml; *ha.max = ma;
+		unsigned long long *cn = lg.conn_of(l);
+		cn[0] = lc; cn[1] = lk; cn[2] = ac; cn[3] = ak;
 	}
 }
 
-// GYSK_FLAG_MERGE_LEVELS, one thread per (logical, cell): cells 0..14 sum the live ring slots of both rolling levels over the members
-// (live0 / live1: the masks gather_slot applies, so a member adds exactly the lvl[] of its own gysk_query_svcs row); the cell-15
-// thread takes the level maxima, the aux words of the last closed window and the largest rtt. Thread 0 also writes this engine's
-// {last flush tsec, -last flush tsec}, whose i64 max over the ranks gives their latest and earliest flush.
-__global__ void fold_levels_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t nl, uint32_t null_slot,
-		uint32_t live0, uint32_t live1, long long flush_tsec, HistCell *__restrict__ l_lvl, unsigned long long *__restrict__ l_aux,
-		long long *__restrict__ l_lvl_max, long long *__restrict__ l_rtt, long long *__restrict__ l_flush)
+// GYSK_FLAG_MERGE_LEVELS, one thread per (logical, cell): cells 0..14 sum the members' level cells (st.levels.cell, what a member's
+// own gysk_query_svcs row holds in lvl[]); the cell-15 thread takes the level maxima, the aux words of the last closed window and the
+// largest rtt. Thread 0 also writes this engine's {last flush tsec, -last flush tsec}, whose i64 max over the ranks gives their
+// latest and earliest flush. It streams the ring: 8 CTAs per SM (32 registers) keep enough loads in flight.
+__global__ void __launch_bounds__(256, 8) fold_levels_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t null_slot,
+		long long flush_tsec, LogicalArrays lg)
 {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (i == 0) { l_flush[0] = flush_tsec; l_flush[1] = -flush_tsec; }
-	if (i >= (uint64_t)nl * HIST_CELLS) return;
+	if (i == 0) { lg.flush[0] = flush_tsec; lg.flush[1] = -flush_tsec; }
+	if (i >= (uint64_t)lg.nl * HIST_CELLS) return;
 	const uint32_t l = (uint32_t)(i >> 4);
 	const int cell = (int)(i & 15);
 	const uint32_t b = offs[l], e = offs[l + 1];
-	const size_t max_svcs = null_slot;		// the null slot is the index past the last one: the ring planes hold max_svcs slots
-	auto ring = [&](int lv, int k, uint32_t s) -> const HistCell & {
-		return st.hist_ring[(((size_t)lv * NSLOTS + k) * max_svcs + s) * HIST_CELLS + cell];
-	};
 
 	if (cell < HIST_MAX_CELL) {
 		HistCell a[NLEVELS] {};
@@ -106,16 +101,11 @@ __global__ void fold_levels_kernel(DevState st, const uint32_t *__restrict__ off
 			if (s == null_slot) continue;
 #pragma unroll
 			for (int lv = 0; lv < NLEVELS; ++lv) {
-				const uint32_t live = lv ? live1 : live0;
-#pragma unroll
-				for (int k = 0; k < NSLOTS; ++k) {
-					if (!((live >> k) & 1u)) continue;
-					const HistCell x = ring(lv, k, s);
-					a[lv].count += x.count; a[lv].sum += x.sum;
-				}
+				const HistCell x = st.levels.cell(lv, s, cell);
+				a[lv].count += x.count; a[lv].sum += x.sum;
 			}
 		}
-		for (int lv = 0; lv < NLEVELS; ++lv) l_lvl[((size_t)lv * nl + l) * HIST_CELLS + cell] = a[lv];
+		for (int lv = 0; lv < NLEVELS; ++lv) lg.hist(GYSK_HIST_RESP_5MIN + lv, l).cells[cell] = a[lv];
 	}
 	else {
 		long long mx[NLEVELS] = {LLONG_MIN, LLONG_MIN};
@@ -124,27 +114,28 @@ __global__ void fold_levels_kernel(DevState st, const uint32_t *__restrict__ off
 		for (uint32_t m = b; m < e; ++m) {
 			const uint32_t s = members[m];
 			if (s == null_slot) continue;
-			for (int lv = 0; lv < NLEVELS; ++lv) {
-				const uint32_t live = lv ? live1 : live0;
-				for (int k = 0; k < NSLOTS; ++k) if ((live >> k) & 1u) mx[lv] = max(mx[lv], ring(lv, k, s).sum);
-			}
+			for (int lv = 0; lv < NLEVELS; ++lv) mx[lv] = max(mx[lv], st.levels.cell(lv, s, HIST_MAX_CELL).sum);
 			const SlotAux x = st.slot_aux[s];
 			ac += (uint32_t)x.act_last; ak += x.act_last >> 32; ce += (uint32_t)x.err_last; se += x.err_last >> 32;
 			rtt = max(rtt, x.rtt_last);
 		}
-		for (int lv = 0; lv < NLEVELS; ++lv) { l_lvl[((size_t)lv * nl + l) * HIST_CELLS + cell] = HistCell {0, 0}; l_lvl_max[2 * l + lv] = mx[lv]; }
-		l_aux[4 * l] = ac; l_aux[4 * l + 1] = ak; l_aux[4 * l + 2] = ce; l_aux[4 * l + 3] = se;
-		l_rtt[l] = rtt;
+		for (int lv = 0; lv < NLEVELS; ++lv) {
+			const LogicalArrays::Hist h = lg.hist(GYSK_HIST_RESP_5MIN + lv, l);
+			h.cells[cell] = HistCell {0, 0}; *h.max = mx[lv];
+		}
+		unsigned long long *a = lg.aux_of(l);
+		a[0] = ac; a[1] = ak; a[2] = ce; a[3] = se;
+		lg.rtt[l] = rtt;
 	}
 }
 
 // one thread per (logical, 4 registers): per-byte max over the member services
-__global__ void fold_hll_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t nl, uint32_t null_slot,
-		uint32_t *__restrict__ l_hll)
+__global__ void fold_hll_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t null_slot,
+		LogicalArrays lg)
 {
 	const uint32_t words = 1u << (st.hll_p - 2);
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= (uint64_t)nl * words) return;
+	if (i >= (uint64_t)lg.nl * words) return;
 	const uint32_t l = (uint32_t)(i / words), w = (uint32_t)(i % words);
 	uint32_t acc = 0;
 
@@ -152,74 +143,66 @@ __global__ void fold_hll_kernel(DevState st, const uint32_t *__restrict__ offs, 
 		if (members[m] == null_slot) continue;
 		acc = __vmaxu4(acc, reinterpret_cast<const uint32_t *>(st.hll + ((size_t)members[m] << st.hll_p))[w]);
 	}
-	l_hll[i] = acc;
+	reinterpret_cast<uint32_t *>(lg.hll_of(l, st.hll_p))[w] = acc;
 }
 
 static constexpr int MG_WARPS = 2;		// 2 x 17.8 KB of scratch: static shared memory
 
-// one warp per logical service: fold member digests one after the other (member order = the order of the map call's list)
+// One warp folds the digests digest(b) .. digest(e - 1) into out, one after the other: each non-empty one is merged into the
+// accumulator and compressed (warp_merge_compress), its total, min and max added. digest(i) gives {head, centroids}, head nullptr
+// for an entry to skip.
+struct DigestRef { const TdHead *head; const Centroid *cent; };
+template <typename Digest>
+__device__ __forceinline__ void fold_digests(TdScratch &S, const TdParams &P, uint32_t b, uint32_t e, Digest digest, SlabEntry &out, int lane)
+{
+	uint32_t nacc = 0;
+	unsigned long long total = 0;
+	double mn = INFINITY, mx = -INFINITY;
+
+	for (uint32_t i = b; i < e; ++i) {
+		const DigestRef d = digest(i);
+		if (!d.head || !d.head->n) continue;
+		nacc = warp_merge_compress(S, S.newc, nacc, d.cent, d.head->n, S.newc, P);
+		total += d.head->total; mn = fmin(mn, d.head->minv); mx = fmax(mx, d.head->maxv);
+	}
+	for (uint32_t c = lane; c < TD_CAP; c += 32) out.cent[c] = c < nacc ? S.newc[c] : Centroid {0.0, 0};
+	if (lane == 0) { TdHead h; h.total = total; h.minv = mn; h.maxv = mx; h.n = nacc; h.pad = 0; out.head = h; }
+	__syncwarp();
+}
+
+// one warp per logical service: its members' digests in map order
 __global__ void __launch_bounds__(MG_WARPS * 32) fold_td_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members,
-		uint32_t nl, uint32_t null_slot, SlabEntry *__restrict__ slab)
+		uint32_t null_slot, LogicalArrays lg)
 {
 	__shared__ TdScratch scratch[MG_WARPS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	TdScratch &S = scratch[wid];
 
-	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < nl; l += gridDim.x * MG_WARPS) {
-		uint32_t nacc = 0;
-		unsigned long long total = 0;
-		double mn = INFINITY, mx = -INFINITY;
-
-		for (uint32_t m = offs[l]; m < offs[l + 1]; ++m) {
+	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS)
+		fold_digests(scratch[wid], st.td, offs[l], offs[l + 1], [&](uint32_t m) {
 			const uint32_t s = members[m];
-			if (s == null_slot) continue;
-			const TdHead h = st.td_head[s];
-			if (!h.n) continue;
-			nacc = warp_merge_compress(S, S.newc, nacc, st.td_cent + (size_t)s * TD_CAP, h.n, S.newc, st.td);
-			total += h.total; mn = fmin(mn, h.minv); mx = fmax(mx, h.maxv);
-		}
-		for (uint32_t c = lane; c < TD_CAP; c += 32) slab[l].cent[c] = c < nacc ? S.newc[c] : Centroid {0.0, 0};
-		if (lane == 0) { TdHead h; h.total = total; h.minv = mn; h.maxv = mx; h.n = nacc; h.pad = 0; slab[l].head = h; }
-		__syncwarp();
-	}
+			return s == null_slot ? DigestRef {nullptr, nullptr} : DigestRef {st.td_head + s, st.td_cent + (size_t)s * TD_CAP};
+		}, lg.slab[l], lane);
 }
 
-// one warp per logical service over the all-gathered slabs [world][nl]
-__global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, uint32_t nl,
-		SlabEntry *__restrict__ out, TdParams P)
+// one warp per logical service over the all-gathered slabs [world][nl], in rank-ascending order => deterministic result
+__global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, LogicalArrays lg, TdParams P)
 {
 	__shared__ TdScratch scratch[MG_WARPS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	TdScratch &S = scratch[wid];
 
-	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < nl; l += gridDim.x * MG_WARPS) {
-		uint32_t nacc = 0;
-		unsigned long long total = 0;
-		double mn = INFINITY, mx = -INFINITY;
-
-		for (uint32_t r = 0; r < world; ++r) {			// fixed rank-ascending order => deterministic result
-			const SlabEntry &e = gathered[(size_t)r * nl + l];
-			if (!e.head.n) continue;
-			nacc = warp_merge_compress(S, S.newc, nacc, e.cent, e.head.n, S.newc, P);
-			total += e.head.total; mn = fmin(mn, e.head.minv); mx = fmax(mx, e.head.maxv);
-		}
-		for (uint32_t c = lane; c < TD_CAP; c += 32) out[l].cent[c] = c < nacc ? S.newc[c] : Centroid {0.0, 0};
-		if (lane == 0) { TdHead h; h.total = total; h.minv = mn; h.maxv = mx; h.n = nacc; h.pad = 0; out[l].head = h; }
-		__syncwarp();
-	}
+	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS)
+		fold_digests(scratch[wid], P, 0, world, [&](uint32_t r) {
+			const SlabEntry &g = gathered[(size_t)r * lg.nl + l];
+			return DigestRef {&g.head, g.cent};
+		}, lg.final_slab[l], lane);
 }
-
-// the merged rolling levels and aux words (GYSK_FLAG_MERGE_LEVELS; lvl == nullptr without it)
-struct LevelArrays { const HistCell *lvl; const unsigned long long *aux; const long long *lvl_max, *rtt; uint32_t nl; };
 
 // read side: one warp per logical service, its merged arrays into a shared-memory SvcRaw, then the row of summarize_warp (the
 // summary of gysk_query_svcs). The merge folds neither the current window, the connection bitmaps nor the per-slot state / qps /
-// active-connection words: they are zero; so are the rolling levels and the aux words unless the engine merges them (lv.lvl).
+// active-connection words: they are zero; so are the rolling levels and the aux words unless the engine merges them (lg.lvl).
 // glob_id is left 0 for the host to fill in.
 static constexpr int LG_WARPS = 4;
-__global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const int32_t *__restrict__ lidx, uint32_t n, uint32_t hll_p,
-		const HistCell *__restrict__ l_last, const HistCell *__restrict__ l_all, const unsigned long long *__restrict__ l_conn,
-		const long long *__restrict__ l_hmax, const uint8_t *__restrict__ l_hll, const SlabEntry *__restrict__ slab, LevelArrays lv,
+__global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const int32_t *__restrict__ lidx, uint32_t n, uint32_t hll_p, LogicalArrays lg,
 		gysk_svc_summary *__restrict__ out)
 {
 	__shared__ SvcRaw raw[LG_WARPS];
@@ -233,36 +216,29 @@ __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const in
 	if (lane == 0) { r.id = 0; r.found = l >= 0; r.slot = (uint32_t)l; }
 	if (l >= 0) {
 		if (lane < HIST_CELLS) {
-			HistCell a = l_last[(size_t)l * HIST_CELLS + lane], b = l_all[(size_t)l * HIST_CELLS + lane];
-			if (lane == HIST_MAX_CELL) { a.sum = l_hmax[2 * l]; b.sum = l_hmax[2 * l + 1]; }
-			r.last[lane] = a; r.all[lane] = b; r.cur[lane] = HistCell {0, 0};
-			for (int k = 0; k < NLEVELS; ++k) {
-				HistCell c {0, 0};
-				if (lv.lvl) {
-					c = lv.lvl[((size_t)k * lv.nl + l) * HIST_CELLS + lane];
-					if (lane == HIST_MAX_CELL) c.sum = lv.lvl_max[2 * l + k];
-				}
-				r.lvl[k][lane] = c;
-			}
+			r.last[lane] = lg.cell(GYSK_HIST_RESP_LAST, l, lane); r.all[lane] = lg.cell(GYSK_HIST_RESP_ALL, l, lane);
+			r.cur[lane] = HistCell {0, 0};
+			for (int k = 0; k < NLEVELS; ++k) r.lvl[k][lane] = lg.lvl ? lg.cell(GYSK_HIST_RESP_5MIN + k, l, lane) : HistCell {0, 0};
 			r.bm_cur[lane] = 0; r.bm_last[lane] = 0;
 			r.qps[lane] = HistCell {0, 0}; r.act[lane] = HistCell {0, 0};
 		}
 		if (lane == 0) {
+			const unsigned long long *cn = lg.conn_of(l);
 			r.conn_cur = 0;
-			r.conn_last = (l_conn[4 * l] & 0xFFFFFFFFull) | (l_conn[4 * l + 1] << 32);
-			r.conn_all_cnt = l_conn[4 * l + 2]; r.conn_all_kb = l_conn[4 * l + 3];
-			r.td = slab[l].head;
+			r.conn_last = (cn[0] & 0xFFFFFFFFull) | (cn[1] << 32);
+			r.conn_all_cnt = cn[2]; r.conn_all_kb = cn[3];
+			r.td = lg.final_slab[l].head;
 			r.aux = SlotAux {0, 0, 0, 0, 0, 0};
-			if (lv.lvl) {
-				const unsigned long long *a = lv.aux + 4 * (size_t)l;
+			if (lg.lvl) {
+				const unsigned long long *a = lg.aux_of(l);
 				r.aux.act_last = (a[0] & 0xFFFFFFFFull) | (a[1] << 32);
 				r.aux.err_last = (a[2] & 0xFFFFFFFFull) | (a[3] << 32);
-				r.aux.rtt_last = (uint32_t)lv.rtt[l];
+				r.aux.rtt_last = (uint32_t)lg.rtt[l];
 			}
 			r.sst = SlotState {0, 0, 0, 0, 0};
 		}
-		for (int i = lane; i < TD_CAP; i += 32) r.cent[i] = slab[l].cent[i];
-		hll_hist_warp(l_hll + ((size_t)l << hll_p), hll_p, r.hll_hist, lane);
+		for (int i = lane; i < TD_CAP; i += 32) r.cent[i] = lg.final_slab[l].cent[i];
+		hll_hist_warp(lg.hll_of(l, hll_p), hll_p, r.hll_hist, lane);
 	}
 	summarize_warp(r, 0, hll_p, summ[wid], out + q, lane);
 }
@@ -374,62 +350,45 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	}
 
 	// (re)allocate the arena
-	auto dfree = [&](void *p) { if (p) { cudaFree(p); e->dallocs.erase(std::remove(e->dallocs.begin(), e->dallocs.end(), p), e->dallocs.end()); } };
-	dfree(mg.d_offsets); dfree(mg.d_members); dfree(mg.d_member_ids); dfree(mg.arena); dfree(mg.slab); dfree(mg.final_slab);
+	dfree(e, mg.d_offsets); dfree(e, mg.d_members); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
 		mg = MergeState {};
 		mg.logical_ids = std::move(ids_keep); mg.index = std::move(idx_keep);
 	}
-	mg.nlogical = nl;
+	LogicalArrays &lg = mg.lg;
+	lg.nl = nl;
 
-	const size_t ncms = (size_t)e->cfg.cms_depth << e->cfg.cms_log2_width;
-	const size_t b_cms = ncms * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell), b_conn = (size_t)nl * 4 * 8;
-	size_t off = 0;
-	mg.off_sum = off;
-	const size_t o_cms_cur = off; off += align256(b_cms);
-	const size_t o_cms_last = off; off += align256(b_cms);
-	const size_t o_hl = off; off += align256(b_hist);
-	const size_t o_ha = off; off += align256(b_hist);
-	const size_t o_conn = off; off += align256(b_conn);
-	// GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX regions: still three regions, three collectives
+	// The arena region by region, each array 256-byte aligned: layout(nullptr) sizes it, layout(arena) places the arrays.
+	// GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX regions: still three regions, three collectives.
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS;
-	size_t o_lvl = 0, o_aux = 0, o_lmax = 0, o_rtt = 0, o_flush = 0;
-	if (levels) {
-		o_lvl = off; off += align256((size_t)NLEVELS * b_hist);
-		o_aux = off; off += align256((size_t)nl * 4 * 8);
-	}
-	mg.bytes_sum = off - mg.off_sum;
-	mg.off_maxi64 = off; const size_t o_hmax = off; off += align256((size_t)nl * 2 * 8);
-	if (levels) {
-		o_lmax = off; off += align256((size_t)nl * NLEVELS * 8);
-		o_rtt = off; off += align256((size_t)nl * 8);
-		o_flush = off; off += align256(2 * 8);
-	}
-	mg.bytes_maxi64 = off - mg.off_maxi64;
-	mg.off_maxu8 = off; const size_t o_hll = off; off += align256((size_t)nl << e->cfg.hll_p); mg.bytes_maxu8 = off - mg.off_maxu8;
-	mg.arena_bytes = off;
-
+	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
+	auto layout = [&](uint8_t *base) {
+		size_t off = 0;
+		auto take = [&](auto *&p, size_t bytes) {
+			if (base) p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + off);
+			off += align256(bytes);
+		};
+		mg.off_sum = off;
+		take(mg.g_cms_cur, b_cms); take(mg.g_cms_last, b_cms); take(lg.last, b_hist); take(lg.all, b_hist); take(lg.conn, (size_t)nl * 4 * 8);
+		if (levels) { take(lg.lvl, NLEVELS * b_hist); take(lg.aux, (size_t)nl * 4 * 8); }
+		mg.bytes_sum = off - mg.off_sum;
+		mg.off_maxi64 = off;
+		take(lg.hmax, (size_t)nl * 2 * 8);
+		if (levels) { take(lg.lvl_max, (size_t)nl * NLEVELS * 8); take(lg.rtt, (size_t)nl * 8); take(lg.flush, 2 * 8); }
+		mg.bytes_maxi64 = off - mg.off_maxi64;
+		mg.off_maxu8 = off;
+		take(lg.hll, (size_t)nl << e->cfg.hll_p);
+		mg.bytes_maxu8 = off - mg.off_maxu8;
+		return off;
+	};
+	mg.arena_bytes = layout(nullptr);
 	int rc = dalloc(e, &mg.arena, mg.arena_bytes);
 	if (rc) return rc;
-	mg.g_cms_cur = reinterpret_cast<unsigned long long *>(mg.arena + o_cms_cur);
-	mg.g_cms_last = reinterpret_cast<unsigned long long *>(mg.arena + o_cms_last);
-	mg.l_hist_last = reinterpret_cast<HistCell *>(mg.arena + o_hl);
-	mg.l_hist_all = reinterpret_cast<HistCell *>(mg.arena + o_ha);
-	mg.l_conn = reinterpret_cast<unsigned long long *>(mg.arena + o_conn);
-	mg.l_hmax = reinterpret_cast<long long *>(mg.arena + o_hmax);
-	mg.l_hll = mg.arena + o_hll;
-	if (levels) {
-		mg.l_lvl = reinterpret_cast<HistCell *>(mg.arena + o_lvl);
-		mg.l_aux = reinterpret_cast<unsigned long long *>(mg.arena + o_aux);
-		mg.l_lvl_max = reinterpret_cast<long long *>(mg.arena + o_lmax);
-		mg.l_rtt = reinterpret_cast<long long *>(mg.arena + o_rtt);
-		mg.l_flush = reinterpret_cast<long long *>(mg.arena + o_flush);
-	}
-	mg.slab_bytes = (size_t)(nl ? nl : 1) * sizeof(SlabEntry);
-	if ((rc = dalloc(e, &mg.slab, mg.slab_bytes))) return rc;
-	if ((rc = dalloc(e, &mg.final_slab, mg.slab_bytes))) return rc;
+	layout(mg.arena);
+	if ((rc = dalloc(e, &lg.slab, nl ? nl : 1))) return rc;
+	if ((rc = dalloc(e, &lg.final_slab, nl ? nl : 1))) return rc;
 	if ((rc = dalloc(e, &mg.d_offsets, (size_t)nl + 1))) return rc;
 	if ((rc = dalloc(e, &mg.d_members, members.size() + 1))) return rc;
 	if ((rc = dalloc(e, &mg.d_member_ids, member_ids.size() + 1))) return rc;
@@ -449,7 +408,7 @@ int gysk_merge_prepare(gysk_engine *e)
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_prepare: call gysk_set_logical_map first");
 
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8;
-	const uint32_t nl = mg.nlogical;
+	const uint32_t nl = mg.lg.nl;
 
 	CU(e, cudaMemcpyAsync(mg.g_cms_cur, e->st.cms_cur, b_cms, cudaMemcpyDeviceToDevice, e->stream));
 	CU(e, cudaMemcpyAsync(mg.g_cms_last, e->st.cms_last, b_cms, cudaMemcpyDeviceToDevice, e->stream));
@@ -459,18 +418,15 @@ int gysk_merge_prepare(gysk_engine *e)
 			resolve_members_kernel<<<div_up(mg.nmembers, 256), 256, 0, e->stream>>>(e->st, mg.d_member_ids, mg.nmembers, mg.d_members, null_slot);
 			e->kernel_launches++;
 		}
-		fold_hist_kernel<<<div_up((uint64_t)nl * HIST_CELLS, 256), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, nl, null_slot,
-				mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax);
-		fold_hll_kernel<<<div_up((uint64_t)nl << (e->cfg.hll_p - 2), 256), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, nl, null_slot,
-				reinterpret_cast<uint32_t *>(mg.l_hll));
-		fold_td_kernel<<<std::min<uint32_t>(div_up(nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, nl, null_slot,
-				reinterpret_cast<SlabEntry *>(mg.slab));
+		fold_hist_kernel<<<div_up((uint64_t)nl * HIST_CELLS, 256), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, null_slot, mg.lg);
+		fold_hll_kernel<<<div_up((uint64_t)nl << (e->cfg.hll_p - 2), 256), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, null_slot, mg.lg);
+		fold_td_kernel<<<std::min<uint32_t>(div_up(nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, null_slot,
+				mg.lg);
 		e->kernel_launches += 3;
 	}
-	if (mg.l_lvl) {		// GYSK_FLAG_MERGE_LEVELS: also with no logical service, for the flush tsec pair
+	if (mg.lg.lvl) {		// GYSK_FLAG_MERGE_LEVELS: also with no logical service, for the flush tsec pair
 		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members,
-				nl, e->cfg.max_svcs, live_mask(e, 0), live_mask(e, 1), (long long)e->last_flush_tsec, mg.l_lvl, mg.l_aux, mg.l_lvl_max, mg.l_rtt,
-				mg.l_flush);
+				e->cfg.max_svcs, (long long)e->last_flush_tsec, mg.lg);
 		e->kernel_launches++;
 	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
@@ -486,7 +442,7 @@ int gysk_merge_buffers(gysk_engine *e, gysk_buffer_desc *out, uint32_t cap, uint
 	MergeState &mg = e->mg;
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_buffers: call gysk_set_logical_map first");
 	if (cap < 3) return GYSK_ERR_NOSPC;
-	const bool lv = mg.l_lvl != nullptr;
+	const bool lv = mg.lg.lvl != nullptr;
 	out[0] = gysk_buffer_desc {lv ? "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn|levels|aux" : "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn",
 			mg.arena + mg.off_sum, mg.bytes_sum, GYSK_RED_SUM_U64, 0};
 	out[1] = gysk_buffer_desc {lv ? "max_i64: hist max_val_seen|level max_val_seen|rtt|flush tsec" : "max_i64: hist max_val_seen",
@@ -501,8 +457,8 @@ int gysk_merge_tdigest_slab(gysk_engine *e, void **dptr, uint64_t *nbytes)
 	CHECK_ENGINE(e);
 	if (!dptr || !nbytes) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Drain);
-	if (!e->mg.slab) return fail(e, GYSK_ERR_INVAL, "gysk_merge_tdigest_slab: call gysk_set_logical_map first");
-	*dptr = e->mg.slab; *nbytes = (uint64_t)e->mg.nlogical * sizeof(SlabEntry);
+	if (!e->mg.lg.slab) return fail(e, GYSK_ERR_INVAL, "gysk_merge_tdigest_slab: call gysk_set_logical_map first");
+	*dptr = e->mg.lg.slab; *nbytes = (uint64_t)e->mg.lg.nl * sizeof(SlabEntry);
 	return GYSK_OK;
 }
 
@@ -513,11 +469,10 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 	MergeState &mg = e->mg;
 	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: call gysk_merge_prepare first");
 	if (!world) world = 1;
-	const SlabEntry *src = d_gathered ? static_cast<const SlabEntry *>(d_gathered) : reinterpret_cast<const SlabEntry *>(mg.slab);
+	const SlabEntry *src = d_gathered ? static_cast<const SlabEntry *>(d_gathered) : mg.lg.slab;
 	if (!d_gathered) world = 1;
-	if (mg.nlogical) {
-		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.nlogical, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.nlogical,
-				reinterpret_cast<SlabEntry *>(mg.final_slab), e->st.td);
+	if (mg.lg.nl) {
+		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.lg.nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.lg, e->st.td);
 		e->kernel_launches++;
 	}
 	mg.finished = true;			// stream-ordered; the query calls synchronise
@@ -538,10 +493,8 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 		lidx[i] = it == mg.index.end() ? -1 : (int32_t)it->second;
 	}
 	const SvcRows rows {e->cfg.hll_p, out};
-	const LevelArrays lv {mg.l_lvl, mg.l_aux, mg.l_lvl_max, mg.l_rtt, mg.nlogical};
 	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(gysk_svc_summary), "query_logical", [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
-		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(reinterpret_cast<const int32_t *>(d_l), m, e->cfg.hll_p,
-				mg.l_hist_last, mg.l_hist_all, mg.l_conn, mg.l_hmax, mg.l_hll, reinterpret_cast<const SlabEntry *>(mg.final_slab), lv,
+		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(reinterpret_cast<const int32_t *>(d_l), m, e->cfg.hll_p, mg.lg,
 				reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
 		return 1;
 	}, [&](const uint8_t *h_rows, uint32_t off, uint32_t m) {
@@ -563,21 +516,11 @@ int gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gys
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_export_logical_hist: no finished merge");
 	const auto it = mg.index.find(logical_id);
 	if (it == mg.index.end()) return GYSK_ERR_NOENT;
-	const uint32_t l = it->second;
-	const HistCell *cells;
-	const long long *mx;
-	if (level) {
-		const int k = which - GYSK_HIST_RESP_5MIN;
-		cells = mg.l_lvl + ((size_t)k * mg.nlogical + l) * HIST_CELLS; mx = mg.l_lvl_max + 2 * (size_t)l + k;
-	}
-	else {
-		const int k = which == GYSK_HIST_RESP_ALL;
-		cells = (k ? mg.l_hist_all : mg.l_hist_last) + (size_t)l * HIST_CELLS; mx = mg.l_hmax + 2 * (size_t)l + k;
-	}
+	const LogicalArrays::Hist src = mg.lg.hist(which, it->second);
 	// the 15 cells, then max_val_seen_ into cell 15 (stream order: behind the merge that wrote them)
 	HistCell *h = reinterpret_cast<HistCell *>(e->h_wstage);
-	CU(e, cudaMemcpyAsync(h, cells, HIST_CELLS * sizeof(HistCell), cudaMemcpyDeviceToHost, e->stream));
-	CU(e, cudaMemcpyAsync(&h[HIST_MAX_CELL].sum, mx, sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaMemcpyAsync(h, src.cells, HIST_CELLS * sizeof(HistCell), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaMemcpyAsync(&h[HIST_MAX_CELL].sum, src.max, sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
 	hist_from_cells(h, 15, out, total, maxv, false);
 	if (level && *total == 0) *maxv = INT64_MIN;		// as gysk_export_hist answers an empty level
@@ -593,7 +536,7 @@ int gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tse
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_merge_flush_range: no finished merge");
 	long long *h = reinterpret_cast<long long *>(e->h_wstage);
-	CU(e, cudaMemcpyAsync(h, mg.l_flush, 2 * sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaMemcpyAsync(h, mg.lg.flush, 2 * sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
 	*max_tsec = (uint32_t)h[0]; *min_tsec = (uint32_t)-h[1];
 	return GYSK_OK;
@@ -662,20 +605,20 @@ int gysk_merge_global(gysk_engine *e, void *comm)
 		NC(e, a->CommCount(c, &world));
 		if (world < 1) return fail(e, GYSK_ERR_INVAL, "gysk_merge_global: empty communicator");
 		if (mg.gathered_world != (uint32_t)world) {
-			if (mg.gathered) { cudaFree(mg.gathered); e->dallocs.erase(std::remove(e->dallocs.begin(), e->dallocs.end(), (void *)mg.gathered), e->dallocs.end()); mg.gathered = nullptr; }
-			if ((rc = dalloc(e, &mg.gathered, mg.slab_bytes * (size_t)world, false))) return rc;
+			dfree(e, mg.gathered);
+			if ((rc = dalloc(e, &mg.gathered, (size_t)(mg.lg.nl ? mg.lg.nl : 1) * world, false))) return rc;
 			mg.gathered_world = (uint32_t)world;
 		}
-		const size_t slab = (size_t)mg.nlogical * sizeof(SlabEntry);
+		const size_t slab = (size_t)mg.lg.nl * sizeof(SlabEntry);
 		NC(e, a->GroupStart());
 		NC(e, a->AllReduce(mg.arena + mg.off_sum, mg.arena + mg.off_sum, mg.bytes_sum / 8, ncclUint64, ncclSum, c, e->stream));
 		NC(e, a->AllReduce(mg.arena + mg.off_maxi64, mg.arena + mg.off_maxi64, mg.bytes_maxi64 / 8, ncclInt64, ncclMax, c, e->stream));
 		NC(e, a->AllReduce(mg.arena + mg.off_maxu8, mg.arena + mg.off_maxu8, mg.bytes_maxu8, ncclUint8, ncclMax, c, e->stream));
-		if (slab) NC(e, a->AllGather(mg.slab, mg.gathered, slab, ncclUint8, c, e->stream));
+		if (slab) NC(e, a->AllGather(mg.lg.slab, mg.gathered, slab, ncclUint8, c, e->stream));
 		NC(e, a->GroupEnd());
 		e->merges++;
 	}
-	return gysk_merge_finish(e, e->mg.nlogical ? e->mg.gathered : nullptr, (uint32_t)world);
+	return gysk_merge_finish(e, e->mg.lg.nl ? e->mg.gathered : nullptr, (uint32_t)world);
 }
 
 } // extern "C"
