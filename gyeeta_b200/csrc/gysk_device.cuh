@@ -78,7 +78,7 @@ static constexpr unsigned long long KEY_TOMBSTONE = ~0ull;	// table entry of an 
 // key flush (about 160 K returning atomics per 100 M-event batch); the connection / process records need no cursor (SortTemp::recq).
 enum { CTR_IN = 0, CTR_DROPPED, CTR_RESP, CTR_TCP, CTR_TASK, CTR_FOREIGN, CTR_NKEYS, CTR_INSERT_FAIL, CTR_NTOUCHED /* short key segments */,
 	CTR_NLONG /* long key segments (batch rows) */, CTR_NEVICT, CTR_EVICTED_TOTAL,
-	CTR_NHOT /* hot rows in use by the batch in flight */, CTR_NHOT_NEXT /* rows handed out so far */, CTR_NWINDOW /* rows of the last window read */,
+	CTR_NHOT /* hot rows in use by the batch in flight */, CTR_NHOT_NEXT /* rows handed out so far */, CTR_NWINDOW /* rows of the last window read (or logical read / logical top-N) */,
 	CTR_NHOSTS /* host rows of the last gysk_query_host_listen */, CTR_MAX };
 
 // ---------------------------------------------------------------------------------------------------

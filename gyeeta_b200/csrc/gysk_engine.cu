@@ -512,6 +512,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &st.qps_hist, ns * HIST_CELLS)); A(dalloc(e, &st.act_hist, ns * HIST_CELLS)); A(dalloc(e, &st.slot_state, ns));
 	SortTemp &tmp = e->tmp;
 	const size_t nsort = std::max<size_t>(std::max<size_t>(ns, nt) + 1, cfg.max_batch);	// RESP keys of a batch; the top-N sorts rank services / tasks
+	tmp.nkeys = nsort;
 	tmp.max_tiles = (uint32_t)((nsort + SORT_TILE - 1) / SORT_TILE);
 	A(dalloc(e, &tmp.keys_a, nsort, false)); A(dalloc(e, &tmp.keys_b, nsort, false));
 	A(dalloc(e, &tmp.tile_status, (size_t)RADIX_MAX * tmp.max_tiles));
@@ -1459,28 +1460,42 @@ static uint32_t host_td_compress(const double *means, const uint64_t *w, uint32_
 	return nout;
 }
 
-int gysk_export_tdigest_pgtext(gysk_engine *e, uint64_t id, char *buf, uint32_t cap)
+} // extern "C"
+
+int gysk::tdigest_pgtext(gysk_engine *e, uint64_t id, ExportTd export_td, char *buf, uint32_t cap)
 {
 	double means[TD_CAP], minv = 0, maxv = 0, om[TD_CAP];
 	uint64_t w[TD_CAP], ow[TD_CAP];
 	uint32_t n = 0;
-	int rc = gysk_export_tdigest(e, id, means, w, TD_CAP, &n, &minv, &maxv);
+	int rc = export_td(e, id, means, w, TD_CAP, &n, &minv, &maxv);
 	if (rc) return rc;
 	const uint32_t no = host_td_compress(means, w, n, 100, om, ow);
 	return gysk_tdigest_to_pgtext(om, ow, no, 100, buf, cap);
 }
 
-int gysk_query_quantiles(gysk_engine *e, uint64_t id, const double *qs, uint32_t nq, double *out)
+int gysk::tdigest_quantiles(gysk_engine *e, uint64_t id, ExportTd export_td, const double *qs, uint32_t nq, double *out)
 {
 	double means[TD_CAP], minv = 0, maxv = 0;
 	uint64_t w[TD_CAP];
 	uint32_t n = 0;
-	int rc = gysk_export_tdigest(e, id, means, w, TD_CAP, &n, &minv, &maxv);
+	int rc = export_td(e, id, means, w, TD_CAP, &n, &minv, &maxv);
 
 	if (rc) return rc;
 	if ((!qs || !out) && nq) return GYSK_ERR_INVAL;
 	for (uint32_t i = 0; i < nq; ++i) out[i] = td_quantile(means, w, n, minv, maxv, qs[i]);
 	return GYSK_OK;
+}
+
+extern "C" {
+
+int gysk_export_tdigest_pgtext(gysk_engine *e, uint64_t id, char *buf, uint32_t cap)
+{
+	return tdigest_pgtext(e, id, gysk_export_tdigest, buf, cap);
+}
+
+int gysk_query_quantiles(gysk_engine *e, uint64_t id, const double *qs, uint32_t nq, double *out)
+{
+	return tdigest_quantiles(e, id, gysk_export_tdigest, qs, nq, out);
 }
 
 int gysk_query_flows(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_est *out)

@@ -136,6 +136,9 @@ struct MergeState
 	std::unordered_map<uint64_t, uint32_t> index;	// logical id -> dense index
 	uint32_t		*d_offsets {nullptr}, *d_members {nullptr};	// CSR: logical -> member slots on this GPU
 	unsigned long long	*d_member_ids {nullptr};			// id each member slot held when the map was set
+	unsigned long long	*d_logical_ids {nullptr};			// [nl] logical_ids on the device: the ids of the rows and top-N entries
+	int32_t			*d_sorted {nullptr};				// [nl] dense indices by ascending logical id (gysk_query_logical_all)
+	int32_t			*d_sel {nullptr};				// [nl] the part of d_sorted an ACTIVE_ONLY read selects
 	uint32_t		nmembers {0};
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
@@ -227,6 +230,10 @@ int submit_stage(gysk_engine *e);
 int drain_all(gysk_engine *e);
 int sync_locked(gysk_engine *e);
 void merge_release(gysk_engine *e);
+// the Postgres text and the quantiles of one exported digest; export_td is gysk_export_tdigest or gysk_export_logical_tdigest
+using ExportTd = int (*)(gysk_engine *, uint64_t, double *, uint64_t *, uint32_t, uint32_t *, double *, double *);
+int tdigest_pgtext(gysk_engine *e, uint64_t id, ExportTd export_td, char *buf, uint32_t cap);
+int tdigest_quantiles(gysk_engine *e, uint64_t id, ExportTd export_td, const double *qs, uint32_t nq, double *out);
 // HIST_SERIAL of 16 cells (cell HIST_MAX_CELL holds max_val_seen_ in .sum); total = the sum of the first nb counts
 void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint64_t *total, int64_t *maxv, bool t_is_int);
 
@@ -302,6 +309,7 @@ static_assert(sizeof(gysk_task_summary) <= sizeof(gysk_svc_summary) && QCHUNK <=
 static_assert(sizeof(SvcRaw) <= STAGE_BYTES && sizeof(TaskRaw) <= STAGE_BYTES, "the stage holds one id's raw state");
 static_assert(HLL_STAGE_REGS + (1u << 16) <= STAGE_BYTES, "the stage holds the found word and 2^16 HLL registers");
 static_assert(QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES && 64 * sizeof(gysk_topn_entry) <= STAGE_BYTES, "the stage holds the flow and top-N rows");
+static_assert(sizeof(SlabEntry) <= STAGE_BYTES, "the stage holds one merged digest");
 
 // A staged read, engine mutex held. The optional input (ids, flow keys or logical indices) travels through h_qids / d_qids in pieces
 // of `piece` entries; without one (the window reads) the pieces only cut the n rows. For each piece, launch(d_in, off, m) writes m

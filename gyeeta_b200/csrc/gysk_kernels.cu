@@ -2085,7 +2085,7 @@ __global__ void topn_task_score_kernel(DevState st, uint32_t ntasks, int metric,
 	keys[slot] = (score << 32) | slot;
 }
 
-// the want best of the sorted keys, with the id and host of their slots (services' or processes')
+// the want best of the sorted keys, with the id and host of their slots (services' or processes'; logical services: host 0)
 __global__ void topn_pick_kernel(const unsigned long long *__restrict__ slot_id, const uint32_t *__restrict__ slot_host,
 		const unsigned long long *__restrict__ sorted, uint32_t nslots, uint32_t want, gysk_topn_entry *__restrict__ out)
 {
@@ -2095,9 +2095,19 @@ __global__ void topn_pick_kernel(const unsigned long long *__restrict__ slot_id,
 	if (i < nslots) {
 		const unsigned long long k = sorted[nslots - 1 - i];		// descending
 		const uint32_t slot = (uint32_t)k;
-		o.glob_id = slot_id[slot]; o.score = k >> 32; o.host_idx = slot_host[slot];
+		o.glob_id = slot_id[slot]; o.score = k >> 32; o.host_idx = slot_host ? slot_host[slot] : 0u;
 	}
 	out[i] = o;
+}
+
+int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_t nkeys, const unsigned long long *ids, const uint32_t *hosts,
+		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s)
+{
+	int which = 0;
+	const int sorted = launch_radix_sort(tmp, d_n, nkeys, 32, 64, 64, 64, &which, s);
+	if (sorted < 0) return sorted;
+	topn_pick_kernel<<<1, 64, 0, s>>>(ids, hosts, which ? tmp.keys_b : tmp.keys_a, nkeys, want, d_out);
+	return sorted + 1;
 }
 
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
@@ -2105,15 +2115,11 @@ int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is
 {
 	if (!nslots) return 0;
 	unsigned long long *d_n = st.counters + CTR_NKEYS;
-	int which = 0, launches = 2;
 	if (is_task) topn_task_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, tmp.keys_a, d_n);
 	else topn_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, host_filter, tmp.keys_a, d_n);
-	const int sorted = launch_radix_sort(tmp, d_n, nslots, 32, 64, 64, 64, &which, s);
-	if (sorted < 0) return sorted;
-	launches += sorted;
-	topn_pick_kernel<<<1, 64, 0, s>>>(is_task ? st.task_slot_id : st.slot_id, is_task ? st.task_slot_host : st.slot_host,
-			which ? tmp.keys_b : tmp.keys_a, nslots, want, d_out);
-	return launches;
+	const int picked = launch_topn_pick(tmp, d_n, nslots, is_task ? st.task_slot_id : st.slot_id, is_task ? st.task_slot_host : st.slot_host,
+			want, d_out, s);
+	return picked < 0 ? picked : 1 + picked;
 }
 
 // per-task window of the three MTASK_HIST histograms: totals now minus totals at the previous flush (nothing on the ingest path)

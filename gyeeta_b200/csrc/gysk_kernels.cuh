@@ -85,7 +85,8 @@ struct DevState
 
 struct SortTemp
 {
-	unsigned long long	*keys_a, *keys_b;	// [max_batch] RESP sort keys of the batch (also the top-N sort keys)
+	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
+	uint64_t		nkeys;			// max(max_batch, max(max_svcs, max_tasks) + 1)
 	unsigned long long	*tile_status;		// [max_tiles][512] look-back status words {pass epoch | state | count}: never cleared
 	uint32_t		*epoch;			// HOST counter of radix passes launched (tags the status words)
 	uint32_t		*os_ghist;		// [8][512] global digit histograms of the one-sweep passes + [8] tile tickets
@@ -161,6 +162,10 @@ int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64
 // the want best services (host_filter < 0: of every host) or processes (is_task) of nslots by one metric; -1: sort failed
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
 		gysk_topn_entry *d_out, cudaStream_t s);
+// the second half of a top-N: the *d_n <= nkeys {score : 32 | index : 32} keys in tmp.keys_a sorted by score (stable), then the want best
+// as entries {ids[index], score, hosts[index]} (hosts nullptr: host 0), the later index first on equal scores; -1: sort failed
+int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_t nkeys, const unsigned long long *ids, const uint32_t *hosts,
+		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
 int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s);
 // the window roll into ring slot st.levels.cur of each level (cleared by the host when it starts a new epoch), the listener states,
 // the idle-service eviction

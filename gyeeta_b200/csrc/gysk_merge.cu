@@ -200,10 +200,10 @@ __global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntr
 // read side: one warp per logical service, its merged arrays into a shared-memory SvcRaw, then the row of summarize_warp (the
 // summary of gysk_query_svcs). The merge folds neither the current window, the connection bitmaps nor the per-slot state / qps /
 // active-connection words: they are zero; so are the rolling levels and the aux words unless the engine merges them (lg.lvl).
-// glob_id is left 0 for the host to fill in.
+// glob_id is the logical id (lids[l]), 0 for an index of -1.
 static constexpr int LG_WARPS = 4;
 __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const int32_t *__restrict__ lidx, uint32_t n, uint32_t hll_p, LogicalArrays lg,
-		gysk_svc_summary *__restrict__ out)
+		const unsigned long long *__restrict__ lids, gysk_svc_summary *__restrict__ out)
 {
 	__shared__ SvcRaw raw[LG_WARPS];
 	__shared__ unsigned long long summ[LG_WARPS][sizeof(gysk_svc_summary) / 8];
@@ -240,7 +240,61 @@ __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const in
 		for (int i = lane; i < TD_CAP; i += 32) r.cent[i] = lg.final_slab[l].cent[i];
 		hll_hist_warp(lg.hll_of(l, hll_p), hll_p, r.hll_hist, lane);
 	}
-	summarize_warp(r, 0, hll_p, summ[wid], out + q, lane);
+	summarize_warp(r, l >= 0 ? lids[l] : 0ull, hll_p, summ[wid], out + q, lane);
+}
+
+// a logical service whose merged last window holds response samples or connection events (GYSK_WINDOW_ACTIVE_ONLY)
+__device__ __forceinline__ bool logical_active(const LogicalArrays &lg, uint32_t l)
+{
+	const HistCell *c = lg.hist(GYSK_HIST_RESP_LAST, l).cells;
+	unsigned long long any = lg.conn_of(l)[0];
+#pragma unroll
+	for (int b = 0; b < HIST_MAX_CELL; ++b) any |= c[b].count;
+	return any != 0;
+}
+
+// One CTA walks the dense indices in ascending logical id and keeps the active ones, in order: a block-wide ballot scan places the
+// kept entries of each 1024-entry tile. *d_n = entries kept.
+__global__ void __launch_bounds__(1024) logical_select_kernel(const int32_t *__restrict__ sorted, LogicalArrays lg, int32_t *__restrict__ sel,
+		unsigned long long *d_n)
+{
+	__shared__ uint32_t wcnt[32];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	uint32_t running = 0;
+
+	for (uint32_t t = 0; t < lg.nl; t += 1024) {
+		const uint32_t i = t + threadIdx.x;
+		const int32_t l = i < lg.nl ? sorted[i] : 0;
+		const bool keep = i < lg.nl && logical_active(lg, (uint32_t)l);
+		const unsigned b = __ballot_sync(0xffffffffu, keep);
+		if (lane == 0) wcnt[wid] = __popc(b);
+		__syncthreads();
+		uint32_t before = 0, total = 0;
+		for (int w = 0; w < 32; ++w) { const uint32_t c = wcnt[w]; before += w < wid ? c : 0; total += c; }
+		if (keep) sel[running + before + __popc(b & ((1u << lane) - 1u))] = l;
+		running += total;
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) *d_n = running;
+}
+
+// top-N keys {score : 32 | dense index : 32} of the logical services, scored as topn_score_kernel scores a service from the merged arrays
+__global__ void logical_topn_score_kernel(LogicalArrays lg, int metric, unsigned long long *__restrict__ keys, unsigned long long *d_n)
+{
+	const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
+	if (l == 0) *d_n = lg.nl;
+	if (l >= lg.nl) return;
+	unsigned long long score = 0;
+
+	if (metric == GYSK_TOPN_QPS) {
+		const HistCell *c = lg.hist(GYSK_HIST_RESP_LAST, l).cells;
+		for (int b = 0; b < HIST_MAX_CELL; ++b) score += c[b].count;
+		if (score > 0xFFFFFFFFull) score = 0xFFFFFFFFull;
+	}
+	else if (metric == GYSK_TOPN_CONNS) score = (uint32_t)lg.conn_of(l)[0];
+	else if (metric == GYSK_TOPN_NET) score = (uint32_t)lg.conn_of(l)[1];
+	else score = (uint32_t)lg.aux_of(l)[0];		// GYSK_TOPN_ACTIVE
+	keys[l] = (score << 32) | l;
 }
 
 } // namespace gysk
@@ -349,8 +403,14 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 		for (uint32_t i = 0; i < n; ++i) member_ids[cur[lidx[i]]++] = glob_ids[i];
 	}
 
+	// dense indices by ascending logical id: the row order of gysk_query_logical_all
+	std::vector<int32_t> sorted(nl);
+	for (uint32_t l = 0; l < nl; ++l) sorted[l] = (int32_t)l;
+	std::sort(sorted.begin(), sorted.end(), [&](int32_t a, int32_t b) { return mg.logical_ids[a] < mg.logical_ids[b]; });
+
 	// (re)allocate the arena
 	dfree(e, mg.d_offsets); dfree(e, mg.d_members); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
+	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
@@ -392,6 +452,13 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	if ((rc = dalloc(e, &mg.d_offsets, (size_t)nl + 1))) return rc;
 	if ((rc = dalloc(e, &mg.d_members, members.size() + 1))) return rc;
 	if ((rc = dalloc(e, &mg.d_member_ids, member_ids.size() + 1))) return rc;
+	if ((rc = dalloc(e, &mg.d_logical_ids, nl ? nl : 1))) return rc;
+	if ((rc = dalloc(e, &mg.d_sorted, nl ? nl : 1))) return rc;
+	if ((rc = dalloc(e, &mg.d_sel, nl ? nl : 1))) return rc;
+	if (nl) {
+		CU(e, cudaMemcpyAsync(mg.d_logical_ids, mg.logical_ids.data(), (size_t)nl * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
+		CU(e, cudaMemcpyAsync(mg.d_sorted, sorted.data(), (size_t)nl * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
+	}
 	mg.nmembers = (uint32_t)members.size();
 	if (!member_ids.empty()) CU(e, cudaMemcpyAsync(mg.d_member_ids, member_ids.data(), member_ids.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
 	CU(e, cudaMemcpyAsync(mg.d_offsets, offs.data(), ((size_t)nl + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
@@ -495,7 +562,7 @@ int gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, 
 	const SvcRows rows {e->cfg.hll_p, out};
 	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(gysk_svc_summary), "query_logical", [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
 		logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(reinterpret_cast<const int32_t *>(d_l), m, e->cfg.hll_p, mg.lg,
-				reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
+				mg.d_logical_ids, reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
 		return 1;
 	}, [&](const uint8_t *h_rows, uint32_t off, uint32_t m) {
 		rows(h_rows, off, m);
@@ -524,6 +591,116 @@ int gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gys
 	CU(e, cudaStreamSynchronize(e->stream));
 	hist_from_cells(h, 15, out, total, maxv, false);
 	if (level && *total == 0) *maxv = INT64_MIN;		// as gysk_export_hist answers an empty level
+	return GYSK_OK;
+}
+
+// every logical service's row in ascending logical id: the uploaded permutation, compacted on the device under ACTIVE_ONLY, read in
+// WIN_ROWS pieces by the summary kernel of gysk_query_logical
+int gysk_query_logical_all(gysk_engine *e, uint32_t flags, gysk_svc_summary *out, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical_all: no finished merge");
+	uint32_t total = mg.lg.nl;
+	const int32_t *sel = mg.d_sorted;
+	if ((flags & GYSK_WINDOW_ACTIVE_ONLY) && total) {
+		unsigned long long *d_n = e->st.counters + CTR_NWINDOW, cnt = 0;
+		logical_select_kernel<<<1, 1024, 0, e->stream>>>(mg.d_sorted, mg.lg, mg.d_sel, d_n);
+		e->kernel_launches++;
+		CU(e, cudaMemcpyAsync(&cnt, d_n, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaStreamSynchronize(e->stream));
+		if (int rc = post_launch(e, "query_logical_all select")) return rc;
+		total = (uint32_t)cnt;
+		sel = mg.d_sel;
+	}
+	int rc = staged_read<uint64_t>(e, nullptr, std::min(cap, total), WIN_ROWS, sizeof(gysk_svc_summary), "query_logical_all",
+			[&](const unsigned long long *, uint32_t off, uint32_t m) {
+				logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(sel + off, m, e->cfg.hll_p, mg.lg, mg.d_logical_ids,
+						reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
+				return 1;
+			}, SvcRows {e->cfg.hll_p, out});
+	if (rc) return rc;
+	*n = total;
+	return GYSK_OK;
+}
+
+// score every logical service, sort the keys, pick the n best: the top-N path of gysk_topn_svcs over the merged arrays
+int gysk_topn_logical(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
+{
+	CHECK_ENGINE(e);
+	if (!out || !nout || n == 0 || n > 64 || metric < GYSK_TOPN_QPS || metric > GYSK_TOPN_ACTIVE || metric == GYSK_TOPN_ISSUE) return GYSK_ERR_INVAL;
+	if (metric == GYSK_TOPN_ACTIVE && !(e->cfg.flags & GYSK_FLAG_MERGE_LEVELS)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_topn_logical: no finished merge");
+	const uint32_t nl = mg.lg.nl;
+	*nout = 0;
+	if (!nl) return GYSK_OK;
+	if (nl > e->tmp.nkeys) return fail(e, GYSK_ERR_NOSPC, "gysk_topn_logical: more logical services than the sort buffers hold");
+	unsigned long long *d_n = e->st.counters + CTR_NWINDOW;
+	gysk_topn_entry *d_out = reinterpret_cast<gysk_topn_entry *>(e->d_wstage);
+	logical_topn_score_kernel<<<div_up(nl, 256), 256, 0, e->stream>>>(mg.lg, metric, e->tmp.keys_a, d_n);
+	const int picked = launch_topn_pick(e->tmp, d_n, nl, mg.d_logical_ids, nullptr, n, d_out, e->stream);
+	if (picked < 0) return fail(e, GYSK_ERR_INVAL, "gysk_topn_logical: sort failed");
+	e->kernel_launches += 1 + picked;
+	CU(e, cudaMemcpyAsync(e->h_wstage, d_out, sizeof(gysk_topn_entry) * n, cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	if (int rc = post_launch(e, "gysk_topn_logical")) return rc;
+	const gysk_topn_entry *h = reinterpret_cast<const gysk_topn_entry *>(e->h_wstage);
+	uint32_t k = 0;
+	for (uint32_t i = 0; i < std::min(n, nl); ++i) if (h[i].score) out[k++] = h[i];
+	*nout = k;
+	return GYSK_OK;
+}
+
+// the merged digest of one logical service, with the contract of gysk_export_tdigest
+int gysk_export_logical_tdigest(gysk_engine *e, uint64_t logical_id, double *means, uint64_t *weights, uint32_t cap, uint32_t *n, double *minv,
+		double *maxv)
+{
+	CHECK_ENGINE(e);
+	if (!means || !weights || !n) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_export_logical_tdigest: no finished merge");
+	const auto it = mg.index.find(logical_id);
+	if (it == mg.index.end()) return GYSK_ERR_NOENT;
+	CU(e, cudaMemcpyAsync(e->h_wstage, mg.lg.final_slab + it->second, sizeof(SlabEntry), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	const SlabEntry &s = *reinterpret_cast<const SlabEntry *>(e->h_wstage);
+	const uint32_t nc = std::min<uint32_t>(std::min<uint32_t>(s.head.n, TD_CAP), cap);
+	for (uint32_t c = 0; c < nc; ++c) { means[c] = s.cent[c].mean; weights[c] = s.cent[c].weight; }
+	*n = nc;
+	if (minv) *minv = s.head.minv;
+	if (maxv) *maxv = s.head.maxv;
+	return s.head.n > cap ? GYSK_ERR_NOSPC : GYSK_OK;
+}
+
+int gysk_export_logical_tdigest_pgtext(gysk_engine *e, uint64_t logical_id, char *buf, uint32_t cap)
+{
+	return tdigest_pgtext(e, logical_id, gysk_export_logical_tdigest, buf, cap);
+}
+
+int gysk_query_logical_quantiles(gysk_engine *e, uint64_t logical_id, const double *qs, uint32_t nq, double *out)
+{
+	return tdigest_quantiles(e, logical_id, gysk_export_logical_tdigest, qs, nq, out);
+}
+
+// the merged HLL registers of one logical service, with the contract of gysk_export_hll
+int gysk_export_logical_hll(gysk_engine *e, uint64_t logical_id, uint8_t *regs)
+{
+	CHECK_ENGINE(e);
+	if (!regs) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_export_logical_hll: no finished merge");
+	const auto it = mg.index.find(logical_id);
+	if (it == mg.index.end()) return GYSK_ERR_NOENT;
+	const size_t nb = (size_t)1 << e->cfg.hll_p;
+	CU(e, cudaMemcpyAsync(e->h_wstage, mg.lg.hll_of(it->second, e->cfg.hll_p), nb, cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	memcpy(regs, e->h_wstage, nb);
 	return GYSK_OK;
 }
 

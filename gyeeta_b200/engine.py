@@ -18,7 +18,7 @@ EVF_CLI_ERROR, EVF_SER_ERROR = 1, 2
 HIST_RESP_CUR, HIST_RESP_LAST, HIST_RESP_ALL, HIST_TASK_CPU_PCT, HIST_TASK_CPU_DELAY, HIST_TASK_BLKIO_DELAY, HIST_RESP_5MIN, HIST_RESP_5DAY, HIST_QPS, HIST_ACTIVE_CONN = range(10)
 STATE_IDLE, STATE_GOOD, STATE_OK, STATE_BAD, STATE_SEVERE, STATE_DOWN = range(6)
 ISSUE_NONE, ISSUE_LISTENER_TASKS, ISSUE_QPS_HIGH, ISSUE_ACTIVE_CONN_HIGH, ISSUE_SERVER_ERRORS, ISSUE_OS_CPU, ISSUE_OS_MEMORY, ISSUE_DEPENDENT, ISSUE_UNKNOWN = range(9)
-TOPN_QPS, TOPN_CONNS, TOPN_NET, TOPN_ISSUE = range(4)
+TOPN_QPS, TOPN_CONNS, TOPN_NET, TOPN_ISSUE, TOPN_ACTIVE = range(5)
 RAW_EVENT32, RAW_TCP_IPV4_EVENT, RAW_TCP_IPV4_RESP, RAW_TCP_IPV6_EVENT, RAW_TCP_IPV6_RESP, RAW_API_TRAN, RAW_RESP16, RAW_TCP24, RAW_TASK24 = range(9)
 RESP16_DTYPE = np.dtype([("svc_id", "<u8"), ("usec", "<u4"), ("host_idx", "<u2"), ("cli_port", "u1"), ("flags", "u1")])
 TCP24_DTYPE = np.dtype([("svc_id", "<u8"), ("flow_key", "<u8"), ("bytes", "<u4"), ("host_idx", "<u2"), ("type", "u1"), ("pad", "u1")])
@@ -228,6 +228,12 @@ def load_library(path=None):
         "gysk_query_logical": (i32, [vp, vp, u32, vp]),
         "gysk_export_logical_hist": (i32, [vp, u64, i32, vp, vp, vp]),
         "gysk_merge_flush_range": (i32, [vp, vp, vp]),
+        "gysk_query_logical_all": (i32, [vp, u32, vp, u32, vp]),
+        "gysk_topn_logical": (i32, [vp, i32, u32, vp, vp]),
+        "gysk_export_logical_tdigest": (i32, [vp, u64, vp, vp, u32, vp, vp, vp]),
+        "gysk_export_logical_tdigest_pgtext": (i32, [vp, u64, vp, u32]),
+        "gysk_query_logical_quantiles": (i32, [vp, u64, vp, u32, vp]),
+        "gysk_export_logical_hll": (i32, [vp, u64, vp]),
         "gysk_query_flows_global": (i32, [vp, vp, u32, i32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
@@ -505,8 +511,11 @@ class Engine:
         return out, total.value, mx.value
 
     def export_hll(self, id_):
+        return self._hll(self.L.gysk_export_hll, id_)
+
+    def _hll(self, fn, id_):
         regs = np.zeros(1 << self.cfg.hll_p, dtype=np.uint8)
-        rc = self.L.gysk_export_hll(self.h, int(id_), _p(regs))
+        rc = fn(self.h, int(id_), _p(regs))
         if rc == -2:
             return None
         self._chk(rc)
@@ -522,18 +531,24 @@ class Engine:
         return masks, cnt
 
     def export_tdigest(self, id_):
+        return self._tdigest(self.L.gysk_export_tdigest, id_)
+
+    def _tdigest(self, fn, id_):
         means = np.zeros(TD_CAP, dtype=np.float64)
         weights = np.zeros(TD_CAP, dtype=np.uint64)
         n, mn, mx = C.c_uint32(), C.c_double(), C.c_double()
-        rc = self.L.gysk_export_tdigest(self.h, int(id_), _p(means), _p(weights), TD_CAP, C.byref(n), C.byref(mn), C.byref(mx))
+        rc = fn(self.h, int(id_), _p(means), _p(weights), TD_CAP, C.byref(n), C.byref(mn), C.byref(mx))
         if rc == -2:
             return None
         self._chk(rc)
         return means[: n.value].copy(), weights[: n.value].copy(), mn.value, mx.value
 
     def export_tdigest_pgtext(self, id_):
+        return self._pgtext(self.L.gysk_export_tdigest_pgtext, id_)
+
+    def _pgtext(self, fn, id_):
         buf = C.create_string_buffer(8192)
-        rc = self.L.gysk_export_tdigest_pgtext(self.h, int(id_), buf, len(buf))
+        rc = fn(self.h, int(id_), buf, len(buf))
         if rc == -2:
             return None
         if rc < 0:
@@ -541,9 +556,12 @@ class Engine:
         return buf.value.decode()
 
     def quantiles(self, id_, qs):
+        return self._quantiles(self.L.gysk_query_quantiles, id_, qs)
+
+    def _quantiles(self, fn, id_, qs):
         qs = np.ascontiguousarray(qs, dtype=np.float64)
         out = np.zeros(len(qs), dtype=np.float64)
-        self._chk(self.L.gysk_query_quantiles(self.h, int(id_), _p(qs), len(qs), _p(out)))
+        self._chk(fn(self.h, int(id_), _p(qs), len(qs), _p(out)))
         return out
 
     # ---- multi-GPU merge ----
@@ -599,6 +617,38 @@ class Engine:
             return None
         self._chk(rc)
         return out, total.value, mx.value
+
+    def query_logical_all(self, active_only=False, cap=None):
+        """gysk_query_logical_all: (SvcSummary rows of the merged logical services in ascending logical id, number of matching rows).
+        cap None = all rows (a count call first); 0 = the count only"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_logical_all(self.h, flags, None, 0, C.byref(n)))
+            cap = n.value
+        out = (SvcSummary * max(cap, 1))()
+        self._chk(self.L.gysk_query_logical_all(self.h, flags, out if cap else None, cap, C.byref(n)))
+        return out[: min(cap, n.value)], n.value
+
+    def topn_logical(self, metric, n=10):
+        """gysk_topn_logical: [(logical id, score, 0)] of the n best logical services of the last merge, best first"""
+        out = (TopnEntry * n)()
+        k = C.c_uint32()
+        self._chk(self.L.gysk_topn_logical(self.h, metric, n, out, C.byref(k)))
+        return [(o.glob_id, o.score, o.host_idx) for o in out[: k.value]]
+
+    def export_logical_tdigest(self, logical_id):
+        """(means, weights, min, max) of a logical service's merged digest; None for an id the map does not have"""
+        return self._tdigest(self.L.gysk_export_logical_tdigest, logical_id)
+
+    def export_logical_tdigest_pgtext(self, logical_id):
+        return self._pgtext(self.L.gysk_export_logical_tdigest_pgtext, logical_id)
+
+    def logical_quantiles(self, logical_id, qs):
+        return self._quantiles(self.L.gysk_query_logical_quantiles, logical_id, qs)
+
+    def export_logical_hll(self, logical_id):
+        return self._hll(self.L.gysk_export_logical_hll, logical_id)
 
     def merge_flush_range(self):
         """gysk_merge_flush_range: (earliest, latest) tsec of the ranks' last flush, as the last merge all-reduced them"""
