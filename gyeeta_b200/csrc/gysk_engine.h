@@ -90,8 +90,12 @@ struct HostTaskTopn
 // one logical service's t-digest in the merge step: fixed size, so that the slabs all-gather as bytes
 struct SlabEntry { TdHead head; Centroid cent[TD_CAP]; };
 
+// LISTEN_SUMM_STATS words of one logical service: the 15 int32 fields of gysk_host_summary before its pad, nstates[0..7] first
+constexpr int STATE_WORDS = 15;
+static_assert(sizeof(gysk_host_summary) == (STATE_WORDS + 1) * sizeof(int32_t), "gysk_host_summary: 15 fields and a pad");
+
 // The merged arrays of the nl logical services: the merge arena's per-logical arrays and the t-digest slabs, passed by value to the
-// merge kernels. lvl .. flush exist with GYSK_FLAG_MERGE_LEVELS only (nullptr without it).
+// merge kernels. lvl .. flush exist with GYSK_FLAG_MERGE_LEVELS only, states with GYSK_FLAG_MERGE_STATES only (nullptr without).
 struct LogicalArrays
 {
 	uint32_t		nl {0};
@@ -99,6 +103,7 @@ struct LogicalArrays
 	unsigned long long	*conn {nullptr};			// SUM [nl][4]: last cnt, last kb, all cnt, all kb
 	HistCell		*lvl {nullptr};				// SUM [2][nl][16]: the live ring slots of the 300-s / 5-day levels, cells 0..14
 	unsigned long long	*aux {nullptr};				// SUM [nl][4]: active conns, active kbytes, client errors, server errors
+	unsigned long long	*states {nullptr};			// SUM [nl][STATE_WORDS]: the members' LISTEN_SUMM_STATS, each word mod 2^32
 	long long		*hmax {nullptr};			// MAX [nl][2]: max_val_seen_ of last, all
 	long long		*lvl_max {nullptr};			// MAX [nl][2]: max_val_seen_ of the 300-s / 5-day levels
 	long long		*rtt {nullptr};				// MAX [nl]: the largest rtt_last bit pattern (a non-negative float's order)
@@ -126,6 +131,13 @@ struct LogicalArrays
 	}
 	__host__ __device__ __forceinline__ unsigned long long *conn_of(uint32_t l) const { return conn + 4 * (size_t)l; }
 	__host__ __device__ __forceinline__ unsigned long long *aux_of(uint32_t l) const { return aux + 4 * (size_t)l; }
+	__host__ __device__ __forceinline__ unsigned long long *states_of(uint32_t l) const { return states + STATE_WORDS * (size_t)l; }
+	// member listeners in STATE_BAD, STATE_SEVERE or STATE_DOWN: MS_CLUSTER_STATE's nsvc_issue (gysk_query_cluster_state)
+	__host__ __device__ __forceinline__ uint32_t nsvc_issue(uint32_t l) const
+	{
+		const unsigned long long *w = states_of(l);
+		return (uint32_t)(w[GYSK_STATE_BAD] + w[GYSK_STATE_SEVERE] + w[GYSK_STATE_DOWN]);
+	}
 	__host__ __device__ __forceinline__ uint8_t *hll_of(uint32_t l, uint32_t hll_p) const { return hll + ((size_t)l << hll_p); }
 };
 
@@ -143,7 +155,7 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux]
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux] [, states]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt, flush tsec]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
@@ -310,6 +322,7 @@ static_assert(sizeof(SvcRaw) <= STAGE_BYTES && sizeof(TaskRaw) <= STAGE_BYTES, "
 static_assert(HLL_STAGE_REGS + (1u << 16) <= STAGE_BYTES, "the stage holds the found word and 2^16 HLL registers");
 static_assert(QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES && 64 * sizeof(gysk_topn_entry) <= STAGE_BYTES, "the stage holds the flow and top-N rows");
 static_assert(sizeof(SlabEntry) <= STAGE_BYTES, "the stage holds one merged digest");
+static_assert(sizeof(gysk_logical_state) == 80 && sizeof(gysk_logical_state) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS state rows");
 
 // A staged read, engine mutex held. The optional input (ids, flow keys or logical indices) travels through h_qids / d_qids in pieces
 // of `piece` entries; without one (the window reads) the pieces only cut the n rows. For each piece, launch(d_in, off, m) writes m

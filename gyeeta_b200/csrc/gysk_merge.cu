@@ -9,11 +9,13 @@
 //                            [u64 SUM region : global CMS cur/last | histogram last/all | conn cells]
 //                            [i64 MAX region : max_val_seen_ last/all]   [u8 MAX region : HLL registers]
 //                          and a fixed t-digest slab (not element-wise mergeable); GYSK_FLAG_MERGE_LEVELS appends the rolling
-//                          levels and aux sums to the SUM region, their maxima, the rtt and the flush tsec pair to the i64 MAX one
+//                          levels and aux sums to the SUM region, their maxima, the rtt and the flush tsec pair to the i64 MAX one;
+//                          GYSK_FLAG_MERGE_STATES appends the members' LISTEN_SUMM_STATS words to the SUM region
 //   (caller)               all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
 //   gysk_export_logical_hist / gysk_merge_flush_range   one merged histogram / the ranks' flush tsec range
+//   gysk_query_logical_states[_all]   the member listeners' state counts per logical service (GYSK_FLAG_MERGE_STATES)
 //
 // It is the additive roll-up of MS_CLUSTER_STATE::STATE_ONE::add_stats (common/gy_comm_proto.h:3199-3214) /
 // SHCONN_HANDLER::aggregate_cluster_state (server/gy_shconnhdlr.cc:4583) and of GY_HISTOGRAM::update_from_serialized
@@ -127,6 +129,40 @@ __global__ void __launch_bounds__(256, 8) fold_levels_kernel(DevState st, const 
 		a[0] = ac; a[1] = ak; a[2] = ce; a[3] = se;
 		lg.rtt[l] = rtt;
 	}
+}
+
+// GYSK_FLAG_MERGE_STATES, one thread per logical service: each member adds LISTEN_SUMM_STATS::update (server/gy_msocket.h:853-864) of
+// the LISTENER_STATE_NOTIFY record gysk_encode_listener_state writes from its gysk_query_svcs row. Every value is the row's own, from
+// the arrays summarize_fields reads: curr_state (slot_state), nqrys_5s (the last window's cells through cells_total, truncated to 32
+// bits), nconns_active and ser_errors (slot_aux), kbytes_5s (conn_last). The u64 words keep the int32 sums modulo 2^32.
+__global__ void fold_states_kernel(DevState st, const uint32_t *__restrict__ offs, const uint32_t *__restrict__ members, uint32_t null_slot,
+		LogicalArrays lg)
+{
+	const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
+	if (l >= lg.nl) return;
+	unsigned long long nst[8] = {}, qps = 0, act = 0, kb_in = 0, ser = 0, nlisten = 0, nactive = 0;
+
+	for (uint32_t m = offs[l]; m < offs[l + 1]; ++m) {
+		const uint32_t s = members[m];
+		if (s == null_slot) continue;
+		const uint8_t state = st.slot_state[s].state;
+		if (state > GYSK_STATE_DOWN) continue;			// never reaches summstats.update (gy_mconnhdlr.cc:11183-11251)
+		uint64_t counts[15];
+		const uint32_t nqrys_5s = (uint32_t)cells_total(st.hist_last + (size_t)s * HIST_CELLS, 15, counts);
+		const SlotAux x = st.slot_aux[s];
+#pragma unroll
+		for (int k = 0; k < 8; ++k) nst[k] += state == k;
+		qps += nqrys_5s / 5;
+		act += (uint32_t)x.act_last;
+		kb_in += (uint32_t)(st.conn_last[s] >> 32);
+		ser += (uint32_t)(x.err_last >> 32);
+		nlisten++;
+		nactive += nqrys_5s != 0;
+	}
+	unsigned long long *w = lg.states_of(l);
+#pragma unroll
+	for (int k = 0; k < 8; ++k) w[k] = nst[k];
+	w[8] = qps; w[9] = act; w[10] = kb_in; w[11] = 0; w[12] = ser; w[13] = nlisten; w[14] = nactive;	// tot_kb_outbound: the encoder's 0
 }
 
 // one thread per (logical, 4 registers): per-byte max over the member services
@@ -293,8 +329,31 @@ __global__ void logical_topn_score_kernel(LogicalArrays lg, int metric, unsigned
 	}
 	else if (metric == GYSK_TOPN_CONNS) score = (uint32_t)lg.conn_of(l)[0];
 	else if (metric == GYSK_TOPN_NET) score = (uint32_t)lg.conn_of(l)[1];
+	else if (metric == GYSK_TOPN_ISSUE) score = lg.nsvc_issue(l);
 	else score = (uint32_t)lg.aux_of(l)[0];		// GYSK_TOPN_ACTIVE
 	keys[l] = (score << 32) | l;
+}
+
+// GYSK_FLAG_MERGE_STATES read side, one thread per row: the merged words of dense index lidx[q] as LISTEN_SUMM_STATS<int> (each word
+// truncated to 32 bits: the int32 wrap-around sum), logical id lids[l]; an index of -1 gives an all-zero row
+__global__ void logical_state_kernel(const int32_t *__restrict__ lidx, uint32_t n, LogicalArrays lg, const unsigned long long *__restrict__ lids,
+		gysk_logical_state *__restrict__ out)
+{
+	const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+	if (q >= n) return;
+	const int32_t l = lidx[q];
+	gysk_logical_state o;
+	memset(&o, 0, sizeof(o));
+	if (l >= 0) {
+		const unsigned long long *w = lg.states_of((uint32_t)l);
+		int32_t f[STATE_WORDS + 1];
+#pragma unroll
+		for (int k = 0; k < STATE_WORDS; ++k) f[k] = (int32_t)(uint32_t)w[k];
+		f[STATE_WORDS] = 0;
+		memcpy(&o.summ, f, sizeof(f));
+		o.logical_id = lids[l]; o.found = 1; o.nsvc_issue = lg.nsvc_issue((uint32_t)l);
+	}
+	out[q] = o;
 }
 
 } // namespace gysk
@@ -421,8 +480,9 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	lg.nl = nl;
 
 	// The arena region by region, each array 256-byte aligned: layout(nullptr) sizes it, layout(arena) places the arrays.
-	// GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX regions: still three regions, three collectives.
-	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS;
+	// GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX regions, GYSK_FLAG_MERGE_STATES its words to the
+	// end of the SUM region after them: still three regions, three collectives.
+	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES;
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
@@ -433,6 +493,7 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 		mg.off_sum = off;
 		take(mg.g_cms_cur, b_cms); take(mg.g_cms_last, b_cms); take(lg.last, b_hist); take(lg.all, b_hist); take(lg.conn, (size_t)nl * 4 * 8);
 		if (levels) { take(lg.lvl, NLEVELS * b_hist); take(lg.aux, (size_t)nl * 4 * 8); }
+		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8);
 		mg.bytes_sum = off - mg.off_sum;
 		mg.off_maxi64 = off;
 		take(lg.hmax, (size_t)nl * 2 * 8);
@@ -490,6 +551,10 @@ int gysk_merge_prepare(gysk_engine *e)
 		fold_td_kernel<<<std::min<uint32_t>(div_up(nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, null_slot,
 				mg.lg);
 		e->kernel_launches += 3;
+		if (mg.lg.states) {		// GYSK_FLAG_MERGE_STATES
+			fold_states_kernel<<<div_up(nl, 256), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members, null_slot, mg.lg);
+			e->kernel_launches++;
+		}
 	}
 	if (mg.lg.lvl) {		// GYSK_FLAG_MERGE_LEVELS: also with no logical service, for the flush tsec pair
 		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.d_offsets, mg.d_members,
@@ -510,8 +575,9 @@ int gysk_merge_buffers(gysk_engine *e, gysk_buffer_desc *out, uint32_t cap, uint
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_buffers: call gysk_set_logical_map first");
 	if (cap < 3) return GYSK_ERR_NOSPC;
 	const bool lv = mg.lg.lvl != nullptr;
-	out[0] = gysk_buffer_desc {lv ? "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn|levels|aux" : "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn",
-			mg.arena + mg.off_sum, mg.bytes_sum, GYSK_RED_SUM_U64, 0};
+	static const char *const sum_names[4] = {"sum_u64: cms_cur|cms_last|hist_last|hist_all|conn", "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn|levels|aux",
+		"sum_u64: cms_cur|cms_last|hist_last|hist_all|conn|states", "sum_u64: cms_cur|cms_last|hist_last|hist_all|conn|levels|aux|states"};
+	out[0] = gysk_buffer_desc {sum_names[lv + 2 * (mg.lg.states != nullptr)], mg.arena + mg.off_sum, mg.bytes_sum, GYSK_RED_SUM_U64, 0};
 	out[1] = gysk_buffer_desc {lv ? "max_i64: hist max_val_seen|level max_val_seen|rtt|flush tsec" : "max_i64: hist max_val_seen",
 			mg.arena + mg.off_maxi64, mg.bytes_maxi64, GYSK_RED_MAX_I64, 0};
 	out[2] = gysk_buffer_desc {"max_u8: hll registers", mg.arena + mg.off_maxu8, mg.bytes_maxu8, GYSK_RED_MAX_U8, 0};
@@ -594,8 +660,35 @@ int gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gys
 	return GYSK_OK;
 }
 
-// every logical service's row in ascending logical id: the uploaded permutation, compacted on the device under ACTIVE_ONLY, read in
-// WIN_ROWS pieces by the summary kernel of gysk_query_logical
+} // extern "C"
+
+namespace {
+
+// The rows of a read over every logical service, engine mutex held: *sel = their dense indices on the device in ascending logical id (the
+// uploaded permutation, compacted on the device under ACTIVE_ONLY), *total = their number
+int logical_rows(gysk_engine *e, uint32_t flags, const int32_t **sel, uint32_t *total, const char *what)
+{
+	MergeState &mg = e->mg;
+	*total = mg.lg.nl;
+	*sel = mg.d_sorted;
+	if ((flags & GYSK_WINDOW_ACTIVE_ONLY) && *total) {
+		unsigned long long *d_n = e->st.counters + CTR_NWINDOW, cnt = 0;
+		logical_select_kernel<<<1, 1024, 0, e->stream>>>(mg.d_sorted, mg.lg, mg.d_sel, d_n);
+		e->kernel_launches++;
+		CU(e, cudaMemcpyAsync(&cnt, d_n, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaStreamSynchronize(e->stream));
+		if (int rc = post_launch(e, what)) return rc;
+		*total = (uint32_t)cnt;
+		*sel = mg.d_sel;
+	}
+	return GYSK_OK;
+}
+
+} // namespace
+
+extern "C" {
+
+// every logical service's row in ascending logical id (logical_rows), read in WIN_ROWS pieces by the summary kernel of gysk_query_logical
 int gysk_query_logical_all(gysk_engine *e, uint32_t flags, gysk_svc_summary *out, uint32_t cap, uint32_t *n)
 {
 	CHECK_ENGINE(e);
@@ -603,18 +696,9 @@ int gysk_query_logical_all(gysk_engine *e, uint32_t flags, gysk_svc_summary *out
 	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical_all: no finished merge");
-	uint32_t total = mg.lg.nl;
-	const int32_t *sel = mg.d_sorted;
-	if ((flags & GYSK_WINDOW_ACTIVE_ONLY) && total) {
-		unsigned long long *d_n = e->st.counters + CTR_NWINDOW, cnt = 0;
-		logical_select_kernel<<<1, 1024, 0, e->stream>>>(mg.d_sorted, mg.lg, mg.d_sel, d_n);
-		e->kernel_launches++;
-		CU(e, cudaMemcpyAsync(&cnt, d_n, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
-		CU(e, cudaStreamSynchronize(e->stream));
-		if (int rc = post_launch(e, "query_logical_all select")) return rc;
-		total = (uint32_t)cnt;
-		sel = mg.d_sel;
-	}
+	uint32_t total = 0;
+	const int32_t *sel = nullptr;
+	if (int rc = logical_rows(e, flags, &sel, &total, "query_logical_all select")) return rc;
 	int rc = staged_read<uint64_t>(e, nullptr, std::min(cap, total), WIN_ROWS, sizeof(gysk_svc_summary), "query_logical_all",
 			[&](const unsigned long long *, uint32_t off, uint32_t m) {
 				logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(sel + off, m, e->cfg.hll_p, mg.lg, mg.d_logical_ids,
@@ -626,11 +710,60 @@ int gysk_query_logical_all(gysk_engine *e, uint32_t flags, gysk_svc_summary *out
 	return GYSK_OK;
 }
 
+// GYSK_FLAG_MERGE_STATES: the members' LISTEN_SUMM_STATS of logical ids, rows made on the device (logical_state_kernel)
+int gysk_query_logical_states(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_logical_state *out)
+{
+	CHECK_ENGINE(e);
+	if ((!logical_ids || !out) && n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_MERGE_STATES)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical_states: no finished merge");
+
+	std::vector<int32_t> lidx(n);		// dense logical index, -1 for an id the map does not have
+	for (uint32_t i = 0; i < n; ++i) {
+		auto it = mg.index.find(logical_ids[i]);
+		lidx[i] = it == mg.index.end() ? -1 : (int32_t)it->second;
+	}
+	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(gysk_logical_state), "query_logical_states", [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
+		logical_state_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(reinterpret_cast<const int32_t *>(d_l), m, mg.lg, mg.d_logical_ids,
+				reinterpret_cast<gysk_logical_state *>(e->d_wstage));
+		return 1;
+	}, [&](const uint8_t *h_rows, uint32_t off, uint32_t m) {
+		memcpy(out + off, h_rows, (size_t)m * sizeof(gysk_logical_state));
+		for (uint32_t i = 0; i < m; ++i) out[off + i].logical_id = logical_ids[off + i];
+	});
+}
+
+// GYSK_FLAG_MERGE_STATES: every logical service's state row, the rows of gysk_query_logical_all (logical_rows)
+int gysk_query_logical_states_all(gysk_engine *e, uint32_t flags, gysk_logical_state *out, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_MERGE_STATES)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_query_logical_states_all: no finished merge");
+	uint32_t total = 0;
+	const int32_t *sel = nullptr;
+	if (int rc = logical_rows(e, flags, &sel, &total, "query_logical_states_all select")) return rc;
+	int rc = staged_read<uint64_t>(e, nullptr, std::min(cap, total), WIN_ROWS, sizeof(gysk_logical_state), "query_logical_states_all",
+			[&](const unsigned long long *, uint32_t off, uint32_t m) {
+				logical_state_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(sel + off, m, mg.lg, mg.d_logical_ids,
+						reinterpret_cast<gysk_logical_state *>(e->d_wstage));
+				return 1;
+			}, CopyRows<gysk_logical_state> {out});
+	if (rc) return rc;
+	*n = total;
+	return GYSK_OK;
+}
+
 // score every logical service, sort the keys, pick the n best: the top-N path of gysk_topn_svcs over the merged arrays
 int gysk_topn_logical(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
 {
 	CHECK_ENGINE(e);
-	if (!out || !nout || n == 0 || n > 64 || metric < GYSK_TOPN_QPS || metric > GYSK_TOPN_ACTIVE || metric == GYSK_TOPN_ISSUE) return GYSK_ERR_INVAL;
+	if (!out || !nout || n == 0 || n > 64 || metric < GYSK_TOPN_QPS || metric > GYSK_TOPN_ACTIVE) return GYSK_ERR_INVAL;
+	if (metric == GYSK_TOPN_ISSUE && !(e->cfg.flags & GYSK_FLAG_MERGE_STATES)) return GYSK_ERR_INVAL;
 	if (metric == GYSK_TOPN_ACTIVE && !(e->cfg.flags & GYSK_FLAG_MERGE_LEVELS)) return GYSK_ERR_NOTSUP;
 	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;

@@ -32,7 +32,7 @@ assert RESP16_DTYPE.itemsize == 16 and TCP24_DTYPE.itemsize == 24 and TASK24_DTY
 NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CONN_STATS = 0x309, 0x30C, 0x310, 0x312
 (HOSTTOP_SVC_ISSUE, HOSTTOP_SVC_QPS, HOSTTOP_SVC_CONNS, HOSTTOP_SVC_NET, HOSTTOP_TASK_ISSUE, HOSTTOP_TASK_NET, HOSTTOP_TASK_CPU, HOSTTOP_TASK_RSS,
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
-FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS = 1, 2
+FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES = 1, 2, 4
 TD_CAP = 256
 
 
@@ -136,6 +136,14 @@ class HostSummary(C.Structure):
                                                                          "tot_ser_errors", "nlisteners", "nactive", "pad")]
 
 
+class LogicalState(C.Structure):
+    """gysk_logical_state: the member listeners' LISTEN_SUMM_STATS of one logical service (GYSK_FLAG_MERGE_STATES)"""
+    _fields_ = [("logical_id", C.c_uint64), ("found", C.c_int32), ("nsvc_issue", C.c_uint32), ("summ", HostSummary)]
+
+
+assert C.sizeof(LogicalState) == 80
+
+
 class ClusterState(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("nhosts", "nsvc_issue", "nsvcissue_hosts", "nsvc", "total_qps", "svc_net_mb")] + [("pad", C.c_uint32 * 2)]
 
@@ -234,6 +242,8 @@ def load_library(path=None):
         "gysk_export_logical_tdigest_pgtext": (i32, [vp, u64, vp, u32]),
         "gysk_query_logical_quantiles": (i32, [vp, u64, vp, u32, vp]),
         "gysk_export_logical_hll": (i32, [vp, u64, vp]),
+        "gysk_query_logical_states": (i32, [vp, vp, u32, vp]),
+        "gysk_query_logical_states_all": (i32, [vp, u32, vp, u32, vp]),
         "gysk_query_flows_global": (i32, [vp, vp, u32, i32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
@@ -260,7 +270,7 @@ class Engine:
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
-                 merge_levels=False):
+                 merge_levels=False, merge_states=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -269,7 +279,8 @@ class Engine:
         cfg.max_batch = max_batch
         cfg.stage_batch = stage_batch
         cfg.idle_evict_secs = idle_evict_secs
-        cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0)
+        cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
+                    (FLAG_MERGE_STATES if merge_states else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -649,6 +660,24 @@ class Engine:
 
     def export_logical_hll(self, logical_id):
         return self._hll(self.L.gysk_export_logical_hll, logical_id)
+
+    def query_logical_states(self, ids):
+        """gysk_query_logical_states: LogicalState rows of logical ids from the last merge (merge_states=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (LogicalState * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_logical_states(self.h, _p(ids), len(ids), out))
+        return out[: len(ids)]
+
+    def query_logical_states_all(self, active_only=False, cap=None):
+        """gysk_query_logical_states_all: (LogicalState rows in ascending logical id, number of matching rows); cap as query_logical_all"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_logical_states_all(self.h, flags, None, 0, C.byref(n)))
+            cap = n.value
+        out = (LogicalState * max(cap, 1))()
+        self._chk(self.L.gysk_query_logical_states_all(self.h, flags, out if cap else None, cap, C.byref(n)))
+        return out[: min(cap, n.value)], n.value
 
     def merge_flush_range(self):
         """gysk_merge_flush_range: (earliest, latest) tsec of the ranks' last flush, as the last merge all-reduced them"""

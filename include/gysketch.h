@@ -191,6 +191,10 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 #define GYSK_FLAG_MERGE_LEVELS		0x2u	/* the merge step also folds the 300-s / 5-day levels, active connections, errors
 						   and max rtt of the member services into each logical service (see
 						   gysk_query_logical); without it the merge arena and its collectives are as before */
+#define GYSK_FLAG_MERGE_STATES		0x4u	/* the merge step also rolls up the listener states of the member services into each
+						   logical service (LISTEN_SUMM_STATS per logical service: gysk_query_logical_states,
+						   GYSK_TOPN_ISSUE of gysk_topn_logical); with or without GYSK_FLAG_MERGE_LEVELS, the
+						   same flags on every rank. Without it the merge arena and its collectives are as before */
 
 typedef struct gysk_config
 {
@@ -552,7 +556,8 @@ int		gysk_nccl_comm_init(gysk_engine *e, const uint8_t uid[GYSK_NCCL_UNIQUE_ID_B
 int		gysk_merge_global(gysk_engine *e, void *nccl_comm);
 /* One gysk_svc_summary per logical id from the last finished merge: glob_id = the logical id, found = 0 for an id not in the map.
  * The merge always folds the last closed window, the all-time histogram, the connection counters, the HLL registers and the
- * t-digest. curr_state, curr_issue, issue_bit_hist and high_resp_bit_hist are always 0: listener states are not merged.
+ * t-digest. curr_state, curr_issue, issue_bit_hist and high_resp_bit_hist are always 0: a logical service is not classified (its
+ * members' states are counted by gysk_query_logical_states with GYSK_FLAG_MERGE_STATES).
  * Without GYSK_FLAG_MERGE_LEVELS nqrys_5min, nqrys_5day, nconns_active, active_kbytes, max_rtt_msec, cli_errors and ser_errors
  * are 0, and p95_5min_resp_ms, p99_5min_resp_ms and p95_5day_resp_ms -1 (the percentiles of an empty histogram).
  * With it those fields are the member services' own, merged exactly at any GPU count:
@@ -585,8 +590,9 @@ int		gysk_query_logical_all(gysk_engine *e, uint32_t flags, gysk_svc_summary *ou
 /* The n <= 64 best logical services of the last finished merge, best first: the global half of the per-host listener rankings
  * (SURVEY.md §8f row 3). Scores as gysk_topn_svcs scores a service, from the merged arrays: GYSK_TOPN_QPS the last window's response
  * samples, GYSK_TOPN_CONNS / GYSK_TOPN_NET its connection events / kbytes (nconns_5s / kbytes_5s of the row), GYSK_TOPN_ACTIVE the
- * merged active connections (nconns_active; GYSK_FLAG_MERGE_LEVELS, GYSK_ERR_NOTSUP without it). GYSK_TOPN_ISSUE is GYSK_ERR_INVAL:
- * logical services have no listener state. Equal scores rank the later logical service of the map (first appearance) first. As in
+ * merged active connections (nconns_active; GYSK_FLAG_MERGE_LEVELS, GYSK_ERR_NOTSUP without it). GYSK_TOPN_ISSUE ranks by the member
+ * listeners in BAD / SEVERE / DOWN (nsvc_issue of gysk_query_logical_states) with GYSK_FLAG_MERGE_STATES, and is GYSK_ERR_INVAL without
+ * it. Equal scores rank the later logical service of the map (first appearance) first. As in
  * gysk_topn_svcs, entries with a zero score are left out, so *nout may be below n. glob_id = the logical id, host_idx = 0.
  * GYSK_ERR_NOSPC for a map of more logical services than max(max_batch, max(max_svcs, max_tasks) + 1). */
 int		gysk_topn_logical(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, uint32_t *nout);
@@ -599,6 +605,25 @@ int		gysk_export_logical_tdigest(gysk_engine *e, uint64_t logical_id, double *me
 int		gysk_export_logical_tdigest_pgtext(gysk_engine *e, uint64_t logical_id, char *buf, uint32_t cap);
 int		gysk_query_logical_quantiles(gysk_engine *e, uint64_t logical_id, const double *qs, uint32_t nq, double *out);
 int		gysk_export_logical_hll(gysk_engine *e, uint64_t logical_id, uint8_t *regs /* 1 << hll_p bytes */);
+
+/* ---- listener states of logical services (GYSK_FLAG_MERGE_STATES): how many instances of a service are in trouble ----
+ * Each member service that holds a slot on a rank adds LISTEN_SUMM_STATS::update (server/gy_msocket.h:853-864) of the
+ * LISTENER_STATE_NOTIFY record gysk_encode_listener_state writes from its own gysk_query_svcs row: nstates[curr_state] += 1,
+ * tot_qps += nqrys_5s / 5, tot_act_conn += nconns_active, tot_kb_inbound += kbytes_5s, tot_kb_outbound += 0, tot_ser_errors += ser_errors,
+ * nlisteners += 1, nactive += !!nqrys_5s; summed over members and ranks with LISTEN_SUMM_STATS<int>'s wrap-around, so exact at any GPU
+ * count. The states are those of each member's last gysk_flush on its rank. A logical service itself is not classified. */
+typedef struct gysk_logical_state
+{
+	uint64_t		logical_id;
+	int32_t			found;		/* 0: not in the map (summ all zero) */
+	uint32_t		nsvc_issue;	/* summ.nstates[BAD] + [SEVERE] + [DOWN], as MS_CLUSTER_STATE counts it */
+	gysk_host_summary	summ;		/* LISTEN_SUMM_STATS over the member listeners, every rank */
+} gysk_logical_state;			/* 80 bytes */
+/* by id, from the last finished merge. GYSK_ERR_NOTSUP without GYSK_FLAG_MERGE_STATES, GYSK_ERR_INVAL before a finished merge */
+int		gysk_query_logical_states(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_logical_state *out);
+/* one row per logical service: the ids, order, GYSK_WINDOW_ACTIVE_ONLY set and count / capacity rules of gysk_query_logical_all */
+int		gysk_query_logical_states_all(gysk_engine *e, uint32_t flags, gysk_logical_state *out, uint32_t cap, uint32_t *n);
+
 int		gysk_query_flows_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_est *out);
 
 /* per-kernel device timing (CUDA events on the launching stream around the ingest kernel and around the sort +
