@@ -211,6 +211,22 @@ __device__ __forceinline__ int bucket_duration(int data)				// DURATION_HASH :18
 	return b;
 }
 
+// Ordered compaction in one 1024-thread CTA that walks its input in tiles of 1024 entries, every thread calling once per tile: a
+// block-wide ballot scan ranks the kept entries, and each thread whose entry is kept calls f(its rank among all entries kept so far).
+// wcnt is the CTA's __shared__ uint32_t[32]; running = the entries the earlier tiles kept, advanced by this tile's.
+template <typename F> __device__ __forceinline__ void tile_rank(bool keep, uint32_t *wcnt, uint32_t &running, F f)
+{
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const unsigned b = __ballot_sync(0xffffffffu, keep);
+	if (lane == 0) wcnt[wid] = __popc(b);
+	__syncthreads();
+	uint32_t before = 0, total = 0;
+	for (int w = 0; w < 32; ++w) { const uint32_t c = wcnt[w]; before += w < wid ? c : 0; total += c; }
+	if (keep) f(running + before + __popc(b & ((1u << lane) - 1u)));
+	running += total;
+	__syncthreads();
+}
+
 // ---------------------------------------------------------------------------------------------------
 // memory helpers
 // ---------------------------------------------------------------------------------------------------

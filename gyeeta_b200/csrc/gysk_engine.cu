@@ -272,6 +272,22 @@ void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint6
 	*maxv = m;
 }
 
+void level_from_cells(const HistCell *cells, gysk_hist_serial *out, uint64_t *total, int64_t *maxv)
+{
+	hist_from_cells(cells, 15, out, total, maxv, false);
+	if (*total == 0) *maxv = INT64_MIN;
+}
+
+int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_t *weights, uint32_t cap, uint32_t *n, double *minv, double *maxv)
+{
+	const uint32_t nc = std::min<uint32_t>(std::min<uint32_t>(head.n, TD_CAP), cap);
+	for (uint32_t c = 0; c < nc; ++c) { means[c] = cent[c].mean; weights[c] = cent[c].weight; }
+	*n = nc;
+	if (minv) *minv = head.minv;
+	if (maxv) *maxv = head.maxv;
+	return head.n > cap ? GYSK_ERR_NOSPC : GYSK_OK;
+}
+
 } // namespace gysk
 
 namespace {
@@ -1307,11 +1323,7 @@ int gysk_export_hist(gysk_engine *e, uint64_t id, int which, gysk_hist_serial ou
 	if (int rc = stage_svc_raw(e, id)) return rc;
 	const SvcRaw &r = *reinterpret_cast<const SvcRaw *>(e->h_wstage);
 	if (!r.found) return GYSK_ERR_NOENT;
-	if (which == GYSK_HIST_RESP_5MIN || which == GYSK_HIST_RESP_5DAY) {
-		hist_from_cells(r.lvl[which - GYSK_HIST_RESP_5MIN], 15, out, total, maxv, false);
-		if (*total == 0) *maxv = INT64_MIN;
-		return GYSK_OK;
-	}
+	if (which == GYSK_HIST_RESP_5MIN || which == GYSK_HIST_RESP_5DAY) { level_from_cells(r.lvl[which - GYSK_HIST_RESP_5MIN], out, total, maxv); return GYSK_OK; }
 	if (which == GYSK_HIST_QPS) { hist_from_cells(r.qps, 15, out, total, maxv, true); return GYSK_OK; }
 	if (which == GYSK_HIST_ACTIVE_CONN) { hist_from_cells(r.act, 14, out, total, maxv, true); return GYSK_OK; }
 	hist_from_cells(which == GYSK_HIST_RESP_CUR ? r.cur : (which == GYSK_HIST_RESP_LAST ? r.last : r.all), 15, out, total, maxv, false);
@@ -1370,12 +1382,7 @@ int gysk_export_tdigest(gysk_engine *e, uint64_t id, double *means, uint64_t *we
 	if (int rc = stage_svc_raw(e, id)) return rc;
 	const SvcRaw &r = *reinterpret_cast<const SvcRaw *>(e->h_wstage);
 	if (!r.found) return GYSK_ERR_NOENT;
-	const uint32_t nc = std::min<uint32_t>(std::min<uint32_t>(r.td.n, TD_CAP), cap);
-	for (uint32_t c = 0; c < nc; ++c) { means[c] = r.cent[c].mean; weights[c] = r.cent[c].weight; }
-	*n = nc;
-	if (minv) *minv = r.td.minv;
-	if (maxv) *maxv = r.td.maxv;
-	return r.td.n > cap ? GYSK_ERR_NOSPC : GYSK_OK;
+	return tdigest_out(r.td, r.cent, means, weights, cap, n, minv, maxv);
 }
 
 // Summary encoder (SURVEY §8f-2, output side): per-service summaries -> one NOTIFY_LISTENER_STATE message body, i.e. the records

@@ -141,12 +141,31 @@ struct LogicalArrays
 	__host__ __device__ __forceinline__ uint8_t *hll_of(uint32_t l, uint32_t hll_p) const { return hll + ((size_t)l << hll_p); }
 };
 
+// The members of each logical service on this GPU, CSR in map order: slots[offs[l] .. offs[l + 1]) are logical l's. A member whose id
+// holds no slot here is written as null_slot (resolve_members_kernel): the engine's null slot max_svcs, which every fold skips.
+struct Members
+{
+	uint32_t		*offs {nullptr}, *slots {nullptr};
+	uint32_t		null_slot {0};
+
+	// f(slot) for each member of logical l that holds a slot, in map order. The walk only reads the map: __restrict__ lets its loads
+	// take the read-only path.
+	template <typename F> __device__ __forceinline__ void each(uint32_t l, F f) const
+	{
+		const uint32_t *__restrict__ o = offs, *__restrict__ sl = slots;
+		for (uint32_t m = o[l]; m < o[l + 1]; ++m) {
+			const uint32_t s = sl[m];
+			if (s != null_slot) f(s);
+		}
+	}
+};
+
 // per-logical-service state of the merge step (SURVEY.md §8e)
 struct MergeState
 {
 	std::vector<uint64_t>	logical_ids;		// dense index -> logical id
 	std::unordered_map<uint64_t, uint32_t> index;	// logical id -> dense index
-	uint32_t		*d_offsets {nullptr}, *d_members {nullptr};	// CSR: logical -> member slots on this GPU
+	Members			members;
 	unsigned long long	*d_member_ids {nullptr};			// id each member slot held when the map was set
 	unsigned long long	*d_logical_ids {nullptr};			// [nl] logical_ids on the device: the ids of the rows and top-N entries
 	int32_t			*d_sorted {nullptr};				// [nl] dense indices by ascending logical id (gysk_query_logical_all)
@@ -158,6 +177,7 @@ struct MergeState
 	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux] [, states]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt, flush tsec]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
+	std::string		name_sum, name_maxi64, name_maxu8;	// the regions' gysk_buffer_desc names: their arrays, in order
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
 	LogicalArrays		lg;
 	bool			prepared {false}, finished {false};
@@ -248,6 +268,10 @@ int tdigest_pgtext(gysk_engine *e, uint64_t id, ExportTd export_td, char *buf, u
 int tdigest_quantiles(gysk_engine *e, uint64_t id, ExportTd export_td, const double *qs, uint32_t nq, double *out);
 // HIST_SERIAL of 16 cells (cell HIST_MAX_CELL holds max_val_seen_ in .sum); total = the sum of the first nb counts
 void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint64_t *total, int64_t *maxv, bool t_is_int);
+// a 5-minute or 5-day level as gysk_export_hist answers it: hist_from_cells, and maxv = INT64_MIN while the level is empty
+void level_from_cells(const HistCell *cells, gysk_hist_serial *out, uint64_t *total, int64_t *maxv);
+// the gysk_export_tdigest answer of one digest: up to min(cap, TD_CAP) centroids, min and max; GYSK_ERR_NOSPC when it has more than cap
+int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_t *weights, uint32_t cap, uint32_t *n, double *minv, double *maxv);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)

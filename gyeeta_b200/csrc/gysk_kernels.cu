@@ -1685,33 +1685,23 @@ __global__ void host_listen_count_kernel(DevState st, const unsigned long long *
 }
 
 // One CTA walks the keys in order and writes the row of every host run whose rank lies in [rlo, rlo + cap): {host, run length, issue,
-// severe}; *d_rows = number of runs. A block-wide ballot scan ranks the run heads of each 1024-key tile.
+// severe}; *d_rows = number of runs. tile_rank ranks the run heads of each 1024-key tile.
 __global__ void __launch_bounds__(1024) host_listen_rows_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *d_n,
 		const unsigned long long *__restrict__ acc, uint32_t rlo, uint32_t cap, gysk_host_listen *__restrict__ out, unsigned long long *d_rows)
 {
 	__shared__ uint32_t wcnt[32];
 	const uint32_t n = (uint32_t)*d_n;
-	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 	uint32_t running = 0;
 
 	for (uint32_t t = 0; t < n; t += 1024) {
 		const uint32_t i = t + threadIdx.x;
 		const uint32_t h = i < n ? (uint32_t)(keys[i] >> 32) : 0;
 		const bool head = i < n && (i == 0 || (uint32_t)(keys[i - 1] >> 32) != h);
-		const unsigned b = __ballot_sync(0xffffffffu, head);
-		if (lane == 0) wcnt[wid] = __popc(b);
-		__syncthreads();
-		uint32_t before = 0, total = 0;
-		for (int w = 0; w < 32; ++w) { const uint32_t c = wcnt[w]; before += w < wid ? c : 0; total += c; }
-		if (head) {
-			const uint32_t r = running + before + __popc(b & ((1u << lane) - 1u));
-			if (r >= rlo && r - rlo < cap) {
-				const unsigned long long a = acc[i];
-				out[r - rlo] = gysk_host_listen {h, host_bound(keys, i + 1, n, h, true) - i, (uint32_t)(a >> 32), (uint32_t)a};
-			}
-		}
-		running += total;
-		__syncthreads();
+		tile_rank(head, wcnt, running, [&](uint32_t r) {
+			if (r < rlo || r - rlo >= cap) return;
+			const unsigned long long a = acc[i];
+			out[r - rlo] = gysk_host_listen {h, host_bound(keys, i + 1, n, h, true) - i, (uint32_t)(a >> 32), (uint32_t)a};
+		});
 	}
 	if (threadIdx.x == 0) *d_rows = running;
 }

@@ -398,20 +398,21 @@ class Engine:
         self._chk(self.L.gysk_encode_listener_state(out, len(ids), buf, len(buf), C.byref(nrecs), C.byref(nbytes)))
         return nrecs.value, buf.raw[: nbytes.value]
 
-    def _window(self, fn, row_type, host_idx, active_only, cap):
+    def _window(self, fn, row_type, args, active_only, cap):
+        """fn(h, *args, flags, out, cap, &n): (rows, number of matching rows); cap None = a count call first, then every row"""
         flags = WINDOW_ACTIVE_ONLY if active_only else 0
         n = C.c_uint32()
         if cap is None:
-            self._chk(fn(self.h, host_idx, flags, None, 0, C.byref(n)))
+            self._chk(fn(self.h, *args, flags, None, 0, C.byref(n)))
             cap = n.value
         out = (row_type * max(cap, 1))()
-        self._chk(fn(self.h, host_idx, flags, out if cap else None, cap, C.byref(n)))
+        self._chk(fn(self.h, *args, flags, out if cap else None, cap, C.byref(n)))
         return out[: min(cap, n.value)], n.value
 
     def query_window(self, host_idx=-1, active_only=False, cap=None):
         """gysk_query_window: (SvcSummary rows grouped by host, ids ascending within a host; number of matching rows).
         cap None = all rows (a count call first); 0 = the count only"""
-        return self._window(self.L.gysk_query_window, SvcSummary, host_idx, active_only, cap)
+        return self._window(self.L.gysk_query_window, SvcSummary, (host_idx,), active_only, cap)
 
     def query_window_hosts(self, host_idx=-1, active_only=False, cap=None):
         """gysk_query_window_hosts: (rows, host_idx of each row as a uint32 array, number of matching rows)"""
@@ -457,7 +458,7 @@ class Engine:
 
     def query_task_window(self, host_idx=-1, active_only=False, cap=None):
         """gysk_query_task_window: (TaskSummary rows in the order of query_window, number of matching rows)"""
-        return self._window(self.L.gysk_query_task_window, TaskSummary, host_idx, active_only, cap)
+        return self._window(self.L.gysk_query_task_window, TaskSummary, (host_idx,), active_only, cap)
 
     def query_flows(self, keys, last_window=False):
         keys = np.ascontiguousarray(keys, dtype=np.uint64)
@@ -632,14 +633,7 @@ class Engine:
     def query_logical_all(self, active_only=False, cap=None):
         """gysk_query_logical_all: (SvcSummary rows of the merged logical services in ascending logical id, number of matching rows).
         cap None = all rows (a count call first); 0 = the count only"""
-        flags = WINDOW_ACTIVE_ONLY if active_only else 0
-        n = C.c_uint32()
-        if cap is None:
-            self._chk(self.L.gysk_query_logical_all(self.h, flags, None, 0, C.byref(n)))
-            cap = n.value
-        out = (SvcSummary * max(cap, 1))()
-        self._chk(self.L.gysk_query_logical_all(self.h, flags, out if cap else None, cap, C.byref(n)))
-        return out[: min(cap, n.value)], n.value
+        return self._window(self.L.gysk_query_logical_all, SvcSummary, (), active_only, cap)
 
     def topn_logical(self, metric, n=10):
         """gysk_topn_logical: [(logical id, score, 0)] of the n best logical services of the last merge, best first"""
@@ -670,14 +664,7 @@ class Engine:
 
     def query_logical_states_all(self, active_only=False, cap=None):
         """gysk_query_logical_states_all: (LogicalState rows in ascending logical id, number of matching rows); cap as query_logical_all"""
-        flags = WINDOW_ACTIVE_ONLY if active_only else 0
-        n = C.c_uint32()
-        if cap is None:
-            self._chk(self.L.gysk_query_logical_states_all(self.h, flags, None, 0, C.byref(n)))
-            cap = n.value
-        out = (LogicalState * max(cap, 1))()
-        self._chk(self.L.gysk_query_logical_states_all(self.h, flags, out if cap else None, cap, C.byref(n)))
-        return out[: min(cap, n.value)], n.value
+        return self._window(self.L.gysk_query_logical_states_all, LogicalState, (), active_only, cap)
 
     def merge_flush_range(self):
         """gysk_merge_flush_range: (earliest, latest) tsec of the ranks' last flush, as the last merge all-reduced them"""

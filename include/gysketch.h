@@ -331,7 +331,7 @@ typedef struct gysk_stats
 enum { GYSK_RED_SUM_U64 = 0, GYSK_RED_MAX_U8 = 1, GYSK_RED_MAX_I64 = 2 };
 typedef struct gysk_buffer_desc
 {
-	const char	*name;
+	const char	*name;			/* name and dptr stay valid until the next gysk_set_logical_map */
 	void		*dptr;			/* device pointer */
 	uint64_t	nbytes;
 	int32_t		redop;			/* GYSK_RED_* */

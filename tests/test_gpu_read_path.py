@@ -1,7 +1,9 @@
 """The read path: every read of the engine goes through one device stage and one page-locked stage. Two things must hold.
 
-1. Each read issues a fixed number of kernel launches: one per 1024-id piece of a by-id read, one per single-id export, and for the
-   window reads the list-and-sort launches plus one per 8192 rows (bench.py reports kernel_launches).
+1. Each read issues a fixed number of kernel launches: one per 1024-id piece of a by-id read, one per single-id export (none for the
+   merged logical services' exports, which copy from the merge arena), and for the window reads the list-and-sort launches plus one
+   per 8192 rows; the reads over every logical service take one select launch under ACTIVE_ONLY, then one per 8192 rows (bench.py
+   reports kernel_launches).
 2. No read sees what another read left in the stage: every read, interleaved with all the others, answers what it answers when the
    reads run in another order on a second engine fed the same stream (top-N up to the order of tied entries), and an unknown id
    gives None or the not-found row."""
@@ -27,9 +29,10 @@ TOPN_LAUNCHES = 7
 
 
 def _engine(seed):
-    """services, processes and flows over two windows, the first one closed; a world-1 merge of the services into logical ids"""
+    """services, processes and flows over two windows, the first one closed; a world-1 merge of the services into logical ids, with
+    their listener states"""
     rng = np.random.default_rng(seed)
-    eng = ge.Engine(max_svcs=1 << 14, max_tasks=1 << 12)
+    eng = ge.Engine(max_svcs=1 << 14, max_tasks=1 << 12, merge_states=True)
     svc_ids = (rng.choice(1 << 40, 1500, replace=False) + 1).astype(np.uint64)
     task_ids = (rng.choice(1 << 40, 1200, replace=False) + (1 << 41)).astype(np.uint64)
     ev = _stream(rng, svc_ids, task_ids, 60000)
@@ -74,6 +77,7 @@ def test_launch_counts_of_every_read():
         assert _launches(eng, lambda: eng.query_flows(flows[:n])) == pieces, n
         assert _launches(eng, lambda: eng.query_flows_global(flows[:n])) == pieces, n
         assert _launches(eng, lambda: eng.query_logical(np.resize(logical, n))) == pieces, n
+        assert _launches(eng, lambda: eng.query_logical_states(np.resize(logical, n))) == pieces, n
         fresh = rng.choice(1 << 40, n, replace=False).astype(np.uint64) + (1 << 43)
         assert _launches(eng, lambda: eng.register_ids(fresh)) == pieces, n
         # window reads: n rows wanted (cap), the table holds more than 1000
@@ -88,6 +92,19 @@ def test_launch_counts_of_every_read():
     for id_ in (int(task_ids[0]), 0xDEAD0001):
         assert _launches(eng, lambda: eng.export_hist(id_, ge.HIST_TASK_CPU_DELAY)) == 1
     assert _launches(eng, lambda: eng.topn(ge.TOPN_QPS)) == TOPN_LAUNCHES
+    # every logical service: the select kernel under ACTIVE_ONLY, then one row launch per 8192 rows
+    for cap in (0, 5, len(logical)):
+        for active in (False, True):
+            for read in (eng.query_logical_all, eng.query_logical_states_all):
+                rows = read(active_only=active, cap=len(logical))[1]
+                assert rows > 5
+                assert _launches(eng, lambda: read(active_only=active, cap=cap)) == active + math.ceil(min(cap, rows) / WIN_ROWS), (read, cap, active)
+    for metric in (ge.TOPN_QPS, ge.TOPN_ISSUE):
+        assert _launches(eng, lambda: eng.topn_logical(metric)) == TOPN_LAUNCHES, metric
+    for id_ in (int(logical[0]), 0xDEAD0001):
+        assert _launches(eng, lambda: eng.export_logical_hist(id_, ge.HIST_RESP_ALL)) == 0
+        assert _launches(eng, lambda: eng.export_logical_tdigest(id_)) == 0
+        assert _launches(eng, lambda: eng.export_logical_hll(id_)) == 0
     assert _launches(eng, lambda: eng.topn_tasks(0)) == TOPN_LAUNCHES
     eng.close()
 
@@ -130,6 +147,7 @@ def _round(eng, k, svc_ids, task_ids, logical, flows, unknown):
     tmix = np.concatenate([task_ids[k * 200: k * 200 + 500], unknown[: 300], np.zeros(30, dtype=np.uint64)])
     keys = np.concatenate([flows[k * 500: k * 500 + 1500], unknown[: 200]])
     lmix = np.concatenate([logical, unknown[: 40]])
+    lid = int(logical[k]) if k % 2 == 0 else int(unknown[k])
     return [
         ("export_hist", sid, lambda: eng.export_hist(sid, ge.HIST_RESP_ALL)),
         ("export_task_hist", tid, lambda: eng.export_hist(tid, ge.HIST_TASK_CPU_PCT + k % 3)),
@@ -146,6 +164,13 @@ def _round(eng, k, svc_ids, task_ids, logical, flows, unknown):
         ("query_window", None, lambda: eng.query_window(active_only=bool(k & 1))),
         ("query_task_window", None, lambda: eng.query_task_window(host_idx=k)),
         ("query_logical", None, lambda: _raw_rows(eng, L.gysk_query_logical, lmix, ge.SvcSummary)),
+        ("query_logical_all", None, lambda: eng.query_logical_all(active_only=bool(k & 1))),
+        ("query_logical_states", None, lambda: _raw_rows(eng, L.gysk_query_logical_states, lmix, ge.LogicalState)),
+        ("query_logical_states_all", None, lambda: eng.query_logical_states_all(active_only=bool(k & 2))),
+        ("topn_logical", None, lambda: eng.topn_logical(k % 4, n=20)),
+        ("export_logical_hist", lid, lambda: eng.export_logical_hist(lid, ge.HIST_RESP_LAST + k % 2)),
+        ("export_logical_tdigest", lid, lambda: eng.export_logical_tdigest(lid)),
+        ("export_logical_hll", lid, lambda: eng.export_logical_hll(lid)),
     ]
 
 
@@ -183,6 +208,11 @@ def test_interleaved_reads_equal_the_same_reads_in_another_order():
                     assert bytes(r) == bytes(ge.SvcSummary(glob_id=r.glob_id, td_p50_us=NAN, td_p95_us=NAN, td_p99_us=NAN)), (k, name)
                 else:
                     assert r.found == 1, (k, name, hex(r.glob_id))
+        for r in interleaved[(k, "query_logical_states")]:
+            if r.logical_id not in live:
+                assert bytes(r) == bytes(ge.LogicalState(logical_id=r.logical_id)), k
+            else:
+                assert r.found == 1, (k, hex(r.logical_id))
         tlive = set(task_ids.tolist())
         for r in interleaved[(k, "query_tasks")]:
             if r.aggr_task_id not in tlive:
