@@ -1447,7 +1447,10 @@ int gysk_tdigest_to_pgtext(const double *means, const uint64_t *weights, uint32_
 
 // The engine keeps delta = 200 internally; the Postgres side of the reference aggregates with public.tdigest(expr, 100)
 // (common/gy_query_common.cc:1855) and the extension refuses to combine digests of different compression, so the export is one
-// more fixed-grid K_1 compress at compression 100 (host side, same rule as the device).
+// more fixed-grid K_1 compress at compression 100 (host side). Each centroid goes to the cell that holds its start: the export
+// compresses a finished digest once, and a cluster widened by one last item (a delta = 200 centroid, half a cell here) stays
+// within the accuracy the export is tested to (tests/test_gpu_td_accuracy.py). The device's centre rule (gysk_tdigest.cuh) is
+// there for the repeated merges, where the start rule's widening compounds.
 static uint32_t host_td_compress(const double *means, const uint64_t *w, uint32_t n, uint32_t delta, double *om, uint64_t *ow)
 {
 	if (!n) return 0;

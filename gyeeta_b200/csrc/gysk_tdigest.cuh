@@ -9,11 +9,14 @@ namespace gysk {
 // K_1 scale function of the merging t-digest (Dunning), k spanning [-delta/2, delta/2]: k(q) = delta/pi asin(2q - 1). The compress
 // step works on the FIXED unit grid of k: cell j = [q_j, q_j+1) with q_j = q(k = -delta/2 + j) = (sin(pi (j/delta - 1/2)) + 1)/2. In
 // weight units cell j starts at T_j = (uint64) (q_j * W) (W = total weight, one double multiply, truncated), and an item of the
-// merged list (sorted by mean, exclusive weight prefix P_i) belongs to the cell that holds its START: T_j <= P_i < T_j+1. All items
-// of one cell become one cluster: at most delta clusters, each no wider than one unit of k plus its last item — the t-digest size
-// bound — with no data-dependent chain: the first item of cell j is lower_bound(P, T_j), delta independent binary searches over
-// the prefix array, which is what makes the step parallel. q_j is computed once on the host (libm sin, same expression in
-// oracle/gysk_oracle.c) so that device, host and oracle use identical doubles.
+// merged list (sorted by mean, exclusive weight prefix P_i, weight w_i) belongs to the cell that holds its weight CENTRE:
+// T_j <= P_i + w_i / 2 < T_j+1. All items of one cell become one cluster: at most delta clusters, each reaching past its cell by at
+// most half of its first and half of its last item — the t-digest size bound — with no data-dependent chain: the first item of
+// cell j is the first i with 2 P_i + w_i >= 2 T_j, i.e. (integers) with C_i = P_i + floor(w_i / 2) >= T_j — C grows with i and
+// never exceeds the total, so no sum overflows — delta independent binary searches over C, which is what makes the step parallel. The centre and not the start: old centroids are items of every later compress, and a start-rule cluster takes its
+// whole last item, so a digest fed through many batches widened with each one and kept far fewer than delta centroids (DESIGN.md
+// §2). q_j is computed once on the host (libm sin, same expression in oracle/gysk_oracle.c) so that device, host and oracle use
+// identical doubles.
 struct TdParams { const double *qtab; uint32_t delta; uint32_t pad; };		// qtab[0 .. delta], device memory
 
 template <int NMAX_>
@@ -89,8 +92,10 @@ __device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid 
 		if (lane == 0) S.pref[0] = 0;
 	}
 	__syncwarp();
+	// the cell-search key of item i, its weight centre rounded down: C_i = P_i + floor(w_i / 2)
+	auto ckey = [&S](uint32_t i) { const unsigned long long p = S.pref[i]; return p + ((S.pref[i + 1] - p) >> 1); };
 
-	// first item of every cell: lower_bound of the cell's start weight in the prefix array; empty cells drop out
+	// first item of every cell: the first item whose weight centre is at or past the cell's start; empty cells drop out
 	uint32_t nout = 0;
 	if (nm) {
 		const unsigned long long Wt = S.pref[nm];
@@ -101,12 +106,12 @@ __device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid 
 		uint32_t lo = 0;
 		for (uint32_t j = lane * cj, jn = 0; jn < cj && j <= P.delta; ++j, ++jn) {
 			const unsigned long long T = j == P.delta ? Wt : (unsigned long long)__dmul_rn(__ldg(P.qtab + j), W);
-			// first i in [0, nm) with pref[i] >= T, nm if none
+			// first i in [0, nm) with ckey(i) >= T (its weight centre at or past T), nm if none
 			uint32_t steps = jn ? 0u : 8u;
-			while (steps < 8u && lo < nm && S.pref[lo] < T) { ++lo; ++steps; }
+			while (steps < 8u && lo < nm && ckey(lo) < T) { ++lo; ++steps; }
 			if (steps == 8u) {
 				uint32_t hi = nm;
-				while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (S.pref[mid] < T) lo = mid + 1; else hi = mid; }
+				while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (ckey(mid) < T) lo = mid + 1; else hi = mid; }
 			}
 			S.nxt[j] = (uint16_t)lo;
 		}

@@ -343,8 +343,11 @@ double gyo_hll_estimate(const uint8_t *regs, uint32_t p)
  * produce the same bits. */
 /* The compress step works on the FIXED unit grid of k: cell j = [q_j, q_j+1), q_j = q(k = -delta/2 + j) = (sin(pi (j/delta - 1/2)) + 1)/2.
  * In weight units cell j starts at T_j = (uint64) (q_j * W); an item of the merged list (sorted by mean; exclusive weight prefix
- * P_i, total W) belongs to the cell that holds its start: T_j <= P_i < T_j+1; all items of one cell become one cluster: at most delta clusters, each no wider than one unit of k plus its
- * last item (the t-digest size bound), and no data-dependent chain — every item finds its cell on its own. The table is
+ * P_i, weight w_i, total W) belongs to the cell that holds its weight centre: T_j <= P_i + w_i / 2 < T_j+1; all items of one cell
+ * become one cluster: at most delta clusters, each reaching past its cell by at most half of its first and half of its last item
+ * (the t-digest size bound), and no data-dependent chain — every item finds its cell on its own. The centre, not the start: once
+ * old centroids are items of the next compress, a start-rule cluster grows by its whole last item at every merge, so a digest fed
+ * through many batches widens and loses centroids; with the centre an old centroid that fits a cell stays in it. The table is
  * computed with libm by this expression here and in gyeeta_b200/csrc/gysk_engine.cu (same host, same bits). */
 #define GYO_TD_MAX_DELTA	256
 static void td_qtab(double delta, double *qtab /* [delta + 1] */)
@@ -361,7 +364,7 @@ void gyo_td_init(gyo_tdigest *t)
 	t->minv = INFINITY; t->maxv = -INFINITY;
 }
 
-/* cell j starts at weight T_j = (uint64) (q_j * W); an item belongs to the cell that holds its start position (exclusive prefix);
+/* cell j starts at weight T_j = (uint64) (q_j * W); an item belongs to the cell that holds its weight centre P_i + w_i / 2;
  * cluster mean = sum(mean * weight) / sum(weight), accumulated in double in input order */
 uint32_t gyo_td_compress(const gyo_centroid *in, uint32_t n, double delta, gyo_centroid *out, uint32_t cap)
 {
@@ -378,8 +381,11 @@ uint32_t gyo_td_compress(const gyo_centroid *in, uint32_t n, double delta, gyo_c
 	for (uint32_t i = 0; i < n; ++i) {
 		uint32_t c = cell;
 
-		/* advance to the cell that holds pref: T_c <= pref < T_c+1 (T_d = W) */
-		while (c + 1 < d && (uint64_t)(qtab[c + 1] * (double)W) <= pref) ++c;
+		/* advance to the cell that holds the item's centre: T_c <= pref + w / 2 < T_c+1 (T_d = W). For integers 2 pref + w >= 2 T
+		 * iff pref + floor(w / 2) >= T, a key that never exceeds W (2 T would overflow near the largest totals) */
+		const uint64_t ckey = pref + in[i].weight / 2;
+
+		while (c + 1 < d && (uint64_t)(qtab[c + 1] * (double)W) <= ckey) ++c;
 		if (i && c != cell) {
 			if (nout < cap) { out[nout].mean = csum / (double)cw; out[nout].weight = cw; }
 			nout++;

@@ -173,7 +173,7 @@ if world > 1:
 
 # t-digest of the merged logical services against the exact quantiles of their samples (the three busiest logical services)
 hot = np.argsort(-tot)[:3]
-tdrows = []
+tdrows, td_bad = [], 0
 for k in hot:
     members = torch.from_numpy(ids[my_logical == k].view(np.int64)).to(dev)
     vals = torch.cat([(b_[:, 2][torch.isin(b_[:, 0], members) & (((b_[:, 3] >> 32) & 0xFFFF) == 5)] & 0xFFFFFFFF) for b_ in batches]).to(torch.int32)
@@ -190,7 +190,16 @@ for k in hot:
         ex = torch.quantile(vals[: 16_000_000].double(), torch.tensor([0.5, 0.95, 0.99], device=dev, dtype=torch.float64), interpolation="lower").cpu().numpy()
         s = gq[int(k)]
         got = np.array([s["td_p50_us"], s["td_p95_us"], s["td_p99_us"]])
-        tdrows.append({"logical": int(k) + 1, "samples": int(vals.numel()), "rel_err_p50_p95_p99": (np.abs(got - ex) / ex).tolist()})
+        # rank error: distance of q from [#{v < g}, #{v <= g}] / n; bound: two K_1 cells at q plus 1 / n (tests/test_gpu_td_accuracy.py)
+        n_ = vals.numel()
+        rk, bd = [], []
+        for q, g in zip((0.5, 0.95, 0.99), got.tolist()):
+            lo, hi = int((vals < g).sum()) / n_, int((vals <= g).sum()) / n_
+            rk.append(max(0.0, lo - q, q - hi))
+            bd.append(2.0 * (np.pi / 200) * np.sqrt(q * (1.0 - q)) + 1.0 / n_)
+        td_bad += int(any(r > b for r, b in zip(rk, bd)))
+        tdrows.append({"logical": int(k) + 1, "samples": int(n_), "rel_err_p50_p95_p99": (np.abs(got - ex) / ex).tolist(),
+                       "rank_err_p50_p95_p99": rk, "rank_bound": bd})
 
 if rank == 0:
     total = per_rank * world
@@ -207,7 +216,7 @@ if rank == 0:
         "parity": {"logical_services_checked": int(tb[1]), "mismatches": int(tb[0]),
                    "fields": "found, nqrys_5s, total_resp_5sec, max_resp_ms, nconns_5s, kbytes_5s, td_count, distinct_clients (HLL estimate of the "
                              "max-merged registers), p95/p99/p25 via the reference's get_percentiles on the summed histogram"},
-        "tdigest_vs_exact_hot_logical": tdrows}))
+        "tdigest_vs_exact_hot_logical": tdrows, "tdigest_rank_bound_exceeded": td_bad}))
 if world > 1:
     dist.destroy_process_group()
-sys.exit(0 if int(tb[0]) == 0 else 1)
+sys.exit(0 if int(tb[0]) == 0 and td_bad == 0 else 1)

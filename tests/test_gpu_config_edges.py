@@ -172,7 +172,7 @@ def _td_equal(eng, orc, id_, ctx):
     return len(ow)
 
 
-def test_td_lists_across_the_shared_memory_limit():
+def test_td_lists_across_the_shared_memory_limit_k1_centres():
     """bins_merge_kernel merges a service's old centroids with its batch items in shared memory while head.n + nitems <= 384
     (TD_SMEM_N) and in the L2 scratch (TdWorkBig, 1120 entries) above that. One service brings exactly 384 - head.n distinct value
     bins, another 385 - head.n; at delta = 256 a third brings every bin a response time can reach (841 of the NBINS = 848) on top of

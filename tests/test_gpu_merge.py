@@ -4,6 +4,7 @@ merged logical-service answers must equal (integers: bit-exact) a single engine 
 import numpy as np
 import pytest
 
+from tests.test_gpu_td_accuracy import rank_bound, rank_error
 from tests.util import td_p99_tolerance
 
 from gyeeta_b200 import dist as gd
@@ -37,11 +38,13 @@ def _emulate_collectives(torch, engines):
         e.merge_finish(gathered.data_ptr(), len(engines))
 
 
-def test_two_shards_merge_to_global_answers():
+def test_two_shards_merge_to_global_answers_and_exact_quantiles():
     import torch
     rng = np.random.default_rng(17)
     nsvc, nhosts = 320, 64
     ev = synth.gen_mixed(rng, 150_000, nsvc, ntask=16, nhosts=nhosts, nclients=4000)
+    resp = ev[(ev["type"] == ge.EV_RESP) & (ev["value"] < 1_000_001_000)]
+    resp_ids, resp_vals = resp["svc_id"], resp["value"].astype(np.float64)
     kw = dict(max_svcs=1024, max_tasks=64, max_batch=1 << 16, cms_log2_width=14)
     shards = [ge.Engine(rank=r, world=2, **kw) for r in range(2)]
     one = ge.Engine(**kw)
@@ -85,10 +88,17 @@ def test_two_shards_merge_to_global_answers():
                 regs = np.maximum(regs, r)
         assert x["distinct_clients"] == po.lib().gyo_hll_estimate(po._p(regs), 12)
         # t-digests: rank-ascending merge of two shard digests vs one engine folding 16 members: same samples, different
-        # clustering => epsilon parity on the quantiles, exact parity on the counts
+        # clustering => epsilon parity on the quantiles, exact parity on the counts. Both answers are held to the rank bound of the
+        # members' exact samples; the 1 % value parity from 5 000 samples on (at ~2 300 samples neighbouring samples near p95 lie
+        # ~1 % apart in value, so two clusterings one sample apart differ by that much)
         if x["td_count"] >= 2000:
-            for f in ("td_p50_us", "td_p95_us"):
-                assert abs(x[f] - z[f]) / z[f] < 0.01, (f, x[f], z[f])
+            sv = np.sort(resp_vals[np.isin(resp_ids, members)])
+            assert len(sv) == x["td_count"]
+            for f, q in (("td_p50_us", 0.5), ("td_p95_us", 0.95), ("td_p99_us", 0.99)):
+                for g in (x[f], z[f]):
+                    assert rank_error(sv, g, q) <= rank_bound(q, len(sv), 200), (int(lid), f, g)
+                if f != "td_p99_us" and x["td_count"] >= 5000:
+                    assert abs(x[f] - z[f]) / z[f] < 0.01, (f, x[f], z[f])
             assert abs(x["td_p99_us"] - z["td_p99_us"]) / z["td_p99_us"] < max(0.03, 2 * td_p99_tolerance(x["td_count"]))   # two clusterings of a few thousand samples
             assert x["td_p50_us"] == y["td_p50_us"]                                          # both ranks computed the same merge
             nonzero += 1

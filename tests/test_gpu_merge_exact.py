@@ -207,7 +207,7 @@ def _digest(rng, n, lo=1.0, hi=1.0e6, wmax=1000):
     return means, w
 
 
-def test_finish_on_crafted_gathered_slabs():
+def test_finish_on_crafted_gathered_slabs_k1_centres():
     """gysk_merge_finish on hand-built gathered slabs of 8 ranks at delta = 256: equal means across ranks, empty ranks between
     non-empty ones (their head fields must not count), all ranks empty, a single centroid, 256 centroids on every rank (the
     512-entry work area filled exactly at every step) and a total weight above 2^53, where (double) W rounds"""

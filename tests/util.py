@@ -124,15 +124,16 @@ def td_merge_compress(a, b, delta):
 
 
 def k1_cell_weights(delta, W):
-    """delta weights summing to W whose exclusive prefixes sit one in each cell of the K_1 grid (item 0 at 0, item j > 0 at the
-    middle of cell j): compressed on its own, such a list keeps all delta items apart — a digest of exactly delta centroids"""
+    """delta weights summing to W, item j filling cell j of the K_1 grid exactly ([T_j, T_j+1)), so that its weight centre lies
+    inside the cell: 2 T_j + w_j >= 2 T_j and < 2 T_j+1. Compressed on its own, such a list keeps all delta items apart — a digest
+    of exactly delta centroids"""
     import math
     q = [0.5 * (math.sin(math.pi * (j / delta - 0.5)) + 1.0) for j in range(delta + 1)]
     q[0], q[delta] = 0.0, 1.0
     T = [int(x * float(W)) for x in q]
-    assert min(b - a for a, b in zip(T, T[1:])) >= 4, "W too small for the narrowest cell"
-    starts = [0] + [(T[j] + T[j + 1]) // 2 for j in range(1, delta)] + [W]
-    return np.diff(np.array(starts, dtype=np.int64)).astype(np.uint64)
+    T[delta] = W
+    assert min(b - a for a, b in zip(T, T[1:])) >= 1, "W too small for the narrowest cell"
+    return np.diff(np.array(T, dtype=np.int64)).astype(np.uint64)
 
 
 class Digest:
