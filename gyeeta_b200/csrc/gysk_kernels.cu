@@ -44,7 +44,8 @@ struct SortPlan { int np; int shift[OS_MAX_PASSES_VK]; int bits[OS_MAX_PASSES_VK
 // exp: ABLATION switches for timing runs only (GYSK_EXP_ABLATE; results are wrong when set): 1 = no batch-extreme / CONN_BITMAP loads and
 // atomics, 2 = no digit histograms, 4 = no TCP drain pass, 8 = no TASK drain pass, 16 = TCP drain pass without the count-min REDs,
 // 32 = TCP drain pass without the HLL register peek / raise, 64 = TASK drain pass drops the updates that miss the CTA's hot table (the
-// end-of-CTA flush stays), 128 = TASK drain pass loads the records and computes the buckets but applies nothing
+// end-of-CTA flush stays), 128 = TASK drain pass loads the records and computes the buckets but applies nothing, 256 = bins_merge_kernel
+// builds the items and histogram cells but skips warp_merge_compress and the digest header update
 
 // ---------------------------------------------------------------------------------------------------
 // state init / registration
@@ -1066,41 +1067,51 @@ __global__ void __launch_bounds__(256) long_sum_kernel(const unsigned long long 
 }
 
 static constexpr int TD_WARPS = 3;		// warps (= services in flight) per CTA
-// longest merged list (old centroids + batch items) that works in shared memory, 10.4 KB per warp: the smaller the work area, the
-// more services a SM has in flight (the kernel is latency-bound: a long chain of dependent warp instructions per service)
-static constexpr int TD_SMEM_N = 384;
+// longest merged list (old centroids + batch items) that works in shared memory, 14.6 KB per warp: 5 CTAs x 3 warps fill the SM's
+// 228 KB. A list that does not fit is merged in the L2 scratch at several times the cost of one that does, so a larger area that
+// fits more lists beats more services in flight (measured on the bench workload, DESIGN.md §7: 384 entries at 7 CTAs 1.48 ms,
+// 440 at 6 CTAs 1.36 ms, 540 at 5 CTAs 1.25 ms; 540 is the most a CTA's 48 KB of static shared memory holds)
+static constexpr int TD_SMEM_N = 540;
 
 // One warp per touched service. Its non-empty bins become the batch's items {mean = exact usec sum / samples, weight = samples} — in
 // value order, because the bin index is monotone — and every bin adds {samples, exact msec sum} to its bucket of the window
 // histogram: GY_HISTOGRAM::add_data for each of its samples (common/gy_statistics.h:596-623); max_val_seen_ and the digest's ends
 // come from the batch's exact extremes. The items are then merged with the old centroids (old first on equal means) and the greedy
-// K_1 pass cuts the list to at most TD_CAP clusters (warp_merge_compress). Lists of up to 2 x TD_CAP entries work in shared memory;
+// K_1 pass cuts the list to at most TD_CAP clusters (warp_merge_compress). Lists of up to TD_SMEM_N entries work in shared memory;
 // longer ones (a first batch can fill several hundred bins) in the warp's L2-resident scratch — same code, same result.
 // Work items, in this order: the hot rows, the batch rows of the long segments (both: dense bins, read in bin order and zeroed),
 // then the short segments, whose keys the warp reads itself.
 __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merge_kernel(DevState st, const unsigned long long *__restrict__ keys,
 		const uint32_t *__restrict__ touched, const unsigned long long *__restrict__ ntouched_p, const uint32_t *__restrict__ long_slot,
 		const unsigned long long *__restrict__ nlong_p, unsigned long long *__restrict__ batch_rows, const BatchSeg *__restrict__ segs,
-		Centroid *__restrict__ items_scratch /* [nwarps][NBINS] */, TdWorkBig *__restrict__ big_scratch /* [nwarps] */)
+		Centroid *__restrict__ items_scratch /* [nwarps][NBINS] */, TdWorkBig *__restrict__ big_scratch /* [nwarps] */, int exp)
 {
 	__shared__ TdWorkT<TD_SMEM_N> work[TD_WARPS];
 	// window histogram of the service's batch: 32-bit shared-memory atomics (native; a 64-bit shared atomicAdd is a CAS loop). A bucket's
 	// sample count of one batch fits 32 bits (max_batch < 2^27); the msec sum is kept as {low word, carries + high words}
 	__shared__ uint32_t hcnt[TD_WARPS][16], hsum_lo[TD_WARPS][16], hsum_hi[TD_WARPS][16];
-	__shared__ uint16_t first_idx[16];
+	// histogram bucket of every bin, per group of 8 bins: {bucket of the group's first bin : 4 | offset of the next bucket's first bin in
+	// the group, 8: none : 4}. Buckets 2..14 start at least 14 bins apart, so a group holds at most one start
+	__shared__ uint8_t bk_tab[NBINS / 8];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 	const uint32_t gw = blockIdx.x * TD_WARPS + wid, nwarps = gridDim.x * TD_WARPS;
 
 	Centroid *items = items_scratch + (size_t)gw * NBINS;
 	const uint32_t ntouched = (uint32_t)*ntouched_p, nlong = (uint32_t)*nlong_p;
 
-	if (threadIdx.x < 16) {
+	for (uint32_t g = threadIdx.x; g < (uint32_t)NBINS / 8; g += blockDim.x) {
 		// thresholds of RESP_TIME_HASH in msec (gy_statistics.h:1677): bucket b >= 2 starts at (thr[b-2] + 1) msec, bucket 1 at 0;
 		// bin index = td_code(usec) + bucket, so bucket b's bins start at td_code(first usec of the bucket) + b
 		constexpr uint32_t thr[13] = {1, 10, 30, 60, 100, 150, 200, 300, 450, 700, 1000, 3000, 15000};
-		const uint32_t bk = threadIdx.x;
-		const uint32_t first_us = bk < 2 ? 0u : (bk > 14 ? 0u : (thr[bk - 2] + 1u) * 1000u);
-		first_idx[bk] = (uint16_t)(bk == 0 ? 0u : (bk > 14 ? 0xFFFFu : td_code(first_us) + bk));
+		auto bucket = [&](uint32_t bin) {
+			uint32_t bk = bin >= 1u;
+			for (int q = 2; q < 15; ++q) bk += bin >= td_code((thr[q - 2] + 1u) * 1000u) + (uint32_t)q;
+			return bk;
+		};
+		const uint32_t b0 = bucket(g * 8);
+		uint32_t off = 8;
+		for (uint32_t o = 7; o >= 1; --o) if (bucket(g * 8 + o) != b0) off = o;
+		bk_tab[g] = (uint8_t)(b0 | (off << 4));
 	}
 	__syncthreads();
 
@@ -1132,14 +1143,17 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 		if (t < nhot && sb.minv == 0xFFFFFFFFu) continue;			// a hot service without a sample in this batch (warp-uniform)
 		if (lane < 16) { hcnt[wid][lane] = 0; hsum_lo[wid][lane] = 0; hsum_hi[wid][lane] = 0; }
 		__syncwarp();
-		// one non-empty bin {samples | remainders, usec sum} -> item j of the batch + GY_HISTOGRAM::add_data of its samples
-		auto take_bin = [&](uint32_t j, unsigned long long cw, unsigned long long us, uint32_t bin) {
+		const uint32_t na = st.td_head[slot].n;		// old centroids of the digest
+		TdWorkT<TD_SMEM_N> &W = work[wid];
+		// one non-empty bin {samples | remainders, usec sum} -> item j of the batch + GY_HISTOGRAM::add_data of its samples. The item
+		// goes to items[j], or with `staged` straight to where warp_merge_compress_staged reads it: mean at W.src[na + j], weight
+		// (a short segment's bin: <= LONG_SEG samples) at W.nxt[j]
+		auto take_bin = [&](uint32_t j, unsigned long long cw, unsigned long long us, uint32_t bin, bool staged) {
 			const unsigned long long cnt = cw & BIN_CNT_MASK, rem = cw >> BIN_CNT_BITS;
-			Centroid c; c.mean = __ddiv_rn((double)us, (double)cnt); c.weight = cnt;	// exact integer sum, one rounding
-			items[j] = c;
-			uint32_t bk = 0;
-#pragma unroll
-			for (int q = 1; q < 15; ++q) bk += bin >= first_idx[q];
+			const double mean = __ddiv_rn((double)us, (double)cnt);	// exact integer sum, one rounding
+			if (staged) { W.src[na + j] = mean; W.nxt[j] = (uint16_t)cnt; }
+			else { Centroid c; c.mean = mean; c.weight = cnt; items[j] = c; }
+			const uint32_t e = bk_tab[bin >> 3], bk = (e & 15u) + ((bin & 7u) >= (e >> 4) ? 1u : 0u);
 			atomicAdd(&hcnt[wid][bk], (uint32_t)cnt);
 			const unsigned long long ms = (us - rem) / 1000ull;		// sum of (usec / 1000) over the bin's samples
 			const uint32_t mlo = (uint32_t)ms, mhi = (uint32_t)(ms >> 32);
@@ -1148,67 +1162,115 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 			if (up) atomicAdd(&hsum_hi[wid][bk], up);
 		};
 		uint32_t nitems = 0, nsamples, binmax = 0;	// binmax: samples in the fullest bin (per lane, reduced when needed)
+		bool staged = false;				// the batch items wait in the work area for warp_merge_compress_staged
 		if (t >= nrow) {
-			// a short segment, read straight from the sorted keys, 4 windows of 32 keys at a time (their loads in flight together).
-			// A bin starts wherever the bin bits change; a segmented scan over each window sums the bin's samples, the bin open at the
-			// end of a window carries into the next, and the bin's last key leaves its totals in the bin's item slot — the numbers a run
-			// of equal {slot, bin} adds up to.
+			// a short segment, read straight from the sorted keys in blocks of 256: lane l holds keys [b0 + 8 l, b0 + 8 l + 8), four
+			// 16-byte loads, and the next block's loads go out before this one is scanned. A bin starts wherever the bin bits change.
+			// Each lane sums its own runs of equal bin; one segmented scan per block joins the runs that cross lanes (and the bin open
+			// from the block before), and the bin's last key leaves its totals {usec sum, samples | remainders | bin} in the bin's raw
+			// slot, j = the bins that start before it — the numbers a run of equal {slot, bin} adds up to. The raw slots of the items
+			// that fit the work area beside the old centroids lie there (the usec sum where the item's mean goes, W.src[na + j],
+			// the rest in W.pref[j], free until the merge), the others in items[j]. Then every lane takes every 32nd bin, as for a row.
 			nsamples = seg.end - seg.key0;
 			// a short segment's bin: samples <= LONG_SEG and remainders < 1000 x LONG_SEG fit below bit 54 of cw
 			constexpr int RAW_BIN_SHIFT = 54;
 			static_assert(BIN_CNT_BITS + 10 + 14 <= RAW_BIN_SHIFT && LONG_SEG <= (1 << 14), "cw of a short segment's bin below the bin bits");
+			const uint32_t room = (uint32_t)TD_SMEM_N - na;		// raw slots in the work area (na <= TD_CAP < TD_SMEM_N)
+			unsigned long long *raw_us = reinterpret_cast<unsigned long long *>(W.src + na), *raw_cw = W.pref;
 			ulonglong2 *raw = reinterpret_cast<ulonglong2 *>(items);
-			uint32_t pbin = ~0u, ccnt = 0, crem = 0;	// bin of the key before the window, the totals of that bin so far
+			auto load8 = [&](uint32_t b0, unsigned long long (&k)[8]) {	// ~0ull: no key of the segment (never a key: bin <= 845)
+				const uint32_t i0 = b0 + (uint32_t)lane * 8u;
+				if (i0 >= seg.key0 && i0 + 8u <= seg.end) {
+#pragma unroll
+					for (int q = 0; q < 4; ++q) {
+						const ulonglong2 v = *reinterpret_cast<const ulonglong2 *>(keys + i0 + 2 * q);
+						k[2 * q] = v.x; k[2 * q + 1] = v.y;
+					}
+				}
+				else {
+#pragma unroll
+					for (int u = 0; u < 8; ++u) k[u] = i0 + u >= seg.key0 && i0 + u < seg.end ? keys[i0 + u] : ~0ull;
+				}
+			};
+			auto rem_of = [](uint32_t v) { return v - (v / 1000u) * 1000u; };
+			uint32_t pbin = ~0u, ccnt = 0, crem = 0;	// bin of the key before the block, the totals of that bin so far
 			unsigned long long cus = 0;
-			for (uint32_t b0 = seg.key0; b0 < seg.end; b0 += 128) {
-				uint32_t bin[4], v[4];
+			const uint32_t a0 = seg.key0 & ~1u;		// even: every lane's keys start 16-byte aligned
+			unsigned long long kk[8], nk[8];
+			load8(a0, kk);
+			for (uint32_t b0 = a0; b0 < seg.end; b0 += 256) {
+				if (b0 + 256u < seg.end) load8(b0 + 256u, nk);
+				else {
 #pragma unroll
-				for (int u = 0; u < 4; ++u) {
-					const uint32_t i = b0 + (uint32_t)u * 32 + lane;
-					const unsigned long long k = i < seg.end ? keys[i] : 0ull;
-					bin[u] = i < seg.end ? key_bin(k) : ~0u;
-					v[u] = key_usec(k);
+					for (int u = 0; u < 8; ++u) nk[u] = ~0ull;
 				}
-				const uint32_t xbin = b0 + 128 < seg.end ? key_bin(keys[b0 + 128]) : ~0u;		// the key after the four windows
+				uint32_t bin[8];
 #pragma unroll
-				for (int u = 0; u < 4; ++u) {
-					if (b0 + (uint32_t)u * 32 >= seg.end) break;
-					uint32_t pb = __shfl_up_sync(0xffffffffu, bin[u], 1), nb = __shfl_down_sync(0xffffffffu, bin[u], 1);
-					const uint32_t nb31 = u < 3 ? __shfl_sync(0xffffffffu, bin[u < 3 ? u + 1 : 0], 0) : xbin;
-					if (lane == 0) pb = pbin;
-					if (lane == 31) nb = nb31;
+				for (int u = 0; u < 8; ++u) bin[u] = kk[u] == ~0ull ? ~0u : key_bin(kk[u]);
+				const uint32_t nfirst = __shfl_sync(0xffffffffu, nk[0] == ~0ull ? ~0u : key_bin(nk[0]), 0);	// the key after the block
+				uint32_t prevb = __shfl_up_sync(0xffffffffu, bin[7], 1), nextb = __shfl_down_sync(0xffffffffu, bin[0], 1);
+				if (lane == 0) prevb = pbin;
+				if (lane == 31) nextb = nfirst;
+				// the lane's bin starts (hc) and the totals of its last run
+				uint32_t hc = 0, tc = 0, tr = 0;
+				unsigned long long tu = 0;
+#pragma unroll
+				for (int u = 0; u < 8; ++u) {
 					const bool valid = bin[u] != ~0u;
-					const uint32_t hm = __ballot_sync(0xffffffffu, valid && bin[u] != pb);
-					const uint32_t upto = hm & (0xFFFFFFFFu >> (31 - lane));		// bin starts at lanes <= this one
-					const int h = upto ? 31 - __clz((int)upto) : 0;			// lane of the bin's first key (0: bin open from before)
-					// {usec & 0xFFFFF} and {usec >> 20 | remainder << 16}: the sums of 32 samples fit every field
-					const uint32_t r = v[u] - (v[u] / 1000u) * 1000u;
-					const uint32_t a = valid ? v[u] & 0xFFFFFu : 0u, b = valid ? (v[u] >> 20) | (r << 16) : 0u;
-					uint32_t ai = a, bi = b;
-#pragma unroll
-					for (int off = 1; off < 32; off <<= 1) {
-						const uint32_t x = __shfl_up_sync(0xffffffffu, ai, off), y = __shfl_up_sync(0xffffffffu, bi, off);
-						if (lane >= off) { ai += x; bi += y; }
-					}
-					const uint32_t as = ai - __shfl_sync(0xffffffffu, ai - a, h), bs = bi - __shfl_sync(0xffffffffu, bi - b, h);
-					uint32_t cnt = (uint32_t)(lane - h) + 1u, rem = bs >> 16;
-					unsigned long long us = (unsigned long long)as + ((unsigned long long)(bs & 0xFFFFu) << 20);
-					if (!upto) { cnt += ccnt; rem += crem; us += cus; }
-					if (valid && bin[u] != nb) {		// the bin's totals, {usec sum, cw | bin << 54}, wait in its item's place
-						raw[nitems + __popc(upto) - 1u] = make_ulonglong2(us, (unsigned long long)cnt | ((unsigned long long)rem << BIN_CNT_BITS) |
-								((unsigned long long)bin[u] << RAW_BIN_SHIFT));
-						binmax = max(binmax, cnt);
-					}
-					ccnt = __shfl_sync(0xffffffffu, cnt, 31); crem = __shfl_sync(0xffffffffu, rem, 31); cus = __shfl_sync(0xffffffffu, us, 31);
-					pbin = __shfl_sync(0xffffffffu, bin[u], 31);
-					nitems += __popc(hm);
+					if (valid && bin[u] != (u ? bin[u - 1] : prevb)) { ++hc; tc = 0; tr = 0; tu = 0; }
+					const uint32_t v = key_usec(kk[u]);
+					if (valid) { ++tc; tr += rem_of(v); tu += v; }
 				}
+				// one scan over the lanes of {usec sum : 40 | bin starts} and {remainders : 18 | samples}: the sums of 256 samples
+				// fit every field. The segmented totals of a lane's last run start at the last lane with a bin start (h).
+				const unsigned long long X = tu | ((unsigned long long)hc << 40);
+				const uint32_t Y = tr | (tc << 18);
+				unsigned long long xi = X;
+				uint32_t yi = Y;
+#pragma unroll
+				for (int off = 1; off < 32; off <<= 1) {
+					const unsigned long long x = __shfl_up_sync(0xffffffffu, xi, off);
+					const uint32_t y = __shfl_up_sync(0xffffffffu, yi, off);
+					if (lane >= off) { xi += x; yi += y; }
+				}
+				const uint32_t hm = __ballot_sync(0xffffffffu, hc != 0);
+				const uint32_t upto = hm & (0xFFFFFFFFu >> (31 - lane));		// lanes <= this one with a bin start
+				const int h = upto ? 31 - __clz((int)upto) : 0;
+				const unsigned long long xs = xi - __shfl_sync(0xffffffffu, xi - X, h);
+				const uint32_t ys = yi - __shfl_sync(0xffffffffu, yi - Y, h);
+				unsigned long long su = xs & ((1ull << 40) - 1u);			// the bin open at the lane's last key, so far
+				uint32_t sc = ys >> 18, sr = ys & 0x3FFFFu;
+				if (!upto) { su += cus; sc += ccnt; sr += crem; }
+				// the bin open at the lane's first key (the lane before's, or the block before's at lane 0)
+				unsigned long long ru = __shfl_up_sync(0xffffffffu, su, 1);
+				uint32_t rc = __shfl_up_sync(0xffffffffu, sc, 1), rr = __shfl_up_sync(0xffffffffu, sr, 1);
+				if (lane == 0) { ru = cus; rc = ccnt; rr = crem; }
+				uint32_t j = nitems + (uint32_t)(xi >> 40) - hc - 1u;		// item of that bin
+#pragma unroll
+				for (int u = 0; u < 8; ++u) {
+					const bool valid = bin[u] != ~0u;
+					if (valid && bin[u] != (u ? bin[u - 1] : prevb)) { ++j; rc = 0; rr = 0; ru = 0; }
+					const uint32_t v = key_usec(kk[u]);
+					if (valid) { ++rc; rr += rem_of(v); ru += v; }
+					if (valid && bin[u] != (u < 7 ? bin[u + 1] : nextb)) {		// the bin's last key
+						const unsigned long long cwb = (unsigned long long)rc | ((unsigned long long)rr << BIN_CNT_BITS) |
+								((unsigned long long)bin[u] << RAW_BIN_SHIFT);
+						if (j < room) { raw_us[j] = ru; raw_cw[j] = cwb; }
+						else raw[j] = make_ulonglong2(ru, cwb);
+						binmax = max(binmax, rc);
+					}
+				}
+				cus = __shfl_sync(0xffffffffu, su, 31); ccnt = __shfl_sync(0xffffffffu, sc, 31); crem = __shfl_sync(0xffffffffu, sr, 31);
+				pbin = __shfl_sync(0xffffffffu, bin[7], 31);
+				nitems += (uint32_t)(__shfl_sync(0xffffffffu, xi, 31) >> 40);
+#pragma unroll
+				for (int u = 0; u < 8; ++u) kk[u] = nk[u];
 			}
-			// then every lane takes every 32nd bin, as for a row: one take_bin per 32 bins, not one per window
+			staged = na + nitems <= (uint32_t)TD_SMEM_N;
 			__syncwarp();
 			for (uint32_t j = lane; j < nitems; j += 32) {
-				const ulonglong2 r = raw[j];
-				take_bin(j, r.y & ((1ull << RAW_BIN_SHIFT) - 1u), r.x, (uint32_t)(r.y >> RAW_BIN_SHIFT));
+				const ulonglong2 r = j < room ? make_ulonglong2(raw_us[j], raw_cw[j]) : raw[j];
+				take_bin(j, r.y & ((1ull << RAW_BIN_SHIFT) - 1u), r.x, (uint32_t)(r.y >> RAW_BIN_SHIFT), staged);
 			}
 		}
 		else {
@@ -1224,7 +1286,7 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 				const bool ne = (v.x & BIN_CNT_MASK) != 0;
 				const uint32_t m = __ballot_sync(0xffffffffu, ne);
 				if (ne) {
-					take_bin(nitems + __popc(m & lt), v.x, v.y, bin);
+					take_bin(nitems + __popc(m & lt), v.x, v.y, bin, false);
 					row[i0] = 0ull; row[i1] = 0ull;
 					mine += (uint32_t)(v.x & BIN_CNT_MASK);
 					binmax = max(binmax, (uint32_t)(v.x & BIN_CNT_MASK));
@@ -1264,12 +1326,14 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 			st.slot_batch[slot] = SlotBatch {0xFFFFFFFFu, 0u, 0u, hot};
 		}
 		__syncwarp();
+		if (exp & 256) continue;		// timing runs only (warp-uniform)
 
 		TdHead head = st.td_head[slot];
 		Centroid *cent = st.td_cent + (size_t)slot * TD_CAP;
 		uint32_t nout;
-		if (head.n + nitems <= (uint32_t)TD_SMEM_N) nout = warp_merge_compress(work[wid], cent, head.n, items, nitems, cent, st.td);
-		else nout = warp_merge_compress(big_scratch[gw], cent, head.n, items, nitems, cent, st.td);
+		if (staged) nout = warp_merge_compress_staged(W, cent, na, nitems, cent, st.td);
+		else if (na + nitems <= (uint32_t)TD_SMEM_N) nout = warp_merge_compress(W, cent, na, items, nitems, cent, st.td);
+		else nout = warp_merge_compress(big_scratch[gw], cent, na, items, nitems, cent, st.td);
 		if (lane == 0) {
 			head.n = nout;
 			head.total += nsamples;
@@ -2029,7 +2093,7 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 	long_sum_kernel<<<nsm * 8, 256, 0, s>>>(src, d_nkeys, segs, d_nlong, tmp.batch_rows);
 	const int merge_ctas = std::min(nsm, TD_MERGE_MAX_SMS) * TD_MERGE_CTAS_PER_SM;
 	bins_merge_kernel<<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
-			tmp.items_scratch, tmp.big_scratch);
+			tmp.items_scratch, tmp.big_scratch, plan.exp);
 	return launches + 3;
 }
 

@@ -96,7 +96,7 @@ struct SortTemp
 	unsigned long long	*batch_rows;		// [batch rows][HOT_ROW_WORDS] dense value bins of the long segments, hot-row layout; zero
 							// between batches (bins_merge_kernel zeroes what it reads)
 	Centroid		*items_scratch;		// [merge warps][NBINS] a warp's list of batch items
-	TdWorkBig		*big_scratch;		// [merge warps] work arrays for merged lists beyond 2 x TD_CAP entries
+	TdWorkBig		*big_scratch;		// [merge warps] work arrays for merged lists beyond the shared-memory work area (TD_SMEM_N entries)
 	uint4			*recq;			// [recq_cap] records {slot, value, flow key}: ingest_kernel resolves the ids of connection and
 							// process events and queues them, the drain passes (launch_drains) apply them. Warp w of the
 							// ingest launch owns region [w * cap, (w + 1) * cap) (RecRegions): its connection records from
@@ -146,7 +146,7 @@ static constexpr int SORT_TILE = 4096;		// keys per CTA tile in the radix passes
 static constexpr int RADIX_MAX_BITS = 9;
 static constexpr int RADIX_MAX = 1 << RADIX_MAX_BITS;
 static constexpr int OS_MAX_PASSES_VK = 5;		// {slot : <= 24 | bin : 10} = <= 34 bits in digits of <= 8 bits
-static constexpr int TD_MERGE_CTAS_PER_SM = 7, TD_MERGE_MAX_SMS = 192;	// bins_merge_kernel grid (<= 4 warps per CTA)
+static constexpr int TD_MERGE_CTAS_PER_SM = 5, TD_MERGE_MAX_SMS = 192;	// bins_merge_kernel grid (<= 4 warps per CTA)
 // a service segment of more than LONG_SEG sorted keys is summed into a batch row by long_sum_kernel; a shorter one is read by one warp
 // of bins_merge_kernel (DESIGN.md §4). Batch rows: min(max_svcs, ceil(max_batch / LONG_SEG)).
 static constexpr int LONG_SEG = 8192;

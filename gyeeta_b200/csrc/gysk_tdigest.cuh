@@ -38,9 +38,11 @@ struct TdScratch : TdWork		// + an accumulator list for the folds of the merge s
 
 // Stable merge by mean of two mean-sorted centroid lists (`a` first on ties), then the greedy K_1 pass; one warp.
 // Both inputs are fully consumed into S.mean / S.pref before `out` is written, so `out` may alias `a` or `b`.
-// a and b may live in shared or global memory. Returns the number of centroids written to out (<= TD_CAP).
-template <typename Work>
-__device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid *a, uint32_t na, const Centroid *b, uint32_t nb,
+// B_STAGED: the caller has put b's means at S.src[na, na + nb) and its weights (< 2^16 each) at S.nxt[0, nb), and `b` is unused
+// (warp_merge_compress_staged); otherwise a and b may live in shared or global memory. Returns the number of centroids written to
+// out (<= TD_CAP).
+template <bool B_STAGED, typename Work>
+__device__ __forceinline__ uint32_t td_merge_compress(Work &S, const Centroid *a, uint32_t na, const Centroid *b, uint32_t nb,
 		Centroid *out, const TdParams &P)
 {
 	const int lane = threadIdx.x & 31;
@@ -51,8 +53,14 @@ __device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid 
 	// entries of each list lie in front of its first output; from there it is a plain two-finger merge. Order = stable merge by mean,
 	// `a` first on equal means — the same list a rank-by-binary-search of every entry gives, at ~1/4 of the instructions.
 	double *am = S.src, *bm = S.src + na;
-	for (uint32_t j = lane; j < na; j += 32) am[j] = a[j].mean;
-	for (uint32_t j = lane; j < nb; j += 32) bm[j] = b[j].mean;
+	for (uint32_t j0 = 0; j0 < na; j0 += 32 * 4) {		// the loads of 4 rounds in flight together (`a` is the L2-resident digest)
+		double v[4];
+#pragma unroll
+		for (int q = 0; q < 4; ++q) { const uint32_t j = j0 + q * 32 + lane; v[q] = j < na ? a[j].mean : 0.0; }
+#pragma unroll
+		for (int q = 0; q < 4; ++q) { const uint32_t j = j0 + q * 32 + lane; if (j < na) am[j] = v[q]; }
+	}
+	if (!B_STAGED) for (uint32_t j = lane; j < nb; j += 32) bm[j] = b[j].mean;
 	__syncwarp();
 	const uint32_t per = (nm + 31u) >> 5;
 	const uint32_t d0 = lane * per < nm ? lane * per : nm, d1 = d0 + per < nm ? d0 + per : nm;
@@ -64,19 +72,28 @@ __device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid 
 		double av = i < na ? am[i] : 0.0, bv = k < nb ? bm[k] : 0.0;
 		// the two-finger walk touches shared memory only: it notes where every output comes from (S.nxt is free until the cell
 		// search) and the weights — which the walk does not need — are fetched afterwards, all loads of a lane in flight together
-		// (a weight load inside the walk put an L2 round trip into every step)
+		// (a weight load inside the walk put an L2 round trip into every step). With b staged, S.nxt holds b's weights: the walk
+		// copies a b weight into S.pref[pos + 1] as it takes the item and leaves the index of an `a` item there, flagged, for the
+		// fetch (S.pref is free until then)
+		constexpr unsigned long long FROM_A = 1ull << 63;
 		for (uint32_t pos = d0; pos < d1; ++pos) {
 			const bool ta = i < na && (k >= nb || av <= bv);
 			S.mean[pos] = ta ? av : bv;
-			S.nxt[pos] = (uint16_t)(ta ? i : (0x8000u | k));
+			if (B_STAGED) S.pref[pos + 1] = ta ? (FROM_A | i) : (unsigned long long)S.nxt[k];
+			else S.nxt[pos] = (uint16_t)(ta ? i : (0x8000u | k));
 			if (ta) { ++i; av = i < na ? am[i] : 0.0; }
 			else { ++k; bv = k < nb ? bm[k] : 0.0; }
 		}
-		for (uint32_t pos = d0; pos < d1; ++pos) {
-			const uint32_t from = S.nxt[pos];
-			const unsigned long long w = (from & 0x8000u) ? b[from & 0x7FFFu].weight : a[from].weight;
-			S.pref[pos + 1] = w;
-			tot += w;
+		for (uint32_t p0 = d0; p0 < d1; p0 += 4) {		// 4 positions at a time: their weight loads in flight together
+			unsigned long long w[4];
+#pragma unroll
+			for (int q = 0; q < 4; ++q) {
+				const uint32_t pos = p0 + q < d1 ? p0 + q : d1 - 1u;
+				if (B_STAGED) { const unsigned long long f = S.pref[pos + 1]; w[q] = (f & FROM_A) ? a[(uint32_t)f].weight : f; }
+				else { const uint32_t from = S.nxt[pos]; w[q] = (from & 0x8000u) ? b[from & 0x7FFFu].weight : a[from].weight; }
+			}
+#pragma unroll
+			for (int q = 0; q < 4; ++q) if (p0 + q < d1) { S.pref[p0 + q + 1] = w[q]; tot += w[q]; }
 		}
 	}
 	// in-place weight prefix: pref[i+1] holds w_i on entry and sum(w_0..w_i) on exit; every lane scans the outputs it produced
@@ -139,6 +156,21 @@ __device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid 
 	}
 	__syncwarp();
 	return nout;
+}
+
+template <typename Work>
+__device__ __forceinline__ uint32_t warp_merge_compress(Work &S, const Centroid *a, uint32_t na, const Centroid *b, uint32_t nb,
+		Centroid *out, const TdParams &P)
+{
+	return td_merge_compress<false>(S, a, na, b, nb, out, P);
+}
+
+// b already in the work area: means at S.src[na, na + nb), weights at S.nxt[0, nb); na + nb <= Work::NMAX
+template <typename Work>
+__device__ __forceinline__ uint32_t warp_merge_compress_staged(Work &S, const Centroid *a, uint32_t na, uint32_t nb, Centroid *out,
+		const TdParams &P)
+{
+	return td_merge_compress<true>(S, a, na, nullptr, nb, out, P);
 }
 
 } // namespace gysk

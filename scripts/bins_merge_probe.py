@@ -1,0 +1,92 @@
+"""Device time of bins_merge_kernel per batch of the bench workload, whole and without its merge-compress half.
+
+    python scripts/bins_merge_probe.py [--batches 8] [--warmup 3]
+
+Builds the bench's two batches (bench.gen_events_gpu, same seeds, same engine sizes), ingests them once (registration) and runs
+the warm-up steps, then times --batches more batches under torch.profiler. That runs twice, each in a process of its own
+(GYSK_EXP_ABLATE is read once per process): as built, and with GYSK_EXP_ABLATE=256, where bins_merge_kernel builds the items and
+histogram cells but skips warp_merge_compress and the digest header update (timing only: the digests are wrong). Prints one JSON
+line: ms per batch of bins_merge_kernel, segs_mark_kernel and the radix passes for both, and the card, its power limit and SM
+clock."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def card():
+    """name, power limit and current SM clock of GPU 0 as nvidia-smi reports them (read only)"""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        return r.stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        return "nvidia-smi failed: %s" % e
+
+
+def child(args):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    import bench
+    from gyeeta_b200 import engine as ge
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(0)
+    n = args.events
+    eng = ge.Engine(device=0, max_svcs=1 << 17, max_tasks=1 << 15, max_batch=(1 << 27) - 1, stage_batch=1 << 23)
+    ev_devs = [bench.gen_events_gpu(torch, n, 1234 + 7919 * b, 0, 1, dev) for b in range(2)]
+    torch.cuda.synchronize()
+    for ev in ev_devs:                      # registers the services and tasks, as bench.py does
+        eng.ingest_device_ptr(ev.data_ptr(), n)
+    for i in range(args.warmup):
+        eng.ingest_device_ptr(ev_devs[i % 2].data_ptr(), n)
+    eng.sync()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for i in range(args.batches):
+            eng.ingest_device_ptr(ev_devs[i % 2].data_ptr(), n)
+        eng.sync()
+        torch.cuda.synchronize()
+    out = {"bins_merge_kernel": 0.0, "segs_mark_kernel": 0.0, "radix_passes": 0.0}
+    for e in prof.key_averages():
+        us = getattr(e, "device_time_total", None)
+        if us is None:
+            us = e.cuda_time_total
+        if "bins_merge_kernel" in e.key:
+            out["bins_merge_kernel"] += us
+        elif "segs_mark_kernel" in e.key:
+            out["segs_mark_kernel"] += us
+        elif "os_pass_kernel" in e.key:
+            out["radix_passes"] += us
+    eng.close()
+    print(json.dumps({k: round(v / 1000.0 / args.batches, 4) for k, v in out.items()}))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batches", type=int, default=8)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--events", type=int, default=100_000_000)
+    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    if args.child:
+        return child(args)
+    res = {"card": card()}
+    for name, bits in (("as_built", "0"), ("ablate_256", "256")):
+        env = dict(os.environ, GYSK_EXP_ABLATE=bits)
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--batches", str(args.batches), "--warmup",
+                            str(args.warmup), "--events", str(args.events)], env=env, capture_output=True, text=True)
+        if r.returncode:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise SystemExit("probe run %s failed" % name)
+        res[name] = json.loads(r.stdout.strip().splitlines()[-1])
+    res["card_after"] = card()
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
