@@ -533,7 +533,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &tmp.keys_a, nsort, false)); A(dalloc(e, &tmp.keys_b, nsort, false));
 	A(dalloc(e, &tmp.tile_status, (size_t)RADIX_MAX * tmp.max_tiles));
 	tmp.epoch = &e->sort_epoch;
-	A(dalloc(e, &tmp.os_ghist, (size_t)8 * RADIX_MAX + 8));
+	A(dalloc(e, &tmp.os_ghist, (size_t)OS_GHIST_WORDS));
 	A(dalloc(e, &tmp.touched, ns));
 	{
 		const size_t nmw = (size_t)TD_MERGE_MAX_SMS * TD_MERGE_CTAS_PER_SM * 4;		// warps of bins_merge_kernel

@@ -137,7 +137,7 @@ extern "C" int gysk_task_groupby(gysk_engine *e, const gysk_proc_sample *samples
 	gb_insert_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(d_recs, n, d_tkeys, d_tvals, tcap - 1, e->tmp.keys_a, d_cnt);
 	int which = 0, bits = 1;
 	while (bits < 32 && (1ull << bits) < n) bits++;			// group numbers are < n
-	int nl = launch_radix_sort(e->tmp, d_cnt + 1, n, 32, 32 + bits, 64, 64, &which, e->stream);
+	int nl = launch_radix_sort(e->tmp, d_cnt + 1, n, 32, 32 + bits, &which, e->stream);
 	if (nl < 0) { release(); return fail(e, GYSK_ERR_INVAL, "gysk_task_groupby: sort plan"); }
 	e->kernel_launches += 1 + nl;
 	// the fold reads the sorted keys from one buffer and leaves the groups' {first index | group} keys in keys_a for the second sort
@@ -147,7 +147,7 @@ extern "C" int gysk_task_groupby(gysk_engine *e, const gysk_proc_sample *samples
 	if (!gkeys) { GB(cudaMalloc(&d_gtmp, (size_t)n * 8)); gkeys = d_gtmp; }
 	gb_fold_kernel<<<(n + 127) / 128, 128, 0, e->stream>>>(sorted, d_recs, n, d_groups, gkeys);
 	if (d_gtmp) GB(cudaMemcpyAsync(e->tmp.keys_a, d_gtmp, (size_t)n * 8, cudaMemcpyDeviceToDevice, e->stream));
-	nl = launch_radix_sort(e->tmp, d_cnt, n, 32, 32 + bits, 64, 64, &which, e->stream);
+	nl = launch_radix_sort(e->tmp, d_cnt, n, 32, 32 + bits, &which, e->stream);
 	if (nl < 0) { release(); cudaFree(d_gtmp); return fail(e, GYSK_ERR_INVAL, "gysk_task_groupby: sort plan"); }
 	gb_emit_kernel<<<(n + 127) / 128, 128, 0, e->stream>>>(which ? e->tmp.keys_b : e->tmp.keys_a, d_cnt, d_groups, d_out, cap);
 	e->kernel_launches += 2 + nl;

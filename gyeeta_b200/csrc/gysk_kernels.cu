@@ -40,7 +40,16 @@ __device__ __forceinline__ uint32_t key_slot(unsigned long long k) { return (uin
 __device__ __forceinline__ uint32_t key_bin(unsigned long long k) { return (uint32_t)(k >> KEY_GROUP_SHIFT) & ((1u << TD_CODE_BITS) - 1u); }
 
 static constexpr int KEY_DIGIT_MAX = 8;				// widest digit of the RESP-key passes (key_sort_plan)
-struct SortPlan { int np; int shift[OS_MAX_PASSES_VK]; int bits[OS_MAX_PASSES_VK]; int exp; };	// digit p = (key >> shift[p]) & ((1 << bits[p]) - 1)
+static constexpr int KEY_SLOT_BITS_MAX = 24;
+// passes of the longest RESP plan: ingest_kernel keeps this many digit histograms in shared memory
+static constexpr int KEY_PASSES_MAX = (TD_CODE_BITS + KEY_SLOT_BITS_MAX + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
+static_assert(KEY_PASSES_MAX <= OS_MAX_PASSES, "a RESP plan fits a SortPlan");
+// which bits of the key each pass of the radix sort takes as its digit, lowest first: pass p sorts on bits [shift[p], shift[p] + bits[p]).
+// key_sort_plan cuts the RESP keys, plain_sort_plan every other sort; ingest_kernel and os_hist_kernel fill the passes' histograms
+// from the plan, os_pass_kernel gets its pass's shift and width.
+struct SortPlan { int np; int shift[OS_MAX_PASSES]; int bits[OS_MAX_PASSES]; };
+__device__ __forceinline__ uint32_t sort_digit(unsigned long long k, int shift, int bits) { return (uint32_t)(k >> shift) & ((1u << bits) - 1u); }
+
 // exp: ABLATION switches for timing runs only (GYSK_EXP_ABLATE; results are wrong when set): 1 = no batch-extreme / CONN_BITMAP loads and
 // atomics, 2 = no digit histograms, 4 = no TCP drain pass, 8 = no TASK drain pass, 16 = TCP drain pass without the count-min REDs,
 // 32 = TCP drain pass without the HLL register peek / raise, 64 = TASK drain pass drops the updates that miss the CTA's hot table (the
@@ -276,11 +285,11 @@ struct IngestShared
 	static constexpr int DH = 1 << KEY_DIGIT_MAX;			// digit values of a RESP-key radix pass
 	struct Warp { unsigned long long kq[KQ_CAP]; IngestRec tcp[RQ_CAP], task[RQ_CAP]; };
 	Warp		w[IngestShape::WARPS];
-	uint32_t	dhist[OS_MAX_PASSES_VK][DH];			// digit histograms of this CTA's keys, one per radix pass
+	uint32_t	dhist[KEY_PASSES_MAX][DH];			// digit histograms of this CTA's keys, one per radix pass
 };
 
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
-		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt)
+		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, int exp)
 {
 	constexpr int WARPS = IngestShape::WARPS, EPT = IngestShape::EPT, CHUNK = IngestShape::CHUNK, DH = IngestShared::DH;
 	extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -292,7 +301,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 	uint32_t nk = 0, ntcp = 0, ntask = 0;				// queue lengths (warp-uniform)
 	unsigned long long t_tcp = 0, t_task = 0;			// queued in total (warp-uniform)
 
-	for (int i = threadIdx.x; i < OS_MAX_PASSES_VK * DH; i += WARPS * 32) (&S.dhist[0][0])[i] = 0;
+	for (int i = threadIdx.x; i < KEY_PASSES_MAX * DH; i += WARPS * 32) (&S.dhist[0][0])[i] = 0;
 	__syncthreads();						// the only block barriers: here and before the retire step
 
 	const uint64_t nchunks = (n + CHUNK - 1) / CHUNK;
@@ -328,8 +337,8 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 		for (uint32_t q = lane; q < nk; q += 32) {
 			const unsigned long long k = W.kq[q];
 #pragma unroll
-			for (int p = 0; p < OS_MAX_PASSES_VK; ++p)
-				if (p < plan.np && !(plan.exp & 2)) atomicAdd(&S.dhist[p][(uint32_t)(k >> plan.shift[p]) & ((1u << plan.bits[p]) - 1u)], 1u);
+			for (int p = 0; p < KEY_PASSES_MAX; ++p)
+				if (p < plan.np && !(exp & 2)) atomicAdd(&S.dhist[p][sort_digit(k, plan.shift[p], plan.bits[p])], 1u);
 			__stcs(keys + base + q, k);
 		}
 		nk = 0;
@@ -392,7 +401,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 				const uint32_t v = rb[k].x, ms = v / 1000u;		// usec -> msec as SVC_INFO_CAP::upd_stats_on_req (gy_proto_parser.cc:2678)
 				const uint32_t b = (uint32_t)bucket_resp_time((long long)ms);
 				bkt[k] = b;
-				if (!(plan.exp & 1)) {
+				if (!(exp & 1)) {
 					sbv[k] = ld_cg_v4(st.slot_batch + slot);
 					mwv[k] = __ldcg(st.bm_cur + (size_t)slot * HIST_CELLS + b);
 				}
@@ -601,17 +610,11 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 }
 
 // ---------------------------------------------------------------------------------------------------
-// stable LSD radix sort, 8- or 9-bit digits, tile = SORT_TILE keys per CTA of 256 threads
-// ---------------------------------------------------------------------------------------------------
-// (used by the top-N rankings: {score | slot} keys over the registered services / tasks)
-// A pass sorts on a digit made of up to two bit fields of the key: digit = ((k >> s1) & m1) | (((k >> s2) & m2) << b1).
-struct DigitSpec { int s1, b1, s2, b2; };
-__device__ __forceinline__ uint32_t key_digit(unsigned long long k, const DigitSpec &D)
-{
-	return ((uint32_t)(k >> D.s1) & ((1u << D.b1) - 1u)) | (((uint32_t)(k >> D.s2) & ((1u << D.b2) - 1u)) << D.b1);
-}
-
-// ---------------------------------------------------------------------------------------------------
+// stable LSD radix sort of 64-bit keys on the bit range of a SortPlan, one digit of 6 to 9 bits per pass (a narrower last digit runs
+// in the 6-bit kernel), tile = SORT_TILE keys per CTA of 256 threads. It sorts every batch's RESP keys by {slot, bin}
+// (launch_batch_merge) and, through launch_radix_sort, the window list by host, the top-N keys of services, processes and logical
+// services by score, and the group-by's keys by group.
+//
 // one-sweep radix pass: 16 B of HBM traffic per key and pass (read once, write once)
 //
 //   os_hist_kernel     one read of the keys fills the GLOBAL digit histograms of every pass (a stable pass does not change how
@@ -628,10 +631,7 @@ __device__ __forceinline__ uint32_t key_digit(unsigned long long k, const DigitS
 static constexpr int OS_THREADS = 256;			// thread t owns digits t, t + 256 in the per-digit steps
 static constexpr int OS_WARPS = OS_THREADS / 32;
 static constexpr int OS_KPT = SORT_TILE / OS_THREADS;	// 16 keys per thread
-static constexpr int OS_MAX_PASSES = 8;
 static constexpr uint32_t OS_FLAG_AGG = 1u << 30, OS_FLAG_PREFIX = 2u << 30, OS_COUNT_MASK = (1u << 30) - 1u;
-
-struct DigitSpecs { DigitSpec d[OS_MAX_PASSES]; int np; };
 
 __device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long *p)
 {
@@ -647,7 +647,7 @@ __device__ __forceinline__ void st_volatile_u64(unsigned long long *p, unsigned 
 // lane-privatised histogram copies (lane & (copies - 1)), skewed by one bank each: 8 copies of 257 words per pass for 8-bit
 // digits, 4 copies of 513 words when a pass has 9 bits
 template <int copies, int stride>
-__global__ void __launch_bounds__(512) os_hist_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *__restrict__ d_n, DigitSpecs P,
+__global__ void __launch_bounds__(512) os_hist_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *__restrict__ d_n, SortPlan P,
 		uint32_t *__restrict__ ghist /* [np][RADIX_MAX] */)
 {
 	extern __shared__ __align__(16) unsigned char osh_smem[];
@@ -669,8 +669,8 @@ __global__ void __launch_bounds__(512) os_hist_kernel(const unsigned long long *
 		for (int p = 0; p < OS_MAX_PASSES; ++p) {
 			if (p < P.np) {
 				uint32_t *hp = h + p * pstride + copy * stride;
-				atomicAdd(hp + key_digit(k0, P.d[p]), 1u);
-				if (two) atomicAdd(hp + key_digit(k1, P.d[p]), 1u);
+				atomicAdd(hp + sort_digit(k0, P.shift[p], P.bits[p]), 1u);
+				if (two) atomicAdd(hp + sort_digit(k1, P.shift[p], P.bits[p]), 1u);
 			}
 		}
 	}
@@ -720,7 +720,7 @@ struct OneSweepSharedT
 
 template <int RBITS>
 __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned long long *__restrict__ in, unsigned long long *__restrict__ out,
-		const unsigned long long *__restrict__ d_n, DigitSpec D, const uint32_t *__restrict__ ghist /* [RADIX] of this pass */,
+		const unsigned long long *__restrict__ d_n, int shift, int bits /* <= RBITS */, const uint32_t *__restrict__ ghist /* [RADIX] of this pass */,
 		unsigned long long *__restrict__ status /* [ntiles][RADIX] */, uint32_t *__restrict__ ticket, uint32_t epoch)
 {
 	constexpr int RADIX = 1 << RBITS;
@@ -731,6 +731,7 @@ __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned l
 	const uint32_t lt_mask = (1u << lane) - 1u;
 	const uint32_t n = (uint32_t)*d_n;
 	const unsigned long long etag = (unsigned long long)epoch << 32;
+	const int width = RBITS > 6 ? RBITS : bits;		// a digit of 7 to 9 bits has its own instantiation, narrower ones share the 6-bit one
 
 	// persistent CTAs: the grid fills the machine once and every CTA keeps taking tile tickets until the keys are used up. The host
 	// sizes nothing by the key count (it never reads it back): with most samples on the hot rows a batch may leave a fraction of
@@ -780,11 +781,11 @@ __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned l
 
 	// rank of every key among the keys of its digit inside this warp's chunk (rounds in order, lanes in order); the group
 	// leader bumps the warp's digit counter and hands the previous value to its group
-	uint32_t dg[OS_KPT / 2];			// two 16-bit digits per word (the VK digit costs a clz + shifts: computed once)
+	uint32_t dg[OS_KPT / 2];			// two 16-bit digits per word
 #pragma unroll
 	for (int r = 0; r < OS_KPT; ++r) {
 		const bool valid = wbase + (uint32_t)r * 32 + lane < n;
-		const uint32_t d = valid ? key_digit(k[r], D) : ((uint32_t)RADIX + lane);
+		const uint32_t d = valid ? sort_digit(k[r], shift, width) : ((uint32_t)RADIX + lane);
 		if (r & 1) dg[r >> 1] |= d << 16; else dg[r >> 1] = d;
 		uint32_t m;
 		if (use_ballot) {
@@ -868,7 +869,7 @@ __global__ void __launch_bounds__(OS_THREADS, 4) os_pass_kernel(const unsigned l
 #pragma unroll 4
 	for (uint32_t i = threadIdx.x; i < nvalid; i += OS_THREADS) {
 		const unsigned long long key = S.keys[i];
-		out[S.goff[key_digit(key, D)] + i] = key;
+		out[S.goff[sort_digit(key, shift, width)] + i] = key;
 	}
 	__syncthreads();		// the tile's shared state is free for the next ticket
 	}
@@ -1875,7 +1876,7 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 	return 1;
 }
 
-// GYSK_EXP_ABLATE: the SortPlan::exp bits, for timing runs only
+// GYSK_EXP_ABLATE: the exp bits listed at the top of this file, for timing runs only
 static int exp_ablate()
 {
 	static const int v = []{ const char *e = getenv("GYSK_EXP_ABLATE"); return e ? atoi(e) : 0; }();
@@ -1888,15 +1889,28 @@ static int exp_ablate()
 static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
 {
 	int slot_bits = 1;
-	while (slot_bits < 24 && (1ull << slot_bits) < max_svcs) slot_bits++;
+	while (slot_bits < KEY_SLOT_BITS_MAX && (1ull << slot_bits) < max_svcs) slot_bits++;
 	const int T = TD_CODE_BITS + slot_bits;
-	const int np = (T + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
-	if (np > OS_MAX_PASSES_VK) return -1;
+	P.np = (T + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
+	if (P.np > KEY_PASSES_MAX) return -1;
 	int at = KEY_GROUP_SHIFT;
-	for (int p = 0; p < np; ++p) { P.bits[p] = T / np + (p < T % np ? 1 : 0); P.shift[p] = at; at += P.bits[p]; }
-	P.np = np;
-	P.exp = exp_ablate();
-	return np;
+	for (int p = 0; p < P.np; ++p) { P.bits[p] = T / P.np + (p < T % P.np ? 1 : 0); P.shift[p] = at; at += P.bits[p]; }
+	return 0;
+}
+
+// every other sort: key bits [lo, hi) in 8-bit digits from lo upwards, the last one short; the first ones are 9 bits wide where
+// that saves a whole pass (18 bits -> 9 9)
+static int plain_sort_plan(int lo, int hi, SortPlan &P)
+{
+	const int T = hi - lo, p8 = (T + 7) / 8, p9 = (T + 8) / 9;
+	int wide = p9 < p8 ? T - 8 * p9 : 0;	// number of 9-bit passes
+	int at = lo;
+	for (P.np = 0; at < hi; at += P.bits[P.np++]) {
+		if (P.np == OS_MAX_PASSES) return -1;
+		P.shift[P.np] = at;
+		P.bits[P.np] = std::min(wide-- > 0 ? 9 : 8, hi - at);
+	}
+	return 0;
 }
 
 int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s)
@@ -1909,7 +1923,7 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	if (st.hot_rows) cudaMemcpyAsync(st.counters + CTR_NHOT, st.counters + CTR_NHOT_NEXT, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s);
 	// key cursor, digit histograms and tile tickets of this batch's sort
 	cudaMemsetAsync(st.counters + CTR_NKEYS, 0, sizeof(unsigned long long), s);
-	cudaMemsetAsync(tmp.os_ghist, 0, (OS_MAX_PASSES * RADIX_MAX + OS_MAX_PASSES) * sizeof(uint32_t), s);
+	cudaMemsetAsync(tmp.os_ghist, 0, OS_GHIST_WORDS * sizeof(uint32_t), s);
 	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
 	static bool attr_set[MAX_DEVICES] = {};
 	if (!attr_set[dev]) {
@@ -1924,7 +1938,7 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	rr.nwarps = grid * WARPS;
 	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
-	ingest_kernel<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt);
+	ingest_kernel<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
 	return 1;
 }
 
@@ -1961,32 +1975,6 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr,
 	return launches;
 }
 
-// plain-key digit plan: the significant bits [lo1, hi1) then [lo2, hi2) (lo2 >= hi1; hi2 <= lo2 for a single range) cut into
-// digits in order, a digit may straddle the gap. Digits are 8 bits wide unless 9-bit digits save a whole pass.
-static int build_digit_specs(int lo1, int hi1, int lo2, int hi2, DigitSpecs &P)
-{
-	int p1 = lo1, p2 = lo2;			// next unsorted bit of each range
-
-	P.np = 0;
-	if (hi2 < lo2) hi2 = lo2;
-	const int T = (hi1 - lo1) + (hi2 - lo2);
-	const int p8 = (T + 7) / 8, p9 = (T + 8) / 9;
-	int wide = p9 < p8 ? T - 8 * p9 : 0;	// number of 9-bit passes (the first ones)
-	while ((p1 < hi1 || p2 < hi2) && P.np < OS_MAX_PASSES) {
-		DigitSpec D {0, 0, 0, 0};
-		int need = wide > 0 ? 9 : 8;
-		if (wide > 0) --wide;
-		if (p1 < hi1) { D.s1 = p1; D.b1 = hi1 - p1 < need ? hi1 - p1 : need; p1 += D.b1; need -= D.b1; }
-		if (need && p1 >= hi1 && p2 < hi2) {
-			const int take = hi2 - p2 < need ? hi2 - p2 : need;
-			if (D.b1) { D.s2 = p2; D.b2 = take; } else { D.s1 = p2; D.b1 = take; }
-			p2 += take;
-		}
-		P.d[P.np++] = D;
-	}
-	return (p1 < hi1 || p2 < hi2) ? -1 : 0;		// more than 64 significant bits cannot happen
-}
-
 static void os_set_attrs(int dev)
 {
 	static bool attr_set[MAX_DEVICES] = {};
@@ -2010,51 +1998,51 @@ static uint32_t next_epoch(const SortTemp &tmp, uint32_t max_tiles, cudaStream_t
 	return e;
 }
 
-// one radix pass with the kernel instantiation of the digit's width: a 7-bit digit has half the per-digit work (per-warp counters to
-// clear and prefix, status words to publish and look back through, ballots per key) of an 8-bit one. The grid is persistent
-// (os_pass_kernel): at most as many CTAs as the SMs hold at once, whatever the number of possible tiles.
-static void launch_os_pass(int bits, uint32_t ntiles, const unsigned long long *in, unsigned long long *out, const unsigned long long *d_n, const DigitSpec &D,
-		const uint32_t *ghist, unsigned long long *status, uint32_t *ticket, uint32_t epoch, cudaStream_t s)
+// the passes of a plan over the *d_n keys in tmp.keys_a, ping-pong with keys_b; tmp.os_ghist holds the passes' histograms and zeroed
+// tickets. Each pass runs the kernel instantiation of its digit's width: a 7-bit digit has half the per-digit work (per-warp
+// counters to clear and prefix, status words to publish and look back through, ballots per key) of an 8-bit one. The grid is
+// persistent (os_pass_kernel): at most as many CTAs as the SMs hold at once, whatever the number of possible tiles.
+// Returns the launches; *which = the buffer that holds the sorted keys
+static int launch_sort_passes(const SortPlan &P, const SortTemp &tmp, const unsigned long long *d_n, uint32_t ntiles, int *which, cudaStream_t s)
 {
+	unsigned long long *bufs[2] = { tmp.keys_a, tmp.keys_b };
 	const uint32_t grid = std::min<uint32_t>(ntiles, (uint32_t)sm_count(current_device()) * 4u);		// __launch_bounds__(OS_THREADS, 4)
-	if (bits > 8) os_pass_kernel<9><<<grid, OS_THREADS, sizeof(OneSweepSharedT<9>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
-	else if (bits == 8) os_pass_kernel<8><<<grid, OS_THREADS, sizeof(OneSweepSharedT<8>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
-	else if (bits == 7) os_pass_kernel<7><<<grid, OS_THREADS, sizeof(OneSweepSharedT<7>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
-	else os_pass_kernel<6><<<grid, OS_THREADS, sizeof(OneSweepSharedT<6>), s>>>(in, out, d_n, D, ghist, status, ticket, epoch);
+	int w = 0;
+
+	for (int p = 0; p < P.np; ++p, w ^= 1) {
+		const uint32_t epoch = next_epoch(tmp, tmp.max_tiles, s);
+		auto pass = [&](auto kernel, size_t smem) {
+			kernel<<<grid, OS_THREADS, smem, s>>>(bufs[w], bufs[w ^ 1], d_n, P.shift[p], P.bits[p], tmp.os_ghist + p * RADIX_MAX, tmp.tile_status,
+					tmp.os_ghist + OS_GHIST_TICKETS + p, epoch);
+		};
+		if (P.bits[p] > 8) pass(os_pass_kernel<9>, sizeof(OneSweepSharedT<9>));
+		else if (P.bits[p] == 8) pass(os_pass_kernel<8>, sizeof(OneSweepSharedT<8>));
+		else if (P.bits[p] == 7) pass(os_pass_kernel<7>, sizeof(OneSweepSharedT<7>));
+		else pass(os_pass_kernel<6>, sizeof(OneSweepSharedT<6>));
+	}
+	*which = w;
+	return P.np;
 }
 
-// stable LSD radix sort of the *d_n keys in keys_a on their own bits (plain mode, the top-N sorts): n_max >= *d_n sizes the grids
-int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo1, int hi1, int lo2, int hi2, int *which, cudaStream_t s)
+// stable LSD radix sort of the *d_n keys in keys_a on their bits [lo, hi): n_max >= *d_n sizes the grids
+int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s)
 {
-	int launches = 0;
-	unsigned long long *bufs[2] = { tmp.keys_a, tmp.keys_b };
-	int w = 0;
-	DigitSpecs P;
+	SortPlan P;
 
 	*which = 0;
 	if (!n_max) return 0;
-	if (build_digit_specs(lo1, hi1, lo2, hi2, P) || n_max >= (1ull << 30)) return -1;	// status words carry 30-bit counts
+	if (plain_sort_plan(lo, hi, P) || n_max >= (1ull << 30)) return -1;	// status words carry 30-bit counts
 	bool any9 = false;
-	for (int p = 0; p < P.np; ++p) any9 |= P.d[p].b1 + P.d[p].b2 > 8;
+	for (int p = 0; p < P.np; ++p) any9 |= P.bits[p] > 8;
 	const int copies = any9 ? 4 : 8, stride = (any9 ? 512 : 256) + 1;
 	const int dev = current_device();
 	os_set_attrs(dev);
-	const uint32_t ntiles = div_up(n_max, SORT_TILE);
-	uint32_t *ghist = tmp.os_ghist, *tickets = tmp.os_ghist + OS_MAX_PASSES * RADIX_MAX;
 
-	cudaMemsetAsync(ghist, 0, (OS_MAX_PASSES * RADIX_MAX + OS_MAX_PASSES) * sizeof(uint32_t), s);
+	cudaMemsetAsync(tmp.os_ghist, 0, OS_GHIST_WORDS * sizeof(uint32_t), s);
 	const uint32_t hgrid = std::min<uint32_t>(div_up(n_max, 512 * 2 * 4), (uint32_t)sm_count(dev) * 3);
-	if (any9) os_hist_kernel<4, 513><<<hgrid, 512, (size_t)P.np * copies * stride * sizeof(uint32_t), s>>>(bufs[w], d_n, P, ghist);
-	else os_hist_kernel<8, 257><<<hgrid, 512, (size_t)P.np * copies * stride * sizeof(uint32_t), s>>>(bufs[w], d_n, P, ghist);
-	launches++;
-	for (int p = 0; p < P.np; ++p) {
-		const uint32_t epoch = next_epoch(tmp, tmp.max_tiles, s);
-		launch_os_pass(P.d[p].b1 + P.d[p].b2, ntiles, bufs[w], bufs[w ^ 1], d_n, P.d[p], ghist + p * RADIX_MAX, tmp.tile_status, tickets + p, epoch, s);
-		launches++;
-		w ^= 1;
-	}
-	*which = w;
-	return launches;
+	if (any9) os_hist_kernel<4, 513><<<hgrid, 512, (size_t)P.np * copies * stride * sizeof(uint32_t), s>>>(tmp.keys_a, d_n, P, tmp.os_ghist);
+	else os_hist_kernel<8, 257><<<hgrid, 512, (size_t)P.np * copies * stride * sizeof(uint32_t), s>>>(tmp.keys_a, d_n, P, tmp.os_ghist);
+	return 1 + launch_sort_passes(P, tmp, d_n, div_up(n_max, SORT_TILE), which, s);
 }
 
 // after the ingest kernel of a batch: sort its RESP keys by {slot, bin}, find every service's key segment, reduce the long ones into
@@ -2064,7 +2052,6 @@ int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s)
 {
 	if (!n_events) return 0;
-	int launches = 0;
 	unsigned long long *d_nkeys = st.counters + CTR_NKEYS, *d_ntouched = st.counters + CTR_NTOUCHED;
 	const int dev = current_device();
 	const int nsm = sm_count(dev);
@@ -2072,18 +2059,9 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 
 	SortPlan plan {};
 	if (key_sort_plan(max_svcs, plan) < 0) return -1;
-	const uint32_t ntiles = div_up(n_events, SORT_TILE);
-	unsigned long long *bufs[2] = { tmp.keys_a, tmp.keys_b };
-	uint32_t *ghist = tmp.os_ghist, *tickets = tmp.os_ghist + OS_MAX_PASSES * RADIX_MAX;
-	int w = 0;
-	for (int p = 0; p < plan.np; ++p) {
-		const DigitSpec D { plan.shift[p], plan.bits[p], 0, 0 };
-		const uint32_t epoch = next_epoch(tmp, tmp.max_tiles, s);
-		launch_os_pass(plan.bits[p], ntiles, bufs[w], bufs[w ^ 1], d_nkeys, D, ghist + p * RADIX_MAX, tmp.tile_status, tickets + p, epoch, s);
-		launches++;
-		w ^= 1;
-	}
-	const unsigned long long *src = bufs[w];
+	int which = 0;
+	const int launches = launch_sort_passes(plan, tmp, d_nkeys, div_up(n_events, SORT_TILE), &which, s);
+	const unsigned long long *src = which ? tmp.keys_b : tmp.keys_a;
 
 	static_assert(CTR_NLONG == CTR_NTOUCHED + 1, "one memset clears both segment counters");
 	unsigned long long *d_nlong = st.counters + CTR_NLONG;
@@ -2093,7 +2071,7 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 	long_sum_kernel<<<nsm * 8, 256, 0, s>>>(src, d_nkeys, segs, d_nlong, tmp.batch_rows);
 	const int merge_ctas = std::min(nsm, TD_MERGE_MAX_SMS) * TD_MERGE_CTAS_PER_SM;
 	bins_merge_kernel<<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
-			tmp.items_scratch, tmp.big_scratch, plan.exp);
+			tmp.items_scratch, tmp.big_scratch, exp_ablate());
 	return launches + 3;
 }
 
@@ -2158,7 +2136,7 @@ int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_
 		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s)
 {
 	int which = 0;
-	const int sorted = launch_radix_sort(tmp, d_n, nkeys, 32, 64, 64, 64, &which, s);
+	const int sorted = launch_radix_sort(tmp, d_n, nkeys, 32, 64, &which, s);
 	if (sorted < 0) return sorted;
 	topn_pick_kernel<<<1, 64, 0, s>>>(ids, hosts, which ? tmp.keys_b : tmp.keys_a, nkeys, want, d_out);
 	return sorted + 1;
@@ -2250,7 +2228,7 @@ int launch_window_list(const DevState &st, const SortTemp &tmp, uint32_t nslots,
 	window_select_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, is_task, host_filter, active_only, active_mark, seen_before, tmp.keys_a, d_n);
 	if (!order) return 1;
 	int which = 0;
-	const int sorted = launch_radix_sort(tmp, d_n, nslots, 32, 64, 64, 64, &which, s);
+	const int sorted = launch_radix_sort(tmp, d_n, nslots, 32, 64, &which, s);
 	if (sorted < 0) return sorted;
 	*keys = which ? tmp.keys_b : tmp.keys_a; *ids = which ? tmp.keys_a : tmp.keys_b;
 	window_ids_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, is_task, *keys, d_n, const_cast<unsigned long long *>(*ids));

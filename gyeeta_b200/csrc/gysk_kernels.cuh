@@ -89,7 +89,8 @@ struct SortTemp
 	uint64_t		nkeys;			// max(max_batch, max(max_svcs, max_tasks) + 1)
 	unsigned long long	*tile_status;		// [max_tiles][512] look-back status words {pass epoch | state | count}: never cleared
 	uint32_t		*epoch;			// HOST counter of radix passes launched (tags the status words)
-	uint32_t		*os_ghist;		// [8][512] global digit histograms of the one-sweep passes + [8] tile tickets
+	uint32_t		*os_ghist;		// [OS_GHIST_WORDS] of one sort: [OS_MAX_PASSES][RADIX_MAX] global digit histograms of its passes, then
+							// from OS_GHIST_TICKETS on one tile ticket per pass
 	uint32_t		*touched;		// [max_svcs] services with RESP samples in the batch
 	uint4			*segs;			// [max_svcs] BatchSeg of each touched service: its keys in the sorted array, its batch row
 	uint32_t		*long_slot;		// [batch rows] slot of each long segment (more than LONG_SEG keys) of the batch
@@ -145,7 +146,8 @@ struct TaskRaw
 static constexpr int SORT_TILE = 4096;		// keys per CTA tile in the radix passes
 static constexpr int RADIX_MAX_BITS = 9;
 static constexpr int RADIX_MAX = 1 << RADIX_MAX_BITS;
-static constexpr int OS_MAX_PASSES_VK = 5;		// {slot : <= 24 | bin : 10} = <= 34 bits in digits of <= 8 bits
+static constexpr int OS_MAX_PASSES = 8;			// radix passes of one sort: 64 key bits in 8-bit digits
+static constexpr int OS_GHIST_TICKETS = OS_MAX_PASSES * RADIX_MAX, OS_GHIST_WORDS = OS_GHIST_TICKETS + OS_MAX_PASSES;	// SortTemp::os_ghist
 static constexpr int TD_MERGE_CTAS_PER_SM = 5, TD_MERGE_MAX_SMS = 192;	// bins_merge_kernel grid (<= 4 warps per CTA)
 // a service segment of more than LONG_SEG sorted keys is summed into a batch row by long_sum_kernel; a shorter one is read by one warp
 // of bins_merge_kernel (DESIGN.md §4). Batch rows: min(max_svcs, ceil(max_batch / LONG_SEG)).
@@ -158,7 +160,8 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
 int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
-int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo1, int hi1, int lo2, int hi2, int *which, cudaStream_t s);
+// sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range, or n_max >= 2^30
+int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);
 // the want best services (host_filter < 0: of every host) or processes (is_task) of nslots by one metric; -1: sort failed
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
 		gysk_topn_entry *d_out, cudaStream_t s);

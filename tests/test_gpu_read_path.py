@@ -21,7 +21,7 @@ pytestmark = pytest.mark.gpu
 
 NAN = float("nan")
 # window_list of a non-empty table with rows wanted: window_select_kernel, one radix sort of the 32 host bits (os_hist_kernel and
-# four 8-bit os_pass_kernel passes: build_digit_specs(32, 64)) and window_ids_kernel; a count-only call (cap 0) runs
+# four 8-bit os_pass_kernel passes: plain_sort_plan(32, 64)) and window_ids_kernel; a count-only call (cap 0) runs
 # window_select_kernel alone. Then one summary launch per 8192 rows.
 WINDOW_LIST_LAUNCHES, WINDOW_COUNT_LAUNCHES, WIN_ROWS = 7, 1, 8192
 # top-N: the score kernel, the same 32-bit radix sort (5 launches) and the pick kernel
