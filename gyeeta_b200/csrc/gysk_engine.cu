@@ -1138,8 +1138,6 @@ int gysk_evicted_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n)
 
 namespace {
 
-uint32_t active_mark(const gysk_engine *e) { return e->last_flush_tsec ? e->last_flush_tsec : 1u; }	// slot_last_active of the closed window (state_kernel)
-
 // the device half of a window read: the listed keys {host | slot} of the selection (seen_before: see launch_window_list), host-sorted
 // with `order`, at *d_keys (their ids at *d_ids); *n of them
 int list_slots(gysk_engine *e, int is_task, int32_t host_idx, uint32_t flags, uint32_t seen_before, bool order, const unsigned long long **d_keys,

@@ -160,6 +160,38 @@ struct Members
 	}
 };
 
+// SUM words of one host cluster (GYSK_FLAG_MERGE_CLUSTERS): the fields of gysk_cluster_state before its pad, in its order
+constexpr int CLUSTER_WORDS = 6;
+static_assert(sizeof(gysk_cluster_state) == (CLUSTER_WORDS + 2) * sizeof(uint32_t), "gysk_cluster_state: 6 fields and a pad");
+static_assert(sizeof(gysk_cluster_row) == 48, "gysk_cluster_row is 48 bytes");
+constexpr uint32_t MAX_CLUSTER_HOST = 1u << 24;		// gysk_set_cluster_map: host_of is indexed by host_idx
+
+// The host clusters on the device, passed by value to the cluster kernels. Each mapped host has a dense index, a cluster's hosts next to
+// each other in map order. host_acc gathers this engine's per-host sums during gysk_merge_prepare and is zero between merges (the host
+// pass clears what it reads).
+struct Clusters
+{
+	uint32_t		nc {0}, nh {0};				// clusters, mapped hosts
+	uint32_t		ntab {0};				// entries of host_of: 1 + the largest mapped host_idx
+	uint32_t		*host_of {nullptr};			// [ntab] host_idx -> dense host index, ~0u: in no cluster
+	uint32_t		*offs {nullptr};			// [nc + 1] the dense hosts of cluster c are offs[c] .. offs[c + 1] - 1
+	uint4			*host_acc {nullptr};			// [nh] {nlisten, nlisten_issue, tot_qps, tot_kb_inbound}, each mod 2^32
+	unsigned long long	*words {nullptr};			// SUM [nc][CLUSTER_WORDS] in the merge arena
+
+	__host__ __device__ __forceinline__ unsigned long long *words_of(uint32_t c) const { return words + CLUSTER_WORDS * (size_t)c; }
+};
+
+// the cluster map of gysk_set_cluster_map (GYSK_FLAG_MERGE_CLUSTERS)
+struct ClusterMap
+{
+	std::vector<uint64_t>	ids;					// dense index -> cluster id
+	std::unordered_map<uint64_t, uint32_t> index;		// cluster id -> dense index
+	Clusters		cl;
+	unsigned long long	*d_ids {nullptr};			// [nc] ids on the device: the ids of the rows
+	int32_t			*d_sorted {nullptr};			// [nc] dense indices by ascending cluster id (gysk_query_cluster_states_all)
+	int32_t			*d_sel {nullptr};			// [nc] the part of d_sorted an ACTIVE_ONLY read selects
+};
+
 // per-logical-service state of the merge step (SURVEY.md §8e)
 struct MergeState
 {
@@ -174,12 +206,13 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux] [, states]
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux] [, states] [, clusters]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt, flush tsec]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	std::string		name_sum, name_maxi64, name_maxu8;	// the regions' gysk_buffer_desc names: their arrays, in order
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
 	LogicalArrays		lg;
+	ClusterMap		clusters;				// kept across gysk_set_logical_map
 	bool			prepared {false}, finished {false};
 	void			*comm {nullptr};			// ncclComm_t of gysk_nccl_comm_init
 	uint32_t		comm_world {0};
@@ -255,6 +288,9 @@ struct gysk_engine
 };
 
 namespace gysk {
+
+// slot_last_active of the window the last flush closed (state_kernel): the active_mark of svc_evaluated / svc_issue
+inline uint32_t active_mark(const gysk_engine *e) { return e->last_flush_tsec ? e->last_flush_tsec : 1u; }
 
 int fail(gysk_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess);
 int post_launch(gysk_engine *e, const char *what);
@@ -347,6 +383,7 @@ static_assert(HLL_STAGE_REGS + (1u << 16) <= STAGE_BYTES, "the stage holds the f
 static_assert(QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES && 64 * sizeof(gysk_topn_entry) <= STAGE_BYTES, "the stage holds the flow and top-N rows");
 static_assert(sizeof(SlabEntry) <= STAGE_BYTES, "the stage holds one merged digest");
 static_assert(sizeof(gysk_logical_state) == 80 && sizeof(gysk_logical_state) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS state rows");
+static_assert(sizeof(gysk_cluster_row) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS cluster rows");
 
 // A staged read, engine mutex held. The optional input (ids, flow keys or logical indices) travels through h_qids / d_qids in pieces
 // of `piece` entries; without one (the window reads) the pieces only cut the n rows. For each piece, launch(d_in, off, m) writes m

@@ -1685,13 +1685,13 @@ __global__ void window_select_kernel(DevState st, uint32_t nslots, int is_task, 
 	uint32_t host = 0;
 	if (slot < nslots) {
 		host = is_task ? st.task_slot_host[slot] : st.slot_host[slot];
-		take = (is_task ? st.task_slot_id[slot] : st.slot_id[slot]) != 0 && (host_filter < 0 || host == (uint32_t)host_filter);
+		take = (is_task ? st.task_slot_id[slot] != 0 : svc_live(st, slot)) && (host_filter < 0 || host == (uint32_t)host_filter);
 		if (take && active_only) {
 			if (is_task) {
 				const HistCell *l = st.task_last + (size_t)slot * 3;
 				take = (l[0].count | l[1].count | l[2].count) != 0;
 			}
-			else take = st.slot_last_active[slot] == active_mark;
+			else take = svc_evaluated(st, slot, active_mark);
 		}
 		if (take && seen_before != ~0u) {
 			const uint32_t first = st.slot_first_seen[slot];
@@ -1741,8 +1741,7 @@ __global__ void host_listen_count_kernel(DevState st, const unsigned long long *
 	if (i >= n) return;
 	const unsigned long long key = keys[i];
 	const uint32_t slot = (uint32_t)key, head = host_bound(keys, 0, i, (uint32_t)(key >> 32), false);
-	const SlotState ss = st.slot_state[slot];
-	const bool issue = st.slot_last_active[slot] == active_mark && (ss.issue_bits & 1u), severe = issue && ss.state >= GYSK_STATE_SEVERE;
+	const bool issue = svc_issue(st, slot, active_mark), severe = issue && st.slot_state[slot].state >= GYSK_STATE_SEVERE;
 	const unsigned run = __match_any_sync(live, head);
 	const unsigned bi = __ballot_sync(run, issue), bs = __ballot_sync(run, severe);
 	if ((threadIdx.x & 31) == __ffs(run) - 1 && bi)

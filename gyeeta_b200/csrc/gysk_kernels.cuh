@@ -83,6 +83,17 @@ struct DevState
 	unsigned long long	*counters;				// [CTR_MAX]
 };
 
+// The service slot rules every per-host read shares (window reads, gysk_query_host_listen, the cluster fold). A slot below the table's
+// count is live while it holds an id. It was evaluated at the last flush when its last window with events is the one that flush closed
+// (active_mark, the rule of state_kernel). It is one of listener_stats_update's nissue (common/gy_socket_stat.cc:4242-4249) when it was
+// evaluated there with issue bit 0 set.
+__device__ __forceinline__ bool svc_live(const DevState &st, uint32_t slot) { return st.slot_id[slot] != 0; }
+__device__ __forceinline__ bool svc_evaluated(const DevState &st, uint32_t slot, uint32_t active_mark) { return st.slot_last_active[slot] == active_mark; }
+__device__ __forceinline__ bool svc_issue(const DevState &st, uint32_t slot, uint32_t active_mark)
+{
+	return svc_evaluated(st, slot, active_mark) && (st.slot_state[slot].issue_bits & 1u);
+}
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)

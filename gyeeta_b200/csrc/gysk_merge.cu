@@ -10,12 +10,14 @@
 //                            [i64 MAX region : max_val_seen_ last/all]   [u8 MAX region : HLL registers]
 //                          and a fixed t-digest slab (not element-wise mergeable); GYSK_FLAG_MERGE_LEVELS appends the rolling
 //                          levels and aux sums to the SUM region, their maxima, the rtt and the flush tsec pair to the i64 MAX one;
-//                          GYSK_FLAG_MERGE_STATES appends the members' LISTEN_SUMM_STATS words to the SUM region
-//   (caller)               all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
+//                          GYSK_FLAG_MERGE_STATES appends the members' LISTEN_SUMM_STATS words to the SUM region,
+//                          GYSK_FLAG_MERGE_CLUSTERS the host clusters' MS_CLUSTER_STATE words after them (gysk_set_cluster_map)
+//   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
 //   gysk_export_logical_hist / gysk_merge_flush_range   one merged histogram / the ranks' flush tsec range
 //   gysk_query_logical_states[_all]   the member listeners' state counts per logical service (GYSK_FLAG_MERGE_STATES)
+//   gysk_query_cluster_states[_all]   the service half of MS_CLUSTER_STATE per host cluster (GYSK_FLAG_MERGE_CLUSTERS)
 //
 // It is the additive roll-up of MS_CLUSTER_STATE::STATE_ONE::add_stats (common/gy_comm_proto.h:3199-3214) /
 // SHCONN_HANDLER::aggregate_cluster_state (server/gy_shconnhdlr.cc:4583) and of GY_HISTOGRAM::update_from_serialized
@@ -150,6 +152,46 @@ __global__ void fold_states_kernel(DevState st, Members mb, LogicalArrays lg)
 	w[8] = qps; w[9] = act; w[10] = kb_in; w[11] = 0; w[12] = ser; w[13] = nlisten; w[14] = nactive;	// tot_kb_outbound: the encoder's 0
 }
 
+// GYSK_FLAG_MERGE_CLUSTERS, pass 1, one thread per service slot: each live slot of a mapped host adds {1, issue, nqrys_5s / 5, kbytes_5s}
+// to its host's words. The first two are the host's gysk_query_host_listen counts (svc_live, svc_issue); the last two are
+// LISTEN_SUMM_STATS::update of the record gysk_encode_listener_state writes from the slot's window row, as fold_states_kernel takes them:
+// nqrys_5s through cells_total truncated to 32 bits, curr_kbytes_inbound_ the last window's kbytes (curr_kbytes_outbound_ is the
+// encoder's 0). Sums mod 2^32 do not depend on the order of the atomics.
+__global__ void fold_cluster_hosts_kernel(DevState st, uint32_t max_svcs, uint32_t active_mark, Clusters cl)
+{
+	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
+	if (slot >= min(*st.svc_tbl.count, max_svcs) || !svc_live(st, slot)) return;
+	const uint32_t host = st.slot_host[slot], h = host < cl.ntab ? cl.host_of[host] : ~0u;
+	if (h == ~0u) return;
+	uint4 *a = cl.host_acc + h;
+	atomicAdd(&a->x, 1u);
+	if (svc_issue(st, slot, active_mark)) atomicAdd(&a->y, 1u);
+	if (st.slot_state[slot].state > GYSK_STATE_DOWN) return;		// never reaches summstats.update (gy_mconnhdlr.cc:11183-11251)
+	uint64_t counts[15];
+	const uint32_t nqrys_5s = (uint32_t)cells_total(st.hist_last + (size_t)slot * HIST_CELLS, 15, counts);
+	atomicAdd(&a->z, nqrys_5s / 5);
+	atomicAdd(&a->w, (uint32_t)(st.conn_last[slot] >> 32));
+}
+
+// GYSK_FLAG_MERGE_CLUSTERS, pass 2, one thread per cluster: each of its hosts with a live service on this engine adds the service half of
+// CLUSTER_STATE_ONE::update_from_state (server/gy_mconnhdlr.cc:16032-16050), svc_net_mb = (tot_kb_inbound + tot_kb_outbound) / 1024 in
+// int32 per host (:16045). Each host's words are cleared for the next merge once read.
+__global__ void fold_clusters_kernel(Clusters cl)
+{
+	const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+	if (c >= cl.nc) return;
+	uint32_t nhosts = 0, issue = 0, issue_hosts = 0, nsvc = 0, qps = 0, mb = 0;
+	for (uint32_t h = cl.offs[c]; h < cl.offs[c + 1]; ++h) {
+		const uint4 a = cl.host_acc[h];
+		if (!a.x) continue;
+		cl.host_acc[h] = make_uint4(0, 0, 0, 0);
+		nhosts++; issue += a.y; issue_hosts += a.y != 0; nsvc += a.x; qps += a.z;
+		mb += (uint32_t)((int32_t)a.w / 1024);
+	}
+	unsigned long long *w = cl.words_of(c);
+	w[0] = nhosts; w[1] = issue; w[2] = issue_hosts; w[3] = nsvc; w[4] = qps; w[5] = mb;
+}
+
 // one thread per (logical, 4 registers): per-byte max over the member services
 __global__ void fold_hll_kernel(DevState st, Members mb, LogicalArrays lg)
 {
@@ -269,18 +311,23 @@ __device__ __forceinline__ bool logical_active(const LogicalArrays &lg, uint32_t
 	return any != 0;
 }
 
-// One CTA walks the dense indices in ascending logical id and keeps the active ones, in order: tile_rank places the kept entries of
-// each 1024-entry tile. *d_n = entries kept.
-__global__ void __launch_bounds__(1024) logical_select_kernel(const int32_t *__restrict__ sorted, LogicalArrays lg, int32_t *__restrict__ sel,
+// the GYSK_WINDOW_ACTIVE_ONLY rule of each all-rows read: a logical service as logical_active, a cluster with a live service on some rank
+struct LogicalActive { LogicalArrays lg; __device__ __forceinline__ bool operator()(uint32_t l) const { return logical_active(lg, l); } };
+struct ClusterActive { Clusters cl; __device__ __forceinline__ bool operator()(uint32_t c) const { return (uint32_t)cl.words_of(c)[3] != 0; } };
+
+// One CTA walks the n dense indices of `sorted` (ascending id) and keeps the active ones, in order: tile_rank places the kept entries
+// of each 1024-entry tile. *d_n = entries kept.
+template <typename Active>
+__global__ void __launch_bounds__(1024) logical_select_kernel(const int32_t *__restrict__ sorted, uint32_t n, Active active, int32_t *__restrict__ sel,
 		unsigned long long *d_n)
 {
 	__shared__ uint32_t wcnt[32];
 	uint32_t running = 0;
 
-	for (uint32_t t = 0; t < lg.nl; t += 1024) {
+	for (uint32_t t = 0; t < n; t += 1024) {
 		const uint32_t i = t + threadIdx.x;
-		const int32_t l = i < lg.nl ? sorted[i] : 0;
-		const bool keep = i < lg.nl && logical_active(lg, (uint32_t)l);
+		const int32_t l = i < n ? sorted[i] : 0;
+		const bool keep = i < n && active((uint32_t)l);
 		tile_rank(keep, wcnt, running, [&](uint32_t r) { sel[r] = l; });
 	}
 	if (threadIdx.x == 0) *d_n = running;
@@ -328,6 +375,25 @@ __global__ void logical_state_kernel(const int32_t *__restrict__ lidx, uint32_t 
 	out[q] = o;
 }
 
+// GYSK_FLAG_MERGE_CLUSTERS read side, one thread per row: the merged words of dense index cidx[q], each truncated to 32 bits (the uint32
+// wrap-around sum), cluster id cids[c]; an index of -1 gives an all-zero row
+__global__ void cluster_row_kernel(const int32_t *__restrict__ cidx, uint32_t n, Clusters cl, const unsigned long long *__restrict__ cids,
+		gysk_cluster_row *__restrict__ out)
+{
+	const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+	if (q >= n) return;
+	const int32_t c = cidx[q];
+	gysk_cluster_row o;
+	memset(&o, 0, sizeof(o));
+	if (c >= 0) {
+		const unsigned long long *w = cl.words_of((uint32_t)c);
+		o.cluster_id = cids[c]; o.found = 1;
+		o.st.nhosts = (uint32_t)w[0]; o.st.nsvc_issue = (uint32_t)w[1]; o.st.nsvcissue_hosts = (uint32_t)w[2];
+		o.st.nsvc = (uint32_t)w[3]; o.st.total_qps = (uint32_t)w[4]; o.st.svc_net_mb = (uint32_t)w[5];
+	}
+	out[q] = o;
+}
+
 } // namespace gysk
 
 namespace {
@@ -335,16 +401,42 @@ namespace {
 inline uint32_t div_up(uint64_t a, uint64_t b) { return (uint32_t)((a + b - 1) / b); }
 inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
-// dense index of a logical id, -1 for an id the map does not have
-int32_t logical_index(const MergeState &mg, uint64_t id)
+// dense index of a logical (or cluster) id, -1 for an id the map does not have
+int32_t dense_index(const std::unordered_map<uint64_t, uint32_t> &index, uint64_t id)
 {
-	const auto it = mg.index.find(id);
-	return it == mg.index.end() ? -1 : (int32_t)it->second;
+	const auto it = index.find(id);
+	return it == index.end() ? -1 : (int32_t)it->second;
+}
+int32_t logical_index(const MergeState &mg, uint64_t id) { return dense_index(mg.index, id); }
+
+// The dense index space of a row type: the logical services (service and state rows) or the host clusters (cluster rows). sorted holds
+// the n indices by ascending id, sel the ACTIVE_ONLY part of them; select launches the selection (*d_n = indices kept).
+struct RowSpace
+{
+	const std::unordered_map<uint64_t, uint32_t> *index;
+	uint32_t n;
+	const int32_t *sorted;
+	int32_t *sel;
+};
+template <typename Row> RowSpace row_space(MergeState &mg, const Row *) { return RowSpace {&mg.index, mg.lg.nl, mg.d_sorted, mg.d_sel}; }
+RowSpace row_space(MergeState &mg, const gysk_cluster_row *)
+{
+	const ClusterMap &cm = mg.clusters;
+	return RowSpace {&cm.index, cm.cl.nc, cm.d_sorted, cm.d_sel};
+}
+template <typename Row> void launch_select(gysk_engine *e, const Row *, unsigned long long *d_n)
+{
+	logical_select_kernel<<<1, 1024, 0, e->stream>>>(e->mg.d_sorted, e->mg.lg.nl, LogicalActive {e->mg.lg}, e->mg.d_sel, d_n);
+}
+void launch_select(gysk_engine *e, const gysk_cluster_row *, unsigned long long *d_n)
+{
+	const ClusterMap &cm = e->mg.clusters;
+	logical_select_kernel<<<1, 1024, 0, e->stream>>>(cm.d_sorted, cm.cl.nc, ClusterActive {cm.cl}, cm.d_sel, d_n);
 }
 
-// Per row type of the logical reads: the launch that makes the rows of the dense indices lidx[0 .. m) in the device stage (an index
-// of -1 gives the not-found row), the finish that copies them out, the field a by-id read stamps with the queried id, and the engine
-// flag the rows need.
+// Per row type of the logical and cluster reads: the launch that makes the rows of the dense indices lidx[0 .. m) in the device stage
+// (an index of -1 gives the not-found row), the finish that copies them out, the field a by-id read stamps with the queried id, and the
+// engine flag the rows need.
 int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_summary *)
 {
 	logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(lidx, m, e->cfg.hll_p, e->mg.lg, e->mg.d_logical_ids,
@@ -356,13 +448,24 @@ int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical
 	logical_state_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(lidx, m, e->mg.lg, e->mg.d_logical_ids, reinterpret_cast<gysk_logical_state *>(e->d_wstage));
 	return 1;
 }
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_cluster_row *)
+{
+	cluster_row_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(lidx, m, e->mg.clusters.cl, e->mg.clusters.d_ids, reinterpret_cast<gysk_cluster_row *>(e->d_wstage));
+	return 1;
+}
 SvcRows logical_finish(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
 CopyRows<gysk_logical_state> logical_finish(const gysk_engine *, gysk_logical_state *out) { return CopyRows<gysk_logical_state> {out}; }
+CopyRows<gysk_cluster_row> logical_finish(const gysk_engine *, gysk_cluster_row *out) { return CopyRows<gysk_cluster_row> {out}; }
 uint64_t &row_id(gysk_svc_summary &r) { return r.glob_id; }
 uint64_t &row_id(gysk_logical_state &r) { return r.logical_id; }
-template <typename Row> constexpr uint32_t logical_flag() { return std::is_same<Row, gysk_logical_state>::value ? GYSK_FLAG_MERGE_STATES : 0; }
+uint64_t &row_id(gysk_cluster_row &r) { return r.cluster_id; }
+template <typename Row> constexpr uint32_t logical_flag()
+{
+	return std::is_same<Row, gysk_logical_state>::value ? GYSK_FLAG_MERGE_STATES : std::is_same<Row, gysk_cluster_row>::value ? GYSK_FLAG_MERGE_CLUSTERS : 0;
+}
 
-// gysk_query_logical / gysk_query_logical_states: the rows of n logical ids, in QCHUNK pieces, each row carrying its queried id
+// gysk_query_logical / gysk_query_logical_states / gysk_query_cluster_states: the rows of n ids, in QCHUNK pieces, each row carrying its
+// queried id
 template <typename Row>
 int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out, const char *what)
 {
@@ -373,8 +476,9 @@ int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, (std::string("gysk_") + what + ": no finished merge").c_str());
 
+	const RowSpace sp = row_space(mg, out);
 	std::vector<int32_t> lidx(n);
-	for (uint32_t i = 0; i < n; ++i) lidx[i] = logical_index(mg, ids[i]);
+	for (uint32_t i = 0; i < n; ++i) lidx[i] = dense_index(*sp.index, ids[i]);
 	const auto rows = logical_finish(e, out);
 	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(Row), what, [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
 		return launch_logical(e, reinterpret_cast<const int32_t *>(d_l), m, out);
@@ -384,8 +488,8 @@ int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out
 	});
 }
 
-// gysk_query_logical_all / gysk_query_logical_states_all: every logical service's row in ascending logical id (the uploaded permutation,
-// compacted on the device by logical_select_kernel under ACTIVE_ONLY), in WIN_ROWS pieces; *n = rows that match
+// gysk_query_logical_all / gysk_query_logical_states_all / gysk_query_cluster_states_all: every row of the index space in ascending id
+// (the uploaded permutation, compacted on the device by logical_select_kernel under ACTIVE_ONLY), in WIN_ROWS pieces; *n = rows that match
 template <typename Row>
 int logical_all_rows(gysk_engine *e, uint32_t flags, Row *out, uint32_t cap, uint32_t *n, const char *what)
 {
@@ -396,17 +500,18 @@ int logical_all_rows(gysk_engine *e, uint32_t flags, Row *out, uint32_t cap, uin
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, (std::string("gysk_") + what + ": no finished merge").c_str());
 
-	uint32_t total = mg.lg.nl;
-	const int32_t *sel = mg.d_sorted;
+	const RowSpace sp = row_space(mg, out);
+	uint32_t total = sp.n;
+	const int32_t *sel = sp.sorted;
 	if ((flags & GYSK_WINDOW_ACTIVE_ONLY) && total) {
 		unsigned long long *d_n = e->st.counters + CTR_NWINDOW, cnt = 0;
-		logical_select_kernel<<<1, 1024, 0, e->stream>>>(mg.d_sorted, mg.lg, mg.d_sel, d_n);
+		launch_select(e, out, d_n);
 		e->kernel_launches++;
 		CU(e, cudaMemcpyAsync(&cnt, d_n, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
 		CU(e, cudaStreamSynchronize(e->stream));
 		if (int rc = post_launch(e, (std::string(what) + " select").c_str())) return rc;
 		total = (uint32_t)cnt;
-		sel = mg.d_sel;
+		sel = sp.sel;
 	}
 	int rc = staged_read<uint64_t>(e, nullptr, std::min(cap, total), WIN_ROWS, sizeof(Row), what,
 			[&](const unsigned long long *, uint32_t off, uint32_t m) { return launch_logical(e, sel + off, m, out); }, logical_finish(e, out));
@@ -481,60 +586,48 @@ void merge_release(gysk_engine *e)
 } // namespace gysk
 
 
-extern "C" {
+namespace {
 
-int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *logical_ids, uint32_t n)
+// A map's keys as dense indices in order of first appearance (identical on every rank when the same list is passed): ids[dense] = key,
+// index[key] = dense. offs / pos: the list positions of each dense index in list order, CSR. sorted: the dense indices by ascending key.
+struct DenseMap { std::vector<uint32_t> offs, pos; std::vector<int32_t> sorted; };
+DenseMap dense_map(const uint64_t *keys, uint32_t n, std::vector<uint64_t> &ids, std::unordered_map<uint64_t, uint32_t> &index)
 {
-	CHECK_ENGINE(e);
-	if ((!glob_ids || !logical_ids) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e, Sync);
-
-	MergeState &mg = e->mg;
-
-	// dense logical index in order of first appearance: identical on every rank when the same list is passed
-	mg.index.clear(); mg.logical_ids.clear();
-	std::vector<uint32_t> lidx(n);
+	index.clear(); ids.clear();
+	std::vector<uint32_t> dense(n);
 	for (uint32_t i = 0; i < n; ++i) {
-		auto it = mg.index.find(logical_ids[i]);
-		if (it == mg.index.end()) {
-			it = mg.index.emplace(logical_ids[i], (uint32_t)mg.logical_ids.size()).first;
-			mg.logical_ids.push_back(logical_ids[i]);
+		auto it = index.find(keys[i]);
+		if (it == index.end()) {
+			it = index.emplace(keys[i], (uint32_t)ids.size()).first;
+			ids.push_back(keys[i]);
 		}
-		lidx[i] = it->second;
+		dense[i] = it->second;
 	}
-	const uint32_t nl = (uint32_t)mg.logical_ids.size();
+	const uint32_t nd = (uint32_t)ids.size();
+	DenseMap m {std::vector<uint32_t>(nd + 1, 0), std::vector<uint32_t>(n), std::vector<int32_t>(nd)};
+	for (uint32_t i = 0; i < n; ++i) m.offs[dense[i] + 1]++;
+	for (uint32_t d = 0; d < nd; ++d) m.offs[d + 1] += m.offs[d];
+	std::vector<uint32_t> cur(m.offs.begin(), m.offs.end() - 1);
+	for (uint32_t i = 0; i < n; ++i) m.pos[cur[dense[i]]++] = i;
+	for (uint32_t d = 0; d < nd; ++d) m.sorted[d] = (int32_t)d;
+	std::sort(m.sorted.begin(), m.sorted.end(), [&](int32_t a, int32_t b) { return ids[a] < ids[b]; });
+	return m;
+}
 
-	// CSR logical -> every {glob_id} mapped to it, in map order; the slots are looked up at merge time (resolve_members_kernel)
-	std::vector<uint32_t> offs(nl + 1, 0);
-	std::vector<uint64_t> member_ids(n);
-	for (uint32_t i = 0; i < n; ++i) offs[lidx[i] + 1]++;
-	for (uint32_t l = 0; l < nl; ++l) offs[l + 1] += offs[l];
-	{
-		std::vector<uint32_t> cur(offs.begin(), offs.end() - 1);
-		for (uint32_t i = 0; i < n; ++i) member_ids[cur[lidx[i]]++] = glob_ids[i];
-	}
-
-	// dense indices by ascending logical id: the row order of gysk_query_logical_all
-	std::vector<int32_t> sorted(nl);
-	for (uint32_t l = 0; l < nl; ++l) sorted[l] = (int32_t)l;
-	std::sort(sorted.begin(), sorted.end(), [&](int32_t a, int32_t b) { return mg.logical_ids[a] < mg.logical_ids[b]; });
-
-	// (re)allocate the arena
-	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
-	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel);
-	{
-		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
-		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
-		mg = MergeState {};
-		mg.logical_ids = std::move(ids_keep); mg.index = std::move(idx_keep);
-	}
+// (Re)allocates the arena for the logical and cluster maps the engine holds; the last merge's results go with the old one.
+int lay_out_arena(gysk_engine *e)
+{
+	MergeState &mg = e->mg;
 	LogicalArrays &lg = mg.lg;
-	lg.nl = nl;
+	const uint32_t nl = lg.nl;
+	dfree(e, mg.arena);
+	mg.prepared = mg.finished = false;
 
 	// The arena region by region, each array 256-byte aligned: layout(nullptr) sizes it, layout(arena) places the arrays. Each array's
 	// name joins its region's gysk_merge_buffers name. GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX
-	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them: still three regions, three collectives.
-	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES;
+	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those:
+	// still three regions, three collectives.
+	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
@@ -549,6 +642,7 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 		take(lg.last, b_hist, "hist_last"); take(lg.all, b_hist, "hist_all"); take(lg.conn, (size_t)nl * 4 * 8, "conn");
 		if (levels) { take(lg.lvl, NLEVELS * b_hist, "levels"); take(lg.aux, (size_t)nl * 4 * 8, "aux"); }
 		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8, "states");
+		if (clusters) take(mg.clusters.cl.words, (size_t)mg.clusters.cl.nc * CLUSTER_WORDS * 8, "clusters");
 		mg.bytes_sum = off - mg.off_sum;
 		mg.name_sum = "sum_u64: " + names;
 		names.clear();
@@ -568,6 +662,35 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	int rc = dalloc(e, &mg.arena, mg.arena_bytes);
 	if (rc) return rc;
 	layout(mg.arena);
+	return 0;
+}
+
+// gysk_set_logical_map, engine held
+int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *logical_ids, uint32_t n)
+{
+	MergeState &mg = e->mg;
+
+	// dense logical index in order of first appearance; CSR logical -> every {glob_id} mapped to it, in map order (the slots are looked
+	// up at merge time, resolve_members_kernel); dense indices by ascending logical id: the row order of gysk_query_logical_all
+	const DenseMap dm = dense_map(logical_ids, n, mg.logical_ids, mg.index);
+	const uint32_t nl = (uint32_t)mg.logical_ids.size();
+	std::vector<uint64_t> member_ids(n);
+	for (uint32_t k = 0; k < n; ++k) member_ids[k] = glob_ids[dm.pos[k]];
+
+	// (re)allocate the arena
+	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
+	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel);
+	{
+		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
+		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
+		ClusterMap clusters_keep(std::move(mg.clusters));
+		mg = MergeState {};
+		mg.logical_ids = std::move(ids_keep); mg.index = std::move(idx_keep); mg.clusters = std::move(clusters_keep);
+	}
+	LogicalArrays &lg = mg.lg;
+	lg.nl = nl;
+	int rc = lay_out_arena(e);
+	if (rc) return rc;
 	if ((rc = dalloc(e, &lg.slab, nl ? nl : 1))) return rc;
 	if ((rc = dalloc(e, &lg.final_slab, nl ? nl : 1))) return rc;
 	if ((rc = dalloc(e, &mg.members.offs, (size_t)nl + 1))) return rc;
@@ -579,14 +702,74 @@ int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_
 	if ((rc = dalloc(e, &mg.d_sel, nl ? nl : 1))) return rc;
 	if (nl) {
 		CU(e, cudaMemcpyAsync(mg.d_logical_ids, mg.logical_ids.data(), (size_t)nl * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-		CU(e, cudaMemcpyAsync(mg.d_sorted, sorted.data(), (size_t)nl * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
+		CU(e, cudaMemcpyAsync(mg.d_sorted, dm.sorted.data(), (size_t)nl * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
 	}
 	// the member slots are written by resolve_members_kernel at every merge, before any fold reads them
 	mg.nmembers = n;
 	if (n) CU(e, cudaMemcpyAsync(mg.d_member_ids, member_ids.data(), (size_t)n * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
-	CU(e, cudaMemcpyAsync(mg.members.offs, offs.data(), ((size_t)nl + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+	CU(e, cudaMemcpyAsync(mg.members.offs, dm.offs.data(), ((size_t)nl + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
 	return post_launch(e, "set_logical_map");
+}
+
+} // namespace
+
+extern "C" {
+
+int gysk_set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *logical_ids, uint32_t n)
+{
+	CHECK_ENGINE(e);
+	if ((!glob_ids || !logical_ids) && n) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Sync);
+	return set_logical_map(e, glob_ids, logical_ids, n);
+}
+
+int gysk_set_cluster_map(gysk_engine *e, const uint32_t *host_idxs, const uint64_t *cluster_ids, uint32_t n)
+{
+	CHECK_ENGINE(e);
+	if ((!host_idxs || !cluster_ids) && n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS)) return GYSK_ERR_NOTSUP;
+	uint32_t ntab = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		if (host_idxs[i] >= MAX_CLUSTER_HOST) return GYSK_ERR_INVAL;
+		ntab = std::max(ntab, host_idxs[i] + 1);
+	}
+	// host -> dense host index: the hosts of each cluster next to each other, in map order
+	std::vector<uint32_t> host_of(ntab, ~0u);
+	std::vector<uint64_t> ids;
+	std::unordered_map<uint64_t, uint32_t> index;
+	const DenseMap dm = dense_map(cluster_ids, n, ids, index);
+	for (uint32_t k = 0; k < n; ++k) {
+		uint32_t &h = host_of[host_idxs[dm.pos[k]]];
+		if (h != ~0u) return GYSK_ERR_INVAL;			// a host listed twice
+		h = k;
+	}
+	GYSK_ENTER(e, Sync);
+	MergeState &mg = e->mg;
+	ClusterMap &cm = mg.clusters;
+	dfree(e, cm.cl.host_of); dfree(e, cm.cl.offs); dfree(e, cm.cl.host_acc); dfree(e, cm.d_ids); dfree(e, cm.d_sorted); dfree(e, cm.d_sel);
+	cm = ClusterMap {};
+	cm.ids = std::move(ids); cm.index = std::move(index);
+	Clusters &cl = cm.cl;
+	cl.nc = (uint32_t)cm.ids.size(); cl.nh = n; cl.ntab = ntab;
+	int rc = 0;
+	if ((rc = dalloc(e, &cl.host_of, ntab ? ntab : 1, false))) return rc;
+	if ((rc = dalloc(e, &cl.offs, (size_t)cl.nc + 1, false))) return rc;
+	if ((rc = dalloc(e, &cl.host_acc, n ? n : 1))) return rc;			// zeroed: the host pass keeps it so between merges
+	if ((rc = dalloc(e, &cm.d_ids, cl.nc ? cl.nc : 1, false))) return rc;
+	if ((rc = dalloc(e, &cm.d_sorted, cl.nc ? cl.nc : 1, false))) return rc;
+	if ((rc = dalloc(e, &cm.d_sel, cl.nc ? cl.nc : 1, false))) return rc;
+	if (ntab) CU(e, cudaMemcpyAsync(cl.host_of, host_of.data(), (size_t)ntab * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+	CU(e, cudaMemcpyAsync(cl.offs, dm.offs.data(), ((size_t)cl.nc + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+	if (cl.nc) {
+		CU(e, cudaMemcpyAsync(cm.d_ids, cm.ids.data(), (size_t)cl.nc * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
+		CU(e, cudaMemcpyAsync(cm.d_sorted, dm.sorted.data(), (size_t)cl.nc * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream));
+	}
+	// the arena, or with no logical map yet an empty one (which lays out the arena): a merge of clusters alone needs nothing more
+	rc = mg.lg.slab ? lay_out_arena(e) : set_logical_map(e, nullptr, nullptr, 0);
+	if (rc) return rc;
+	CU(e, cudaStreamSynchronize(e->stream));
+	return post_launch(e, "set_cluster_map");
 }
 
 int gysk_merge_prepare(gysk_engine *e)
@@ -619,6 +802,11 @@ int gysk_merge_prepare(gysk_engine *e)
 		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.members,
 				(long long)e->last_flush_tsec, mg.lg);
 		e->kernel_launches++;
+	}
+	if (const uint32_t nc = mg.clusters.cl.nc) {		// GYSK_FLAG_MERGE_CLUSTERS with a cluster map
+		fold_cluster_hosts_kernel<<<div_up(e->cfg.max_svcs, 256), 256, 0, e->stream>>>(e->st, e->cfg.max_svcs, active_mark(e), mg.clusters.cl);
+		fold_clusters_kernel<<<div_up(nc, 256), 256, 0, e->stream>>>(mg.clusters.cl);
+		e->kernel_launches += 2;
 	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
@@ -688,6 +876,18 @@ int gysk_query_logical_states(gysk_engine *e, const uint64_t *logical_ids, uint3
 int gysk_query_logical_states_all(gysk_engine *e, uint32_t flags, gysk_logical_state *out, uint32_t cap, uint32_t *n)
 {
 	return logical_all_rows(e, flags, out, cap, n, "query_logical_states_all");
+}
+
+// GYSK_FLAG_MERGE_CLUSTERS: the merged service half of MS_CLUSTER_STATE of cluster ids, rows made on the device (cluster_row_kernel)
+int gysk_query_cluster_states(gysk_engine *e, const uint64_t *cluster_ids, uint32_t n, gysk_cluster_row *out)
+{
+	return logical_query_rows(e, cluster_ids, n, out, "query_cluster_states");
+}
+
+// GYSK_FLAG_MERGE_CLUSTERS: every cluster's row in ascending cluster id
+int gysk_query_cluster_states_all(gysk_engine *e, uint32_t flags, gysk_cluster_row *out, uint32_t cap, uint32_t *n)
+{
+	return logical_all_rows(e, flags, out, cap, n, "query_cluster_states_all");
 }
 
 int gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS], uint64_t *total,

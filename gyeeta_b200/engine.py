@@ -32,7 +32,7 @@ assert RESP16_DTYPE.itemsize == 16 and TCP24_DTYPE.itemsize == 24 and TASK24_DTY
 NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CONN_STATS = 0x309, 0x30C, 0x310, 0x312
 (HOSTTOP_SVC_ISSUE, HOSTTOP_SVC_QPS, HOSTTOP_SVC_CONNS, HOSTTOP_SVC_NET, HOSTTOP_TASK_ISSUE, HOSTTOP_TASK_NET, HOSTTOP_TASK_CPU, HOSTTOP_TASK_RSS,
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
-FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES = 1, 2, 4
+FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS = 1, 2, 4, 8
 TD_CAP = 256
 
 
@@ -148,6 +148,14 @@ class ClusterState(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("nhosts", "nsvc_issue", "nsvcissue_hosts", "nsvc", "total_qps", "svc_net_mb")] + [("pad", C.c_uint32 * 2)]
 
 
+class ClusterRow(C.Structure):
+    """gysk_cluster_row: the service half of MS_CLUSTER_STATE of one host cluster over every rank (GYSK_FLAG_MERGE_CLUSTERS)"""
+    _fields_ = [("cluster_id", C.c_uint64), ("found", C.c_int32), ("pad", C.c_uint32), ("st", ClusterState)]
+
+
+assert C.sizeof(ClusterRow) == 48
+
+
 class TopnEntry(C.Structure):
     _fields_ = [("glob_id", C.c_uint64), ("score", C.c_uint64), ("host_idx", C.c_uint32), ("pad", C.c_uint32)]
 
@@ -244,6 +252,9 @@ def load_library(path=None):
         "gysk_export_logical_hll": (i32, [vp, u64, vp]),
         "gysk_query_logical_states": (i32, [vp, vp, u32, vp]),
         "gysk_query_logical_states_all": (i32, [vp, u32, vp, u32, vp]),
+        "gysk_set_cluster_map": (i32, [vp, vp, vp, u32]),
+        "gysk_query_cluster_states": (i32, [vp, vp, u32, vp]),
+        "gysk_query_cluster_states_all": (i32, [vp, u32, vp, u32, vp]),
         "gysk_query_flows_global": (i32, [vp, vp, u32, i32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
@@ -270,7 +281,7 @@ class Engine:
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
-                 merge_levels=False, merge_states=False):
+                 merge_levels=False, merge_states=False, merge_clusters=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -280,7 +291,7 @@ class Engine:
         cfg.stage_batch = stage_batch
         cfg.idle_evict_secs = idle_evict_secs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
-                    (FLAG_MERGE_STATES if merge_states else 0)
+                    (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -583,6 +594,13 @@ class Engine:
         assert len(g) == len(l)
         self._chk(self.L.gysk_set_logical_map(self.h, _p(g), _p(l), len(g)))
 
+    def set_cluster_map(self, host_idxs, cluster_ids):
+        """gysk_set_cluster_map: host_idxs[i] belongs to cluster cluster_ids[i] (merge_clusters=True)"""
+        h = np.ascontiguousarray(host_idxs, dtype=np.uint32)
+        c = np.ascontiguousarray(cluster_ids, dtype=np.uint64)
+        assert len(h) == len(c)
+        self._chk(self.L.gysk_set_cluster_map(self.h, _p(h), _p(c), len(h)))
+
     def merge_prepare(self):
         self._chk(self.L.gysk_merge_prepare(self.h))
 
@@ -665,6 +683,17 @@ class Engine:
     def query_logical_states_all(self, active_only=False, cap=None):
         """gysk_query_logical_states_all: (LogicalState rows in ascending logical id, number of matching rows); cap as query_logical_all"""
         return self._window(self.L.gysk_query_logical_states_all, LogicalState, (), active_only, cap)
+
+    def query_cluster_states(self, ids):
+        """gysk_query_cluster_states: ClusterRow rows of cluster ids from the last merge (merge_clusters=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (ClusterRow * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_cluster_states(self.h, _p(ids), len(ids), out))
+        return out[: len(ids)]
+
+    def query_cluster_states_all(self, active_only=False, cap=None):
+        """gysk_query_cluster_states_all: (ClusterRow rows in ascending cluster id, number of matching rows); cap as query_logical_all"""
+        return self._window(self.L.gysk_query_cluster_states_all, ClusterRow, (), active_only, cap)
 
     def merge_flush_range(self):
         """gysk_merge_flush_range: (earliest, latest) tsec of the ranks' last flush, as the last merge all-reduced them"""

@@ -326,4 +326,32 @@ private :
 	std::vector<gysk_svc_summary> summ_;
 };
 
+// MCONN_HANDLER::send_cluster_state (server/gy_mconnhdlr.cc:16052-16110) with GYSK_FLAG_MERGE_CLUSTERS: the service half of one
+// MS_CLUSTER_STATE::STATE_ONE (common/gy_comm_proto.h:3181-3216) from a gysk_query_cluster_states row, every rank's hosts included.
+// StateOne is comm::MS_CLUSTER_STATE::STATE_ONE (or a POD mirror); its other fields are left as they are.
+template <typename StateOne>
+void cluster_state_one(const gysk_cluster_row & r, StateOne & one) noexcept
+{
+	one.nhosts_		= r.st.nhosts;
+	one.nsvc_issue_		= r.st.nsvc_issue;
+	one.nsvcissue_hosts_	= r.st.nsvcissue_hosts;
+	one.nsvc_		= r.st.nsvc;
+	one.total_qps_		= r.st.total_qps;
+	one.svc_net_mb_		= r.st.svc_net_mb;
+}
+
+// ... and the rest of CLUSTER_STATE_ONE::update_from_state (:16032-16050) for one of this madhava's hosts of the cluster, from its
+// HOST_STATE_NOTIFY (comm::HOST_STATE_NOTIFY, as host_state filled it): the task, cpu and memory counters, and nhosts_ for a host the
+// engine did not count because it has no live service (nlisten_ == 0)
+template <typename StateOne, typename HostStateNotify>
+void cluster_add_host_state(StateOne & one, const HostStateNotify & state) noexcept
+{
+	one.nhosts_		+= !state.nlisten_;
+	one.ntasks_issue_	+= state.ntasks_issue_;
+	one.ntaskissue_hosts_	+= !!state.ntasks_issue_;
+	one.ntasks_		+= state.ntasks_;
+	one.ncpu_issue_		+= state.cpu_issue_;
+	one.nmem_issue_		+= state.mem_issue_;
+}
+
 } // namespace gysk_shim

@@ -195,6 +195,9 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   logical service (LISTEN_SUMM_STATS per logical service: gysk_query_logical_states,
 						   GYSK_TOPN_ISSUE of gysk_topn_logical); with or without GYSK_FLAG_MERGE_LEVELS, the
 						   same flags on every rank. Without it the merge arena and its collectives are as before */
+#define GYSK_FLAG_MERGE_CLUSTERS	0x8u	/* the merge step also rolls up the service state of each host cluster (gysk_set_cluster_map,
+						   gysk_query_cluster_states); combines freely with the two flags above, the same flags on
+						   every rank. Without it the merge arena and its collectives are as before */
 
 typedef struct gysk_config
 {
@@ -274,7 +277,7 @@ typedef struct gysk_host_summary
  * memory issue counters come from the host agent's HOST_STATE_NOTIFY and stay zero here. */
 typedef struct gysk_cluster_state
 {
-	uint32_t	nhosts;			/* hosts with a listener-state summary */
+	uint32_t	nhosts;			/* hosts with a listener-state summary (gysk_cluster_row: hosts with a live service) */
 	uint32_t	nsvc_issue;		/* listeners in STATE_BAD / STATE_SEVERE / STATE_DOWN */
 	uint32_t	nsvcissue_hosts;	/* hosts with at least one such listener */
 	uint32_t	nsvc;			/* += nlisteners */
@@ -623,6 +626,39 @@ typedef struct gysk_logical_state
 int		gysk_query_logical_states(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_logical_state *out);
 /* one row per logical service: the ids, order, GYSK_WINDOW_ACTIVE_ONLY set and count / capacity rules of gysk_query_logical_all */
 int		gysk_query_logical_states_all(gysk_engine *e, uint32_t flags, gysk_logical_state *out, uint32_t cap, uint32_t *n);
+
+/* ---- host clusters (GYSK_FLAG_MERGE_CLUSTERS): MS_CLUSTER_STATE across every rank ----
+ * Which host belongs to which cluster: host_idxs[i] -> cluster_ids[i] (the caller hashes PARTHA_INFO::cluster_name_ into the id). The same
+ * list on every rank; dense cluster indices follow first appearance. A host that is not in the list belongs to no cluster; a host listed
+ * twice is GYSK_ERR_INVAL, as is a host_idx >= 2^24. GYSK_ERR_NOTSUP without the flag. The call may come before or after
+ * gysk_set_logical_map: either one lays out the merge arena again (the last merge's results are gone), and each keeps the other's map. A
+ * merge of clusters alone needs no gysk_set_logical_map: this call also sets up an empty logical map when the engine has none. */
+int		gysk_set_cluster_map(gysk_engine *e, const uint32_t *host_idxs, const uint64_t *cluster_ids, uint32_t n);
+/* One cluster's row. st is the service half of CLUSTER_STATE_ONE::update_from_state (server/gy_mconnhdlr.cc:16032-16050), summed over
+ * every host of the cluster on every rank; each uint32 wraps, as the reference's counters do. For each host with at least one live
+ * service (a row of gysk_query_window_hosts(-1, 0)), with nlisten / nlisten_issue its gysk_query_host_listen row:
+ *   nhosts += 1, nsvc += nlisten, nsvc_issue += nlisten_issue, nsvcissue_hosts += !!nlisten_issue,
+ * and with LISTEN_SUMM_STATS<int> over the host's gysk_query_window_hosts(-1, 0) rows (each the record gysk_encode_listener_state writes,
+ * LISTEN_SUMM_STATS::update, server/gy_msocket.h:853-864):
+ *   total_qps += tot_qps, svc_net_mb += (tot_kb_inbound + tot_kb_outbound) / 1024, divided per host in int32 before the cluster sum (:16045).
+ * nsvc_issue counts the services evaluated at the last gysk_flush with issue bit 0 set there, the HOST_STATE_NOTIFY::nlisten_issue_ the
+ * reference sums; gysk_query_cluster_state counts the host summaries' BAD / SEVERE / DOWN listeners instead. The two differ by the services
+ * that had no events in the window the last flush closed: such a service is not evaluated there, so it is no issue here, but its row
+ * keeps the state of its last evaluation, which gysk_query_cluster_state counts when that is BAD or worse.
+ * Left to the caller (HOST_STATE_NOTIFY): ntasks_issue, ntaskissue_hosts, ntasks, ncpu_issue, nmem_issue, and the hosts without listeners,
+ * which the reference's nhosts also counts (gy_gysk_shim.h: cluster_state_one). The states are those of each rank's last gysk_flush. */
+typedef struct gysk_cluster_row
+{
+	uint64_t		cluster_id;
+	int32_t			found;		/* 0: not in the map (st all zero) */
+	uint32_t		pad;
+	gysk_cluster_state	st;
+} gysk_cluster_row;			/* 48 bytes */
+/* by id, from the last finished merge. GYSK_ERR_NOTSUP without GYSK_FLAG_MERGE_CLUSTERS, GYSK_ERR_INVAL before a finished merge */
+int		gysk_query_cluster_states(gysk_engine *e, const uint64_t *cluster_ids, uint32_t n, gysk_cluster_row *out);
+/* one row per cluster of the map in ascending cluster id; GYSK_WINDOW_ACTIVE_ONLY keeps the clusters with nsvc > 0. Count and capacity as
+ * gysk_query_logical_all */
+int		gysk_query_cluster_states_all(gysk_engine *e, uint32_t flags, gysk_cluster_row *out, uint32_t cap, uint32_t *n);
 
 int		gysk_query_flows_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_est *out);
 
