@@ -192,6 +192,32 @@ struct ClusterMap
 	int32_t			*d_sel {nullptr};			// [nc] the part of d_sorted an ACTIVE_ONLY read selects
 };
 
+// GYSK_FLAG_MERGE_TOPN: the TOPN_K best services by each service metric (GYSK_TOPN_QPS .. GYSK_TOPN_ACTIVE) and processes by each task
+// metric (GYSK_TOPN_TASK_CPU .. _BLKIO_DELAY), list m = the service metric or TOPN_SVC_LISTS + the task metric. One rank's candidates
+// (appended to its t-digest slab, so the all-gather carries them) and the merge's winners have the same layout: the entries of every list
+// [TOPN_LISTS][TOPN_K], best first, then the rows of the service lists and of the task lists, each row its owner's gysk_query_svcs /
+// gysk_query_tasks row (the service rows before the host's hll_finish). Every offset is 16-byte aligned.
+constexpr uint32_t TOPN_K = 64, TOPN_SVC_LISTS = 5, TOPN_LISTS = TOPN_SVC_LISTS + 3;
+struct TopnLists
+{
+	static constexpr size_t ENT = 0, SVC_ROW = ENT + (size_t)TOPN_LISTS * TOPN_K * sizeof(gysk_topn_entry),
+		TASK_ROW = SVC_ROW + (size_t)TOPN_SVC_LISTS * TOPN_K * sizeof(gysk_svc_summary),
+		BYTES = TASK_ROW + (size_t)(TOPN_LISTS - TOPN_SVC_LISTS) * TOPN_K * sizeof(gysk_task_summary);
+	uint8_t			*base;
+
+	__host__ __device__ __forceinline__ gysk_topn_entry *ent(uint32_t m) const { return reinterpret_cast<gysk_topn_entry *>(base + ENT) + (size_t)m * TOPN_K; }
+	__host__ __device__ __forceinline__ static size_t row_bytes(uint32_t m) { return m < TOPN_SVC_LISTS ? sizeof(gysk_svc_summary) : sizeof(gysk_task_summary); }
+	// row i of list m
+	__host__ __device__ __forceinline__ uint8_t *row(uint32_t m, uint32_t i) const
+	{
+		return m < TOPN_SVC_LISTS ? base + SVC_ROW + ((size_t)m * TOPN_K + i) * sizeof(gysk_svc_summary)
+					  : base + TASK_ROW + ((size_t)(m - TOPN_SVC_LISTS) * TOPN_K + i) * sizeof(gysk_task_summary);
+	}
+};
+static_assert(TopnLists::SVC_ROW % 16 == 0 && TopnLists::TASK_ROW % 16 == 0 && sizeof(SlabEntry) % 16 == 0, "16-byte aligned rows");
+// the candidates' whole SlabEntrys after a rank's nl digests
+constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
+
 // per-logical-service state of the merge step (SURVEY.md §8e)
 struct MergeState
 {
@@ -219,6 +245,10 @@ struct MergeState
 	bool			comm_owned {false};
 	SlabEntry		*gathered {nullptr};			// [world] slabs, target of the all-gather
 	uint32_t		gathered_world {0};
+	// GYSK_FLAG_MERGE_TOPN: lg.slab holds slab_entries = nl + TOPN_SLAB_ENTRIES (nl without the flag), the candidates from lg.slab + nl
+	uint32_t		slab_entries {0};
+	unsigned long long	*topn_slots {nullptr};			// [TOPN_LISTS][TOPN_K] this rank's candidate slots (the rows' input)
+	uint8_t			*topn_final {nullptr};			// TopnLists::BYTES: the winners of the last finished merge
 };
 
 } // namespace gysk

@@ -2097,6 +2097,7 @@ __global__ void topn_score_kernel(DevState st, uint32_t nslots, int metric, int 
 			const SlotState ss = st.slot_state[slot];
 			score = ss.state > GYSK_STATE_OK && ss.state <= GYSK_STATE_DOWN ? ss.state : 0;
 		}
+		else if (metric == GYSK_TOPN_ACTIVE) score = (uint32_t)st.slot_aux[slot].act_last;	// nconns_active (is_comp_active_conn; gysk_topn_global only)
 		else score = st.conn_last[slot] >> 32;
 	}
 	if (score > 0xFFFFFFFFull) score = 0xFFFFFFFFull;
@@ -2116,40 +2117,44 @@ __global__ void topn_task_score_kernel(DevState st, uint32_t ntasks, int metric,
 	keys[slot] = (score << 32) | slot;
 }
 
-// the want best of the sorted keys, with the id and host of their slots (services' or processes'; logical services: host 0)
+// the want best of the sorted keys, with the id and host of their slots (services' or processes'; logical services: host 0); with
+// slots != nullptr also the slot (index) of each entry, 0 past the end of the keys
 __global__ void topn_pick_kernel(const unsigned long long *__restrict__ slot_id, const uint32_t *__restrict__ slot_host,
-		const unsigned long long *__restrict__ sorted, uint32_t nslots, uint32_t want, gysk_topn_entry *__restrict__ out)
+		const unsigned long long *__restrict__ sorted, uint32_t nslots, uint32_t want, gysk_topn_entry *__restrict__ out,
+		unsigned long long *__restrict__ slots)
 {
 	const uint32_t i = threadIdx.x;
 	if (i >= want) return;
 	gysk_topn_entry o; o.glob_id = 0; o.score = 0; o.host_idx = 0; o.pad = 0;
+	uint32_t slot = 0;
 	if (i < nslots) {
 		const unsigned long long k = sorted[nslots - 1 - i];		// descending
-		const uint32_t slot = (uint32_t)k;
+		slot = (uint32_t)k;
 		o.glob_id = slot_id[slot]; o.score = k >> 32; o.host_idx = slot_host ? slot_host[slot] : 0u;
 	}
 	out[i] = o;
+	if (slots) slots[i] = slot;
 }
 
 int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_t nkeys, const unsigned long long *ids, const uint32_t *hosts,
-		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s)
+		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s, unsigned long long *d_slots)
 {
 	int which = 0;
 	const int sorted = launch_radix_sort(tmp, d_n, nkeys, 32, 64, &which, s);
 	if (sorted < 0) return sorted;
-	topn_pick_kernel<<<1, 64, 0, s>>>(ids, hosts, which ? tmp.keys_b : tmp.keys_a, nkeys, want, d_out);
+	topn_pick_kernel<<<1, 64, 0, s>>>(ids, hosts, which ? tmp.keys_b : tmp.keys_a, nkeys, want, d_out, d_slots);
 	return sorted + 1;
 }
 
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
-		gysk_topn_entry *d_out, cudaStream_t s)
+		gysk_topn_entry *d_out, cudaStream_t s, unsigned long long *d_slots)
 {
 	if (!nslots) return 0;
 	unsigned long long *d_n = st.counters + CTR_NKEYS;
 	if (is_task) topn_task_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, tmp.keys_a, d_n);
 	else topn_score_kernel<<<div_up(nslots, 256), 256, 0, s>>>(st, nslots, metric, host_filter, tmp.keys_a, d_n);
 	const int picked = launch_topn_pick(tmp, d_n, nslots, is_task ? st.task_slot_id : st.slot_id, is_task ? st.task_slot_host : st.slot_host,
-			want, d_out, s);
+			want, d_out, s, d_slots);
 	return picked < 0 ? picked : 1 + picked;
 }
 

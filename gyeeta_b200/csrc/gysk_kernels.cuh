@@ -173,13 +173,15 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range, or n_max >= 2^30
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);
-// the want best services (host_filter < 0: of every host) or processes (is_task) of nslots by one metric; -1: sort failed
+// the want best services (host_filter < 0: of every host) or processes (is_task) of nslots by one metric, and with d_slots their slots;
+// -1: sort failed
 int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is_task, int metric, int host_filter, uint32_t want,
-		gysk_topn_entry *d_out, cudaStream_t s);
+		gysk_topn_entry *d_out, cudaStream_t s, unsigned long long *d_slots = nullptr);
 // the second half of a top-N: the *d_n <= nkeys {score : 32 | index : 32} keys in tmp.keys_a sorted by score (stable), then the want best
-// as entries {ids[index], score, hosts[index]} (hosts nullptr: host 0), the later index first on equal scores; -1: sort failed
+// as entries {ids[index], score, hosts[index]} (hosts nullptr: host 0), the later index first on equal scores, and with d_slots each
+// entry's index (0 past the keys); -1: sort failed
 int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_t nkeys, const unsigned long long *ids, const uint32_t *hosts,
-		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s);
+		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s, unsigned long long *d_slots = nullptr);
 int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s);
 // the window roll into ring slot st.levels.cur of each level (cleared by the host when it starts a new epoch), the listener states,
 // the idle-service eviction

@@ -11,13 +11,15 @@
 //                          and a fixed t-digest slab (not element-wise mergeable); GYSK_FLAG_MERGE_LEVELS appends the rolling
 //                          levels and aux sums to the SUM region, their maxima, the rtt and the flush tsec pair to the i64 MAX one;
 //                          GYSK_FLAG_MERGE_STATES appends the members' LISTEN_SUMM_STATS words to the SUM region,
-//                          GYSK_FLAG_MERGE_CLUSTERS the host clusters' MS_CLUSTER_STATE words after them (gysk_set_cluster_map)
+//                          GYSK_FLAG_MERGE_CLUSTERS the host clusters' MS_CLUSTER_STATE words after them (gysk_set_cluster_map);
+//                          GYSK_FLAG_MERGE_TOPN appends this rank's 64 best services / processes per metric, with their rows, to the slab
 //   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
-//   gysk_merge_finish      rank-ascending merge + compress of the gathered digests
+//   gysk_merge_finish      rank-ascending merge + compress of the gathered digests [, the global pick of the gathered top-N candidates]
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
 //   gysk_export_logical_hist / gysk_merge_flush_range   one merged histogram / the ranks' flush tsec range
 //   gysk_query_logical_states[_all]   the member listeners' state counts per logical service (GYSK_FLAG_MERGE_STATES)
 //   gysk_query_cluster_states[_all]   the service half of MS_CLUSTER_STATE per host cluster (GYSK_FLAG_MERGE_CLUSTERS)
+//   gysk_topn_global[_tasks]          the best services / processes of every rank, with their rows (GYSK_FLAG_MERGE_TOPN)
 //
 // It is the additive roll-up of MS_CLUSTER_STATE::STATE_ONE::add_stats (common/gy_comm_proto.h:3199-3214) /
 // SHCONN_HANDLER::aggregate_cluster_state (server/gy_shconnhdlr.cc:4583) and of GY_HISTOGRAM::update_from_serialized
@@ -242,17 +244,58 @@ __global__ void __launch_bounds__(MG_WARPS * 32) fold_td_kernel(DevState st, Mem
 		}, lg.slab[l], lane);
 }
 
-// one warp per logical service over the all-gathered slabs [world][nl], in rank-ascending order => deterministic result
-__global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, LogicalArrays lg, TdParams P)
+// one warp per logical service over the all-gathered slabs [world][stride] (each rank's nl digests first), in rank-ascending order =>
+// deterministic result
+__global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, uint32_t stride, LogicalArrays lg,
+		TdParams P)
 {
 	__shared__ TdScratch scratch[MG_WARPS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 
 	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS)
 		fold_digests(scratch[wid], P, 0, world, [&](uint32_t r) {
-			const SlabEntry &g = gathered[(size_t)r * lg.nl + l];
+			const SlabEntry &g = gathered[(size_t)r * stride + l];
 			return DigestRef {&g.head, g.cent};
 		}, lg.final_slab[l], lane);
+}
+
+// GYSK_FLAG_MERGE_TOPN, one CTA per list m, one thread per candidate of the gathered slabs (rank r's lists at gathered + r * stride + nl,
+// each best first). Candidates with a non-zero score are ordered by score descending, then rank ascending, then local order, so the place
+// of rank r's entry i is i plus, in every other rank's list, the entries with a greater score or an equal one on a lower rank (a binary
+// search: the lists are sorted). Every global winner is among its own rank's TOPN_K best, so places 0 .. TOPN_K - 1 are exact; they take the
+// candidate's entry and row, the places no candidate reaches stay zero.
+__global__ void __launch_bounds__(256) topn_global_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, uint32_t stride, uint32_t nl,
+		TopnLists out)
+{
+	const uint32_t m = blockIdx.x;
+	const size_t row_words = TopnLists::row_bytes(m) / 8;
+	auto cands = [&](uint32_t r) { return TopnLists {reinterpret_cast<uint8_t *>(const_cast<SlabEntry *>(gathered + (size_t)r * stride + nl))}; };
+
+	for (uint32_t i = threadIdx.x; i < TOPN_K; i += blockDim.x) out.ent(m)[i] = gysk_topn_entry {0, 0, 0, 0};
+	__syncthreads();
+	for (uint32_t c = threadIdx.x; c < world * TOPN_K; c += blockDim.x) {
+		const uint32_t r = c / TOPN_K, i = c % TOPN_K;
+		const gysk_topn_entry x = cands(r).ent(m)[i];
+		if (!x.score) continue;
+		uint32_t place = i;
+		for (uint32_t q = 0; q < world && place < TOPN_K; ++q) {
+			if (q == r) continue;
+			const gysk_topn_entry *l = cands(q).ent(m);
+			uint32_t lo = 0, hi = TOPN_K;
+			while (lo < hi) {
+				const uint32_t mid = (lo + hi) >> 1;
+				const unsigned long long s = l[mid].score;
+				if (s > x.score || (s == x.score && q < r)) lo = mid + 1;
+				else hi = mid;
+			}
+			place += lo;
+		}
+		if (place >= TOPN_K) continue;
+		out.ent(m)[place] = x;
+		const unsigned long long *src = reinterpret_cast<const unsigned long long *>(cands(r).row(m, i));
+		unsigned long long *dst = reinterpret_cast<unsigned long long *>(out.row(m, place));
+		for (size_t k = 0; k < row_words; ++k) dst[k] = src[k];
+	}
 }
 
 // read side: one warp per logical service, its merged arrays into a shared-memory SvcRaw, then the row of summarize_warp (the
@@ -520,6 +563,40 @@ int logical_all_rows(gysk_engine *e, uint32_t flags, Row *out, uint32_t cap, uin
 	return GYSK_OK;
 }
 
+// gysk_topn_global / gysk_topn_global_tasks: the first n winners of one list and their rows, the entries with a zero score left out
+SvcRows topn_finish(const gysk_engine *e, gysk_svc_summary *rows) { return SvcRows {e->cfg.hll_p, rows}; }
+CopyRows<gysk_task_summary> topn_finish(const gysk_engine *, gysk_task_summary *rows) { return CopyRows<gysk_task_summary> {rows}; }
+template <typename Row>
+int topn_global_rows(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, Row *rows, uint32_t *nout, const char *what)
+{
+	constexpr bool task = std::is_same<Row, gysk_task_summary>::value;
+	CHECK_ENGINE(e);
+	if (!out || !nout || n == 0 || n > TOPN_K || metric < 0 || (uint32_t)metric >= (task ? TOPN_LISTS - TOPN_SVC_LISTS : TOPN_SVC_LISTS))
+		return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_MERGE_TOPN)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, (std::string("gysk_") + what + ": no finished merge").c_str());
+	const uint32_t m = task ? TOPN_SVC_LISTS + (uint32_t)metric : (uint32_t)metric;
+	const TopnLists w {mg.topn_final};
+	constexpr size_t row_off = TOPN_K * sizeof(gysk_topn_entry);
+	static_assert(row_off + TOPN_K * sizeof(gysk_svc_summary) <= STAGE_BYTES, "the stage holds one list's entries and rows");
+	CU(e, cudaMemcpyAsync(e->h_wstage, w.ent(m), n * sizeof(gysk_topn_entry), cudaMemcpyDeviceToHost, e->stream));
+	if (rows) CU(e, cudaMemcpyAsync(e->h_wstage + row_off, w.row(m, 0), n * sizeof(Row), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	if (int rc = post_launch(e, what)) return rc;
+	const gysk_topn_entry *h = reinterpret_cast<const gysk_topn_entry *>(e->h_wstage);
+	const auto finish = topn_finish(e, rows);
+	uint32_t k = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		if (!h[i].glob_id || !h[i].score) continue;
+		if (rows) finish(e->h_wstage + row_off + i * sizeof(Row), k, 1);
+		out[k++] = h[i];
+	}
+	*nout = k;
+	return GYSK_OK;
+}
+
 } // namespace
 
 // ---- NCCL inside the library (SURVEY.md §8e): the whole merge step of one query window as ONE call -------------------
@@ -679,19 +756,30 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 
 	// (re)allocate the arena
 	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
-	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel);
+	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel); dfree(e, mg.topn_slots); dfree(e, mg.topn_final);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
 		ClusterMap clusters_keep(std::move(mg.clusters));
+		void *comm_keep = mg.comm;
+		const uint32_t world_keep = mg.comm_world;
+		const bool owned_keep = mg.comm_owned;
 		mg = MergeState {};
 		mg.logical_ids = std::move(ids_keep); mg.index = std::move(idx_keep); mg.clusters = std::move(clusters_keep);
+		mg.comm = comm_keep; mg.comm_world = world_keep; mg.comm_owned = owned_keep;		// gysk_nccl_comm_init's communicator stays
 	}
 	LogicalArrays &lg = mg.lg;
 	lg.nl = nl;
 	int rc = lay_out_arena(e);
 	if (rc) return rc;
-	if ((rc = dalloc(e, &lg.slab, nl ? nl : 1))) return rc;
+	// GYSK_FLAG_MERGE_TOPN: the candidates after the digests, in whole SlabEntrys, so the slab stays one all-gather
+	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN;
+	mg.slab_entries = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
+	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
+	if (topn) {
+		if ((rc = dalloc(e, &mg.topn_slots, (size_t)TOPN_LISTS * TOPN_K))) return rc;
+		if ((rc = dalloc(e, &mg.topn_final, TopnLists::BYTES))) return rc;
+	}
 	if ((rc = dalloc(e, &lg.final_slab, nl ? nl : 1))) return rc;
 	if ((rc = dalloc(e, &mg.members.offs, (size_t)nl + 1))) return rc;
 	if ((rc = dalloc(e, &mg.members.slots, (size_t)n + 1))) return rc;
@@ -777,6 +865,10 @@ int gysk_merge_prepare(gysk_engine *e)
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Submit);
 	MergeState &mg = e->mg;
+	// GYSK_FLAG_MERGE_TOPN needs no map: without one, an empty logical map (as gysk_set_cluster_map sets up)
+	if (!mg.arena && (e->cfg.flags & GYSK_FLAG_MERGE_TOPN)) {
+		if (int rc = set_logical_map(e, nullptr, nullptr, 0)) return rc;
+	}
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_prepare: call gysk_set_logical_map first");
 
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8;
@@ -808,6 +900,24 @@ int gysk_merge_prepare(gysk_engine *e)
 		fold_clusters_kernel<<<div_up(nc, 256), 256, 0, e->stream>>>(mg.clusters.cl);
 		e->kernel_launches += 2;
 	}
+	if (mg.topn_final) {		// GYSK_FLAG_MERGE_TOPN
+		// each list: the score kernel, radix sort and pick of gysk_topn_svcs / gysk_topn_tasks over every slot (max_svcs / max_tasks: the
+		// slots past the table's count score 0, and the count stays on the device), its entries into the slab, its slots beside them; then
+		// the rows of all the slots through the summary path of gysk_query_svcs / gysk_query_tasks. max_svcs, max_tasks >= 1: every pick
+		// writes all TOPN_K entries and slots
+		const TopnLists cand {reinterpret_cast<uint8_t *>(mg.lg.slab + nl)};
+		for (uint32_t m = 0; m < TOPN_LISTS; ++m) {
+			const bool task = m >= TOPN_SVC_LISTS;
+			const int k = launch_topn(e->st, e->tmp, task ? e->cfg.max_tasks : e->cfg.max_svcs, task, task ? (int)(m - TOPN_SVC_LISTS) : (int)m, -1,
+					TOPN_K, cand.ent(m), e->stream, mg.topn_slots + (size_t)m * TOPN_K);
+			if (k < 0) return fail(e, GYSK_ERR_INVAL, "gysk_merge_prepare: top-N sort failed");
+			e->kernel_launches += k;
+		}
+		e->kernel_launches += launch_svc_summaries(e->st, nullptr, mg.topn_slots, TOPN_SVC_LISTS * TOPN_K,
+				reinterpret_cast<gysk_svc_summary *>(cand.row(0, 0)), e->stream);
+		e->kernel_launches += launch_task_summaries(e->st, nullptr, mg.topn_slots + (size_t)TOPN_SVC_LISTS * TOPN_K, (TOPN_LISTS - TOPN_SVC_LISTS) * TOPN_K,
+				reinterpret_cast<gysk_task_summary *>(cand.row(TOPN_SVC_LISTS, 0)), e->stream);
+	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
 	return post_launch(e, "merge_prepare");
@@ -834,7 +944,7 @@ int gysk_merge_tdigest_slab(gysk_engine *e, void **dptr, uint64_t *nbytes)
 	if (!dptr || !nbytes) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Drain);
 	if (!e->mg.lg.slab) return fail(e, GYSK_ERR_INVAL, "gysk_merge_tdigest_slab: call gysk_set_logical_map first");
-	*dptr = e->mg.lg.slab; *nbytes = (uint64_t)e->mg.lg.nl * sizeof(SlabEntry);
+	*dptr = e->mg.lg.slab; *nbytes = (uint64_t)e->mg.slab_entries * sizeof(SlabEntry);
 	return GYSK_OK;
 }
 
@@ -848,7 +958,12 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 	const SlabEntry *src = d_gathered ? static_cast<const SlabEntry *>(d_gathered) : mg.lg.slab;
 	if (!d_gathered) world = 1;
 	if (mg.lg.nl) {
-		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.lg.nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.lg, e->st.td);
+		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.lg.nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.slab_entries, mg.lg,
+				e->st.td);
+		e->kernel_launches++;
+	}
+	if (mg.topn_final) {		// GYSK_FLAG_MERGE_TOPN
+		topn_global_kernel<<<TOPN_LISTS, 256, 0, e->stream>>>(src, world, mg.slab_entries, mg.lg.nl, TopnLists {mg.topn_final});
 		e->kernel_launches++;
 	}
 	mg.finished = true;			// stream-ordered; the query calls synchronise
@@ -1067,10 +1182,10 @@ int gysk_merge_global(gysk_engine *e, void *comm)
 		if (world < 1) return fail(e, GYSK_ERR_INVAL, "gysk_merge_global: empty communicator");
 		if (mg.gathered_world != (uint32_t)world) {
 			dfree(e, mg.gathered);
-			if ((rc = dalloc(e, &mg.gathered, (size_t)(mg.lg.nl ? mg.lg.nl : 1) * world, false))) return rc;
+			if ((rc = dalloc(e, &mg.gathered, (size_t)(mg.slab_entries ? mg.slab_entries : 1) * world, false))) return rc;
 			mg.gathered_world = (uint32_t)world;
 		}
-		const size_t slab = (size_t)mg.lg.nl * sizeof(SlabEntry);
+		const size_t slab = (size_t)mg.slab_entries * sizeof(SlabEntry);
 		NC(e, a->GroupStart());
 		NC(e, a->AllReduce(mg.arena + mg.off_sum, mg.arena + mg.off_sum, mg.bytes_sum / 8, ncclUint64, ncclSum, c, e->stream));
 		NC(e, a->AllReduce(mg.arena + mg.off_maxi64, mg.arena + mg.off_maxi64, mg.bytes_maxi64 / 8, ncclInt64, ncclMax, c, e->stream));
@@ -1079,7 +1194,18 @@ int gysk_merge_global(gysk_engine *e, void *comm)
 		NC(e, a->GroupEnd());
 		e->merges++;
 	}
-	return gysk_merge_finish(e, e->mg.lg.nl ? e->mg.gathered : nullptr, (uint32_t)world);
+	return gysk_merge_finish(e, e->mg.slab_entries ? e->mg.gathered : nullptr, (uint32_t)world);
+}
+
+// GYSK_FLAG_MERGE_TOPN: the winners of the last finished merge (topn_global_kernel)
+int gysk_topn_global(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, gysk_svc_summary *rows, uint32_t *nout)
+{
+	return topn_global_rows(e, metric, n, out, rows, nout, "topn_global");
+}
+
+int gysk_topn_global_tasks(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, gysk_task_summary *rows, uint32_t *nout)
+{
+	return topn_global_rows(e, metric, n, out, rows, nout, "topn_global_tasks");
 }
 
 } // extern "C"

@@ -32,7 +32,8 @@ assert RESP16_DTYPE.itemsize == 16 and TCP24_DTYPE.itemsize == 24 and TASK24_DTY
 NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CONN_STATS = 0x309, 0x30C, 0x310, 0x312
 (HOSTTOP_SVC_ISSUE, HOSTTOP_SVC_QPS, HOSTTOP_SVC_CONNS, HOSTTOP_SVC_NET, HOSTTOP_TASK_ISSUE, HOSTTOP_TASK_NET, HOSTTOP_TASK_CPU, HOSTTOP_TASK_RSS,
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
-FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS = 1, 2, 4, 8
+FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, FLAG_MERGE_TOPN = 1, 2, 4, 8, 16
+TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
 
@@ -255,6 +256,8 @@ def load_library(path=None):
         "gysk_set_cluster_map": (i32, [vp, vp, vp, u32]),
         "gysk_query_cluster_states": (i32, [vp, vp, u32, vp]),
         "gysk_query_cluster_states_all": (i32, [vp, u32, vp, u32, vp]),
+        "gysk_topn_global": (i32, [vp, i32, u32, vp, vp, vp]),
+        "gysk_topn_global_tasks": (i32, [vp, i32, u32, vp, vp, vp]),
         "gysk_query_flows_global": (i32, [vp, vp, u32, i32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
@@ -281,7 +284,7 @@ class Engine:
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
-                 merge_levels=False, merge_states=False, merge_clusters=False):
+                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -291,7 +294,8 @@ class Engine:
         cfg.stage_batch = stage_batch
         cfg.idle_evict_secs = idle_evict_secs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
-                    (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0)
+                    (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
+                    (FLAG_MERGE_TOPN if merge_topn else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -694,6 +698,22 @@ class Engine:
     def query_cluster_states_all(self, active_only=False, cap=None):
         """gysk_query_cluster_states_all: (ClusterRow rows in ascending cluster id, number of matching rows); cap as query_logical_all"""
         return self._window(self.L.gysk_query_cluster_states_all, ClusterRow, (), active_only, cap)
+
+    def _topn_global(self, fn, row_type, metric, n, rows):
+        out = (TopnEntry * max(n, 1))()
+        rws = (row_type * max(n, 1))() if rows else None
+        k = C.c_uint32()
+        self._chk(fn(self.h, metric, n, out, rws, C.byref(k)))
+        return out[: k.value], (rws[: k.value] if rows else None)
+
+    def topn_global(self, metric, n=10, rows=True):
+        """gysk_topn_global: (TopnEntry list, SvcSummary rows or None) of the n best services over every rank, best first, from the last
+        merge (merge_topn=True)"""
+        return self._topn_global(self.L.gysk_topn_global, SvcSummary, metric, n, rows)
+
+    def topn_global_tasks(self, metric, n=10, rows=True):
+        """gysk_topn_global_tasks: (TopnEntry list, TaskSummary rows or None) of the n best processes over every rank (merge_topn=True)"""
+        return self._topn_global(self.L.gysk_topn_global_tasks, TaskSummary, metric, n, rows)
 
     def merge_flush_range(self):
         """gysk_merge_flush_range: (earliest, latest) tsec of the ranks' last flush, as the last merge all-reduced them"""
