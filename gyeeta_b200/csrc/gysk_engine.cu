@@ -355,6 +355,55 @@ int roll_levels(gysk_engine *e, uint32_t tsec)
 	return 0;
 }
 
+// ---- capacity: the per-slot arrays --------------------------------------------------------------------------------
+//
+// Every device array indexed by service or process slot, with its elements per slot: f(pointer, elements per slot, kind). Svc arrays
+// hold max_svcs + 1 slots (slot max_svcs is the null slot), the level ring max_svcs rows in each of its NLEVELS x NSLOTS planes
+// (LevelRing::stride), Task arrays max_tasks slots. gysk_create allocates exactly these, gysk_grow moves them, slot_bytes sums them.
+enum class SlotKind { Svc, Ring, Task };
+
+template <typename F>
+void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, F f)
+{
+	f(st.slot_id, 1, SlotKind::Svc); f(st.slot_host, 1, SlotKind::Svc);
+	f(st.slot_first_seen, 1, SlotKind::Svc); f(st.slot_last_active, 1, SlotKind::Svc);
+	f(st.evict_list, 1, SlotKind::Svc); f(st.evict_ids, 1, SlotKind::Svc); f(st.svc_tbl.free_slots, 1, SlotKind::Svc);
+	f(st.hist_cur, HIST_CELLS, SlotKind::Svc); f(st.hist_last, HIST_CELLS, SlotKind::Svc); f(st.hist_all, HIST_CELLS, SlotKind::Svc);
+	f(st.levels.ring, (size_t)NLEVELS * NSLOTS * HIST_CELLS, SlotKind::Ring);
+	f(st.conn_cur, 1, SlotKind::Svc); f(st.conn_last, 1, SlotKind::Svc); f(st.conn_all_cnt, 1, SlotKind::Svc); f(st.conn_all_kb, 1, SlotKind::Svc);
+	f(st.bm_cur, HIST_CELLS, SlotKind::Svc); f(st.bm_last, HIST_CELLS, SlotKind::Svc);
+	f(st.hll, (size_t)1 << hll_p, SlotKind::Svc);
+	f(st.td_cent, TD_CAP, SlotKind::Svc); f(st.td_head, 1, SlotKind::Svc);
+	f(st.slot_batch, 1, SlotKind::Svc); f(st.slot_aux, 1, SlotKind::Svc);
+	f(st.qps_hist, HIST_CELLS, SlotKind::Svc); f(st.act_hist, HIST_CELLS, SlotKind::Svc); f(st.slot_state, 1, SlotKind::Svc);
+	f(tmp.touched, 1, SlotKind::Svc); f(tmp.segs, 1, SlotKind::Svc);
+	f(st.task_hist, 3 * HIST_CELLS, SlotKind::Task); f(st.task_prev, 3, SlotKind::Task); f(st.task_last, 3, SlotKind::Task);
+	f(st.task_slot_id, 1, SlotKind::Task); f(st.task_slot_host, 1, SlotKind::Task);
+}
+
+// device bytes of one service slot (its ring rows included) and of one process slot: the sums of each_slot_array
+void slot_bytes(uint32_t hll_p, uint64_t *svc, uint64_t *task)
+{
+	DevState st {};
+	SortTemp tmp {};
+	uint64_t b[3] = {0, 0, 0};
+	each_slot_array(st, tmp, hll_p, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
+	*svc = b[(int)SlotKind::Svc] + b[(int)SlotKind::Ring];
+	*task = b[(int)SlotKind::Task];
+}
+
+size_t slots_of(SlotKind kind, uint32_t max_svcs, uint32_t max_tasks)
+{
+	return kind == SlotKind::Svc ? (size_t)max_svcs + 1 : kind == SlotKind::Ring ? (size_t)max_svcs : (size_t)max_tasks;
+}
+
+// the arrays sized by capacity beside the per-slot ones: an id table's entries, the sort buffers' keys and look-back tiles, the batch
+// rows of the long key segments
+uint32_t table_cap(uint32_t slots) { return pow2_at_least((uint64_t)slots * 2); }
+size_t sort_keys(const gysk_config &cfg) { return std::max<size_t>(std::max<size_t>((size_t)cfg.max_svcs + 1, cfg.max_tasks) + 1, cfg.max_batch); }
+uint32_t sort_tiles(size_t nkeys) { return (uint32_t)((nkeys + SORT_TILE - 1) / SORT_TILE); }
+size_t batch_rows(const gysk_config &cfg) { return std::min<size_t>((size_t)cfg.max_svcs + 1, ((size_t)cfg.max_batch + LONG_SEG - 1) / LONG_SEG); }
+
 SvcRows finish_rows(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
 CopyRows<gysk_task_summary> finish_rows(const gysk_engine *, gysk_task_summary *out) { return CopyRows<gysk_task_summary> {out}; }
 CopyRows<gysk_listener_day_stats> finish_rows(const gysk_engine *, gysk_listener_day_stats *out) { return CopyRows<gysk_listener_day_stats> {out}; }
@@ -419,7 +468,8 @@ void gysk_destroy(gysk_engine *e)
 	}
 	for (cudaEvent_t ev : e->prof_events) cudaEventDestroy(ev);
 	if (e->ev_evict) cudaEventDestroy(e->ev_evict);
-	for (void *p : e->dallocs) cudaFree(p);
+	if (e->ev_used) cudaEventDestroy(e->ev_used);
+	for (auto &a : e->dallocs) cudaFree(a.first);
 	for (void *p : e->hallocs) cudaFreeHost(p);
 	if (e->stream) cudaStreamDestroy(e->stream);
 	if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
@@ -470,33 +520,27 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	}
 
 	DevState &st = e->st;
-	const size_t ns = (size_t)cfg.max_svcs + 1, nt = cfg.max_tasks;		// slot max_svcs = the null slot: never handed out, always pristine
-	const uint32_t scap = pow2_at_least((uint64_t)ns * 2), tcap = pow2_at_least((uint64_t)nt * 2);
+	const size_t ns = (size_t)cfg.max_svcs + 1;		// slot max_svcs = the null slot: never handed out, always pristine
+	const uint32_t scap = table_cap(cfg.max_svcs + 1), tcap = table_cap(cfg.max_tasks);
 
 #define A(call) do { if ((rc = (call)) != 0) return bail(rc); } while (0)
 	A(dalloc(e, &st.counters, (size_t)CTR_MAX));
 	A(dalloc(e, &st.svc_tbl.ent, scap)); st.svc_tbl.mask = scap - 1; st.svc_tbl.max_slots = cfg.max_svcs;
 	A(dalloc(e, &st.svc_tbl.count, 1));
-	A(dalloc(e, &st.slot_id, ns)); A(dalloc(e, &st.slot_host, ns));
+	A(dalloc(e, &st.svc_tbl.free_n, 1));
+	A(dalloc(e, &st.task_tbl.ent, tcap)); st.task_tbl.mask = tcap - 1; st.task_tbl.max_slots = cfg.max_tasks;
+	A(dalloc(e, &st.task_tbl.count, 1));
+	SortTemp &tmp = e->tmp;
+	each_slot_array(st, tmp, cfg.hll_p, [&](auto *&p, size_t k, SlotKind kind) { if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks) * k); });
+	if (rc) return bail(rc);
+	st.levels.stride = cfg.max_svcs;
 	st.svc_tbl.slot_id = st.slot_id; st.svc_tbl.slot_host = st.slot_host;
-	A(dalloc(e, &st.slot_first_seen, ns)); A(dalloc(e, &st.slot_last_active, ns));
-	A(dalloc(e, &st.evict_list, ns)); A(dalloc(e, &st.evict_ids, ns));
-	A(dalloc(e, &st.svc_tbl.free_n, 1)); A(dalloc(e, &st.svc_tbl.free_slots, ns));
+	st.task_tbl.slot_id = st.task_slot_id; st.task_tbl.slot_host = st.task_slot_host;
 	A(halloc(e, &e->h_evict, ns + 2));
 	e->h_evict[0] = 0; e->h_evict[cfg.max_svcs + 1] = 0;
 	if ((ce = cudaEventCreateWithFlags(&e->ev_evict, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
-	A(dalloc(e, &st.task_tbl.ent, tcap)); st.task_tbl.mask = tcap - 1; st.task_tbl.max_slots = cfg.max_tasks;
-	A(dalloc(e, &st.task_tbl.count, 1));
-	A(dalloc(e, &st.hist_cur, ns * HIST_CELLS)); A(dalloc(e, &st.hist_last, ns * HIST_CELLS)); A(dalloc(e, &st.hist_all, ns * HIST_CELLS));
-	A(dalloc(e, &st.levels.ring, (size_t)NLEVELS * NSLOTS * cfg.max_svcs * HIST_CELLS)); st.levels.stride = cfg.max_svcs;
-	A(dalloc(e, &st.conn_cur, ns)); A(dalloc(e, &st.conn_last, ns)); A(dalloc(e, &st.conn_all_cnt, ns)); A(dalloc(e, &st.conn_all_kb, ns));
-	A(dalloc(e, &st.bm_cur, ns * HIST_CELLS)); A(dalloc(e, &st.bm_last, ns * HIST_CELLS));
-	A(dalloc(e, &st.hll, ns << cfg.hll_p));
-	A(dalloc(e, &st.td_cent, ns * TD_CAP)); A(dalloc(e, &st.td_head, ns));
-	A(dalloc(e, &st.task_hist, nt * 3 * HIST_CELLS));
-	A(dalloc(e, &st.task_prev, nt * 3)); A(dalloc(e, &st.task_last, nt * 3));
-	A(dalloc(e, &st.task_slot_id, nt)); A(dalloc(e, &st.task_slot_host, nt));
-	st.task_tbl.slot_id = st.task_slot_id; st.task_tbl.slot_host = st.task_slot_host;
+	A(halloc(e, &e->h_used, 4));
+	if ((ce = cudaEventCreateWithFlags(&e->ev_used, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
 	A(dalloc(e, &st.cms_cur, (size_t)cfg.cms_depth << cfg.cms_log2_width)); A(dalloc(e, &st.cms_last, (size_t)cfg.cms_depth << cfg.cms_log2_width));
 	st.cms_depth = cfg.cms_depth; st.cms_log2w = cfg.cms_log2_width; st.cms_wmask = (1u << cfg.cms_log2_width) - 1; st.hll_p = cfg.hll_p;
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
@@ -508,7 +552,6 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		if ((ce = cudaMemcpy(d_q, qtab.data(), qtab.size() * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "qtab", ce); return bail(GYSK_ERR_CUDA); }
 		st.td.qtab = d_q; st.td.delta = cfg.td_compression; st.td.pad = 0;
 	}
-	A(dalloc(e, &st.slot_batch, ns)); A(dalloc(e, &st.slot_aux, ns));
 	{
 		// dense value bins of the hot services (DESIGN.md §4): GYSK_HOT_ROWS rows of 16 KB (default 2048, 0 switches the path off); a
 		// service turns hot with GYSK_HOT_MIN (default 4096) .. GYSK_HOT_MAX samples in one batch unless its fullest bin holds more
@@ -525,22 +568,19 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		st.hot_rows = nullptr; st.hot_slot = nullptr;
 		if (rows) { A(dalloc(e, &st.hot_rows, (size_t)rows * HOT_ROW_WORDS)); A(dalloc(e, &st.hot_slot, (size_t)rows)); }
 	}
-	A(dalloc(e, &st.qps_hist, ns * HIST_CELLS)); A(dalloc(e, &st.act_hist, ns * HIST_CELLS)); A(dalloc(e, &st.slot_state, ns));
-	SortTemp &tmp = e->tmp;
-	const size_t nsort = std::max<size_t>(std::max<size_t>(ns, nt) + 1, cfg.max_batch);	// RESP keys of a batch; the top-N sorts rank services / tasks
+	const size_t nsort = sort_keys(cfg);		// RESP keys of a batch; the top-N sorts rank services / tasks
 	tmp.nkeys = nsort;
-	tmp.max_tiles = (uint32_t)((nsort + SORT_TILE - 1) / SORT_TILE);
+	tmp.max_tiles = sort_tiles(nsort);
 	A(dalloc(e, &tmp.keys_a, nsort, false)); A(dalloc(e, &tmp.keys_b, nsort, false));
 	A(dalloc(e, &tmp.tile_status, (size_t)RADIX_MAX * tmp.max_tiles));
 	tmp.epoch = &e->sort_epoch;
 	A(dalloc(e, &tmp.os_ghist, (size_t)OS_GHIST_WORDS));
-	A(dalloc(e, &tmp.touched, ns));
 	{
 		const size_t nmw = (size_t)TD_MERGE_MAX_SMS * TD_MERGE_CTAS_PER_SM * 4;		// warps of bins_merge_kernel
 		// a batch has fewer than max_batch / LONG_SEG segments of more than LONG_SEG keys, and no more than one per service. The
 		// rows start at zero and bins_merge_kernel leaves them so.
-		const size_t nbrows = std::min<size_t>(ns, ((size_t)cfg.max_batch + LONG_SEG - 1) / LONG_SEG);
-		A(dalloc(e, &tmp.segs, ns)); A(dalloc(e, &tmp.long_slot, nbrows, false)); A(dalloc(e, &tmp.batch_rows, nbrows * HOT_ROW_WORDS));
+		const size_t nbrows = batch_rows(cfg);
+		A(dalloc(e, &tmp.long_slot, nbrows, false)); A(dalloc(e, &tmp.batch_rows, nbrows * HOT_ROW_WORDS));
 		A(dalloc(e, &tmp.items_scratch, nmw * NBINS, false)); A(dalloc(e, &tmp.big_scratch, nmw, false));
 		// the batch's connection / process record queue: one region per ingest warp (SortTemp::recq)
 		const uint32_t nsm = (uint32_t)prop.multiProcessorCount;
@@ -565,7 +605,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &e->d_wstage, STAGE_BYTES, false)); A(halloc(e, &e->h_wstage, STAGE_BYTES));
 #undef A
 
-	e->kernel_launches += launch_init_state(st, cfg.max_svcs + 1, cfg.max_tasks, e->stream);
+	e->kernel_launches += launch_init_slots(st, 0, cfg.max_svcs + 1, 0, cfg.max_tasks, e->stream);
 	if ((ce = cudaStreamSynchronize(e->stream)) != cudaSuccess || (ce = cudaGetLastError()) != cudaSuccess) {
 		fail(e, GYSK_ERR_CUDA, "engine init", ce); return bail(GYSK_ERR_CUDA);
 	}
@@ -1091,11 +1131,244 @@ int gysk_sync(gysk_engine *e)
 	return GYSK_OK;
 }
 
+} // extern "C"
+
+// ---- capacity growth ------------------------------------------------------------------------------------------------
+namespace {
+
+// bytes of device buffer p (0: none)
+size_t dsize(const gysk_engine *e, const void *p)
+{
+	for (const auto &a : e->dallocs) if (a.first == p) return a.second;
+	return 0;
+}
+
+// the copies of the slot -> id / host arrays an IdTable carries
+void link_tables(DevState &st)
+{
+	st.svc_tbl.slot_id = st.slot_id; st.svc_tbl.slot_host = st.slot_host;
+	st.task_tbl.slot_id = st.task_slot_id; st.task_tbl.slot_host = st.task_slot_host;
+}
+
+// Moves one device array whose first old_n elements are valid into a new one of new_n: the prefix copied, the tail zeroed, the old
+// array freed before the caller moves on to the next one (the peak is the new footprint plus the largest old array). An array that
+// already holds new_n elements (moved by an earlier growth that stopped half way; its tail is still zero: nothing at the old capacity
+// writes there) stays. A failed allocation leaves p as it was. Stream synchronised on return.
+template <typename T>
+int regrow(gysk_engine *e, T *&p, size_t old_n, size_t new_n)
+{
+	if (dsize(e, p) >= new_n * sizeof(T)) return 0;
+	T *q = nullptr;
+	if (int rc = dalloc(e, &q, new_n, false)) return rc;
+	if (old_n) CU(e, cudaMemcpyAsync(q, p, old_n * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
+	CU(e, cudaMemsetAsync(q + old_n, 0, (new_n - old_n) * sizeof(T), e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	dfree(e, p);
+	p = q;
+	return 0;
+}
+
+// The level ring [NLEVELS][NSLOTS][stride][16] at the stride new_ms: each of its NLEVELS x NSLOTS planes (stride rows, contiguous)
+// moves with one copy to the head of its new plane, the rows behind it zeroed. The source pitch is the ring's own stride, which an
+// earlier growth that stopped half way may already have raised.
+int regrow_ring(gysk_engine *e, uint32_t new_ms)
+{
+	LevelRing &lv = e->st.levels;
+	if (lv.stride >= new_ms) return 0;
+	const size_t row = (size_t)HIST_CELLS * sizeof(HistCell), planes = (size_t)NLEVELS * NSLOTS;
+	HistCell *q = nullptr;
+	if (int rc = dalloc(e, &q, planes * new_ms * HIST_CELLS)) return rc;
+	for (size_t k = 0; k < planes; ++k)
+		CU(e, cudaMemcpyAsync(q + k * new_ms * HIST_CELLS, lv.ring + k * lv.stride * HIST_CELLS, lv.stride * row, cudaMemcpyDeviceToDevice, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	dfree(e, lv.ring);
+	lv.ring = q;
+	lv.stride = new_ms;
+	return 0;
+}
+
+// The device bytes gysk_grow adds to the engine going from cfg to (ms, mt), the largest array it frees on the way (held beside the
+// new one while it is copied), and the allocations it makes (each may be rounded up to the allocator's 2 MiB granularity)
+void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, size_t *largest_old, size_t *nalloc)
+{
+	const gysk_config &cfg = e->cfg;
+	gysk_config to = cfg;
+	to.max_svcs = ms; to.max_tasks = mt;
+	DevState st {};
+	SortTemp tmp {};
+	size_t a = 0, big = 0, n = 0;
+	auto move = [&](size_t elem, size_t old_n, size_t new_n) {
+		if (new_n <= old_n) return;
+		a += (new_n - old_n) * elem;
+		big = std::max(big, old_n * elem);
+		n++;
+	};
+	each_slot_array(st, tmp, cfg.hll_p, [&](auto *&p, size_t k, SlotKind kind) {
+		move(k * sizeof(*p), slots_of(kind, cfg.max_svcs, cfg.max_tasks), slots_of(kind, ms, mt));
+	});
+	if (ms != cfg.max_svcs) move(sizeof(TblEntry), table_cap(cfg.max_svcs + 1), table_cap(ms + 1));
+	if (mt != cfg.max_tasks) move(sizeof(TblEntry), table_cap(cfg.max_tasks), table_cap(mt));
+	const size_t k0 = sort_keys(cfg), k1 = sort_keys(to);
+	move(sizeof(unsigned long long), k0, k1); move(sizeof(unsigned long long), k0, k1);
+	move((size_t)RADIX_MAX * sizeof(unsigned long long), sort_tiles(k0), sort_tiles(k1));
+	move(sizeof(uint32_t), batch_rows(cfg), batch_rows(to)); move((size_t)HOT_ROW_WORDS * sizeof(unsigned long long), batch_rows(cfg), batch_rows(to));
+	*add = a; *largest_old = big; *nalloc = n;
+}
+
+// gysk_grow, engine held and both streams idle.
+// Phase 1 moves the per-slot arrays, the sort buffers and the batch rows one by one. The engine stays at its old capacity throughout:
+// a moved array is only longer, its valid prefix unchanged and its tail zero, and the IdTable copies of the slot arrays follow each
+// move. A cudaMalloc that fails there (the pre-check passed, but another tenant of the device took the memory since) ends the growth
+// with GYSK_ERR_NOMEM and an engine that answers as before at its old capacity; a later gysk_grow finds the arrays already moved.
+// Phase 2 allocates the new id tables and the eviction buffer while the old ones still serve (a failure: the same). Phase 3 commits
+// the new capacity and allocates nothing.
+int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
+{
+	gysk_config &cfg = e->cfg;
+	if (ms < cfg.max_svcs || mt < cfg.max_tasks || ms > (1u << 24) || mt > (1u << 24)) return fail(e, GYSK_ERR_INVAL, "gysk_grow: shrink or beyond 1 << 24");
+	if (ms == cfg.max_svcs && mt == cfg.max_tasks) return GYSK_OK;
+	size_t add = 0, big = 0, nalloc = 0, nfree = 0, ntotal = 0;
+	grow_bytes(e, ms, mt, &add, &big, &nalloc);
+	CU(e, cudaMemGetInfo(&nfree, &ntotal));
+	if (add + big + nalloc * (2u << 20) > nfree) return fail(e, GYSK_ERR_NOMEM, "gysk_grow: the new arrays do not fit the device's free memory");
+
+	if (int rc = collect_evicted(e)) return rc;		// h_evict moves: nothing may still be on its way into it
+	const uint32_t os = cfg.max_svcs, ot = cfg.max_tasks;
+	DevState &st = e->st;
+	SortTemp &tmp = e->tmp;
+	gysk_config to = cfg;
+	to.max_svcs = ms; to.max_tasks = mt;
+	int rc = 0;
+	// phase 1
+	each_slot_array(st, tmp, cfg.hll_p, [&](auto *&p, size_t k, SlotKind kind) {
+		if (rc) return;
+		if (kind == SlotKind::Ring) rc = regrow_ring(e, ms);
+		else rc = regrow(e, p, slots_of(kind, os, ot) * k, slots_of(kind, ms, mt) * k);
+		link_tables(st);
+	});
+	const size_t k0 = sort_keys(cfg), k1 = sort_keys(to), b0 = batch_rows(cfg), b1 = batch_rows(to);
+	if (!rc && !(rc = regrow(e, tmp.keys_a, k0, k1)) && !(rc = regrow(e, tmp.keys_b, k0, k1)) &&
+			!(rc = regrow(e, tmp.tile_status, (size_t)RADIX_MAX * sort_tiles(k0), (size_t)RADIX_MAX * sort_tiles(k1)))) {
+		tmp.nkeys = std::max(tmp.nkeys, k1); tmp.max_tiles = std::max(tmp.max_tiles, sort_tiles(k1));
+	}
+	if (!rc && !(rc = regrow(e, tmp.long_slot, b0, b1))) rc = regrow(e, tmp.batch_rows, b0 * HOT_ROW_WORDS, b1 * HOT_ROW_WORDS);
+	if (rc) return rc;
+	// phase 2
+	TblEntry *sent = nullptr, *tent = nullptr;
+	unsigned long long *hev = nullptr;
+	if ((ms != os && (rc = dalloc(e, &sent, table_cap(ms + 1), false))) || (mt != ot && (rc = dalloc(e, &tent, table_cap(mt), false))) ||
+			(ms != os && (rc = halloc(e, &hev, (size_t)ms + 3)))) {
+		dfree(e, sent); dfree(e, tent);
+		return rc;
+	}
+	// phase 3: the old null slot and every new slot in their just-created state (the new null slot is the last one), then both id
+	// tables rebuilt at their new capacity: slot numbers, hot rows (SlotBatch::hot of the slot) and the free stack stay. A rebuild
+	// also drops tombstones and the dead entries of lost insert races, as gysk_flush's does.
+	cfg = to;
+	e->kernel_launches += launch_init_slots(st, os, ms + 1, ot, mt, e->stream);
+	auto swap_table = [&](IdTable &t, TblEntry *ent, uint32_t slots, uint32_t max_slots) {
+		TblEntry *old = t.ent;
+		t.ent = ent; t.mask = table_cap(slots) - 1; t.max_slots = max_slots;
+		e->kernel_launches += launch_rebuild_table(t, max_slots, e->stream);
+		dfree(e, old);
+	};
+	if (ms != os) {
+		hev[0] = 0; hev[ms + 1] = e->h_evict[os + 1];		// the insert-fail word of h_evict sits at [max_svcs + 1]
+		hfree(e, e->h_evict);
+		e->h_evict = hev;
+		swap_table(st.svc_tbl, sent, ms + 1, ms);
+		unsigned long long fails = 0;
+		CU(e, cudaMemcpyAsync(&fails, st.counters + CTR_INSERT_FAIL, sizeof(fails), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaStreamSynchronize(e->stream));
+		e->tombstones = 0; e->insert_fail_seen = fails;
+	}
+	if (mt != ot) swap_table(st.task_tbl, tent, mt, mt);
+	e->mg.members.null_slot = ms;			// the member slots are resolved again at every gysk_merge_prepare
+	e->ngrows++;
+	CU(e, cudaStreamSynchronize(e->stream));
+	return post_launch(e, "grow");
+}
+
+// Auto-grow at gysk_flush: each table whose slots in use as of the previous flush reached half its capacity doubles, up to its
+// limit. The counts were copied behind that flush's kernels, a window ago: the event wait finds them long landed.
+int auto_grow(gysk_engine *e)
+{
+	if (!e->used_pending) return 0;
+	CU(e, cudaEventSynchronize(e->ev_used));
+	e->used_pending = false;
+	const uint32_t ms = e->cfg.max_svcs, mt = e->cfg.max_tasks;
+	const uint64_t svcs = (uint64_t)std::min(e->h_used[0], ms) - (uint64_t)std::max((int32_t)e->h_used[1], 0);
+	const uint64_t tasks = std::min(e->h_used[2], mt);
+	auto next = [](uint32_t cap, uint64_t used, uint32_t limit) {
+		return limit > cap && 2 * used >= cap ? (uint32_t)std::min<uint64_t>(2ull * cap, limit) : cap;
+	};
+	const uint32_t ns = next(ms, svcs, e->grow_limit_svcs), nt = next(mt, tasks, e->grow_limit_tasks);
+	if (ns == ms && nt == mt) return 0;
+	if (int rc = sync_locked(e)) return rc;
+	// GYSK_ERR_NOMEM leaves the engine as it was at its capacity (grow_locked): the flush goes on there, and the next one tries again
+	const int rc = grow_locked(e, ns, nt);
+	return rc == GYSK_ERR_NOMEM ? 0 : rc;
+}
+
+} // namespace
+
+extern "C" {
+
+int gysk_grow(gysk_engine *e, uint32_t max_svcs, uint32_t max_tasks)
+{
+	CHECK_ENGINE(e);
+	GYSK_ENTER(e, Sync);
+	return grow_locked(e, max_svcs, max_tasks);
+}
+
+int gysk_set_auto_grow(gysk_engine *e, uint32_t max_svcs_limit, uint32_t max_tasks_limit)
+{
+	CHECK_ENGINE(e);
+	if (max_svcs_limit > (1u << 24) || max_tasks_limit > (1u << 24)) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Drain);
+	e->grow_limit_svcs = max_svcs_limit; e->grow_limit_tasks = max_tasks_limit;
+	return GYSK_OK;
+}
+
+int gysk_capacity_info(gysk_engine *e, gysk_capacity *out)
+{
+	CHECK_ENGINE(e);
+	if (!out) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Sync);
+	uint32_t cnt[2] = {0, 0};
+	int32_t nfree = 0;
+	CU(e, cudaMemcpy(&cnt[0], e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	CU(e, cudaMemcpy(&cnt[1], e->st.task_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	CU(e, cudaMemcpy(&nfree, e->st.svc_tbl.free_n, sizeof(nfree), cudaMemcpyDeviceToHost));
+	memset(out, 0, sizeof(*out));
+	out->max_svcs = e->cfg.max_svcs; out->max_tasks = e->cfg.max_tasks;
+	out->svcs_in_use = std::min(cnt[0], e->cfg.max_svcs) - (uint32_t)std::max(nfree, 0);
+	out->tasks_in_use = std::min(cnt[1], e->cfg.max_tasks);
+	out->ngrows = e->ngrows;
+	out->device_bytes = e->dbytes;
+	return GYSK_OK;
+}
+
+int gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes)
+{
+	if (!svc_slot_bytes || !task_slot_bytes) return GYSK_ERR_INVAL;
+	gysk_config c;
+	gysk_config_default(&c);
+	if (cfg) {
+		if (cfg->struct_size != sizeof(gysk_config)) return GYSK_ERR_INVAL;
+		c = *cfg;
+	}
+	if (c.hll_p < 4 || c.hll_p > 16) return GYSK_ERR_INVAL;
+	slot_bytes(c.hll_p, svc_slot_bytes, task_slot_bytes);
+	return GYSK_OK;
+}
+
 int gysk_flush(gysk_engine *e, uint32_t tsec)
 {
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Submit);
 
+	if (int rc = auto_grow(e)) return rc;
 	if (int rc = roll_levels(e, tsec)) return rc;
 	e->last_flush_tsec = tsec;
 
@@ -1103,11 +1376,19 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 	// tombstones lengthen probe chains: once they fill an eighth of the table, rebuild it from the live slots
 	const uint64_t dead = e->h_evict_fail > e->insert_fail_seen ? e->h_evict_fail - e->insert_fail_seen : 0;
 	if (e->tombstones + dead > ((uint64_t)e->st.svc_tbl.mask + 1) / 8) {
-		e->kernel_launches += launch_rebuild_table(e->st, e->cfg.max_svcs, e->stream);
+		e->kernel_launches += launch_rebuild_table(e->st.svc_tbl, e->cfg.max_svcs, e->stream);
 		e->tombstones = 0; e->insert_fail_seen = e->h_evict_fail;
 	}
 	e->kernel_launches += launch_flush(e->st, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
 	e->kernel_launches += launch_task_flush(e->st, e->cfg.max_tasks, e->stream);
+	if (e->grow_limit_svcs > e->cfg.max_svcs || e->grow_limit_tasks > e->cfg.max_tasks) {
+		// auto-grow: the slot counts travel to the host behind the kernels, for the next flush's decision
+		CU(e, cudaMemcpyAsync(e->h_used, e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaMemcpyAsync(e->h_used + 1, e->st.svc_tbl.free_n, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaMemcpyAsync(e->h_used + 2, e->st.task_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaEventRecord(e->ev_used, e->stream));
+		e->used_pending = true;
+	}
 	if (e->cfg.idle_evict_secs) {
 		// count + ids travel to the host behind the kernels; nobody waits for them here
 		CU(e, cudaMemcpyAsync(e->h_evict, e->st.counters + CTR_NEVICT, sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));

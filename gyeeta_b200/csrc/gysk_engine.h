@@ -260,8 +260,17 @@ struct gysk_engine
 	cudaStream_t		stream {nullptr}, copy_stream {nullptr};
 	gysk::DevState		st {};
 	gysk::SortTemp		tmp {};
-	std::vector<void *>	dallocs;
+	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
+	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
 	std::vector<void *>	hallocs;
+
+	// capacity growth (gysk_grow, gysk_set_auto_grow): the auto-grow ceilings (0 = never), and the slot counts as of the last flush,
+	// copied behind its kernels and read at the next one ({services handed out, services on the free stack, processes handed out})
+	uint32_t		grow_limit_svcs {0}, grow_limit_tasks {0};
+	uint32_t		ngrows {0};
+	uint32_t		*h_used {nullptr};
+	cudaEvent_t		ev_used {nullptr};
+	bool			used_pending {false};
 
 	// staging: per-thread page-locked chunks -> device event buffers (double-buffered) -> kernels
 	uint64_t		uid {0};
@@ -371,8 +380,12 @@ int dalloc(gysk_engine *e, T **p, size_t n, bool zero = true)
 	void *q = nullptr;
 	cudaError_t ce = cudaMalloc(&q, n * sizeof(T));
 
-	if (ce != cudaSuccess) return fail(e, GYSK_ERR_NOMEM, "cudaMalloc", ce);
-	e->dallocs.push_back(q);
+	if (ce != cudaSuccess) {
+		cudaGetLastError();		// an allocation failure is not sticky: it must not surface at the next launch check
+		return fail(e, GYSK_ERR_NOMEM, "cudaMalloc", ce);
+	}
+	e->dallocs.emplace_back(q, n * sizeof(T));
+	e->dbytes += n * sizeof(T);
 	if (zero) {
 		ce = cudaMemsetAsync(q, 0, n * sizeof(T), e->stream);
 		if (ce != cudaSuccess) return fail(e, GYSK_ERR_CUDA, "cudaMemsetAsync", ce);
@@ -387,7 +400,22 @@ void dfree(gysk_engine *e, T *&p)
 {
 	if (!p) return;
 	cudaFree(p);
-	e->dallocs.erase(std::remove(e->dallocs.begin(), e->dallocs.end(), (void *)p), e->dallocs.end());
+	for (size_t i = 0; i < e->dallocs.size(); ++i) {
+		if (e->dallocs[i].first != (void *)p) continue;
+		e->dbytes -= e->dallocs[i].second;
+		e->dallocs.erase(e->dallocs.begin() + i);
+		break;
+	}
+	p = nullptr;
+}
+
+// frees a buffer of halloc and clears the pointer
+template <typename T>
+void hfree(gysk_engine *e, T *&p)
+{
+	if (!p) return;
+	cudaFreeHost(p);
+	e->hallocs.erase(std::remove(e->hallocs.begin(), e->hallocs.end(), (void *)p), e->hallocs.end());
 	p = nullptr;
 }
 
@@ -397,7 +425,10 @@ int halloc(gysk_engine *e, T **p, size_t n)
 	void *q = nullptr;
 	cudaError_t ce = cudaHostAlloc(&q, n * sizeof(T), cudaHostAllocDefault);
 
-	if (ce != cudaSuccess) return fail(e, GYSK_ERR_NOMEM, "cudaHostAlloc", ce);
+	if (ce != cudaSuccess) {
+		cudaGetLastError();
+		return fail(e, GYSK_ERR_NOMEM, "cudaHostAlloc", ce);
+	}
 	e->hallocs.push_back(q);
 	*p = static_cast<T *>(q);
 	return 0;

@@ -165,7 +165,8 @@ static constexpr int TD_MERGE_CTAS_PER_SM = 5, TD_MERGE_MAX_SMS = 192;	// bins_m
 static constexpr int LONG_SEG = 8192;
 
 // every launcher returns the number of kernel launches it issued
-int launch_init_state(const DevState &st, uint32_t max_svcs, uint32_t max_tasks, cudaStream_t s);
+// service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state (the arrays zeroed before)
+int launch_init_slots(const DevState &st, uint32_t s_lo, uint32_t s_hi, uint32_t t_lo, uint32_t t_hi, cudaStream_t s);
 int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_t n, int is_task, cudaStream_t s);
 // -1: no sort plan for max_svcs, or the launch's record regions do not fit the buffers
 int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s);
@@ -186,7 +187,8 @@ int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s);
 // the window roll into ring slot st.levels.cur of each level (cleared by the host when it starts a new epoch), the listener states,
 // the idle-service eviction
 int launch_flush(const DevState &st, uint32_t max_svcs, uint32_t tsec, uint32_t idle_secs, cudaStream_t s);
-int launch_rebuild_table(const DevState &st, uint32_t max_svcs, cudaStream_t s);
+// clears table t and re-inserts the ids t.slot_id holds in slots [0, nslots)
+int launch_rebuild_table(const IdTable &t, uint32_t nslots, cudaStream_t s);
 // the single-id exports: the raw state of n ids (id 0 and unknown ids: found = 0); the HLL registers of the id d_ids[0]
 int launch_gather_svcs(const DevState &st, const unsigned long long *d_ids, uint32_t n, SvcRaw *d_out, cudaStream_t s);
 int launch_gather_tasks(const DevState &st, const unsigned long long *d_ids, uint32_t n, TaskRaw *d_out, cudaStream_t s);

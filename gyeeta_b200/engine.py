@@ -169,6 +169,31 @@ class Stats(C.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class Capacity(C.Structure):
+    """gysk_capacity: current capacities, slots in use, growths so far and the device bytes the engine holds"""
+    _fields_ = [(n, C.c_uint32) for n in ("max_svcs", "max_tasks", "svcs_in_use", "tasks_in_use", "ngrows", "pad")] + \
+               [("device_bytes", C.c_uint64)]
+
+    def asdict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_ if f != "pad"}
+
+
+assert C.sizeof(Capacity) == 32
+
+
+def slot_bytes(hll_p=12):
+    """gysk_slot_bytes (no device needed): (device bytes of one service slot, of one process slot) at this hll_p"""
+    L = load_library()
+    cfg = Config()
+    L.gysk_config_default(C.byref(cfg))
+    cfg.hll_p = hll_p
+    s, t = C.c_uint64(), C.c_uint64()
+    rc = L.gysk_slot_bytes(C.byref(cfg), C.byref(s), C.byref(t))
+    if rc:
+        raise GyskError(rc, "gysk_slot_bytes")
+    return s.value, t.value
+
+
 class BufferDesc(C.Structure):
     _fields_ = [("name", C.c_char_p), ("dptr", C.c_void_p), ("nbytes", C.c_uint64), ("redop", C.c_int32), ("pad", C.c_int32)]
 
@@ -265,6 +290,10 @@ def load_library(path=None):
         "gysk_stream": (vp, [vp]),
         "gysk_profile_enable": (i32, [vp, i32]),
         "gysk_profile_read": (i32, [vp, vp, vp, vp]),
+        "gysk_grow": (i32, [vp, u32, u32]),
+        "gysk_set_auto_grow": (i32, [vp, u32, u32]),
+        "gysk_capacity_info": (i32, [vp, vp]),
+        "gysk_slot_bytes": (i32, [vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = the library does not export what the header declares
@@ -376,6 +405,27 @@ class Engine:
         a, b, n = C.c_double(), C.c_double(), C.c_uint64()
         self._chk(self.L.gysk_profile_read(self.h, C.byref(a), C.byref(b), C.byref(n)))
         return a.value, b.value, n.value
+
+    # ---- capacity ----
+    def grow(self, max_svcs=None, max_tasks=None):
+        """gysk_grow: raise the service / process capacity (None: keep that one). Every answer stays as an engine created at the
+        new capacity would give it."""
+        cap = self.capacity()
+        ms = cap["max_svcs"] if max_svcs is None else max_svcs
+        mt = cap["max_tasks"] if max_tasks is None else max_tasks
+        self._chk(self.L.gysk_grow(self.h, ms, mt))
+        self.cfg.max_svcs, self.cfg.max_tasks = ms, mt
+
+    def set_auto_grow(self, max_svcs_limit=0, max_tasks_limit=0):
+        """gysk_set_auto_grow: at each flush, double a table that was half full at the previous flush, up to its limit (0 = never)"""
+        self._chk(self.L.gysk_set_auto_grow(self.h, max_svcs_limit, max_tasks_limit))
+
+    def capacity(self):
+        """gysk_capacity_info as a dict; also brings self.cfg's capacities up to date after automatic growth"""
+        c = Capacity()
+        self._chk(self.L.gysk_capacity_info(self.h, C.byref(c)))
+        self.cfg.max_svcs, self.cfg.max_tasks = c.max_svcs, c.max_tasks
+        return c.asdict()
 
     # ---- queries ----
     def stats(self):

@@ -365,6 +365,41 @@ uint32_t	gysk_hot_row_word(uint32_t bin);
 /* diagnostic: response samples of the last device batch that travelled as sort keys (the rest updated hot rows). Negative = GYSK_ERR_*. */
 int64_t		gysk_last_batch_keys(gysk_engine *e);
 
+/* ---- capacity: growing the service / process tables of a live engine ---- */
+/* Raise the service / process capacity of a live engine (either may equal the current value; neither may shrink, both <= 1 << 24).
+ * Slot numbers, every per-slot state, the free stack of recycled slots, the hot rows, the last flush's evicted ids, the maps of
+ * gysk_set_logical_map / gysk_set_cluster_map and the last finished merge's results are kept: every read answers afterwards exactly as an
+ * engine created with the new capacity and given the same calls would. Serialised with the ingest threads like a reader (their stages
+ * are drained first). Between gysk_merge_prepare and gysk_merge_finish it is allowed: the prepared buffers do not depend on the
+ * capacity. GYSK_ERR_INVAL: shrink or beyond 1 << 24. GYSK_ERR_NOMEM: the new arrays do not fit the device's free memory; this is
+ * checked before anything is allocated, and the engine is unchanged. Arrays move one at a time, so the device holds at most the new
+ * footprint plus the largest old array while it runs. Should an allocation still fail after the check (another user of the device
+ * took the memory meanwhile), the result is GYSK_ERR_NOMEM too: the engine keeps its capacity and answers every read as before, the
+ * arrays already moved keep their larger size (device_bytes shows it), and a later gysk_grow reuses them. */
+int		gysk_grow(gysk_engine *e, uint32_t max_svcs, uint32_t max_tasks);
+
+/* Auto-grow: at gysk_flush, a table whose slots in use (handed out minus the free stack) reached half its capacity is doubled, up to the
+ * limit (0 = never grow that table; the default). The decision uses the counts as of the PREVIOUS gysk_flush (copied to page-locked
+ * memory there, read after an event wait on work that is one window old), so neither the ingest path nor gysk_flush gains a
+ * synchronisation, and growth points depend only on the sequence of calls. A growth the device's free memory refuses leaves the table
+ * as it is (the flush goes on). GYSK_ERR_INVAL: a limit beyond 1 << 24. */
+int		gysk_set_auto_grow(gysk_engine *e, uint32_t max_svcs_limit, uint32_t max_tasks_limit);
+
+typedef struct gysk_capacity
+{
+	uint32_t	max_svcs, max_tasks;		/* current capacities */
+	uint32_t	svcs_in_use, tasks_in_use;	/* handed out minus the free stack */
+	uint32_t	ngrows, pad;			/* gysk_grow calls that changed something, explicit or automatic */
+	uint64_t	device_bytes;			/* device memory the engine holds */
+} gysk_capacity;
+int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the ingest stream */
+
+/* host only, no device needed: the device bytes one service slot (its rolling-level rows included) and one process slot take in an
+ * engine of this configuration (NULL: the defaults); they depend on hll_p only. An engine's footprint is about
+ * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
+ * buffers and the count-min tables. */
+int		gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes);
+
 /* ---- registration (control path; mirrors partha_listener_info registering listeners before state arrives) ---- */
 int		gysk_register_ids(gysk_engine *e, const uint64_t *ids, uint32_t n, int is_task);
 
