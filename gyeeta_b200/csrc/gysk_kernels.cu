@@ -1911,9 +1911,11 @@ static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
 }
 
 // every other sort: key bits [lo, hi) in 8-bit digits from lo upwards, the last one short; the first ones are 9 bits wide where
-// that saves a whole pass (18 bits -> 9 9)
+// that saves a whole pass (18 bits -> 9 9). A range outside the key's 64 bits has no plan: [0, 72) would fit in 8 passes of 9 bits,
+// and a shift of 64 or more is undefined.
 static int plain_sort_plan(int lo, int hi, SortPlan &P)
 {
+	if (lo < 0 || hi > 64 || lo > hi) return -1;
 	const int T = hi - lo, p8 = (T + 7) / 8, p9 = (T + 8) / 9;
 	int wide = p9 < p8 ? T - 8 * p9 : 0;	// number of 9-bit passes
 	int at = lo;

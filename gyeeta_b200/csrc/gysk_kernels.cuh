@@ -172,7 +172,8 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
 int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
-// sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range, or n_max >= 2^30
+// sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
+// bits outside [0, 64)), or n_max >= 2^30
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);
 // the want best services (host_filter < 0: of every host) or processes (is_task) of nslots by one metric, and with d_slots their slots;
 // -1: sort failed

@@ -378,3 +378,20 @@ def test_task_groupby_equals_the_walk_of_the_reference():
     eng.sync()
     st = eng.stats()
     assert st["events_task"] == int((recs["aggr_task_id"] != 0).sum()) and st["wire_msgs_ok"] == 1
+
+
+def test_task_groupby_at_the_sort_edges():
+    """the group-by's two sorts on a field of ceil(log2 n) bits at new plan shapes: 65 537 samples (17 bits: a 9-bit pass with its
+    carry, then 8), 262 145 (19 bits: 8, 8, 3); and 4097 groups, so the sort of the groups' first arrivals ends one key into a tile"""
+    from gyeeta_b200 import wire
+    rng = np.random.default_rng(43)
+    eng = ge.Engine(max_svcs=64, max_tasks=1 << 14, max_batch=1 << 19)
+    for n, ngroups in ((65_537, 3000), (262_145, 40_000), (12_000, 4097), (65_537, 4097)):
+        s = _proc_samples(rng, n, ngroups)
+        if ngroups == 4097:         # every group present
+            s["aggr_task_id"] = synth.splitmix64(rng.permutation(np.arange(n) % ngroups).astype(np.uint64) + np.uint64(1 << 42))
+        want = po.task_groupby(s, wire.TASK)
+        got, ng = eng.task_groupby(s)
+        assert ng == len(want) == len(np.unique(s["aggr_task_id"]))
+        assert ngroups != 4097 or ng == 4097
+        assert got.tobytes() == want.tobytes(), (n, ngroups)
