@@ -288,6 +288,15 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 	return head.n > cap ? GYSK_ERR_NOSPC : GYSK_OK;
 }
 
+int query_flows_in(gysk_engine *e, const unsigned long long *tbl, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what)
+{
+	DevState st = e->st;
+	st.cms_cur = const_cast<unsigned long long *>(tbl);
+	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
+		return launch_query_flows(st, d_keys, m, 0, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
+	}, CopyRows<gysk_flow_est> {out});
+}
+
 } // namespace gysk
 
 namespace {
@@ -330,20 +339,23 @@ int launch_rows(gysk_engine *e, const unsigned long long *, const unsigned long 
 	return launch_day_stats(e->st, d_slots, m, reinterpret_cast<gysk_listener_day_stats *>(e->d_wstage), e->stream);
 }
 // The rolling levels at the flush of tsec: the closing window goes to ring slot (tsec / width) % NSLOTS of each level, and a slot
-// still holding an older epoch is cleared first. Then the live slots, whose epochs lie in the level's last NSLOTS: what every
-// reader of the levels sums until the next flush. Slot widths: Level_5s_5min_5days_all durations {300 s, 432000 s} / 10 slots
+// still holding an older epoch is cleared first (LevelRing::fresh records it). Then the live slots, whose epochs lie in the level's
+// last NSLOTS: what every reader of the levels sums until the next flush. GYSK_FLAG_FLOW_LEVEL's count-min ring takes level 0's
+// decision as it is (launch_cms_level_roll). Slot widths: Level_5s_5min_5days_all durations {300 s, 432000 s} / 10 slots
 // (gy_statistics.h:1548, :1105).
 int roll_levels(gysk_engine *e, uint32_t tsec)
 {
 	static constexpr uint32_t width[NLEVELS] = {30, 43200};
 	LevelRing &lv = e->st.levels;
 
+	lv.fresh = 0;
 	for (int l = 0; l < NLEVELS; ++l) {
 		const uint64_t epoch = tsec / width[l];
 		const uint32_t k = (uint32_t)(epoch % NSLOTS);
 		if (e->ring_epoch[l][k] != epoch) {
 			CU(e, cudaMemsetAsync(lv.row(l, k, 0), 0, (size_t)lv.stride * HIST_CELLS * sizeof(HistCell), e->stream));
 			e->ring_epoch[l][k] = epoch;
+			lv.fresh |= 1u << l;
 		}
 		lv.cur[l] = k;
 		lv.live[l] = 0;
@@ -542,6 +554,11 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(halloc(e, &e->h_used, 4));
 	if ((ce = cudaEventCreateWithFlags(&e->ev_used, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
 	A(dalloc(e, &st.cms_cur, (size_t)cfg.cms_depth << cfg.cms_log2_width)); A(dalloc(e, &st.cms_last, (size_t)cfg.cms_depth << cfg.cms_log2_width));
+	if (cfg.flags & GYSK_FLAG_FLOW_LEVEL) {
+		// not per slot: outside each_slot_array, so gysk_grow leaves them; device_bytes counts them
+		A(dalloc(e, &st.cms_ring, (size_t)NSLOTS * ((size_t)cfg.cms_depth << cfg.cms_log2_width)));
+		A(dalloc(e, &st.cms_5min, (size_t)cfg.cms_depth << cfg.cms_log2_width));
+	}
 	st.cms_depth = cfg.cms_depth; st.cms_log2w = cfg.cms_log2_width; st.cms_wmask = (1u << cfg.cms_log2_width) - 1; st.hll_p = cfg.hll_p;
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
 	st.td_delta = (double)cfg.td_compression;
@@ -1397,6 +1414,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		CU(e, cudaEventRecord(e->ev_evict, e->stream));
 		e->evict_pending = true;
 	}
+	if (e->st.cms_ring) e->kernel_launches += launch_cms_level_roll(e->st, e->stream);		// GYSK_FLAG_FLOW_LEVEL
 	std::swap(e->st.cms_cur, e->st.cms_last);
 	CU(e, cudaMemsetAsync(e->st.cms_cur, 0, sizeof(unsigned long long) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), e->stream));
 	return post_launch(e, "flush");
@@ -1792,9 +1810,16 @@ int gysk_query_flows(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_
 	CHECK_ENGINE(e);
 	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Submit);
-	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_est), "query_flows", [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
-		return launch_query_flows(e->st, d_keys, m, last_window, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
-	}, CopyRows<gysk_flow_est> {out});
+	return query_flows_in(e, last_window ? e->st.cms_last : e->st.cms_cur, keys, n, out, "query_flows");
+}
+
+int gysk_query_flows_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_est *out)
+{
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Submit);
+	return query_flows_in(e, e->st.cms_5min, keys, n, out, "query_flows_5min");
 }
 
 int gysk_topn_svcs(gysk_engine *e, int metric, int32_t host_idx, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
@@ -1874,6 +1899,16 @@ int gysk_export_cms(gysk_engine *e, int last_window, uint64_t *cells)
 	GYSK_ENTER(e, Sync);
 	CU(e, cudaMemcpy(cells, last_window ? e->st.cms_last : e->st.cms_cur, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width),
 			cudaMemcpyDeviceToHost));
+	return GYSK_OK;
+}
+
+int gysk_export_cms_5min(gysk_engine *e, uint64_t *cells)
+{
+	CHECK_ENGINE(e);
+	if (!cells) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Sync);
+	CU(e, cudaMemcpy(cells, e->st.cms_5min, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), cudaMemcpyDeviceToHost));
 	return GYSK_OK;
 }
 

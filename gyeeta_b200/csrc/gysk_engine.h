@@ -95,7 +95,8 @@ constexpr int STATE_WORDS = 15;
 static_assert(sizeof(gysk_host_summary) == (STATE_WORDS + 1) * sizeof(int32_t), "gysk_host_summary: 15 fields and a pad");
 
 // The merged arrays of the nl logical services: the merge arena's per-logical arrays and the t-digest slabs, passed by value to the
-// merge kernels. lvl .. flush exist with GYSK_FLAG_MERGE_LEVELS only, states with GYSK_FLAG_MERGE_STATES only (nullptr without).
+// merge kernels. lvl .. rtt exist with GYSK_FLAG_MERGE_LEVELS only, flush with it or GYSK_FLAG_FLOW_LEVEL, states with
+// GYSK_FLAG_MERGE_STATES only (nullptr without).
 struct LogicalArrays
 {
 	uint32_t		nl {0};
@@ -232,11 +233,13 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last, hist last/all, conn [, levels, aux] [, states] [, clusters]
-	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt, flush tsec]
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min], hist last/all, conn [, levels, aux] [, states]
+									//           [, clusters]
+	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt] [, flush tsec]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	std::string		name_sum, name_maxi64, name_maxu8;	// the regions' gysk_buffer_desc names: their arrays, in order
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
+	unsigned long long	*g_cms_5min {nullptr};				// GYSK_FLAG_FLOW_LEVEL: the count-min level, summed over ranks
 	LogicalArrays		lg;
 	ClusterMap		clusters;				// kept across gysk_set_logical_map
 	bool			prepared {false}, finished {false};
@@ -347,6 +350,8 @@ void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint6
 void level_from_cells(const HistCell *cells, gysk_hist_serial *out, uint64_t *total, int64_t *maxv);
 // the gysk_export_tdigest answer of one digest: up to min(cap, TD_CAP) centroids, min and max; GYSK_ERR_NOSPC when it has more than cap
 int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_t *weights, uint32_t cap, uint32_t *n, double *minv, double *maxv);
+// the count-min point queries of gysk_query_flows on table tbl (one of the engine's tables, a merged one or a level), engine held
+int query_flows_in(gysk_engine *e, const unsigned long long *tbl, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)

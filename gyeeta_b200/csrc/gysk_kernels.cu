@@ -1862,6 +1862,32 @@ __global__ void query_flows_kernel(DevState st, const unsigned long long *__rest
 	out[i].flow_key = key; out[i].count = cnt; out[i].kbytes = kb;
 }
 
+// GYSK_FLAG_FLOW_LEVEL: the count-min level at a flush, one grid-stride pass over the cells in 16-byte pairs. Ring slot k takes the
+// closing window cur, added to what the slot holds or, when the flush started a new epoch there, in its place (which stands in for
+// clearing the slot). The level becomes the sum of the live slots, slot k's new content included. So the pass reads cur and the live
+// slots and writes slot k and the level, every cell mod 2^64 as RED.ADD.64 builds cur. The ring and the level are streamed
+// (evict-first) so that the pass does not push out of L2 the count-min lines the ingest path keeps resident.
+__global__ void __launch_bounds__(256) cms_level_roll_kernel(const ulonglong2 *__restrict__ cur, ulonglong2 *__restrict__ ring,
+		ulonglong2 *__restrict__ level, uint64_t npair, uint32_t k, uint32_t live, uint32_t fresh)
+{
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < npair; i += (uint64_t)gridDim.x * blockDim.x) {
+		ulonglong2 r = cur[i];
+		if (!fresh) {
+			const ulonglong2 o = __ldcs(ring + k * npair + i);
+			r.x += o.x; r.y += o.y;
+		}
+		__stcs(ring + k * npair + i, r);
+		ulonglong2 a = make_ulonglong2(0, 0);
+#pragma unroll
+		for (uint32_t j = 0; j < NSLOTS; ++j) {
+			if (!((live >> j) & 1u)) continue;
+			const ulonglong2 x = j == k ? r : __ldcs(ring + j * npair + i);
+			a.x += x.x; a.y += x.y;
+		}
+		__stcs(level + i, a);
+	}
+}
+
 // ---------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------
@@ -2234,6 +2260,15 @@ int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uin
 {
 	if (!n) return 0;
 	query_flows_kernel<<<div_up(n, 256), 256, 0, s>>>(st, d_keys, n, last_window, d_out);
+	return 1;
+}
+
+int launch_cms_level_roll(const DevState &st, cudaStream_t s)
+{
+	const uint64_t npair = ((uint64_t)st.cms_depth << st.cms_log2w) / 2;		// log2w >= 4: whole pairs
+	const uint32_t grid = std::min<uint32_t>(div_up(npair, 256), (uint32_t)sm_count(current_device()) * 8u);
+	cms_level_roll_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const ulonglong2 *>(st.cms_cur), reinterpret_cast<ulonglong2 *>(st.cms_ring),
+			reinterpret_cast<ulonglong2 *>(st.cms_5min), npair, st.levels.cur[0], st.levels.live[0], st.levels.fresh & 1u);
 	return 1;
 }
 

@@ -13,14 +13,16 @@ static constexpr int NLEVELS = 2;			// rolling levels beyond the 5-s window: 300
 static constexpr int NSLOTS = 10;			// slots per level (gy_statistics.h:1105)
 
 // The rolling 300-s / 5-day levels: per level NSLOTS ring slots, each a plane of `stride` service rows of 16 cells
-// ([NLEVELS][NSLOTS][stride][16]). stride is max_svcs: the null slot (index max_svcs) has no ring row. live and cur are set by the
-// host at every flush (roll_levels in gysk_engine.cu); both are 0 until the first one.
+// ([NLEVELS][NSLOTS][stride][16]). stride is max_svcs: the null slot (index max_svcs) has no ring row. live, cur and fresh are set by
+// the host at every flush (roll_levels in gysk_engine.cu); all are 0 until the first one. The count-min level of GYSK_FLAG_FLOW_LEVEL
+// follows level 0's decision (cms_level_roll_kernel).
 struct LevelRing
 {
 	HistCell		*ring;
 	uint32_t		stride;
 	uint32_t		live[NLEVELS];		// the ring slots inside each level's span at the last flush
 	uint32_t		cur[NLEVELS];		// the ring slot of each level the last flush wrote
+	uint32_t		fresh;			// bit l: the last flush started a new epoch in level l's slot cur (its old content cleared)
 
 	__host__ __device__ __forceinline__ HistCell *row(int l, uint32_t k, uint32_t slot) const
 	{
@@ -76,6 +78,8 @@ struct DevState
 	uint32_t		*task_slot_host;
 	// flow sketch
 	unsigned long long	*cms_cur, *cms_last;			// [depth][1 << log2w]
+	unsigned long long	*cms_ring, *cms_5min;			// GYSK_FLAG_FLOW_LEVEL (nullptr without): [NSLOTS][depth][1 << log2w] level-0
+									// ring slots of closed windows, and the sum of the live ones
 	uint32_t		cms_depth, cms_wmask, cms_log2w, hll_p;
 	uint32_t		rank, world, auto_register;
 	double			td_delta;
@@ -214,5 +218,8 @@ int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, co
 int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, gysk_task_summary *d_out,
 		cudaStream_t s);
 int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uint32_t n, int last_window, gysk_flow_est *d_out, cudaStream_t s);
+// GYSK_FLAG_FLOW_LEVEL, at the flush before the cms_cur / cms_last swap: cms_cur into ring slot st.levels.cur[0] (replacing it when
+// the slot is fresh), then cms_5min = the sum of the live slots
+int launch_cms_level_roll(const DevState &st, cudaStream_t s);
 
 } // namespace gysk

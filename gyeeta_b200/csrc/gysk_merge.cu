@@ -12,7 +12,9 @@
 //                          levels and aux sums to the SUM region, their maxima, the rtt and the flush tsec pair to the i64 MAX one;
 //                          GYSK_FLAG_MERGE_STATES appends the members' LISTEN_SUMM_STATS words to the SUM region,
 //                          GYSK_FLAG_MERGE_CLUSTERS the host clusters' MS_CLUSTER_STATE words after them (gysk_set_cluster_map);
-//                          GYSK_FLAG_MERGE_TOPN appends this rank's 64 best services / processes per metric, with their rows, to the slab
+//                          GYSK_FLAG_MERGE_TOPN appends this rank's 64 best services / processes per metric, with their rows, to the slab;
+//                          GYSK_FLAG_FLOW_LEVEL puts the count-min level after cms cur/last and, as GYSK_FLAG_MERGE_LEVELS does,
+//                          the flush tsec pair in the i64 MAX region (once when both are set)
 //   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests [, the global pick of the gathered top-N candidates]
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
@@ -702,9 +704,11 @@ int lay_out_arena(gysk_engine *e)
 
 	// The arena region by region, each array 256-byte aligned: layout(nullptr) sizes it, layout(arena) places the arrays. Each array's
 	// name joins its region's gysk_merge_buffers name. GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX
-	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those:
+	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those.
+	// GYSK_FLAG_FLOW_LEVEL puts the count-min level after the two window tables, and needs the flush tsec pair as the levels do:
 	// still three regions, three collectives.
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
+	const bool flow_level = e->cfg.flags & GYSK_FLAG_FLOW_LEVEL;
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
@@ -716,6 +720,7 @@ int lay_out_arena(gysk_engine *e)
 		};
 		mg.off_sum = off;
 		take(mg.g_cms_cur, b_cms, "cms_cur"); take(mg.g_cms_last, b_cms, "cms_last");
+		if (flow_level) take(mg.g_cms_5min, b_cms, "cms_5min");
 		take(lg.last, b_hist, "hist_last"); take(lg.all, b_hist, "hist_all"); take(lg.conn, (size_t)nl * 4 * 8, "conn");
 		if (levels) { take(lg.lvl, NLEVELS * b_hist, "levels"); take(lg.aux, (size_t)nl * 4 * 8, "aux"); }
 		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8, "states");
@@ -725,7 +730,8 @@ int lay_out_arena(gysk_engine *e)
 		names.clear();
 		mg.off_maxi64 = off;
 		take(lg.hmax, (size_t)nl * 2 * 8, "hist max_val_seen");
-		if (levels) { take(lg.lvl_max, (size_t)nl * NLEVELS * 8, "level max_val_seen"); take(lg.rtt, (size_t)nl * 8, "rtt"); take(lg.flush, 2 * 8, "flush tsec"); }
+		if (levels) { take(lg.lvl_max, (size_t)nl * NLEVELS * 8, "level max_val_seen"); take(lg.rtt, (size_t)nl * 8, "rtt"); }
+		if (levels || flow_level) take(lg.flush, 2 * 8, "flush tsec");
 		mg.bytes_maxi64 = off - mg.off_maxi64;
 		mg.name_maxi64 = "max_i64: " + names;
 		names.clear();
@@ -876,6 +882,7 @@ int gysk_merge_prepare(gysk_engine *e)
 
 	CU(e, cudaMemcpyAsync(mg.g_cms_cur, e->st.cms_cur, b_cms, cudaMemcpyDeviceToDevice, e->stream));
 	CU(e, cudaMemcpyAsync(mg.g_cms_last, e->st.cms_last, b_cms, cudaMemcpyDeviceToDevice, e->stream));
+	if (mg.g_cms_5min) CU(e, cudaMemcpyAsync(mg.g_cms_5min, e->st.cms_5min, b_cms, cudaMemcpyDeviceToDevice, e->stream));		// GYSK_FLAG_FLOW_LEVEL
 	if (nl) {
 		if (mg.nmembers) {
 			resolve_members_kernel<<<div_up(mg.nmembers, 256), 256, 0, e->stream>>>(e->st, mg.d_member_ids, mg.nmembers, mg.members);
@@ -890,9 +897,11 @@ int gysk_merge_prepare(gysk_engine *e)
 			e->kernel_launches++;
 		}
 	}
-	if (mg.lg.lvl) {		// GYSK_FLAG_MERGE_LEVELS: also with no logical service, for the flush tsec pair
-		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.members,
-				(long long)e->last_flush_tsec, mg.lg);
+	if (mg.lg.flush) {		// GYSK_FLAG_MERGE_LEVELS or GYSK_FLAG_FLOW_LEVEL: also with no logical service, for the flush tsec pair
+		LogicalArrays lg = mg.lg;
+		if (!lg.lvl) lg.nl = 0;		// GYSK_FLAG_FLOW_LEVEL alone: the pair only
+		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)lg.nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.members,
+				(long long)e->last_flush_tsec, lg);
 		e->kernel_launches++;
 	}
 	if (const uint32_t nc = mg.clusters.cl.nc) {		// GYSK_FLAG_MERGE_CLUSTERS with a cluster map
@@ -1107,7 +1116,7 @@ int gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tse
 {
 	CHECK_ENGINE(e);
 	if (!min_tsec || !max_tsec) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_MERGE_LEVELS)) return GYSK_ERR_NOTSUP;
+	if (!(e->cfg.flags & (GYSK_FLAG_MERGE_LEVELS | GYSK_FLAG_FLOW_LEVEL))) return GYSK_ERR_NOTSUP;
 	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_merge_flush_range: no finished merge");
@@ -1126,11 +1135,19 @@ int gysk_query_flows_global(gysk_engine *e, const uint64_t *keys, uint32_t n, in
 	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global: no merge");
-	DevState st = e->st;
-	st.cms_cur = mg.g_cms_cur; st.cms_last = mg.g_cms_last;
-	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_est), "query_flows_global", [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
-		return launch_query_flows(st, d_keys, m, last_window, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
-	}, CopyRows<gysk_flow_est> {out});
+	return query_flows_in(e, last_window ? mg.g_cms_last : mg.g_cms_cur, keys, n, out, "query_flows_global");
+}
+
+// GYSK_FLAG_FLOW_LEVEL: the point query on the count-min level summed over the ranks
+int gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_est *out)
+{
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global_5min: no merge");
+	return query_flows_in(e, mg.g_cms_5min, keys, n, out, "query_flows_global_5min");
 }
 
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)

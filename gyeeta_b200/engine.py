@@ -32,7 +32,7 @@ assert RESP16_DTYPE.itemsize == 16 and TCP24_DTYPE.itemsize == 24 and TASK24_DTY
 NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CONN_STATS = 0x309, 0x30C, 0x310, 0x312
 (HOSTTOP_SVC_ISSUE, HOSTTOP_SVC_QPS, HOSTTOP_SVC_CONNS, HOSTTOP_SVC_NET, HOSTTOP_TASK_ISSUE, HOSTTOP_TASK_NET, HOSTTOP_TASK_CPU, HOSTTOP_TASK_RSS,
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
-FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, FLAG_MERGE_TOPN = 1, 2, 4, 8, 16
+FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, FLAG_MERGE_TOPN, FLAG_FLOW_LEVEL = 1, 2, 4, 8, 16, 32
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
@@ -284,6 +284,9 @@ def load_library(path=None):
         "gysk_topn_global": (i32, [vp, i32, u32, vp, vp, vp]),
         "gysk_topn_global_tasks": (i32, [vp, i32, u32, vp, vp, vp]),
         "gysk_query_flows_global": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_flows_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_export_cms_5min": (i32, [vp, vp]),
+        "gysk_query_flows_global_5min": (i32, [vp, vp, u32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -313,7 +316,7 @@ class Engine:
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
-                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False):
+                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -324,7 +327,7 @@ class Engine:
         cfg.idle_evict_secs = idle_evict_secs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
-                    (FLAG_MERGE_TOPN if merge_topn else 0)
+                    (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -529,6 +532,13 @@ class Engine:
         keys = np.ascontiguousarray(keys, dtype=np.uint64)
         out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
         self._chk(self.L.gysk_query_flows(self.h, _p(keys), len(keys), int(last_window), _p(out)))
+        return out
+
+    def query_flows_5min(self, keys):
+        """gysk_query_flows_5min: the point query on the rolling 300-s count-min level (flow_level=True)"""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
+        self._chk(self.L.gysk_query_flows_5min(self.h, _p(keys), len(keys), _p(out)))
         return out
 
     def topn(self, metric, n=10, host_idx=-1):
@@ -777,7 +787,20 @@ class Engine:
         self._chk(self.L.gysk_query_flows_global(self.h, _p(keys), len(keys), int(last_window), _p(out)))
         return out
 
+    def query_flows_global_5min(self, keys):
+        """gysk_query_flows_global_5min: the point query on the 300-s count-min level summed over the ranks by the last merge"""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
+        self._chk(self.L.gysk_query_flows_global_5min(self.h, _p(keys), len(keys), _p(out)))
+        return out
+
     def export_cms(self, last_window=False):
         out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
         self._chk(self.L.gysk_export_cms(self.h, int(last_window), _p(out)))
+        return out
+
+    def export_cms_5min(self):
+        """gysk_export_cms_5min: the cells of the rolling 300-s count-min level (flow_level=True)"""
+        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
+        self._chk(self.L.gysk_export_cms_5min(self.h, _p(out)))
         return out

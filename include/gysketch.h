@@ -203,6 +203,11 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   every rank. Its candidates travel in the t-digest slab: gysk_merge_tdigest_slab reports
 						   the larger size, the collectives stay the same. A merge needs no gysk_set_logical_map.
 						   Without it the merge slab, arena and collectives are as before */
+#define GYSK_FLAG_FLOW_LEVEL		0x20u	/* a rolling 300-s count-min level beside the current and last windows' tables
+						   (gysk_query_flows_5min, gysk_export_cms_5min); with it the merge step also sums the
+						   level across ranks (gysk_query_flows_global_5min; the same flags on every rank).
+						   Costs NSLOTS + 1 = 11 more tables of depth << log2_width cells. Without it nothing is
+						   allocated, every other call answers as before and the three calls are GYSK_ERR_NOTSUP */
 
 typedef struct gysk_config
 {
@@ -397,7 +402,8 @@ int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the
 /* host only, no device needed: the device bytes one service slot (its rolling-level rows included) and one process slot take in an
  * engine of this configuration (NULL: the defaults); they depend on hll_p only. An engine's footprint is about
  * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
- * buffers and the count-min tables. */
+ * buffers and the count-min tables: 2 tables of cms_depth << cms_log2_width 8-byte cells, 11 more with GYSK_FLAG_FLOW_LEVEL (its 10 ring
+ * slots and the level: 352 MiB more at the default 4 x 2^20). The count-min tables do not depend on capacity, so gysk_grow leaves them. */
 int		gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes);
 
 /* ---- registration (control path; mirrors partha_listener_info registering listeners before state arrives) ---- */
@@ -533,6 +539,22 @@ int		gysk_export_tdigest(gysk_engine *e, uint64_t glob_id, double *means, uint64
 int		gysk_query_quantiles(gysk_engine *e, uint64_t glob_id, const double *qs, uint32_t nq, double *out);
 int		gysk_export_cms(gysk_engine *e, int last_window, uint64_t *cells /* depth << log2_width entries */);
 
+/* ---- the rolling 300-s flow level (GYSK_FLAG_FLOW_LEVEL): connections and kbytes of a flow in the last five minutes ----
+ * The level holds every flow update, from any ingest route, of the windows closed by the flushes the 300-s response level holds:
+ * those whose tsec / 30 lies within the last 10 epochs of the last gysk_flush's tsec / 30 (ring slot (tsec / 30) % 10, a slot
+ * holding an older epoch cleared first). It follows that level's rule over gaps and repeated tsec exactly, and is empty before the
+ * first flush. The open window is not in it. Because the count-min is linear, the level is the cell-wise sum of those windows'
+ * gysk_export_cms(last_window = 1) tables, each packed {count | kbytes << 32} cell mod 2^64 like the table itself.
+ * gysk_query_flows_5min: the point query of gysk_query_flows on the level, the minimum over rows of each half.
+ * gysk_export_cms_5min: the level's cells (depth << log2_width entries).
+ * gysk_query_flows_global_5min: the point query on the level summed over the ranks by the last merge (GYSK_ERR_INVAL before
+ * gysk_merge_prepare). A rank's level is relative to its own last flush: gysk_merge_flush_range shows whether the ranks had closed
+ * the same window.
+ * All three are GYSK_ERR_NOTSUP without the flag. */
+int		gysk_query_flows_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_est *out);
+int		gysk_export_cms_5min(gysk_engine *e, uint64_t *cells /* depth << log2_width entries */);
+int		gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_est *out);
+
 /* ---- row a15b: the per-process -> per-aggregate-process group-by in front of partha_aggr_task_state ----
  * One record per process and 5-s tick, holding what TASK_HANDLER's walk has at hand when it folds the process into
  * aggrnotmap.try_emplace(aggr_task_id) (common/gy_task_handler.cc:752-880). */
@@ -616,8 +638,8 @@ int		gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n,
  * GYSK_ERR_INVAL before a finished merge or for another `which`. */
 int		gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS],
 				uint64_t *total_count, int64_t *max_val);
-/* The earliest and latest tsec of the ranks' last gysk_flush, as all-reduced by the last finished merge (GYSK_FLAG_MERGE_LEVELS;
- * GYSK_ERR_NOTSUP without it, GYSK_ERR_INVAL before a finished merge). Each rank's level slots are relative to its own last
+/* The earliest and latest tsec of the ranks' last gysk_flush, as all-reduced by the last finished merge (GYSK_FLAG_MERGE_LEVELS or
+ * GYSK_FLAG_FLOW_LEVEL; GYSK_ERR_NOTSUP without both, GYSK_ERR_INVAL before a finished merge). Each rank's level slots are relative to its own last
  * flush, so *min_tsec != *max_tsec means the ranks had closed different windows and the merged levels mix them. That is not an
  * error: the collectives cannot fail on one rank alone, so the caller decides what to do with such an answer. */
 int		gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tsec);
