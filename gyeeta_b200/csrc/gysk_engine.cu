@@ -90,6 +90,12 @@ int collect_evicted(gysk_engine *e)
 	e->h_evict_fail = e->h_evict[e->cfg.max_svcs + 1];
 	e->evicted_ids.assign(e->h_evict + 1, e->h_evict + 1 + cnt);
 	e->tombstones += cnt; e->evicted_total += cnt;
+	if (e->h_tevict) {
+		const uint64_t tcnt = std::min<uint64_t>(e->h_tevict[0], e->cfg.max_tasks);
+		e->evicted_task_ids.assign(e->h_tevict + 1, e->h_tevict + 1 + tcnt);
+		std::sort(e->evicted_task_ids.begin(), e->evicted_task_ids.end());		// the list's order depends on the device's atomics
+		e->task_tombstones += tcnt; e->task_evicted_total += tcnt;
+	}
 	e->evict_pending = false;
 	return 0;
 }
@@ -372,10 +378,11 @@ int roll_levels(gysk_engine *e, uint32_t tsec)
 // Every device array indexed by service or process slot, with its elements per slot: f(pointer, elements per slot, kind). Svc arrays
 // hold max_svcs + 1 slots (slot max_svcs is the null slot), the level ring max_svcs rows in each of its NLEVELS x NSLOTS planes
 // (LevelRing::stride), Task arrays max_tasks slots. gysk_create allocates exactly these, gysk_grow moves them, slot_bytes sums them.
+// The process eviction's arrays exist only with task_idle_evict_secs (task_evict).
 enum class SlotKind { Svc, Ring, Task };
 
 template <typename F>
-void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, F f)
+void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, bool task_evict, F f)
 {
 	f(st.slot_id, 1, SlotKind::Svc); f(st.slot_host, 1, SlotKind::Svc);
 	f(st.slot_first_seen, 1, SlotKind::Svc); f(st.slot_last_active, 1, SlotKind::Svc);
@@ -391,15 +398,19 @@ void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, F f)
 	f(tmp.touched, 1, SlotKind::Svc); f(tmp.segs, 1, SlotKind::Svc);
 	f(st.task_hist, 3 * HIST_CELLS, SlotKind::Task); f(st.task_prev, 3, SlotKind::Task); f(st.task_last, 3, SlotKind::Task);
 	f(st.task_slot_id, 1, SlotKind::Task); f(st.task_slot_host, 1, SlotKind::Task);
+	if (task_evict) {
+		f(st.task_last_active, 1, SlotKind::Task); f(st.task_evict_list, 1, SlotKind::Task); f(st.task_evict_ids, 1, SlotKind::Task);
+		f(st.task_tbl.free_slots, 1, SlotKind::Task);
+	}
 }
 
 // device bytes of one service slot (its ring rows included) and of one process slot: the sums of each_slot_array
-void slot_bytes(uint32_t hll_p, uint64_t *svc, uint64_t *task)
+void slot_bytes(uint32_t hll_p, bool task_evict, uint64_t *svc, uint64_t *task)
 {
 	DevState st {};
 	SortTemp tmp {};
 	uint64_t b[3] = {0, 0, 0};
-	each_slot_array(st, tmp, hll_p, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
+	each_slot_array(st, tmp, hll_p, task_evict, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
 	*svc = b[(int)SlotKind::Svc] + b[(int)SlotKind::Ring];
 	*task = b[(int)SlotKind::Task];
 }
@@ -542,8 +553,9 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &st.svc_tbl.free_n, 1));
 	A(dalloc(e, &st.task_tbl.ent, tcap)); st.task_tbl.mask = tcap - 1; st.task_tbl.max_slots = cfg.max_tasks;
 	A(dalloc(e, &st.task_tbl.count, 1));
+	if (cfg.task_idle_evict_secs) A(dalloc(e, &st.task_tbl.free_n, 1));		// without it the process table has no free stack
 	SortTemp &tmp = e->tmp;
-	each_slot_array(st, tmp, cfg.hll_p, [&](auto *&p, size_t k, SlotKind kind) { if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks) * k); });
+	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) { if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks) * k); });
 	if (rc) return bail(rc);
 	st.levels.stride = cfg.max_svcs;
 	st.svc_tbl.slot_id = st.slot_id; st.svc_tbl.slot_host = st.slot_host;
@@ -551,7 +563,13 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(halloc(e, &e->h_evict, ns + 2));
 	e->h_evict[0] = 0; e->h_evict[cfg.max_svcs + 1] = 0;
 	if ((ce = cudaEventCreateWithFlags(&e->ev_evict, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
+	if (cfg.task_idle_evict_secs) {
+		A(halloc(e, &e->h_tevict, (size_t)cfg.max_tasks + 1, cudaHostAllocMapped));
+		e->h_tevict[0] = 0;
+		if ((ce = cudaHostGetDevicePointer((void **)&e->d_tevict, e->h_tevict, 0)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaHostGetDevicePointer", ce); return bail(GYSK_ERR_CUDA); }
+	}
 	A(halloc(e, &e->h_used, 4));
+	e->h_used[3] = 0;		// processes on the free stack: stays 0 without process eviction
 	if ((ce = cudaEventCreateWithFlags(&e->ev_used, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
 	A(dalloc(e, &st.cms_cur, (size_t)cfg.cms_depth << cfg.cms_log2_width)); A(dalloc(e, &st.cms_last, (size_t)cfg.cms_depth << cfg.cms_log2_width));
 	if (cfg.flags & GYSK_FLAG_FLOW_LEVEL) {
@@ -676,7 +694,9 @@ int gysk_get_stats(gysk_engine *e, gysk_stats *out)
 	CU(e, cudaMemcpy(&nfree, e->st.svc_tbl.free_n, sizeof(nfree), cudaMemcpyDeviceToHost));
 	out->nsvcs = std::min<uint64_t>((uint32_t)e->h_counters[CTR_MAX], e->cfg.max_svcs) - (uint64_t)std::max(nfree, 0);
 	out->svcs_evicted = e->evicted_total;
-	out->ntasks = std::min<uint64_t>((uint32_t)e->h_counters[CTR_MAX + 1], e->cfg.max_tasks);
+	int32_t tfree = 0;
+	if (e->st.task_tbl.free_n) CU(e, cudaMemcpy(&tfree, e->st.task_tbl.free_n, sizeof(tfree), cudaMemcpyDeviceToHost));
+	out->ntasks = std::min<uint64_t>((uint32_t)e->h_counters[CTR_MAX + 1], e->cfg.max_tasks) - (uint64_t)std::max(tfree, 0);
 	out->batches = e->batches; out->kernel_launches = e->kernel_launches;
 	out->wire_msgs_ok = e->wire_ok; out->wire_msgs_bad = e->wire_bad;
 	return GYSK_OK;
@@ -1220,7 +1240,7 @@ void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, siz
 		big = std::max(big, old_n * elem);
 		n++;
 	};
-	each_slot_array(st, tmp, cfg.hll_p, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) {
 		move(k * sizeof(*p), slots_of(kind, cfg.max_svcs, cfg.max_tasks), slots_of(kind, ms, mt));
 	});
 	if (ms != cfg.max_svcs) move(sizeof(TblEntry), table_cap(cfg.max_svcs + 1), table_cap(ms + 1));
@@ -1257,7 +1277,7 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 	to.max_svcs = ms; to.max_tasks = mt;
 	int rc = 0;
 	// phase 1
-	each_slot_array(st, tmp, cfg.hll_p, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) {
 		if (rc) return;
 		if (kind == SlotKind::Ring) rc = regrow_ring(e, ms);
 		else rc = regrow(e, p, slots_of(kind, os, ot) * k, slots_of(kind, ms, mt) * k);
@@ -1272,11 +1292,16 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 	if (rc) return rc;
 	// phase 2
 	TblEntry *sent = nullptr, *tent = nullptr;
-	unsigned long long *hev = nullptr;
+	unsigned long long *hev = nullptr, *htev = nullptr, *dtev = nullptr;
 	if ((ms != os && (rc = dalloc(e, &sent, table_cap(ms + 1), false))) || (mt != ot && (rc = dalloc(e, &tent, table_cap(mt), false))) ||
-			(ms != os && (rc = halloc(e, &hev, (size_t)ms + 3)))) {
-		dfree(e, sent); dfree(e, tent);
+			(ms != os && (rc = halloc(e, &hev, (size_t)ms + 3))) ||
+			(mt != ot && e->h_tevict && (rc = halloc(e, &htev, (size_t)mt + 1, cudaHostAllocMapped)))) {
+		dfree(e, sent); dfree(e, tent); hfree(e, hev);
 		return rc;
+	}
+	if (htev) {
+		const cudaError_t ce = cudaHostGetDevicePointer((void **)&dtev, htev, 0);
+		if (ce != cudaSuccess) { dfree(e, sent); dfree(e, tent); hfree(e, hev); hfree(e, htev); return fail(e, GYSK_ERR_CUDA, "cudaHostGetDevicePointer", ce); }
 	}
 	// phase 3: the old null slot and every new slot in their just-created state (the new null slot is the last one), then both id
 	// tables rebuilt at their new capacity: slot numbers, hot rows (SlotBatch::hot of the slot) and the free stack stay. A rebuild
@@ -1299,7 +1324,15 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 		CU(e, cudaStreamSynchronize(e->stream));
 		e->tombstones = 0; e->insert_fail_seen = fails;
 	}
-	if (mt != ot) swap_table(st.task_tbl, tent, mt, mt);
+	if (mt != ot) {
+		if (htev) {
+			htev[0] = 0;
+			hfree(e, e->h_tevict);
+			e->h_tevict = htev; e->d_tevict = dtev;
+		}
+		swap_table(st.task_tbl, tent, mt, mt);
+		e->task_tombstones = 0;
+	}
 	e->mg.members.null_slot = ms;			// the member slots are resolved again at every gysk_merge_prepare
 	e->ngrows++;
 	CU(e, cudaStreamSynchronize(e->stream));
@@ -1315,7 +1348,7 @@ int auto_grow(gysk_engine *e)
 	e->used_pending = false;
 	const uint32_t ms = e->cfg.max_svcs, mt = e->cfg.max_tasks;
 	const uint64_t svcs = (uint64_t)std::min(e->h_used[0], ms) - (uint64_t)std::max((int32_t)e->h_used[1], 0);
-	const uint64_t tasks = std::min(e->h_used[2], mt);
+	const uint64_t tasks = (uint64_t)std::min(e->h_used[2], mt) - (uint64_t)std::max((int32_t)e->h_used[3], 0);
 	auto next = [](uint32_t cap, uint64_t used, uint32_t limit) {
 		return limit > cap && 2 * used >= cap ? (uint32_t)std::min<uint64_t>(2ull * cap, limit) : cap;
 	};
@@ -1353,14 +1386,15 @@ int gysk_capacity_info(gysk_engine *e, gysk_capacity *out)
 	if (!out) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Sync);
 	uint32_t cnt[2] = {0, 0};
-	int32_t nfree = 0;
+	int32_t nfree = 0, tfree = 0;
 	CU(e, cudaMemcpy(&cnt[0], e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
 	CU(e, cudaMemcpy(&cnt[1], e->st.task_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
 	CU(e, cudaMemcpy(&nfree, e->st.svc_tbl.free_n, sizeof(nfree), cudaMemcpyDeviceToHost));
+	if (e->st.task_tbl.free_n) CU(e, cudaMemcpy(&tfree, e->st.task_tbl.free_n, sizeof(tfree), cudaMemcpyDeviceToHost));
 	memset(out, 0, sizeof(*out));
 	out->max_svcs = e->cfg.max_svcs; out->max_tasks = e->cfg.max_tasks;
 	out->svcs_in_use = std::min(cnt[0], e->cfg.max_svcs) - (uint32_t)std::max(nfree, 0);
-	out->tasks_in_use = std::min(cnt[1], e->cfg.max_tasks);
+	out->tasks_in_use = std::min(cnt[1], e->cfg.max_tasks) - (uint32_t)std::max(tfree, 0);
 	out->ngrows = e->ngrows;
 	out->device_bytes = e->dbytes;
 	return GYSK_OK;
@@ -1376,7 +1410,7 @@ int gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *
 		c = *cfg;
 	}
 	if (c.hll_p < 4 || c.hll_p > 16) return GYSK_ERR_INVAL;
-	slot_bytes(c.hll_p, svc_slot_bytes, task_slot_bytes);
+	slot_bytes(c.hll_p, c.task_idle_evict_secs != 0, svc_slot_bytes, task_slot_bytes);
 	return GYSK_OK;
 }
 
@@ -1396,13 +1430,18 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->kernel_launches += launch_rebuild_table(e->st.svc_tbl, e->cfg.max_svcs, e->stream);
 		e->tombstones = 0; e->insert_fail_seen = e->h_evict_fail;
 	}
+	if (e->task_tombstones > ((uint64_t)e->st.task_tbl.mask + 1) / 8) {		// the same for the process table
+		e->kernel_launches += launch_rebuild_table(e->st.task_tbl, e->cfg.max_tasks, e->stream);
+		e->task_tombstones = 0;
+	}
 	e->kernel_launches += launch_flush(e->st, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
-	e->kernel_launches += launch_task_flush(e->st, e->cfg.max_tasks, e->stream);
+	e->kernel_launches += launch_task_flush(e->st, e->cfg.max_tasks, tsec, e->cfg.task_idle_evict_secs, e->d_tevict, e->stream);
 	if (e->grow_limit_svcs > e->cfg.max_svcs || e->grow_limit_tasks > e->cfg.max_tasks) {
 		// auto-grow: the slot counts travel to the host behind the kernels, for the next flush's decision
 		CU(e, cudaMemcpyAsync(e->h_used, e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
 		CU(e, cudaMemcpyAsync(e->h_used + 1, e->st.svc_tbl.free_n, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
 		CU(e, cudaMemcpyAsync(e->h_used + 2, e->st.task_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+		if (e->st.task_tbl.free_n) CU(e, cudaMemcpyAsync(e->h_used + 3, e->st.task_tbl.free_n, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
 		CU(e, cudaEventRecord(e->ev_used, e->stream));
 		e->used_pending = true;
 	}
@@ -1411,6 +1450,8 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		CU(e, cudaMemcpyAsync(e->h_evict, e->st.counters + CTR_NEVICT, sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
 		CU(e, cudaMemcpyAsync(e->h_evict + e->cfg.max_svcs + 1, e->st.counters + CTR_INSERT_FAIL, sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
 		CU(e, cudaMemcpyAsync(e->h_evict + 1, e->st.evict_ids, (size_t)e->cfg.max_svcs * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
+	}
+	if (e->cfg.idle_evict_secs || e->cfg.task_idle_evict_secs) {		// the process list is written to h_tevict by its eviction kernel
 		CU(e, cudaEventRecord(e->ev_evict, e->stream));
 		e->evict_pending = true;
 	}
@@ -1428,6 +1469,27 @@ int gysk_evicted_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n)
 	if (int rc = collect_evicted(e)) return rc;
 	*n = (uint32_t)e->evicted_ids.size();
 	for (uint32_t i = 0; i < *n && i < cap; ++i) out[i] = e->evicted_ids[i];
+	return GYSK_OK;
+}
+
+int gysk_evicted_task_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!n || (!out && cap)) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Drain);
+	if (int rc = collect_evicted(e)) return rc;
+	*n = (uint32_t)e->evicted_task_ids.size();
+	for (uint32_t i = 0; i < *n && i < cap; ++i) out[i] = e->evicted_task_ids[i];
+	return GYSK_OK;
+}
+
+int gysk_task_evict_count(gysk_engine *e, uint64_t *total)
+{
+	CHECK_ENGINE(e);
+	if (!total) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Drain);
+	if (int rc = collect_evicted(e)) return rc;
+	*total = e->task_evicted_total;
 	return GYSK_OK;
 }
 

@@ -268,7 +268,8 @@ struct gysk_engine
 	std::vector<void *>	hallocs;
 
 	// capacity growth (gysk_grow, gysk_set_auto_grow): the auto-grow ceilings (0 = never), and the slot counts as of the last flush,
-	// copied behind its kernels and read at the next one ({services handed out, services on the free stack, processes handed out})
+	// copied behind its kernels and read at the next one ({services handed out, services on the free stack, processes handed out,
+	// processes on the free stack})
 	uint32_t		grow_limit_svcs {0}, grow_limit_tasks {0};
 	uint32_t		ngrows {0};
 	uint32_t		*h_used {nullptr};
@@ -313,6 +314,11 @@ struct gysk_engine
 	uint64_t		tombstones {0}, evicted_total {0};
 	uint64_t		h_evict_fail {0};			// CTR_INSERT_FAIL as of the last collected flush
 	uint64_t		insert_fail_seen {0};			// CTR_INSERT_FAIL at the last table rebuild
+	// process eviction (task_idle_evict_secs): the eviction kernel writes the count and ids of each flush straight into h_tevict (page-
+	// locked and mapped, d_tevict on the device: [0] = count, [1 .. max_tasks] = ids); collected with the services' list, under ev_evict
+	unsigned long long	*h_tevict {nullptr}, *d_tevict {nullptr};
+	std::vector<uint64_t>	evicted_task_ids;			// of the last completed flush, ascending
+	uint64_t		task_tombstones {0}, task_evicted_total {0};
 	uint32_t		sort_epoch {0};				// radix passes launched so far (tags the look-back status words)
 
 	std::mutex		host_mtx;					// the per-host control-plane state below
@@ -425,10 +431,10 @@ void hfree(gysk_engine *e, T *&p)
 }
 
 template <typename T>
-int halloc(gysk_engine *e, T **p, size_t n)
+int halloc(gysk_engine *e, T **p, size_t n, unsigned flags = cudaHostAllocDefault)
 {
 	void *q = nullptr;
-	cudaError_t ce = cudaHostAlloc(&q, n * sizeof(T), cudaHostAllocDefault);
+	cudaError_t ce = cudaHostAlloc(&q, n * sizeof(T), flags);
 
 	if (ce != cudaSuccess) {
 		cudaGetLastError();

@@ -14,6 +14,7 @@
 //   flush_kernel         5-s window roll                                               common/gy_socket_stat.cc:3898
 //   state_kernel         listener state of the closed window (get_curr_state)          common/gy_socket_stat.cc:2020-2875
 //   evict_kernel         idle listeners leave, slots recycled                          common/gy_socket_stat.cc:3968-4037
+//                        idle aggregated processes too (task_idle_evict_secs)         server/gy_mconnhdlr.cc:16492-16541
 //   gather_* / query_* / topn_*   read side
 //   window_* / task_summary_kernel  window reads: every live id, summarised on the device (gysk_summary.cuh)
 #include "gysk_kernels.cuh"
@@ -89,22 +90,33 @@ __device__ __forceinline__ void slot_reset(const DevState &st, uint32_t slot, ui
 	for (uint32_t w = t; w < (uint32_t)TD_CAP; w += nt) st.td_cent[(size_t)slot * TD_CAP + w] = Centroid {0.0, 0ull};
 }
 
-// service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state, one CTA per slot (grid-stride): gysk_create
-// over every slot, gysk_grow over the new ones
+// The just-created state of one process slot, written by threads t = 0 .. nt - 1 together: three empty histograms, an empty last window,
+// no id. What a slot holds before its first id, and again once its id is evicted. The eviction list and the free stack are not per-slot
+// state.
+__device__ __forceinline__ void task_slot_reset(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt)
+{
+	for (uint32_t c = t; c < 3u * HIST_CELLS; c += nt)
+		st.task_hist[(size_t)slot * 3 * HIST_CELLS + c] = HistCell {0, c % HIST_CELLS == HIST_MAX_CELL ? LLONG_MIN : 0};
+	for (uint32_t h = t; h < 3u; h += nt) { st.task_prev[(size_t)slot * 3 + h] = HistCell {0, 0}; st.task_last[(size_t)slot * 3 + h] = HistCell {0, 0}; }
+	if (t == 0) {
+		st.task_slot_id[slot] = 0; st.task_slot_host[slot] = 0;
+		if (st.task_last_active) st.task_last_active[slot] = 0;
+	}
+}
+
+// the slot-reset functions evict_kernel takes
+struct SvcSlotReset { __device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const { slot_reset(st, slot, t, nt); } };
+struct TaskSlotReset { __device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const { task_slot_reset(st, slot, t, nt); } };
+
+// service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state: one CTA per service slot, one thread per
+// process slot (grid-stride): gysk_create over every slot, gysk_grow over the new ones
 __global__ void __launch_bounds__(256) init_slots_kernel(DevState st, uint32_t s_lo, uint32_t s_hi, uint32_t t_lo, uint32_t t_hi)
 {
 	for (uint32_t s = s_lo + blockIdx.x; s < s_hi; s += gridDim.x) {
 		slot_reset(st, s, threadIdx.x, blockDim.x);
 		if (threadIdx.x == 0) st.slot_batch[s] = SlotBatch {0xFFFFFFFFu, 0u, 0u, 0u};
 	}
-	for (uint32_t i = t_lo + blockIdx.x * blockDim.x + threadIdx.x; i < t_hi; i += gridDim.x * blockDim.x) {
-		for (int h = 0; h < 3; ++h) {
-			HistCell *c = st.task_hist + ((size_t)i * 3 + h) * HIST_CELLS;
-			for (int b = 0; b < HIST_CELLS; ++b) c[b] = HistCell {0, b == HIST_MAX_CELL ? LLONG_MIN : 0};
-			st.task_prev[(size_t)i * 3 + h] = HistCell {0, 0}; st.task_last[(size_t)i * 3 + h] = HistCell {0, 0};
-		}
-		st.task_slot_id[i] = 0; st.task_slot_host[i] = 0;
-	}
+	for (uint32_t i = t_lo + blockIdx.x * blockDim.x + threadIdx.x; i < t_hi; i += gridDim.x * blockDim.x) task_slot_reset(st, i, 0, 1);
 }
 
 __global__ void register_kernel(DevState st, const unsigned long long *ids, uint32_t n, int is_task)
@@ -1585,28 +1597,33 @@ __global__ void __launch_bounds__(DAY_WARPS * 32) day_stats_kernel(DevState st, 
 	out[q] = r;
 }
 
-// one CTA per evicted slot (grid-stride): the id's table entry becomes a tombstone, every per-slot array returns to its
-// just-created state and the slot number goes on the free stack for the next unknown id
-__global__ void __launch_bounds__(256) evict_kernel(DevState st)
+// one CTA per evicted slot (grid-stride) of the list {slots, ids} of *nev entries: the id's entry of table t becomes a tombstone, the
+// slot returns to its just-created state (reset) and its number goes on t's free stack for the next unknown id. Services and processes
+// alike; host_ids (optional, page-locked and mapped) receives the count and the ids.
+template <typename Reset>
+__global__ void __launch_bounds__(256) evict_kernel(DevState st, IdTable t, const uint32_t *__restrict__ slots, const unsigned long long *__restrict__ ids,
+		const unsigned long long *nev_p, unsigned long long *total, unsigned long long *host_ids, Reset reset)
 {
-	const uint32_t nev = (uint32_t)st.counters[CTR_NEVICT];
+	const uint32_t nev = (uint32_t)*nev_p;
 
+	if (host_ids && blockIdx.x == 0 && threadIdx.x == 0) host_ids[0] = nev;
 	for (uint32_t q = blockIdx.x; q < nev; q += gridDim.x) {
-		const uint32_t slot = st.evict_list[q];
-		const unsigned long long id = st.evict_ids[q];
+		const uint32_t slot = slots[q];
+		const unsigned long long id = ids[q];
 
 		if (threadIdx.x == 0) {
-			uint32_t pos = table_hash(id) & st.svc_tbl.mask;
-			for (uint32_t probe = 0; probe <= st.svc_tbl.mask; ++probe, pos = (pos + 1) & st.svc_tbl.mask) {
-				TblEntry *e = &st.svc_tbl.ent[pos];
+			uint32_t pos = table_hash(id) & t.mask;
+			for (uint32_t probe = 0; probe <= t.mask; ++probe, pos = (pos + 1) & t.mask) {
+				TblEntry *e = &t.ent[pos];
 				if (e->key == id) { e->key = KEY_TOMBSTONE; e->slot1 = 0; break; }
 				if (e->key == 0) break;
 			}
-			const int32_t f = atomicAdd(st.svc_tbl.free_n, 1);
-			st.svc_tbl.free_slots[f] = slot;
-			atomicAdd(st.counters + CTR_EVICTED_TOTAL, 1ull);
+			const int32_t f = atomicAdd(t.free_n, 1);
+			t.free_slots[f] = slot;
+			if (total) atomicAdd(total, 1ull);
+			if (host_ids) host_ids[1 + q] = id;
 		}
-		slot_reset(st, slot, threadIdx.x, blockDim.x);
+		reset(st, slot, threadIdx.x, blockDim.x);
 	}
 }
 
@@ -2199,8 +2216,12 @@ int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is
 	return picked < 0 ? picked : 1 + picked;
 }
 
-// per-task window of the three MTASK_HIST histograms: totals now minus totals at the previous flush (nothing on the ingest path)
-__global__ void task_flush_kernel(DevState st, uint32_t max_tasks)
+// per-task window of the three MTASK_HIST histograms: totals now minus totals at the previous flush (nothing on the ingest path).
+// With idle_secs, the process eviction (MCONN_HANDLER::cleanup_partha_unused_aggr_tasks, server/gy_mconnhdlr.cc:16492-16541: a MAGGR_TASK
+// whose last_tusec_ is older than 30 min goes): the thread of a live slot's first histogram stamps the slot with tsec when the window
+// it closes holds samples (every sample adds to all three histograms) or the slot has no stamp yet, and lists it when its stamp
+// + idle_secs < tsec.
+__global__ void task_flush_kernel(DevState st, uint32_t max_tasks, uint32_t tsec, uint32_t idle_secs)
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;		// (task, histogram)
 	if (i >= max_tasks * 3u) return;
@@ -2208,14 +2229,29 @@ __global__ void task_flush_kernel(DevState st, uint32_t max_tasks)
 	HistCell tot {0, 0};
 	for (int b = 0; b < HIST_MAX_CELL; ++b) { tot.count += h[b].count; tot.sum += h[b].sum; }
 	const HistCell prev = st.task_prev[i];
-	st.task_last[i] = HistCell {tot.count - prev.count, tot.sum - prev.sum};
+	const HistCell last {tot.count - prev.count, tot.sum - prev.sum};
+	st.task_last[i] = last;
 	st.task_prev[i] = tot;
+
+	const uint32_t slot = i / 3u;
+	if (!idle_secs || i % 3u || !st.task_slot_id[slot]) return;
+	uint32_t t = st.task_last_active[slot];
+	if (last.count || !t) { t = tsec ? tsec : 1u; st.task_last_active[slot] = t; }
+	if ((uint64_t)t + idle_secs < tsec) {
+		const unsigned long long k = atomicAdd(st.counters + CTR_TASK_NEVICT, 1ull);
+		st.task_evict_list[k] = slot;
+		st.task_evict_ids[k] = st.task_slot_id[slot];
+	}
 }
 
-int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s)
+int launch_task_flush(const DevState &st, uint32_t max_tasks, uint32_t tsec, uint32_t idle_secs, unsigned long long *host_ids, cudaStream_t s)
 {
-	task_flush_kernel<<<div_up((uint64_t)max_tasks * 3, 256), 256, 0, s>>>(st, max_tasks);
-	return 1;
+	if (idle_secs) cudaMemsetAsync(st.counters + CTR_TASK_NEVICT, 0, sizeof(unsigned long long), s);
+	task_flush_kernel<<<div_up((uint64_t)max_tasks * 3, 256), 256, 0, s>>>(st, max_tasks, tsec, idle_secs);
+	if (!idle_secs) return 1;
+	evict_kernel<<<296, 256, 0, s>>>(st, st.task_tbl, st.task_evict_list, st.task_evict_ids, st.counters + CTR_TASK_NEVICT, nullptr, host_ids,
+			TaskSlotReset {});
+	return 2;
 }
 
 int launch_flush(const DevState &st, uint32_t nslots, uint32_t tsec, uint32_t idle_secs, cudaStream_t s)
@@ -2225,7 +2261,8 @@ int launch_flush(const DevState &st, uint32_t nslots, uint32_t tsec, uint32_t id
 	flush_kernel<<<div_up((uint64_t)nslots * HIST_CELLS, 256), 256, 0, s>>>(st, nslots, tsec, idle_secs);
 	state_kernel<<<div_up(nslots, 128), 128, 0, s>>>(st, nslots, tsec);
 	if (!idle_secs) return 2;
-	evict_kernel<<<296, 256, 0, s>>>(st);		// grid-stride over the (device-side) eviction list
+	evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL, nullptr,
+			SvcSlotReset {});		// grid-stride over the (device-side) eviction list
 	return 3;
 }
 

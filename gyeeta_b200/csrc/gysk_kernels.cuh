@@ -76,6 +76,11 @@ struct DevState
 	HistCell		*task_prev, *task_last;			// [max_tasks][3] {count, sum}: totals at the last flush / of the last closed window
 	unsigned long long	*task_slot_id;				// [max_tasks] slot -> aggr_task_id
 	uint32_t		*task_slot_host;
+	// process eviction (task_idle_evict_secs; nullptr without): tsec of the last flush whose closed window held samples of the slot
+	// (of the first flush that saw it until then), and the slots evicted by the last flush with their ids
+	uint32_t		*task_last_active;			// [max_tasks]
+	uint32_t		*task_evict_list;			// [max_tasks]
+	unsigned long long	*task_evict_ids;			// [max_tasks]
 	// flow sketch
 	unsigned long long	*cms_cur, *cms_last;			// [depth][1 << log2w]
 	unsigned long long	*cms_ring, *cms_5min;			// GYSK_FLAG_FLOW_LEVEL (nullptr without): [NSLOTS][depth][1 << log2w] level-0
@@ -188,7 +193,9 @@ int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is
 // entry's index (0 past the keys); -1: sort failed
 int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_t nkeys, const unsigned long long *ids, const uint32_t *hosts,
 		uint32_t want, gysk_topn_entry *d_out, cudaStream_t s, unsigned long long *d_slots = nullptr);
-int launch_task_flush(const DevState &st, uint32_t max_tasks, cudaStream_t s);
+// the closed window of every process slot; with idle_secs the process eviction too: the evicted ids go to host_ids (page-locked,
+// mapped: [0] = count, [1..] = ids in eviction-list order)
+int launch_task_flush(const DevState &st, uint32_t max_tasks, uint32_t tsec, uint32_t idle_secs, unsigned long long *host_ids, cudaStream_t s);
 // the window roll into ring slot st.levels.cur of each level (cleared by the host when it starts a new epoch), the listener states,
 // the idle-service eviction
 int launch_flush(const DevState &st, uint32_t max_svcs, uint32_t tsec, uint32_t idle_secs, cudaStream_t s);

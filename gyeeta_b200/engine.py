@@ -47,7 +47,8 @@ class Config(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("device", C.c_int32), ("max_svcs", C.c_uint32), ("max_tasks", C.c_uint32),
                 ("cms_depth", C.c_uint32), ("cms_log2_width", C.c_uint32), ("hll_p", C.c_uint32),
                 ("td_compression", C.c_uint32), ("max_batch", C.c_uint32), ("flags", C.c_uint32), ("rank", C.c_uint32),
-                ("world", C.c_uint32), ("stage_batch", C.c_uint32), ("idle_evict_secs", C.c_uint32), ("reserved", C.c_uint32 * 2)]
+                ("world", C.c_uint32), ("stage_batch", C.c_uint32), ("idle_evict_secs", C.c_uint32),
+                ("task_idle_evict_secs", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class SvcSummary(C.Structure):
@@ -181,12 +182,14 @@ class Capacity(C.Structure):
 assert C.sizeof(Capacity) == 32
 
 
-def slot_bytes(hll_p=12):
-    """gysk_slot_bytes (no device needed): (device bytes of one service slot, of one process slot) at this hll_p"""
+def slot_bytes(hll_p=12, task_idle_evict_secs=0):
+    """gysk_slot_bytes (no device needed): (device bytes of one service slot, of one process slot) at this hll_p, with or without
+    process eviction"""
     L = load_library()
     cfg = Config()
     L.gysk_config_default(C.byref(cfg))
     cfg.hll_p = hll_p
+    cfg.task_idle_evict_secs = task_idle_evict_secs
     s, t = C.c_uint64(), C.c_uint64()
     rc = L.gysk_slot_bytes(C.byref(cfg), C.byref(s), C.byref(t))
     if rc:
@@ -230,6 +233,8 @@ def load_library(path=None):
         "gysk_sync": (i32, [vp]),
         "gysk_flush": (i32, [vp, u32]),
         "gysk_evicted_ids": (i32, [vp, vp, u32, vp]),
+        "gysk_evicted_task_ids": (i32, [vp, vp, u32, vp]),
+        "gysk_task_evict_count": (i32, [vp, vp]),
         "gysk_query_svcs": (i32, [vp, vp, u32, vp]),
         "gysk_query_flows": (i32, [vp, vp, u32, i32, vp]),
         "gysk_query_window": (i32, [vp, C.c_int32, u32, vp, u32, vp]),
@@ -316,7 +321,7 @@ class Engine:
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
-                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False):
+                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -325,6 +330,7 @@ class Engine:
         cfg.max_batch = max_batch
         cfg.stage_batch = stage_batch
         cfg.idle_evict_secs = idle_evict_secs
+        cfg.task_idle_evict_secs = task_idle_evict_secs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0)
@@ -397,6 +403,19 @@ class Engine:
         n = C.c_uint32()
         self._chk(self.L.gysk_evicted_ids(self.h, _p(out), cap, C.byref(n)))
         return out[:min(n.value, cap)].copy()
+
+    def evicted_task_ids(self, cap=1 << 16):
+        """aggregated-process ids evicted by the most recent flush (task_idle_evict_secs), ascending"""
+        out = np.zeros(cap, dtype=np.uint64)
+        n = C.c_uint32()
+        self._chk(self.L.gysk_evicted_task_ids(self.h, _p(out), cap, C.byref(n)))
+        return out[:min(n.value, cap)].copy()
+
+    def task_evict_count(self):
+        """aggregated processes evicted so far"""
+        t = C.c_uint64()
+        self._chk(self.L.gysk_task_evict_count(self.h, C.byref(t)))
+        return t.value
 
     def stream(self):
         return self.L.gysk_stream(self.h)

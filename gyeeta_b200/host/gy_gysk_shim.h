@@ -133,6 +133,34 @@ public :
 		return true;
 	}
 
+	// The same, plus what MCONN_HANDLER::cleanup_partha_unused_aggr_tasks does with an aggregated process idle for 30 minutes
+	// (server/gy_mconnhdlr.cc:16492-16541, a PING_TASK_AGGR with keep_task_ = false): with gysk_config.task_idle_evict_secs set, the
+	// process ids the engine evicted at this flush are handed to `on_task_delete(aggr_task_id)` — the place to drop the MAGGR_TASK of
+	// that id from the partha's task_aggr_tbl_ and its row from the aggregated-task table of the database.
+	template <typename OnDelete, typename OnTaskDelete>
+	bool flush_window(uint32_t tsec, OnDelete && on_delete, OnTaskDelete && on_task_delete) noexcept
+	{
+		if (!flush_window(tsec, on_delete)) return false;
+		try {
+			uint32_t n = 0;
+			if (0 != gysk_evicted_task_ids(engine_, evicted_.data(), (uint32_t)evicted_.size(), &n)) return false;
+			if (n > evicted_.size()) {
+				evicted_.resize(n);
+				if (0 != gysk_evicted_task_ids(engine_, evicted_.data(), (uint32_t)evicted_.size(), &n)) return false;
+			}
+			for (uint32_t i = 0; i < n && i < evicted_.size(); ++i) on_task_delete(evicted_[i]);
+		}
+		catch (...) { return false; }
+		return true;
+	}
+
+	// aggregated processes the engine has evicted so far (-1 on failure)
+	int64_t task_evict_count() noexcept
+	{
+		uint64_t t = 0;
+		return 0 == gysk_task_evict_count(engine_, &t) ? (int64_t)t : -1;
+	}
+
 	// Engine output in the reference's own record form: the LISTENER_STATE_NOTIFY batch of the given listeners (<= 512 per call,
 	// common/gy_comm_proto.h:2222), ready for the unchanged partha_listener_state / MTCP_LISTENER::set_state path.
 	// `out` must hold n * 88 bytes. Returns the number of records written, -1 on failure.

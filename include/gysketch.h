@@ -227,7 +227,11 @@ typedef struct gysk_config
 	uint32_t	idle_evict_secs;	/* a service without events for this long (and older than twice that) is evicted at
 						   gysk_flush: TIMEOUT_INET_DIAG_SECS 300, common/gy_socket_stat.h:997, rule of
 						   common/gy_socket_stat.cc:3968-3982. 0 (default) = never */
-	uint32_t	reserved[2];
+	uint32_t	task_idle_evict_secs;	/* an aggregated process whose last sample arrived in a window closed more than this many
+						   seconds before the tsec of a gysk_flush is evicted by that flush: the rule of
+						   MCONN_HANDLER::cleanup_partha_unused_aggr_tasks (server/gy_mconnhdlr.cc:16492-16541), whose
+						   value is 1800 (last_tusec_ older than 30 min). 0 (default) = never; "process eviction" below */
+	uint32_t	reserved;
 } gysk_config;
 
 typedef struct gysk_engine gysk_engine;
@@ -400,7 +404,7 @@ typedef struct gysk_capacity
 int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the ingest stream */
 
 /* host only, no device needed: the device bytes one service slot (its rolling-level rows included) and one process slot take in an
- * engine of this configuration (NULL: the defaults); they depend on hll_p only. An engine's footprint is about
+ * engine of this configuration (NULL: the defaults); they depend on hll_p and on whether task_idle_evict_secs is set. An engine's footprint is about
  * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
  * buffers and the count-min tables: 2 tables of cms_depth << cms_log2_width 8-byte cells, 11 more with GYSK_FLAG_FLOW_LEVEL (its 10 ring
  * slots and the level: 352 MiB more at the default 4 x 2^20). The count-min tables do not depend on capacity, so gysk_grow leaves them. */
@@ -426,6 +430,27 @@ int		gysk_flush(gysk_engine *e, uint32_t tsec);
 /* ids evicted by the most recent gysk_flush (the LISTEN_FLAG_DELETE notifications of common/gy_socket_stat.cc:4023-4033);
  * synchronises the ingest stream. *n = number of ids (may exceed cap: then only cap are written) */
 int		gysk_evicted_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n);
+
+/* ---- process eviction (gysk_config.task_idle_evict_secs != 0) ----
+ * Arrival is known to the window: a process's last-activity time is the tsec of the last gysk_flush whose closed window held one of its
+ * samples, or of the first flush that saw it when no flush has yet closed a window with its samples (a process registered by
+ * gysk_register_ids counts from that flush on, as a MAGGR_TASK's last_tusec_ counts from its creation). gysk_flush(tsec) evicts every
+ * process whose time t has t + task_idle_evict_secs < tsec (strict): the decision uses the window that flush closes, so samples that
+ * arrive in it keep the process. The rule applies to each process on its own, whatever its host. An evicted process's table entry
+ * becomes a tombstone, its slot gets the state of a never-used one and goes on the process table's free stack; the next unknown id takes
+ * it. So, from that flush on:
+ *  - gysk_query_tasks gives found = 0 for the id, gysk_export_task_hist GYSK_ERR_NOENT, gysk_query_task_window no row;
+ *  - gysk_topn_tasks never returns it, nor does gysk_topn_global_tasks as of the first merge after the flush;
+ *  - the same id seen again takes a slot with three empty histograms and an empty last window;
+ *  - gysk_capacity_info.tasks_in_use (and gysk_stats.ntasks) no longer count it, and auto-grow decides on that count;
+ *  - gysk_grow keeps the free stack.
+ * The per-host queues of gysk_topn_host are what the hosts sent and are not touched; gysk_task_groupby keeps no state and is not affected.
+ * The setting adds 20 bytes to each process slot (gysk_slot_bytes counts them only when it is set). */
+/* ids evicted by the most recent gysk_flush, in ascending id order: where madhava deletes the MAGGR_TASK of each and its row. The
+ * contract of gysk_evicted_ids: synchronises the ingest stream, *n = number of ids (may exceed cap: then only cap are written) */
+int		gysk_evicted_task_ids(gysk_engine *e, uint64_t *out, uint32_t cap, uint32_t *n);
+/* processes evicted so far */
+int		gysk_task_evict_count(gysk_engine *e, uint64_t *total);
 
 /* ---- queries ---- */
 int		gysk_query_svcs(gysk_engine *e, const uint64_t *glob_ids, uint32_t n, gysk_svc_summary *out);
