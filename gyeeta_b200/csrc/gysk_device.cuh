@@ -79,7 +79,8 @@ static constexpr unsigned long long KEY_TOMBSTONE = ~0ull;	// table entry of an 
 enum { CTR_IN = 0, CTR_DROPPED, CTR_RESP, CTR_TCP, CTR_TASK, CTR_FOREIGN, CTR_NKEYS, CTR_INSERT_FAIL, CTR_NTOUCHED /* short key segments */,
 	CTR_NLONG /* long key segments (batch rows) */, CTR_NEVICT, CTR_EVICTED_TOTAL,
 	CTR_NHOT /* hot rows in use by the batch in flight */, CTR_NHOT_NEXT /* rows handed out so far */, CTR_NWINDOW /* rows of the last window read (or logical read / logical top-N) */,
-	CTR_NHOSTS /* host rows of the last gysk_query_host_listen */, CTR_TASK_NEVICT /* processes evicted by the last flush */, CTR_MAX };
+	CTR_NHOSTS /* host rows of the last gysk_query_host_listen */, CTR_TASK_NEVICT /* processes evicted by the last flush */,
+	CTR_FLOW_DIRECT /* connection records of the last batch whose count-min update bypassed the flow table */, CTR_MAX };
 
 // ---------------------------------------------------------------------------------------------------
 // jhash: Bob Jenkins lookup2 in the form the reference uses (common/jhash.h:22-35,121-134); seed 0xceedfead
@@ -274,6 +275,14 @@ __device__ __forceinline__ uint32_t ld_na_hint_u32(const uint32_t *p, unsigned l
 {
 	uint32_t v;
 	asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+	return v;
+}
+
+// 64-bit load from L2 (not cached in L1) that allocates with the policy's priority
+__device__ __forceinline__ unsigned long long ld_cg_hint_u64(const unsigned long long *p, unsigned long long pol)
+{
+	unsigned long long v;
+	asm volatile("ld.global.cg.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol));
 	return v;
 }
 

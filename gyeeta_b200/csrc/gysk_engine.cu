@@ -622,6 +622,10 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		tmp.rec_cnt_cap = nsm * IngestShape::WARPS * IngestShape::MIN_CTAS;
 		tmp.recq_cap = (uint64_t)cfg.max_batch + (uint64_t)tmp.rec_cnt_cap * IngestShape::CHUNK;
 		A(dalloc(e, &tmp.recq, (size_t)tmp.recq_cap, false)); A(dalloc(e, &tmp.rec_cnt, (size_t)tmp.rec_cnt_cap, false));
+		// the batch's flow table (FlowTable): zero here, and the TASK drain pass leaves it so after every batch. Not per slot: outside
+		// each_slot_array, so gysk_grow leaves it
+		tmp.flow_cap = std::min<uint32_t>(FLOW_ENT_MAX, pow2_at_least(2ull * cfg.max_batch));
+		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
 
@@ -728,6 +732,26 @@ int64_t gysk_last_batch_keys(gysk_engine *e)
 	unsigned long long n = 0;
 	CU(e, cudaMemcpy(&n, e->st.counters + CTR_NKEYS, sizeof(n), cudaMemcpyDeviceToHost));
 	return (int64_t)n;
+}
+
+// diagnostic: connection records of the last device batch whose count-min update bypassed the flow table
+int64_t gysk_last_batch_flow_direct(gysk_engine *e)
+{
+	CHECK_ENGINE(e);
+	GYSK_ENTER(e, Sync);
+	unsigned long long n = 0;
+	CU(e, cudaMemcpy(&n, e->st.counters + CTR_FLOW_DIRECT, sizeof(n), cudaMemcpyDeviceToHost));
+	return (int64_t)n;
+}
+
+// diagnostic: entries of the flow table that are not zero (a key or a sum left behind); 0 whenever no batch is in flight
+int64_t gysk_flow_table_used(gysk_engine *e)
+{
+	CHECK_ENGINE(e);
+	GYSK_ENTER(e, Sync);
+	std::vector<FlowEnt> t(e->tmp.flow_cap);
+	CU(e, cudaMemcpy(t.data(), e->tmp.flow, t.size() * sizeof(FlowEnt), cudaMemcpyDeviceToHost));
+	return (int64_t)std::count_if(t.begin(), t.end(), [](const FlowEnt &f) { return f.key || f.inc; });
 }
 
 int gysk_register_ids(gysk_engine *e, const uint64_t *ids, uint32_t n, int is_task)

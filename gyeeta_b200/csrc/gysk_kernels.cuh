@@ -103,6 +103,15 @@ __device__ __forceinline__ bool svc_issue(const DevState &st, uint32_t slot, uin
 	return svc_evaluated(st, slot, active_mark) && (st.slot_state[slot].issue_bits & 1u);
 }
 
+// Flow table of one batch: the TCP pass sums each flow's count-min increments {count 1 | kbytes << 32} in an entry keyed by its two
+// hashes, key = h2 << 32 | h1 (0 = empty), and the TASK pass adds every entry to the flow's cells once and empties the table. u64
+// addition is associative, so every cell ends as it would with one RED per record. mask + 1 entries, a power of two.
+struct alignas(16) FlowEnt { unsigned long long key, inc; };
+struct FlowTable { FlowEnt *ent; uint32_t mask; };
+static constexpr uint32_t FLOW_PROBES = 16;		// linear probe limit; past it a record updates the count-min cells directly
+static constexpr uint32_t FLOW_ENT_MAX = 1u << 21;	// 32 MB; a batch takes the smallest power of two >= 2 x its events, up to this
+static constexpr uint32_t FLOW_SWEEP = 4;		// entries per thread and step of the TASK pass's sweep
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
@@ -125,6 +134,8 @@ struct SortTemp
 	uint2			*rec_cnt;		// [rec_cnt_cap] {connection, process} records of each region, written by every warp of the launch
 	uint64_t		recq_cap;		// max_batch + the regions' rounding (one chunk per warp of a full ingest grid)
 	uint32_t		rec_cnt_cap;		// warps of a full ingest grid
+	FlowEnt			*flow;			// [flow_cap] the flow table (FlowTable): zero between batches
+	uint32_t		flow_cap;		// min(FLOW_ENT_MAX, smallest power of two >= 2 x max_batch)
 	uint32_t		max_tiles;
 };
 

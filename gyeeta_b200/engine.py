@@ -224,6 +224,8 @@ def load_library(path=None):
         "gysk_get_stats": (i32, [vp, vp]),
         "gysk_hot_rows_in_use": (C.c_int64, [vp]),
         "gysk_last_batch_keys": (C.c_int64, [vp]),
+        "gysk_last_batch_flow_direct": (C.c_int64, [vp]),
+        "gysk_flow_table_used": (C.c_int64, [vp]),
         "gysk_register_ids": (i32, [vp, vp, u32, i32]),
         "gysk_ingest": (i32, [vp, vp, u32, u32, vp, u32, vp]),
         "gysk_ingest_msg": (i32, [vp, vp, u32, vp, u32]),
@@ -465,6 +467,20 @@ class Engine:
     def last_batch_keys(self):
         """response samples of the last device batch that travelled as sort keys (diagnostic)"""
         n = self.L.gysk_last_batch_keys(self.h)
+        if n < 0:
+            self._chk(int(n))
+        return int(n)
+
+    def last_batch_flow_direct(self):
+        """connection records of the last device batch whose count-min update bypassed the flow table (diagnostic)"""
+        n = self.L.gysk_last_batch_flow_direct(self.h)
+        if n < 0:
+            self._chk(int(n))
+        return int(n)
+
+    def flow_table_used(self):
+        """non-zero entries of the batch flow table: 0 whenever no batch is in flight (diagnostic)"""
+        n = self.L.gysk_flow_table_used(self.h)
         if n < 0:
             self._chk(int(n))
         return int(n)

@@ -373,6 +373,12 @@ int64_t		gysk_hot_rows_in_use(gysk_engine *e);
 uint32_t	gysk_hot_row_word(uint32_t bin);
 /* diagnostic: response samples of the last device batch that travelled as sort keys (the rest updated hot rows). Negative = GYSK_ERR_*. */
 int64_t		gysk_last_batch_keys(gysk_engine *e);
+/* diagnostic: connection records of the last device batch whose count-min update did not go through the batch's flow table (its probe
+ * limit reached: more flows than the table holds). Routing only, as above. Negative = GYSK_ERR_*. */
+int64_t		gysk_last_batch_flow_direct(gysk_engine *e);
+/* diagnostic: entries of the batch flow table left non-zero; 0 whenever no batch is in flight. Copies the table (up to 32 MB) to the
+ * host. Negative = GYSK_ERR_*. */
+int64_t		gysk_flow_table_used(gysk_engine *e);
 
 /* ---- capacity: growing the service / process tables of a live engine ---- */
 /* Raise the service / process capacity of a live engine (either may equal the current value; neither may shrink, both <= 1 << 24).
