@@ -47,6 +47,9 @@ namespace {
 
 uint32_t pow2_at_least(uint64_t v) { uint32_t p = 16; while (p < v) p <<= 1; return p; }
 
+// the values the slot field of a batch's sort keys takes: the service slots, and with trace rows the null slot and one pseudo-slot per row
+uint32_t key_slots(const gysk_engine *e) { return e->cfg.max_svcs + (e->st.trace.rows ? 1u + e->st.trace.rows : 0u); }
+
 // one device batch: ingest kernel, the TCP and TASK drain passes over the records it queued, then the sort + t-digest chain over
 // the keys it emitted. `consumed` (optional) is recorded once the ingest kernel has read the events: the event buffer may be refilled
 // from there on, so that the next H2D copy overlaps the drain and merge kernels.
@@ -68,14 +71,14 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	RecRegions rr;
-	const int li = launch_ingest(e->st, e->tmp, d_ev, n, e->cfg.max_svcs, rr, e->stream);
+	const int li = launch_ingest(e->st, e->tmp, d_ev, n, key_slots(e), rr, e->stream);
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
 	e->kernel_launches += launch_drains(e->st, e->tmp, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
-	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, e->cfg.max_svcs, e->stream);
+	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[2], e->stream));
 	e->batches++;
 	return post_launch(e, "ingest batch");
@@ -378,8 +381,9 @@ int roll_levels(gysk_engine *e, uint32_t tsec)
 // Every device array indexed by service or process slot, with its elements per slot: f(pointer, elements per slot, kind). Svc arrays
 // hold max_svcs + 1 slots (slot max_svcs is the null slot), the level ring max_svcs rows in each of its NLEVELS x NSLOTS planes
 // (LevelRing::stride), Task arrays max_tasks slots. gysk_create allocates exactly these, gysk_grow moves them, slot_bytes sums them.
-// The process eviction's arrays exist only with task_idle_evict_secs (task_evict).
-enum class SlotKind { Svc, Ring, Task };
+// The process eviction's arrays exist only with task_idle_evict_secs (task_evict). The batch's segment arrays (Seg) are indexed by the
+// slot field of the sort keys: max_svcs + 1 entries, and one more per trace row (max_trace_svcs) beyond the null slot.
+enum class SlotKind { Svc, Ring, Task, Seg };
 
 template <typename F>
 void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, bool task_evict, F f)
@@ -395,7 +399,7 @@ void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, bool task_evic
 	f(st.td_cent, TD_CAP, SlotKind::Svc); f(st.td_head, 1, SlotKind::Svc);
 	f(st.slot_batch, 1, SlotKind::Svc); f(st.slot_aux, 1, SlotKind::Svc);
 	f(st.qps_hist, HIST_CELLS, SlotKind::Svc); f(st.act_hist, HIST_CELLS, SlotKind::Svc); f(st.slot_state, 1, SlotKind::Svc);
-	f(tmp.touched, 1, SlotKind::Svc); f(tmp.segs, 1, SlotKind::Svc);
+	f(tmp.touched, 1, SlotKind::Seg); f(tmp.segs, 1, SlotKind::Seg);
 	f(st.task_hist, 3 * HIST_CELLS, SlotKind::Task); f(st.task_prev, 3, SlotKind::Task); f(st.task_last, 3, SlotKind::Task);
 	f(st.task_slot_id, 1, SlotKind::Task); f(st.task_slot_host, 1, SlotKind::Task);
 	if (task_evict) {
@@ -409,23 +413,29 @@ void slot_bytes(uint32_t hll_p, bool task_evict, uint64_t *svc, uint64_t *task)
 {
 	DevState st {};
 	SortTemp tmp {};
-	uint64_t b[3] = {0, 0, 0};
+	uint64_t b[4] = {0, 0, 0, 0};
 	each_slot_array(st, tmp, hll_p, task_evict, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
-	*svc = b[(int)SlotKind::Svc] + b[(int)SlotKind::Ring];
+	*svc = b[(int)SlotKind::Svc] + b[(int)SlotKind::Ring] + b[(int)SlotKind::Seg];
 	*task = b[(int)SlotKind::Task];
 }
 
-size_t slots_of(SlotKind kind, uint32_t max_svcs, uint32_t max_tasks)
+size_t slots_of(SlotKind kind, uint32_t max_svcs, uint32_t max_tasks, uint32_t max_trace)
 {
-	return kind == SlotKind::Svc ? (size_t)max_svcs + 1 : kind == SlotKind::Ring ? (size_t)max_svcs : (size_t)max_tasks;
+	return kind == SlotKind::Svc ? (size_t)max_svcs + 1 : kind == SlotKind::Ring ? (size_t)max_svcs :
+			kind == SlotKind::Seg ? (size_t)max_svcs + 1 + max_trace : (size_t)max_tasks;
 }
 
 // the arrays sized by capacity beside the per-slot ones: an id table's entries, the sort buffers' keys and look-back tiles, the batch
 // rows of the long key segments
 uint32_t table_cap(uint32_t slots) { return pow2_at_least((uint64_t)slots * 2); }
-size_t sort_keys(const gysk_config &cfg) { return std::max<size_t>(std::max<size_t>((size_t)cfg.max_svcs + 1, cfg.max_tasks) + 1, cfg.max_batch); }
+size_t sort_keys(const gysk_config &cfg)
+{
+	return std::max<size_t>(std::max<size_t>(std::max<size_t>((size_t)cfg.max_svcs + 1, cfg.max_tasks) + 1, cfg.max_batch), (size_t)cfg.max_trace_svcs + 1);
+}
 uint32_t sort_tiles(size_t nkeys) { return (uint32_t)((nkeys + SORT_TILE - 1) / SORT_TILE); }
-size_t batch_rows(const gysk_config &cfg) { return std::min<size_t>((size_t)cfg.max_svcs + 1, ((size_t)cfg.max_batch + LONG_SEG - 1) / LONG_SEG); }
+size_t batch_rows(const gysk_config &cfg) { return std::min<size_t>((size_t)cfg.max_svcs + 1 + cfg.max_trace_svcs, ((size_t)cfg.max_batch + LONG_SEG - 1) / LONG_SEG); }
+// trace rows fit the 24-bit slot field of the sort keys as pseudo-slots max_svcs + 1 .. max_svcs + max_trace_svcs
+bool trace_fits(uint32_t max_svcs, uint32_t max_trace) { return !max_trace || (uint64_t)max_svcs + 1 + max_trace <= (1ull << 24); }
 
 SvcRows finish_rows(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
 CopyRows<gysk_task_summary> finish_rows(const gysk_engine *, gysk_task_summary *out) { return CopyRows<gysk_task_summary> {out}; }
@@ -515,7 +525,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	if (cfg.max_svcs < 1 || cfg.max_svcs > (1u << 24) || cfg.max_tasks < 1 || cfg.max_tasks > (1u << 24) || cfg.cms_depth < 1 ||
 			cfg.cms_depth > 8 || cfg.cms_log2_width < 4 || cfg.cms_log2_width > 28 || cfg.hll_p < 4 || cfg.hll_p > 16 ||
 			cfg.td_compression < 10 || cfg.td_compression > (uint32_t)TD_CAP || cfg.max_batch < 1024 || cfg.max_batch >= (1u << 27) ||
-			cfg.rank >= cfg.world)
+			cfg.rank >= cfg.world || !trace_fits(cfg.max_svcs, cfg.max_trace_svcs))
 		return fail(nullptr, GYSK_ERR_INVAL, "gysk_config out of range");
 
 	int ndev = 0;
@@ -555,7 +565,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &st.task_tbl.count, 1));
 	if (cfg.task_idle_evict_secs) A(dalloc(e, &st.task_tbl.free_n, 1));		// without it the process table has no free stack
 	SortTemp &tmp = e->tmp;
-	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) { if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks) * k); });
+	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) { if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs) * k); });
 	if (rc) return bail(rc);
 	st.levels.stride = cfg.max_svcs;
 	st.svc_tbl.slot_id = st.slot_id; st.svc_tbl.slot_host = st.slot_host;
@@ -628,6 +638,22 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
+	if (cfg.max_trace_svcs) {
+		// trace rows (TraceTable): not per service slot but per row, so gysk_slot_bytes leaves them out and device_bytes counts them; only
+		// the slot -> row map grows with the service table
+		TraceTable &tr = st.trace;
+		const size_t nr = cfg.max_trace_svcs;
+		tr.rows = cfg.max_trace_svcs; tr.par = 0; tr.base = cfg.max_svcs + 1;
+		A(dalloc(e, &tr.row_of, ns)); A(dalloc(e, &tr.row_slot, nr, false)); A(dalloc(e, &tr.free_rows, nr, false));
+		A(dalloc(e, &tr.cnt, 2 * nr * TRACE_WORDS)); A(dalloc(e, &tr.head, 2 * nr)); A(dalloc(e, &tr.cent, 2 * nr * TRACE_TD_CAP));
+		A(dalloc(e, &tr.count, 1)); A(dalloc(e, &tr.free_n, 1)); A(dalloc(e, &tr.dropped, 1));
+		if ((ce = cudaMemsetAsync(tr.row_slot, 0xFF, nr * sizeof(uint32_t), e->stream)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "trace rows", ce); return bail(GYSK_ERR_CUDA); }
+		const std::vector<double> qtab = k1_grid(TRACE_TD_DELTA);
+		double *d_q = nullptr;
+		A(dalloc(e, &d_q, qtab.size(), false));
+		if ((ce = cudaMemcpy(d_q, qtab.data(), qtab.size() * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "trace qtab", ce); return bail(GYSK_ERR_CUDA); }
+		tr.td.qtab = d_q; tr.td.delta = TRACE_TD_DELTA; tr.td.pad = 0;
+	}
 
 	for (int k = 0; k < NBUF; ++k) {
 		A(dalloc(e, &e->d_events[k], (size_t)cfg.stage_batch, false));
@@ -970,6 +996,18 @@ inline bool decode_wire(const ApiTran &r, uint32_t host_idx, gysk_event &o)
 	o.flags = err == 0 ? 0 : (err >= 500 ? GYSK_EVF_SER_ERROR : GYSK_EVF_CLI_ERROR);
 	return true;
 }
+// the record's GYSK_EV_TRACE (engines with trace rows): reqlen_ 24, reslen_ 32, reqnum_ 40
+inline bool decode_trace(const ApiTran &r, uint32_t host_idx, gysk_event &o)
+{
+	const int32_t err = r.at<int32_t>(152);
+	o.svc_id = r.at<uint64_t>(120);
+	o.flow_key = (uint64_t)clamp32(r.at<uint64_t>(24)) | ((uint64_t)clamp32(r.at<uint64_t>(32)) << 32);
+	o.value = clamp32(r.at<uint64_t>(48));
+	o.host_idx = host_idx; o.tsec = (uint32_t)(r.at<uint64_t>(16) / 1000000ull);
+	o.type = GYSK_EV_TRACE;
+	o.flags = (err != 0 ? GYSK_EVF_TRACE_ERROR : 0u) | (r.at<uint64_t>(40) == 0 ? GYSK_EVF_TRACE_NEWCONN : 0u);
+	return true;
+}
 
 } // namespace gysk
 
@@ -1067,8 +1105,11 @@ int gysk_ingest_raw(gysk_engine *e, const uint8_t host_id[16], uint32_t host_idx
 
 	if (kind == GYSK_RAW_EVENT32) return stage_events(e, ts, static_cast<const gysk_event *>(events), n);
 	if (kind == GYSK_RAW_API_TRAN) {
-		for (ApiTran r {p}; n; --n, r.p += r.get_elem_size())
+		const bool trace = e->cfg.max_trace_svcs != 0;
+		for (ApiTran r {p}; n; --n, r.p += r.get_elem_size()) {
 			if (int rc = stage_record(e, ts, [&](gysk_event &o) { return decode_wire(r, host_idx, o); })) return rc;
+			if (trace) if (int rc = stage_record(e, ts, [&](gysk_event &o) { return decode_trace(r, host_idx, o); })) return rc;
+		}
 		return GYSK_OK;
 	}
 	const uint32_t stride = raw_stride(kind);
@@ -1265,8 +1306,9 @@ void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, siz
 		n++;
 	};
 	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) {
-		move(k * sizeof(*p), slots_of(kind, cfg.max_svcs, cfg.max_tasks), slots_of(kind, ms, mt));
+		move(k * sizeof(*p), slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs), slots_of(kind, ms, mt, cfg.max_trace_svcs));
 	});
+	if (cfg.max_trace_svcs) move(sizeof(uint32_t), (size_t)cfg.max_svcs + 1, (size_t)ms + 1);		// TraceTable::row_of
 	if (ms != cfg.max_svcs) move(sizeof(TblEntry), table_cap(cfg.max_svcs + 1), table_cap(ms + 1));
 	if (mt != cfg.max_tasks) move(sizeof(TblEntry), table_cap(cfg.max_tasks), table_cap(mt));
 	const size_t k0 = sort_keys(cfg), k1 = sort_keys(to);
@@ -1287,6 +1329,7 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 {
 	gysk_config &cfg = e->cfg;
 	if (ms < cfg.max_svcs || mt < cfg.max_tasks || ms > (1u << 24) || mt > (1u << 24)) return fail(e, GYSK_ERR_INVAL, "gysk_grow: shrink or beyond 1 << 24");
+	if (!trace_fits(ms, cfg.max_trace_svcs)) return fail(e, GYSK_ERR_INVAL, "gysk_grow: max_svcs + 1 + max_trace_svcs beyond 1 << 24");
 	if (ms == cfg.max_svcs && mt == cfg.max_tasks) return GYSK_OK;
 	size_t add = 0, big = 0, nalloc = 0, nfree = 0, ntotal = 0;
 	grow_bytes(e, ms, mt, &add, &big, &nalloc);
@@ -1304,9 +1347,10 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) {
 		if (rc) return;
 		if (kind == SlotKind::Ring) rc = regrow_ring(e, ms);
-		else rc = regrow(e, p, slots_of(kind, os, ot) * k, slots_of(kind, ms, mt) * k);
+		else rc = regrow(e, p, slots_of(kind, os, ot, cfg.max_trace_svcs) * k, slots_of(kind, ms, mt, cfg.max_trace_svcs) * k);
 		link_tables(st);
 	});
+	if (!rc && st.trace.rows) rc = regrow(e, st.trace.row_of, (size_t)os + 1, (size_t)ms + 1);
 	const size_t k0 = sort_keys(cfg), k1 = sort_keys(to), b0 = batch_rows(cfg), b1 = batch_rows(to);
 	if (!rc && !(rc = regrow(e, tmp.keys_a, k0, k1)) && !(rc = regrow(e, tmp.keys_b, k0, k1)) &&
 			!(rc = regrow(e, tmp.tile_status, (size_t)RADIX_MAX * sort_tiles(k0), (size_t)RADIX_MAX * sort_tiles(k1)))) {
@@ -1358,6 +1402,7 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 		e->task_tombstones = 0;
 	}
 	e->mg.members.null_slot = ms;			// the member slots are resolved again at every gysk_merge_prepare
+	if (st.trace.rows) st.trace.base = ms + 1;	// the pseudo-slots of the next batch's trace keys
 	e->ngrows++;
 	CU(e, cudaStreamSynchronize(e->stream));
 	return post_launch(e, "grow");
@@ -1460,6 +1505,12 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 	}
 	e->kernel_launches += launch_flush(e->st, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
 	e->kernel_launches += launch_task_flush(e->st, e->cfg.max_tasks, tsec, e->cfg.task_idle_evict_secs, e->d_tevict, e->stream);
+	if (e->st.trace.rows) {
+		// trace rows: the open window closes, the other half (the window before it) is cleared and opens
+		const uint32_t open = e->st.trace.par ^ 1u;
+		e->kernel_launches += launch_trace_roll(e->st, open, e->st.trace.rows, e->stream);
+		e->st.trace.par = open;
+	}
 	if (e->grow_limit_svcs > e->cfg.max_svcs || e->grow_limit_tasks > e->cfg.max_tasks) {
 		// auto-grow: the slot counts travel to the host behind the kernels, for the next flush's decision
 		CU(e, cudaMemcpyAsync(e->h_used, e->st.svc_tbl.count, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
@@ -2063,5 +2114,122 @@ double gysk_tdigest_quantile(const double *means, const uint64_t *weights, uint3
 uint32_t gysk_uint64_hash(uint64_t key) { return uint64_hash(key); }
 
 // ---- multi-GPU merge: implemented in gysk_merge.cu ------------------------------------------------------------
+
+} // extern "C"
+
+// ---- request traces (gysk_config.max_trace_svcs) --------------------------------------------------------------
+
+namespace {
+
+constexpr uint32_t TRACE_WIN_ROWS = (uint32_t)(STAGE_BYTES / sizeof(gysk_trace_row));		// trace rows per window-read pass
+static_assert(sizeof(gysk_trace_row) == 320 && QCHUNK <= TRACE_WIN_ROWS, "the stage holds a chunk of trace rows");
+static_assert(sizeof(TraceRaw) <= STAGE_BYTES, "the stage holds one trace digest");
+
+// rows handed out so far (engine held, stream synchronised on return)
+int trace_rows_out(gysk_engine *e, uint32_t *nrows)
+{
+	uint32_t c = 0;
+	CU(e, cudaMemcpyAsync(&c, e->st.trace.count, sizeof(c), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	*nrows = std::min(c, e->st.trace.rows);
+	return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+int gysk_query_traces(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_trace_row *out)
+{
+	CHECK_ENGINE(e);
+	if (!e->st.trace.rows) return GYSK_ERR_NOTSUP;
+	if ((!ids || !out) && n) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Submit);
+	return staged_read(e, ids, n, QCHUNK, sizeof(gysk_trace_row), "trace_rows", [&](const unsigned long long *d_ids, uint32_t, uint32_t m) {
+		return launch_trace_rows(e->st, d_ids, nullptr, m, reinterpret_cast<gysk_trace_row *>(e->d_wstage), e->stream);
+	}, CopyRows<gysk_trace_row> {out});
+}
+
+// the rows of the selection listed on the device, ordered by id on the host, then read by row in stage-sized passes
+int gysk_query_trace_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_trace_row *out, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!e->st.trace.rows) return GYSK_ERR_NOTSUP;
+	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Sync);
+	uint32_t nrows = 0;
+	if (int rc = trace_rows_out(e, &nrows)) return rc;
+	unsigned long long *d_n = e->st.counters + CTR_NWINDOW;
+	e->kernel_launches += launch_trace_list(e->st, nrows, host_idx, flags & GYSK_WINDOW_ACTIVE_ONLY, e->tmp.keys_b, e->tmp.keys_a, d_n, e->stream);
+	unsigned long long cnt = 0;
+	CU(e, cudaMemcpyAsync(&cnt, d_n, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	if (int rc = post_launch(e, "trace list")) return rc;
+	const uint32_t total = (uint32_t)cnt, m = std::min(cap, total);
+	if (m) {
+		std::vector<uint64_t> &ids = e->win_ids, &rows = e->win_keys;
+		ids.resize(total); rows.resize(total);
+		CU(e, cudaMemcpyAsync(ids.data(), e->tmp.keys_b, total * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaMemcpyAsync(rows.data(), e->tmp.keys_a, total * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+		CU(e, cudaStreamSynchronize(e->stream));
+		std::vector<std::pair<uint64_t, uint64_t>> &order = e->win_rows;
+		order.resize(total);
+		for (uint32_t i = 0; i < total; ++i) order[i] = {ids[i], rows[i]};
+		std::sort(order.begin(), order.end());		// ids are unique; the list's order depends on the device's atomics
+		for (uint32_t i = 0; i < m; ++i) rows[i] = order[i].second;
+		CU(e, cudaMemcpyAsync(e->tmp.keys_a, rows.data(), (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
+		int rc = staged_read<uint64_t>(e, nullptr, m, TRACE_WIN_ROWS, sizeof(gysk_trace_row), "trace_rows", [&](const unsigned long long *, uint32_t off, uint32_t k) {
+			return launch_trace_rows(e->st, nullptr, e->tmp.keys_a + off, k, reinterpret_cast<gysk_trace_row *>(e->d_wstage), e->stream);
+		}, CopyRows<gysk_trace_row> {out});
+		if (rc) return rc;
+	}
+	*n = total;
+	return GYSK_OK;
+}
+
+int gysk_export_trace_tdigest(gysk_engine *e, uint64_t id, int last_window, double *means, uint64_t *weights, uint32_t cap, uint32_t *n,
+		double *minv, double *maxv)
+{
+	CHECK_ENGINE(e);
+	if (!e->st.trace.rows) return GYSK_ERR_NOTSUP;
+	if (!means || !weights || !n) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Submit);
+	int rc = stage_one(e, id, sizeof(TraceRaw), "gather_trace", [&](const unsigned long long *d_ids, uint32_t, uint32_t) {
+		return launch_gather_trace(e->st, d_ids, last_window, reinterpret_cast<TraceRaw *>(e->d_wstage), e->stream);
+	});
+	if (rc) return rc;
+	const TraceRaw &r = *reinterpret_cast<const TraceRaw *>(e->h_wstage);
+	if (!r.found) return GYSK_ERR_NOENT;
+	TdHead h;
+	h.total = r.total; h.minv = r.minv; h.maxv = r.maxv; h.n = r.n; h.pad = 0;
+	return tdigest_out(h, r.cent, means, weights, cap, n, minv, maxv);
+}
+
+int gysk_export_trace_tdigest_pgtext(gysk_engine *e, uint64_t id, int last_window, char *buf, uint32_t cap)
+{
+	double means[TRACE_TD_CAP], mn, mx;
+	uint64_t weights[TRACE_TD_CAP];
+	uint32_t n = 0;
+	int rc = gysk_export_trace_tdigest(e, id, last_window, means, weights, TRACE_TD_CAP, &n, &mn, &mx);
+	if (rc) return rc;
+	return gysk_tdigest_to_pgtext(means, weights, n, TRACE_TD_DELTA, buf, cap);		// at compression 100 already: no recompress
+}
+
+int gysk_trace_info(gysk_engine *e, uint32_t *rows_in_use, uint64_t *dropped)
+{
+	CHECK_ENGINE(e);
+	if (!e->st.trace.rows) return GYSK_ERR_NOTSUP;
+	if (!rows_in_use || !dropped) return GYSK_ERR_INVAL;
+	GYSK_ENTER(e, Sync);
+	int32_t nfree = 0;
+	unsigned long long d = 0;
+	CU(e, cudaMemcpy(&nfree, e->st.trace.free_n, sizeof(nfree), cudaMemcpyDeviceToHost));
+	CU(e, cudaMemcpy(&d, e->st.trace.dropped, sizeof(d), cudaMemcpyDeviceToHost));
+	uint32_t nrows = 0;
+	if (int rc = trace_rows_out(e, &nrows)) return rc;
+	*rows_in_use = nrows - (uint32_t)std::max(nfree, 0);
+	*dropped = d;
+	return GYSK_OK;
+}
 
 } // extern "C"

@@ -10,6 +10,7 @@
 //   os_pass_kernel       stable one-sweep LSD radix pass (RESP keys of a batch on {slot, bin}; the top-N rankings)
 //   segs_mark_kernel     sorted keys -> one segment per service, touched list (short segments), batch rows (long segments)
 //   long_sum_kernel      keys of the long segments -> per-bin samples and exact usec sums in their batch rows
+//   trace_keys_kernel    trace rows (max_trace_svcs): requests, usec sum / max, response buckets of each row from the tail of the sorted keys
 //   bins_merge_kernel    per touched service: bins -> GY_HISTOGRAM::add_data for every sample (RESP_TIME_HASH, common/gy_statistics.h:
 //                        596-623, :1698) and -> the merging t-digest (K_1 scale)               DESIGN.md §2
 //   flush_kernel         5-s window roll                                               common/gy_socket_stat.cc:3898
@@ -106,8 +107,35 @@ __device__ __forceinline__ void task_slot_reset(const DevState &st, uint32_t slo
 	}
 }
 
+// An evicted service's trace row, by threads t = 0 .. nt - 1 of one CTA together: both windows zeroed, the row on the free stack, the
+// slot without a row
+__device__ __forceinline__ void trace_release(const TraceTable &tr, uint32_t slot, uint32_t t, uint32_t nt)
+{
+	const uint32_t r1 = tr.row_of[slot];
+	__syncthreads();			// every thread has read the entry before thread 0 clears it
+	if (r1 == 0 || r1 == TRACE_BUSY) return;
+	const uint32_t r = r1 - 1u;
+	for (uint32_t h = 0; h < 2u; ++h) {
+		for (uint32_t w = t; w < (uint32_t)TRACE_WORDS; w += nt) tr.words(h, r)[w] = 0ull;
+		for (uint32_t c = t; c < (uint32_t)TRACE_TD_CAP; c += nt) tr.cents(h, r)[c] = Centroid {0.0, 0ull};
+		if (t == 0) { TdHead z; z.total = 0; z.minv = INFINITY; z.maxv = -INFINITY; z.n = 0; z.pad = 0; *tr.hd(h, r) = z; }
+	}
+	if (t == 0) {
+		tr.row_of[slot] = 0; tr.row_slot[r] = ~0u;
+		const int32_t f = atomicAdd(tr.free_n, 1);
+		tr.free_rows[f] = r;
+	}
+}
+
 // the slot-reset functions evict_kernel takes
-struct SvcSlotReset { __device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const { slot_reset(st, slot, t, nt); } };
+struct SvcSlotReset
+{
+	__device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const
+	{
+		slot_reset(st, slot, t, nt);
+		if (st.trace.rows) trace_release(st.trace, slot, t, nt);
+	}
+};
 struct TaskSlotReset { __device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const { task_slot_reset(st, slot, t, nt); } };
 
 // service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state: one CTA per service slot, one thread per
@@ -347,6 +375,78 @@ __device__ __forceinline__ void drain_task_group(const DevState &st, HotTable &h
 }
 
 
+// ---- trace rows on the ingest side ----
+__device__ __forceinline__ void red_max_u64(unsigned long long *p, unsigned long long v)
+{
+	asm volatile("red.global.max.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+}
+
+// The trace row of a service slot: the one it holds, else one taken now (a freed row first, else the next fresh one), published in
+// row_of; -1 when no row is left. Racing events of the same slot wait for the taker, as table_resolve_slow's readers do.
+__device__ __forceinline__ int trace_row_take(const TraceTable &tr, uint32_t slot)
+{
+	uint32_t r1 = __ldcg(tr.row_of + slot);
+	if (r1 != 0 && r1 != TRACE_BUSY) return (int)(r1 - 1u);
+	if (r1 == 0 && (r1 = atomicCAS(tr.row_of + slot, 0u, TRACE_BUSY)) == 0) {
+		uint32_t r = ~0u;
+		const int32_t f = atomicSub(tr.free_n, 1);
+		if (f > 0) r = tr.free_rows[f - 1];
+		else {
+			atomicAdd(tr.free_n, 1);
+			const uint32_t c = atomicAdd(tr.count, 1u);
+			if (c < tr.rows) r = c;
+			else atomicSub(tr.count, 1u);
+		}
+		if (r != ~0u) tr.row_slot[r] = slot;
+		st_volatile_u32(tr.row_of + slot, r == ~0u ? 0u : r + 1u);
+		return r == ~0u ? -1 : (int)r;
+	}
+	while (r1 == TRACE_BUSY) { __nanosleep(20); r1 = ld_volatile_u32(tr.row_of + slot); }
+	return r1 ? (int)(r1 - 1u) : -1;
+}
+
+// The counters ingest_kernel adds per trace event (nerr, nconns, bytes in / out and their maxima), summed over a warp's lanes of one row
+// and held warp-uniform until a different row comes along or the kernel ends: one traced service brings millions of events per batch,
+// and REDs on one line are applied one after the other.
+struct TraceAcc
+{
+	int row;
+	unsigned long long nerr, nconns, bin, bout;
+	uint32_t min_, mout;
+
+	__device__ __forceinline__ void clear() { row = -1; nerr = nconns = bin = bout = 0; min_ = mout = 0; }
+	__device__ __forceinline__ void flush(const TraceTable &tr, int lane)
+	{
+		if (row >= 0 && lane == 0) {
+			unsigned long long *w = tr.words(tr.par, (uint32_t)row);
+			if (nerr) red_add_u64(w + TW_NERR, nerr);
+			if (nconns) red_add_u64(w + TW_NCONNS, nconns);
+			if (bin) red_add_u64(w + TW_BYTES_IN, bin);
+			if (bout) red_add_u64(w + TW_BYTES_OUT, bout);
+			if (min_) red_max_u64(w + TW_MAX_IN, min_);
+			if (mout) red_max_u64(w + TW_MAX_OUT, mout);
+		}
+		clear();
+	}
+	// the lanes' events (row < 0: none), all 32 lanes
+	__device__ __forceinline__ void add(const TraceTable &tr, int r_lane, uint32_t flags, unsigned long long fk, int lane)
+	{
+		const uint32_t lo = (uint32_t)fk, hi = (uint32_t)(fk >> 32);
+		for (uint32_t todo = __ballot_sync(0xffffffffu, r_lane >= 0); todo; ) {
+			const int r = __shfl_sync(0xffffffffu, r_lane, __ffs(todo) - 1);
+			const bool in = r_lane == r;
+			todo &= ~__ballot_sync(0xffffffffu, in);
+			const uint32_t ec = __reduce_add_sync(0xffffffffu, in ? (flags & GYSK_EVF_TRACE_ERROR ? 1u : 0u) | (flags & GYSK_EVF_TRACE_NEWCONN ? 1u << 16 : 0u) : 0u);
+			const unsigned long long bi = __reduce_add_sync(0xffffffffu, in ? lo & 0xFFFFu : 0u) + ((unsigned long long)__reduce_add_sync(0xffffffffu, in ? lo >> 16 : 0u) << 16);
+			const unsigned long long bo = __reduce_add_sync(0xffffffffu, in ? hi & 0xFFFFu : 0u) + ((unsigned long long)__reduce_add_sync(0xffffffffu, in ? hi >> 16 : 0u) << 16);
+			const uint32_t mi = __reduce_max_sync(0xffffffffu, in ? lo : 0u), mo = __reduce_max_sync(0xffffffffu, in ? hi : 0u);
+			if (r != row) { flush(tr, lane); row = r; }
+			nerr += ec & 0xFFFFu; nconns += ec >> 16; bin += bi; bout += bo;
+			min_ = max(min_, mi); mout = max(mout, mo);
+		}
+	}
+};
+
 struct IngestShared
 {
 	static constexpr int KQ_CAP = 192, KQ_FLUSH = KQ_CAP - IngestShape::CHUNK;	// a flush leaves room for a whole chunk of RESP events
@@ -357,6 +457,8 @@ struct IngestShared
 	uint32_t	dhist[KEY_PASSES_MAX][DH];			// digit histograms of this CTA's keys, one per radix pass
 };
 
+// TRACE: the engine has trace rows (a separate instance, so that an engine without them runs the kernel without the trace path)
+template <bool TRACE>
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
 		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, int exp)
 {
@@ -367,6 +469,9 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 	IngestShared::Warp &W = S.w[wid];
 	const uint32_t lt = (1u << lane) - 1u;
 	uint32_t c_in = 0, c_foreign = 0, n_resp = 0, n_active = 0;	// per thread: < 2^32 events per launch
+	uint32_t n_trace = 0, n_trace_drop = 0;				// trace events kept / dropped for want of a row
+	TraceAcc tacc;
+	tacc.clear();
 	uint32_t nk = 0, ntcp = 0, ntask = 0;				// queue lengths (warp-uniform)
 	unsigned long long t_tcp = 0, t_task = 0;			// queued in total (warp-uniform)
 
@@ -438,6 +543,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 			const uint32_t type = rb[k].w & 0xFFFFu;
 			const bool is_resp = type == GYSK_EV_RESP, is_task = type == GYSK_EV_TASK;
 			const bool is_tcp = type >= GYSK_EV_CONNECT && type <= GYSK_EV_CLOSE_SER, is_active = type == GYSK_EV_ACTIVE;
+			const bool is_trace = TRACE && type == GYSK_EV_TRACE;	// every response time: the row counts those beyond the rule too
 			bool mine = type != 0xFFFFu;
 
 			kind[k] = 0; ppos[k] = 0; praw[k] = make_uint4(0, 0, 0, 0);
@@ -446,15 +552,16 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 				c_in++;
 				// usec -> msec as SVC_INFO_CAP::upd_stats_on_req (gy_proto_parser.cc:2678); validity rule of
 				// handle_ipv4_resp_event (gy_socket_stat.cc:1519-1524): drop beyond 1 000 000 msec
-				if (svc + 1ull > 1ull && (is_tcp || is_task || is_active || (is_resp && value < 1000001000u))) {	// id not 0 / ~0 (tombstone); msec <= 1 000 000
-					kind[k] = is_resp ? (uint32_t)GYSK_EV_RESP : (is_task ? (uint32_t)GYSK_EV_TASK : (is_active ? (uint32_t)GYSK_EV_ACTIVE : (uint32_t)GYSK_EV_ACCEPT));
+				if (svc + 1ull > 1ull && (is_tcp || is_task || is_active || is_trace || (is_resp && value < 1000001000u))) {	// id not 0 / ~0 (tombstone); msec <= 1 000 000
+					kind[k] = is_resp ? (uint32_t)GYSK_EV_RESP : (is_task ? (uint32_t)GYSK_EV_TASK : (is_active ? (uint32_t)GYSK_EV_ACTIVE :
+							(is_trace ? (uint32_t)GYSK_EV_TRACE : (uint32_t)GYSK_EV_ACCEPT)));
 					praw[k] = table_probe_first(is_task ? st.task_tbl : st.svc_tbl, svc, ppos[k]);
 				}
 			}
 		}
 		// resolve every slot, then put the second round of loads (the slot's batch record and CONN_BITMAP word) of all EPT events
 		// in flight together, and fire the bin REDs — nothing below waits for them
-		int slotv[EPT];
+		int slotv[EPT], trow[EPT];
 		uint4 sbv[EPT];
 		uint32_t mwv[EPT], bkt[EPT];
 #pragma unroll
@@ -465,7 +572,11 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 				// one id lookup for all three event kinds (services and tasks live in separate tables)
 				slot = table_resolve(is_task ? st.task_tbl : st.svc_tbl, ((unsigned long long)ra[k].y << 32) | ra[k].x, st.auto_register, rb[k].y, ppos[k], praw[k]);
 			}
-			slotv[k] = slot; sbv[k] = make_uint4(0, 0, 0, 0); mwv[k] = 0; bkt[k] = 0;
+			slotv[k] = slot; sbv[k] = make_uint4(0, 0, 0, 0); mwv[k] = 0; bkt[k] = 0; trow[k] = -1;
+			if (TRACE && slot >= 0 && kind[k] == GYSK_EV_TRACE) {
+				trow[k] = trace_row_take(st.trace, (uint32_t)slot);
+				if (trow[k] >= 0) n_trace++; else n_trace_drop++;
+			}
 			if (slot >= 0 && is_resp) {
 				const uint32_t v = rb[k].x, ms = v / 1000u;		// usec -> msec as SVC_INFO_CAP::upd_stats_on_req (gy_proto_parser.cc:2678)
 				const uint32_t b = (uint32_t)bucket_resp_time((long long)ms);
@@ -486,7 +597,9 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 			// a hot service (sbv.w = 1 + its row of dense value bins, handed out by bins_merge_kernel after an earlier batch) takes its
 			// sample as two REDs into the L2-resident row; everybody else's sample becomes a sort key
 			const uint32_t hotrow = (ok && is_resp) ? sbv[k].w : 0u;
-			const uint32_t m_resp = __ballot_sync(0xffffffffu, ok && is_resp && !hotrow), m_tcp = __ballot_sync(0xffffffffu, ok && is_tcp),
+			// a trace sample within the RESP validity rule becomes a sort key of its row's pseudo-slot (a trace row: trow >= 0)
+			const bool tr_key = TRACE && trow[k] >= 0 && rb[k].x < 1000001000u;
+			const uint32_t m_resp = __ballot_sync(0xffffffffu, (ok && is_resp && !hotrow) || tr_key), m_tcp = __ballot_sync(0xffffffffu, ok && is_tcp),
 					m_task = __ballot_sync(0xffffffffu, ok && is_task);
 			if (ok) {
 				if (is_resp) {
@@ -510,6 +623,20 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					const uint32_t ef = rb[k].w >> 16;			// API_TRAN error flags: rare
 					if (ef & 3u) red_add_u64(&st.slot_aux[slot].err_cur, (unsigned long long)(ef & 1u) | ((unsigned long long)((ef >> 1) & 1u) << 32));
 				}
+				else if (TRACE && kind[k] == GYSK_EV_TRACE) {
+					const uint32_t v = rb[k].x;
+					// the value bins of a RESP key (td_code + RESP_TIME_HASH bucket): the batch items are those of the service digest's path
+					if (tr_key) W.kq[nk + __popc(m_resp & lt)] = ((unsigned long long)(st.trace.base + (uint32_t)trow[k]) << KEY_SLOT_SHIFT) |
+							((unsigned long long)(td_code(v) + (uint32_t)bucket_resp_time((long long)(v / 1000u))) << KEY_GROUP_SHIFT) | v;
+					else if (trow[k] >= 0) {
+						// beyond the validity rule (rare): no key, the counters the key would have brought straight into the row
+						unsigned long long *w = st.trace.words(st.trace.par, (uint32_t)trow[k]);
+						red_add_u64(w + TW_NREQ, 1ull);
+						red_add_u64(w + TW_SUM_US, (unsigned long long)v);
+						red_max_u64(w + TW_MAX_US, (unsigned long long)v);
+						red_add_u64(w + TW_BKT + 7, 1ull);
+					}
+				}
 				else if (kind[k] == GYSK_EV_ACTIVE) {
 					// one pre-aggregated {listener, client process} record of the 15-s inet_diag scan (gy_socket_stat.cc:6156-6194): a few
 					// per flow and minute — handled on the spot. The flow sketch takes its connections and kbytes, the service its totals.
@@ -532,6 +659,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 				}
 			}
 			nk += __popc(m_resp); ntcp += __popc(m_tcp); ntask += __popc(m_task);
+			if (TRACE) tacc.add(st.trace, trow[k], rb[k].w >> 16, ((unsigned long long)ra[k].w << 32) | ra[k].z, lane);
 		}
 		__syncwarp();
 
@@ -543,6 +671,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 	if (ntcp) { drain_tcp(ntcp); t_tcp += ntcp; }
 	if (ntask) { drain_task(ntask); t_task += ntask; }
 	if (nk) flush_keys();
+	if (TRACE) tacc.flush(st.trace, lane);
 	if (lane == 0) rec_cnt[gwarp] = make_uint2((uint32_t)t_tcp, (uint32_t)t_task);	// every warp of the launch: no memset needed
 
 	__syncthreads();
@@ -557,14 +686,17 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 	c_foreign = __reduce_add_sync(0xffffffffu, c_foreign);
 	const unsigned long long t_resp = __reduce_add_sync(0xffffffffu, n_resp);
 	t_tcp += __reduce_add_sync(0xffffffffu, n_active);		// counted with the connection events
+	const unsigned long long t_trace = __reduce_add_sync(0xffffffffu, n_trace);
+	n_trace_drop = __reduce_add_sync(0xffffffffu, n_trace_drop);
 	if (lane == 0) {
+		if (TRACE && n_trace_drop) atomicAdd(st.trace.dropped, (unsigned long long)n_trace_drop);
 		if (c_in) atomicAdd(st.counters + CTR_IN, (unsigned long long)c_in);
 		if (c_foreign) atomicAdd(st.counters + CTR_FOREIGN, (unsigned long long)c_foreign);
 		if (t_resp) atomicAdd(st.counters + CTR_RESP, t_resp);
 		if (t_tcp) atomicAdd(st.counters + CTR_TCP, t_tcp);
 		if (t_task) atomicAdd(st.counters + CTR_TASK, t_task);
 		// dropped = taken in but not queued (svc_id 0, bad type or value, table full, unknown id); two's complement arithmetic
-		const unsigned long long q = t_resp + t_tcp + t_task;
+		const unsigned long long q = t_resp + t_tcp + t_task + t_trace;
 		if (c_in != q) atomicAdd(st.counters + CTR_DROPPED, (unsigned long long)c_in - q);
 	}
 }
@@ -1155,6 +1287,74 @@ __global__ void __launch_bounds__(256) long_sum_kernel(const unsigned long long 
 	}
 }
 
+// The counters of the trace rows that their keys carry: requests, usec sum and maximum, the eight response buckets and the digest's
+// extremes. Trace keys have the highest slot numbers (pseudo-slots base + row), so they form the tail of the sorted array; each warp
+// takes an even share of the tail in rounds of 32 consecutive keys, sums each round per row with warp reductions and adds a row's sums to
+// it when the next row comes along (one RED per counter and row, not per key). A batch without trace keys leaves after the search.
+struct TraceKeyAcc
+{
+	int row;
+	unsigned long long nreq, sum, bkt[8];
+	uint32_t maxv, nmin;
+
+	__device__ __forceinline__ void clear() { row = -1; nreq = sum = 0; maxv = nmin = 0;
+#pragma unroll
+		for (int b = 0; b < 8; ++b) bkt[b] = 0;
+	}
+	__device__ __forceinline__ void flush(const TraceTable &tr, int lane)
+	{
+		if (row >= 0 && lane == 0) {
+			unsigned long long *w = tr.words(tr.par, (uint32_t)row);
+			red_add_u64(w + TW_NREQ, nreq);
+			red_add_u64(w + TW_SUM_US, sum);
+			red_max_u64(w + TW_MAX_US, maxv);
+#pragma unroll
+			for (int b = 0; b < 8; ++b) if (bkt[b]) red_add_u64(w + TW_BKT + b, bkt[b]);
+			red_max_u64(w + TW_TD_NMIN, nmin);
+			red_max_u64(w + TW_TD_MAX, maxv);
+		}
+		clear();
+	}
+};
+
+__global__ void __launch_bounds__(256) trace_keys_kernel(TraceTable tr, const unsigned long long *__restrict__ keys, const unsigned long long *__restrict__ d_n)
+{
+	const uint64_t n = *d_n;
+	uint64_t lo = 0, hi = n;		// the first trace key
+	while (lo < hi) { const uint64_t mid = (lo + hi) >> 1; if (key_slot(keys[mid]) < tr.base) lo = mid + 1; else hi = mid; }
+	if (lo == n) return;
+	const int lane = threadIdx.x & 31;
+	const uint64_t gw = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+	const uint64_t rounds = (n - lo + 31) >> 5, per = (rounds + nwarps - 1) / nwarps;
+	const uint64_t q1 = min(rounds, (gw + 1) * per);
+	TraceKeyAcc a;
+	a.clear();
+	for (uint64_t q = gw * per; q < q1; ++q) {
+		const uint64_t i = lo + (q << 5) + lane;
+		int row = -1;
+		uint32_t v = 0;
+		if (i < n) { const unsigned long long k = keys[i]; row = (int)(key_slot(k) - tr.base); v = key_usec(k); }
+		const uint32_t b = trace_bucket(v);
+		for (uint32_t todo = __ballot_sync(0xffffffffu, row >= 0); todo; ) {
+			const int r = __shfl_sync(0xffffffffu, row, __ffs(todo) - 1);
+			const bool in = row == r;
+			const uint32_t m = __ballot_sync(0xffffffffu, in);
+			todo &= ~m;
+			// per-bucket counts of the round (<= 32 each) packed 8 bits apiece; v < 2^30: 16-bit halves sum without overflow
+			const uint32_t pk0 = __reduce_add_sync(0xffffffffu, in && b < 4u ? 1u << (8u * b) : 0u);
+			const uint32_t pk1 = __reduce_add_sync(0xffffffffu, in && b >= 4u ? 1u << (8u * (b - 4u)) : 0u);
+			const unsigned long long sm = __reduce_add_sync(0xffffffffu, in ? v & 0xFFFFu : 0u) +
+					((unsigned long long)__reduce_add_sync(0xffffffffu, in ? v >> 16 : 0u) << 16);
+			const uint32_t mx = __reduce_max_sync(0xffffffffu, in ? v : 0u), nmn = __reduce_max_sync(0xffffffffu, in ? ~v : 0u);
+			if (r != a.row) { a.flush(tr, lane); a.row = r; }
+			a.nreq += __popc(m); a.sum += sm; a.maxv = max(a.maxv, mx); a.nmin = max(a.nmin, nmn);
+#pragma unroll
+			for (int j = 0; j < 4; ++j) { a.bkt[j] += (pk0 >> (8 * j)) & 0xFFu; a.bkt[4 + j] += (pk1 >> (8 * j)) & 0xFFu; }
+		}
+	}
+	a.flush(tr, lane);
+}
+
 static constexpr int TD_WARPS = 3;		// warps (= services in flight) per CTA
 // longest merged list (old centroids + batch items) that works in shared memory, 14.6 KB per warp: 5 CTAs x 3 warps fill the SM's
 // 228 KB. A list that does not fit is merged in the L2 scratch at several times the cost of one that does, so a larger area that
@@ -1170,6 +1370,7 @@ static constexpr int TD_SMEM_N = 540;
 // longer ones (a first batch can fill several hundred bins) in the warp's L2-resident scratch — same code, same result.
 // Work items, in this order: the hot rows, the batch rows of the long segments (both: dense bins, read in bin order and zeroed),
 // then the short segments, whose keys the warp reads itself.
+template <bool TRACE>
 __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merge_kernel(DevState st, const unsigned long long *__restrict__ keys,
 		const uint32_t *__restrict__ touched, const unsigned long long *__restrict__ ntouched_p, const uint32_t *__restrict__ long_slot,
 		const unsigned long long *__restrict__ nlong_p, unsigned long long *__restrict__ batch_rows, const BatchSeg *__restrict__ segs,
@@ -1212,27 +1413,36 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 	const uint32_t lt = (1u << lane) - 1u;
 	auto slot_of = [&](uint32_t t) { return t < nhot ? st.hot_slot[t] : (t < nrow ? long_slot[t - nhot] : touched[t - nrow]); };
 	uint32_t nslot = gw < total ? slot_of(gw) : 0u;
+	// a trace row's segment (slot >= the pseudo-slot base): its digest at compression TRACE_TD_DELTA, no histogram, no hot row
+	const uint32_t tbase = TRACE ? st.trace.base : 0xFFFFFFFFu;
 	for (uint32_t t = gw; t < total; t += nwarps) {
 		const uint32_t slot = nslot;
+		const bool trace = TRACE && slot >= tbase;		// warp-uniform
 		const bool has_next = t + nwarps < total;
 		// the loads of item t + nwarps go out before item t is merged: its slot here; its batch extremes, digest header and centroid
 		// lines (TD_CAP x 16 B = 32 lines, one per lane) as L2 prefetches as soon as the slot arrives, its segment as a value and
 		// its first keys as L2 prefetches further down. The chain of the next item then starts from L2 instead of DRAM.
 		nslot = has_next ? slot_of(t + nwarps) : 0u;
-		const SlotBatch sb = st.slot_batch[slot];
+		const SlotBatch sb = trace ? SlotBatch {0xFFFFFFFFu, 0u, 0u, 0u} : st.slot_batch[slot];
 		BatchSeg seg {0u, 0u, 0u, 0u};
 		if (t >= nrow) seg = segs[slot];
 		uint2 nseg = make_uint2(0u, 0u);
-		if (has_next) {
+		if (TRACE && has_next && nslot >= tbase) {
+			if (lane * 8 < TRACE_TD_CAP) prefetch_l2(st.trace.cents(st.trace.par, nslot - tbase) + lane * 8);
+		}
+		else if (has_next) {
 			prefetch_l2(st.td_cent + (size_t)nslot * TD_CAP + lane * (TD_CAP / 32));
 			if (lane == 0) prefetch_l2(st.slot_batch + nslot);
 			else if (lane == 1) prefetch_l2(st.td_head + nslot);
+		}
+		if (has_next) {
 			if (t + nwarps >= nrow) { const BatchSeg ns = segs[nslot]; nseg = make_uint2(ns.key0, ns.end); }
 		}
 		if (t < nhot && sb.minv == 0xFFFFFFFFu) continue;			// a hot service without a sample in this batch (warp-uniform)
 		if (lane < 16) { hcnt[wid][lane] = 0; hsum_lo[wid][lane] = 0; hsum_hi[wid][lane] = 0; }
 		__syncwarp();
-		const uint32_t na = st.td_head[slot].n;		// old centroids of the digest
+		TdHead *const hp = trace ? st.trace.hd(st.trace.par, slot - tbase) : st.td_head + slot;
+		const uint32_t na = hp->n;		// old centroids of the digest
 		TdWorkT<TD_SMEM_N> &W = work[wid];
 		// one non-empty bin {samples | remainders, usec sum} -> item j of the batch + GY_HISTOGRAM::add_data of its samples. The item
 		// goes to items[j], or with `staged` straight to where warp_merge_compress_staged reads it: mean at W.src[na + j], weight
@@ -1242,6 +1452,7 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 			const double mean = __ddiv_rn((double)us, (double)cnt);	// exact integer sum, one rounding
 			if (staged) { W.src[na + j] = mean; W.nxt[j] = (uint16_t)cnt; }
 			else { Centroid c; c.mean = mean; c.weight = cnt; items[j] = c; }
+			if (trace) return;
 			const uint32_t e = bk_tab[bin >> 3], bk = (e & 15u) + ((bin & 7u) >= (e >> 4) ? 1u : 0u);
 			atomicAdd(&hcnt[wid][bk], (uint32_t)cnt);
 			const unsigned long long ms = (us - rem) / 1000ull;		// sum of (usec / 1000) over the bin's samples
@@ -1391,7 +1602,8 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 		binmax = __reduce_max_sync(0xffffffffu, binmax);
 		__syncwarp();
 		// nobody else touches this slot's window histogram while the batch is merged (same stream as the flush): plain updates
-		if (lane < HIST_MAX_CELL) {
+		if (trace) {}
+		else if (lane < HIST_MAX_CELL) {
 			if (hcnt[wid][lane]) {
 				HistCell *c = st.hist_cur + (size_t)slot * HIST_CELLS + lane;
 				c->count += hcnt[wid][lane]; c->sum += (long long)(((unsigned long long)hsum_hi[wid][lane] << 32) | hsum_lo[wid][lane]);
@@ -1417,18 +1629,20 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 		__syncwarp();
 		if (exp & 256) continue;		// timing runs only (warp-uniform)
 
-		TdHead head = st.td_head[slot];
-		Centroid *cent = st.td_cent + (size_t)slot * TD_CAP;
+		TdHead head = *hp;
+		Centroid *cent = trace ? st.trace.cents(st.trace.par, slot - tbase) : st.td_cent + (size_t)slot * TD_CAP;
+		const TdParams P = trace ? st.trace.td : st.td;
 		uint32_t nout;
-		if (staged) nout = warp_merge_compress_staged(W, cent, na, nitems, cent, st.td);
-		else if (na + nitems <= (uint32_t)TD_SMEM_N) nout = warp_merge_compress(W, cent, na, items, nitems, cent, st.td);
-		else nout = warp_merge_compress(big_scratch[gw], cent, na, items, nitems, cent, st.td);
+		if (staged) nout = warp_merge_compress_staged(W, cent, na, nitems, cent, P);
+		else if (na + nitems <= (uint32_t)TD_SMEM_N) nout = warp_merge_compress(W, cent, na, items, nitems, cent, P);
+		else nout = warp_merge_compress(big_scratch[gw], cent, na, items, nitems, cent, P);
 		if (lane == 0) {
 			head.n = nout;
 			head.total += nsamples;
-			if ((double)sb.minv < head.minv) head.minv = (double)sb.minv;
-			if ((double)sb.maxv > head.maxv) head.maxv = (double)sb.maxv;
-			st.td_head[slot] = head;
+			// a trace digest's extremes are counter words of its window (trace_keys_kernel)
+			if (!trace && (double)sb.minv < head.minv) head.minv = (double)sb.minv;
+			if (!trace && (double)sb.maxv > head.maxv) head.maxv = (double)sb.maxv;
+			*hp = head;
 		}
 		__syncwarp();
 	}
@@ -2018,12 +2232,12 @@ static int plain_sort_plan(int lo, int hi, SortPlan &P)
 	return 0;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
 	const int dev = current_device();
 	SortPlan plan {};
-	if (key_sort_plan(max_svcs, plan) < 0) return -1;
+	if (key_sort_plan(key_slots, plan) < 0) return -1;
 	// the hot rows handed out by the batches so far are in use from this batch on
 	if (st.hot_rows) cudaMemcpyAsync(st.counters + CTR_NHOT, st.counters + CTR_NHOT_NEXT, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s);
 	// key cursor, digit histograms and tile tickets of this batch's sort
@@ -2032,7 +2246,8 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
 	static bool attr_set[MAX_DEVICES] = {};
 	if (!attr_set[dev]) {
-		cudaFuncSetAttribute(ingest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cudaFuncSetAttribute(ingest_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cudaFuncSetAttribute(ingest_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
 		attr_set[dev] = true;
 	}
 	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
@@ -2043,7 +2258,8 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	rr.nwarps = grid * WARPS;
 	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
-	ingest_kernel<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
+	if (st.trace.rows) ingest_kernel<true><<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
+	else ingest_kernel<false><<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
 	return 1;
 }
 
@@ -2161,7 +2377,7 @@ int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64
 // batch rows and fold every touched service's bins into its window histogram and its digest. Nothing here needs a number from the
 // device on the host: the key count lives in st.counters[CTR_NKEYS], the digit histograms in tmp.os_ghist (both written by
 // ingest_kernel); grids are sized by n_events, the largest possible key count, and surplus CTAs leave at once.
-int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s)
+int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	unsigned long long *d_nkeys = st.counters + CTR_NKEYS, *d_ntouched = st.counters + CTR_NTOUCHED;
@@ -2170,7 +2386,7 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 	os_set_attrs(dev);
 
 	SortPlan plan {};
-	if (key_sort_plan(max_svcs, plan) < 0) return -1;
+	if (key_sort_plan(key_slots, plan) < 0) return -1;
 	int which = 0;
 	const int launches = launch_sort_passes(plan, tmp, d_nkeys, div_up(n_events, SORT_TILE), &which, s);
 	const unsigned long long *src = which ? tmp.keys_b : tmp.keys_a;
@@ -2181,10 +2397,15 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 	cudaMemsetAsync(d_ntouched, 0, 2 * sizeof(unsigned long long), s);
 	segs_mark_kernel<<<div_up(n_events, SG_THREADS * SG_V), SG_THREADS, 0, s>>>(src, d_nkeys, segs, tmp.touched, d_ntouched, tmp.long_slot, d_nlong);
 	long_sum_kernel<<<nsm * 8, 256, 0, s>>>(src, d_nkeys, segs, d_nlong, tmp.batch_rows);
+	if (st.trace.rows) trace_keys_kernel<<<nsm * 4, 256, 0, s>>>(st.trace, src, d_nkeys);
 	const int merge_ctas = std::min(nsm, TD_MERGE_MAX_SMS) * TD_MERGE_CTAS_PER_SM;
-	bins_merge_kernel<<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
-			tmp.items_scratch, tmp.big_scratch, exp_ablate());
-	return launches + 3;
+	if (st.trace.rows)
+		bins_merge_kernel<true><<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
+				tmp.items_scratch, tmp.big_scratch, exp_ablate());
+	else
+		bins_merge_kernel<false><<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
+				tmp.items_scratch, tmp.big_scratch, exp_ablate());
+	return launches + 3 + (st.trace.rows ? 1 : 0);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -2417,6 +2638,137 @@ int launch_host_listen_rows(const unsigned long long *keys, const unsigned long 
 		gysk_host_listen *d_out, unsigned long long *d_rows, cudaStream_t s)
 {
 	host_listen_rows_kernel<<<1, 1024, 0, s>>>(keys, d_n, acc, rlo, cap, d_out, d_rows);
+	return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// trace rows: window roll, reads
+// ---------------------------------------------------------------------------------------------------
+// gysk_flush: the half that becomes the open window, cleared in every row handed out (its centroids are dead behind n = 0)
+__global__ void trace_roll_kernel(TraceTable tr, uint32_t open, uint32_t nrows)
+{
+	const uint64_t nw = (uint64_t)nrows * TRACE_WORDS;
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nw; i += (uint64_t)gridDim.x * blockDim.x) {
+		const uint32_t r = (uint32_t)(i / TRACE_WORDS), w = (uint32_t)(i % TRACE_WORDS);
+		tr.words(open, r)[w] = 0ull;
+		if (w == 0) { TdHead z; z.total = 0; z.minv = INFINITY; z.maxv = -INFINITY; z.n = 0; z.pad = 0; *tr.hd(open, r) = z; }
+	}
+}
+
+// one window of a row as gysk_trace_window
+__device__ __forceinline__ void trace_window_out(const TraceTable &tr, uint32_t half, uint32_t r, gysk_trace_window &o)
+{
+	const unsigned long long *w = tr.words(half, r);
+	o.nreq = w[TW_NREQ]; o.nerr = w[TW_NERR]; o.nconns = w[TW_NCONNS];
+	o.sum_resp_us = w[TW_SUM_US]; o.max_resp_us = w[TW_MAX_US];
+	o.bytes_in = w[TW_BYTES_IN]; o.bytes_out = w[TW_BYTES_OUT]; o.max_bytes_in = w[TW_MAX_IN]; o.max_bytes_out = w[TW_MAX_OUT];
+	for (int b = 0; b < 8; ++b) o.resp_buckets[b] = w[TW_BKT + b];
+	const TdHead h = *tr.hd(half, r);
+	o.td_count = h.total;
+	o.p99_resp_us = h.n ? td_quantile_seq(TdCentroids {tr.cents(half, r)}, h.n, (double)(0xFFFFFFFFu - (uint32_t)w[TW_TD_NMIN]), (double)w[TW_TD_MAX], 0.99)
+			: (double)NAN;
+}
+
+// one thread per row: by id (ids: the service table's lookup, then the slot's row) or by row (rows)
+__global__ void trace_rows_kernel(DevState st, const unsigned long long *__restrict__ ids, const unsigned long long *__restrict__ rows, uint32_t n,
+		gysk_trace_row *__restrict__ out)
+{
+	const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+	if (q >= n) return;
+	gysk_trace_row o;
+	memset(&o, 0, sizeof(o));
+	int r = -1, slot = -1;
+	if (ids) {
+		const unsigned long long id = ids[q];
+		o.glob_id = id;
+		slot = id + 1ull > 1ull ? table_lookup(st.svc_tbl, id, false) : -1;
+		if (slot >= 0) { const uint32_t r1 = st.trace.row_of[slot]; if (r1 != 0 && r1 != TRACE_BUSY) r = (int)(r1 - 1u); }
+	}
+	else {
+		r = (int)rows[q];
+		slot = (int)st.trace.row_slot[r];
+		o.glob_id = st.slot_id[slot];
+	}
+	if (r >= 0) {
+		o.found = 1;
+		o.host_idx = st.slot_host[slot];
+		trace_window_out(st.trace, st.trace.par, (uint32_t)r, o.cur);
+		trace_window_out(st.trace, st.trace.par ^ 1u, (uint32_t)r, o.last);
+	}
+	out[q] = o;
+}
+
+__global__ void trace_list_kernel(DevState st, uint32_t nrows, int host_filter, uint32_t active_only, unsigned long long *__restrict__ ids,
+		unsigned long long *__restrict__ rows, unsigned long long *d_n)
+{
+	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+	bool keep = false;
+	uint32_t slot = 0;
+	if (r < nrows) {
+		slot = st.trace.row_slot[r];
+		keep = slot != ~0u && (host_filter < 0 || st.slot_host[slot] == (uint32_t)host_filter) &&
+				(!active_only || st.trace.words(st.trace.par ^ 1u, r)[TW_NREQ] != 0);
+	}
+	const uint32_t m = __ballot_sync(0xffffffffu, keep);
+	unsigned long long base = 0;
+	if ((threadIdx.x & 31) == 0 && m) base = atomicAdd(d_n, (unsigned long long)__popc(m));
+	base = __shfl_sync(0xffffffffu, base, 0);
+	if (keep) {
+		const unsigned long long i = base + __popc(m & ((1u << (threadIdx.x & 31)) - 1u));
+		ids[i] = st.slot_id[slot]; rows[i] = r;
+	}
+}
+
+// one id's digest of one window, by one warp
+__global__ void gather_trace_kernel(DevState st, const unsigned long long *__restrict__ d_id, int last_window, TraceRaw *__restrict__ out)
+{
+	const int lane = threadIdx.x & 31;
+	const unsigned long long id = *d_id;
+	int r = -1;
+	if (id + 1ull > 1ull) {
+		const int slot = table_lookup(st.svc_tbl, id, false);
+		if (slot >= 0) { const uint32_t r1 = st.trace.row_of[slot]; if (r1 != 0 && r1 != TRACE_BUSY) r = (int)(r1 - 1u); }
+	}
+	if (r < 0) { if (lane == 0) out->found = 0; return; }
+	const uint32_t half = st.trace.par ^ (last_window ? 1u : 0u);
+	const TdHead h = *st.trace.hd(half, (uint32_t)r);
+	const Centroid *c = st.trace.cents(half, (uint32_t)r);
+	for (uint32_t i = lane; i < h.n; i += 32) out->cent[i] = c[i];
+	if (lane == 0) {
+		const unsigned long long *w = st.trace.words(half, (uint32_t)r);
+		out->found = 1; out->n = h.n; out->total = h.total;
+		out->minv = h.n ? (double)(0xFFFFFFFFu - (uint32_t)w[TW_TD_NMIN]) : INFINITY;
+		out->maxv = h.n ? (double)w[TW_TD_MAX] : -INFINITY;
+	}
+}
+
+int launch_trace_roll(const DevState &st, uint32_t open, uint32_t nrows, cudaStream_t s)
+{
+	if (!nrows) return 0;
+	const uint32_t grid = std::min<uint32_t>(div_up((uint64_t)nrows * TRACE_WORDS, 256), (uint32_t)sm_count(current_device()) * 8u);
+	trace_roll_kernel<<<grid, 256, 0, s>>>(st.trace, open, nrows);
+	return 1;
+}
+
+int launch_trace_rows(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_rows, uint32_t n, gysk_trace_row *d_out, cudaStream_t s)
+{
+	if (!n) return 0;
+	trace_rows_kernel<<<div_up(n, 128), 128, 0, s>>>(st, d_ids, d_rows, n, d_out);
+	return 1;
+}
+
+int launch_trace_list(const DevState &st, uint32_t nrows, int host_filter, uint32_t active_only, unsigned long long *ids, unsigned long long *rows,
+		unsigned long long *d_n, cudaStream_t s)
+{
+	cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s);
+	if (!nrows) return 0;
+	trace_list_kernel<<<div_up(nrows, 256), 256, 0, s>>>(st, nrows, host_filter, active_only, ids, rows, d_n);
+	return 1;
+}
+
+int launch_gather_trace(const DevState &st, const unsigned long long *d_id, int last_window, TraceRaw *d_out, cudaStream_t s)
+{
+	gather_trace_kernel<<<1, 32, 0, s>>>(st, d_id, last_window, d_out);
 	return 1;
 }
 

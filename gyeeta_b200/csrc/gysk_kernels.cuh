@@ -46,6 +46,44 @@ struct LevelRing
 	}
 };
 
+// Trace rows (gysk_config.max_trace_svcs): per row two windows, half `par` the open one. A window is TRACE_WORDS counters — line 0
+// the ones ingest_kernel adds per event (nerr, nconns, bytes), line 1 the ones trace_keys_kernel takes from the sorted keys — a digest
+// header ({total, n} used; the extremes are counter words) and TRACE_TD_CAP centroids. A trace sample's sort key carries the pseudo-slot
+// base + row in its slot field, so it rides the batch's radix sort and bins_merge_kernel compresses its segment into the row's digest.
+static constexpr int TRACE_WORDS = 32;
+static constexpr int TRACE_TD_DELTA = 100;		// public.tdigest(response, 100) of the trace view
+static constexpr int TRACE_TD_CAP = TRACE_TD_DELTA;	// the K_1 compress keeps at most delta clusters
+static constexpr uint32_t TRACE_BUSY = 0xFFFFFFFFu;	// row_of entry of a slot whose row is being taken
+enum {
+	TW_NERR = 0, TW_NCONNS, TW_BYTES_IN, TW_MAX_IN, TW_BYTES_OUT, TW_MAX_OUT,
+	TW_NREQ = 16, TW_SUM_US, TW_MAX_US, TW_BKT /* 8 words */, TW_TD_NMIN = TW_BKT + 8 /* max of ~usec of the digested samples */, TW_TD_MAX,
+};
+static_assert(TW_TD_MAX < TRACE_WORDS, "a window's counters fit TRACE_WORDS");
+struct TraceTable
+{
+	uint32_t		*row_of;			// [max_svcs + 1] 1 + the trace row of a service slot, 0 = none, TRACE_BUSY
+	uint32_t		*row_slot;			// [rows] service slot of a row, ~0u = free
+	unsigned long long	*cnt;				// [2][rows][TRACE_WORDS]
+	TdHead			*head;				// [2][rows]
+	Centroid		*cent;				// [2][rows][TRACE_TD_CAP]
+	uint32_t		*count;				// rows handed out so far
+	int32_t			*free_n;			// freed rows on the stack
+	uint32_t		*free_rows;			// [rows]
+	unsigned long long	*dropped;			// events dropped for want of a row
+	uint32_t		rows;				// capacity; 0 = off (every pointer nullptr)
+	uint32_t		par;				// the half of every array that holds the open window
+	uint32_t		base;				// pseudo-slot of row 0 in the sort keys: max_svcs + 1
+	TdParams		td;				// compression TRACE_TD_DELTA
+	__host__ __device__ __forceinline__ unsigned long long *words(uint32_t half, uint32_t r) const { return cnt + ((size_t)half * rows + r) * TRACE_WORDS; }
+	__host__ __device__ __forceinline__ TdHead *hd(uint32_t half, uint32_t r) const { return head + (size_t)half * rows + r; }
+	__host__ __device__ __forceinline__ Centroid *cents(uint32_t half, uint32_t r) const { return cent + ((size_t)half * rows + r) * TRACE_TD_CAP; }
+};
+// bucket of a response time in the trace view's eight response columns
+__host__ __device__ __forceinline__ uint32_t trace_bucket(uint32_t us)
+{
+	return (us >= 300u) + (us >= 1000u) + (us >= 10000u) + (us >= 30000u) + (us >= 100000u) + (us >= 300000u) + (us >= 1000000u);
+}
+
 struct DevState
 {
 	// id tables
@@ -90,6 +128,7 @@ struct DevState
 	double			td_delta;
 	TdParams		td;
 	unsigned long long	*counters;				// [CTR_MAX]
+	TraceTable		trace;					// trace rows (trace.rows == 0: off)
 };
 
 // The service slot rules every per-host read shares (window reads, gysk_query_host_listen, the cluster fold). A slot below the table's
@@ -189,8 +228,9 @@ static constexpr int LONG_SEG = 8192;
 int launch_init_slots(const DevState &st, uint32_t s_lo, uint32_t s_hi, uint32_t t_lo, uint32_t t_hi, cudaStream_t s);
 int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_t n, int is_task, cudaStream_t s);
 // -1: no sort plan for max_svcs, or the launch's record regions do not fit the buffers
-int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t max_svcs, RecRegions &rr, cudaStream_t s);
-int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
+// key_slots: the values the slot field of a sort key takes (max_svcs, or max_svcs + 1 + trace rows with trace rows)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s);
+int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
 int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
 // bits outside [0, 64)), or n_max >= 2^30
@@ -239,5 +279,16 @@ int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uin
 // GYSK_FLAG_FLOW_LEVEL, at the flush before the cms_cur / cms_last swap: cms_cur into ring slot st.levels.cur[0] (replacing it when
 // the slot is fresh), then cms_5min = the sum of the live slots
 int launch_cms_level_roll(const DevState &st, cudaStream_t s);
+// trace rows at gysk_flush: the half `open` (the one the flush opens) of rows [0, nrows) cleared
+int launch_trace_roll(const DevState &st, uint32_t open, uint32_t nrows, cudaStream_t s);
+// trace rows by id (d_ids) or by row (d_rows)
+int launch_trace_rows(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_rows, uint32_t n, gysk_trace_row *d_out, cudaStream_t s);
+// the rows in use of [0, nrows) that pass the host filter and (active_only) hold requests in their last window: ids at ids[i], rows at
+// rows[i], *d_n of them
+int launch_trace_list(const DevState &st, uint32_t nrows, int host_filter, uint32_t active_only, unsigned long long *ids, unsigned long long *rows,
+		unsigned long long *d_n, cudaStream_t s);
+// one id's digest of one window: TraceRaw
+struct TraceRaw { int32_t found; uint32_t n; unsigned long long total; double minv, maxv; Centroid cent[TRACE_TD_CAP]; };
+int launch_gather_trace(const DevState &st, const unsigned long long *d_id, int last_window, TraceRaw *d_out, cudaStream_t s);
 
 } // namespace gysk

@@ -48,7 +48,7 @@ class Config(C.Structure):
                 ("cms_depth", C.c_uint32), ("cms_log2_width", C.c_uint32), ("hll_p", C.c_uint32),
                 ("td_compression", C.c_uint32), ("max_batch", C.c_uint32), ("flags", C.c_uint32), ("rank", C.c_uint32),
                 ("world", C.c_uint32), ("stage_batch", C.c_uint32), ("idle_evict_secs", C.c_uint32),
-                ("task_idle_evict_secs", C.c_uint32), ("reserved", C.c_uint32)]
+                ("task_idle_evict_secs", C.c_uint32), ("max_trace_svcs", C.c_uint32)]
 
 
 class SvcSummary(C.Structure):
@@ -238,6 +238,11 @@ def load_library(path=None):
         "gysk_evicted_task_ids": (i32, [vp, vp, u32, vp]),
         "gysk_task_evict_count": (i32, [vp, vp]),
         "gysk_query_svcs": (i32, [vp, vp, u32, vp]),
+        "gysk_query_traces": (i32, [vp, vp, u32, vp]),
+        "gysk_query_trace_window": (i32, [vp, i32, u32, vp, u32, vp]),
+        "gysk_export_trace_tdigest": (i32, [vp, u64, i32, vp, vp, u32, vp, vp, vp]),
+        "gysk_export_trace_tdigest_pgtext": (i32, [vp, u64, i32, vp, u32]),
+        "gysk_trace_info": (i32, [vp, vp, vp]),
         "gysk_query_flows": (i32, [vp, vp, u32, i32, vp]),
         "gysk_query_window": (i32, [vp, C.c_int32, u32, vp, u32, vp]),
         "gysk_query_window_hosts": (i32, [vp, C.c_int32, u32, vp, vp, u32, vp]),
@@ -318,12 +323,38 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+class TraceWindow(C.Structure):
+    """gysk_trace_window: one 5-s window of a service's request traces (the trace view's columns)"""
+    _fields_ = [(n, C.c_uint64) for n in ("nreq", "nerr", "nconns", "sum_resp_us", "max_resp_us", "bytes_in", "bytes_out",
+                                          "max_bytes_in", "max_bytes_out")] + \
+               [("resp_buckets", C.c_uint64 * 8), ("td_count", C.c_uint64), ("p99_resp_us", C.c_double)]
+
+    def asdict(self):
+        d = {f: getattr(self, f) for f, _ in self._fields_}
+        d["resp_buckets"] = list(self.resp_buckets)
+        return d
+
+
+class TraceRow(C.Structure):
+    _fields_ = [("glob_id", C.c_uint64), ("found", C.c_int32), ("host_idx", C.c_uint32), ("cur", TraceWindow), ("last", TraceWindow)]
+
+    def asdict(self):
+        return {"glob_id": self.glob_id, "found": self.found, "host_idx": self.host_idx, "cur": self.cur.asdict(), "last": self.last.asdict()}
+
+
+assert C.sizeof(TraceWindow) == 152 and C.sizeof(TraceRow) == 320
+TRACE_TD_CAP = 100
+EV_TRACE = 8
+EVF_TRACE_ERROR, EVF_TRACE_NEWCONN = 0x1, 0x2
+
+
 class Engine:
     """One engine = one GPU. Mirrors the C ABI one to one."""
 
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
-                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0):
+                 merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
+                 max_trace_svcs=0):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -333,6 +364,7 @@ class Engine:
         cfg.stage_batch = stage_batch
         cfg.idle_evict_secs = idle_evict_secs
         cfg.task_idle_evict_secs = task_idle_evict_secs
+        cfg.max_trace_svcs = max_trace_svcs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0)
@@ -412,6 +444,51 @@ class Engine:
         n = C.c_uint32()
         self._chk(self.L.gysk_evicted_task_ids(self.h, _p(out), cap, C.byref(n)))
         return out[:min(n.value, cap)].copy()
+
+    def query_traces(self, ids):
+        """gysk_query_traces: one TraceRow per id"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (TraceRow * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_traces(self.h, _p(ids), len(ids), out))
+        return out[:len(ids)]
+
+    def query_trace_window(self, host_idx=-1, active_only=False, cap=None):
+        """gysk_query_trace_window: (TraceRow rows in ascending glob_id, number of matching rows); cap None = all rows"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_trace_window(self.h, host_idx, flags, None, 0, C.byref(n)))
+            cap = n.value
+        out = (TraceRow * max(cap, 1))()
+        self._chk(self.L.gysk_query_trace_window(self.h, host_idx, flags, out if cap else None, cap, C.byref(n)))
+        return out[:min(cap, n.value)], n.value
+
+    def export_trace_tdigest(self, id_, last_window=False):
+        """gysk_export_trace_tdigest: (means, weights, min, max) of one window's digest, None for an id without a trace row"""
+        means = np.zeros(TRACE_TD_CAP, dtype=np.float64)
+        weights = np.zeros(TRACE_TD_CAP, dtype=np.uint64)
+        n, mn, mx = C.c_uint32(), C.c_double(), C.c_double()
+        rc = self.L.gysk_export_trace_tdigest(self.h, int(id_), int(bool(last_window)), _p(means), _p(weights), TRACE_TD_CAP, C.byref(n),
+                                              C.byref(mn), C.byref(mx))
+        if rc == -2:
+            return None
+        self._chk(rc)
+        return means[: n.value].copy(), weights[: n.value].copy(), mn.value, mx.value
+
+    def export_trace_tdigest_pgtext(self, id_, last_window=False):
+        buf = C.create_string_buffer(8192)
+        rc = self.L.gysk_export_trace_tdigest_pgtext(self.h, int(id_), int(bool(last_window)), buf, len(buf))
+        if rc == -2:
+            return None
+        if rc < 0:
+            self._chk(rc)
+        return buf.value.decode()
+
+    def trace_info(self):
+        """gysk_trace_info: (rows in use, trace events dropped for want of a row)"""
+        rows, dropped = C.c_uint32(), C.c_uint64()
+        self._chk(self.L.gysk_trace_info(self.h, C.byref(rows), C.byref(dropped)))
+        return rows.value, dropped.value
 
     def task_evict_count(self):
         """aggregated processes evicted so far"""

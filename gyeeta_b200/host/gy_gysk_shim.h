@@ -104,6 +104,32 @@ public :
 				GYSK_RAW_API_TRAN, ptran, n);
 	}
 
+	// handle_trace_requests (server/gy_mconnhdlr.cc:5883-6060) with trace rows (gysk_config.max_trace_svcs): the records go to the engine,
+	// which stages each one's RESP and trace events, instead of one tracereqtbl row per request. What reaches the database is one row per
+	// traced service and window: trace_window_rows after each flush_window.
+	template <typename ParthaInfo>
+	bool handle_trace_requests(const std::shared_ptr<ParthaInfo> & partha_shr, const void *ptran, uint32_t n) noexcept
+	{
+		return handle_api_trans(partha_shr, ptran, n);
+	}
+
+	// the closed window of every traced service with requests in it, ascending glob_id: on_row(row, pgtext) once per service, with the
+	// window's compression-100 digest as Postgres tdigest text for the row's digest column (NULL when it has no digested sample)
+	template <typename OnRow>
+	bool trace_window_rows(OnRow && on_row) noexcept
+	{
+		uint32_t n = 0;
+		if (0 != gysk_query_trace_window(engine_, -1, GYSK_WINDOW_ACTIVE_ONLY, nullptr, 0, &n)) return false;
+		std::vector<gysk_trace_row> rows(n);
+		if (n && 0 != gysk_query_trace_window(engine_, -1, GYSK_WINDOW_ACTIVE_ONLY, rows.data(), n, &n)) return false;
+		std::vector<char> buf(8192);
+		for (const gysk_trace_row & r : rows) {
+			const int len = r.last.td_count ? gysk_export_trace_tdigest_pgtext(engine_, r.glob_id, 1, buf.data(), (uint32_t)buf.size()) : 0;
+			on_row(r, len > 0 ? (const char *)buf.data() : (const char *)nullptr);
+		}
+		return true;
+	}
+
 	// the 5-s reducer tick (TCP_SOCK_HANDLER::listener_stats_update cadence, common/gy_socket_stat.cc:3898)
 	bool flush_window(uint32_t tsec) noexcept
 	{

@@ -64,11 +64,22 @@ enum {
 	GYSK_EV_TASK		= 6,	/* per-process 5-s sample (AGGR_TASK_STATE_NOTIFY) */
 	GYSK_EV_ACTIVE		= 7,	/* one ACTIVE_CONN_STATS record (common/gy_comm_proto.h:2766): the 15-s inet_diag group-by
 					   {ser_glob_id, cli_task_aggr_id} of upd_conn_from_diag (common/gy_socket_stat.cc:6156-6194) */
+	GYSK_EV_TRACE		= 8,	/* one request trace (an API_TRAN, the row handle_trace_requests writes to tracereqtbl,
+					   server/gy_mconnhdlr.cc:5883-6060), kept only by an engine with trace rows
+					   (gysk_config.max_trace_svcs; dropped without). Fields reused as by ACTIVE:
+					     svc_id   = glob_id_
+					     flow_key = min(reqlen_, 2^32 - 1) | min(reslen_, 2^32 - 1) << 32   (bytes in | bytes out)
+					     value    = response_usec_ clamped to 32 bits
+					     flags    = GYSK_EVF_TRACE_ERROR (errorcode_ != 0) | GYSK_EVF_TRACE_NEWCONN (reqnum_ == 0)
+					   gysk_ingest_raw(GYSK_RAW_API_TRAN) stages one next to the record's GYSK_EV_RESP */
 };
 
 /* gysk_event.flags of a GYSK_EV_RESP event that came from an API_TRAN (SVC_INFO_CAP::upd_stats_on_req, gy_proto_parser.cc:2678-2694) */
 #define GYSK_EVF_CLI_ERROR		0x1u	/* stats_.ncli_errors_++ */
 #define GYSK_EVF_SER_ERROR		0x2u	/* stats_.nser_errors_++ */
+/* gysk_event.flags of a GYSK_EV_TRACE event */
+#define GYSK_EVF_TRACE_ERROR		0x1u	/* errorcode_ != 0: counted in nerr */
+#define GYSK_EVF_TRACE_NEWCONN		0x2u	/* reqnum_ == 0: counted in nconns */
 
 typedef struct gysk_event
 {
@@ -231,7 +242,11 @@ typedef struct gysk_config
 						   seconds before the tsec of a gysk_flush is evicted by that flush: the rule of
 						   MCONN_HANDLER::cleanup_partha_unused_aggr_tasks (server/gy_mconnhdlr.cc:16492-16541), whose
 						   value is 1800 (last_tusec_ older than 30 min). 0 (default) = never; "process eviction" below */
-	uint32_t	reserved;
+	uint32_t	max_trace_svcs;		/* trace rows: services whose request traces (GYSK_EV_TRACE) are summed per 5-s window on the
+					   device ("request traces" below). 0 (default) = off: GYSK_EV_TRACE events are dropped, nothing
+					   is allocated and the trace calls are GYSK_ERR_NOTSUP. max_svcs + 1 + max_trace_svcs <= 1 << 24
+					   (gysk_create and gysk_grow refuse more). This was the last spare word of the struct: a new
+					   setting needs a new ABI version */
 } gysk_config;
 
 typedef struct gysk_engine gysk_engine;
@@ -386,7 +401,7 @@ int64_t		gysk_flow_table_used(gysk_engine *e);
  * gysk_set_logical_map / gysk_set_cluster_map and the last finished merge's results are kept: every read answers afterwards exactly as an
  * engine created with the new capacity and given the same calls would. Serialised with the ingest threads like a reader (their stages
  * are drained first). Between gysk_merge_prepare and gysk_merge_finish it is allowed: the prepared buffers do not depend on the
- * capacity. GYSK_ERR_INVAL: shrink or beyond 1 << 24. GYSK_ERR_NOMEM: the new arrays do not fit the device's free memory; this is
+ * capacity. GYSK_ERR_INVAL: shrink or beyond 1 << 24, or max_svcs + 1 + max_trace_svcs beyond 1 << 24 (the engine unchanged). GYSK_ERR_NOMEM: the new arrays do not fit the device's free memory; this is
  * checked before anything is allocated, and the engine is unchanged. Arrays move one at a time, so the device holds at most the new
  * footprint plus the largest old array while it runs. Should an allocation still fail after the check (another user of the device
  * took the memory meanwhile), the result is GYSK_ERR_NOMEM too: the engine keeps its capacity and answers every read as before, the
@@ -413,7 +428,8 @@ int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the
  * engine of this configuration (NULL: the defaults); they depend on hll_p and on whether task_idle_evict_secs is set. An engine's footprint is about
  * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
  * buffers and the count-min tables: 2 tables of cms_depth << cms_log2_width 8-byte cells, 11 more with GYSK_FLAG_FLOW_LEVEL (its 10 ring
- * slots and the level: 352 MiB more at the default 4 x 2^20). The count-min tables do not depend on capacity, so gysk_grow leaves them. */
+ * slots and the level: 352 MiB more at the default 4 x 2^20). The count-min tables do not depend on capacity, so gysk_grow leaves them.
+ * Trace rows (max_trace_svcs) are not per service slot and not counted here: 3784 bytes each, in gysk_capacity.device_bytes. */
 int		gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes);
 
 /* ---- registration (control path; mirrors partha_listener_info registering listeners before state arrives) ---- */
@@ -585,6 +601,58 @@ int		gysk_export_cms(gysk_engine *e, int last_window, uint64_t *cells /* depth <
 int		gysk_query_flows_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_est *out);
 int		gysk_export_cms_5min(gysk_engine *e, uint64_t *cells /* depth << log2_width entries */);
 int		gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_est *out);
+
+/* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
+ * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
+ * aggregates those rows per service and time bucket in SQL (tracereq_aggr_info, common/gy_json_field_maps.h:2628-2664). Here each traced
+ * service holds a trace row on the device, and each window of it carries that aggregate's columns, so one row per service and window
+ * reaches the database instead of one per request:
+ *  - a service takes a row with its first GYSK_EV_TRACE event, from the rows an evicted service freed first, else the next fresh one.
+ *    With every row taken, the events of services without one are dropped (gysk_trace_info's dropped, and gysk_stats.events_dropped).
+ *    An evicted service's row is zeroed and freed; the same id seen again starts from empty windows;
+ *  - a sample lands in the window open when it arrives, as every other sample; gysk_flush closes it into `last` and opens an empty one;
+ *  - every sample counts in every counter. A response beyond the GYSK_EV_RESP validity rule (1 000 000 msec) stays out of the digest,
+ *    as it stays out of the service's;
+ *  - the digest is a merging t-digest at compression 100, the public.tdigest(response, 100) of the trace view's p99respus: its
+ *    pgtext export is stored as it is, and Postgres merges a range of windows with public.tdigest(col). p99_resp_us is its 0.99
+ *    quantile (the rule of gysk_tdigest_quantile), NaN while it is empty. */
+typedef struct gysk_trace_window
+{
+	uint64_t	nreq;			/* count(*) */
+	uint64_t	nerr;			/* errorcode != 0 */
+	uint64_t	nconns;			/* reqnum = 0 */
+	uint64_t	sum_resp_us;		/* avgrespus = sum_resp_us / nreq */
+	uint64_t	max_resp_us;		/* maxrespus */
+	uint64_t	bytes_in, bytes_out;	/* sum(bytesin), sum(bytesout) */
+	uint64_t	max_bytes_in, max_bytes_out;
+	uint64_t	resp_buckets[8];	/* resplt300us, resplt1ms, resplt10ms, resplt30ms, resplt100ms, resplt300ms, resplt1sec, respgt1sec:
+						   [0, 300), [300, 1000), [1000, 10000), [10000, 30000), [30000, 100000), [100000, 300000),
+						   [300000, 1000000), [1000000, inf) usec */
+	uint64_t	td_count;		/* samples in the digest (nreq less those beyond the validity rule) */
+	double		p99_resp_us;		/* p99respus; NaN when the digest is empty */
+} gysk_trace_window;			/* 152 bytes */
+
+typedef struct gysk_trace_row
+{
+	uint64_t		glob_id;
+	int32_t			found;		/* 0: unknown id, or a service without a trace row (the windows are then zero) */
+	uint32_t		host_idx;	/* host of the event that created the service's slot */
+	gysk_trace_window	cur, last;	/* the window being filled and the last closed one */
+} gysk_trace_row;			/* 320 bytes */
+
+/* the rows of n ids. GYSK_ERR_NOTSUP without trace rows */
+int		gysk_query_traces(gysk_engine *e, const uint64_t *glob_ids, uint32_t n, gysk_trace_row *out);
+/* one row per service holding a trace row, in ascending glob_id; each equals the gysk_query_traces row of its id. host_idx < 0 reads
+ * every host; GYSK_WINDOW_ACTIVE_ONLY keeps the rows whose last window holds requests. Count and capacity as gysk_query_window */
+int		gysk_query_trace_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_trace_row *out, uint32_t cap, uint32_t *n);
+/* the digest of a service's open (last_window = 0) or last closed window: the contract of gysk_export_tdigest (min / max: the extremes
+ * of the digested samples, +inf / -inf while empty). GYSK_ERR_NOENT for an id without a trace row */
+int		gysk_export_trace_tdigest(gysk_engine *e, uint64_t glob_id, int last_window, double *means, uint64_t *weights, uint32_t cap,
+				uint32_t *n, double *min_val, double *max_val);
+/* the same digest as Postgres tdigest text (gysk_tdigest_to_pgtext at compression 100, no recompress); the string length or GYSK_ERR_* */
+int		gysk_export_trace_tdigest_pgtext(gysk_engine *e, uint64_t glob_id, int last_window, char *buf, uint32_t cap);
+/* rows in use (handed out less the freed ones) and the trace events dropped so far for want of a row */
+int		gysk_trace_info(gysk_engine *e, uint32_t *rows_in_use, uint64_t *dropped);
 
 /* ---- row a15b: the per-process -> per-aggregate-process group-by in front of partha_aggr_task_state ----
  * One record per process and 5-s tick, holding what TASK_HANDLER's walk has at hand when it folds the process into
