@@ -147,9 +147,21 @@ __host__ __device__ __forceinline__ unsigned long long cms_increment(uint32_t by
 	return 1ull | ((unsigned long long)(bytes >> 10) << 32);
 }
 
+// murmur3's 64-bit finalizer. The HyperLogLog takes its register index from the top p bits of the word and its rank from the
+// rest, so every output bit must depend on every key bit. Two one-round lookup2 words do not do that: on keys built as
+// (client ip << 32) | port, h2's top bits reached only 3 341 of 4 096 registers at p = 12 for 20 000 keys (64 ports per ip),
+// and the estimate came out 65 % low. The count-min indexes low bits of h1 + r * (h2 | 1) and keeps the unmixed words.
+__host__ __device__ __forceinline__ unsigned long long fmix64(unsigned long long h)
+{
+	h ^= h >> 33; h *= 0xff51afd7ed558ccdull;
+	h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull;
+	h ^= h >> 33;
+	return h;
+}
+
 __device__ __forceinline__ void hll_idx_rank2(uint32_t h1, uint32_t h2, uint32_t p, uint32_t &idx, uint32_t &rank)
 {
-	const unsigned long long h = ((unsigned long long)h2 << 32) | h1;
+	const unsigned long long h = fmix64(((unsigned long long)h2 << 32) | h1);
 	const unsigned long long w = h << p;
 
 	idx = (uint32_t)(h >> (64 - p));

@@ -291,12 +291,19 @@ uint64_t gyo_cms_increment(uint32_t bytes)
 	return 1ull | ((uint64_t)(bytes >> 10) << 32);
 }
 
+/* murmur3's 64-bit finalizer over h2:h1: the register index is the top p bits of the word, and the two one-round lookup2
+ * words leave those bits poorly mixed on structured keys ((client ip << 32) | port undercounted by up to 65 %). */
 uint64_t gyo_hll_hash(uint64_t flow_key)
 {
 	uint32_t h1, h2;
+	uint64_t h;
 
 	gyo_flow_hashes(flow_key, &h1, &h2);
-	return ((uint64_t)h2 << 32) | h1;
+	h = ((uint64_t)h2 << 32) | h1;
+	h ^= h >> 33; h *= 0xff51afd7ed558ccdull;
+	h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull;
+	h ^= h >> 33;
+	return h;
 }
 
 void gyo_hll_idx_rank(uint64_t flow_key, uint32_t p, uint32_t *idx, uint8_t *rank)
@@ -306,6 +313,17 @@ void gyo_hll_idx_rank(uint64_t flow_key, uint32_t p, uint32_t *idx, uint8_t *ran
 
 	*idx = (uint32_t)(h >> (64 - p));
 	*rank = (uint8_t)(w ? (uint32_t)(__builtin_clzll(w) + 1) : (64u - p + 1u));
+}
+
+/* raise the 1 << p registers regs with n keys (registers are not cleared first, so sets can be added in several calls) */
+void gyo_hll_registers(const uint64_t *keys, uint64_t n, uint32_t p, uint8_t *regs)
+{
+	for (uint64_t i = 0; i < n; ++i) {
+		uint32_t idx; uint8_t rank;
+
+		gyo_hll_idx_rank(keys[i], p, &idx, &rank);
+		if (regs[idx] < rank) regs[idx] = rank;
+	}
 }
 
 /* Flajolet et al. 2007 raw estimator + linear counting for the small range; 64-bit hash => no large-range

@@ -88,9 +88,10 @@ int	gyo_hist_run(int cls, int tkind, const int64_t *vals, size_t n, const float 
 uint32_t gyo_cms_index(uint64_t flow_key, uint32_t row, uint32_t log2_width);
 uint64_t gyo_cms_increment(uint32_t bytes);		/* 1 | (bytes >> 10) << 32 */
 void	gyo_flow_hashes(uint64_t flow_key, uint32_t *h1, uint32_t *h2);
-uint64_t gyo_hll_hash(uint64_t flow_key);
+uint64_t gyo_hll_hash(uint64_t flow_key);	/* fmix64(h2:h1) */
 uint32_t gyo_td_code(uint32_t usec);	/* log-linear bin of a response time, 32 bins per octave */
 void	gyo_hll_idx_rank(uint64_t flow_key, uint32_t p, uint32_t *idx, uint8_t *rank);
+void	gyo_hll_registers(const uint64_t *keys, uint64_t n, uint32_t p, uint8_t *regs);	/* regs[idx] = max(regs[idx], rank) per key */
 double	gyo_hll_estimate(const uint8_t *regs, uint32_t p);
 
 void	gyo_td_init(gyo_tdigest *t);

@@ -77,6 +77,7 @@ def lib():
         L.gyo_hll_hash.restype = C.c_uint64
         L.gyo_hll_hash.argtypes = [C.c_uint64]
         L.gyo_hll_idx_rank.argtypes = [C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p]
+        L.gyo_hll_registers.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
         L.gyo_hll_estimate.restype = C.c_double
         L.gyo_hll_estimate.argtypes = [C.c_void_p, C.c_uint32]
         L.gyo_td_init.argtypes = [C.c_void_p]
@@ -264,6 +265,22 @@ class OracleEngine:
 
     def merge_from(self, other):
         self.L.gyo_merge_from(self.h, other.h)
+
+
+def hll_registers(keys, p, regs=None):
+    """gyo_hll_registers: the 1 << p registers of the keys (raised in place when regs is given)"""
+    keys = np.ascontiguousarray(keys, dtype=np.uint64)
+    if regs is None:
+        regs = np.zeros(1 << p, dtype=np.uint8)
+    assert regs.dtype == np.uint8 and regs.flags.c_contiguous and len(regs) == 1 << p
+    lib().gyo_hll_registers(_p(keys), len(keys), p, _p(regs))
+    return regs
+
+
+def hll_estimate(regs, p):
+    regs = np.ascontiguousarray(regs, dtype=np.uint8)
+    assert len(regs) == 1 << p
+    return lib().gyo_hll_estimate(_p(regs), p)
 
 
 def td_quantile(td, q):
