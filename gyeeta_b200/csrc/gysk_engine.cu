@@ -527,6 +527,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 			cfg.td_compression < 10 || cfg.td_compression > (uint32_t)TD_CAP || cfg.max_batch < 1024 || cfg.max_batch >= (1u << 27) ||
 			cfg.rank >= cfg.world || !trace_fits(cfg.max_svcs, cfg.max_trace_svcs))
 		return fail(nullptr, GYSK_ERR_INVAL, "gysk_config out of range");
+	if ((cfg.flags & GYSK_FLAG_MERGE_TRACES) && !cfg.max_trace_svcs)
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_MERGE_TRACES needs trace rows (gysk_config.max_trace_svcs > 0)");
 
 	int ndev = 0;
 	cudaError_t ce = cudaGetDeviceCount(&ndev);

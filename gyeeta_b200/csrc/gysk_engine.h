@@ -89,6 +89,17 @@ struct HostTaskTopn
 
 // one logical service's t-digest in the merge step: fixed size, so that the slabs all-gather as bytes
 struct SlabEntry { TdHead head; Centroid cent[TD_CAP]; };
+// GYSK_FLAG_MERGE_TRACES: one logical service's trace digest (compression TRACE_TD_DELTA keeps at most TRACE_TD_CAP centroids)
+struct TraceSlab { TdHead head; Centroid cent[TRACE_TD_CAP]; };
+static_assert(sizeof(TraceSlab) == 1632 && sizeof(TraceSlab) % 16 == 0, "TraceSlab: 32-byte head, 100 centroids");
+// the trace digests of nl logical services in whole SlabEntrys, packed after the rank's digests and top-N candidates
+inline uint32_t trace_slab_entries(uint32_t nl) { return (uint32_t)(((size_t)nl * sizeof(TraceSlab) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry)); }
+// u64 SUM words of one logical service's merged trace window: the sums of gysk_trace_window in its order, then the members holding a row
+enum { LT_NREQ = 0, LT_NERR, LT_NCONNS, LT_SUM_US, LT_BYTES_IN, LT_BYTES_OUT, LT_BKT /* 8 words */, LT_TD_COUNT = LT_BKT + 8, LT_NTRACED,
+	LT_WORDS };
+// i64 MAX words: max_resp_us, max_bytes_in, max_bytes_out
+enum { LT_MAX_US = 0, LT_MAX_IN, LT_MAX_OUT, LT_MAX_WORDS };
+static_assert(LT_WORDS == 16, "15 sums and ntraced");
 
 // LISTEN_SUMM_STATS words of one logical service: the 15 int32 fields of gysk_host_summary before its pad, nstates[0..7] first
 constexpr int STATE_WORDS = 15;
@@ -112,6 +123,11 @@ struct LogicalArrays
 	uint8_t			*hll {nullptr};				// MAX [nl][1 << hll_p]
 	SlabEntry		*slab {nullptr};			// [nl] this engine's folded digests
 	SlabEntry		*final_slab {nullptr};			// [nl] merged over ranks
+	// GYSK_FLAG_MERGE_TRACES (nullptr without): the members' last trace windows
+	unsigned long long	*traces {nullptr};			// SUM [nl][LT_WORDS]
+	long long		*trace_max {nullptr};			// MAX [nl][LT_MAX_WORDS]
+	TraceSlab		*trace_slab {nullptr};			// [nl] this engine's folded trace digests, inside the slab (MergeState::trace_off)
+	TraceSlab		*trace_final {nullptr};			// [nl] merged over ranks
 
 	// histogram `which` (GYSK_HIST_RESP_LAST, _ALL, _5MIN or _5DAY) of logical service l: its cells 0..14 and its max_val_seen_
 	struct Hist { HistCell *cells; long long *max; };
@@ -140,6 +156,8 @@ struct LogicalArrays
 		return (uint32_t)(w[GYSK_STATE_BAD] + w[GYSK_STATE_SEVERE] + w[GYSK_STATE_DOWN]);
 	}
 	__host__ __device__ __forceinline__ uint8_t *hll_of(uint32_t l, uint32_t hll_p) const { return hll + ((size_t)l << hll_p); }
+	__host__ __device__ __forceinline__ unsigned long long *traces_of(uint32_t l) const { return traces + LT_WORDS * (size_t)l; }
+	__host__ __device__ __forceinline__ long long *trace_max_of(uint32_t l) const { return trace_max + LT_MAX_WORDS * (size_t)l; }
 };
 
 // The members of each logical service on this GPU, CSR in map order: slots[offs[l] .. offs[l + 1]) are logical l's. A member whose id
@@ -234,8 +252,9 @@ struct MergeState
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
 	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min], hist last/all, conn [, levels, aux] [, states]
-									//           [, clusters]
+									//           [, clusters] [, traces]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt] [, flush tsec]
+									//           [, trace max]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	std::string		name_sum, name_maxi64, name_maxu8;	// the regions' gysk_buffer_desc names: their arrays, in order
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
@@ -248,8 +267,10 @@ struct MergeState
 	bool			comm_owned {false};
 	SlabEntry		*gathered {nullptr};			// [world] slabs, target of the all-gather
 	uint32_t		gathered_world {0};
-	// GYSK_FLAG_MERGE_TOPN: lg.slab holds slab_entries = nl + TOPN_SLAB_ENTRIES (nl without the flag), the candidates from lg.slab + nl
+	// GYSK_FLAG_MERGE_TOPN: lg.slab holds slab_entries = nl + TOPN_SLAB_ENTRIES (nl without the flag), the candidates from lg.slab + nl;
+	// GYSK_FLAG_MERGE_TRACES: trace_slab_entries(nl) more from lg.slab + trace_off, the trace digests
 	uint32_t		slab_entries {0};
+	uint32_t		trace_off {0};
 	unsigned long long	*topn_slots {nullptr};			// [TOPN_LISTS][TOPN_K] this rank's candidate slots (the rows' input)
 	uint8_t			*topn_final {nullptr};			// TopnLists::BYTES: the winners of the last finished merge
 };
@@ -456,6 +477,8 @@ static_assert(QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES && 64 * sizeof(gysk_
 static_assert(sizeof(SlabEntry) <= STAGE_BYTES, "the stage holds one merged digest");
 static_assert(sizeof(gysk_logical_state) == 80 && sizeof(gysk_logical_state) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS state rows");
 static_assert(sizeof(gysk_cluster_row) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS cluster rows");
+static_assert(sizeof(gysk_logical_trace) == 168 && sizeof(gysk_logical_trace) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS logical trace rows");
+static_assert(sizeof(TraceSlab) <= STAGE_BYTES, "the stage holds one merged trace digest");
 
 // A staged read, engine mutex held. The optional input (ids, flow keys or logical indices) travels through h_qids / d_qids in pieces
 // of `piece` entries; without one (the window reads) the pieces only cut the n rows. For each piece, launch(d_in, off, m) writes m

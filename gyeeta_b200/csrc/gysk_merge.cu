@@ -209,14 +209,67 @@ __global__ void fold_hll_kernel(DevState st, Members mb, LogicalArrays lg)
 	reinterpret_cast<uint32_t *>(lg.hll_of(l, st.hll_p))[w] = acc;
 }
 
+// GYSK_FLAG_MERGE_TRACES, one thread per (logical, word): words 0 .. LT_TD_COUNT sum the members' last closed trace windows (the half
+// par ^ 1 of the row a member slot holds; a slot without a row, or whose row is being taken, adds nothing), the LT_NTRACED thread counts
+// those rows and takes the three maxima.
+__global__ void fold_traces_kernel(DevState st, Members mb, LogicalArrays lg)
+{
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= (uint64_t)lg.nl * LT_WORDS) return;
+	const uint32_t l = (uint32_t)(i / LT_WORDS);
+	const int k = (int)(i % LT_WORDS);
+	const TraceTable &tr = st.trace;
+	const uint32_t half = tr.par ^ 1u;
+	// the row word of LT_NREQ .. LT_BYTES_OUT, 8 bits apiece; the buckets follow in both layouts
+	constexpr unsigned long long SRC = (unsigned long long)TW_NREQ | (unsigned long long)TW_NERR << 8 | (unsigned long long)TW_NCONNS << 16 |
+		(unsigned long long)TW_SUM_US << 24 | (unsigned long long)TW_BYTES_IN << 32 | (unsigned long long)TW_BYTES_OUT << 40;
+	const int src = k < LT_BKT ? (int)((SRC >> (8 * k)) & 0xFF) : TW_BKT + (k - LT_BKT);
+	unsigned long long acc = 0;
+	long long mx[LT_MAX_WORDS] = {0, 0, 0};
+
+	mb.each(l, [&](uint32_t s) {
+		const uint32_t r1 = tr.row_of[s];
+		if (r1 == 0 || r1 == TRACE_BUSY) return;
+		const uint32_t r = r1 - 1u;
+		if (k == LT_TD_COUNT) acc += tr.hd(half, r)->total;
+		else if (k == LT_NTRACED) {
+			const unsigned long long *w = tr.words(half, r);
+			acc++;
+			mx[LT_MAX_US] = max(mx[LT_MAX_US], (long long)w[TW_MAX_US]);
+			mx[LT_MAX_IN] = max(mx[LT_MAX_IN], (long long)w[TW_MAX_IN]);
+			mx[LT_MAX_OUT] = max(mx[LT_MAX_OUT], (long long)w[TW_MAX_OUT]);
+		}
+		else acc += tr.words(half, r)[src];
+	});
+	lg.traces_of(l)[k] = acc;
+	if (k == LT_NTRACED) {
+		long long *m = lg.trace_max_of(l);
+		m[LT_MAX_US] = mx[LT_MAX_US]; m[LT_MAX_IN] = mx[LT_MAX_IN]; m[LT_MAX_OUT] = mx[LT_MAX_OUT];
+	}
+}
+
 static constexpr int MG_WARPS = 2;		// 2 x 17.8 KB of scratch: static shared memory
 
-// One warp folds the digests digest(b) .. digest(e - 1) into out, one after the other: each non-empty one is merged into the
-// accumulator and compressed (warp_merge_compress), its total, min and max added. digest(i) gives {head, centroids}, head nullptr
-// for an entry to skip.
-struct DigestRef { const TdHead *head; const Centroid *cent; };
-template <typename Digest>
-__device__ __forceinline__ void fold_digests(TdScratch &S, const TdParams &P, uint32_t b, uint32_t e, Digest digest, SlabEntry &out, int lane)
+// One warp folds the digests digest(b) .. digest(e - 1) into {out_head, out_cent[CAP]}, one after the other: each non-empty one is
+// merged into the accumulator and compressed (warp_merge_compress), its total, min and max added. digest(i) gives {n, total, min, max,
+// centroids}, n = 0 for an entry to skip.
+struct DigestRef { uint32_t n; unsigned long long total; double minv, maxv; const Centroid *cent; };
+__device__ __forceinline__ DigestRef digest_ref(const TdHead &h, const Centroid *c) { return DigestRef {h.n, h.total, h.minv, h.maxv, c}; }
+__device__ __forceinline__ DigestRef no_digest() { return DigestRef {0, 0, 0.0, 0.0, nullptr}; }
+// the last closed window's digest of the trace row a service slot holds; a trace digest's extremes are counter words of its window
+__device__ __forceinline__ DigestRef trace_digest(const TraceTable &tr, uint32_t slot)
+{
+	const uint32_t r1 = tr.row_of[slot];
+	if (r1 == 0 || r1 == TRACE_BUSY) return no_digest();
+	const uint32_t r = r1 - 1u, half = tr.par ^ 1u;
+	const TdHead h = *tr.hd(half, r);
+	const unsigned long long *w = tr.words(half, r);
+	return DigestRef {h.n, h.total, (double)(0xFFFFFFFFu - (uint32_t)w[TW_TD_NMIN]), (double)w[TW_TD_MAX], tr.cents(half, r)};
+}
+
+template <int CAP, typename Digest>
+__device__ __forceinline__ void fold_digests(TdScratch &S, const TdParams &P, uint32_t b, uint32_t e, Digest digest, TdHead &out_head,
+		Centroid *out_cent, int lane)
 {
 	uint32_t nacc = 0;
 	unsigned long long total = 0;
@@ -224,41 +277,54 @@ __device__ __forceinline__ void fold_digests(TdScratch &S, const TdParams &P, ui
 
 	for (uint32_t i = b; i < e; ++i) {
 		const DigestRef d = digest(i);
-		if (!d.head || !d.head->n) continue;
-		nacc = warp_merge_compress(S, S.newc, nacc, d.cent, d.head->n, S.newc, P);
-		total += d.head->total; mn = fmin(mn, d.head->minv); mx = fmax(mx, d.head->maxv);
+		if (!d.n) continue;
+		nacc = warp_merge_compress(S, S.newc, nacc, d.cent, d.n, S.newc, P);
+		total += d.total; mn = fmin(mn, d.minv); mx = fmax(mx, d.maxv);
 	}
-	for (uint32_t c = lane; c < TD_CAP; c += 32) out.cent[c] = c < nacc ? S.newc[c] : Centroid {0.0, 0};
-	if (lane == 0) { TdHead h; h.total = total; h.minv = mn; h.maxv = mx; h.n = nacc; h.pad = 0; out.head = h; }
+	for (uint32_t c = lane; c < (uint32_t)CAP; c += 32) out_cent[c] = c < nacc ? S.newc[c] : Centroid {0.0, 0};
+	if (lane == 0) { TdHead h; h.total = total; h.minv = mn; h.maxv = mx; h.n = nacc; h.pad = 0; out_head = h; }
 	__syncwarp();
 }
 
-// one warp per logical service: its members' digests in map order
+// one warp per logical service: its members' digests in map order; with GYSK_FLAG_MERGE_TRACES (lg.trace_slab) then their last trace
+// windows' digests, in map order at the trace rows' compression
 __global__ void __launch_bounds__(MG_WARPS * 32) fold_td_kernel(DevState st, Members mb, LogicalArrays lg)
 {
 	__shared__ TdScratch scratch[MG_WARPS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 
-	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS)
-		fold_digests(scratch[wid], st.td, mb.offs[l], mb.offs[l + 1], [&](uint32_t m) {
+	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS) {
+		fold_digests<TD_CAP>(scratch[wid], st.td, mb.offs[l], mb.offs[l + 1], [&](uint32_t m) {
 			const uint32_t s = mb.slots[m];
-			return s == mb.null_slot ? DigestRef {nullptr, nullptr} : DigestRef {st.td_head + s, st.td_cent + (size_t)s * TD_CAP};
-		}, lg.slab[l], lane);
+			return s == mb.null_slot ? no_digest() : digest_ref(st.td_head[s], st.td_cent + (size_t)s * TD_CAP);
+		}, lg.slab[l].head, lg.slab[l].cent, lane);
+		if (lg.trace_slab)
+			fold_digests<TRACE_TD_CAP>(scratch[wid], st.trace.td, mb.offs[l], mb.offs[l + 1], [&](uint32_t m) {
+				const uint32_t s = mb.slots[m];
+				return s == mb.null_slot ? no_digest() : trace_digest(st.trace, s);
+			}, lg.trace_slab[l].head, lg.trace_slab[l].cent, lane);
+	}
 }
 
-// one warp per logical service over the all-gathered slabs [world][stride] (each rank's nl digests first), in rank-ascending order =>
-// deterministic result
+// one warp per logical service over the all-gathered slabs [world][stride] (each rank's nl digests first, its trace digests from entry
+// trace_off), in rank-ascending order => deterministic result
 __global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, uint32_t stride, LogicalArrays lg,
-		TdParams P)
+		TdParams P, uint32_t trace_off, TdParams PT)
 {
 	__shared__ TdScratch scratch[MG_WARPS];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 
-	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS)
-		fold_digests(scratch[wid], P, 0, world, [&](uint32_t r) {
+	for (uint32_t l = blockIdx.x * MG_WARPS + wid; l < lg.nl; l += gridDim.x * MG_WARPS) {
+		fold_digests<TD_CAP>(scratch[wid], P, 0, world, [&](uint32_t r) {
 			const SlabEntry &g = gathered[(size_t)r * stride + l];
-			return DigestRef {&g.head, g.cent};
-		}, lg.final_slab[l], lane);
+			return digest_ref(g.head, g.cent);
+		}, lg.final_slab[l].head, lg.final_slab[l].cent, lane);
+		if (lg.trace_final)
+			fold_digests<TRACE_TD_CAP>(scratch[wid], PT, 0, world, [&](uint32_t r) {
+				const TraceSlab &g = reinterpret_cast<const TraceSlab *>(gathered + (size_t)r * stride + trace_off)[l];
+				return digest_ref(g.head, g.cent);
+			}, lg.trace_final[l].head, lg.trace_final[l].cent, lane);
+	}
 }
 
 // GYSK_FLAG_MERGE_TOPN, one CTA per list m, one thread per candidate of the gathered slabs (rank r's lists at gathered + r * stride + nl,
@@ -359,6 +425,8 @@ __device__ __forceinline__ bool logical_active(const LogicalArrays &lg, uint32_t
 // the GYSK_WINDOW_ACTIVE_ONLY rule of each all-rows read: a logical service as logical_active, a cluster with a live service on some rank
 struct LogicalActive { LogicalArrays lg; __device__ __forceinline__ bool operator()(uint32_t l) const { return logical_active(lg, l); } };
 struct ClusterActive { Clusters cl; __device__ __forceinline__ bool operator()(uint32_t c) const { return (uint32_t)cl.words_of(c)[3] != 0; } };
+// ... and a logical service whose merged trace window holds requests
+struct TraceActive { LogicalArrays lg; __device__ __forceinline__ bool operator()(uint32_t l) const { return lg.traces_of(l)[LT_NREQ] != 0; } };
 
 // One CTA walks the n dense indices of `sorted` (ascending id) and keeps the active ones, in order: tile_rank places the kept entries
 // of each 1024-entry tile. *d_n = entries kept.
@@ -439,6 +507,34 @@ __global__ void cluster_row_kernel(const int32_t *__restrict__ cidx, uint32_t n,
 	out[q] = o;
 }
 
+// GYSK_FLAG_MERGE_TRACES read side, one thread per row: the merged trace window of dense index lidx[q], logical id lids[l], p99 from the
+// merged digest (NaN while it is empty, as trace_window_out); an index of -1 gives an all-zero row
+__global__ void logical_trace_kernel(const int32_t *__restrict__ lidx, uint32_t n, LogicalArrays lg, const unsigned long long *__restrict__ lids,
+		gysk_logical_trace *__restrict__ out)
+{
+	const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+	if (q >= n) return;
+	const int32_t l = lidx[q];
+	gysk_logical_trace o;
+	memset(&o, 0, sizeof(o));
+	if (l >= 0) {
+		const unsigned long long *w = lg.traces_of((uint32_t)l);
+		const long long *m = lg.trace_max_of((uint32_t)l);
+		const TraceSlab &d = lg.trace_final[l];
+		gysk_trace_window &t = o.last;
+		o.logical_id = lids[l]; o.found = 1; o.ntraced = (uint32_t)w[LT_NTRACED];
+		t.nreq = w[LT_NREQ]; t.nerr = w[LT_NERR]; t.nconns = w[LT_NCONNS]; t.sum_resp_us = w[LT_SUM_US];
+		t.max_resp_us = (unsigned long long)m[LT_MAX_US];
+		t.bytes_in = w[LT_BYTES_IN]; t.bytes_out = w[LT_BYTES_OUT];
+		t.max_bytes_in = (unsigned long long)m[LT_MAX_IN]; t.max_bytes_out = (unsigned long long)m[LT_MAX_OUT];
+		for (int b = 0; b < 8; ++b) t.resp_buckets[b] = w[LT_BKT + b];
+		t.td_count = w[LT_TD_COUNT];
+		const TdHead h = d.head;
+		t.p99_resp_us = h.n ? td_quantile_seq(TdCentroids {d.cent}, h.n, h.minv, h.maxv, 0.99) : (double)NAN;
+	}
+	out[q] = o;
+}
+
 } // namespace gysk
 
 namespace {
@@ -478,6 +574,10 @@ void launch_select(gysk_engine *e, const gysk_cluster_row *, unsigned long long 
 	const ClusterMap &cm = e->mg.clusters;
 	logical_select_kernel<<<1, 1024, 0, e->stream>>>(cm.d_sorted, cm.cl.nc, ClusterActive {cm.cl}, cm.d_sel, d_n);
 }
+void launch_select(gysk_engine *e, const gysk_logical_trace *, unsigned long long *d_n)
+{
+	logical_select_kernel<<<1, 1024, 0, e->stream>>>(e->mg.d_sorted, e->mg.lg.nl, TraceActive {e->mg.lg}, e->mg.d_sel, d_n);
+}
 
 // Per row type of the logical and cluster reads: the launch that makes the rows of the dense indices lidx[0 .. m) in the device stage
 // (an index of -1 gives the not-found row), the finish that copies them out, the field a by-id read stamps with the queried id, and the
@@ -498,15 +598,23 @@ int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_cluster
 	cluster_row_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(lidx, m, e->mg.clusters.cl, e->mg.clusters.d_ids, reinterpret_cast<gysk_cluster_row *>(e->d_wstage));
 	return 1;
 }
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical_trace *)
+{
+	logical_trace_kernel<<<div_up(m, 128), 128, 0, e->stream>>>(lidx, m, e->mg.lg, e->mg.d_logical_ids, reinterpret_cast<gysk_logical_trace *>(e->d_wstage));
+	return 1;
+}
 SvcRows logical_finish(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
 CopyRows<gysk_logical_state> logical_finish(const gysk_engine *, gysk_logical_state *out) { return CopyRows<gysk_logical_state> {out}; }
 CopyRows<gysk_cluster_row> logical_finish(const gysk_engine *, gysk_cluster_row *out) { return CopyRows<gysk_cluster_row> {out}; }
+CopyRows<gysk_logical_trace> logical_finish(const gysk_engine *, gysk_logical_trace *out) { return CopyRows<gysk_logical_trace> {out}; }
 uint64_t &row_id(gysk_svc_summary &r) { return r.glob_id; }
 uint64_t &row_id(gysk_logical_state &r) { return r.logical_id; }
 uint64_t &row_id(gysk_cluster_row &r) { return r.cluster_id; }
+uint64_t &row_id(gysk_logical_trace &r) { return r.logical_id; }
 template <typename Row> constexpr uint32_t logical_flag()
 {
-	return std::is_same<Row, gysk_logical_state>::value ? GYSK_FLAG_MERGE_STATES : std::is_same<Row, gysk_cluster_row>::value ? GYSK_FLAG_MERGE_CLUSTERS : 0;
+	return std::is_same<Row, gysk_logical_state>::value ? GYSK_FLAG_MERGE_STATES : std::is_same<Row, gysk_cluster_row>::value ? GYSK_FLAG_MERGE_CLUSTERS :
+		std::is_same<Row, gysk_logical_trace>::value ? GYSK_FLAG_MERGE_TRACES : 0;
 }
 
 // gysk_query_logical / gysk_query_logical_states / gysk_query_cluster_states: the rows of n ids, in QCHUNK pieces, each row carrying its
@@ -706,9 +814,10 @@ int lay_out_arena(gysk_engine *e)
 	// name joins its region's gysk_merge_buffers name. GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX
 	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those.
 	// GYSK_FLAG_FLOW_LEVEL puts the count-min level after the two window tables, and needs the flush tsec pair as the levels do:
-	// still three regions, three collectives.
+	// still three regions, three collectives. GYSK_FLAG_MERGE_TRACES puts its words at the end of the SUM region, its maxima at the end of
+	// the i64 MAX one, and needs the flush tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
-	const bool flow_level = e->cfg.flags & GYSK_FLAG_FLOW_LEVEL;
+	const bool flow_level = e->cfg.flags & GYSK_FLAG_FLOW_LEVEL, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
@@ -725,13 +834,15 @@ int lay_out_arena(gysk_engine *e)
 		if (levels) { take(lg.lvl, NLEVELS * b_hist, "levels"); take(lg.aux, (size_t)nl * 4 * 8, "aux"); }
 		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8, "states");
 		if (clusters) take(mg.clusters.cl.words, (size_t)mg.clusters.cl.nc * CLUSTER_WORDS * 8, "clusters");
+		if (traces) take(lg.traces, (size_t)nl * LT_WORDS * 8, "traces");
 		mg.bytes_sum = off - mg.off_sum;
 		mg.name_sum = "sum_u64: " + names;
 		names.clear();
 		mg.off_maxi64 = off;
 		take(lg.hmax, (size_t)nl * 2 * 8, "hist max_val_seen");
 		if (levels) { take(lg.lvl_max, (size_t)nl * NLEVELS * 8, "level max_val_seen"); take(lg.rtt, (size_t)nl * 8, "rtt"); }
-		if (levels || flow_level) take(lg.flush, 2 * 8, "flush tsec");
+		if (levels || flow_level || traces) take(lg.flush, 2 * 8, "flush tsec");
+		if (traces) take(lg.trace_max, (size_t)nl * LT_MAX_WORDS * 8, "trace max");
 		mg.bytes_maxi64 = off - mg.off_maxi64;
 		mg.name_maxi64 = "max_i64: " + names;
 		names.clear();
@@ -762,7 +873,7 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 
 	// (re)allocate the arena
 	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
-	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel); dfree(e, mg.topn_slots); dfree(e, mg.topn_final);
+	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel); dfree(e, mg.topn_slots); dfree(e, mg.topn_final); dfree(e, mg.lg.trace_final);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
@@ -778,13 +889,19 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	lg.nl = nl;
 	int rc = lay_out_arena(e);
 	if (rc) return rc;
-	// GYSK_FLAG_MERGE_TOPN: the candidates after the digests, in whole SlabEntrys, so the slab stays one all-gather
-	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN;
-	mg.slab_entries = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
+	// GYSK_FLAG_MERGE_TOPN: the candidates after the digests, in whole SlabEntrys, so the slab stays one all-gather; GYSK_FLAG_MERGE_TRACES:
+	// the trace digests after them, packed as TraceSlabs in whole SlabEntrys
+	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
+	mg.trace_off = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
+	mg.slab_entries = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
 	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
 	if (topn) {
 		if ((rc = dalloc(e, &mg.topn_slots, (size_t)TOPN_LISTS * TOPN_K))) return rc;
 		if ((rc = dalloc(e, &mg.topn_final, TopnLists::BYTES))) return rc;
+	}
+	if (traces) {
+		lg.trace_slab = reinterpret_cast<TraceSlab *>(lg.slab + mg.trace_off);
+		if ((rc = dalloc(e, &lg.trace_final, nl ? nl : 1))) return rc;
 	}
 	if ((rc = dalloc(e, &lg.final_slab, nl ? nl : 1))) return rc;
 	if ((rc = dalloc(e, &mg.members.offs, (size_t)nl + 1))) return rc;
@@ -896,10 +1013,14 @@ int gysk_merge_prepare(gysk_engine *e)
 			fold_states_kernel<<<div_up(nl, 256), 256, 0, e->stream>>>(e->st, mg.members, mg.lg);
 			e->kernel_launches++;
 		}
+		if (mg.lg.traces) {		// GYSK_FLAG_MERGE_TRACES: the counter words (the digests are in fold_td_kernel's pass)
+			fold_traces_kernel<<<div_up((uint64_t)nl * LT_WORDS, 256), 256, 0, e->stream>>>(e->st, mg.members, mg.lg);
+			e->kernel_launches++;
+		}
 	}
-	if (mg.lg.flush) {		// GYSK_FLAG_MERGE_LEVELS or GYSK_FLAG_FLOW_LEVEL: also with no logical service, for the flush tsec pair
+	if (mg.lg.flush) {		// GYSK_FLAG_MERGE_LEVELS, GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_MERGE_TRACES: also with no logical service, for the flush tsec pair
 		LogicalArrays lg = mg.lg;
-		if (!lg.lvl) lg.nl = 0;		// GYSK_FLAG_FLOW_LEVEL alone: the pair only
+		if (!lg.lvl) lg.nl = 0;		// without GYSK_FLAG_MERGE_LEVELS: the pair only
 		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)lg.nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.members,
 				(long long)e->last_flush_tsec, lg);
 		e->kernel_launches++;
@@ -968,7 +1089,7 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 	if (!d_gathered) world = 1;
 	if (mg.lg.nl) {
 		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.lg.nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.slab_entries, mg.lg,
-				e->st.td);
+				e->st.td, mg.trace_off, e->st.trace.td);
 		e->kernel_launches++;
 	}
 	if (mg.topn_final) {		// GYSK_FLAG_MERGE_TOPN
@@ -1012,6 +1133,46 @@ int gysk_query_cluster_states(gysk_engine *e, const uint64_t *cluster_ids, uint3
 int gysk_query_cluster_states_all(gysk_engine *e, uint32_t flags, gysk_cluster_row *out, uint32_t cap, uint32_t *n)
 {
 	return logical_all_rows(e, flags, out, cap, n, "query_cluster_states_all");
+}
+
+// GYSK_FLAG_MERGE_TRACES: the members' last trace windows merged, rows made on the device (logical_trace_kernel)
+int gysk_query_logical_traces(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_logical_trace *out)
+{
+	return logical_query_rows(e, logical_ids, n, out, "query_logical_traces");
+}
+
+// GYSK_FLAG_MERGE_TRACES: every logical service's trace row, in the order of gysk_query_logical_all
+int gysk_query_logical_traces_all(gysk_engine *e, uint32_t flags, gysk_logical_trace *out, uint32_t cap, uint32_t *n)
+{
+	return logical_all_rows(e, flags, out, cap, n, "query_logical_traces_all");
+}
+
+// GYSK_FLAG_MERGE_TRACES: the merged trace digest of one logical service, with the contract of gysk_export_logical_tdigest
+int gysk_export_logical_trace_tdigest(gysk_engine *e, uint64_t logical_id, double *means, uint64_t *weights, uint32_t cap, uint32_t *n,
+		double *minv, double *maxv)
+{
+	CHECK_ENGINE(e);
+	if (!means || !weights || !n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_MERGE_TRACES)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_export_logical_trace_tdigest: no finished merge");
+	const int32_t l = logical_index(mg, logical_id);
+	if (l < 0) return GYSK_ERR_NOENT;
+	CU(e, cudaMemcpyAsync(e->h_wstage, mg.lg.trace_final + l, sizeof(TraceSlab), cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	const TraceSlab &s = *reinterpret_cast<const TraceSlab *>(e->h_wstage);
+	return tdigest_out(s.head, s.cent, means, weights, cap, n, minv, maxv);
+}
+
+int gysk_export_logical_trace_tdigest_pgtext(gysk_engine *e, uint64_t logical_id, char *buf, uint32_t cap)
+{
+	double means[TRACE_TD_CAP], mn, mx;
+	uint64_t weights[TRACE_TD_CAP];
+	uint32_t n = 0;
+	int rc = gysk_export_logical_trace_tdigest(e, logical_id, means, weights, TRACE_TD_CAP, &n, &mn, &mx);
+	if (rc) return rc;
+	return gysk_tdigest_to_pgtext(means, weights, n, TRACE_TD_DELTA, buf, cap);		// at compression 100 already: no recompress
 }
 
 int gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS], uint64_t *total,
@@ -1116,7 +1277,7 @@ int gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tse
 {
 	CHECK_ENGINE(e);
 	if (!min_tsec || !max_tsec) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & (GYSK_FLAG_MERGE_LEVELS | GYSK_FLAG_FLOW_LEVEL))) return GYSK_ERR_NOTSUP;
+	if (!(e->cfg.flags & (GYSK_FLAG_MERGE_LEVELS | GYSK_FLAG_FLOW_LEVEL | GYSK_FLAG_MERGE_TRACES))) return GYSK_ERR_NOTSUP;
 	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_merge_flush_range: no finished merge");

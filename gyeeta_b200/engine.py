@@ -33,6 +33,7 @@ NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CO
 (HOSTTOP_SVC_ISSUE, HOSTTOP_SVC_QPS, HOSTTOP_SVC_CONNS, HOSTTOP_SVC_NET, HOSTTOP_TASK_ISSUE, HOSTTOP_TASK_NET, HOSTTOP_TASK_CPU, HOSTTOP_TASK_RSS,
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
 FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, FLAG_MERGE_TOPN, FLAG_FLOW_LEVEL = 1, 2, 4, 8, 16, 32
+FLAG_MERGE_TRACES = 64
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
@@ -290,6 +291,10 @@ def load_library(path=None):
         "gysk_export_logical_hll": (i32, [vp, u64, vp]),
         "gysk_query_logical_states": (i32, [vp, vp, u32, vp]),
         "gysk_query_logical_states_all": (i32, [vp, u32, vp, u32, vp]),
+        "gysk_query_logical_traces": (i32, [vp, vp, u32, vp]),
+        "gysk_query_logical_traces_all": (i32, [vp, u32, vp, u32, vp]),
+        "gysk_export_logical_trace_tdigest": (i32, [vp, u64, vp, vp, u32, vp, vp, vp]),
+        "gysk_export_logical_trace_tdigest_pgtext": (i32, [vp, u64, vp, u32]),
         "gysk_set_cluster_map": (i32, [vp, vp, vp, u32]),
         "gysk_query_cluster_states": (i32, [vp, vp, u32, vp]),
         "gysk_query_cluster_states_all": (i32, [vp, u32, vp, u32, vp]),
@@ -342,7 +347,17 @@ class TraceRow(C.Structure):
         return {"glob_id": self.glob_id, "found": self.found, "host_idx": self.host_idx, "cur": self.cur.asdict(), "last": self.last.asdict()}
 
 
-assert C.sizeof(TraceWindow) == 152 and C.sizeof(TraceRow) == 320
+
+
+class LogicalTrace(C.Structure):
+    """gysk_logical_trace: the members' last closed trace windows of one logical service, merged over every rank (GYSK_FLAG_MERGE_TRACES)"""
+    _fields_ = [("logical_id", C.c_uint64), ("found", C.c_int32), ("ntraced", C.c_uint32), ("last", TraceWindow)]
+
+    def asdict(self):
+        return {"logical_id": self.logical_id, "found": self.found, "ntraced": self.ntraced, "last": self.last.asdict()}
+
+
+assert C.sizeof(TraceWindow) == 152 and C.sizeof(TraceRow) == 320 and C.sizeof(LogicalTrace) == 168
 TRACE_TD_CAP = 100
 EV_TRACE = 8
 EVF_TRACE_ERROR, EVF_TRACE_NEWCONN = 0x1, 0x2
@@ -354,7 +369,7 @@ class Engine:
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
-                 max_trace_svcs=0):
+                 max_trace_svcs=0, merge_traces=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -367,7 +382,7 @@ class Engine:
         cfg.max_trace_svcs = max_trace_svcs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
-                    (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0)
+                    (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -859,6 +874,32 @@ class Engine:
     def query_logical_states_all(self, active_only=False, cap=None):
         """gysk_query_logical_states_all: (LogicalState rows in ascending logical id, number of matching rows); cap as query_logical_all"""
         return self._window(self.L.gysk_query_logical_states_all, LogicalState, (), active_only, cap)
+
+    def query_logical_traces(self, ids):
+        """gysk_query_logical_traces: LogicalTrace rows of logical ids from the last merge (merge_traces=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (LogicalTrace * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_logical_traces(self.h, _p(ids), len(ids), out))
+        return out[: len(ids)]
+
+    def query_logical_traces_all(self, active_only=False, cap=None):
+        """gysk_query_logical_traces_all: (LogicalTrace rows in ascending logical id, number of matching rows); cap as query_logical_all"""
+        return self._window(self.L.gysk_query_logical_traces_all, LogicalTrace, (), active_only, cap)
+
+    def export_logical_trace_tdigest(self, logical_id):
+        """(means, weights, min, max) of a logical service's merged trace digest; None for an id the map does not have"""
+        means = np.zeros(TRACE_TD_CAP, dtype=np.float64)
+        weights = np.zeros(TRACE_TD_CAP, dtype=np.uint64)
+        n, mn, mx = C.c_uint32(), C.c_double(), C.c_double()
+        rc = self.L.gysk_export_logical_trace_tdigest(self.h, int(logical_id), _p(means), _p(weights), TRACE_TD_CAP, C.byref(n), C.byref(mn),
+                                                      C.byref(mx))
+        if rc == -2:
+            return None
+        self._chk(rc)
+        return means[: n.value].copy(), weights[: n.value].copy(), mn.value, mx.value
+
+    def export_logical_trace_tdigest_pgtext(self, logical_id):
+        return self._pgtext(self.L.gysk_export_logical_trace_tdigest_pgtext, logical_id)
 
     def query_cluster_states(self, ids):
         """gysk_query_cluster_states: ClusterRow rows of cluster ids from the last merge (merge_clusters=True)"""

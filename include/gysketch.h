@@ -219,6 +219,11 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   level across ranks (gysk_query_flows_global_5min; the same flags on every rank).
 						   Costs NSLOTS + 1 = 11 more tables of depth << log2_width cells. Without it nothing is
 						   allocated, every other call answers as before and the three calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_MERGE_TRACES		0x40u	/* the merge step also merges the members' last closed trace windows into each logical
+						   service (gysk_query_logical_traces, "request traces of logical services" below); combines
+						   freely with the flags above, the same flags on every rank. Needs trace rows: gysk_create
+						   refuses it with max_trace_svcs == 0. Without it the merge arena, slab and collectives are
+						   as before */
 
 typedef struct gysk_config
 {
@@ -737,9 +742,10 @@ int		gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n,
  * GYSK_ERR_INVAL before a finished merge or for another `which`. */
 int		gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS],
 				uint64_t *total_count, int64_t *max_val);
-/* The earliest and latest tsec of the ranks' last gysk_flush, as all-reduced by the last finished merge (GYSK_FLAG_MERGE_LEVELS or
- * GYSK_FLAG_FLOW_LEVEL; GYSK_ERR_NOTSUP without both, GYSK_ERR_INVAL before a finished merge). Each rank's level slots are relative to its own last
- * flush, so *min_tsec != *max_tsec means the ranks had closed different windows and the merged levels mix them. That is not an
+/* The earliest and latest tsec of the ranks' last gysk_flush, as all-reduced by the last finished merge (GYSK_FLAG_MERGE_LEVELS,
+ * GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_MERGE_TRACES; GYSK_ERR_NOTSUP without all three, GYSK_ERR_INVAL before a finished merge). Each rank's
+ * level slots and last trace window are relative to its own last flush, so *min_tsec != *max_tsec means the ranks had closed different
+ * windows and the merged levels or trace windows mix them. That is not an
  * error: the collectives cannot fail on one rank alone, so the caller decides what to do with such an answer. */
 int		gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tsec);
 
@@ -787,6 +793,35 @@ typedef struct gysk_logical_state
 int		gysk_query_logical_states(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_logical_state *out);
 /* one row per logical service: the ids, order, GYSK_WINDOW_ACTIVE_ONLY set and count / capacity rules of gysk_query_logical_all */
 int		gysk_query_logical_states_all(gysk_engine *e, uint32_t flags, gysk_logical_state *out, uint32_t cap, uint32_t *n);
+
+/* ---- request traces of logical services (GYSK_FLAG_MERGE_TRACES): the trace view of each logical service's last window ----
+ * Each member service that holds a slot and a trace row on a rank adds the last closed window of its row (the `last` of its
+ * gysk_query_traces row); members without a row add nothing. Over members and ranks:
+ *   nreq, nerr, nconns, sum_resp_us, bytes_in, bytes_out, resp_buckets[8] and td_count are sums;
+ *   max_resp_us, max_bytes_in and max_bytes_out are maxima;
+ *   the digest is the members' window digests merged in map order on each rank, then the ranks' in ascending rank, at compression 100;
+ *   p99_resp_us is its 0.99 quantile (the rule of gysk_tdigest_quantile), NaN when it is empty.
+ * Integer fields are exact at any GPU count. Each rank folds its own last closed window: gysk_merge_flush_range tells whether every rank
+ * had closed the same one. The layout of the merge buffers depends only on the flags and the logical map, not on max_trace_svcs. */
+typedef struct gysk_logical_trace
+{
+	uint64_t		logical_id;
+	int32_t			found;		/* 1 for a mapped logical id, as gysk_query_logical_states; 0: not in the map (all zero) */
+	uint32_t		ntraced;	/* member services holding a trace row, summed over the ranks */
+	gysk_trace_window	last;		/* the members' last closed windows merged */
+} gysk_logical_trace;			/* 168 bytes */
+/* by id, from the last finished merge. GYSK_ERR_NOTSUP without GYSK_FLAG_MERGE_TRACES, GYSK_ERR_INVAL before a finished merge */
+int		gysk_query_logical_traces(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_logical_trace *out);
+/* one row per logical service in the order of gysk_query_logical_all; GYSK_WINDOW_ACTIVE_ONLY keeps the rows whose merged window has
+ * nreq != 0. Count and capacity as gysk_query_logical_all */
+int		gysk_query_logical_traces_all(gysk_engine *e, uint32_t flags, gysk_logical_trace *out, uint32_t cap, uint32_t *n);
+/* the merged trace digest of one logical service: the contract of gysk_export_logical_tdigest (min / max: the extremes of the digested
+ * samples, +inf / -inf while empty; GYSK_ERR_NOENT for an id the map does not have) */
+int		gysk_export_logical_trace_tdigest(gysk_engine *e, uint64_t logical_id, double *means, uint64_t *weights, uint32_t cap,
+				uint32_t *n, double *min_val, double *max_val);
+/* the same digest as Postgres tdigest text (gysk_tdigest_to_pgtext at compression 100, no recompress): what a per-logical-service
+ * trace table stores for public.tdigest(col) to merge over a time range. The string length or GYSK_ERR_* */
+int		gysk_export_logical_trace_tdigest_pgtext(gysk_engine *e, uint64_t logical_id, char *buf, uint32_t cap);
 
 /* ---- host clusters (GYSK_FLAG_MERGE_CLUSTERS): MS_CLUSTER_STATE across every rank ----
  * Which host belongs to which cluster: host_idxs[i] -> cluster_ids[i] (the caller hashes PARTHA_INFO::cluster_name_ into the id). The same
