@@ -976,38 +976,40 @@ inline bool decode_wire(const wire::ACTIVE_CONN_STATS &r, uint32_t host_idx, gys
 	return true;
 }
 
-// API_TRAN, common/gy_proto_common.h:140-204 (probe-confirmed offsets: response_usec_ 48, glob_id_ 120, errorcode_ 152, cliport_ 166,
-// request_len_ 170, lenext_ 172, padlen_ 174, sizeof 176; get_elem_size() = sizeof + request_len_ + lenext_ + padlen_).
+// API_TRAN, common/gy_proto_common.h:140-204, read at the offsets of wire::API_TRAN_OFF.
 // SVC_INFO_CAP::upd_stats_on_req (gy_proto_parser.cc:2678-2694): nrequests_++, resp_cache_.add_cache(response_usec_ / 1000),
 // error counters. is_error / is_serv_err are the parser's verdict; the record carries errorcode_: != 0 is an error, >= 500 a
 // server error (HTTP status convention of the reference's http parser).
 struct ApiTran
 {
+	using O = wire::API_TRAN_OFF;
 	const uint8_t *p;
 	template <typename T> T at(size_t off) const { T v; memcpy(&v, p + off, sizeof(T)); return v; }
-	size_t get_elem_size() const { return 176 + at<uint16_t>(170) + at<uint16_t>(172) + p[174]; }
+	size_t get_elem_size() const { return O::SIZE + at<uint16_t>(O::REQUEST_LEN) + at<uint16_t>(O::LENEXT) + p[O::PADLEN]; }
 };
 inline bool decode_wire(const ApiTran &r, uint32_t host_idx, gysk_event &o)
 {
-	const int32_t err = r.at<int32_t>(152);
-	o.svc_id = r.at<uint64_t>(120);
-	o.flow_key = r.at<uint16_t>(166);					// cliport_ (host order): CONN_BITMAP index
-	o.value = clamp32(r.at<uint64_t>(48));					// beyond 1 000 000 msec: dropped by the validity rule on the device
-	o.host_idx = host_idx; o.tsec = (uint32_t)(r.at<uint64_t>(16) / 1000000ull);	// tupd_usec_
+	using O = ApiTran::O;
+	const int32_t err = r.at<int32_t>(O::ERRORCODE);
+	o.svc_id = r.at<uint64_t>(O::GLOB_ID);
+	o.flow_key = r.at<uint16_t>(O::CLIPORT);				// cliport_ (host order): CONN_BITMAP index
+	o.value = clamp32(r.at<uint64_t>(O::RESPONSE_USEC));			// beyond 1 000 000 msec: dropped by the validity rule on the device
+	o.host_idx = host_idx; o.tsec = (uint32_t)(r.at<uint64_t>(O::TUPD_USEC) / 1000000ull);
 	o.type = GYSK_EV_RESP;
 	o.flags = err == 0 ? 0 : (err >= 500 ? GYSK_EVF_SER_ERROR : GYSK_EVF_CLI_ERROR);
 	return true;
 }
-// the record's GYSK_EV_TRACE (engines with trace rows): reqlen_ 24, reslen_ 32, reqnum_ 40
+// the record's GYSK_EV_TRACE (engines with trace rows): bytes in / out from reqlen_ / reslen_, a new connection when reqnum_ is 0
 inline bool decode_trace(const ApiTran &r, uint32_t host_idx, gysk_event &o)
 {
-	const int32_t err = r.at<int32_t>(152);
-	o.svc_id = r.at<uint64_t>(120);
-	o.flow_key = (uint64_t)clamp32(r.at<uint64_t>(24)) | ((uint64_t)clamp32(r.at<uint64_t>(32)) << 32);
-	o.value = clamp32(r.at<uint64_t>(48));
-	o.host_idx = host_idx; o.tsec = (uint32_t)(r.at<uint64_t>(16) / 1000000ull);
+	using O = ApiTran::O;
+	const int32_t err = r.at<int32_t>(O::ERRORCODE);
+	o.svc_id = r.at<uint64_t>(O::GLOB_ID);
+	o.flow_key = (uint64_t)clamp32(r.at<uint64_t>(O::REQLEN)) | ((uint64_t)clamp32(r.at<uint64_t>(O::RESLEN)) << 32);
+	o.value = clamp32(r.at<uint64_t>(O::RESPONSE_USEC));
+	o.host_idx = host_idx; o.tsec = (uint32_t)(r.at<uint64_t>(O::TUPD_USEC) / 1000000ull);
 	o.type = GYSK_EV_TRACE;
-	o.flags = (err != 0 ? GYSK_EVF_TRACE_ERROR : 0u) | (r.at<uint64_t>(40) == 0 ? GYSK_EVF_TRACE_NEWCONN : 0u);
+	o.flags = (err != 0 ? GYSK_EVF_TRACE_ERROR : 0u) | (r.at<uint64_t>(O::REQNUM) == 0 ? GYSK_EVF_TRACE_NEWCONN : 0u);
 	return true;
 }
 

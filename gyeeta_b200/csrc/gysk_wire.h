@@ -1,7 +1,8 @@
 // gysk_wire.h — host-side restatement of the wire records that reach MCONN_HANDLER::handle_l2_misc
 // (server/gy_mconnhdlr.cc:4700-4800) and of their L1 validators (common/gy_comm_proto.cc:840-996).
 // Plain-old-data mirrors with static_asserts on size and the offsets the decoder reads; the layouts follow
-// common/gy_comm_proto.h (alignas(8), host endian, variable stride = sizeof + string + padding_len_).
+// common/gy_comm_proto.h (alignas(8), host endian, variable stride = sizeof + string + padding_len_). Every size, alignment and
+// offset here is pinned to the reference's own compiled structs by tests/test_wire_layout_host.py.
 #pragma once
 
 #include <cstdint>
@@ -252,6 +253,16 @@ struct alignas(8) HOST_STATE_NOTIFY					// common/gy_comm_proto.h:2289-2330 (one
 static_assert(sizeof(HOST_STATE_NOTIFY) == 56 && offsetof(HOST_STATE_NOTIFY, nlisten_issue_) == 20 && offsetof(HOST_STATE_NOTIFY, nlisten_) == 28 &&
 		offsetof(HOST_STATE_NOTIFY, curr_state_) == 32 && offsetof(HOST_STATE_NOTIFY, severe_mem_issue_) == 37 &&
 		offsetof(HOST_STATE_NOTIFY, total_cpu_delayms_) == 40, "HOST_STATE_NOTIFY");
+
+// API_TRAN, common/gy_proto_common.h:140-204: read at these offsets (the record embeds two GY_IP_ADDR, which the library does not
+// mirror). Pinned to the reference's own struct by tests/test_wire_layout_host.py. get_elem_size() = SIZE + request_len_ + lenext_
+// + padlen_; the widths are u64 for the times, lengths and ids, i32 errorcode_, u16 cliport_ / request_len_ / lenext_, u8 padlen_.
+struct API_TRAN_OFF
+{
+	static constexpr size_t	SIZE = 176;
+	static constexpr size_t	TUPD_USEC = 16, REQLEN = 24, RESLEN = 32, REQNUM = 40, RESPONSE_USEC = 48, GLOB_ID = 120;
+	static constexpr size_t	ERRORCODE = 152, CLIPORT = 166, REQUEST_LEN = 170, LENEXT = 172, PADLEN = 174;
+};
 
 // The shape shared by TCP_CONN_NOTIFY::validate / AGGR_TASK_STATE_NOTIFY::validate / LISTENER_STATE_NOTIFY::validate
 // (common/gy_comm_proto.cc:840-881, :912-953, :955-996): nevents <= MAX, every element size a multiple of 8 and

@@ -150,6 +150,79 @@ def ref():
     return _ref
 
 
+_refwire = None
+
+
+def refwire():
+    """the reference's own wire / eBPF / API_TRAN record types compiled into oracle/_ref/libgyrefwire.so (oracle/ref_wire.cc);
+    None when it is not available."""
+    global _refwire
+    if _refwire is None:
+        path = os.path.join(HERE, "_ref", "libgyrefwire.so")
+        if not os.path.exists(path):
+            return None
+        R = C.CDLL(path)
+        R.gyref_wire_val_bytes.restype = R.gyref_wire_nstructs.restype = R.gyref_wire_nfields.restype = C.c_uint32
+        R.gyref_wire_struct.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+        R.gyref_wire_field.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        R.gyref_wire_build.restype = C.c_int64
+        R.gyref_wire_build.argtypes = [C.c_char_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_uint64]
+        R.gyref_wire_msg.restype = C.c_int64
+        R.gyref_wire_msg.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
+        R.gyref_wire_const.restype = C.c_uint32
+        R.gyref_wire_const.argtypes = [C.c_char_p]
+        _refwire = R
+    return _refwire
+
+
+def wire_layout(R):
+    """(structs, fields): {name: (sizeof, alignof)} and [(struct, field, offset, size)] in ref_wire.cc's order"""
+    name, fld = C.c_char_p(), C.c_char_p()
+    a, b, c = C.c_uint32(), C.c_uint32(), C.c_uint32()
+    structs = {}
+    for i in range(R.gyref_wire_nstructs()):
+        R.gyref_wire_struct(i, C.byref(name), C.byref(a), C.byref(b))
+        structs[name.value.decode()] = (a.value, b.value)
+    fields = []
+    for i in range(R.gyref_wire_nfields()):
+        R.gyref_wire_field(i, C.byref(name), C.byref(fld), C.byref(a), C.byref(b))
+        fields.append((name.value.decode(), fld.value.decode(), a.value, b.value))
+    return structs, fields
+
+
+def wire_build(R, strct, values, tails=None):
+    """records of the reference type strct: values = {field name: array of n values} (scalars as their own dtype, wider fields as
+    (n, nbytes) uint8), tails = list of n byte strings (variable-stride kinds). Returns the bytes the reference wrote."""
+    names = list(values)
+    n = len(next(iter(values.values())))
+    vb = R.gyref_wire_val_bytes()
+    vals = np.zeros((n, len(names), vb), dtype=np.uint8)
+    for j, k in enumerate(names):
+        col = np.ascontiguousarray(values[k]).view(np.uint8).reshape(n, -1)
+        vals[:, j, : col.shape[1]] = col
+    tails = tails if tails is not None else [b""] * n
+    toff = np.zeros(n + 1, dtype=np.uint64)
+    toff[1:] = np.cumsum([len(t) for t in tails])
+    tail = np.frombuffer(b"".join(tails) + b"\0", dtype=np.uint8)
+    cname = (C.c_char_p * len(names))(*[k.encode() for k in names])
+    cap = n * 1024 + int(toff[-1]) + 64
+    out = np.zeros(cap, dtype=np.uint8)
+    got = R.gyref_wire_build(strct.encode(), n, cname, len(names), _p(vals), _p(tail), _p(toff), _p(out), cap)
+    assert got >= 0, f"gyref_wire_build({strct}) = {got}"
+    return out[:got].copy()
+
+
+def wire_msg(R, subtype, nevents, body):
+    """COMM_HEADER + EVENT_NOTIFY + body, the header set by the reference's own constructor"""
+    body = np.ascontiguousarray(body, dtype=np.uint8)
+    cap = len(body) + 64
+    out = np.zeros(cap, dtype=np.uint8)
+    got = R.gyref_wire_msg(subtype, nevents, _p(body), len(body), _p(out), cap)
+    assert got >= 0, f"gyref_wire_msg = {got}"
+    return out[:got].copy()
+
+
 def hist_run(L, fn, cls, tkind, vals, pcts=()):
     """run a fresh histogram over vals with either library; returns dict(stats, total, max, pct, buckets, avg, nb)."""
     vals = np.ascontiguousarray(vals, dtype=np.int64)

@@ -9,21 +9,12 @@ import pytest
 from gyeeta_b200 import engine as ge
 from gyeeta_b200 import synth
 from oracle import pyoracle as po
+from gyeeta_b200.wire import ACTIVE, CONN6, RESP4, RESP6
 from tests.test_gpu_wire import COMM_EVENT_NOTIFY, HDR, PM_MAGIC, TASK, TCP_CONN, build_msg
 from tests.util import assert_hist_equal
 
 pytestmark = pytest.mark.gpu
 
-ACTIVE = np.dtype([("listener_glob_id", "<u8"), ("cli_aggr_task_id", "<u8"), ("ser_comm", "S16"), ("cli_comm", "S16"), ("machid", "<u8", 2),
-                   ("remote_madhava_id", "<u8"), ("bytes_sent", "<u8"), ("bytes_received", "<u8"), ("cli_delay_msec", "<u4"),
-                   ("ser_delay_msec", "<u4"), ("max_rtt_msec", "<f4"), ("active_conns", "<u2"), ("flags", "u1"), ("pad", "u1")])
-RESP4 = np.dtype([("saddr", "<u4"), ("daddr", "<u4"), ("netns", "<u4"), ("sport", "<u2"), ("dport", "<u2"), ("lsndtime", "<u4"), ("lrcvtime", "<u4")])
-RESP6 = np.dtype([("saddr", "<u4", 4), ("daddr", "<u4", 4), ("netns", "<u4"), ("sport", "<u2"), ("dport", "<u2"), ("pad", "<u4", 2),
-                  ("lsndtime", "<u4"), ("lrcvtime", "<u4"), ("tail", "<u4", 2)])
-CONN6 = np.dtype([("ts_ns", "<u8"), ("bytes_received", "<u8"), ("bytes_acked", "<u8"), ("pid", "<u4"), ("tid", "<u4"), ("comm", "S16"),
-                  ("saddr", "<u4", 4), ("daddr", "<u4", 4), ("netns", "<u4"), ("sport", "<u2"), ("dport", "<u2"), ("ipver", "u1"), ("type", "u1"),
-                  ("pad", "u1", 6)])
-assert ACTIVE.itemsize == 104 and RESP4.itemsize == 24 and RESP6.itemsize == 64 and CONN6.itemsize == 96
 
 
 def fixed_msg(subtype, recs):

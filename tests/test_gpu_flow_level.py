@@ -8,20 +8,16 @@ import numpy as np
 import pytest
 
 from gyeeta_b200 import engine as ge
-from gyeeta_b200.wire import TCP_CONN, build_msg
+from gyeeta_b200.wire import ACTIVE, CONN4, CONN6, TCP_CONN, build_msg
 from oracle import pyoracle as po
 from tests.flow_level import M32, SEQUENCES, FlowLevelRing, exact_flows, flow_events, held_windows, level_of_history, point_query
-from tests.test_gpu_boundary import ACTIVE, CONN6, fixed_msg
+from tests.test_gpu_boundary import fixed_msg
 from tests.test_gpu_merge import _emulate_collectives
 
 pytestmark = pytest.mark.gpu
 
 NOTSUP = -95
 CFG = dict(max_svcs=1024, max_tasks=64, max_batch=1 << 14, cms_log2_width=12)
-CONN4 = np.dtype([("ts_ns", "<u8"), ("bytes_received", "<u8"), ("bytes_acked", "<u8"), ("pid", "<u4"), ("tid", "<u4"), ("comm", "S16"),
-                  ("saddr", "<u4"), ("daddr", "<u4"), ("netns", "<u4"), ("sport", "<u2"), ("dport", "<u2"), ("ipver", "u1"), ("type", "u1")],
-                 align=True)
-assert CONN4.itemsize == 72
 
 
 def _ocfg(kw):

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from gyeeta_b200 import engine as ge, synth
-from gyeeta_b200.wire import TCP_CONN, build_msg
+from gyeeta_b200.wire import CONN6, TCP_CONN, build_msg
 from oracle import pyoracle as po
 from tests.util import assert_hist_equal
 
@@ -133,10 +133,7 @@ def test_every_ingest_path_leaves_the_same_state():
             assert_hist_equal(e, orc, t, w)
 
 
-IPV6_EVENT = np.dtype(dict(names=["ts_ns", "bytes_received", "bytes_acked", "pid", "tid", "comm", "saddr", "daddr", "netns", "sport", "dport",
-                                  "ipver", "type"],
-                           formats=["<u8", "<u8", "<u8", "<u4", "<u4", "S16", ("<u4", 4), ("<u4", 4), "<u4", "<u2", "<u2", "u1", "u1"],
-                           offsets=[0, 8, 16, 24, 28, 32, 48, 64, 80, 84, 86, 88, 89], itemsize=96))
+IPV6_EVENT = CONN6
 
 
 def test_wide_raw_records_bulk_and_pieces():

@@ -9,15 +9,12 @@ import numpy as np
 import pytest
 
 from gyeeta_b200 import engine as ge
+from gyeeta_b200.wire import API_TRAN
 from tests import listener_rules as lr
 from tests.util import make_pair
 
 pytestmark = pytest.mark.gpu
 
-API_TRAN = np.dtype([("_a", "V16"), ("tupd_usec", "<u8"), ("_b", "V24"), ("response_usec", "<u8"), ("_c", "V64"), ("glob_id", "<u8"),
-                     ("_d", "V24"), ("errorcode", "<u4"), ("_e", "V10"), ("cli_port", "<u2"), ("_f", "V2"), ("request_len", "<u2"),
-                     ("ext_len", "<u2"), ("padding_len", "u1"), ("_g", "V1")])
-assert API_TRAN.itemsize == 176
 
 
 def by_id_rows(eng, ids):
@@ -48,7 +45,7 @@ def api_tran(ev):
     """the responses of ev as API_TRAN records (errorcode 500 for a server error, 200 otherwise)"""
     rec = np.zeros(len(ev), dtype=API_TRAN)
     rec["tupd_usec"] = 1_700_000_000_000_000 + np.arange(len(ev))
-    rec["response_usec"], rec["glob_id"], rec["cli_port"] = ev["value"], ev["svc_id"], ev["flow_key"]
+    rec["response_usec"], rec["glob_id"], rec["cliport"] = ev["value"], ev["svc_id"], ev["flow_key"]
     rec["errorcode"] = np.where(ev["flags"] & ge.EVF_SER_ERROR, 500, 200)
     return rec
 

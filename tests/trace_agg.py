@@ -12,16 +12,8 @@ import ctypes as C
 import numpy as np
 
 from gyeeta_b200 import engine as ge
+from gyeeta_b200.wire import API_TRAN
 from oracle import pyoracle as po
-
-# API_TRAN, common/gy_proto_common.h:140-204 (176 bytes, no request string here)
-API_TRAN = np.dtype([("treq_usec", "<u8"), ("tres_usec", "<u8"), ("tupd_usec", "<u8"), ("reqlen", "<u8"), ("reslen", "<u8"),
-                     ("reqnum", "<u8"), ("response_usec", "<u8"), ("reaction_usec", "<u8"), ("tconnect_usec", "<u8"), ("_ip", "V48"),
-                     ("glob_id", "<u8"), ("conn_id", "<u8"), ("comm", "S16"), ("errorcode", "<i4"), ("app_sleep_ms", "<u4"),
-                     ("tran_type", "<u4"), ("proto", "<u2"), ("cliport", "<u2"), ("serport", "<u2"), ("request_len", "<u2"),
-                     ("lenext", "<u2"), ("padlen", "u1"), ("_pad", "V1")])
-assert API_TRAN.itemsize == 176 and API_TRAN.fields["glob_id"][1] == 120 and API_TRAN.fields["errorcode"][1] == 152
-assert API_TRAN.fields["cliport"][1] == 166 and API_TRAN.fields["request_len"][1] == 170
 
 U32 = 0xFFFFFFFF
 VALID_USEC = 1000001000          # GYSK_EV_RESP validity rule: response msec <= 1 000 000
