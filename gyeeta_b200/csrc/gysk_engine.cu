@@ -71,11 +71,11 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	RecRegions rr;
-	const int li = launch_ingest(e->st, e->tmp, d_ev, n, key_slots(e), rr, e->stream);
+	const int li = launch_ingest(e->st, e->tmp, e->fq, d_ev, n, key_slots(e), rr, e->stream);
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, rr, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
@@ -296,6 +296,9 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 	if (maxv) *maxv = head.maxv;
 	return head.n > cap ? GYSK_ERR_NOSPC : GYSK_OK;
 }
+
+static_assert(sizeof(gysk_flow_qry_est) == sizeof(gysk_flow_est) && offsetof(gysk_flow_qry_est, queries) == offsetof(gysk_flow_est, count) &&
+		offsetof(gysk_flow_qry_est, resp_ms) == offsetof(gysk_flow_est, kbytes), "a flow query row is read as a gysk_flow_est");
 
 int query_flows_in(gysk_engine *e, const unsigned long long *tbl, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what)
 {
@@ -589,6 +592,9 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &st.cms_ring, (size_t)NSLOTS * ((size_t)cfg.cms_depth << cfg.cms_log2_width)));
 		A(dalloc(e, &st.cms_5min, (size_t)cfg.cms_depth << cfg.cms_log2_width));
 	}
+	if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) {		// not per slot either
+		A(dalloc(e, &e->fq.cur, (size_t)cfg.cms_depth << cfg.cms_log2_width)); A(dalloc(e, &e->fq.last, (size_t)cfg.cms_depth << cfg.cms_log2_width));
+	}
 	st.cms_depth = cfg.cms_depth; st.cms_log2w = cfg.cms_log2_width; st.cms_wmask = (1u << cfg.cms_log2_width) - 1; st.hll_p = cfg.hll_p;
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
 	st.td_delta = (double)cfg.td_compression;
@@ -638,6 +644,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		// each_slot_array, so gysk_grow leaves it
 		tmp.flow_cap = std::min<uint32_t>(FLOW_ENT_MAX, pow2_at_least(2ull * cfg.max_batch));
 		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
+		if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) A(dalloc(e, &e->fq.flow, (size_t)tmp.flow_cap));		// the query flow table, alike
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
 	if (cfg.max_trace_svcs) {
@@ -772,14 +779,31 @@ int64_t gysk_last_batch_flow_direct(gysk_engine *e)
 	return (int64_t)n;
 }
 
-// diagnostic: entries of the flow table that are not zero (a key or a sum left behind); 0 whenever no batch is in flight
+// diagnostic: response samples of the last device batch whose flow query update bypassed the query flow table (GYSK_FLAG_FLOW_QUERIES)
+int64_t gysk_last_batch_flow_query_direct(gysk_engine *e)
+{
+	CHECK_ENGINE(e);
+	if (!e->fq.cur) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Sync);
+	unsigned long long n = 0;
+	CU(e, cudaMemcpy(&n, e->st.counters + CTR_FLOWQ_DIRECT, sizeof(n), cudaMemcpyDeviceToHost));
+	return (int64_t)n;
+}
+
+// diagnostic: entries of the flow table (and of the query flow table, GYSK_FLAG_FLOW_QUERIES) that are not zero (a key or a sum left
+// behind); 0 whenever no batch is in flight
 int64_t gysk_flow_table_used(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Sync);
 	std::vector<FlowEnt> t(e->tmp.flow_cap);
-	CU(e, cudaMemcpy(t.data(), e->tmp.flow, t.size() * sizeof(FlowEnt), cudaMemcpyDeviceToHost));
-	return (int64_t)std::count_if(t.begin(), t.end(), [](const FlowEnt &f) { return f.key || f.inc; });
+	int64_t used = 0;
+	for (const FlowEnt *tbl : {e->tmp.flow, e->fq.flow}) {
+		if (!tbl) continue;
+		CU(e, cudaMemcpy(t.data(), tbl, t.size() * sizeof(FlowEnt), cudaMemcpyDeviceToHost));
+		used += (int64_t)std::count_if(t.begin(), t.end(), [](const FlowEnt &f) { return f.key || f.inc; });
+	}
+	return used;
 }
 
 int gysk_register_ids(gysk_engine *e, const uint64_t *ids, uint32_t n, int is_task)
@@ -1537,6 +1561,10 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 	if (e->st.cms_ring) e->kernel_launches += launch_cms_level_roll(e->st, e->stream);		// GYSK_FLAG_FLOW_LEVEL
 	std::swap(e->st.cms_cur, e->st.cms_last);
 	CU(e, cudaMemsetAsync(e->st.cms_cur, 0, sizeof(unsigned long long) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), e->stream));
+	if (e->fq.cur) {		// GYSK_FLAG_FLOW_QUERIES: the same window rule
+		std::swap(e->fq.cur, e->fq.last);
+		CU(e, cudaMemsetAsync(e->fq.cur, 0, sizeof(unsigned long long) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), e->stream));
+	}
 	return post_launch(e, "flush");
 }
 
@@ -1963,6 +1991,16 @@ int gysk_query_flows_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk
 	return query_flows_in(e, e->st.cms_5min, keys, n, out, "query_flows_5min");
 }
 
+// GYSK_FLAG_FLOW_QUERIES: the point query of gysk_query_flows on the flow query tables; gysk_flow_qry_est is gysk_flow_est's layout
+int gysk_query_flow_queries(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_qry_est *out)
+{
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_FLOW_QUERIES)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Submit);
+	return query_flows_in(e, last_window ? e->fq.last : e->fq.cur, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries");
+}
+
 int gysk_topn_svcs(gysk_engine *e, int metric, int32_t host_idx, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
 {
 	CHECK_ENGINE(e);
@@ -2050,6 +2088,17 @@ int gysk_export_cms_5min(gysk_engine *e, uint64_t *cells)
 	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
 	GYSK_ENTER(e, Sync);
 	CU(e, cudaMemcpy(cells, e->st.cms_5min, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), cudaMemcpyDeviceToHost));
+	return GYSK_OK;
+}
+
+int gysk_export_cms_queries(gysk_engine *e, int last_window, uint64_t *cells)
+{
+	CHECK_ENGINE(e);
+	if (!cells) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_FLOW_QUERIES)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Sync);
+	CU(e, cudaMemcpy(cells, last_window ? e->fq.last : e->fq.cur, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width),
+			cudaMemcpyDeviceToHost));
 	return GYSK_OK;
 }
 

@@ -251,7 +251,7 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min], hist last/all, conn [, levels, aux] [, states]
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min] [, cmsq cur/last], hist last/all, conn [, levels, aux] [, states]
 									//           [, clusters] [, traces]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt] [, flush tsec]
 									//           [, trace max]
@@ -259,6 +259,7 @@ struct MergeState
 	std::string		name_sum, name_maxi64, name_maxu8;	// the regions' gysk_buffer_desc names: their arrays, in order
 	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
 	unsigned long long	*g_cms_5min {nullptr};				// GYSK_FLAG_FLOW_LEVEL: the count-min level, summed over ranks
+	unsigned long long	*g_cmsq_cur {nullptr}, *g_cmsq_last {nullptr};	// GYSK_FLAG_FLOW_QUERIES: the flow query tables, summed over ranks
 	LogicalArrays		lg;
 	ClusterMap		clusters;				// kept across gysk_set_logical_map
 	bool			prepared {false}, finished {false};
@@ -284,6 +285,7 @@ struct gysk_engine
 	cudaStream_t		stream {nullptr}, copy_stream {nullptr};
 	gysk::DevState		st {};
 	gysk::SortTemp		tmp {};
+	gysk::FlowQueries	fq {};				// GYSK_FLAG_FLOW_QUERIES (every pointer nullptr without)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
 	std::vector<void *>	hallocs;

@@ -291,11 +291,12 @@ __device__ __forceinline__ IngestRec ld_rec(const IngestRec *p)
 
 // One connection record's count-min increment into the batch's flow table, given the key k of entry pos (the first probe): a RED into the
 // flow's entry, claimed with a CAS on the key if need be. Past FLOW_PROBES entries, or for key 0, the record updates its count-min
-// cells directly (normal priority: nothing is left for the TASK pass to reset) and is counted in CTR_FLOW_DIRECT, one RED per group of
+// cells (cms) directly (normal priority: nothing is left for the TASK pass to reset) and is counted in counter ctr, one RED per group of
 // converged lanes, since a table too small for the batch's flows sends most records this way. Entries only go from empty to a key
-// during the pass, so a record never misses its flow's entry; should a flow still hold two, the TASK pass applies both.
-__device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft, unsigned long long key, uint32_t pos, unsigned long long k,
-		unsigned long long inc, unsigned long long pol_last)
+// during the pass, so a record never misses its flow's entry; should a flow still hold two, the TASK pass applies both. A response
+// sample of GYSK_FLAG_FLOW_QUERIES takes the same path with the query flow table, cells and counter.
+__device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft, unsigned long long *cms, int ctr, unsigned long long key,
+		uint32_t pos, unsigned long long k, unsigned long long inc, unsigned long long pol_last)
 {
 	if (key) {
 		for (uint32_t p = 0; ; ) {
@@ -307,10 +308,10 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 		}
 	}
 	const uint32_t am = __activemask();
-	if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(st.counters + CTR_FLOW_DIRECT, (unsigned long long)__popc(am));
+	if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(st.counters + ctr, (unsigned long long)__popc(am));
 	const uint32_t h1 = (uint32_t)key, h2 = (uint32_t)(key >> 32);
 	for (uint32_t row = 0; row < st.cms_depth; ++row)
-		red_add_u64(st.cms_cur + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
+		red_add_u64(cms + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
 }
 
 // m queued connection records (all 32 lanes call): two lookup2 hashes per flow key -> the flow's entry in the batch's flow table (the
@@ -320,34 +321,44 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // tail, pushed the 32 MB of randomly updated lines out of the 50 MB L2 and many REDs became DRAM read-modify-writes. The drain_kernel
 // TASK pass sets the lines back to evict_normal. pol_hll / pol_last: l2_policy_evict_first / _last.
 // exp (timing runs only): 16 = no count-min updates (neither flow table nor cells), 32 = no HLL peek / raise
-template <typename HotTable>
+// QRY (GYSK_FLAG_FLOW_QUERIES): a record with slot QRY_REC is a response sample {usec, flow key}; it adds {1 | msec << 32} to its flow's
+// entry of the query flow table fq (cells fq_cms past the probe limit) and touches neither the HLL nor a service cell.
+template <bool QRY, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
-		int lane, unsigned long long pol_hll, unsigned long long pol_last, int exp)
+		int lane, unsigned long long pol_hll, unsigned long long pol_last, int exp, const FlowTable &fq, unsigned long long *fq_cms)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
+		bool qry = false;
 		uint32_t cell = 0, idx = 0, rank = 0, hw = 0, pos = 0; int kb = 0;
 		unsigned long long key = 0, inc = 0, k = 0;
 		if (act) {
 			const IngestRec r = ld_rec(q + i);
+			qry = QRY && r.slot == QRY_REC;
+			FlowEnt *const tent = qry ? fq.ent : ft.ent;		// field by field: a selected reference would copy both tables to the stack
+			const uint32_t tmask = qry ? fq.mask : ft.mask;
 			uint32_t h1, h2;
 			flow_hashes(r.flow_key, h1, h2);
 			// the HLL register word and the flow table's first probe are asked for together and looked at after the cell update, which
 			// hides their latency (a stale register is harmless: the CAS re-validates)
-			if (!(exp & 32)) {
+			if (!(exp & 32) && !qry) {
 				hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
 				hw = ld_na_hint_u32(reinterpret_cast<const uint32_t *>(st.hll + ((size_t)r.slot << st.hll_p)) + (idx >> 2), pol_hll);
 			}
 			key = ((unsigned long long)h2 << 32) | h1;
-			inc = cms_increment(r.value);
-			pos = table_hash(key) & ft.mask;
-			if (key && !(exp & 16)) k = ld_cg_hint_u64(&ft.ent[pos].key, pol_last);
+			// usec -> msec as the histogram takes it (ingest_kernel)
+			inc = qry ? 1ull | ((unsigned long long)(r.value / 1000u) << 32) : cms_increment(r.value);
+			pos = table_hash(key) & tmask;
+			if (key && !(exp & 16)) k = ld_cg_hint_u64(&tent[pos].key, pol_last);
 			cell = r.slot;
 			kb = (int)(r.value >> 10);
 		}
-		cell_add(st, hot, act, cell, kb);
-		if (act && !(exp & 16)) flow_add(st, ft, key, pos, k, inc, pol_last);
-		if (act && !(exp & 32)) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
+		cell_add(st, hot, act && !qry, cell, kb);
+		if (act && !(exp & 16)) {
+			if (qry) flow_add(st, fq, fq_cms, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
+			else flow_add(st, ft, st.cms_cur, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last);
+		}
+		if (act && !qry && !(exp & 32)) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
 	}
 }
 
@@ -457,8 +468,10 @@ struct IngestShared
 	uint32_t	dhist[KEY_PASSES_MAX][DH];			// digit histograms of this CTA's keys, one per radix pass
 };
 
-// TRACE: the engine has trace rows (a separate instance, so that an engine without them runs the kernel without the trace path)
-template <bool TRACE>
+// TRACE: the engine has trace rows (a separate instance, so that an engine without them runs the kernel without the trace path).
+// QRY: GYSK_FLAG_FLOW_QUERIES (a separate instance too): every response sample that reaches its service's histogram, by the key or the
+// hot-row route, also joins the connection queue as a record {QRY_REC, usec, flow key} for the TCP drain pass.
+template <bool TRACE, bool QRY>
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
 		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, int exp)
 {
@@ -599,8 +612,8 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 			const uint32_t hotrow = (ok && is_resp) ? sbv[k].w : 0u;
 			// a trace sample within the RESP validity rule becomes a sort key of its row's pseudo-slot (a trace row: trow >= 0)
 			const bool tr_key = TRACE && trow[k] >= 0 && rb[k].x < 1000001000u;
-			const uint32_t m_resp = __ballot_sync(0xffffffffu, (ok && is_resp && !hotrow) || tr_key), m_tcp = __ballot_sync(0xffffffffu, ok && is_tcp),
-					m_task = __ballot_sync(0xffffffffu, ok && is_task);
+			const uint32_t m_resp = __ballot_sync(0xffffffffu, (ok && is_resp && !hotrow) || tr_key),
+					m_tcp = __ballot_sync(0xffffffffu, ok && (is_tcp || (QRY && is_resp))), m_task = __ballot_sync(0xffffffffu, ok && is_task);
 			if (ok) {
 				if (is_resp) {
 					const uint32_t bin = td_code(rb[k].x) + bkt[k];
@@ -622,6 +635,10 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					if (!(mwv[k] & bit)) atomicOr(st.bm_cur + (size_t)slot * HIST_CELLS + bkt[k], bit);
 					const uint32_t ef = rb[k].w >> 16;			// API_TRAN error flags: rare
 					if (ef & 3u) red_add_u64(&st.slot_aux[slot].err_cur, (unsigned long long)(ef & 1u) | ((unsigned long long)((ef >> 1) & 1u) << 32));
+					if (QRY) {
+						IngestRec r; r.slot = QRY_REC; r.value = v; r.flow_key = ((unsigned long long)ra[k].w << 32) | ra[k].z;
+						W.tcp[ntcp + __popc(m_tcp & lt)] = r;
+					}
 				}
 				else if (TRACE && kind[k] == GYSK_EV_TRACE) {
 					const uint32_t v = rb[k].x;
@@ -685,6 +702,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 	c_in = __reduce_add_sync(0xffffffffu, c_in);
 	c_foreign = __reduce_add_sync(0xffffffffu, c_foreign);
 	const unsigned long long t_resp = __reduce_add_sync(0xffffffffu, n_resp);
+	if (QRY) t_tcp -= t_resp;					// each counted response sample was queued once as a QRY_REC record
 	t_tcp += __reduce_add_sync(0xffffffffu, n_active);		// counted with the connection events
 	const unsigned long long t_trace = __reduce_add_sync(0xffffffffu, n_trace);
 	n_trace_drop = __reduce_add_sync(0xffffffffu, n_trace_drop);
@@ -721,17 +739,20 @@ template <> struct DrainShape<true> { static constexpr int WARPS = 16, HOT_BITS 
 // The records sit in the ingest launch's per-warp regions (RecRegions). Each CTA scans the regions' counts into a table of where
 // each region's groups of 32 records start, and every warp takes an equal, contiguous share of all groups: the regions' sizes
 // differ, the drain warps' work does not.
-template <bool TASK>
+// QRY (GYSK_FLAG_FLOW_QUERIES): the TCP pass also sums the queued response samples in the query flow table fq, and the TASK pass applies
+// that table to the query cells fq_cms after the connection flow table.
+template <bool TASK, bool QRY>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, int exp)
+		RecRegions rr, int exp, FlowTable fq, unsigned long long *fq_cms)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
 	if (TASK) {
-		// the flow table the TCP pass filled: each entry's sum into its flow's count-min cells (the key holds the two hashes), then
-		// the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a priority they keep after it ends: back
-		// to normal, so that they do not hold L2 against the next batch's ingest_kernel and chain. A thread takes FLOW_SWEEP entries a
-		// step, one grid stride apart, their loads in flight together (the REDs' memory clobber keeps a load from moving past them).
+		// the flow table the TCP pass filled (then, with QRY, the query flow table): each entry's sum into its flow's cells (the key holds
+		// the two hashes), then the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a priority they keep
+		// after it ends: back to normal, so that they do not hold L2 against the next batch's ingest_kernel and chain. A thread takes
+		// FLOW_SWEEP entries a step, one grid stride apart, their loads in flight together (the REDs' memory clobber keeps a load from
+		// moving past them).
 		const uint32_t stride = gridDim.x * blockDim.x;
 		for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= ft.mask; i0 += FLOW_SWEEP * stride) {
 			FlowEnt f[FLOW_SWEEP];
@@ -747,6 +768,28 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 					ft.ent[i] = FlowEnt {0ull, 0ull};
 				}
 				if (i <= ft.mask && !(i & 7u)) l2_evict_normal_line(ft.ent + i);
+			}
+		}
+		// the same sweep over the query flow table into its cells. Written out a second time: one loop or one helper over both tables
+		// changes the code of the connection table's sweep, which an engine without the flag runs as before.
+		if (QRY) {
+			const FlowTable &t = fq;
+			unsigned long long *const cms = fq_cms;
+			for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= t.mask; i0 += FLOW_SWEEP * stride) {
+				FlowEnt f[FLOW_SWEEP];
+#pragma unroll
+				for (uint32_t u = 0; u < FLOW_SWEEP; ++u) if (i0 + u * stride <= t.mask) f[u] = t.ent[i0 + u * stride]; else f[u] = FlowEnt {0ull, 0ull};
+#pragma unroll
+				for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
+					const uint32_t i = i0 + u * stride;
+					if (f[u].key) {
+						const uint32_t h1 = (uint32_t)f[u].key, h2 = (uint32_t)(f[u].key >> 32);
+						for (uint32_t row = 0; row < st.cms_depth; ++row)
+							red_add_u64(cms + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), f[u].inc);
+						t.ent[i] = FlowEnt {0ull, 0ull};
+					}
+					if (i <= t.mask && !(i & 7u)) l2_evict_normal_line(t.ent + i);
+				}
 			}
 		}
 	}
@@ -819,7 +862,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, exp);
+			drain_tcp_recs<QRY>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, exp, fq, fq_cms);
 		}
 	}
 
@@ -2232,7 +2275,8 @@ static int plain_sort_plan(int lo, int hi, SortPlan &P)
 	return 0;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
+		RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
 	const int dev = current_device();
@@ -2246,8 +2290,10 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
 	static bool attr_set[MAX_DEVICES] = {};
 	if (!attr_set[dev]) {
-		cudaFuncSetAttribute(ingest_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		cudaFuncSetAttribute(ingest_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cudaFuncSetAttribute(ingest_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cudaFuncSetAttribute(ingest_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cudaFuncSetAttribute(ingest_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cudaFuncSetAttribute(ingest_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
 		attr_set[dev] = true;
 	}
 	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
@@ -2258,37 +2304,49 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_e
 	rr.nwarps = grid * WARPS;
 	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
-	if (st.trace.rows) ingest_kernel<true><<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
-	else ingest_kernel<false><<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
+	// a counted response sample takes a connection-queue entry, as one connection event does: the regions hold one record per event
+	auto k = st.trace.rows ? (fq.cur ? ingest_kernel<true, true> : ingest_kernel<true, false>) : (fq.cur ? ingest_kernel<false, true> : ingest_kernel<false, false>);
+	k<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
 	return 1;
 }
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
-template <bool TASK>
+template <bool TASK, bool QRY>
 static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int exp, int dev,
-		cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, cudaStream_t s)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
 		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+		cudaFuncSetAttribute(drain_kernel<TASK, QRY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK>, WARPS * 32, smem_max);
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY>, WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, exp);
+	drain_kernel<TASK, QRY><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, exp, fq, fq_cms);
+}
+
+template <bool QRY>
+static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int exp, int dev,
+		const FlowTable &fq, unsigned long long *fq_cms, cudaStream_t s)
+{
+	int launches = 0;
+	if (!(exp & 4)) { launch_drain_pass<false, QRY>(st, ft, tmp, rr, n_events, exp, dev, fq, fq_cms, s); launches++; }
+	launch_drain_pass<true, QRY>(st, ft, tmp, rr, n_events, exp, dev, fq, fq_cms, s); launches++;
+	return launches;
 }
 
 // the batch's queued connection records -> flow table, HLL, exact cells; then the flow table -> count-min and its process records ->
 // process histograms. The TASK pass always runs: it leaves the flow table empty. The table takes the smallest power of two >= 2 x the
 // batch's events (the flows are fewer than the connection records), up to what tmp holds, so that a small batch sweeps a small table.
-int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
+// With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size.
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
@@ -2297,10 +2355,9 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr,
 	while (n < tmp.flow_cap && n < 2 * n_events) n <<= 1;
 	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
-	int launches = 0;
-	if (!(exp & 4)) { launch_drain_pass<false>(st, ft, tmp, rr, n_events, exp, dev, s); launches++; }
-	launch_drain_pass<true>(st, ft, tmp, rr, n_events, exp, dev, s); launches++;
-	return launches;
+	if (!fq.cur) return launch_drain_passes<false>(st, ft, tmp, rr, n_events, exp, dev, FlowTable {nullptr, 0u}, nullptr, s);
+	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
+	return launch_drain_passes<true>(st, ft, tmp, rr, n_events, exp, dev, FlowTable {fq.flow, n - 1u}, fq.cur, s);
 }
 
 static void os_set_attrs(int dev)

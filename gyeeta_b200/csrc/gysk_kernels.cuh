@@ -151,6 +151,14 @@ static constexpr uint32_t FLOW_PROBES = 16;		// linear probe limit; past it a re
 static constexpr uint32_t FLOW_ENT_MAX = 1u << 21;	// 32 MB; a batch takes the smallest power of two >= 2 x its events, up to this
 static constexpr uint32_t FLOW_SWEEP = 4;		// entries per thread and step of the TASK pass's sweep
 
+// GYSK_FLAG_FLOW_QUERIES: the count-min of the response samples that reach a service histogram, cells {queries | response msec << 32}
+// with the depth, width and row hashes of cms_cur / cms_last, and the batch flow table the TCP pass sums them in before the TASK pass
+// applies it (as FlowTable does for the connection records). ingest_kernel queues each such sample as a connection-queue record whose
+// slot is QRY_REC. Kept out of DevState so that the kernels without the flag keep their parameter layout: the drain passes take it as
+// parameters of their own. Every pointer nullptr: off.
+struct FlowQueries { unsigned long long *cur, *last; FlowEnt *flow; };
+static constexpr uint32_t QRY_REC = 0xFFFFFFFFu;	// slot field of a queued response sample (service slots are < 2^24)
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
@@ -229,9 +237,11 @@ int launch_init_slots(const DevState &st, uint32_t s_lo, uint32_t s_hi, uint32_t
 int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_t n, int is_task, cudaStream_t s);
 // -1: no sort plan for max_svcs, or the launch's record regions do not fit the buffers
 // key_slots: the values the slot field of a sort key takes (max_svcs, or max_svcs + 1 + trace rows with trace rows)
-int launch_ingest(const DevState &st, const SortTemp &tmp, const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s);
+// fq.cur != nullptr: the response samples are queued for the flow query table too (GYSK_FLAG_FLOW_QUERIES)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
+		RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
-int launch_drains(const DevState &st, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
 // bits outside [0, 64)), or n_max >= 2^30
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);

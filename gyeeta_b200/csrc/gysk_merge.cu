@@ -14,7 +14,8 @@
 //                          GYSK_FLAG_MERGE_CLUSTERS the host clusters' MS_CLUSTER_STATE words after them (gysk_set_cluster_map);
 //                          GYSK_FLAG_MERGE_TOPN appends this rank's 64 best services / processes per metric, with their rows, to the slab;
 //                          GYSK_FLAG_FLOW_LEVEL puts the count-min level after cms cur/last and, as GYSK_FLAG_MERGE_LEVELS does,
-//                          the flush tsec pair in the i64 MAX region (once when both are set)
+//                          the flush tsec pair in the i64 MAX region (once when both are set); GYSK_FLAG_FLOW_QUERIES puts the
+//                          flow query tables cur/last after the count-min tables
 //   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests [, the global pick of the gathered top-N candidates]
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
@@ -814,10 +815,12 @@ int lay_out_arena(gysk_engine *e)
 	// name joins its region's gysk_merge_buffers name. GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX
 	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those.
 	// GYSK_FLAG_FLOW_LEVEL puts the count-min level after the two window tables, and needs the flush tsec pair as the levels do:
-	// still three regions, three collectives. GYSK_FLAG_MERGE_TRACES puts its words at the end of the SUM region, its maxima at the end of
-	// the i64 MAX one, and needs the flush tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
+	// still three regions, three collectives. GYSK_FLAG_FLOW_QUERIES puts the two flow query tables after the count-min ones.
+	// GYSK_FLAG_MERGE_TRACES puts its words at the end of the SUM region, its maxima at the end of the i64 MAX one, and needs the flush
+	// tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
 	const bool flow_level = e->cfg.flags & GYSK_FLAG_FLOW_LEVEL, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
+	const bool flow_queries = e->cfg.flags & GYSK_FLAG_FLOW_QUERIES;
 	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
@@ -830,6 +833,7 @@ int lay_out_arena(gysk_engine *e)
 		mg.off_sum = off;
 		take(mg.g_cms_cur, b_cms, "cms_cur"); take(mg.g_cms_last, b_cms, "cms_last");
 		if (flow_level) take(mg.g_cms_5min, b_cms, "cms_5min");
+		if (flow_queries) { take(mg.g_cmsq_cur, b_cms, "cms_qry_cur"); take(mg.g_cmsq_last, b_cms, "cms_qry_last"); }
 		take(lg.last, b_hist, "hist_last"); take(lg.all, b_hist, "hist_all"); take(lg.conn, (size_t)nl * 4 * 8, "conn");
 		if (levels) { take(lg.lvl, NLEVELS * b_hist, "levels"); take(lg.aux, (size_t)nl * 4 * 8, "aux"); }
 		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8, "states");
@@ -1000,6 +1004,10 @@ int gysk_merge_prepare(gysk_engine *e)
 	CU(e, cudaMemcpyAsync(mg.g_cms_cur, e->st.cms_cur, b_cms, cudaMemcpyDeviceToDevice, e->stream));
 	CU(e, cudaMemcpyAsync(mg.g_cms_last, e->st.cms_last, b_cms, cudaMemcpyDeviceToDevice, e->stream));
 	if (mg.g_cms_5min) CU(e, cudaMemcpyAsync(mg.g_cms_5min, e->st.cms_5min, b_cms, cudaMemcpyDeviceToDevice, e->stream));		// GYSK_FLAG_FLOW_LEVEL
+	if (mg.g_cmsq_cur) {		// GYSK_FLAG_FLOW_QUERIES
+		CU(e, cudaMemcpyAsync(mg.g_cmsq_cur, e->fq.cur, b_cms, cudaMemcpyDeviceToDevice, e->stream));
+		CU(e, cudaMemcpyAsync(mg.g_cmsq_last, e->fq.last, b_cms, cudaMemcpyDeviceToDevice, e->stream));
+	}
 	if (nl) {
 		if (mg.nmembers) {
 			resolve_members_kernel<<<div_up(mg.nmembers, 256), 256, 0, e->stream>>>(e->st, mg.d_member_ids, mg.nmembers, mg.members);
@@ -1309,6 +1317,18 @@ int gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t 
 	MergeState &mg = e->mg;
 	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global_5min: no merge");
 	return query_flows_in(e, mg.g_cms_5min, keys, n, out, "query_flows_global_5min");
+}
+
+// GYSK_FLAG_FLOW_QUERIES: the point query on the flow query tables summed over the ranks
+int gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_qry_est *out)
+{
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_FLOW_QUERIES)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flow_queries_global: no merge");
+	return query_flows_in(e, last_window ? mg.g_cmsq_last : mg.g_cmsq_cur, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_global");
 }
 
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)

@@ -12,6 +12,7 @@ EVENT_DTYPE = np.dtype([("svc_id", "<u8"), ("flow_key", "<u8"), ("value", "<u4")
 assert EVENT_DTYPE.itemsize == 32
 SERIAL_DTYPE = np.dtype([("count", "<u8"), ("sum", "<i8")])
 FLOW_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("count", "<u4"), ("kbytes", "<u4")])
+FLOW_QRY_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("queries", "<u4"), ("resp_ms", "<u4")])     # gysk_flow_qry_est
 
 EV_CONNECT, EV_ACCEPT, EV_CLOSE_CLI, EV_CLOSE_SER, EV_RESP, EV_TASK, EV_ACTIVE = 1, 2, 3, 4, 5, 6, 7
 EVF_CLI_ERROR, EVF_SER_ERROR = 1, 2
@@ -34,6 +35,7 @@ NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CO
  HOSTTOP_TASK_CPU_DELAY, HOSTTOP_TASK_VM_DELAY, HOSTTOP_TASK_BLKIO_DELAY) = range(11)
 FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, FLAG_MERGE_TOPN, FLAG_FLOW_LEVEL = 1, 2, 4, 8, 16, 32
 FLAG_MERGE_TRACES = 64
+FLAG_FLOW_QUERIES = 128
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
@@ -304,6 +306,10 @@ def load_library(path=None):
         "gysk_query_flows_5min": (i32, [vp, vp, u32, vp]),
         "gysk_export_cms_5min": (i32, [vp, vp]),
         "gysk_query_flows_global_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_query_flow_queries": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_export_cms_queries": (i32, [vp, i32, vp]),
+        "gysk_query_flow_queries_global": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_last_batch_flow_query_direct": (C.c_int64, [vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -369,7 +375,7 @@ class Engine:
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
-                 max_trace_svcs=0, merge_traces=False):
+                 max_trace_svcs=0, merge_traces=False, flow_queries=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -382,7 +388,8 @@ class Engine:
         cfg.max_trace_svcs = max_trace_svcs
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
-                    (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0)
+                    (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
+                    (FLAG_FLOW_QUERIES if flow_queries else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -570,8 +577,16 @@ class Engine:
             self._chk(int(n))
         return int(n)
 
+    def last_batch_flow_query_direct(self):
+        """response samples of the last device batch whose flow query update bypassed the query flow table (flow_queries=True)"""
+        n = self.L.gysk_last_batch_flow_query_direct(self.h)
+        if n < 0:
+            self._chk(int(n))
+        return int(n)
+
     def flow_table_used(self):
-        """non-zero entries of the batch flow table: 0 whenever no batch is in flight (diagnostic)"""
+        """non-zero entries of the batch flow tables (the query one too with flow_queries=True): 0 whenever no batch is in flight
+        (diagnostic)"""
         n = self.L.gysk_flow_table_used(self.h)
         if n < 0:
             self._chk(int(n))
@@ -666,6 +681,13 @@ class Engine:
         keys = np.ascontiguousarray(keys, dtype=np.uint64)
         out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
         self._chk(self.L.gysk_query_flows_5min(self.h, _p(keys), len(keys), _p(out)))
+        return out
+
+    def query_flow_queries(self, keys, last_window=False):
+        """gysk_query_flow_queries: requests and response msec per flow key, min over rows (flow_queries=True)"""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        out = np.zeros(len(keys), dtype=FLOW_QRY_EST_DTYPE)
+        self._chk(self.L.gysk_query_flow_queries(self.h, _p(keys), len(keys), int(last_window), _p(out)))
         return out
 
     def topn(self, metric, n=10, host_idx=-1):
@@ -950,6 +972,19 @@ class Engine:
     def export_cms(self, last_window=False):
         out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
         self._chk(self.L.gysk_export_cms(self.h, int(last_window), _p(out)))
+        return out
+
+    def export_cms_queries(self, last_window=False):
+        """gysk_export_cms_queries: the cells {queries | resp msec << 32} of the flow query table (flow_queries=True)"""
+        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
+        self._chk(self.L.gysk_export_cms_queries(self.h, int(last_window), _p(out)))
+        return out
+
+    def query_flow_queries_global(self, keys, last_window=False):
+        """gysk_query_flow_queries_global: the point query on the flow query tables summed over the ranks by the last merge"""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        out = np.zeros(len(keys), dtype=FLOW_QRY_EST_DTYPE)
+        self._chk(self.L.gysk_query_flow_queries_global(self.h, _p(keys), len(keys), int(last_window), _p(out)))
         return out
 
     def export_cms_5min(self):

@@ -224,6 +224,12 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   freely with the flags above, the same flags on every rank. Needs trace rows: gysk_create
 						   refuses it with max_trace_svcs == 0. Without it the merge arena, slab and collectives are
 						   as before */
+#define GYSK_FLAG_FLOW_QUERIES		0x80u	/* a count-min of response samples per flow beside the connection count-min: requests and
+						   response msec of a client in the open and the last window (gysk_query_flow_queries,
+						   "flow queries" below); with it the merge step also sums those tables across ranks (the
+						   same flags on every rank). Costs 2 more tables of depth << log2_width cells and a second
+						   batch flow table. Without it nothing is allocated, every other call answers as before and
+						   the flow query calls are GYSK_ERR_NOTSUP */
 
 typedef struct gysk_config
 {
@@ -352,6 +358,14 @@ typedef struct gysk_flow_est
 	uint32_t	kbytes;			/* min over rows of the kbytes halves */
 } gysk_flow_est;
 
+/* a point query on the flow query tables (GYSK_FLAG_FLOW_QUERIES): the layout of gysk_flow_est */
+typedef struct gysk_flow_qry_est
+{
+	uint64_t	flow_key;
+	uint32_t	queries;		/* min over rows of the query halves */
+	uint32_t	resp_ms;		/* min over rows of the response msec halves */
+} gysk_flow_qry_est;
+
 typedef struct gysk_stats
 {
 	uint64_t	events_in;		/* events handed to the device */
@@ -399,6 +413,9 @@ int64_t		gysk_last_batch_flow_direct(gysk_engine *e);
 /* diagnostic: entries of the batch flow table left non-zero; 0 whenever no batch is in flight. Copies the table (up to 32 MB) to the
  * host. Negative = GYSK_ERR_*. */
 int64_t		gysk_flow_table_used(gysk_engine *e);
+/* diagnostic (GYSK_FLAG_FLOW_QUERIES): response samples of the last device batch whose flow query update did not go through the batch's
+ * query flow table (its probe limit reached). Routing only. GYSK_ERR_NOTSUP without the flag; negative = GYSK_ERR_*. */
+int64_t		gysk_last_batch_flow_query_direct(gysk_engine *e);
 
 /* ---- capacity: growing the service / process tables of a live engine ---- */
 /* Raise the service / process capacity of a live engine (either may equal the current value; neither may shrink, both <= 1 << 24).
@@ -433,7 +450,8 @@ int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the
  * engine of this configuration (NULL: the defaults); they depend on hll_p and on whether task_idle_evict_secs is set. An engine's footprint is about
  * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
  * buffers and the count-min tables: 2 tables of cms_depth << cms_log2_width 8-byte cells, 11 more with GYSK_FLAG_FLOW_LEVEL (its 10 ring
- * slots and the level: 352 MiB more at the default 4 x 2^20). The count-min tables do not depend on capacity, so gysk_grow leaves them.
+ * slots and the level: 352 MiB more at the default 4 x 2^20), 2 more with GYSK_FLAG_FLOW_QUERIES (64 MiB at 4 x 2^20, plus a second
+ * batch flow table of up to 32 MiB). The count-min tables do not depend on capacity, so gysk_grow leaves them.
  * Trace rows (max_trace_svcs) are not per service slot and not counted here: 3784 bytes each, in gysk_capacity.device_bytes. */
 int		gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes);
 
@@ -606,6 +624,29 @@ int		gysk_export_cms(gysk_engine *e, int last_window, uint64_t *cells /* depth <
 int		gysk_query_flows_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_est *out);
 int		gysk_export_cms_5min(gysk_engine *e, uint64_t *cells /* depth << log2_width entries */);
 int		gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_est *out);
+
+/* ---- flow queries (GYSK_FLAG_FLOW_QUERIES): requests and response time per client flow ----
+ * The connection count-min counts connections and kbytes; a pooled keep-alive client opens one connection and sends thousands of
+ * requests. These tables count the requests. They have the depth, width and row hashes of the connection count-min (gysk_export_cms), so
+ * a key lands in the same columns of both. Each cell is one u64 {queries : low 32 | response msec sum : high 32}, mod 2^64 like the
+ * connection cells; msec = usec / 1000, the step the response histogram takes.
+ * A response sample counts iff it reaches its service's response histogram: a known service (a slot) and a value within the RESP
+ * validity rule (<= 1 000 000 msec), on every route. Unknown ids, dropped events and GYSK_EV_TRACE events do not count; an API_TRAN
+ * counts through the GYSK_EV_RESP it stages. So for every row the low halves of the open window's cells sum to the nqrys of every
+ * service's open window (mod 2^32). The window rule is the count-min's: gysk_flush closes the open table and opens an empty one.
+ * The key of a sample is its event's flow_key, which each route sets as follows:
+ *   GYSK_RAW_TCP_IPV4_RESP / _IPV6_RESP : (client ip << 32) | client port (an IPv6 address folded to 32 bits), the key the same
+ *                                         client's connection events carry, so one key answers both sketches
+ *   GYSK_RAW_EVENT32, gysk_ingest_device : the feeder's flow_key
+ *   GYSK_RAW_RESP16, GYSK_RAW_API_TRAN   : the client port alone: their samples count under the port, not under a client
+ * gysk_query_flow_queries: per key the minimum over rows of each half (a count-min estimate: never below the exact count).
+ * gysk_export_cms_queries: the open (last_window = 0) or last closed table, depth << log2_width cells.
+ * gysk_query_flow_queries_global: the point query on the tables summed over the ranks by the last merge (GYSK_ERR_INVAL before
+ * gysk_merge_prepare). gysk_grow and eviction leave the tables alone: they do not depend on the service table.
+ * All three are GYSK_ERR_NOTSUP without the flag. */
+int		gysk_query_flow_queries(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_qry_est *out);
+int		gysk_export_cms_queries(gysk_engine *e, int last_window, uint64_t *cells /* depth << log2_width entries */);
+int		gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_qry_est *out);
 
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
