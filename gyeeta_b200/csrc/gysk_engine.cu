@@ -300,18 +300,46 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 static_assert(sizeof(gysk_flow_qry_est) == sizeof(gysk_flow_est) && offsetof(gysk_flow_qry_est, queries) == offsetof(gysk_flow_est, count) &&
 		offsetof(gysk_flow_qry_est, resp_ms) == offsetof(gysk_flow_est, kbytes), "a flow query row is read as a gysk_flow_est");
 
-int query_flows_in(gysk_engine *e, const unsigned long long *tbl, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what)
+int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what)
 {
-	DevState st = e->st;
-	st.cms_cur = const_cast<unsigned long long *>(tbl);
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!cms_held(e->cfg, t)) return GYSK_ERR_NOTSUP;
+	Entry entry(e, merged ? Pending::Drain : Pending::Submit);
+	if (entry.rc) return entry.rc;
+	if (merged && !e->mg.prepared) return fail(e, GYSK_ERR_INVAL, ("gysk_" + std::string(what) + ": no merge").c_str());
+	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[t].live(e);
 	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
-		return launch_query_flows(st, d_keys, m, 0, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
+		return launch_query_flows(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, m, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
 	}, CopyRows<gysk_flow_est> {out});
 }
 
 } // namespace gysk
 
 namespace {
+
+// the cells of count-min table t (gysk_export_cms and its kin), after every event handed in has run; GYSK_ERR_NOTSUP when the engine
+// does not hold t
+int export_cms(gysk_engine *e, int t, uint64_t *cells)
+{
+	CHECK_ENGINE(e);
+	if (!cells) return GYSK_ERR_INVAL;
+	if (!cms_held(e->cfg, t)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Sync);
+	CU(e, cudaMemcpy(cells, CMS_TABLES[t].live(e), sizeof(uint64_t) * cms_cells(e->cfg), cudaMemcpyDeviceToHost));
+	return GYSK_OK;
+}
+
+// diagnostic counter word ctr as of the last device batch, after every event handed in has run (kept false: 0, the engine does not
+// keep that counter)
+int64_t read_counter(gysk_engine *e, int ctr, bool kept = true)
+{
+	GYSK_ENTER(e, Sync);
+	if (!kept) return 0;
+	unsigned long long n = 0;
+	CU(e, cudaMemcpy(&n, e->st.counters + ctr, sizeof(n), cudaMemcpyDeviceToHost));
+	return (int64_t)n;
+}
 
 // the unit grid of the K_1 scale: q_j = (sin(pi (j/delta - 1/2)) + 1)/2 — libm on the host, the same expression as the oracle. The
 // device's grid and the pgtext export's compress both come from here.
@@ -586,15 +614,10 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(halloc(e, &e->h_used, 4));
 	e->h_used[3] = 0;		// processes on the free stack: stays 0 without process eviction
 	if ((ce = cudaEventCreateWithFlags(&e->ev_used, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
-	A(dalloc(e, &st.cms_cur, (size_t)cfg.cms_depth << cfg.cms_log2_width)); A(dalloc(e, &st.cms_last, (size_t)cfg.cms_depth << cfg.cms_log2_width));
-	if (cfg.flags & GYSK_FLAG_FLOW_LEVEL) {
-		// not per slot: outside each_slot_array, so gysk_grow leaves them; device_bytes counts them
-		A(dalloc(e, &st.cms_ring, (size_t)NSLOTS * ((size_t)cfg.cms_depth << cfg.cms_log2_width)));
-		A(dalloc(e, &st.cms_5min, (size_t)cfg.cms_depth << cfg.cms_log2_width));
-	}
-	if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) {		// not per slot either
-		A(dalloc(e, &e->fq.cur, (size_t)cfg.cms_depth << cfg.cms_log2_width)); A(dalloc(e, &e->fq.last, (size_t)cfg.cms_depth << cfg.cms_log2_width));
-	}
+	// the count-min tables, and with GYSK_FLAG_FLOW_LEVEL the level's ring: not per slot, outside each_slot_array, so gysk_grow leaves
+	// them; device_bytes counts them
+	for (int t = 0; t < NCMS; ++t) if (cms_held(cfg, t)) A(dalloc(e, &CMS_TABLES[t].live(e), cms_cells(cfg)));
+	if (cfg.flags & GYSK_FLAG_FLOW_LEVEL) A(dalloc(e, &st.cms_ring, NSLOTS * cms_cells(cfg)));
 	st.cms_depth = cfg.cms_depth; st.cms_log2w = cfg.cms_log2_width; st.cms_wmask = (1u << cfg.cms_log2_width) - 1; st.hll_p = cfg.hll_p;
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
 	st.td_delta = (double)cfg.td_compression;
@@ -745,11 +768,7 @@ int gysk_get_stats(gysk_engine *e, gysk_stats *out)
 int64_t gysk_hot_rows_in_use(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
-	GYSK_ENTER(e, Sync);
-	if (!e->st.hot_rows) return 0;
-	unsigned long long n = 0;
-	CU(e, cudaMemcpy(&n, e->st.counters + CTR_NHOT_NEXT, sizeof(n), cudaMemcpyDeviceToHost));
-	return (int64_t)n;
+	return read_counter(e, CTR_NHOT_NEXT, e->st.hot_rows != nullptr);
 }
 
 // introspection (no device needed): word of value bin `bin` inside a hot row's {samples | remainders} half; the usec sum of the bin
@@ -763,31 +782,22 @@ uint32_t gysk_hot_row_word(uint32_t bin)
 int64_t gysk_last_batch_keys(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
-	GYSK_ENTER(e, Sync);
-	unsigned long long n = 0;
-	CU(e, cudaMemcpy(&n, e->st.counters + CTR_NKEYS, sizeof(n), cudaMemcpyDeviceToHost));
-	return (int64_t)n;
+	return read_counter(e, CTR_NKEYS);
 }
 
 // diagnostic: connection records of the last device batch whose count-min update bypassed the flow table
 int64_t gysk_last_batch_flow_direct(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
-	GYSK_ENTER(e, Sync);
-	unsigned long long n = 0;
-	CU(e, cudaMemcpy(&n, e->st.counters + CTR_FLOW_DIRECT, sizeof(n), cudaMemcpyDeviceToHost));
-	return (int64_t)n;
+	return read_counter(e, CTR_FLOW_DIRECT);
 }
 
 // diagnostic: response samples of the last device batch whose flow query update bypassed the query flow table (GYSK_FLAG_FLOW_QUERIES)
 int64_t gysk_last_batch_flow_query_direct(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
-	if (!e->fq.cur) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Sync);
-	unsigned long long n = 0;
-	CU(e, cudaMemcpy(&n, e->st.counters + CTR_FLOWQ_DIRECT, sizeof(n), cudaMemcpyDeviceToHost));
-	return (int64_t)n;
+	if (!cms_held(e->cfg, CMS_QRY_CUR)) return GYSK_ERR_NOTSUP;
+	return read_counter(e, CTR_FLOWQ_DIRECT);
 }
 
 // diagnostic: entries of the flow table (and of the query flow table, GYSK_FLAG_FLOW_QUERIES) that are not zero (a key or a sum left
@@ -1559,11 +1569,11 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->evict_pending = true;
 	}
 	if (e->st.cms_ring) e->kernel_launches += launch_cms_level_roll(e->st, e->stream);		// GYSK_FLAG_FLOW_LEVEL
-	std::swap(e->st.cms_cur, e->st.cms_last);
-	CU(e, cudaMemsetAsync(e->st.cms_cur, 0, sizeof(unsigned long long) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), e->stream));
-	if (e->fq.cur) {		// GYSK_FLAG_FLOW_QUERIES: the same window rule
-		std::swap(e->fq.cur, e->fq.last);
-		CU(e, cudaMemsetAsync(e->fq.cur, 0, sizeof(unsigned long long) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), e->stream));
+	for (int t : {CMS_CUR, CMS_QRY_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
+		if (!cms_held(e->cfg, t)) continue;
+		unsigned long long *&open = CMS_TABLES[t].live(e);
+		std::swap(open, CMS_TABLES[t + 1].live(e));
+		CU(e, cudaMemsetAsync(open, 0, sizeof(unsigned long long) * cms_cells(e->cfg), e->stream));
 	}
 	return post_launch(e, "flush");
 }
@@ -1976,29 +1986,18 @@ int gysk_query_quantiles(gysk_engine *e, uint64_t id, const double *qs, uint32_t
 
 int gysk_query_flows(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_est *out)
 {
-	CHECK_ENGINE(e);
-	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e, Submit);
-	return query_flows_in(e, last_window ? e->st.cms_last : e->st.cms_cur, keys, n, out, "query_flows");
+	return query_cms(e, last_window ? CMS_LAST : CMS_CUR, false, keys, n, out, "query_flows");
 }
 
 int gysk_query_flows_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_est *out)
 {
-	CHECK_ENGINE(e);
-	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Submit);
-	return query_flows_in(e, e->st.cms_5min, keys, n, out, "query_flows_5min");
+	return query_cms(e, CMS_5MIN, false, keys, n, out, "query_flows_5min");
 }
 
 // GYSK_FLAG_FLOW_QUERIES: the point query of gysk_query_flows on the flow query tables; gysk_flow_qry_est is gysk_flow_est's layout
 int gysk_query_flow_queries(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_qry_est *out)
 {
-	CHECK_ENGINE(e);
-	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_FLOW_QUERIES)) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Submit);
-	return query_flows_in(e, last_window ? e->fq.last : e->fq.cur, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries");
+	return query_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, false, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries");
 }
 
 int gysk_topn_svcs(gysk_engine *e, int metric, int32_t host_idx, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
@@ -2073,33 +2072,17 @@ int gysk_topn_host(gysk_engine *e, int what, int32_t host_idx, uint32_t n, gysk_
 
 int gysk_export_cms(gysk_engine *e, int last_window, uint64_t *cells)
 {
-	CHECK_ENGINE(e);
-	if (!cells) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e, Sync);
-	CU(e, cudaMemcpy(cells, last_window ? e->st.cms_last : e->st.cms_cur, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width),
-			cudaMemcpyDeviceToHost));
-	return GYSK_OK;
+	return export_cms(e, last_window ? CMS_LAST : CMS_CUR, cells);
 }
 
 int gysk_export_cms_5min(gysk_engine *e, uint64_t *cells)
 {
-	CHECK_ENGINE(e);
-	if (!cells) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Sync);
-	CU(e, cudaMemcpy(cells, e->st.cms_5min, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width), cudaMemcpyDeviceToHost));
-	return GYSK_OK;
+	return export_cms(e, CMS_5MIN, cells);
 }
 
 int gysk_export_cms_queries(gysk_engine *e, int last_window, uint64_t *cells)
 {
-	CHECK_ENGINE(e);
-	if (!cells) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_FLOW_QUERIES)) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Sync);
-	CU(e, cudaMemcpy(cells, last_window ? e->fq.last : e->fq.cur, sizeof(uint64_t) * ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width),
-			cudaMemcpyDeviceToHost));
-	return GYSK_OK;
+	return export_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, cells);
 }
 
 // ---- pure helpers ------------------------------------------------------------------------------------------------

@@ -237,6 +237,14 @@ static_assert(TopnLists::SVC_ROW % 16 == 0 && TopnLists::TASK_ROW % 16 == 0 && s
 // the candidates' whole SlabEntrys after a rank's nl digests
 constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
 
+// The count-min tables an engine can hold, each [cms_depth][1 << cms_log2_width] cells (CMS_TABLES below says which flag each one
+// needs, its array in the merge arena and where the engine keeps it). Each windowed pair is an open table and, right after it, the
+// table of the window the last flush closed.
+enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, NCMS };
+
+// the cells of one count-min table
+inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
+
 // per-logical-service state of the merge step (SURVEY.md §8e)
 struct MergeState
 {
@@ -257,9 +265,7 @@ struct MergeState
 									//           [, trace max]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
 	std::string		name_sum, name_maxi64, name_maxu8;	// the regions' gysk_buffer_desc names: their arrays, in order
-	unsigned long long	*g_cms_cur {nullptr}, *g_cms_last {nullptr};
-	unsigned long long	*g_cms_5min {nullptr};				// GYSK_FLAG_FLOW_LEVEL: the count-min level, summed over ranks
-	unsigned long long	*g_cmsq_cur {nullptr}, *g_cmsq_last {nullptr};	// GYSK_FLAG_FLOW_QUERIES: the flow query tables, summed over ranks
+	unsigned long long	*g_cms[NCMS] {};			// the engine's count-min tables summed over ranks (nullptr: not held)
 	LogicalArrays		lg;
 	ClusterMap		clusters;				// kept across gysk_set_logical_map
 	bool			prepared {false}, finished {false};
@@ -363,6 +369,23 @@ namespace gysk {
 // slot_last_active of the window the last flush closed (state_kernel): the active_mark of svc_evaluated / svc_issue
 inline uint32_t active_mark(const gysk_engine *e) { return e->last_flush_tsec ? e->last_flush_tsec : 1u; }
 
+// one count-min table of CmsTable: the gysk_config flag it needs (0: every engine holds it), its array in the merge arena's SUM region
+// (gysk_merge_buffers), and the engine's live table
+struct CmsTableDesc
+{
+	uint32_t		flag;
+	const char		*name;
+	unsigned long long	*&(*live)(gysk_engine *);
+};
+inline const CmsTableDesc CMS_TABLES[NCMS] = {
+	{0, "cms_cur", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_cur; }},
+	{0, "cms_last", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_last; }},
+	{GYSK_FLAG_FLOW_LEVEL, "cms_5min", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_5min; }},
+	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_cur", [](gysk_engine *e) -> unsigned long long *& { return e->fq.cur; }},
+	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_last", [](gysk_engine *e) -> unsigned long long *& { return e->fq.last; }},
+};
+inline bool cms_held(const gysk_config &cfg, int t) { return !CMS_TABLES[t].flag || (cfg.flags & CMS_TABLES[t].flag); }
+
 int fail(gysk_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess);
 int post_launch(gysk_engine *e, const char *what);
 int submit_stage(gysk_engine *e);
@@ -379,8 +402,9 @@ void hist_from_cells(const HistCell *cells, int nb, gysk_hist_serial *out, uint6
 void level_from_cells(const HistCell *cells, gysk_hist_serial *out, uint64_t *total, int64_t *maxv);
 // the gysk_export_tdigest answer of one digest: up to min(cap, TD_CAP) centroids, min and max; GYSK_ERR_NOSPC when it has more than cap
 int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_t *weights, uint32_t cap, uint32_t *n, double *minv, double *maxv);
-// the count-min point queries of gysk_query_flows on table tbl (one of the engine's tables, a merged one or a level), engine held
-int query_flows_in(gysk_engine *e, const unsigned long long *tbl, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
+// The count-min point queries of the flow query ABI calls on table t: the engine's own (the batch of the events handed in runs first) or,
+// merged, the last merge's sum over the ranks. GYSK_ERR_NOTSUP when the engine does not hold t; `what` names the call.
+int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)

@@ -289,6 +289,13 @@ __device__ __forceinline__ IngestRec ld_rec(const IngestRec *p)
 	return r;
 }
 
+// inc into the cells of the flow with hashes h1, h2 in count-min table cms (the geometry of st), one RED per row
+__device__ __forceinline__ void cms_add(const DevState &st, unsigned long long *cms, uint32_t h1, uint32_t h2, unsigned long long inc)
+{
+	for (uint32_t row = 0; row < st.cms_depth; ++row)
+		red_add_u64(cms + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
+}
+
 // One connection record's count-min increment into the batch's flow table, given the key k of entry pos (the first probe): a RED into the
 // flow's entry, claimed with a CAS on the key if need be. Past FLOW_PROBES entries, or for key 0, the record updates its count-min
 // cells (cms) directly (normal priority: nothing is left for the TASK pass to reset) and is counted in counter ctr, one RED per group of
@@ -309,9 +316,7 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 	}
 	const uint32_t am = __activemask();
 	if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(st.counters + ctr, (unsigned long long)__popc(am));
-	const uint32_t h1 = (uint32_t)key, h2 = (uint32_t)(key >> 32);
-	for (uint32_t row = 0; row < st.cms_depth; ++row)
-		red_add_u64(cms + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
+	cms_add(st, cms, (uint32_t)key, (uint32_t)(key >> 32), inc);
 }
 
 // m queued connection records (all 32 lanes call): two lookup2 hashes per flow key -> the flow's entry in the batch's flow table (the
@@ -661,6 +666,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					const unsigned long long inc = (unsigned long long)(rb[k].w >> 16) | ((unsigned long long)rb[k].x << 32);
 					uint32_t h1, h2, idx, rank;
 					flow_hashes(fk, h1, h2);
+					// cms_add written out: the call changes the register allocation of every ingest_kernel instance
 					for (uint32_t row = 0; row < st.cms_depth; ++row)
 						red_add_u64(st.cms_cur + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
 					hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
@@ -762,9 +768,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 			for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
 				const uint32_t i = i0 + u * stride;
 				if (f[u].key) {
-					const uint32_t h1 = (uint32_t)f[u].key, h2 = (uint32_t)(f[u].key >> 32);
-					for (uint32_t row = 0; row < st.cms_depth; ++row)
-						red_add_u64(st.cms_cur + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), f[u].inc);
+					cms_add(st, st.cms_cur, (uint32_t)f[u].key, (uint32_t)(f[u].key >> 32), f[u].inc);
 					ft.ent[i] = FlowEnt {0ull, 0ull};
 				}
 				if (i <= ft.mask && !(i & 7u)) l2_evict_normal_line(ft.ent + i);
@@ -783,9 +787,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 				for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
 					const uint32_t i = i0 + u * stride;
 					if (f[u].key) {
-						const uint32_t h1 = (uint32_t)f[u].key, h2 = (uint32_t)(f[u].key >> 32);
-						for (uint32_t row = 0; row < st.cms_depth; ++row)
-							red_add_u64(cms + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), f[u].inc);
+						cms_add(st, cms, (uint32_t)f[u].key, (uint32_t)(f[u].key >> 32), f[u].inc);
 						t.ent[i] = FlowEnt {0ull, 0ull};
 					}
 					if (i <= t.mask && !(i & 7u)) l2_evict_normal_line(t.ent + i);
@@ -2168,16 +2170,16 @@ __global__ void gather_hll_kernel(DevState st, const unsigned long long *__restr
 	for (uint32_t i = threadIdx.x; i < (1u << st.hll_p); i += blockDim.x) out[i] = regs[i];
 }
 
-__global__ void query_flows_kernel(DevState st, const unsigned long long *__restrict__ keys, uint32_t n, int last_window, gysk_flow_est *__restrict__ out)
+__global__ void query_flows_kernel(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, const unsigned long long *__restrict__ keys,
+		uint32_t n, gysk_flow_est *__restrict__ out)
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
-	const unsigned long long *tbl = last_window ? st.cms_last : st.cms_cur;
 	const unsigned long long key = keys[i];
 	uint32_t cnt = 0xFFFFFFFFu, kb = 0xFFFFFFFFu;
 
-	for (uint32_t r = 0; r < st.cms_depth; ++r) {
-		const unsigned long long c = tbl[((size_t)r << st.cms_log2w) + cms_index(key, r, st.cms_wmask)];
+	for (uint32_t r = 0; r < depth; ++r) {
+		const unsigned long long c = tbl[((size_t)r << log2w) + cms_index(key, r, (1u << log2w) - 1)];
 		cnt = min(cnt, (uint32_t)c);
 		kb = min(kb, (uint32_t)(c >> 32));
 	}
@@ -2626,10 +2628,11 @@ int launch_gather_hll(const DevState &st, const unsigned long long *d_ids, int32
 	return 1;
 }
 
-int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uint32_t n, int last_window, gysk_flow_est *d_out, cudaStream_t s)
+int launch_query_flows(const unsigned long long *tbl, uint32_t depth, uint32_t log2w, const unsigned long long *d_keys, uint32_t n, gysk_flow_est *d_out,
+		cudaStream_t s)
 {
 	if (!n) return 0;
-	query_flows_kernel<<<div_up(n, 256), 256, 0, s>>>(st, d_keys, n, last_window, d_out);
+	query_flows_kernel<<<div_up(n, 256), 256, 0, s>>>(tbl, depth, log2w, d_keys, n, d_out);
 	return 1;
 }
 

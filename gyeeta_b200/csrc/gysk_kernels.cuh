@@ -285,7 +285,9 @@ int launch_svc_summaries(const DevState &st, const unsigned long long *d_ids, co
 		cudaStream_t s);
 int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n, gysk_task_summary *d_out,
 		cudaStream_t s);
-int launch_query_flows(const DevState &st, const unsigned long long *d_keys, uint32_t n, int last_window, gysk_flow_est *d_out, cudaStream_t s);
+// the count-min point queries of n flow keys on table tbl ([depth][1 << log2w] cells)
+int launch_query_flows(const unsigned long long *tbl, uint32_t depth, uint32_t log2w, const unsigned long long *d_keys, uint32_t n, gysk_flow_est *d_out,
+		cudaStream_t s);
 // GYSK_FLAG_FLOW_LEVEL, at the flush before the cms_cur / cms_last swap: cms_cur into ring slot st.levels.cur[0] (replacing it when
 // the slot is fresh), then cms_5min = the sum of the live slots
 int launch_cms_level_roll(const DevState &st, cudaStream_t s);

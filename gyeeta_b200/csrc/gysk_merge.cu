@@ -820,8 +820,7 @@ int lay_out_arena(gysk_engine *e)
 	// tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
 	const bool flow_level = e->cfg.flags & GYSK_FLAG_FLOW_LEVEL, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
-	const bool flow_queries = e->cfg.flags & GYSK_FLAG_FLOW_QUERIES;
-	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8, b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
+	const size_t b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
 		std::string names;
@@ -831,9 +830,7 @@ int lay_out_arena(gysk_engine *e)
 			names += (names.empty() ? "" : "|") + std::string(name);
 		};
 		mg.off_sum = off;
-		take(mg.g_cms_cur, b_cms, "cms_cur"); take(mg.g_cms_last, b_cms, "cms_last");
-		if (flow_level) take(mg.g_cms_5min, b_cms, "cms_5min");
-		if (flow_queries) { take(mg.g_cmsq_cur, b_cms, "cms_qry_cur"); take(mg.g_cmsq_last, b_cms, "cms_qry_last"); }
+		for (int t = 0; t < NCMS; ++t) if (cms_held(e->cfg, t)) take(mg.g_cms[t], cms_cells(e->cfg) * 8, CMS_TABLES[t].name);
 		take(lg.last, b_hist, "hist_last"); take(lg.all, b_hist, "hist_all"); take(lg.conn, (size_t)nl * 4 * 8, "conn");
 		if (levels) { take(lg.lvl, NLEVELS * b_hist, "levels"); take(lg.aux, (size_t)nl * 4 * 8, "aux"); }
 		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8, "states");
@@ -998,16 +995,10 @@ int gysk_merge_prepare(gysk_engine *e)
 	}
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_prepare: call gysk_set_logical_map first");
 
-	const size_t b_cms = ((size_t)e->cfg.cms_depth << e->cfg.cms_log2_width) * 8;
 	const uint32_t nl = mg.lg.nl;
 
-	CU(e, cudaMemcpyAsync(mg.g_cms_cur, e->st.cms_cur, b_cms, cudaMemcpyDeviceToDevice, e->stream));
-	CU(e, cudaMemcpyAsync(mg.g_cms_last, e->st.cms_last, b_cms, cudaMemcpyDeviceToDevice, e->stream));
-	if (mg.g_cms_5min) CU(e, cudaMemcpyAsync(mg.g_cms_5min, e->st.cms_5min, b_cms, cudaMemcpyDeviceToDevice, e->stream));		// GYSK_FLAG_FLOW_LEVEL
-	if (mg.g_cmsq_cur) {		// GYSK_FLAG_FLOW_QUERIES
-		CU(e, cudaMemcpyAsync(mg.g_cmsq_cur, e->fq.cur, b_cms, cudaMemcpyDeviceToDevice, e->stream));
-		CU(e, cudaMemcpyAsync(mg.g_cmsq_last, e->fq.last, b_cms, cudaMemcpyDeviceToDevice, e->stream));
-	}
+	for (int t = 0; t < NCMS; ++t)
+		if (mg.g_cms[t]) CU(e, cudaMemcpyAsync(mg.g_cms[t], CMS_TABLES[t].live(e), cms_cells(e->cfg) * 8, cudaMemcpyDeviceToDevice, e->stream));
 	if (nl) {
 		if (mg.nmembers) {
 			resolve_members_kernel<<<div_up(mg.nmembers, 256), 256, 0, e->stream>>>(e->st, mg.d_member_ids, mg.nmembers, mg.members);
@@ -1299,36 +1290,19 @@ int gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tse
 // global count-min point query on the merged table
 int gysk_query_flows_global(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_est *out)
 {
-	CHECK_ENGINE(e);
-	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	GYSK_ENTER(e, Drain);
-	MergeState &mg = e->mg;
-	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global: no merge");
-	return query_flows_in(e, last_window ? mg.g_cms_last : mg.g_cms_cur, keys, n, out, "query_flows_global");
+	return query_cms(e, last_window ? CMS_LAST : CMS_CUR, true, keys, n, out, "query_flows_global");
 }
 
 // GYSK_FLAG_FLOW_LEVEL: the point query on the count-min level summed over the ranks
 int gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_est *out)
 {
-	CHECK_ENGINE(e);
-	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_FLOW_LEVEL)) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Drain);
-	MergeState &mg = e->mg;
-	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flows_global_5min: no merge");
-	return query_flows_in(e, mg.g_cms_5min, keys, n, out, "query_flows_global_5min");
+	return query_cms(e, CMS_5MIN, true, keys, n, out, "query_flows_global_5min");
 }
 
 // GYSK_FLAG_FLOW_QUERIES: the point query on the flow query tables summed over the ranks
 int gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_qry_est *out)
 {
-	CHECK_ENGINE(e);
-	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & GYSK_FLAG_FLOW_QUERIES)) return GYSK_ERR_NOTSUP;
-	GYSK_ENTER(e, Drain);
-	MergeState &mg = e->mg;
-	if (!mg.prepared) return fail(e, GYSK_ERR_INVAL, "gysk_query_flow_queries_global: no merge");
-	return query_flows_in(e, last_window ? mg.g_cmsq_last : mg.g_cmsq_cur, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_global");
+	return query_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, true, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_global");
 }
 
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)

@@ -556,33 +556,28 @@ class Engine:
         self._chk(self.L.gysk_get_stats(self.h, C.byref(s)))
         return s.asdict()
 
-    def hot_rows_in_use(self):
-        """rows of dense value bins handed out to hot services so far (diagnostic; results never depend on it)"""
-        n = self.L.gysk_hot_rows_in_use(self.h)
+    def _counter(self, fn):
+        """one int64 diagnostic of fn (a negative value is an error code)"""
+        n = fn(self.h)
         if n < 0:
             self._chk(int(n))
         return int(n)
+
+    def hot_rows_in_use(self):
+        """rows of dense value bins handed out to hot services so far (diagnostic; results never depend on it)"""
+        return self._counter(self.L.gysk_hot_rows_in_use)
 
     def last_batch_keys(self):
         """response samples of the last device batch that travelled as sort keys (diagnostic)"""
-        n = self.L.gysk_last_batch_keys(self.h)
-        if n < 0:
-            self._chk(int(n))
-        return int(n)
+        return self._counter(self.L.gysk_last_batch_keys)
 
     def last_batch_flow_direct(self):
         """connection records of the last device batch whose count-min update bypassed the flow table (diagnostic)"""
-        n = self.L.gysk_last_batch_flow_direct(self.h)
-        if n < 0:
-            self._chk(int(n))
-        return int(n)
+        return self._counter(self.L.gysk_last_batch_flow_direct)
 
     def last_batch_flow_query_direct(self):
         """response samples of the last device batch whose flow query update bypassed the query flow table (flow_queries=True)"""
-        n = self.L.gysk_last_batch_flow_query_direct(self.h)
-        if n < 0:
-            self._chk(int(n))
-        return int(n)
+        return self._counter(self.L.gysk_last_batch_flow_query_direct)
 
     def flow_table_used(self):
         """non-zero entries of the batch flow tables (the query one too with flow_queries=True): 0 whenever no batch is in flight
@@ -670,25 +665,29 @@ class Engine:
         """gysk_query_task_window: (TaskSummary rows in the order of query_window, number of matching rows)"""
         return self._window(self.L.gysk_query_task_window, TaskSummary, (host_idx,), active_only, cap)
 
-    def query_flows(self, keys, last_window=False):
+    def _point_query(self, fn, dtype, keys, *window):
+        """a count-min point query fn(h, keys, n, [last_window,] out): one row of dtype per key"""
         keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
-        self._chk(self.L.gysk_query_flows(self.h, _p(keys), len(keys), int(last_window), _p(out)))
+        out = np.zeros(len(keys), dtype=dtype)
+        self._chk(fn(self.h, _p(keys), len(keys), *window, _p(out)))
         return out
+
+    def _export_cells(self, fn, *window):
+        """the cells of a count-min table, fn(h, [last_window,] cells)"""
+        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
+        self._chk(fn(self.h, *window, _p(out)))
+        return out
+
+    def query_flows(self, keys, last_window=False):
+        return self._point_query(self.L.gysk_query_flows, FLOW_EST_DTYPE, keys, int(last_window))
 
     def query_flows_5min(self, keys):
         """gysk_query_flows_5min: the point query on the rolling 300-s count-min level (flow_level=True)"""
-        keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
-        self._chk(self.L.gysk_query_flows_5min(self.h, _p(keys), len(keys), _p(out)))
-        return out
+        return self._point_query(self.L.gysk_query_flows_5min, FLOW_EST_DTYPE, keys)
 
     def query_flow_queries(self, keys, last_window=False):
         """gysk_query_flow_queries: requests and response msec per flow key, min over rows (flow_queries=True)"""
-        keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        out = np.zeros(len(keys), dtype=FLOW_QRY_EST_DTYPE)
-        self._chk(self.L.gysk_query_flow_queries(self.h, _p(keys), len(keys), int(last_window), _p(out)))
-        return out
+        return self._point_query(self.L.gysk_query_flow_queries, FLOW_QRY_EST_DTYPE, keys, int(last_window))
 
     def topn(self, metric, n=10, host_idx=-1):
         out = (TopnEntry * n)()
@@ -957,38 +956,23 @@ class Engine:
         return lo.value, hi.value
 
     def query_flows_global(self, keys, last_window=False):
-        keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
-        self._chk(self.L.gysk_query_flows_global(self.h, _p(keys), len(keys), int(last_window), _p(out)))
-        return out
+        return self._point_query(self.L.gysk_query_flows_global, FLOW_EST_DTYPE, keys, int(last_window))
 
     def query_flows_global_5min(self, keys):
         """gysk_query_flows_global_5min: the point query on the 300-s count-min level summed over the ranks by the last merge"""
-        keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        out = np.zeros(len(keys), dtype=FLOW_EST_DTYPE)
-        self._chk(self.L.gysk_query_flows_global_5min(self.h, _p(keys), len(keys), _p(out)))
-        return out
+        return self._point_query(self.L.gysk_query_flows_global_5min, FLOW_EST_DTYPE, keys)
 
     def export_cms(self, last_window=False):
-        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
-        self._chk(self.L.gysk_export_cms(self.h, int(last_window), _p(out)))
-        return out
+        return self._export_cells(self.L.gysk_export_cms, int(last_window))
 
     def export_cms_queries(self, last_window=False):
         """gysk_export_cms_queries: the cells {queries | resp msec << 32} of the flow query table (flow_queries=True)"""
-        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
-        self._chk(self.L.gysk_export_cms_queries(self.h, int(last_window), _p(out)))
-        return out
+        return self._export_cells(self.L.gysk_export_cms_queries, int(last_window))
 
     def query_flow_queries_global(self, keys, last_window=False):
         """gysk_query_flow_queries_global: the point query on the flow query tables summed over the ranks by the last merge"""
-        keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        out = np.zeros(len(keys), dtype=FLOW_QRY_EST_DTYPE)
-        self._chk(self.L.gysk_query_flow_queries_global(self.h, _p(keys), len(keys), int(last_window), _p(out)))
-        return out
+        return self._point_query(self.L.gysk_query_flow_queries_global, FLOW_QRY_EST_DTYPE, keys, int(last_window))
 
     def export_cms_5min(self):
         """gysk_export_cms_5min: the cells of the rolling 300-s count-min level (flow_level=True)"""
-        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
-        self._chk(self.L.gysk_export_cms_5min(self.h, _p(out)))
-        return out
+        return self._export_cells(self.L.gysk_export_cms_5min)
