@@ -1124,6 +1124,9 @@ int ingest_raw_bulk(gysk_engine *e, ThreadStage *ts, uint32_t kind, uint32_t hos
 		e->raw_cur = (r + 1) % NBUF;
 		src += m * stride; n -= m;
 	}
+	// cur now names the chunk of the piece before last (or the one flush_stage handed over), whose copy may still wait behind the
+	// compute stream: the next staged record of this thread, or of the thread that adopts this stage, is written into it at once
+	if (!pinned) CU(e, cudaEventSynchronize(ts->copied[ts->cur]));
 	return post_launch(e, "raw decode");
 }
 

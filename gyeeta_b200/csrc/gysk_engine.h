@@ -27,7 +27,8 @@ constexpr uint32_t RAW_BULK_MIN = 16384;		// raw fixed-stride batches from this 
 							// per-call copy / launch / event calls under the engine mutex cost more than the
 							// ~20 ns per record of expanding on the calling thread (bench.py e2e_wire)
 
-// a calling thread's page-locked staging: filled without the engine mutex (see gysk_engine.cu)
+// a calling thread's page-locked staging: filled without the engine mutex (see gysk_engine.cu). Invariant whenever m is released:
+// buf[cur] has no H2D copy in flight, so a staging write into it never waits (the other chunk's copy may still be queued)
 struct ThreadStage
 {
 	std::mutex		m;
