@@ -28,7 +28,6 @@
 #include <cmath>
 #include <algorithm>
 #include <type_traits>
-#include <cstdlib>
 #include <cstring>
 
 namespace gysk {
@@ -52,13 +51,6 @@ static_assert(KEY_PASSES_MAX <= OS_MAX_PASSES, "a RESP plan fits a SortPlan");
 // from the plan, os_pass_kernel gets its pass's shift and width.
 struct SortPlan { int np; int shift[OS_MAX_PASSES]; int bits[OS_MAX_PASSES]; };
 __device__ __forceinline__ uint32_t sort_digit(unsigned long long k, int shift, int bits) { return (uint32_t)(k >> shift) & ((1u << bits) - 1u); }
-
-// exp: ABLATION switches for timing runs only (GYSK_EXP_ABLATE; results are wrong when set): 1 = no batch-extreme / CONN_BITMAP loads and
-// atomics, 2 = no digit histograms, 4 = no TCP drain pass, 8 = TASK drain pass without the process records (its flow-table sweep
-// stays), 16 = TCP drain pass without the count-min updates (neither the flow table nor the cells),
-// 32 = TCP drain pass without the HLL register peek / raise, 64 = TASK drain pass drops the updates that miss the CTA's hot table (the
-// end-of-CTA flush stays), 128 = TASK drain pass loads the records and computes the buckets but applies nothing, 256 = bins_merge_kernel
-// builds the items and histogram cells but skips warp_merge_compress and the digest header update
 
 // ---------------------------------------------------------------------------------------------------
 // state init / registration
@@ -196,9 +188,8 @@ __device__ __forceinline__ void cell_add_global(const DevState &st, uint32_t cel
 // Group sums use a shuffle loop bounded by the largest group of the warp (typically 1-4): redux with per-lane masks would
 // make the compiler iterate over every distinct group. No global load anywhere: the updates are fire-and-forget REDs.
 // A cell that misses the table takes a free candidate entry when it shows up ADMIT times in this call (on first sight with ADMIT = 1).
-// to_global == false (timing runs only, GYSK_EXP_ABLATE bit 64) drops the updates that miss the hot table.
 template <int ADMIT = 2, typename HotTable>
-__device__ __forceinline__ void cell_add(const DevState &st, HotTable &hot, bool active, uint32_t cell, int data, bool to_global = true)
+__device__ __forceinline__ void cell_add(const DevState &st, HotTable &hot, bool active, uint32_t cell, int data)
 {
 	const int lane = threadIdx.x & 31;
 	const uint32_t id = active ? cell : (0x80000000u | (uint32_t)lane);
@@ -235,7 +226,7 @@ __device__ __forceinline__ void cell_add(const DevState &st, HotTable &hot, bool
 		}
 	}
 	if (hit) { atomicAdd(&hot.count[h], cnt); atomicAdd(&hot.sum[h], (unsigned long long)sum); atomicMax(&hot.vmax[h], gmax); }
-	else if (to_global) cell_add_global(st, cell, cnt, (unsigned long long)sum, gmax);
+	else cell_add_global(st, cell, cnt, (unsigned long long)sum, gmax);
 }
 
 // HLL register update in two halves, so that the caller can put other work between the load of the register word and its use
@@ -325,12 +316,11 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // evict-first (ld_rec). At normal priority the 20 M HLL sectors of a 100 M-event batch, spread over hundreds of MB by the services' Zipf
 // tail, pushed the 32 MB of randomly updated lines out of the 50 MB L2 and many REDs became DRAM read-modify-writes. The drain_kernel
 // TASK pass sets the lines back to evict_normal. pol_hll / pol_last: l2_policy_evict_first / _last.
-// exp (timing runs only): 16 = no count-min updates (neither flow table nor cells), 32 = no HLL peek / raise
 // QRY (GYSK_FLAG_FLOW_QUERIES): a record with slot QRY_REC is a response sample {usec, flow key}; it adds {1 | msec << 32} to its flow's
 // entry of the query flow table fq (cells fq_cms past the probe limit) and touches neither the HLL nor a service cell.
 template <bool QRY, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
-		int lane, unsigned long long pol_hll, unsigned long long pol_last, int exp, const FlowTable &fq, unsigned long long *fq_cms)
+		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
@@ -346,7 +336,7 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 			flow_hashes(r.flow_key, h1, h2);
 			// the HLL register word and the flow table's first probe are asked for together and looked at after the cell update, which
 			// hides their latency (a stale register is harmless: the CAS re-validates)
-			if (!(exp & 32) && !qry) {
+			if (!qry) {
 				hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
 				hw = ld_na_hint_u32(reinterpret_cast<const uint32_t *>(st.hll + ((size_t)r.slot << st.hll_p)) + (idx >> 2), pol_hll);
 			}
@@ -354,26 +344,24 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 			// usec -> msec as the histogram takes it (ingest_kernel)
 			inc = qry ? 1ull | ((unsigned long long)(r.value / 1000u) << 32) : cms_increment(r.value);
 			pos = table_hash(key) & tmask;
-			if (key && !(exp & 16)) k = ld_cg_hint_u64(&tent[pos].key, pol_last);
+			if (key) k = ld_cg_hint_u64(&tent[pos].key, pol_last);
 			cell = r.slot;
 			kb = (int)(r.value >> 10);
 		}
 		cell_add(st, hot, act && !qry, cell, kb);
-		if (act && !(exp & 16)) {
+		if (act) {
 			if (qry) flow_add(st, fq, fq_cms, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
 			else flow_add(st, ft, st.cms_cur, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last);
 		}
-		if (act && !qry && !(exp & 32)) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
+		if (act && !qry) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
 	}
 }
 
 // one group of queued process records, one record per lane (act: the lane holds one): the three histograms of
 // MAGGR_TASK::set_local_task_state, one cell_add per histogram over the whole warp, so that the records of a busy process are summed
 // over the group before they reach the hot table or L2.
-// exp (timing runs only): 64 = updates that miss the hot table are dropped, 128 = nothing is applied (sink keeps the loads and
-// buckets alive)
 template <int ADMIT, typename HotTable>
-__device__ __forceinline__ void drain_task_group(const DevState &st, HotTable &hot, const IngestRec &r, bool act, int exp, uint32_t &sink)
+__device__ __forceinline__ void drain_task_group(const DevState &st, HotTable &hot, const IngestRec &r, bool act)
 {
 	// GY_HISTOGRAM<int, ...>::add_data(int): the three values narrow to int (server/gy_msocket.h:1014-1016)
 	const int d[3] = {(int)r.value, (int)(uint32_t)r.flow_key, (int)(uint32_t)(r.flow_key >> 32)};
@@ -384,10 +372,7 @@ __device__ __forceinline__ void drain_task_group(const DevState &st, HotTable &h
 		cell[h] = CELL_TASK | (r.slot * 3u * HIST_CELLS + h * HIST_CELLS + b);
 	}
 #pragma unroll
-	for (int h = 0; h < 3; ++h) {
-		if (exp & 128) sink += act ? cell[h] : 0u;
-		else cell_add<ADMIT>(st, hot, act, cell[h], d[h], !(exp & 64));
-	}
+	for (int h = 0; h < 3; ++h) cell_add<ADMIT>(st, hot, act, cell[h], d[h]);
 }
 
 
@@ -478,7 +463,7 @@ struct IngestShared
 // hot-row route, also joins the connection queue as a record {QRY_REC, usec, flow key} for the TCP drain pass.
 template <bool TRACE, bool QRY>
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
-		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, int exp)
+		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt)
 {
 	constexpr int WARPS = IngestShape::WARPS, EPT = IngestShape::EPT, CHUNK = IngestShape::CHUNK, DH = IngestShared::DH;
 	extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -530,7 +515,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 			const unsigned long long k = W.kq[q];
 #pragma unroll
 			for (int p = 0; p < KEY_PASSES_MAX; ++p)
-				if (p < plan.np && !(exp & 2)) atomicAdd(&S.dhist[p][sort_digit(k, plan.shift[p], plan.bits[p])], 1u);
+				if (p < plan.np) atomicAdd(&S.dhist[p][sort_digit(k, plan.shift[p], plan.bits[p])], 1u);
 			__stcs(keys + base + q, k);
 		}
 		nk = 0;
@@ -599,11 +584,8 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 				const uint32_t v = rb[k].x, ms = v / 1000u;		// usec -> msec as SVC_INFO_CAP::upd_stats_on_req (gy_proto_parser.cc:2678)
 				const uint32_t b = (uint32_t)bucket_resp_time((long long)ms);
 				bkt[k] = b;
-				if (!(exp & 1)) {
-					sbv[k] = ld_cg_v4(st.slot_batch + slot);
-					mwv[k] = __ldcg(st.bm_cur + (size_t)slot * HIST_CELLS + b);
-				}
-				else { sbv[k] = make_uint4(0u, 0xFFFFFFFFu, 0u, 0u); mwv[k] = 0xFFFFFFFFu; }
+				sbv[k] = ld_cg_v4(st.slot_batch + slot);
+				mwv[k] = __ldcg(st.bm_cur + (size_t)slot * HIST_CELLS + b);
 				n_resp++;
 			}
 		}
@@ -666,9 +648,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					const unsigned long long inc = (unsigned long long)(rb[k].w >> 16) | ((unsigned long long)rb[k].x << 32);
 					uint32_t h1, h2, idx, rank;
 					flow_hashes(fk, h1, h2);
-					// cms_add written out: the call changes the register allocation of every ingest_kernel instance
-					for (uint32_t row = 0; row < st.cms_depth; ++row)
-						red_add_u64(st.cms_cur + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
+					cms_add(st, st.cms_cur, h1, h2, inc);
 					hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
 					hll_update(st.hll + ((size_t)slot << st.hll_p), idx, rank);
 					red_add_u64(&st.slot_aux[slot].act_cur, inc);
@@ -742,6 +722,30 @@ template <> struct DrainShape<false> { static constexpr int WARPS = 8, HOT_BITS 
 // cost three L2 REDs each, and they were most of the pass's time
 template <> struct DrainShape<true> { static constexpr int WARPS = 16, HOT_BITS = 13, ADMIT = 1; };
 
+// A flow table the TCP pass filled, swept by the whole grid of the TASK pass: each entry's sum into its flow's cells of count-min table
+// cms (the key holds the two hashes), then the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a
+// priority they keep after it ends: back to normal, so that they do not hold L2 against the next batch's ingest_kernel and chain. A
+// thread takes FLOW_SWEEP entries a step, one grid stride apart, their loads in flight together (the REDs' memory clobber keeps a load
+// from moving past them).
+__device__ __forceinline__ void flow_sweep(const DevState &st, const FlowTable &t, unsigned long long *cms)
+{
+	const uint32_t stride = gridDim.x * blockDim.x;
+	for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= t.mask; i0 += FLOW_SWEEP * stride) {
+		FlowEnt f[FLOW_SWEEP];
+#pragma unroll
+		for (uint32_t u = 0; u < FLOW_SWEEP; ++u) if (i0 + u * stride <= t.mask) f[u] = t.ent[i0 + u * stride]; else f[u] = FlowEnt {0ull, 0ull};
+#pragma unroll
+		for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
+			const uint32_t i = i0 + u * stride;
+			if (f[u].key) {
+				cms_add(st, cms, (uint32_t)f[u].key, (uint32_t)(f[u].key >> 32), f[u].inc);
+				t.ent[i] = FlowEnt {0ull, 0ull};
+			}
+			if (i <= t.mask && !(i & 7u)) l2_evict_normal_line(t.ent + i);
+		}
+	}
+}
+
 // The records sit in the ingest launch's per-warp regions (RecRegions). Each CTA scans the regions' counts into a table of where
 // each region's groups of 32 records start, and every warp takes an equal, contiguous share of all groups: the regions' sizes
 // differ, the drain warps' work does not.
@@ -749,51 +753,13 @@ template <> struct DrainShape<true> { static constexpr int WARPS = 16, HOT_BITS 
 // that table to the query cells fq_cms after the connection flow table.
 template <bool TASK, bool QRY>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, int exp, FlowTable fq, unsigned long long *fq_cms)
+		RecRegions rr, FlowTable fq, unsigned long long *fq_cms)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
 	if (TASK) {
-		// the flow table the TCP pass filled (then, with QRY, the query flow table): each entry's sum into its flow's cells (the key holds
-		// the two hashes), then the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a priority they keep
-		// after it ends: back to normal, so that they do not hold L2 against the next batch's ingest_kernel and chain. A thread takes
-		// FLOW_SWEEP entries a step, one grid stride apart, their loads in flight together (the REDs' memory clobber keeps a load from
-		// moving past them).
-		const uint32_t stride = gridDim.x * blockDim.x;
-		for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= ft.mask; i0 += FLOW_SWEEP * stride) {
-			FlowEnt f[FLOW_SWEEP];
-#pragma unroll
-			for (uint32_t u = 0; u < FLOW_SWEEP; ++u) if (i0 + u * stride <= ft.mask) f[u] = ft.ent[i0 + u * stride]; else f[u] = FlowEnt {0ull, 0ull};
-#pragma unroll
-			for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
-				const uint32_t i = i0 + u * stride;
-				if (f[u].key) {
-					cms_add(st, st.cms_cur, (uint32_t)f[u].key, (uint32_t)(f[u].key >> 32), f[u].inc);
-					ft.ent[i] = FlowEnt {0ull, 0ull};
-				}
-				if (i <= ft.mask && !(i & 7u)) l2_evict_normal_line(ft.ent + i);
-			}
-		}
-		// the same sweep over the query flow table into its cells. Written out a second time: one loop or one helper over both tables
-		// changes the code of the connection table's sweep, which an engine without the flag runs as before.
-		if (QRY) {
-			const FlowTable &t = fq;
-			unsigned long long *const cms = fq_cms;
-			for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= t.mask; i0 += FLOW_SWEEP * stride) {
-				FlowEnt f[FLOW_SWEEP];
-#pragma unroll
-				for (uint32_t u = 0; u < FLOW_SWEEP; ++u) if (i0 + u * stride <= t.mask) f[u] = t.ent[i0 + u * stride]; else f[u] = FlowEnt {0ull, 0ull};
-#pragma unroll
-				for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
-					const uint32_t i = i0 + u * stride;
-					if (f[u].key) {
-						cms_add(st, cms, (uint32_t)f[u].key, (uint32_t)(f[u].key >> 32), f[u].inc);
-						t.ent[i] = FlowEnt {0ull, 0ull};
-					}
-					if (i <= t.mask && !(i & 7u)) l2_evict_normal_line(t.ent + i);
-				}
-			}
-		}
+		flow_sweep(st, ft, st.cms_cur);
+		if (QRY) flow_sweep(st, fq, fq_cms);
 	}
 	const unsigned long long pol_hll = TASK ? 0 : l2_policy_evict_first(), pol_last = TASK ? 0 : l2_policy_evict_last();
 	extern __shared__ __align__(16) unsigned char drain_smem[];
@@ -825,9 +791,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 	__syncthreads();
 
 	const uint32_t gw = blockIdx.x * WARPS + wid, nw = gridDim.x * WARPS;
-	const uint32_t gbeg = (uint32_t)((unsigned long long)ngroups * gw / nw);
-	// exp bit 8 (timing runs only): the TASK pass applies no process record; its flow-table sweep stays
-	const uint32_t gend = (TASK && (exp & 8)) ? gbeg : (uint32_t)((unsigned long long)ngroups * (gw + 1) / nw);
+	const uint32_t gbeg = (uint32_t)((unsigned long long)ngroups * gw / nw), gend = (uint32_t)((unsigned long long)ngroups * (gw + 1) / nw);
 	const IngestRec *recs = reinterpret_cast<const IngestRec *>(q);
 	// region of group gbeg: the last one that starts at or before it
 	uint32_t r = 0;
@@ -842,7 +806,6 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 	if (TASK) {
 		// one record per lane and group, read once: process records grow from the back of their region, so a group is one coalesced
 		// backward read. The next group's records are in flight while the current group is applied.
-		uint32_t sink = 0;
 		auto fetch = [&](uint32_t g, uint32_t &m) {
 			uint32_t off;
 			locate(g, off, m);
@@ -856,15 +819,14 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 			const IngestRec cur = next;
 			const bool act = (uint32_t)lane < m;
 			if (g + 1 < gend) next = fetch(g + 1, m);
-			drain_task_group<DrainShape<TASK>::ADMIT>(st, hot, cur, act, exp, sink);
+			drain_task_group<DrainShape<TASK>::ADMIT>(st, hot, cur, act);
 		}
-		if (sink == 1u) atomicAdd(&hot.count[0], 1u);
 	}
 	else {
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs<QRY>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, exp, fq, fq_cms);
+			drain_tcp_recs<QRY>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms);
 		}
 	}
 
@@ -1419,7 +1381,7 @@ template <bool TRACE>
 __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merge_kernel(DevState st, const unsigned long long *__restrict__ keys,
 		const uint32_t *__restrict__ touched, const unsigned long long *__restrict__ ntouched_p, const uint32_t *__restrict__ long_slot,
 		const unsigned long long *__restrict__ nlong_p, unsigned long long *__restrict__ batch_rows, const BatchSeg *__restrict__ segs,
-		Centroid *__restrict__ items_scratch /* [nwarps][NBINS] */, TdWorkBig *__restrict__ big_scratch /* [nwarps] */, int exp)
+		Centroid *__restrict__ items_scratch /* [nwarps][NBINS] */, TdWorkBig *__restrict__ big_scratch /* [nwarps] */)
 {
 	__shared__ TdWorkT<TD_SMEM_N> work[TD_WARPS];
 	// window histogram of the service's batch: 32-bit shared-memory atomics (native; a 64-bit shared atomicAdd is a CAS loop). A bucket's
@@ -1672,7 +1634,6 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 			st.slot_batch[slot] = SlotBatch {0xFFFFFFFFu, 0u, 0u, hot};
 		}
 		__syncwarp();
-		if (exp & 256) continue;		// timing runs only (warp-uniform)
 
 		TdHead head = *hp;
 		Centroid *cent = trace ? st.trace.cents(st.trace.par, slot - tbase) : st.td_cent + (size_t)slot * TD_CAP;
@@ -2238,13 +2199,6 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 	return 1;
 }
 
-// GYSK_EXP_ABLATE: the exp bits listed at the top of this file, for timing runs only
-static int exp_ablate()
-{
-	static const int v = []{ const char *e = getenv("GYSK_EXP_ABLATE"); return e ? atoi(e) : 0; }();
-	return v;
-}
-
 // the radix passes of the RESP keys sort on {slot | bin} = key bits [30, 40 + slot bits): TD_CODE_BITS + slot bits significant
 // bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible (27 bits -> 7 7 7 6). Not 9 bits, even
 // where that would save a pass: a 9-bit pass has two look-back rows per thread and nine ballots per key.
@@ -2308,14 +2262,14 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
 	// a counted response sample takes a connection-queue entry, as one connection event does: the regions hold one record per event
 	auto k = st.trace.rows ? (fq.cur ? ingest_kernel<true, true> : ingest_kernel<true, false>) : (fq.cur ? ingest_kernel<false, true> : ingest_kernel<false, false>);
-	k<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, exp_ablate());
+	k<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt);
 	return 1;
 }
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
 template <bool TASK, bool QRY>
-static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int exp, int dev,
+static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, cudaStream_t s)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
@@ -2331,17 +2285,16 @@ static void launch_drain_pass(const DevState &st, const FlowTable &ft, const Sor
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, exp, fq, fq_cms);
+	drain_kernel<TASK, QRY><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq, fq_cms);
 }
 
 template <bool QRY>
-static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int exp, int dev,
+static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, cudaStream_t s)
 {
-	int launches = 0;
-	if (!(exp & 4)) { launch_drain_pass<false, QRY>(st, ft, tmp, rr, n_events, exp, dev, fq, fq_cms, s); launches++; }
-	launch_drain_pass<true, QRY>(st, ft, tmp, rr, n_events, exp, dev, fq, fq_cms, s); launches++;
-	return launches;
+	launch_drain_pass<false, QRY>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, s);
+	launch_drain_pass<true, QRY>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, s);
+	return 2;
 }
 
 // the batch's queued connection records -> flow table, HLL, exact cells; then the flow table -> count-min and its process records ->
@@ -2352,14 +2305,13 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
-	const int exp = exp_ablate();
 	uint32_t n = 16;
 	while (n < tmp.flow_cap && n < 2 * n_events) n <<= 1;
 	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
-	if (!fq.cur) return launch_drain_passes<false>(st, ft, tmp, rr, n_events, exp, dev, FlowTable {nullptr, 0u}, nullptr, s);
+	if (!fq.cur) return launch_drain_passes<false>(st, ft, tmp, rr, n_events, dev, FlowTable {nullptr, 0u}, nullptr, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
-	return launch_drain_passes<true>(st, ft, tmp, rr, n_events, exp, dev, FlowTable {fq.flow, n - 1u}, fq.cur, s);
+	return launch_drain_passes<true>(st, ft, tmp, rr, n_events, dev, FlowTable {fq.flow, n - 1u}, fq.cur, s);
 }
 
 static void os_set_attrs(int dev)
@@ -2460,10 +2412,10 @@ int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_event
 	const int merge_ctas = std::min(nsm, TD_MERGE_MAX_SMS) * TD_MERGE_CTAS_PER_SM;
 	if (st.trace.rows)
 		bins_merge_kernel<true><<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
-				tmp.items_scratch, tmp.big_scratch, exp_ablate());
+				tmp.items_scratch, tmp.big_scratch);
 	else
 		bins_merge_kernel<false><<<merge_ctas, TD_WARPS * 32, 0, s>>>(st, src, tmp.touched, d_ntouched, tmp.long_slot, d_nlong, tmp.batch_rows, segs,
-				tmp.items_scratch, tmp.big_scratch, exp_ablate());
+				tmp.items_scratch, tmp.big_scratch);
 	return launches + 3 + (st.trace.rows ? 1 : 0);
 }
 

@@ -1,13 +1,10 @@
-"""Device time of bins_merge_kernel per batch of the bench workload, whole and without its merge-compress half.
+"""Device time of bins_merge_kernel per batch of the bench workload.
 
     python scripts/bins_merge_probe.py [--batches 8] [--warmup 3]
 
 Builds the bench's two batches (bench.gen_events_gpu, same seeds, same engine sizes), ingests them once (registration) and runs
-the warm-up steps, then times --batches more batches under torch.profiler. That runs twice, each in a process of its own
-(GYSK_EXP_ABLATE is read once per process): as built, and with GYSK_EXP_ABLATE=256, where bins_merge_kernel builds the items and
-histogram cells but skips warp_merge_compress and the digest header update (timing only: the digests are wrong). Prints one JSON
-line: ms per batch of bins_merge_kernel, segs_mark_kernel and the radix passes for both, and the card, its power limit and SM
-clock."""
+the warm-up steps, then times --batches more batches under torch.profiler. Prints one JSON line: ms per batch of bins_merge_kernel,
+segs_mark_kernel and the radix passes, and the card, its power limit and SM clock before and after the run."""
 import argparse
 import json
 import os
@@ -28,13 +25,20 @@ def card():
         return "nvidia-smi failed: %s" % e
 
 
-def child(args):
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batches", type=int, default=8)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--events", type=int, default=100_000_000)
+    args = ap.parse_args()
+
     import torch
     from torch.profiler import ProfilerActivity, profile
 
     import bench
     from gyeeta_b200 import engine as ge
 
+    res = {"card": card()}
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
     n = args.events
@@ -63,27 +67,7 @@ def child(args):
         elif "os_pass_kernel" in e.key:
             out["radix_passes"] += us
     eng.close()
-    print(json.dumps({k: round(v / 1000.0 / args.batches, 4) for k, v in out.items()}))
-
-
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--batches", type=int, default=8)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--events", type=int, default=100_000_000)
-    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
-    args = ap.parse_args()
-    if args.child:
-        return child(args)
-    res = {"card": card()}
-    for name, bits in (("as_built", "0"), ("ablate_256", "256")):
-        env = dict(os.environ, GYSK_EXP_ABLATE=bits)
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--batches", str(args.batches), "--warmup",
-                            str(args.warmup), "--events", str(args.events)], env=env, capture_output=True, text=True)
-        if r.returncode:
-            sys.stderr.write(r.stdout + r.stderr)
-            raise SystemExit("probe run %s failed" % name)
-        res[name] = json.loads(r.stdout.strip().splitlines()[-1])
+    res.update({k: round(v / 1000.0 / args.batches, 4) for k, v in out.items()})
     res["card_after"] = card()
     print(json.dumps(res))
 

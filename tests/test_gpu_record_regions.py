@@ -24,7 +24,6 @@ WARPS, MIN_CTAS, EPT = 8, 3, 2
 
 # every GYSK_ string the library reads from the environment, and why no test here sets it
 NOT_RUN = {
-    "GYSK_EXP_ABLATE": "timing runs only: each bit skips part of the work, so the results are wrong by definition",
     "GYSK_HOT_ROWS": "read per engine, so a test can set it: tests/test_gpu_hot_rows.py",
     "GYSK_HOT_MIN": "read per engine, so a test can set it: tests/test_gpu_hot_rows.py",
     "GYSK_HOT_MAX": "read per engine, so a test can set it: tests/test_gpu_hot_rows.py",
