@@ -380,8 +380,8 @@ int launch_rows(gysk_engine *e, const unsigned long long *, const unsigned long 
 }
 // The rolling levels at the flush of tsec: the closing window goes to ring slot (tsec / width) % NSLOTS of each level, and a slot
 // still holding an older epoch is cleared first (LevelRing::fresh records it). Then the live slots, whose epochs lie in the level's
-// last NSLOTS: what every reader of the levels sums until the next flush. GYSK_FLAG_FLOW_LEVEL's count-min ring takes level 0's
-// decision as it is (launch_cms_level_roll). Slot widths: Level_5s_5min_5days_all durations {300 s, 432000 s} / 10 slots
+// last NSLOTS: what every reader of the levels sums until the next flush. The count-min rings (CMS_RINGS) take level 0's decision as
+// it is (launch_cms_level_roll). Slot widths: Level_5s_5min_5days_all durations {300 s, 432000 s} / 10 slots
 // (gy_statistics.h:1548, :1105).
 int roll_levels(gysk_engine *e, uint32_t tsec)
 {
@@ -560,6 +560,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		return fail(nullptr, GYSK_ERR_INVAL, "gysk_config out of range");
 	if ((cfg.flags & GYSK_FLAG_MERGE_TRACES) && !cfg.max_trace_svcs)
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_MERGE_TRACES needs trace rows (gysk_config.max_trace_svcs > 0)");
+	if ((cfg.flags & GYSK_FLAG_FLOW_QUERY_LEVEL) && !(cfg.flags & GYSK_FLAG_FLOW_QUERIES))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_QUERY_LEVEL needs GYSK_FLAG_FLOW_QUERIES");
 
 	int ndev = 0;
 	cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -614,10 +616,10 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(halloc(e, &e->h_used, 4));
 	e->h_used[3] = 0;		// processes on the free stack: stays 0 without process eviction
 	if ((ce = cudaEventCreateWithFlags(&e->ev_used, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
-	// the count-min tables, and with GYSK_FLAG_FLOW_LEVEL the level's ring: not per slot, outside each_slot_array, so gysk_grow leaves
-	// them; device_bytes counts them
+	// the count-min tables, and with each rolling level its ring: not per slot, outside each_slot_array, so gysk_grow leaves them;
+	// device_bytes counts them
 	for (int t = 0; t < NCMS; ++t) if (cms_held(cfg, t)) A(dalloc(e, &CMS_TABLES[t].live(e), cms_cells(cfg)));
-	if (cfg.flags & GYSK_FLAG_FLOW_LEVEL) A(dalloc(e, &st.cms_ring, NSLOTS * cms_cells(cfg)));
+	for (const CmsRingDesc &r : CMS_RINGS) if (cms_held(cfg, r.level)) A(dalloc(e, &r.ring(e), NSLOTS * cms_cells(cfg)));
 	st.cms_depth = cfg.cms_depth; st.cms_log2w = cfg.cms_log2_width; st.cms_wmask = (1u << cfg.cms_log2_width) - 1; st.hll_p = cfg.hll_p;
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
 	st.td_delta = (double)cfg.td_compression;
@@ -1571,7 +1573,11 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		CU(e, cudaEventRecord(e->ev_evict, e->stream));
 		e->evict_pending = true;
 	}
-	if (e->st.cms_ring) e->kernel_launches += launch_cms_level_roll(e->st, e->stream);		// GYSK_FLAG_FLOW_LEVEL
+	for (const CmsRingDesc &r : CMS_RINGS) {		// each rolling level takes the closing window
+		if (!cms_held(e->cfg, r.level)) continue;
+		e->kernel_launches += launch_cms_level_roll(CMS_TABLES[r.open].live(e), r.ring(e), CMS_TABLES[r.level].live(e), cms_cells(e->cfg),
+				e->st.levels, e->stream);
+	}
 	for (int t : {CMS_CUR, CMS_QRY_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
 		if (!cms_held(e->cfg, t)) continue;
 		unsigned long long *&open = CMS_TABLES[t].live(e);
@@ -2003,6 +2009,12 @@ int gysk_query_flow_queries(gysk_engine *e, const uint64_t *keys, uint32_t n, in
 	return query_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, false, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries");
 }
 
+// GYSK_FLAG_FLOW_QUERY_LEVEL: the point query on the rolling 300-s level of the flow query tables
+int gysk_query_flow_queries_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_qry_est *out)
+{
+	return query_cms(e, CMS_QRY_5MIN, false, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_5min");
+}
+
 int gysk_topn_svcs(gysk_engine *e, int metric, int32_t host_idx, uint32_t n, gysk_topn_entry *out, uint32_t *nout)
 {
 	CHECK_ENGINE(e);
@@ -2086,6 +2098,11 @@ int gysk_export_cms_5min(gysk_engine *e, uint64_t *cells)
 int gysk_export_cms_queries(gysk_engine *e, int last_window, uint64_t *cells)
 {
 	return export_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, cells);
+}
+
+int gysk_export_cms_queries_5min(gysk_engine *e, uint64_t *cells)
+{
+	return export_cms(e, CMS_QRY_5MIN, cells);
 }
 
 // ---- pure helpers ------------------------------------------------------------------------------------------------

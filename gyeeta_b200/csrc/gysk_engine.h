@@ -107,7 +107,7 @@ constexpr int STATE_WORDS = 15;
 static_assert(sizeof(gysk_host_summary) == (STATE_WORDS + 1) * sizeof(int32_t), "gysk_host_summary: 15 fields and a pad");
 
 // The merged arrays of the nl logical services: the merge arena's per-logical arrays and the t-digest slabs, passed by value to the
-// merge kernels. lvl .. rtt exist with GYSK_FLAG_MERGE_LEVELS only, flush with it or GYSK_FLAG_FLOW_LEVEL, states with
+// merge kernels. lvl .. rtt exist with GYSK_FLAG_MERGE_LEVELS only, flush with it, a count-min level or GYSK_FLAG_MERGE_TRACES, states with
 // GYSK_FLAG_MERGE_STATES only (nullptr without).
 struct LogicalArrays
 {
@@ -240,8 +240,8 @@ constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(Sla
 
 // The count-min tables an engine can hold, each [cms_depth][1 << cms_log2_width] cells (CMS_TABLES below says which flag each one
 // needs, its array in the merge arena and where the engine keeps it). Each windowed pair is an open table and, right after it, the
-// table of the window the last flush closed.
-enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, NCMS };
+// table of the window the last flush closed. A new table goes last, so that every engine without it keeps its merge arena.
+enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, NCMS };
 
 // the cells of one count-min table
 inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
@@ -260,7 +260,7 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min] [, cmsq cur/last], hist last/all, conn [, levels, aux] [, states]
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min] [, cmsq cur/last [, 5min]], hist last/all, conn [, levels, aux] [, states]
 									//           [, clusters] [, traces]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt] [, flush tsec]
 									//           [, trace max]
@@ -384,8 +384,22 @@ inline const CmsTableDesc CMS_TABLES[NCMS] = {
 	{GYSK_FLAG_FLOW_LEVEL, "cms_5min", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_5min; }},
 	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_cur", [](gysk_engine *e) -> unsigned long long *& { return e->fq.cur; }},
 	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_last", [](gysk_engine *e) -> unsigned long long *& { return e->fq.last; }},
+	{GYSK_FLAG_FLOW_QUERY_LEVEL, "cms_qry_5min", [](gysk_engine *e) -> unsigned long long *& { return e->fq.level; }},
 };
 inline bool cms_held(const gysk_config &cfg, int t) { return !CMS_TABLES[t].flag || (cfg.flags & CMS_TABLES[t].flag); }
+
+// A rolling 300-s level of a windowed pair: at each flush the open table `open` goes into a ring of NSLOTS tables by level 0's decision of
+// roll_levels, and the level table `level` becomes the sum of the live slots (launch_cms_level_roll). The engine holds the ring with the
+// level table.
+struct CmsRingDesc
+{
+	int			open, level;
+	unsigned long long	*&(*ring)(gysk_engine *);
+};
+inline const CmsRingDesc CMS_RINGS[] = {
+	{CMS_CUR, CMS_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_ring; }},
+	{CMS_QRY_CUR, CMS_QRY_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->fq.ring; }},
+};
 
 int fail(gysk_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess);
 int post_launch(gysk_engine *e, const char *what);

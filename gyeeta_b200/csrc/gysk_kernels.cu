@@ -2147,9 +2147,9 @@ __global__ void query_flows_kernel(const unsigned long long *__restrict__ tbl, u
 	out[i].flow_key = key; out[i].count = cnt; out[i].kbytes = kb;
 }
 
-// GYSK_FLAG_FLOW_LEVEL: the count-min level at a flush, one grid-stride pass over the cells in 16-byte pairs. Ring slot k takes the
-// closing window cur, added to what the slot holds or, when the flush started a new epoch there, in its place (which stands in for
-// clearing the slot). The level becomes the sum of the live slots, slot k's new content included. So the pass reads cur and the live
+// A rolling count-min level (GYSK_FLAG_FLOW_LEVEL, GYSK_FLAG_FLOW_QUERY_LEVEL) at a flush, one grid-stride pass over the cells in
+// 16-byte pairs. Ring slot k takes the closing window cur, added to what the slot holds or, when the flush started a new epoch there,
+// in its place (which stands in for clearing the slot). The level becomes the sum of the live slots, slot k's new content included. So the pass reads cur and the live
 // slots and writes slot k and the level, every cell mod 2^64 as RED.ADD.64 builds cur. The ring and the level are streamed
 // (evict-first) so that the pass does not push out of L2 the count-min lines the ingest path keeps resident.
 __global__ void __launch_bounds__(256) cms_level_roll_kernel(const ulonglong2 *__restrict__ cur, ulonglong2 *__restrict__ ring,
@@ -2588,12 +2588,13 @@ int launch_query_flows(const unsigned long long *tbl, uint32_t depth, uint32_t l
 	return 1;
 }
 
-int launch_cms_level_roll(const DevState &st, cudaStream_t s)
+int launch_cms_level_roll(const unsigned long long *cur, unsigned long long *ring, unsigned long long *level, size_t cells, const LevelRing &lv,
+		cudaStream_t s)
 {
-	const uint64_t npair = ((uint64_t)st.cms_depth << st.cms_log2w) / 2;		// log2w >= 4: whole pairs
+	const uint64_t npair = cells / 2;		// log2w >= 4: whole pairs
 	const uint32_t grid = std::min<uint32_t>(div_up(npair, 256), (uint32_t)sm_count(current_device()) * 8u);
-	cms_level_roll_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const ulonglong2 *>(st.cms_cur), reinterpret_cast<ulonglong2 *>(st.cms_ring),
-			reinterpret_cast<ulonglong2 *>(st.cms_5min), npair, st.levels.cur[0], st.levels.live[0], st.levels.fresh & 1u);
+	cms_level_roll_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const ulonglong2 *>(cur), reinterpret_cast<ulonglong2 *>(ring),
+			reinterpret_cast<ulonglong2 *>(level), npair, lv.cur[0], lv.live[0], lv.fresh & 1u);
 	return 1;
 }
 

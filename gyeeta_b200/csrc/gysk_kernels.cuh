@@ -14,8 +14,8 @@ static constexpr int NSLOTS = 10;			// slots per level (gy_statistics.h:1105)
 
 // The rolling 300-s / 5-day levels: per level NSLOTS ring slots, each a plane of `stride` service rows of 16 cells
 // ([NLEVELS][NSLOTS][stride][16]). stride is max_svcs: the null slot (index max_svcs) has no ring row. live, cur and fresh are set by
-// the host at every flush (roll_levels in gysk_engine.cu); all are 0 until the first one. The count-min level of GYSK_FLAG_FLOW_LEVEL
-// follows level 0's decision (cms_level_roll_kernel).
+// the host at every flush (roll_levels in gysk_engine.cu); all are 0 until the first one. The count-min levels of GYSK_FLAG_FLOW_LEVEL
+// and GYSK_FLAG_FLOW_QUERY_LEVEL follow level 0's decision (cms_level_roll_kernel).
 struct LevelRing
 {
 	HistCell		*ring;
@@ -155,8 +155,9 @@ static constexpr uint32_t FLOW_SWEEP = 4;		// entries per thread and step of the
 // with the depth, width and row hashes of cms_cur / cms_last, and the batch flow table the TCP pass sums them in before the TASK pass
 // applies it (as FlowTable does for the connection records). ingest_kernel queues each such sample as a connection-queue record whose
 // slot is QRY_REC. Kept out of DevState so that the kernels without the flag keep their parameter layout: the drain passes take it as
-// parameters of their own. Every pointer nullptr: off.
-struct FlowQueries { unsigned long long *cur, *last; FlowEnt *flow; };
+// parameters of their own. Every pointer nullptr: off. ring and level: GYSK_FLAG_FLOW_QUERY_LEVEL's rolling 300-s level of the tables,
+// laid out as DevState::cms_ring / cms_5min (nullptr without).
+struct FlowQueries { unsigned long long *cur, *last; FlowEnt *flow; unsigned long long *ring, *level; };
 static constexpr uint32_t QRY_REC = 0xFFFFFFFFu;	// slot field of a queued response sample (service slots are < 2^24)
 
 struct SortTemp
@@ -288,9 +289,10 @@ int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, c
 // the count-min point queries of n flow keys on table tbl ([depth][1 << log2w] cells)
 int launch_query_flows(const unsigned long long *tbl, uint32_t depth, uint32_t log2w, const unsigned long long *d_keys, uint32_t n, gysk_flow_est *d_out,
 		cudaStream_t s);
-// GYSK_FLAG_FLOW_LEVEL, at the flush before the cms_cur / cms_last swap: cms_cur into ring slot st.levels.cur[0] (replacing it when
-// the slot is fresh), then cms_5min = the sum of the live slots
-int launch_cms_level_roll(const DevState &st, cudaStream_t s);
+// a rolling count-min level at the flush, before its window pair's swap: the open table cur ([cells]) into ring slot lv.cur[0]
+// (replacing it when the slot is fresh), then level = the sum of the live slots (level 0's decision of lv)
+int launch_cms_level_roll(const unsigned long long *cur, unsigned long long *ring, unsigned long long *level, size_t cells, const LevelRing &lv,
+		cudaStream_t s);
 // trace rows at gysk_flush: the half `open` (the one the flush opens) of rows [0, nrows) cleared
 int launch_trace_roll(const DevState &st, uint32_t open, uint32_t nrows, cudaStream_t s);
 // trace rows by id (d_ids) or by row (d_rows)

@@ -15,7 +15,8 @@
 //                          GYSK_FLAG_MERGE_TOPN appends this rank's 64 best services / processes per metric, with their rows, to the slab;
 //                          GYSK_FLAG_FLOW_LEVEL puts the count-min level after cms cur/last and, as GYSK_FLAG_MERGE_LEVELS does,
 //                          the flush tsec pair in the i64 MAX region (once when both are set); GYSK_FLAG_FLOW_QUERIES puts the
-//                          flow query tables cur/last after the count-min tables
+//                          flow query tables cur/last after the count-min tables, GYSK_FLAG_FLOW_QUERY_LEVEL their level after
+//                          them with the flush tsec pair as GYSK_FLAG_FLOW_LEVEL
 //   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests [, the global pick of the gathered top-N candidates]
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
@@ -815,11 +816,12 @@ int lay_out_arena(gysk_engine *e)
 	// name joins its region's gysk_merge_buffers name. GYSK_FLAG_MERGE_LEVELS appends its arrays to the ends of the SUM and i64 MAX
 	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those.
 	// GYSK_FLAG_FLOW_LEVEL puts the count-min level after the two window tables, and needs the flush tsec pair as the levels do:
-	// still three regions, three collectives. GYSK_FLAG_FLOW_QUERIES puts the two flow query tables after the count-min ones.
+	// still three regions, three collectives. GYSK_FLAG_FLOW_QUERIES puts the two flow query tables after the count-min ones, and
+	// GYSK_FLAG_FLOW_QUERY_LEVEL their level after them, with the flush tsec pair.
 	// GYSK_FLAG_MERGE_TRACES puts its words at the end of the SUM region, its maxima at the end of the i64 MAX one, and needs the flush
 	// tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
-	const bool flow_level = e->cfg.flags & GYSK_FLAG_FLOW_LEVEL, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
+	const bool flow_level = e->cfg.flags & (GYSK_FLAG_FLOW_LEVEL | GYSK_FLAG_FLOW_QUERY_LEVEL), traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
 	const size_t b_hist = (size_t)nl * HIST_CELLS * sizeof(HistCell);
 	auto layout = [&](uint8_t *base) {
 		size_t off = 0;
@@ -1017,7 +1019,7 @@ int gysk_merge_prepare(gysk_engine *e)
 			e->kernel_launches++;
 		}
 	}
-	if (mg.lg.flush) {		// GYSK_FLAG_MERGE_LEVELS, GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_MERGE_TRACES: also with no logical service, for the flush tsec pair
+	if (mg.lg.flush) {		// GYSK_FLAG_MERGE_LEVELS, a count-min level or GYSK_FLAG_MERGE_TRACES: also with no logical service, for the flush tsec pair
 		LogicalArrays lg = mg.lg;
 		if (!lg.lvl) lg.nl = 0;		// without GYSK_FLAG_MERGE_LEVELS: the pair only
 		fold_levels_kernel<<<std::max<uint32_t>(div_up((uint64_t)lg.nl * HIST_CELLS, 256), 1), 256, 0, e->stream>>>(e->st, mg.members,
@@ -1276,7 +1278,7 @@ int gysk_merge_flush_range(gysk_engine *e, uint32_t *min_tsec, uint32_t *max_tse
 {
 	CHECK_ENGINE(e);
 	if (!min_tsec || !max_tsec) return GYSK_ERR_INVAL;
-	if (!(e->cfg.flags & (GYSK_FLAG_MERGE_LEVELS | GYSK_FLAG_FLOW_LEVEL | GYSK_FLAG_MERGE_TRACES))) return GYSK_ERR_NOTSUP;
+	if (!(e->cfg.flags & (GYSK_FLAG_MERGE_LEVELS | GYSK_FLAG_FLOW_LEVEL | GYSK_FLAG_FLOW_QUERY_LEVEL | GYSK_FLAG_MERGE_TRACES))) return GYSK_ERR_NOTSUP;
 	GYSK_ENTER(e, Drain);
 	MergeState &mg = e->mg;
 	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_merge_flush_range: no finished merge");
@@ -1303,6 +1305,12 @@ int gysk_query_flows_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t 
 int gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_qry_est *out)
 {
 	return query_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, true, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_global");
+}
+
+// GYSK_FLAG_FLOW_QUERY_LEVEL: the point query on the flow query level summed over the ranks
+int gysk_query_flow_queries_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_qry_est *out)
+{
+	return query_cms(e, CMS_QRY_5MIN, true, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_global_5min");
 }
 
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)

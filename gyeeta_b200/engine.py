@@ -36,6 +36,7 @@ NOTIFY_LISTENER_STATE, NOTIFY_TCP_CONN, NOTIFY_AGGR_TASK_STATE, NOTIFY_ACTIVE_CO
 FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, FLAG_MERGE_TOPN, FLAG_FLOW_LEVEL = 1, 2, 4, 8, 16, 32
 FLAG_MERGE_TRACES = 64
 FLAG_FLOW_QUERIES = 128
+FLAG_FLOW_QUERY_LEVEL = 0x100
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
@@ -309,6 +310,9 @@ def load_library(path=None):
         "gysk_query_flow_queries": (i32, [vp, vp, u32, i32, vp]),
         "gysk_export_cms_queries": (i32, [vp, i32, vp]),
         "gysk_query_flow_queries_global": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_flow_queries_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_export_cms_queries_5min": (i32, [vp, vp]),
+        "gysk_query_flow_queries_global_5min": (i32, [vp, vp, u32, vp]),
         "gysk_last_batch_flow_query_direct": (C.c_int64, [vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
@@ -375,7 +379,7 @@ class Engine:
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
-                 max_trace_svcs=0, merge_traces=False, flow_queries=False):
+                 max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -389,7 +393,7 @@ class Engine:
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
-                    (FLAG_FLOW_QUERIES if flow_queries else 0)
+                    (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -689,6 +693,10 @@ class Engine:
         """gysk_query_flow_queries: requests and response msec per flow key, min over rows (flow_queries=True)"""
         return self._point_query(self.L.gysk_query_flow_queries, FLOW_QRY_EST_DTYPE, keys, int(last_window))
 
+    def query_flow_queries_5min(self, keys):
+        """gysk_query_flow_queries_5min: the point query on the rolling 300-s flow query level (flow_query_level=True)"""
+        return self._point_query(self.L.gysk_query_flow_queries_5min, FLOW_QRY_EST_DTYPE, keys)
+
     def topn(self, metric, n=10, host_idx=-1):
         out = (TopnEntry * n)()
         k = C.c_uint32()
@@ -972,6 +980,14 @@ class Engine:
     def query_flow_queries_global(self, keys, last_window=False):
         """gysk_query_flow_queries_global: the point query on the flow query tables summed over the ranks by the last merge"""
         return self._point_query(self.L.gysk_query_flow_queries_global, FLOW_QRY_EST_DTYPE, keys, int(last_window))
+
+    def export_cms_queries_5min(self):
+        """gysk_export_cms_queries_5min: the cells of the rolling 300-s flow query level (flow_query_level=True)"""
+        return self._export_cells(self.L.gysk_export_cms_queries_5min)
+
+    def query_flow_queries_global_5min(self, keys):
+        """gysk_query_flow_queries_global_5min: the point query on the 300-s flow query level summed over the ranks by the last merge"""
+        return self._point_query(self.L.gysk_query_flow_queries_global_5min, FLOW_QRY_EST_DTYPE, keys)
 
     def export_cms_5min(self):
         """gysk_export_cms_5min: the cells of the rolling 300-s count-min level (flow_level=True)"""

@@ -230,6 +230,12 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   same flags on every rank). Costs 2 more tables of depth << log2_width cells and a second
 						   batch flow table. Without it nothing is allocated, every other call answers as before and
 						   the flow query calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_FLOW_QUERY_LEVEL	0x100u	/* a rolling 300-s level of the flow query tables (gysk_query_flow_queries_5min,
+						   gysk_export_cms_queries_5min); with it the merge step also sums the level across ranks
+						   (gysk_query_flow_queries_global_5min; the same flags on every rank). Needs
+						   GYSK_FLAG_FLOW_QUERIES: gysk_create refuses it without; combines freely with every other
+						   flag. Costs NSLOTS + 1 = 11 more tables of depth << log2_width cells. Without it nothing is
+						   allocated, every other call answers as before and the three calls are GYSK_ERR_NOTSUP */
 
 typedef struct gysk_config
 {
@@ -451,7 +457,8 @@ int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the
  * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
  * buffers and the count-min tables: 2 tables of cms_depth << cms_log2_width 8-byte cells, 11 more with GYSK_FLAG_FLOW_LEVEL (its 10 ring
  * slots and the level: 352 MiB more at the default 4 x 2^20), 2 more with GYSK_FLAG_FLOW_QUERIES (64 MiB at 4 x 2^20, plus a second
- * batch flow table of up to 32 MiB). The count-min tables do not depend on capacity, so gysk_grow leaves them.
+ * batch flow table of up to 32 MiB), 11 more with GYSK_FLAG_FLOW_QUERY_LEVEL (352 MiB at 4 x 2^20, 2.8 GiB at 8 x 2^22). The count-min
+ * tables do not depend on capacity, so gysk_grow and eviction leave them; gysk_capacity.device_bytes counts them.
  * Trace rows (max_trace_svcs) are not per service slot and not counted here: 3784 bytes each, in gysk_capacity.device_bytes. */
 int		gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes);
 
@@ -648,6 +655,22 @@ int		gysk_query_flow_queries(gysk_engine *e, const uint64_t *flow_keys, uint32_t
 int		gysk_export_cms_queries(gysk_engine *e, int last_window, uint64_t *cells /* depth << log2_width entries */);
 int		gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_qry_est *out);
 
+/* ---- the rolling 300-s flow query level (GYSK_FLAG_FLOW_QUERY_LEVEL): requests and response time of a flow in the last five minutes ----
+ * The level holds the flow query tables of the windows closed by the flushes the 300-s response level holds, by the rule of the
+ * connection count-min's level (GYSK_FLAG_FLOW_LEVEL): ring slot (tsec / 30) % 10, a slot holding an older epoch replaced, the same
+ * behaviour over gaps, repeated tsec and a step back, empty before the first flush. The open window is not in it. Each cell is the
+ * cell-wise sum mod 2^64 of those windows' gysk_export_cms_queries(last_window = 1) tables: the table one window fed all their samples
+ * would hold, {queries | response msec << 32} with the carry of the table itself.
+ * gysk_query_flow_queries_5min: the point query of gysk_query_flow_queries on the level, the minimum over rows of each half.
+ * gysk_export_cms_queries_5min: the level's cells (depth << log2_width entries).
+ * gysk_query_flow_queries_global_5min: the point query on the level summed over the ranks by the last merge (GYSK_ERR_INVAL before
+ * gysk_merge_prepare). A rank's level is relative to its own last flush: gysk_merge_flush_range shows whether the ranks had closed
+ * the same window.
+ * All three are GYSK_ERR_NOTSUP without the flag. */
+int		gysk_query_flow_queries_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_qry_est *out);
+int		gysk_export_cms_queries_5min(gysk_engine *e, uint64_t *cells /* depth << log2_width entries */);
+int		gysk_query_flow_queries_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_qry_est *out);
+
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
  * aggregates those rows per service and time bucket in SQL (tracereq_aggr_info, common/gy_json_field_maps.h:2628-2664). Here each traced
@@ -784,7 +807,8 @@ int		gysk_query_logical(gysk_engine *e, const uint64_t *logical_ids, uint32_t n,
 int		gysk_export_logical_hist(gysk_engine *e, uint64_t logical_id, int which, gysk_hist_serial out[GYSK_HIST_MAX_BUCKETS],
 				uint64_t *total_count, int64_t *max_val);
 /* The earliest and latest tsec of the ranks' last gysk_flush, as all-reduced by the last finished merge (GYSK_FLAG_MERGE_LEVELS,
- * GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_MERGE_TRACES; GYSK_ERR_NOTSUP without all three, GYSK_ERR_INVAL before a finished merge). Each rank's
+ * GYSK_FLAG_FLOW_LEVEL, GYSK_FLAG_FLOW_QUERY_LEVEL or GYSK_FLAG_MERGE_TRACES; GYSK_ERR_NOTSUP without all four, GYSK_ERR_INVAL before a
+ * finished merge). Each rank's
  * level slots and last trace window are relative to its own last flush, so *min_tsec != *max_tsec means the ranks had closed different
  * windows and the merged levels or trace windows mix them. That is not an
  * error: the collectives cannot fail on one rank alone, so the caller decides what to do with such an answer. */
