@@ -75,7 +75,7 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, rr, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
@@ -299,6 +299,8 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 
 static_assert(sizeof(gysk_flow_qry_est) == sizeof(gysk_flow_est) && offsetof(gysk_flow_qry_est, queries) == offsetof(gysk_flow_est, count) &&
 		offsetof(gysk_flow_qry_est, resp_ms) == offsetof(gysk_flow_est, kbytes), "a flow query row is read as a gysk_flow_est");
+static_assert(sizeof(gysk_flow_resp_est) == 96 && offsetof(gysk_flow_resp_est, counts) == 8 && offsetof(gysk_flow_resp_est, total) == 68 &&
+		offsetof(gysk_flow_resp_est, p25_ms) == 72 && offsetof(gysk_flow_resp_est, p99_ms) == 88, "gysk_flow_resp_est: 96 bytes as documented");
 
 int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what)
 {
@@ -314,19 +316,34 @@ int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t
 	}, CopyRows<gysk_flow_est> {out});
 }
 
+int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what)
+{
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!cms_held(e->cfg, t)) return GYSK_ERR_NOTSUP;
+	Entry entry(e, merged ? Pending::Drain : Pending::Submit);
+	if (entry.rc) return entry.rc;
+	if (merged && !e->mg.prepared) return fail(e, GYSK_ERR_INVAL, ("gysk_" + std::string(what) + ": no merge").c_str());
+	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[t].live(e);
+	return staged_read(e, keys, n, QCHUNK, sizeof(gysk_flow_resp_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
+		return launch_query_flow_resp(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, m, reinterpret_cast<gysk_flow_resp_est *>(e->d_wstage),
+				e->stream);
+	}, CopyRows<gysk_flow_resp_est> {out});
+}
+
 } // namespace gysk
 
 namespace {
 
-// the cells of count-min table t (gysk_export_cms and its kin), after every event handed in has run; GYSK_ERR_NOTSUP when the engine
-// does not hold t
+// the cells of count-min table t (gysk_export_cms and its kin), every word of them, after every event handed in has run; GYSK_ERR_NOTSUP
+// when the engine does not hold t
 int export_cms(gysk_engine *e, int t, uint64_t *cells)
 {
 	CHECK_ENGINE(e);
 	if (!cells) return GYSK_ERR_INVAL;
 	if (!cms_held(e->cfg, t)) return GYSK_ERR_NOTSUP;
 	GYSK_ENTER(e, Sync);
-	CU(e, cudaMemcpy(cells, CMS_TABLES[t].live(e), sizeof(uint64_t) * cms_cells(e->cfg), cudaMemcpyDeviceToHost));
+	CU(e, cudaMemcpy(cells, CMS_TABLES[t].live(e), sizeof(uint64_t) * cms_words(e->cfg, t), cudaMemcpyDeviceToHost));
 	return GYSK_OK;
 }
 
@@ -554,7 +571,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	if (!cfg.world) cfg.world = 1;
 	if (!cfg.stage_batch || cfg.stage_batch > cfg.max_batch) cfg.stage_batch = std::min<uint32_t>(cfg.max_batch, 1u << 22);
 	if (cfg.max_svcs < 1 || cfg.max_svcs > (1u << 24) || cfg.max_tasks < 1 || cfg.max_tasks > (1u << 24) || cfg.cms_depth < 1 ||
-			cfg.cms_depth > 8 || cfg.cms_log2_width < 4 || cfg.cms_log2_width > 28 || cfg.hll_p < 4 || cfg.hll_p > 16 ||
+			cfg.cms_depth > 8 || cfg.cms_log2_width < 4 || cfg.cms_log2_width > (int)CMS_LOG2W_MAX || cfg.hll_p < 4 || cfg.hll_p > 16 ||
 			cfg.td_compression < 10 || cfg.td_compression > (uint32_t)TD_CAP || cfg.max_batch < 1024 || cfg.max_batch >= (1u << 27) ||
 			cfg.rank >= cfg.world || !trace_fits(cfg.max_svcs, cfg.max_trace_svcs))
 		return fail(nullptr, GYSK_ERR_INVAL, "gysk_config out of range");
@@ -562,6 +579,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_MERGE_TRACES needs trace rows (gysk_config.max_trace_svcs > 0)");
 	if ((cfg.flags & GYSK_FLAG_FLOW_QUERY_LEVEL) && !(cfg.flags & GYSK_FLAG_FLOW_QUERIES))
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_QUERY_LEVEL needs GYSK_FLAG_FLOW_QUERIES");
+	if ((cfg.flags & GYSK_FLAG_FLOW_RESP_HIST) && !(cfg.flags & GYSK_FLAG_FLOW_QUERIES))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_RESP_HIST needs GYSK_FLAG_FLOW_QUERIES");
 
 	int ndev = 0;
 	cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -618,8 +637,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	if ((ce = cudaEventCreateWithFlags(&e->ev_used, cudaEventDisableTiming)) != cudaSuccess) { fail(e, GYSK_ERR_CUDA, "cudaEventCreate", ce); return bail(GYSK_ERR_CUDA); }
 	// the count-min tables, and with each rolling level its ring: not per slot, outside each_slot_array, so gysk_grow leaves them;
 	// device_bytes counts them
-	for (int t = 0; t < NCMS; ++t) if (cms_held(cfg, t)) A(dalloc(e, &CMS_TABLES[t].live(e), cms_cells(cfg)));
-	for (const CmsRingDesc &r : CMS_RINGS) if (cms_held(cfg, r.level)) A(dalloc(e, &r.ring(e), NSLOTS * cms_cells(cfg)));
+	for (int t = 0; t < NCMS; ++t) if (cms_held(cfg, t)) A(dalloc(e, &CMS_TABLES[t].live(e), cms_words(cfg, t)));
+	for (const CmsRingDesc &r : CMS_RINGS) if (cms_held(cfg, r.level)) A(dalloc(e, &r.ring(e), NSLOTS * cms_words(cfg, r.level)));
 	st.cms_depth = cfg.cms_depth; st.cms_log2w = cfg.cms_log2_width; st.cms_wmask = (1u << cfg.cms_log2_width) - 1; st.hll_p = cfg.hll_p;
 	st.rank = cfg.rank; st.world = cfg.world; st.auto_register = (cfg.flags & GYSK_FLAG_AUTO_REGISTER) ? 1 : 0;
 	st.td_delta = (double)cfg.td_compression;
@@ -670,6 +689,7 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		tmp.flow_cap = std::min<uint32_t>(FLOW_ENT_MAX, pow2_at_least(2ull * cfg.max_batch));
 		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
 		if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) A(dalloc(e, &e->fq.flow, (size_t)tmp.flow_cap));		// the query flow table, alike
+		if (cfg.flags & GYSK_FLAG_FLOW_RESP_HIST) A(dalloc(e, &e->fr.flow, (size_t)tmp.flow_cap));		// the response flow table, alike
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
 	if (cfg.max_trace_svcs) {
@@ -802,15 +822,24 @@ int64_t gysk_last_batch_flow_query_direct(gysk_engine *e)
 	return read_counter(e, CTR_FLOWQ_DIRECT);
 }
 
-// diagnostic: entries of the flow table (and of the query flow table, GYSK_FLAG_FLOW_QUERIES) that are not zero (a key or a sum left
-// behind); 0 whenever no batch is in flight
+// diagnostic (GYSK_FLAG_FLOW_RESP_HIST): response samples of the last device batch whose flow response histogram update bypassed the
+// response flow table
+int64_t gysk_last_batch_flow_resp_direct(gysk_engine *e)
+{
+	CHECK_ENGINE(e);
+	if (!cms_held(e->cfg, CMS_RESP_CUR)) return GYSK_ERR_NOTSUP;
+	return read_counter(e, CTR_FLOWR_DIRECT);
+}
+
+// diagnostic: entries of the flow table (and of the query and response flow tables, GYSK_FLAG_FLOW_QUERIES / GYSK_FLAG_FLOW_RESP_HIST)
+// that are not zero (a key or a sum left behind); 0 whenever no batch is in flight
 int64_t gysk_flow_table_used(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Sync);
 	std::vector<FlowEnt> t(e->tmp.flow_cap);
 	int64_t used = 0;
-	for (const FlowEnt *tbl : {e->tmp.flow, e->fq.flow}) {
+	for (const FlowEnt *tbl : {e->tmp.flow, e->fq.flow, e->fr.flow}) {
 		if (!tbl) continue;
 		CU(e, cudaMemcpy(t.data(), tbl, t.size() * sizeof(FlowEnt), cudaMemcpyDeviceToHost));
 		used += (int64_t)std::count_if(t.begin(), t.end(), [](const FlowEnt &f) { return f.key || f.inc; });
@@ -1575,14 +1604,14 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 	}
 	for (const CmsRingDesc &r : CMS_RINGS) {		// each rolling level takes the closing window
 		if (!cms_held(e->cfg, r.level)) continue;
-		e->kernel_launches += launch_cms_level_roll(CMS_TABLES[r.open].live(e), r.ring(e), CMS_TABLES[r.level].live(e), cms_cells(e->cfg),
+		e->kernel_launches += launch_cms_level_roll(CMS_TABLES[r.open].live(e), r.ring(e), CMS_TABLES[r.level].live(e), cms_words(e->cfg, r.open),
 				e->st.levels, e->stream);
 	}
-	for (int t : {CMS_CUR, CMS_QRY_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
+	for (int t : {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
 		if (!cms_held(e->cfg, t)) continue;
 		unsigned long long *&open = CMS_TABLES[t].live(e);
 		std::swap(open, CMS_TABLES[t + 1].live(e));
-		CU(e, cudaMemsetAsync(open, 0, sizeof(unsigned long long) * cms_cells(e->cfg), e->stream));
+		CU(e, cudaMemsetAsync(open, 0, sizeof(unsigned long long) * cms_words(e->cfg, t), e->stream));
 	}
 	return post_launch(e, "flush");
 }
@@ -2103,6 +2132,27 @@ int gysk_export_cms_queries(gysk_engine *e, int last_window, uint64_t *cells)
 int gysk_export_cms_queries_5min(gysk_engine *e, uint64_t *cells)
 {
 	return export_cms(e, CMS_QRY_5MIN, cells);
+}
+
+// GYSK_FLAG_FLOW_RESP_HIST: the point query on the flow response histograms, their cells, and the same on their rolling 300-s level
+int gysk_query_flow_resp(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_resp_est *out)
+{
+	return query_cms_resp(e, last_window ? CMS_RESP_LAST : CMS_RESP_CUR, false, keys, n, out, "query_flow_resp");
+}
+
+int gysk_export_cms_resp(gysk_engine *e, int last_window, uint64_t *words)
+{
+	return export_cms(e, last_window ? CMS_RESP_LAST : CMS_RESP_CUR, words);
+}
+
+int gysk_query_flow_resp_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out)
+{
+	return query_cms_resp(e, CMS_RESP_5MIN, false, keys, n, out, "query_flow_resp_5min");
+}
+
+int gysk_export_cms_resp_5min(gysk_engine *e, uint64_t *words)
+{
+	return export_cms(e, CMS_RESP_5MIN, words);
 }
 
 // ---- pure helpers ------------------------------------------------------------------------------------------------

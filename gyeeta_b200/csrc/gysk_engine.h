@@ -238,10 +238,11 @@ static_assert(TopnLists::SVC_ROW % 16 == 0 && TopnLists::TASK_ROW % 16 == 0 && s
 // the candidates' whole SlabEntrys after a rank's nl digests
 constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
 
-// The count-min tables an engine can hold, each [cms_depth][1 << cms_log2_width] cells (CMS_TABLES below says which flag each one
-// needs, its array in the merge arena and where the engine keeps it). Each windowed pair is an open table and, right after it, the
-// table of the window the last flush closed. A new table goes last, so that every engine without it keeps its merge arena.
-enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, NCMS };
+// The count-min tables an engine can hold, each [cms_depth][1 << cms_log2_width] cells of one or more u64 words (CMS_TABLES below says
+// which flag each one needs, its array in the merge arena, where the engine keeps it and its words per cell). Each windowed pair is an
+// open table and, right after it, the table of the window the last flush closed. A new table goes last, so that every engine without it
+// keeps its merge arena.
+enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, CMS_RESP_CUR, CMS_RESP_LAST, CMS_RESP_5MIN, NCMS };
 
 // the cells of one count-min table
 inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
@@ -260,8 +261,8 @@ struct MergeState
 	// one arena so that each reduction kind is a single collective
 	uint8_t			*arena {nullptr};
 	size_t			arena_bytes {0};
-	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min] [, cmsq cur/last [, 5min]], hist last/all, conn [, levels, aux] [, states]
-									//           [, clusters] [, traces]
+	size_t			off_sum {0}, bytes_sum {0};		// u64 SUM : cms cur/last [, 5min] [, cmsq cur/last [, 5min]] [, cmsr cur/last [, 5min]], hist
+									//           last/all, conn [, levels, aux] [, states] [, clusters] [, traces]
 	size_t			off_maxi64 {0}, bytes_maxi64 {0};	// i64 MAX : histogram max_val_seen_ [, level maxima, rtt] [, flush tsec]
 									//           [, trace max]
 	size_t			off_maxu8 {0}, bytes_maxu8 {0};		// u8  MAX : HLL registers
@@ -293,6 +294,7 @@ struct gysk_engine
 	gysk::DevState		st {};
 	gysk::SortTemp		tmp {};
 	gysk::FlowQueries	fq {};				// GYSK_FLAG_FLOW_QUERIES (every pointer nullptr without)
+	gysk::FlowRespHist	fr {};				// GYSK_FLAG_FLOW_RESP_HIST (every pointer nullptr without)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
 	std::vector<void *>	hallocs;
@@ -370,23 +372,30 @@ namespace gysk {
 // slot_last_active of the window the last flush closed (state_kernel): the active_mark of svc_evaluated / svc_issue
 inline uint32_t active_mark(const gysk_engine *e) { return e->last_flush_tsec ? e->last_flush_tsec : 1u; }
 
-// one count-min table of CmsTable: the gysk_config flag it needs (0: every engine holds it), its array in the merge arena's SUM region
-// (gysk_merge_buffers), and the engine's live table
+// one count-min table of CmsTable: the gysk_config flags it needs (0: every engine holds it), its array in the merge arena's SUM region
+// (gysk_merge_buffers), the engine's live table, and the u64 words of one cell
 struct CmsTableDesc
 {
 	uint32_t		flag;
 	const char		*name;
 	unsigned long long	*&(*live)(gysk_engine *);
+	uint32_t		words;
 };
 inline const CmsTableDesc CMS_TABLES[NCMS] = {
-	{0, "cms_cur", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_cur; }},
-	{0, "cms_last", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_last; }},
-	{GYSK_FLAG_FLOW_LEVEL, "cms_5min", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_5min; }},
-	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_cur", [](gysk_engine *e) -> unsigned long long *& { return e->fq.cur; }},
-	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_last", [](gysk_engine *e) -> unsigned long long *& { return e->fq.last; }},
-	{GYSK_FLAG_FLOW_QUERY_LEVEL, "cms_qry_5min", [](gysk_engine *e) -> unsigned long long *& { return e->fq.level; }},
+	{0, "cms_cur", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_cur; }, 1},
+	{0, "cms_last", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_last; }, 1},
+	{GYSK_FLAG_FLOW_LEVEL, "cms_5min", [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_5min; }, 1},
+	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_cur", [](gysk_engine *e) -> unsigned long long *& { return e->fq.cur; }, 1},
+	{GYSK_FLAG_FLOW_QUERIES, "cms_qry_last", [](gysk_engine *e) -> unsigned long long *& { return e->fq.last; }, 1},
+	{GYSK_FLAG_FLOW_QUERY_LEVEL, "cms_qry_5min", [](gysk_engine *e) -> unsigned long long *& { return e->fq.level; }, 1},
+	{GYSK_FLAG_FLOW_RESP_HIST, "cms_resp_cur", [](gysk_engine *e) -> unsigned long long *& { return e->fr.cur; }, RESP_HIST_WORDS},
+	{GYSK_FLAG_FLOW_RESP_HIST, "cms_resp_last", [](gysk_engine *e) -> unsigned long long *& { return e->fr.last; }, RESP_HIST_WORDS},
+	{GYSK_FLAG_FLOW_RESP_HIST | GYSK_FLAG_FLOW_QUERY_LEVEL, "cms_resp_5min", [](gysk_engine *e) -> unsigned long long *& { return e->fr.level; },
+			RESP_HIST_WORDS},
 };
-inline bool cms_held(const gysk_config &cfg, int t) { return !CMS_TABLES[t].flag || (cfg.flags & CMS_TABLES[t].flag); }
+inline bool cms_held(const gysk_config &cfg, int t) { return (cfg.flags & CMS_TABLES[t].flag) == CMS_TABLES[t].flag; }
+// the u64 words of count-min table t
+inline size_t cms_words(const gysk_config &cfg, int t) { return cms_cells(cfg) * CMS_TABLES[t].words; }
 
 // A rolling 300-s level of a windowed pair: at each flush the open table `open` goes into a ring of NSLOTS tables by level 0's decision of
 // roll_levels, and the level table `level` becomes the sum of the live slots (launch_cms_level_roll). The engine holds the ring with the
@@ -399,6 +408,7 @@ struct CmsRingDesc
 inline const CmsRingDesc CMS_RINGS[] = {
 	{CMS_CUR, CMS_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_ring; }},
 	{CMS_QRY_CUR, CMS_QRY_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->fq.ring; }},
+	{CMS_RESP_CUR, CMS_RESP_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->fr.ring; }},
 };
 
 int fail(gysk_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess);
@@ -420,6 +430,8 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 // The count-min point queries of the flow query ABI calls on table t: the engine's own (the batch of the events handed in runs first) or,
 // merged, the last merge's sum over the ranks. GYSK_ERR_NOTSUP when the engine does not hold t; `what` names the call.
 int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
+// the same on a flow response histogram table (CMS_RESP_*)
+int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what);
 
 #define CU(e, call) do { cudaError_t ce__ = (call); if (ce__ != cudaSuccess) return gysk::fail((e), GYSK_ERR_CUDA, #call, ce__); } while (0)
 #define CHECK_ENGINE(e) do { if (!(e)) return GYSK_ERR_INVAL; if ((e)->sticky) return GYSK_ERR_CUDA; } while (0)

@@ -287,13 +287,52 @@ __device__ __forceinline__ void cms_add(const DevState &st, unsigned long long *
 		red_add_u64(cms + ((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask), inc);
 }
 
+// How a batch flow table entry {key, inc} reaches its cells, in the TASK pass's sweep and on the direct path of flow_add.
+// CmsApply: a count-min of one u64 per cell (connections, flow queries), key = h2 << 32 | h1.
+struct CmsApply
+{
+	const DevState &st;
+	unsigned long long *cms;
+	__device__ __forceinline__ void operator()(unsigned long long key, unsigned long long inc) const
+	{
+		cms_add(st, cms, (uint32_t)key, (uint32_t)(key >> 32), inc);
+	}
+};
+
+// GYSK_FLAG_FLOW_RESP_HIST: the key of a response sample in bucket b of the flow with hashes h1, h2, one per cell word:
+// ((b >> 1) + 1) << 56 | (h2 & wmask) << 28 | (h1 & wmask), its entry summing the word increments 1 << 32 * (b & 1). Row r's column
+// (h1 + r * (h2 | 1)) & wmask depends only on those low bits, and each field holds every width gysk_create accepts (CMS_LOG2W_MAX), so two
+// flows with the same key share every cell and their increments may be summed in one entry; the two buckets of a word share it too. The
+// key is never 0.
+static_assert(2 * CMS_LOG2W_MAX + 4 <= 64 && CMS_LOG2W_MAX <= 28, "resp_hist_key: two column fields of 28 bits and a word field");
+__device__ __forceinline__ unsigned long long resp_hist_key(uint32_t h1, uint32_t h2, uint32_t b, uint32_t wmask)
+{
+	return ((unsigned long long)((b >> 1) + 1u) << 56) | ((unsigned long long)(h2 & wmask) << 28) | (h1 & wmask);
+}
+__device__ __forceinline__ unsigned long long resp_hist_inc(uint32_t b) { return 1ull << (32u * (b & 1u)); }
+
+// RespHistApply: the summed increment inc of a resp_hist_key into its word of the table's cells, one RED.ADD.64 per row
+struct RespHistApply
+{
+	const DevState &st;
+	unsigned long long *tbl;
+	__device__ __forceinline__ void operator()(unsigned long long key, unsigned long long inc) const
+	{
+		const uint32_t w = (uint32_t)(key >> 56) - 1u, h1 = (uint32_t)key & 0xFFFFFFFu, h2 = (uint32_t)(key >> 28) & 0xFFFFFFFu;
+		for (uint32_t row = 0; row < st.cms_depth; ++row)
+			red_add_u64(tbl + ((((size_t)row << st.cms_log2w) + cms_index2(h1, h2, row, st.cms_wmask)) * RESP_HIST_WORDS + w), inc);
+	}
+};
+
 // One connection record's count-min increment into the batch's flow table, given the key k of entry pos (the first probe): a RED into the
 // flow's entry, claimed with a CAS on the key if need be. Past FLOW_PROBES entries, or for key 0, the record updates its count-min
-// cells (cms) directly (normal priority: nothing is left for the TASK pass to reset) and is counted in counter ctr, one RED per group of
-// converged lanes, since a table too small for the batch's flows sends most records this way. Entries only go from empty to a key
-// during the pass, so a record never misses its flow's entry; should a flow still hold two, the TASK pass applies both. A response
-// sample of GYSK_FLAG_FLOW_QUERIES takes the same path with the query flow table, cells and counter.
-__device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft, unsigned long long *cms, int ctr, unsigned long long key,
+// cells directly through apply (normal priority: nothing is left for the TASK pass to reset) and is counted in counter ctr, one RED per
+// group of converged lanes, since a table too small for the batch's flows sends most records this way. Entries only go from empty to a
+// key during the pass, so a record never misses its flow's entry; should a flow still hold two, the TASK pass applies both. A response
+// sample of GYSK_FLAG_FLOW_QUERIES takes the same path with the query flow table, cells and counter, and with GYSK_FLAG_FLOW_RESP_HIST
+// once more with the response flow table.
+template <typename Apply>
+__device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft, const Apply &apply, int ctr, unsigned long long key,
 		uint32_t pos, unsigned long long k, unsigned long long inc, unsigned long long pol_last)
 {
 	if (key) {
@@ -307,7 +346,7 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 	}
 	const uint32_t am = __activemask();
 	if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(st.counters + ctr, (unsigned long long)__popc(am));
-	cms_add(st, cms, (uint32_t)key, (uint32_t)(key >> 32), inc);
+	apply(key, inc);
 }
 
 // m queued connection records (all 32 lanes call): two lookup2 hashes per flow key -> the flow's entry in the batch's flow table (the
@@ -318,15 +357,18 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // TASK pass sets the lines back to evict_normal. pol_hll / pol_last: l2_policy_evict_first / _last.
 // QRY (GYSK_FLAG_FLOW_QUERIES): a record with slot QRY_REC is a response sample {usec, flow key}; it adds {1 | msec << 32} to its flow's
 // entry of the query flow table fq (cells fq_cms past the probe limit) and touches neither the HLL nor a service cell.
-template <bool QRY, typename HotTable>
+// RH (GYSK_FLAG_FLOW_RESP_HIST, only with QRY): such a record also adds its word increment to the entry of its resp_hist_key in the
+// response flow table fr (cells fr_cms past the probe limit).
+template <bool QRY, bool RH, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
-		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms)
+		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr,
+		unsigned long long *fr_cms)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
 		bool qry = false;
-		uint32_t cell = 0, idx = 0, rank = 0, hw = 0, pos = 0; int kb = 0;
-		unsigned long long key = 0, inc = 0, k = 0;
+		uint32_t cell = 0, idx = 0, rank = 0, hw = 0, pos = 0, rpos = 0; int kb = 0;
+		unsigned long long key = 0, inc = 0, k = 0, rkey = 0, rk = 0, rinc = 0;
 		if (act) {
 			const IngestRec r = ld_rec(q + i);
 			qry = QRY && r.slot == QRY_REC;
@@ -345,13 +387,21 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 			inc = qry ? 1ull | ((unsigned long long)(r.value / 1000u) << 32) : cms_increment(r.value);
 			pos = table_hash(key) & tmask;
 			if (key) k = ld_cg_hint_u64(&tent[pos].key, pol_last);
+			if (RH && qry) {
+				const uint32_t b = (uint32_t)bucket_resp_time((long long)(r.value / 1000u));
+				rkey = resp_hist_key(h1, h2, b, st.cms_wmask);
+				rinc = resp_hist_inc(b);
+				rpos = table_hash(rkey) & fr.mask;
+				rk = ld_cg_hint_u64(&fr.ent[rpos].key, pol_last);
+			}
 			cell = r.slot;
 			kb = (int)(r.value >> 10);
 		}
 		cell_add(st, hot, act && !qry, cell, kb);
 		if (act) {
-			if (qry) flow_add(st, fq, fq_cms, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
-			else flow_add(st, ft, st.cms_cur, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last);
+			if (qry) flow_add(st, fq, CmsApply {st, fq_cms}, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
+			else flow_add(st, ft, CmsApply {st, st.cms_cur}, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last);
+			if (RH && qry) flow_add(st, fr, RespHistApply {st, fr_cms}, CTR_FLOWR_DIRECT, rkey, rpos, rk, rinc, pol_last);
 		}
 		if (act && !qry) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
 	}
@@ -722,12 +772,13 @@ template <> struct DrainShape<false> { static constexpr int WARPS = 8, HOT_BITS 
 // cost three L2 REDs each, and they were most of the pass's time
 template <> struct DrainShape<true> { static constexpr int WARPS = 16, HOT_BITS = 13, ADMIT = 1; };
 
-// A flow table the TCP pass filled, swept by the whole grid of the TASK pass: each entry's sum into its flow's cells of count-min table
-// cms (the key holds the two hashes), then the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a
+// A flow table the TCP pass filled, swept by the whole grid of the TASK pass: each entry's sum into its flow's cells through apply (the
+// key holds what picks them), then the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a
 // priority they keep after it ends: back to normal, so that they do not hold L2 against the next batch's ingest_kernel and chain. A
 // thread takes FLOW_SWEEP entries a step, one grid stride apart, their loads in flight together (the REDs' memory clobber keeps a load
 // from moving past them).
-__device__ __forceinline__ void flow_sweep(const DevState &st, const FlowTable &t, unsigned long long *cms)
+template <typename Apply>
+__device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &apply)
 {
 	const uint32_t stride = gridDim.x * blockDim.x;
 	for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= t.mask; i0 += FLOW_SWEEP * stride) {
@@ -738,7 +789,7 @@ __device__ __forceinline__ void flow_sweep(const DevState &st, const FlowTable &
 		for (uint32_t u = 0; u < FLOW_SWEEP; ++u) {
 			const uint32_t i = i0 + u * stride;
 			if (f[u].key) {
-				cms_add(st, cms, (uint32_t)f[u].key, (uint32_t)(f[u].key >> 32), f[u].inc);
+				apply(f[u].key, f[u].inc);
 				t.ent[i] = FlowEnt {0ull, 0ull};
 			}
 			if (i <= t.mask && !(i & 7u)) l2_evict_normal_line(t.ent + i);
@@ -751,15 +802,17 @@ __device__ __forceinline__ void flow_sweep(const DevState &st, const FlowTable &
 // differ, the drain warps' work does not.
 // QRY (GYSK_FLAG_FLOW_QUERIES): the TCP pass also sums the queued response samples in the query flow table fq, and the TASK pass applies
 // that table to the query cells fq_cms after the connection flow table.
-template <bool TASK, bool QRY>
+// RH (GYSK_FLAG_FLOW_RESP_HIST, only with QRY): the same once more with the response flow table fr and the response histogram cells fr_cms.
+template <bool TASK, bool QRY, bool RH>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, FlowTable fq, unsigned long long *fq_cms)
+		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
 	if (TASK) {
-		flow_sweep(st, ft, st.cms_cur);
-		if (QRY) flow_sweep(st, fq, fq_cms);
+		flow_sweep(ft, CmsApply {st, st.cms_cur});
+		if (QRY) flow_sweep(fq, CmsApply {st, fq_cms});
+		if (RH) flow_sweep(fr, RespHistApply {st, fr_cms});
 	}
 	const unsigned long long pol_hll = TASK ? 0 : l2_policy_evict_first(), pol_last = TASK ? 0 : l2_policy_evict_last();
 	extern __shared__ __align__(16) unsigned char drain_smem[];
@@ -826,7 +879,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs<QRY>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms);
+			drain_tcp_recs<QRY, RH>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms);
 		}
 	}
 
@@ -2147,6 +2200,37 @@ __global__ void query_flows_kernel(const unsigned long long *__restrict__ tbl, u
 	out[i].flow_key = key; out[i].count = cnt; out[i].kbytes = kb;
 }
 
+// GYSK_FLAG_FLOW_RESP_HIST: per key and bucket the minimum over rows of the 8-word cells, then the response percentiles of those counts by
+// the rule of the service summaries' p95_5s_resp_ms (hist_percentile of RESP_TIME_HASH: GY_HISTOGRAM::get_percentiles), the full sum as the
+// total
+__global__ void query_flow_resp_kernel(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, const unsigned long long *__restrict__ keys,
+		uint32_t n, gysk_flow_resp_est *__restrict__ out)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const unsigned long long key = keys[i];
+	uint32_t mn[16];
+#pragma unroll
+	for (int b = 0; b < 16; ++b) mn[b] = 0xFFFFFFFFu;
+	for (uint32_t r = 0; r < depth; ++r) {
+		const ulonglong2 *c = reinterpret_cast<const ulonglong2 *>(tbl + (((size_t)r << log2w) + cms_index(key, r, (1u << log2w) - 1)) * RESP_HIST_WORDS);
+#pragma unroll
+		for (int w = 0; w < (int)RESP_HIST_WORDS / 2; ++w) {
+			const ulonglong2 v = c[w];
+			mn[4 * w] = min(mn[4 * w], (uint32_t)v.x); mn[4 * w + 1] = min(mn[4 * w + 1], (uint32_t)(v.x >> 32));
+			mn[4 * w + 2] = min(mn[4 * w + 2], (uint32_t)v.y); mn[4 * w + 3] = min(mn[4 * w + 3], (uint32_t)(v.y >> 32));
+		}
+	}
+	uint64_t counts[15], total = 0;
+#pragma unroll
+	for (int b = 0; b < 15; ++b) { counts[b] = mn[b]; total += mn[b]; out[i].counts[b] = mn[b]; }
+	out[i].flow_key = key;
+	out[i].total = (uint32_t)total;
+	out[i].p25_ms = hist_percentile(GYSK_CLS_RESP_TIME, false, counts, total, 25.0f);
+	out[i].p95_ms = hist_percentile(GYSK_CLS_RESP_TIME, false, counts, total, 95.0f);
+	out[i].p99_ms = hist_percentile(GYSK_CLS_RESP_TIME, false, counts, total, 99.0f);
+}
+
 // A rolling count-min level (GYSK_FLAG_FLOW_LEVEL, GYSK_FLAG_FLOW_QUERY_LEVEL) at a flush, one grid-stride pass over the cells in
 // 16-byte pairs. Ring slot k takes the closing window cur, added to what the slot holds or, when the flush started a new epoch there,
 // in its place (which stands in for clearing the slot). The level becomes the sum of the live slots, slot k's new content included. So the pass reads cur and the live
@@ -2268,40 +2352,42 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
-template <bool TASK, bool QRY>
+template <bool TASK, bool QRY, bool RH>
 static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, cudaStream_t s)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
 		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK, QRY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY>, WARPS * 32, smem_max);
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH>, WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq, fq_cms);
+	drain_kernel<TASK, QRY, RH><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq, fq_cms, fr, fr_cms);
 }
 
-template <bool QRY>
+template <bool QRY, bool RH>
 static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, cudaStream_t s)
 {
-	launch_drain_pass<false, QRY>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, s);
-	launch_drain_pass<true, QRY>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, s);
+	launch_drain_pass<false, QRY, RH>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, s);
+	launch_drain_pass<true, QRY, RH>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, s);
 	return 2;
 }
 
 // the batch's queued connection records -> flow table, HLL, exact cells; then the flow table -> count-min and its process records ->
 // process histograms. The TASK pass always runs: it leaves the flow table empty. The table takes the smallest power of two >= 2 x the
 // batch's events (the flows are fewer than the connection records), up to what tmp holds, so that a small batch sweeps a small table.
-// With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size.
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
+// With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size, and
+// with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too.
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const RecRegions &rr, uint64_t n_events,
+		cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
@@ -2309,9 +2395,13 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	while (n < tmp.flow_cap && n < 2 * n_events) n <<= 1;
 	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
-	if (!fq.cur) return launch_drain_passes<false>(st, ft, tmp, rr, n_events, dev, FlowTable {nullptr, 0u}, nullptr, s);
+	const FlowTable none {nullptr, 0u};
+	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
-	return launch_drain_passes<true>(st, ft, tmp, rr, n_events, dev, FlowTable {fq.flow, n - 1u}, fq.cur, s);
+	const FlowTable fqt {fq.flow, n - 1u};
+	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, s);
+	cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
+	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, s);
 }
 
 static void os_set_attrs(int dev)
@@ -2585,6 +2675,14 @@ int launch_query_flows(const unsigned long long *tbl, uint32_t depth, uint32_t l
 {
 	if (!n) return 0;
 	query_flows_kernel<<<div_up(n, 256), 256, 0, s>>>(tbl, depth, log2w, d_keys, n, d_out);
+	return 1;
+}
+
+int launch_query_flow_resp(const unsigned long long *tbl, uint32_t depth, uint32_t log2w, const unsigned long long *d_keys, uint32_t n,
+		gysk_flow_resp_est *d_out, cudaStream_t s)
+{
+	if (!n) return 0;
+	query_flow_resp_kernel<<<div_up(n, 128), 128, 0, s>>>(tbl, depth, log2w, d_keys, n, d_out);
 	return 1;
 }
 

@@ -160,6 +160,15 @@ static constexpr uint32_t FLOW_SWEEP = 4;		// entries per thread and step of the
 struct FlowQueries { unsigned long long *cur, *last; FlowEnt *flow; unsigned long long *ring, *level; };
 static constexpr uint32_t QRY_REC = 0xFFFFFFFFu;	// slot field of a queued response sample (service slots are < 2^24)
 
+// GYSK_FLAG_FLOW_RESP_HIST: the count-min of the same samples by RESP_TIME_HASH bucket, with the depth, width and row hashes of cms_cur.
+// A cell is RESP_HIST_WORDS u64 words: bucket b counts in half b & 1 of word b >> 1 (word 7's high half stays 0), every word summed
+// mod 2^64. The TCP pass sums the QRY_REC records in the batch flow table `flow` under the key resp_hist_key (the cell word and the low
+// bits of the two hashes that pick the cells: flows that share it share every cell), the TASK pass applies it. Laid out and kept out of
+// DevState as FlowQueries; every pointer nullptr: off. ring and level: with GYSK_FLAG_FLOW_QUERY_LEVEL too, the rolling 300-s level.
+struct FlowRespHist { unsigned long long *cur, *last; FlowEnt *flow; unsigned long long *ring, *level; };
+static constexpr uint32_t RESP_HIST_WORDS = 8;
+static constexpr uint32_t CMS_LOG2W_MAX = 28;		// the widest count-min gysk_create accepts (1 << 28 columns)
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
@@ -242,7 +251,9 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
 		RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
+// fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const RecRegions &rr, uint64_t n_events,
+		cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
 // bits outside [0, 64)), or n_max >= 2^30
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);
@@ -289,6 +300,9 @@ int launch_task_summaries(const DevState &st, const unsigned long long *d_ids, c
 // the count-min point queries of n flow keys on table tbl ([depth][1 << log2w] cells)
 int launch_query_flows(const unsigned long long *tbl, uint32_t depth, uint32_t log2w, const unsigned long long *d_keys, uint32_t n, gysk_flow_est *d_out,
 		cudaStream_t s);
+// the same on a flow response histogram table ([depth][1 << log2w][RESP_HIST_WORDS] words): bucket counts, total and percentiles
+int launch_query_flow_resp(const unsigned long long *tbl, uint32_t depth, uint32_t log2w, const unsigned long long *d_keys, uint32_t n,
+		gysk_flow_resp_est *d_out, cudaStream_t s);
 // a rolling count-min level at the flush, before its window pair's swap: the open table cur ([cells]) into ring slot lv.cur[0]
 // (replacing it when the slot is fresh), then level = the sum of the live slots (level 0's decision of lv)
 int launch_cms_level_roll(const unsigned long long *cur, unsigned long long *ring, unsigned long long *level, size_t cells, const LevelRing &lv,

@@ -16,7 +16,8 @@
 //                          GYSK_FLAG_FLOW_LEVEL puts the count-min level after cms cur/last and, as GYSK_FLAG_MERGE_LEVELS does,
 //                          the flush tsec pair in the i64 MAX region (once when both are set); GYSK_FLAG_FLOW_QUERIES puts the
 //                          flow query tables cur/last after the count-min tables, GYSK_FLAG_FLOW_QUERY_LEVEL their level after
-//                          them with the flush tsec pair as GYSK_FLAG_FLOW_LEVEL
+//                          them with the flush tsec pair as GYSK_FLAG_FLOW_LEVEL; GYSK_FLAG_FLOW_RESP_HIST the flow response
+//                          histograms cur/last [, 5min] after those
 //   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests [, the global pick of the gathered top-N candidates]
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
@@ -817,7 +818,8 @@ int lay_out_arena(gysk_engine *e)
 	// regions, GYSK_FLAG_MERGE_STATES its words to the end of the SUM region after them, GYSK_FLAG_MERGE_CLUSTERS its words after those.
 	// GYSK_FLAG_FLOW_LEVEL puts the count-min level after the two window tables, and needs the flush tsec pair as the levels do:
 	// still three regions, three collectives. GYSK_FLAG_FLOW_QUERIES puts the two flow query tables after the count-min ones, and
-	// GYSK_FLAG_FLOW_QUERY_LEVEL their level after them, with the flush tsec pair.
+	// GYSK_FLAG_FLOW_QUERY_LEVEL their level after them, with the flush tsec pair. GYSK_FLAG_FLOW_RESP_HIST puts the flow response
+	// histograms (and with GYSK_FLAG_FLOW_QUERY_LEVEL their level) after all of them: 8 words a cell, summed like every other word.
 	// GYSK_FLAG_MERGE_TRACES puts its words at the end of the SUM region, its maxima at the end of the i64 MAX one, and needs the flush
 	// tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
@@ -832,7 +834,7 @@ int lay_out_arena(gysk_engine *e)
 			names += (names.empty() ? "" : "|") + std::string(name);
 		};
 		mg.off_sum = off;
-		for (int t = 0; t < NCMS; ++t) if (cms_held(e->cfg, t)) take(mg.g_cms[t], cms_cells(e->cfg) * 8, CMS_TABLES[t].name);
+		for (int t = 0; t < NCMS; ++t) if (cms_held(e->cfg, t)) take(mg.g_cms[t], cms_words(e->cfg, t) * 8, CMS_TABLES[t].name);
 		take(lg.last, b_hist, "hist_last"); take(lg.all, b_hist, "hist_all"); take(lg.conn, (size_t)nl * 4 * 8, "conn");
 		if (levels) { take(lg.lvl, NLEVELS * b_hist, "levels"); take(lg.aux, (size_t)nl * 4 * 8, "aux"); }
 		if (states) take(lg.states, (size_t)nl * STATE_WORDS * 8, "states");
@@ -1000,7 +1002,7 @@ int gysk_merge_prepare(gysk_engine *e)
 	const uint32_t nl = mg.lg.nl;
 
 	for (int t = 0; t < NCMS; ++t)
-		if (mg.g_cms[t]) CU(e, cudaMemcpyAsync(mg.g_cms[t], CMS_TABLES[t].live(e), cms_cells(e->cfg) * 8, cudaMemcpyDeviceToDevice, e->stream));
+		if (mg.g_cms[t]) CU(e, cudaMemcpyAsync(mg.g_cms[t], CMS_TABLES[t].live(e), cms_words(e->cfg, t) * 8, cudaMemcpyDeviceToDevice, e->stream));
 	if (nl) {
 		if (mg.nmembers) {
 			resolve_members_kernel<<<div_up(mg.nmembers, 256), 256, 0, e->stream>>>(e->st, mg.d_member_ids, mg.nmembers, mg.members);
@@ -1311,6 +1313,17 @@ int gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *keys, uint32_
 int gysk_query_flow_queries_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_qry_est *out)
 {
 	return query_cms(e, CMS_QRY_5MIN, true, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries_global_5min");
+}
+
+// GYSK_FLAG_FLOW_RESP_HIST: the point query on the flow response histograms (and their level) summed over the ranks
+int gysk_query_flow_resp_global(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_resp_est *out)
+{
+	return query_cms_resp(e, last_window ? CMS_RESP_LAST : CMS_RESP_CUR, true, keys, n, out, "query_flow_resp_global");
+}
+
+int gysk_query_flow_resp_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out)
+{
+	return query_cms_resp(e, CMS_RESP_5MIN, true, keys, n, out, "query_flow_resp_global_5min");
 }
 
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)

@@ -13,6 +13,9 @@ assert EVENT_DTYPE.itemsize == 32
 SERIAL_DTYPE = np.dtype([("count", "<u8"), ("sum", "<i8")])
 FLOW_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("count", "<u4"), ("kbytes", "<u4")])
 FLOW_QRY_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("queries", "<u4"), ("resp_ms", "<u4")])     # gysk_flow_qry_est
+FLOW_RESP_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("counts", "<u4", (15,)), ("total", "<u4"), ("p25_ms", "<i8"), ("p95_ms", "<i8"),
+                                ("p99_ms", "<i8")])                                                   # gysk_flow_resp_est
+RESP_HIST_WORDS = 8     # u64 words of one flow response histogram cell
 
 EV_CONNECT, EV_ACCEPT, EV_CLOSE_CLI, EV_CLOSE_SER, EV_RESP, EV_TASK, EV_ACTIVE = 1, 2, 3, 4, 5, 6, 7
 EVF_CLI_ERROR, EVF_SER_ERROR = 1, 2
@@ -37,6 +40,7 @@ FLAG_AUTO_REGISTER, FLAG_MERGE_LEVELS, FLAG_MERGE_STATES, FLAG_MERGE_CLUSTERS, F
 FLAG_MERGE_TRACES = 64
 FLAG_FLOW_QUERIES = 128
 FLAG_FLOW_QUERY_LEVEL = 0x100
+FLAG_FLOW_RESP_HIST = 0x200
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
@@ -314,6 +318,13 @@ def load_library(path=None):
         "gysk_export_cms_queries_5min": (i32, [vp, vp]),
         "gysk_query_flow_queries_global_5min": (i32, [vp, vp, u32, vp]),
         "gysk_last_batch_flow_query_direct": (C.c_int64, [vp]),
+        "gysk_query_flow_resp": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_export_cms_resp": (i32, [vp, i32, vp]),
+        "gysk_query_flow_resp_global": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_flow_resp_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_export_cms_resp_5min": (i32, [vp, vp]),
+        "gysk_query_flow_resp_global_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_last_batch_flow_resp_direct": (C.c_int64, [vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -379,7 +390,7 @@ class Engine:
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
-                 max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False):
+                 max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -393,7 +404,8 @@ class Engine:
         cfg.flags = (FLAG_AUTO_REGISTER if auto_register else 0) | (FLAG_MERGE_LEVELS if merge_levels else 0) | \
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
-                    (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0)
+                    (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
+                    (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -583,9 +595,13 @@ class Engine:
         """response samples of the last device batch whose flow query update bypassed the query flow table (flow_queries=True)"""
         return self._counter(self.L.gysk_last_batch_flow_query_direct)
 
+    def last_batch_flow_resp_direct(self):
+        """response samples of the last device batch whose flow response histogram update bypassed its flow table (flow_resp_hist=True)"""
+        return self._counter(self.L.gysk_last_batch_flow_resp_direct)
+
     def flow_table_used(self):
-        """non-zero entries of the batch flow tables (the query one too with flow_queries=True): 0 whenever no batch is in flight
-        (diagnostic)"""
+        """non-zero entries of the batch flow tables (the query one too with flow_queries=True, the response one with
+        flow_resp_hist=True): 0 whenever no batch is in flight (diagnostic)"""
         n = self.L.gysk_flow_table_used(self.h)
         if n < 0:
             self._chk(int(n))
@@ -676,11 +692,11 @@ class Engine:
         self._chk(fn(self.h, _p(keys), len(keys), *window, _p(out)))
         return out
 
-    def _export_cells(self, fn, *window):
-        """the cells of a count-min table, fn(h, [last_window,] cells)"""
-        out = np.zeros(self.cfg.cms_depth << self.cfg.cms_log2_width, dtype=np.uint64)
+    def _export_cells(self, fn, *window, words=1):
+        """the cells of a count-min table, fn(h, [last_window,] cells); words > 1: shape (cells, words)"""
+        out = np.zeros((self.cfg.cms_depth << self.cfg.cms_log2_width) * words, dtype=np.uint64)
         self._chk(fn(self.h, *window, _p(out)))
-        return out
+        return out if words == 1 else out.reshape(-1, words)
 
     def query_flows(self, keys, last_window=False):
         return self._point_query(self.L.gysk_query_flows, FLOW_EST_DTYPE, keys, int(last_window))
@@ -980,6 +996,32 @@ class Engine:
     def query_flow_queries_global(self, keys, last_window=False):
         """gysk_query_flow_queries_global: the point query on the flow query tables summed over the ranks by the last merge"""
         return self._point_query(self.L.gysk_query_flow_queries_global, FLOW_QRY_EST_DTYPE, keys, int(last_window))
+
+    def query_flow_resp(self, keys, last_window=False):
+        """gysk_query_flow_resp: per flow key the response-time bucket counts (min over rows), their total and p25 / p95 / p99 msec
+        (flow_resp_hist=True)"""
+        return self._point_query(self.L.gysk_query_flow_resp, FLOW_RESP_EST_DTYPE, keys, int(last_window))
+
+    def export_cms_resp(self, last_window=False):
+        """gysk_export_cms_resp: the flow response histogram cells, shape (depth << log2_width, 8) (flow_resp_hist=True)"""
+        return self._export_cells(self.L.gysk_export_cms_resp, int(last_window), words=RESP_HIST_WORDS)
+
+    def query_flow_resp_global(self, keys, last_window=False):
+        """gysk_query_flow_resp_global: the point query on the flow response histograms summed over the ranks by the last merge"""
+        return self._point_query(self.L.gysk_query_flow_resp_global, FLOW_RESP_EST_DTYPE, keys, int(last_window))
+
+    def query_flow_resp_5min(self, keys):
+        """gysk_query_flow_resp_5min: the point query on the rolling 300-s level of the flow response histograms
+        (flow_resp_hist=True, flow_query_level=True)"""
+        return self._point_query(self.L.gysk_query_flow_resp_5min, FLOW_RESP_EST_DTYPE, keys)
+
+    def export_cms_resp_5min(self):
+        """gysk_export_cms_resp_5min: the cells of that level, shape (depth << log2_width, 8)"""
+        return self._export_cells(self.L.gysk_export_cms_resp_5min, words=RESP_HIST_WORDS)
+
+    def query_flow_resp_global_5min(self, keys):
+        """gysk_query_flow_resp_global_5min: the point query on that level summed over the ranks by the last merge"""
+        return self._point_query(self.L.gysk_query_flow_resp_global_5min, FLOW_RESP_EST_DTYPE, keys)
 
     def export_cms_queries_5min(self):
         """gysk_export_cms_queries_5min: the cells of the rolling 300-s flow query level (flow_query_level=True)"""

@@ -236,6 +236,20 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   GYSK_FLAG_FLOW_QUERIES: gysk_create refuses it without; combines freely with every other
 						   flag. Costs NSLOTS + 1 = 11 more tables of depth << log2_width cells. Without it nothing is
 						   allocated, every other call answers as before and the three calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_FLOW_RESP_HIST	0x200u	/* a count-min of the flow query samples by response-time bucket: each client flow's
+						   response histogram and its p25 / p95 / p99 in the open and the last window
+						   (gysk_query_flow_resp, "flow response histograms" below), with GYSK_FLAG_FLOW_QUERY_LEVEL
+						   also over the rolling 300 s; with it the merge step also sums those tables across ranks
+						   (the same flags on every rank). Needs GYSK_FLAG_FLOW_QUERIES: gysk_create refuses it
+						   without. Costs 8x the words of a query table: 2 tables of depth << log2_width 64-byte
+						   cells (512 MiB at 4 x 2^20), 11 more with GYSK_FLAG_FLOW_QUERY_LEVEL (2.75 GiB), and a
+						   third batch flow table; gysk_merge_prepare's arena holds one more copy of each held
+						   table (512 MiB more, 768 MiB with the level). Measured on one H100 80GB HBM3 at 700 W with the bench workload
+						   (100 M-event batches, against GYSK_FLAG_FLOW_QUERIES alone): the TCP drain pass 6.4 ->
+						   24.5 ms and the TASK pass 0.9 -> 1.2 ms per batch (its flows x cell words overflow the
+						   batch table, so 10 M samples a batch update the cells directly), gysk_flush 0.51 -> 0.63
+						   ms (1.92 ms with the level), gysk_merge_prepare +0.41 ms (+0.56 ms with the level). Without it nothing is allocated, every other
+						   call answers as before and the flow response calls are GYSK_ERR_NOTSUP */
 
 typedef struct gysk_config
 {
@@ -372,6 +386,17 @@ typedef struct gysk_flow_qry_est
 	uint32_t	resp_ms;		/* min over rows of the response msec halves */
 } gysk_flow_qry_est;
 
+/* a point query on the flow response histograms (GYSK_FLAG_FLOW_RESP_HIST), 96 bytes */
+typedef struct gysk_flow_resp_est
+{
+	uint64_t	flow_key;
+	uint32_t	counts[15];		/* per RESP_TIME_HASH bucket the minimum over rows */
+	uint32_t	total;			/* the sum of counts (mod 2^32) */
+	int64_t		p25_ms, p95_ms, p99_ms;	/* GY_HISTOGRAM::get_percentiles of RESP_TIME_HASH on counts (the full sum as the
+						   total): the rule of gysk_svc_summary::p95_5s_resp_ms, so gysk_hist_percentiles(GYSK_CLS_RESP_TIME,
+						   0, ...) on the same counts; -1 when the cut-off falls in bucket 0 (an empty histogram) */
+} gysk_flow_resp_est;
+
 typedef struct gysk_stats
 {
 	uint64_t	events_in;		/* events handed to the device */
@@ -422,6 +447,9 @@ int64_t		gysk_flow_table_used(gysk_engine *e);
 /* diagnostic (GYSK_FLAG_FLOW_QUERIES): response samples of the last device batch whose flow query update did not go through the batch's
  * query flow table (its probe limit reached). Routing only. GYSK_ERR_NOTSUP without the flag; negative = GYSK_ERR_*. */
 int64_t		gysk_last_batch_flow_query_direct(gysk_engine *e);
+/* diagnostic (GYSK_FLAG_FLOW_RESP_HIST): response samples of the last device batch whose flow response histogram update did not go
+ * through the batch's response flow table (its probe limit reached). Routing only. GYSK_ERR_NOTSUP without the flag. */
+int64_t		gysk_last_batch_flow_resp_direct(gysk_engine *e);
 
 /* ---- capacity: growing the service / process tables of a live engine ---- */
 /* Raise the service / process capacity of a live engine (either may equal the current value; neither may shrink, both <= 1 << 24).
@@ -457,8 +485,11 @@ int		gysk_capacity_info(gysk_engine *e, gysk_capacity *out);	/* synchronises the
  * max_svcs x svc_slot_bytes + max_tasks x task_slot_bytes, plus the id tables (16 B x the power of two >= 2 x slots each), the sort
  * buffers and the count-min tables: 2 tables of cms_depth << cms_log2_width 8-byte cells, 11 more with GYSK_FLAG_FLOW_LEVEL (its 10 ring
  * slots and the level: 352 MiB more at the default 4 x 2^20), 2 more with GYSK_FLAG_FLOW_QUERIES (64 MiB at 4 x 2^20, plus a second
- * batch flow table of up to 32 MiB), 11 more with GYSK_FLAG_FLOW_QUERY_LEVEL (352 MiB at 4 x 2^20, 2.8 GiB at 8 x 2^22). The count-min
- * tables do not depend on capacity, so gysk_grow and eviction leave them; gysk_capacity.device_bytes counts them.
+ * batch flow table of up to 32 MiB), 11 more with GYSK_FLAG_FLOW_QUERY_LEVEL (352 MiB at 4 x 2^20, 2.8 GiB at 8 x 2^22), 2 tables of
+ * 64-byte cells with GYSK_FLAG_FLOW_RESP_HIST (512 MiB at 4 x 2^20, plus a third batch flow table) and 11 more with it and
+ * GYSK_FLAG_FLOW_QUERY_LEVEL (2.75 GiB at 4 x 2^20). The count-min tables do not depend on capacity, so gysk_grow and eviction leave
+ * them; gysk_capacity.device_bytes counts them. The merge arena (gysk_merge_prepare, in device_bytes) holds one more copy of every
+ * count-min table the engine holds.
  * Trace rows (max_trace_svcs) are not per service slot and not counted here: 3784 bytes each, in gysk_capacity.device_bytes. */
 int		gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *task_slot_bytes);
 
@@ -670,6 +701,31 @@ int		gysk_query_flow_queries_global(gysk_engine *e, const uint64_t *flow_keys, u
 int		gysk_query_flow_queries_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_qry_est *out);
 int		gysk_export_cms_queries_5min(gysk_engine *e, uint64_t *cells /* depth << log2_width entries */);
 int		gysk_query_flow_queries_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_qry_est *out);
+
+/* ---- flow response histograms (GYSK_FLAG_FLOW_RESP_HIST): how slow a client's slow requests were ----
+ * The flow query tables give a client's mean response time; these give its response histogram, so its p95 / p99. They count exactly
+ * the samples the flow query tables count, under the same keys (RESP16 and API_TRAN samples under the client port alone), with the
+ * depth, width and row hashes of the connection count-min: a key lands in the same columns of all three table families. A cell is 8 u64
+ * words (64 bytes): the count of RESP_TIME_HASH bucket b (0 .. 14, of msec = usec / 1000) sits in half b & 1 (low 32 bits: 0) of word
+ * b >> 1, word 7's high half is always 0. Every word is summed mod 2^64 like every other count-min cell; a known edge: a bucket count
+ * past 2^32 in one cell carries into its neighbour bucket, as the query half of a flow query cell carries into its msec half. So for
+ * every row and column the 15 counts of a cell sum to the query half of the same flow query cell (mod 2^32), and for every row and
+ * bucket the column sum equals that bucket summed over every service's response histogram of the same window.
+ * The windows: the open table and the last closed one, by the count-min's flush rule; with GYSK_FLAG_FLOW_QUERY_LEVEL also the rolling
+ * 300-s level by the rule of gysk_query_flow_queries_5min: the cell-wise sum of the held windows' gysk_export_cms_resp(last_window = 1)
+ * tables.
+ * gysk_query_flow_resp: per key and bucket the minimum over rows (a count-min estimate: never below the key's exact count), their sum and
+ *   the percentiles of those counts (gysk_flow_resp_est). A key alone in its columns gets its exact histogram and percentiles.
+ * gysk_export_cms_resp: the open (last_window = 0) or last closed table, (depth << log2_width) x 8 words, cell-major.
+ * gysk_query_flow_resp_global: the point query on the tables summed over the ranks by the last merge (GYSK_ERR_INVAL before
+ *   gysk_merge_prepare). The _5min triple: the same on the level (GYSK_ERR_NOTSUP without GYSK_FLAG_FLOW_QUERY_LEVEL).
+ * gysk_grow and eviction leave the tables alone. Every call is GYSK_ERR_NOTSUP without the flag. */
+int		gysk_query_flow_resp(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_resp_est *out);
+int		gysk_export_cms_resp(gysk_engine *e, int last_window, uint64_t *words /* (depth << log2_width) x 8 entries */);
+int		gysk_query_flow_resp_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_resp_est *out);
+int		gysk_query_flow_resp_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_resp_est *out);
+int		gysk_export_cms_resp_5min(gysk_engine *e, uint64_t *words /* (depth << log2_width) x 8 entries */);
+int		gysk_query_flow_resp_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_resp_est *out);
 
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
