@@ -71,15 +71,24 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	RecRegions rr;
-	const int li = launch_ingest(e->st, e->tmp, e->fq, d_ev, n, key_slots(e), rr, e->stream);
+	const int li = launch_ingest(e->st, e->tmp, e->fq, e->topk.tk, d_ev, n, key_slots(e), rr, e->stream);
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, rr, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[2], e->stream));
+	// GYSK_FLAG_FLOW_TOPK: each held table's open set from its candidates, once all of the batch's increments are in the table. After the
+	// batch merge, whose sort buffers it takes.
+	for (int w = 0; w < 2; ++w) {
+		if (!e->topk.tk.list[w].keys) continue;
+		const int k = launch_topk_select(e->tmp, e->topk.tk.list[w], TOPK_K + n, CMS_TABLES[TOPK_TABLE[w]].live(e), e->cfg.cms_depth,
+				e->cfg.cms_log2_width, TOPK_HALF[w], e->topk.open[w], true, e->stream);
+		if (k < 0) return fail(e, GYSK_ERR_INVAL, "heaviest-flow selection: no sort plan");
+		e->kernel_launches += k;
+	}
 	e->batches++;
 	return post_launch(e, "ingest batch");
 }
@@ -316,6 +325,32 @@ int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t
 	}, CopyRows<gysk_flow_est> {out});
 }
 
+int topk_read(gysk_engine *e, int which, int last_window, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout, const char *what)
+{
+	CHECK_ENGINE(e);
+	if (!nout || (!out && n)) return GYSK_ERR_INVAL;
+	if (!e->topk.open[which]) return GYSK_ERR_NOTSUP;
+	Entry entry(e, merged ? Pending::Drain : Pending::Submit);
+	if (entry.rc) return entry.rc;
+	if (merged && !e->mg.topk_done) return fail(e, GYSK_ERR_INVAL, ("gysk_" + std::string(what) + ": no finished merge").c_str());
+	const unsigned long long *set = merged ? e->mg.topk_final + (size_t)which * TOPK_SET_WORDS : last_window ? e->topk.last[which] : e->topk.open[which];
+	std::vector<uint64_t> keys(TOPK_SET_WORDS);
+	CU(e, cudaMemcpyAsync(keys.data(), set, sizeof(uint64_t) * TOPK_SET_WORDS, cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	const uint32_t m = (uint32_t)std::min<uint64_t>({keys[0], (uint64_t)n, (uint64_t)TOPK_K});
+	const int t = TOPK_TABLE[which] + 1;		// the table of the last window (merged: the summed one)
+	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[last_window ? t : t - 1].live(e);
+	std::vector<gysk_flow_est> rows(m);
+	int rc = staged_read(e, keys.data() + 2, m, QCHUNK, sizeof(gysk_flow_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t k) {
+		return launch_query_flows(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, k, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
+	}, CopyRows<gysk_flow_est> {rows.data()});
+	if (rc) return rc;
+	uint32_t k = 0;
+	for (const gysk_flow_est &r : rows) if (TOPK_HALF[which] ? r.kbytes : r.count) out[k++] = r;
+	*nout = k;
+	return GYSK_OK;
+}
+
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what)
 {
 	CHECK_ENGINE(e);
@@ -478,7 +513,9 @@ size_t slots_of(SlotKind kind, uint32_t max_svcs, uint32_t max_tasks, uint32_t m
 uint32_t table_cap(uint32_t slots) { return pow2_at_least((uint64_t)slots * 2); }
 size_t sort_keys(const gysk_config &cfg)
 {
-	return std::max<size_t>(std::max<size_t>(std::max<size_t>((size_t)cfg.max_svcs + 1, cfg.max_tasks) + 1, cfg.max_batch), (size_t)cfg.max_trace_svcs + 1);
+	// GYSK_FLAG_FLOW_TOPK: a batch's heaviest-flow candidates are its open set and up to one key per event
+	const size_t batch = (size_t)cfg.max_batch + ((cfg.flags & GYSK_FLAG_FLOW_TOPK) ? TOPK_K : 0);
+	return std::max<size_t>(std::max<size_t>(std::max<size_t>((size_t)cfg.max_svcs + 1, cfg.max_tasks) + 1, batch), (size_t)cfg.max_trace_svcs + 1);
 }
 uint32_t sort_tiles(size_t nkeys) { return (uint32_t)((nkeys + SORT_TILE - 1) / SORT_TILE); }
 size_t batch_rows(const gysk_config &cfg) { return std::min<size_t>((size_t)cfg.max_svcs + 1 + cfg.max_trace_svcs, ((size_t)cfg.max_batch + LONG_SEG - 1) / LONG_SEG); }
@@ -690,6 +727,14 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
 		if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) A(dalloc(e, &e->fq.flow, (size_t)tmp.flow_cap));		// the query flow table, alike
 		if (cfg.flags & GYSK_FLAG_FLOW_RESP_HIST) A(dalloc(e, &e->fr.flow, (size_t)tmp.flow_cap));		// the response flow table, alike
+		// GYSK_FLAG_FLOW_TOPK: per held table its candidate list, the keys beside its batch flow table and its two sets, all empty
+		for (int w = 0; w < 2 && (cfg.flags & GYSK_FLAG_FLOW_TOPK); ++w) {
+			if (!cms_held(cfg, TOPK_TABLE[w])) continue;
+			TopkList &l = e->topk.tk.list[w];
+			l.cap = (uint64_t)TOPK_K + cfg.max_batch;
+			A(dalloc(e, &l.keys, (size_t)l.cap, false)); A(dalloc(e, &l.n, 1)); A(dalloc(e, &l.ekeys, (size_t)tmp.flow_cap, false));
+			A(dalloc(e, &e->topk.open[w], (size_t)TOPK_SET_WORDS)); A(dalloc(e, &e->topk.last[w], (size_t)TOPK_SET_WORDS));
+		}
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
 	if (cfg.max_trace_svcs) {
@@ -1613,6 +1658,12 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		std::swap(open, CMS_TABLES[t + 1].live(e));
 		CU(e, cudaMemsetAsync(open, 0, sizeof(unsigned long long) * cms_words(e->cfg, t), e->stream));
 	}
+	for (int w = 0; w < 2; ++w) {		// GYSK_FLAG_FLOW_TOPK: each heaviest-flow set with its table, and no candidates yet
+		if (!e->topk.open[w]) continue;
+		std::swap(e->topk.open[w], e->topk.last[w]);
+		CU(e, cudaMemsetAsync(e->topk.open[w], 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
+		CU(e, cudaMemsetAsync(e->topk.tk.list[w].n, 0, sizeof(unsigned long long), e->stream));
+	}
 	return post_launch(e, "flush");
 }
 
@@ -2036,6 +2087,17 @@ int gysk_query_flows_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk
 int gysk_query_flow_queries(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_qry_est *out)
 {
 	return query_cms(e, last_window ? CMS_QRY_LAST : CMS_QRY_CUR, false, keys, n, reinterpret_cast<gysk_flow_est *>(out), "query_flow_queries");
+}
+
+// GYSK_FLAG_FLOW_TOPK: the heaviest flows of the open or last window
+int gysk_topk_flows(gysk_engine *e, int last_window, uint32_t n, gysk_flow_est *out, uint32_t *nout)
+{
+	return topk_read(e, 0, last_window, false, n, out, nout, "topk_flows");
+}
+
+int gysk_topk_flow_queries(gysk_engine *e, int last_window, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout)
+{
+	return topk_read(e, 1, last_window, false, n, reinterpret_cast<gysk_flow_est *>(out), nout, "topk_flow_queries");
 }
 
 // GYSK_FLAG_FLOW_QUERY_LEVEL: the point query on the rolling 300-s level of the flow query tables

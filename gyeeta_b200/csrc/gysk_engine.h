@@ -244,6 +244,15 @@ constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(Sla
 // keeps its merge arena.
 enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, CMS_RESP_CUR, CMS_RESP_LAST, CMS_RESP_5MIN, NCMS };
 
+// GYSK_FLAG_FLOW_TOPK (every pointer nullptr without): the candidate lists and the open / last heaviest-flow sets ([TOPK_SET_WORDS]
+// each) of the connection table [0] and, with GYSK_FLAG_FLOW_QUERIES, the flow query table [1]. Outside DevState, so that the kernels
+// without the flag keep their parameter layout; not per slot, so gysk_grow and eviction leave them.
+struct TopkSets { FlowTopk tk; unsigned long long *open[2], *last[2]; };
+// the count-min table of each set, and the half of its cells that scores (1: kbytes, the high half; 0: queries, the low half)
+constexpr int TOPK_TABLE[2] = {CMS_CUR, CMS_QRY_CUR}, TOPK_HALF[2] = {1, 0};
+// both sets of a rank in the merge slab, in whole SlabEntrys after the rest of its content
+constexpr uint32_t TOPK_SLAB_ENTRIES = (uint32_t)((2 * TOPK_SET_WORDS * sizeof(unsigned long long) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
+
 // the cells of one count-min table
 inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
 
@@ -282,6 +291,13 @@ struct MergeState
 	uint32_t		trace_off {0};
 	unsigned long long	*topn_slots {nullptr};			// [TOPN_LISTS][TOPN_K] this rank's candidate slots (the rows' input)
 	uint8_t			*topn_final {nullptr};			// TopnLists::BYTES: the winners of the last finished merge
+	// GYSK_FLAG_FLOW_TOPK: the rank's last-window sets ride from slab entry topk_off (TOPK_SLAB_ENTRIES); the merged sets of the last
+	// finished merge ([2][TOPK_SET_WORDS]); the union's candidates and sort buffers (3 x topk_cap keys, with their look-back tiles)
+	uint32_t		topk_off {0};
+	unsigned long long	*topk_final {nullptr};
+	bool			topk_done {false};
+	unsigned long long	*topk_buf {nullptr}, *topk_n {nullptr}, *topk_tiles {nullptr};
+	uint64_t		topk_cap {0};
 };
 
 } // namespace gysk
@@ -295,6 +311,7 @@ struct gysk_engine
 	gysk::SortTemp		tmp {};
 	gysk::FlowQueries	fq {};				// GYSK_FLAG_FLOW_QUERIES (every pointer nullptr without)
 	gysk::FlowRespHist	fr {};				// GYSK_FLAG_FLOW_RESP_HIST (every pointer nullptr without)
+	gysk::TopkSets		topk {};			// GYSK_FLAG_FLOW_TOPK (every pointer nullptr without)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
 	std::vector<void *>	hallocs;
@@ -430,6 +447,10 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 // The count-min point queries of the flow query ABI calls on table t: the engine's own (the batch of the events handed in runs first) or,
 // merged, the last merge's sum over the ranks. GYSK_ERR_NOTSUP when the engine does not hold t; `what` names the call.
 int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
+// GYSK_FLAG_FLOW_TOPK: the first min(n, K) flows of heaviest-flow set `which` (0: connections, 1: flow queries), best first, with their
+// estimates on its table: the engine's open (last_window = 0) or last set, or merged, the last finished merge's set on the summed table.
+// Flows with a zero score are left out.
+int topk_read(gysk_engine *e, int which, int last_window, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout, const char *what);
 // the same on a flow response histogram table (CMS_RESP_*)
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what);
 

@@ -324,20 +324,50 @@ struct RespHistApply
 	}
 };
 
+// GYSK_FLAG_FLOW_TOPK: flow key fk appended to candidate list l, one cursor atomic per group of converged lanes
+__device__ __forceinline__ void topk_append(const TopkList &l, unsigned long long fk)
+{
+	const uint32_t am = __activemask(), lane = threadIdx.x & 31, leader = __ffs(am) - 1;
+	unsigned long long base = 0;
+	if (lane == leader) base = atomicAdd(l.n, (unsigned long long)__popc(am));
+	base = __shfl_sync(am, base, leader) + __popc(am & ((1u << lane) - 1u));
+	if (base < l.cap) l.keys[base] = fk;
+}
+
+// What flow_add and flow_sweep record of the flow keys for GYSK_FLAG_FLOW_TOPK: NoCapture nothing; TopkCapture the key of the record that
+// claims an entry (beside the entry, for the sweep) and of a record on the direct path (into the candidates).
+struct NoCapture
+{
+	__device__ __forceinline__ void claim(uint32_t, unsigned long long) const {}
+	__device__ __forceinline__ void direct(unsigned long long) const {}
+	__device__ __forceinline__ void swept(uint32_t) const {}
+};
+struct TopkCapture
+{
+	const TopkList &l;
+	__device__ __forceinline__ void claim(uint32_t pos, unsigned long long fk) const { l.ekeys[pos] = fk; }
+	__device__ __forceinline__ void direct(unsigned long long fk) const { topk_append(l, fk); }
+	__device__ __forceinline__ void swept(uint32_t pos) const { topk_append(l, l.ekeys[pos]); }
+};
+
 // One connection record's count-min increment into the batch's flow table, given the key k of entry pos (the first probe): a RED into the
 // flow's entry, claimed with a CAS on the key if need be. Past FLOW_PROBES entries, or for key 0, the record updates its count-min
 // cells directly through apply (normal priority: nothing is left for the TASK pass to reset) and is counted in counter ctr, one RED per
 // group of converged lanes, since a table too small for the batch's flows sends most records this way. Entries only go from empty to a
 // key during the pass, so a record never misses its flow's entry; should a flow still hold two, the TASK pass applies both. A response
 // sample of GYSK_FLAG_FLOW_QUERIES takes the same path with the query flow table, cells and counter, and with GYSK_FLAG_FLOW_RESP_HIST
-// once more with the response flow table.
-template <typename Apply>
+// once more with the response flow table. cap records the record's flow key fk (GYSK_FLAG_FLOW_TOPK).
+template <typename Apply, typename Capture = NoCapture>
 __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft, const Apply &apply, int ctr, unsigned long long key,
-		uint32_t pos, unsigned long long k, unsigned long long inc, unsigned long long pol_last)
+		uint32_t pos, unsigned long long k, unsigned long long inc, unsigned long long pol_last, const Capture &cap = Capture {},
+		unsigned long long fk = 0)
 {
 	if (key) {
 		for (uint32_t p = 0; ; ) {
-			if (k == 0) k = atomicCAS(&ft.ent[pos].key, 0ull, key);
+			if (k == 0) {
+				k = atomicCAS(&ft.ent[pos].key, 0ull, key);
+				if (k == 0) cap.claim(pos, fk);
+			}
 			if (k == 0 || k == key) { red_add_u64_hint(&ft.ent[pos].inc, inc, pol_last); return; }
 			if (++p == FLOW_PROBES) break;
 			pos = (pos + 1) & ft.mask;
@@ -347,6 +377,7 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 	const uint32_t am = __activemask();
 	if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(st.counters + ctr, (unsigned long long)__popc(am));
 	apply(key, inc);
+	cap.direct(fk);
 }
 
 // m queued connection records (all 32 lanes call): two lookup2 hashes per flow key -> the flow's entry in the batch's flow table (the
@@ -359,18 +390,21 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // entry of the query flow table fq (cells fq_cms past the probe limit) and touches neither the HLL nor a service cell.
 // RH (GYSK_FLAG_FLOW_RESP_HIST, only with QRY): such a record also adds its word increment to the entry of its resp_hist_key in the
 // response flow table fr (cells fr_cms past the probe limit).
-template <bool QRY, bool RH, typename HotTable>
+// TOPK (GYSK_FLAG_FLOW_TOPK): the record that claims an entry of the connection or query flow table stores its flow key beside the entry,
+// and a record on the direct path appends it to the table's candidates (tk).
+template <bool QRY, bool RH, bool TOPK, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
 		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr,
-		unsigned long long *fr_cms)
+		unsigned long long *fr_cms, const FlowTopk &tk)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
 		bool qry = false;
 		uint32_t cell = 0, idx = 0, rank = 0, hw = 0, pos = 0, rpos = 0; int kb = 0;
-		unsigned long long key = 0, inc = 0, k = 0, rkey = 0, rk = 0, rinc = 0;
+		unsigned long long key = 0, inc = 0, k = 0, rkey = 0, rk = 0, rinc = 0, fk = 0;
 		if (act) {
 			const IngestRec r = ld_rec(q + i);
+			fk = r.flow_key;
 			qry = QRY && r.slot == QRY_REC;
 			FlowEnt *const tent = qry ? fq.ent : ft.ent;		// field by field: a selected reference would copy both tables to the stack
 			const uint32_t tmask = qry ? fq.mask : ft.mask;
@@ -399,7 +433,11 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 		}
 		cell_add(st, hot, act && !qry, cell, kb);
 		if (act) {
-			if (qry) flow_add(st, fq, CmsApply {st, fq_cms}, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
+			if (TOPK) {
+				if (qry) flow_add(st, fq, CmsApply {st, fq_cms}, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last, TopkCapture {tk.list[1]}, fk);
+				else flow_add(st, ft, CmsApply {st, st.cms_cur}, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last, TopkCapture {tk.list[0]}, fk);
+			}
+			else if (qry) flow_add(st, fq, CmsApply {st, fq_cms}, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
 			else flow_add(st, ft, CmsApply {st, st.cms_cur}, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last);
 			if (RH && qry) flow_add(st, fr, RespHistApply {st, fr_cms}, CTR_FLOWR_DIRECT, rkey, rpos, rk, rinc, pol_last);
 		}
@@ -511,9 +549,11 @@ struct IngestShared
 // TRACE: the engine has trace rows (a separate instance, so that an engine without them runs the kernel without the trace path).
 // QRY: GYSK_FLAG_FLOW_QUERIES (a separate instance too): every response sample that reaches its service's histogram, by the key or the
 // hot-row route, also joins the connection queue as a record {QRY_REC, usec, flow key} for the TCP drain pass.
-template <bool TRACE, bool QRY>
+// TOPK: GYSK_FLAG_FLOW_TOPK (a separate instance too): the flow key of each ACTIVE record, which updates the count-min here, joins the
+// connection table's candidates tl.
+template <bool TRACE, bool QRY, bool TOPK>
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
-		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt)
+		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, TopkList tl)
 {
 	constexpr int WARPS = IngestShape::WARPS, EPT = IngestShape::EPT, CHUNK = IngestShape::CHUNK, DH = IngestShared::DH;
 	extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -699,6 +739,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					uint32_t h1, h2, idx, rank;
 					flow_hashes(fk, h1, h2);
 					cms_add(st, st.cms_cur, h1, h2, inc);
+					if (TOPK) topk_append(tl, fk);
 					hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
 					hll_update(st.hll + ((size_t)slot << st.hll_p), idx, rank);
 					red_add_u64(&st.slot_aux[slot].act_cur, inc);
@@ -776,9 +817,9 @@ template <> struct DrainShape<true> { static constexpr int WARPS = 16, HOT_BITS 
 // key holds what picks them), then the entry emptied for the next batch. The TCP pass left the table's lines evict_last, a
 // priority they keep after it ends: back to normal, so that they do not hold L2 against the next batch's ingest_kernel and chain. A
 // thread takes FLOW_SWEEP entries a step, one grid stride apart, their loads in flight together (the REDs' memory clobber keeps a load
-// from moving past them).
-template <typename Apply>
-__device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &apply)
+// from moving past them). cap records the flow key stored beside each entry the sweep applies (GYSK_FLAG_FLOW_TOPK).
+template <typename Apply, typename Capture = NoCapture>
+__device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &apply, const Capture &cap = Capture {})
 {
 	const uint32_t stride = gridDim.x * blockDim.x;
 	for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 <= t.mask; i0 += FLOW_SWEEP * stride) {
@@ -790,6 +831,7 @@ __device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &appl
 			const uint32_t i = i0 + u * stride;
 			if (f[u].key) {
 				apply(f[u].key, f[u].inc);
+				cap.swept(i);
 				t.ent[i] = FlowEnt {0ull, 0ull};
 			}
 			if (i <= t.mask && !(i & 7u)) l2_evict_normal_line(t.ent + i);
@@ -803,13 +845,20 @@ __device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &appl
 // QRY (GYSK_FLAG_FLOW_QUERIES): the TCP pass also sums the queued response samples in the query flow table fq, and the TASK pass applies
 // that table to the query cells fq_cms after the connection flow table.
 // RH (GYSK_FLAG_FLOW_RESP_HIST, only with QRY): the same once more with the response flow table fr and the response histogram cells fr_cms.
-template <bool TASK, bool QRY, bool RH>
+// TOPK (GYSK_FLAG_FLOW_TOPK): the TCP pass keeps the flow keys of the connection and query records (drain_tcp_recs), and the TASK pass's
+// sweeps append the key beside each applied entry to that table's candidates tk.
+template <bool TASK, bool QRY, bool RH, bool TOPK>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms)
+		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
-	if (TASK) {
+	if (TASK && TOPK) {
+		flow_sweep(ft, CmsApply {st, st.cms_cur}, TopkCapture {tk.list[0]});
+		if (QRY) flow_sweep(fq, CmsApply {st, fq_cms}, TopkCapture {tk.list[1]});
+		if (RH) flow_sweep(fr, RespHistApply {st, fr_cms});
+	}
+	else if (TASK) {
 		flow_sweep(ft, CmsApply {st, st.cms_cur});
 		if (QRY) flow_sweep(fq, CmsApply {st, fq_cms});
 		if (RH) flow_sweep(fr, RespHistApply {st, fr_cms});
@@ -879,7 +928,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs<QRY, RH>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms);
+			drain_tcp_recs<QRY, RH, TOPK>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms, tk);
 		}
 	}
 
@@ -2184,19 +2233,26 @@ __global__ void gather_hll_kernel(DevState st, const unsigned long long *__restr
 	for (uint32_t i = threadIdx.x; i < (1u << st.hll_p); i += blockDim.x) out[i] = regs[i];
 }
 
+// the point estimate of a flow key on a count-min of one u64 per cell: the minimum over rows of each half
+__device__ __forceinline__ void cms_point(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, unsigned long long key,
+		uint32_t &lo, uint32_t &hi)
+{
+	lo = 0xFFFFFFFFu; hi = 0xFFFFFFFFu;
+	for (uint32_t r = 0; r < depth; ++r) {
+		const unsigned long long c = tbl[((size_t)r << log2w) + cms_index(key, r, (1u << log2w) - 1)];
+		lo = min(lo, (uint32_t)c);
+		hi = min(hi, (uint32_t)(c >> 32));
+	}
+}
+
 __global__ void query_flows_kernel(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, const unsigned long long *__restrict__ keys,
 		uint32_t n, gysk_flow_est *__restrict__ out)
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
 	const unsigned long long key = keys[i];
-	uint32_t cnt = 0xFFFFFFFFu, kb = 0xFFFFFFFFu;
-
-	for (uint32_t r = 0; r < depth; ++r) {
-		const unsigned long long c = tbl[((size_t)r << log2w) + cms_index(key, r, (1u << log2w) - 1)];
-		cnt = min(cnt, (uint32_t)c);
-		kb = min(kb, (uint32_t)(c >> 32));
-	}
+	uint32_t cnt, kb;
+	cms_point(tbl, depth, log2w, key, cnt, kb);
 	out[i].flow_key = key; out[i].count = cnt; out[i].kbytes = kb;
 }
 
@@ -2315,8 +2371,8 @@ static int plain_sort_plan(int lo, int hi, SortPlan &P)
 	return 0;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
-		RecRegions &rr, cudaStream_t s)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const gysk_event *d_ev, uint64_t n,
+		uint32_t key_slots, RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
 	const int dev = current_device();
@@ -2329,12 +2385,24 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	cudaMemsetAsync(tmp.os_ghist, 0, OS_GHIST_WORDS * sizeof(uint32_t), s);
 	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
 	static bool attr_set[MAX_DEVICES] = {};
+	using IngestFn = void (*)(DevState, const gysk_event *, uint64_t, unsigned long long *, uint32_t *, SortPlan, uint4 *, uint2 *, TopkList);
+	// [TRACE][QRY][TOPK]
+	static const IngestFn fns[2][2][2] = {
+		{{ingest_kernel<false, false, false>, ingest_kernel<false, false, true>}, {ingest_kernel<false, true, false>, ingest_kernel<false, true, true>}},
+		{{ingest_kernel<true, false, false>, ingest_kernel<true, false, true>}, {ingest_kernel<true, true, false>, ingest_kernel<true, true, true>}}};
+	// the instances of GYSK_FLAG_FLOW_TOPK only once an engine with it launches: setting a kernel's attribute loads it, which can wait for
+	// the work already on the device
+	static bool topk_attr_set[MAX_DEVICES] = {};
+	const int topk = tk.list[0].keys ? 1 : 0;
 	if (!attr_set[dev]) {
-		cudaFuncSetAttribute(ingest_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		cudaFuncSetAttribute(ingest_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		cudaFuncSetAttribute(ingest_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		cudaFuncSetAttribute(ingest_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		for (const IngestFn f : {fns[0][0][0], fns[1][0][0], fns[0][1][0], fns[1][1][0]})
+			cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
 		attr_set[dev] = true;
+	}
+	if (topk && !topk_attr_set[dev]) {
+		for (const IngestFn f : {fns[0][0][1], fns[1][0][1], fns[0][1][1], fns[1][1][1]})
+			cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		topk_attr_set[dev] = true;
 	}
 	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
 	const uint64_t full = (uint64_t)sm_count(dev) * IngestShape::MIN_CTAS;
@@ -2345,39 +2413,46 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
 	// a counted response sample takes a connection-queue entry, as one connection event does: the regions hold one record per event
-	auto k = st.trace.rows ? (fq.cur ? ingest_kernel<true, true> : ingest_kernel<true, false>) : (fq.cur ? ingest_kernel<false, true> : ingest_kernel<false, false>);
-	k<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt);
+	const IngestFn k = fns[st.trace.rows ? 1 : 0][fq.cur ? 1 : 0][topk];
+	k<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, tk.list[0]);
 	return 1;
 }
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
-template <bool TASK, bool QRY, bool RH>
+template <bool TASK, bool QRY, bool RH, bool TOPK>
 static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, cudaStream_t s)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
 		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH>, WARPS * 32, smem_max);
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK>, WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY, RH><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq, fq_cms, fr, fr_cms);
+	drain_kernel<TASK, QRY, RH, TOPK><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq, fq_cms,
+			fr, fr_cms, tk);
 }
 
 template <bool QRY, bool RH>
 static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, cudaStream_t s)
 {
-	launch_drain_pass<false, QRY, RH>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, s);
-	launch_drain_pass<true, QRY, RH>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, s);
+	if (tk.list[0].keys) {
+		launch_drain_pass<false, QRY, RH, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
+		launch_drain_pass<true, QRY, RH, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
+	}
+	else {
+		launch_drain_pass<false, QRY, RH, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
+		launch_drain_pass<true, QRY, RH, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
+	}
 	return 2;
 }
 
@@ -2386,8 +2461,8 @@ static int launch_drain_passes(const DevState &st, const FlowTable &ft, const So
 // batch's events (the flows are fewer than the connection records), up to what tmp holds, so that a small batch sweeps a small table.
 // With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size, and
 // with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too.
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const RecRegions &rr, uint64_t n_events,
-		cudaStream_t s)
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, const RecRegions &rr,
+		uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
@@ -2396,12 +2471,12 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable none {nullptr, 0u};
-	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, s);
+	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable fqt {fq.flow, n - 1u};
-	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, s);
+	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
-	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, s);
+	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, s);
 }
 
 static void os_set_attrs(int dev)
@@ -2591,6 +2666,87 @@ int launch_topn(const DevState &st, const SortTemp &tmp, uint32_t nslots, int is
 	const int picked = launch_topn_pick(tmp, d_n, nslots, is_task ? st.task_slot_id : st.slot_id, is_task ? st.task_slot_host : st.slot_host,
 			want, d_out, s, d_slots);
 	return picked < 0 ? picked : 1 + picked;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// GYSK_FLAG_FLOW_TOPK: the heaviest-flow set of one table after a batch (or the merge's union): the candidates sorted by key, each
+// distinct one scored, the rank keys sorted by score, the K best read from the end
+// ---------------------------------------------------------------------------------------------------
+// The rank key of candidate i of the *d_n sorted keys: a distinct key (not equal to its predecessor) is {score : 32 | 1 : 1 | i : 31},
+// a repeat only i, below every distinct key. It goes to position n - 1 - i, so the stable sort by bits [31, 64) leaves a larger key
+// before a smaller one of equal score, and the read from the end takes the smaller key first.
+__global__ void __launch_bounds__(256) topk_score_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *__restrict__ d_n,
+		const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, int half, unsigned long long *__restrict__ rank)
+{
+	const uint64_t n = *d_n;
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+		const unsigned long long k = keys[i];
+		unsigned long long r = i;
+		if (i == 0 || keys[i - 1] != k) {
+			uint32_t lo, hi;
+			cms_point(tbl, depth, log2w, k, lo, hi);
+			r |= ((unsigned long long)(half ? hi : lo) << 32) | (1ull << 31);
+		}
+		rank[n - 1 - i] = r;
+	}
+}
+
+// the K best of the sorted rank keys into set (word 0 its size, then the keys, 0 past the size): the distinct keys are a suffix
+__global__ void __launch_bounds__(256) topk_pick_kernel(const unsigned long long *__restrict__ rank, const unsigned long long *__restrict__ d_n,
+		const unsigned long long *__restrict__ keys, unsigned long long *__restrict__ set)
+{
+	const uint64_t n = *d_n;
+	const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+	if (j >= TOPK_K) return;
+	auto valid = [&](uint64_t q) { return q < n && ((rank[n - 1 - q] >> 31) & 1ull); };
+	const bool v = valid(j);
+	set[2 + j] = v ? keys[rank[n - 1 - j] & 0x7FFFFFFFull] : 0ull;
+	if (v && (j + 1 == TOPK_K || !valid(j + 1))) set[0] = j + 1;
+	if (j == 0) { if (!v) set[0] = 0; set[1] = 0; }
+}
+
+int launch_topk_select(const SortTemp &tmp, const TopkList &l, uint64_t n_max, const unsigned long long *tbl, uint32_t depth, uint32_t log2w,
+		int half, unsigned long long *set, bool reseed, cudaStream_t s)
+{
+	// three buffers of at least n_max keys: the candidates, and tmp's two; the key sort ping-pongs between the first two, the rank sort
+	// between the two the sorted keys leave free
+	unsigned long long *buf[3] = {l.keys, tmp.keys_a, tmp.keys_b};
+	SortTemp t = tmp;
+	t.keys_a = buf[0]; t.keys_b = buf[1];
+	int which = 0;
+	const int n1 = launch_radix_sort(t, l.n, n_max, 0, 64, &which, s);
+	if (n1 < 0) return -1;
+	const unsigned long long *sorted = buf[which];
+	t.keys_a = buf[which ^ 1]; t.keys_b = buf[2];
+	const uint32_t grid = std::min<uint32_t>(div_up(n_max, 256), (uint32_t)sm_count(current_device()) * 8u);
+	topk_score_kernel<<<grid ? grid : 1, 256, 0, s>>>(sorted, l.n, tbl, depth, log2w, half, t.keys_a);
+	const unsigned long long *ranked[2] = {t.keys_a, t.keys_b};
+	const int n2 = launch_radix_sort(t, l.n, n_max, 31, 64, &which, s);
+	if (n2 < 0) return -1;
+	topk_pick_kernel<<<div_up(TOPK_K, 256), 256, 0, s>>>(ranked[which], l.n, sorted, set);
+	if (reseed) {		// the set opens the next batch's candidates
+		cudaMemcpyAsync(l.keys, set + 2, (size_t)TOPK_K * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s);
+		cudaMemcpyAsync(l.n, set, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s);
+	}
+	return n1 + n2 + 2;
+}
+
+// one CTA per rank: the size-word-counted keys of its set appended to l
+__global__ void __launch_bounds__(256) topk_gather_kernel(const unsigned long long *__restrict__ sets, size_t stride, TopkList l)
+{
+	const unsigned long long *set = sets + blockIdx.x * stride;
+	const uint32_t m = (uint32_t)min(set[0], (unsigned long long)TOPK_K);
+	__shared__ unsigned long long base;
+	if (threadIdx.x == 0) base = atomicAdd(l.n, (unsigned long long)m);
+	__syncthreads();
+	for (uint32_t j = threadIdx.x; j < m; j += blockDim.x) l.keys[base + j] = set[2 + j];
+}
+
+int launch_topk_gather(const unsigned long long *sets, uint32_t world, size_t stride, const TopkList &l, cudaStream_t s)
+{
+	cudaMemsetAsync(l.n, 0, sizeof(unsigned long long), s);
+	topk_gather_kernel<<<world, 256, 0, s>>>(sets, stride, l);
+	return 1;
 }
 
 // per-task window of the three MTASK_HIST histograms: totals now minus totals at the previous flush (nothing on the ingest path).

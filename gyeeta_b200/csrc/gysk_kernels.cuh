@@ -169,6 +169,17 @@ struct FlowRespHist { unsigned long long *cur, *last; FlowEnt *flow; unsigned lo
 static constexpr uint32_t RESP_HIST_WORDS = 8;
 static constexpr uint32_t CMS_LOG2W_MAX = 28;		// the widest count-min gysk_create accepts (1 << 28 columns)
 
+// GYSK_FLAG_FLOW_TOPK: the candidates of one windowed table's heaviest-flow set in a batch. keys [0, *n) hold the open set (written at the
+// end of the previous batch's selection, emptied by gysk_flush), then every flow key the batch brings: ingest_kernel appends each
+// NOTIFY_ACTIVE_CONN_STATS record's (connection table), the TCP pass each record's that takes the direct path of flow_add, and the TASK
+// pass, sweeping the batch flow table, the key its claimer stored in ekeys beside the entry. cap = K + max_batch: a record appends at most
+// once, directly or by claiming an entry. Every pointer nullptr: not held.
+struct TopkList { unsigned long long *keys, *n, *ekeys; unsigned long long cap; };
+// a heaviest-flow set: [TOPK_SET_WORDS] u64, word 0 its size, word 1 zero, then the K keys best first
+static constexpr uint32_t TOPK_K = GYSK_FLOW_TOPK_CAP, TOPK_SET_WORDS = TOPK_K + 2;
+// the held lists: [0] the connection table's, [1] the flow query table's
+struct FlowTopk { TopkList list[2]; };
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
@@ -248,12 +259,22 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 // -1: no sort plan for max_svcs, or the launch's record regions do not fit the buffers
 // key_slots: the values the slot field of a sort key takes (max_svcs, or max_svcs + 1 + trace rows with trace rows)
 // fq.cur != nullptr: the response samples are queued for the flow query table too (GYSK_FLAG_FLOW_QUERIES)
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
-		RecRegions &rr, cudaStream_t s);
+// tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the flow keys of the ACTIVE records join the connection table's candidates
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const gysk_event *d_ev, uint64_t n,
+		uint32_t key_slots, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
-// fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const RecRegions &rr, uint64_t n_events,
-		cudaStream_t s);
+// fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms;
+// tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the passes gather each held table's candidates
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, const RecRegions &rr,
+		uint64_t n_events, cudaStream_t s);
+// GYSK_FLAG_FLOW_TOPK, after the batch merge (it takes tmp's sort buffers, of at least n_max keys): the *l.n candidates (n_max >= *l.n)
+// sorted by key in l.keys, the distinct ones scored on table tbl (half = 0: the low half, 1: the high half of a cell, the estimate of
+// query_flows_kernel) and the K best by (score descending, key ascending) written to set; then, unless reseed is false, set back into
+// l as the next batch's first candidates. -1: no sort plan
+int launch_topk_select(const SortTemp &tmp, const TopkList &l, uint64_t n_max, const unsigned long long *tbl, uint32_t depth, uint32_t log2w,
+		int half, unsigned long long *set, bool reseed, cudaStream_t s);
+// the merge's union into l (its count reset first): the keys of world sets, rank r's at sets + r * stride words
+int launch_topk_gather(const unsigned long long *sets, uint32_t world, size_t stride, const TopkList &l, cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
 // bits outside [0, 64)), or n_max >= 2^30
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);

@@ -879,6 +879,7 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// (re)allocate the arena
 	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
 	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel); dfree(e, mg.topn_slots); dfree(e, mg.topn_final); dfree(e, mg.lg.trace_final);
+	dfree(e, mg.topk_final); dfree(e, mg.topk_buf); dfree(e, mg.topk_n); dfree(e, mg.topk_tiles);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
@@ -897,9 +898,16 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// GYSK_FLAG_MERGE_TOPN: the candidates after the digests, in whole SlabEntrys, so the slab stays one all-gather; GYSK_FLAG_MERGE_TRACES:
 	// the trace digests after them, packed as TraceSlabs in whole SlabEntrys
 	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
+	// GYSK_FLAG_FLOW_TOPK: the rank's last-window heaviest-flow sets after everything else
+	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK;
 	mg.trace_off = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
-	mg.slab_entries = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
+	mg.topk_off = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
+	mg.slab_entries = mg.topk_off + (topk ? TOPK_SLAB_ENTRIES : 0);
 	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
+	if (topk) {
+		if ((rc = dalloc(e, &mg.topk_final, 2 * (size_t)TOPK_SET_WORDS))) return rc;
+		if ((rc = dalloc(e, &mg.topk_n, 1))) return rc;
+	}
 	if (topn) {
 		if ((rc = dalloc(e, &mg.topn_slots, (size_t)TOPN_LISTS * TOPN_K))) return rc;
 		if ((rc = dalloc(e, &mg.topn_final, TopnLists::BYTES))) return rc;
@@ -993,8 +1001,8 @@ int gysk_merge_prepare(gysk_engine *e)
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Submit);
 	MergeState &mg = e->mg;
-	// GYSK_FLAG_MERGE_TOPN needs no map: without one, an empty logical map (as gysk_set_cluster_map sets up)
-	if (!mg.arena && (e->cfg.flags & GYSK_FLAG_MERGE_TOPN)) {
+	// GYSK_FLAG_MERGE_TOPN and GYSK_FLAG_FLOW_TOPK need no map: without one, an empty logical map (as gysk_set_cluster_map sets up)
+	if (!mg.arena && (e->cfg.flags & (GYSK_FLAG_MERGE_TOPN | GYSK_FLAG_FLOW_TOPK))) {
 		if (int rc = set_logical_map(e, nullptr, nullptr, 0)) return rc;
 	}
 	if (!mg.arena) return fail(e, GYSK_ERR_INVAL, "gysk_merge_prepare: call gysk_set_logical_map first");
@@ -1051,6 +1059,14 @@ int gysk_merge_prepare(gysk_engine *e)
 		e->kernel_launches += launch_task_summaries(e->st, nullptr, mg.topn_slots + (size_t)TOPN_SVC_LISTS * TOPN_K, (TOPN_LISTS - TOPN_SVC_LISTS) * TOPN_K,
 				reinterpret_cast<gysk_task_summary *>(cand.row(TOPN_SVC_LISTS, 0)), e->stream);
 	}
+	if (mg.topk_final) {		// GYSK_FLAG_FLOW_TOPK: the last-window sets (a set the engine does not hold: empty)
+		unsigned long long *dst = reinterpret_cast<unsigned long long *>(mg.lg.slab + mg.topk_off);
+		for (int w = 0; w < 2; ++w) {
+			unsigned long long *d = dst + (size_t)w * TOPK_SET_WORDS;
+			if (e->topk.last[w]) CU(e, cudaMemcpyAsync(d, e->topk.last[w], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
+			else CU(e, cudaMemsetAsync(d, 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
+		}
+	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
 	return post_launch(e, "merge_prepare");
@@ -1098,6 +1114,33 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 	if (mg.topn_final) {		// GYSK_FLAG_MERGE_TOPN
 		topn_global_kernel<<<TOPN_LISTS, 256, 0, e->stream>>>(src, world, mg.slab_entries, mg.lg.nl, TopnLists {mg.topn_final});
 		e->kernel_launches++;
+	}
+	if (mg.topk_final) {		// GYSK_FLAG_FLOW_TOPK: per held set the union of every rank's, scored on the summed last-window table
+		const uint64_t need = (uint64_t)world * TOPK_K;
+		if (need > mg.topk_cap) {
+			dfree(e, mg.topk_buf); dfree(e, mg.topk_tiles);
+			mg.topk_cap = 0;
+			if (int rc = dalloc(e, &mg.topk_buf, 3 * (size_t)need, false)) return rc;
+			if (int rc = dalloc(e, &mg.topk_tiles, (size_t)RADIX_MAX * ((need + SORT_TILE - 1) / SORT_TILE))) return rc;
+			mg.topk_cap = need;
+		}
+		// the union's own candidates and sort buffers: the engine's stay with its open sets
+		SortTemp t = e->tmp;
+		t.keys_a = mg.topk_buf + mg.topk_cap; t.keys_b = mg.topk_buf + 2 * mg.topk_cap;
+		t.tile_status = mg.topk_tiles; t.max_tiles = (uint32_t)((mg.topk_cap + SORT_TILE - 1) / SORT_TILE);
+		const TopkList l {mg.topk_buf, mg.topk_n, nullptr, mg.topk_cap};
+		const size_t stride = (size_t)mg.slab_entries * sizeof(SlabEntry) / sizeof(unsigned long long);
+		for (int w = 0; w < 2; ++w) {
+			unsigned long long *set = mg.topk_final + (size_t)w * TOPK_SET_WORDS;
+			if (!e->topk.last[w]) continue;
+			e->kernel_launches += launch_topk_gather(reinterpret_cast<const unsigned long long *>(src + mg.topk_off) + (size_t)w * TOPK_SET_WORDS, world,
+					stride, l, e->stream);
+			const int k = launch_topk_select(t, l, need, mg.g_cms[TOPK_TABLE[w] + 1], e->cfg.cms_depth, e->cfg.cms_log2_width, TOPK_HALF[w], set, false,
+					e->stream);
+			if (k < 0) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: heaviest-flow sort failed");
+			e->kernel_launches += k;
+		}
+		mg.topk_done = true;
 	}
 	mg.finished = true;			// stream-ordered; the query calls synchronise
 	return post_launch(e, "merge_finish");
@@ -1391,6 +1434,17 @@ int gysk_merge_global(gysk_engine *e, void *comm)
 }
 
 // GYSK_FLAG_MERGE_TOPN: the winners of the last finished merge (topn_global_kernel)
+// GYSK_FLAG_FLOW_TOPK: the heaviest flows of the last finished merge
+int gysk_topk_flows_global(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout)
+{
+	return topk_read(e, 0, 1, true, n, out, nout, "topk_flows_global");
+}
+
+int gysk_topk_flow_queries_global(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout)
+{
+	return topk_read(e, 1, 1, true, n, reinterpret_cast<gysk_flow_est *>(out), nout, "topk_flow_queries_global");
+}
+
 int gysk_topn_global(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, gysk_svc_summary *rows, uint32_t *nout)
 {
 	return topn_global_rows(e, metric, n, out, rows, nout, "topn_global");

@@ -41,6 +41,8 @@ FLAG_MERGE_TRACES = 64
 FLAG_FLOW_QUERIES = 128
 FLAG_FLOW_QUERY_LEVEL = 0x100
 FLAG_FLOW_RESP_HIST = 0x200
+FLAG_FLOW_TOPK = 0x400
+FLOW_TOPK_CAP = 4096
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
 
@@ -325,6 +327,10 @@ def load_library(path=None):
         "gysk_export_cms_resp_5min": (i32, [vp, vp]),
         "gysk_query_flow_resp_global_5min": (i32, [vp, vp, u32, vp]),
         "gysk_last_batch_flow_resp_direct": (C.c_int64, [vp]),
+        "gysk_topk_flows": (i32, [vp, i32, u32, vp, vp]),
+        "gysk_topk_flow_queries": (i32, [vp, i32, u32, vp, vp]),
+        "gysk_topk_flows_global": (i32, [vp, u32, vp, vp]),
+        "gysk_topk_flow_queries_global": (i32, [vp, u32, vp, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -390,7 +396,8 @@ class Engine:
     def __init__(self, device=0, max_svcs=1 << 14, max_tasks=1 << 12, cms_depth=4, cms_log2_width=20, hll_p=12,
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
-                 max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False):
+                 max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False,
+                 flow_topk=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -405,7 +412,7 @@ class Engine:
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
                     (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
-                    (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0)
+                    (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -712,6 +719,29 @@ class Engine:
     def query_flow_queries_5min(self, keys):
         """gysk_query_flow_queries_5min: the point query on the rolling 300-s flow query level (flow_query_level=True)"""
         return self._point_query(self.L.gysk_query_flow_queries_5min, FLOW_QRY_EST_DTYPE, keys)
+
+    def _topk(self, fn, dtype, n, *window):
+        """a heaviest-flow read fn(h, [last_window,] n, out, nout): the rows, best first"""
+        out = np.zeros(n, dtype=dtype)
+        k = C.c_uint32()
+        self._chk(fn(self.h, *window, n, _p(out), C.byref(k)))
+        return out[: k.value]
+
+    def topk_flows(self, n=FLOW_TOPK_CAP, last_window=False):
+        """gysk_topk_flows: the n heaviest flows by kbytes of the open or last window, with their estimates (flow_topk=True)"""
+        return self._topk(self.L.gysk_topk_flows, FLOW_EST_DTYPE, n, int(last_window))
+
+    def topk_flow_queries(self, n=FLOW_TOPK_CAP, last_window=False):
+        """gysk_topk_flow_queries: the n heaviest flows by queries of the open or last window (flow_topk=True, flow_queries=True)"""
+        return self._topk(self.L.gysk_topk_flow_queries, FLOW_QRY_EST_DTYPE, n, int(last_window))
+
+    def topk_flows_global(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flows_global: the n heaviest flows by kbytes over every rank, from the last finished merge (flow_topk=True)"""
+        return self._topk(self.L.gysk_topk_flows_global, FLOW_EST_DTYPE, n)
+
+    def topk_flow_queries_global(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_queries_global: the n heaviest flows by queries over every rank, from the last finished merge"""
+        return self._topk(self.L.gysk_topk_flow_queries_global, FLOW_QRY_EST_DTYPE, n)
 
     def topn(self, metric, n=10, host_idx=-1):
         out = (TopnEntry * n)()

@@ -250,6 +250,12 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   batch table, so 10 M samples a batch update the cells directly), gysk_flush 0.51 -> 0.63
 						   ms (1.92 ms with the level), gysk_merge_prepare +0.41 ms (+0.56 ms with the level). Without it nothing is allocated, every other
 						   call answers as before and the flow response calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_FLOW_TOPK		0x400u	/* the GYSK_FLOW_TOPK_CAP heaviest client flows of each window beside the connection
+						   count-min (by kbytes) and, with GYSK_FLAG_FLOW_QUERIES, the flow query tables (by
+						   queries), ranked on each rank and across ranks (gysk_topk_flows, "heaviest flows"
+						   below). Needs no other flag. Without it nothing is allocated, every other call answers
+						   as before and the four calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLOW_TOPK_CAP		4096u	/* K: the flows each heaviest-flow set holds (fixed: gysk_config has no word for it) */
 
 typedef struct gysk_config
 {
@@ -726,6 +732,35 @@ int		gysk_query_flow_resp_global(gysk_engine *e, const uint64_t *flow_keys, uint
 int		gysk_query_flow_resp_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_resp_est *out);
 int		gysk_export_cms_resp_5min(gysk_engine *e, uint64_t *words /* (depth << log2_width) x 8 entries */);
 int		gysk_query_flow_resp_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_resp_est *out);
+
+/* ---- heaviest flows (GYSK_FLAG_FLOW_TOPK): which clients to ask the flow tables about ----
+ * Every flow table answers a point query on a key the caller already has; these sets name the keys. There is one set per held windowed
+ * table: the connection count-min, scored by the kbytes half, and with GYSK_FLAG_FLOW_QUERIES the flow query table, scored by the queries
+ * half. A flow's score is the point estimate of that half: the minimum over rows, what gysk_query_flows / gysk_query_flow_queries return.
+ * The rule, after each device batch, once all of the batch's increments are in the open table: let B be the distinct flow keys whose
+ * records reached that table in the batch (connection records of services that hold a slot, from every route including
+ * NOTIFY_ACTIVE_CONN_STATS; counted response samples for the query table; dropped events, unknown ids and GYSK_EV_TRACE events never
+ * enter B). The open set C becomes the K = GYSK_FLOW_TOPK_CAP best of C u B by (score descending, flow key ascending), scored on the
+ * table as it is after the batch. gysk_flush moves the open set to the last window's set and starts the open set empty, as it swaps the
+ * tables. Two keys whose two lookup2 hashes both agree are one flow to every count-min: the set may name either.
+ * Guarantee: if no cell half wraps during the window, every flow whose exact score in the window exceeds the smallest score of a full set
+ * (K members) is in that set; a window of at most K flows has every one of them in its set. (Scores never fall within a window, so the
+ * K-th score of the set never falls; a flow that leaves the set, or is never admitted, scores at most the K-th at that batch, and its
+ * exact score is at most its estimate.)
+ * Across ranks: gysk_merge_prepare carries each rank's last-window sets in the t-digest slab (no logical map needed); gysk_merge_finish
+ * scores the union U of every rank's sets on the summed last-window tables and keeps the K best by the same order. A flow whose exact
+ * global score exceeds sum over ranks of thr_r is in U (thr_r: the smallest score of rank r's set when it is full, else 0).
+ * Cost: per held table a candidate list of K + max_batch flow keys and a key per batch flow-table entry (8 B each); each batch sorts its
+ * candidates by key, scores the distinct ones and sorts them by score. DESIGN.md section 7 has the measured times.
+ * gysk_topk_flows: the first min(n, K) of the open (last_window = 0) or last set, best first, with their current estimates; entries with
+ *   a zero score are left out, so *nout may be below n. gysk_topk_flow_queries: the same for the query table (GYSK_ERR_NOTSUP without
+ *   GYSK_FLAG_FLOW_QUERIES). The _global pair: the merged lists of the last gysk_merge_finish, with their estimates on the summed tables
+ *   (GYSK_ERR_INVAL before the first one). Every call is GYSK_ERR_NOTSUP without the flag.
+ * Not covered: sets for the 300-s levels, a set scored by the response histograms, per-(service, client) pairs, a configurable K. */
+int		gysk_topk_flows(gysk_engine *e, int last_window, uint32_t n, gysk_flow_est *out, uint32_t *nout);
+int		gysk_topk_flow_queries(gysk_engine *e, int last_window, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout);
+int		gysk_topk_flows_global(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout);
+int		gysk_topk_flow_queries_global(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout);
 
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
