@@ -325,21 +325,24 @@ int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t
 	}, CopyRows<gysk_flow_est> {out});
 }
 
-int topk_read(gysk_engine *e, int which, int last_window, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout, const char *what)
+int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout,
+		uint64_t *bound, const char *what)
 {
 	CHECK_ENGINE(e);
 	if (!nout || (!out && n)) return GYSK_ERR_INVAL;
-	if (!e->topk.open[which]) return GYSK_ERR_NOTSUP;
+	if (!(level ? e->topk5.level[which] : e->topk.open[which])) return GYSK_ERR_NOTSUP;
 	Entry entry(e, merged ? Pending::Drain : Pending::Submit);
 	if (entry.rc) return entry.rc;
 	if (merged && !e->mg.topk_done) return fail(e, GYSK_ERR_INVAL, ("gysk_" + std::string(what) + ": no finished merge").c_str());
-	const unsigned long long *set = merged ? e->mg.topk_final + (size_t)which * TOPK_SET_WORDS : last_window ? e->topk.last[which] : e->topk.open[which];
+	const size_t off = (size_t)which * TOPK_SET_WORDS;
+	const unsigned long long *set = level ? (merged ? e->mg.topk5_final + off : e->topk5.level[which])
+					      : merged ? e->mg.topk_final + off : last_window ? e->topk.last[which] : e->topk.open[which];
 	std::vector<uint64_t> keys(TOPK_SET_WORDS);
 	CU(e, cudaMemcpyAsync(keys.data(), set, sizeof(uint64_t) * TOPK_SET_WORDS, cudaMemcpyDeviceToHost, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
 	const uint32_t m = (uint32_t)std::min<uint64_t>({keys[0], (uint64_t)n, (uint64_t)TOPK_K});
-	const int t = TOPK_TABLE[which] + 1;		// the table of the last window (merged: the summed one)
-	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[last_window ? t : t - 1].live(e);
+	const int t = level ? TOPK5_LEVEL[which] : TOPK_TABLE[which] + (merged || last_window ? 1 : 0);	// merged: the summed table
+	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[t].live(e);
 	std::vector<gysk_flow_est> rows(m);
 	int rc = staged_read(e, keys.data() + 2, m, QCHUNK, sizeof(gysk_flow_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t k) {
 		return launch_query_flows(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, k, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
@@ -348,6 +351,7 @@ int topk_read(gysk_engine *e, int which, int last_window, bool merged, uint32_t 
 	uint32_t k = 0;
 	for (const gysk_flow_est &r : rows) if (TOPK_HALF[which] ? r.kbytes : r.count) out[k++] = r;
 	*nout = k;
+	if (bound) *bound = keys[1];
 	return GYSK_OK;
 }
 
@@ -459,6 +463,37 @@ int roll_levels(gysk_engine *e, uint32_t tsec)
 	return 0;
 }
 
+// GYSK_FLAG_FLOW_TOPK_5MIN at the flush of level w (CMS_RINGS[w], whose open table is TOPK_TABLE[w]), once launch_cms_level_roll has
+// put the closing window into ring slot s = lv.cur[0] and before the window sets swap: the slot fold, then the level set (the rule of
+// gysk_topk_flows_5min). All stream-ordered on the device: the slot and the live mask are roll_levels' own decision. The selections
+// take the batch's sort buffers, as the window sets' do.
+static int topk5_roll(gysk_engine *e, int w)
+{
+	const LevelRing &lv = e->st.levels;
+	const Topk5min &t5 = e->topk5;
+	const CmsRingDesc &r = CMS_RINGS[w];
+	const uint32_t d = e->cfg.cms_depth, lw = e->cfg.cms_log2_width;
+	const int half = TOPK_HALF[w];
+	unsigned long long *slot = t5.slots[w] + (size_t)lv.cur[0] * TOPK_SET_WORDS, *level = t5.level[w];
+	const unsigned long long *win = e->topk.open[w];		// W, still the open window's set
+	const unsigned long long *slot_tbl = r.ring(e) + (size_t)lv.cur[0] * cms_words(e->cfg, r.open), *level_tbl = CMS_TABLES[r.level].live(e);
+	if (lv.fresh & 1u) CU(e, cudaMemsetAsync(slot, 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
+	// 1. B_s + thr(W) aside (the selection writes word 1 of S_s), S_s u W, the K best on the slot, B_s = max(thr(S_s), B_s + thr(W))
+	int k = launch_topk_bound(win, CMS_TABLES[r.open].live(e), d, lw, half, slot + 1, 0, 1, 1u, true, t5.acc, e->stream);
+	k += launch_topk_gather_mask(slot, 0, 1u, t5.list, true, e->stream);
+	k += launch_topk_gather_mask(win, 0, 1u, t5.list, false, e->stream);
+	const int k1 = launch_topk_select(e->tmp, t5.list, 2 * (uint64_t)TOPK_K, slot_tbl, d, lw, half, slot, false, e->stream);
+	if (k1 < 0) return fail(e, GYSK_ERR_INVAL, "flush: 300-s heaviest-flow slot fold: no sort plan");
+	k += k1 + launch_topk_bound(slot, slot_tbl, d, lw, half, t5.acc, 0, 1, 1u, false, slot + 1, e->stream);
+	// 2. the live slots' sets, the K best on the level, B_L = max(thr(L), sum of the live B_s)
+	k += launch_topk_gather_mask(t5.slots[w], TOPK_SET_WORDS, lv.live[0], t5.list, true, e->stream);
+	const int k2 = launch_topk_select(e->tmp, t5.list, (uint64_t)NSLOTS * TOPK_K, level_tbl, d, lw, half, level, false, e->stream);
+	if (k2 < 0) return fail(e, GYSK_ERR_INVAL, "flush: 300-s heaviest-flow level set: no sort plan");
+	k += k2 + launch_topk_bound(level, level_tbl, d, lw, half, t5.slots[w] + 1, TOPK_SET_WORDS, NSLOTS, lv.live[0], false, level + 1, e->stream);
+	e->kernel_launches += k;
+	return 0;
+}
+
 // ---- capacity: the per-slot arrays --------------------------------------------------------------------------------
 //
 // Every device array indexed by service or process slot, with its elements per slot: f(pointer, elements per slot, kind). Svc arrays
@@ -514,7 +549,9 @@ uint32_t table_cap(uint32_t slots) { return pow2_at_least((uint64_t)slots * 2); 
 size_t sort_keys(const gysk_config &cfg)
 {
 	// GYSK_FLAG_FLOW_TOPK: a batch's heaviest-flow candidates are its open set and up to one key per event
-	const size_t batch = (size_t)cfg.max_batch + ((cfg.flags & GYSK_FLAG_FLOW_TOPK) ? TOPK_K : 0);
+	size_t batch = (size_t)cfg.max_batch + ((cfg.flags & GYSK_FLAG_FLOW_TOPK) ? TOPK_K : 0);
+	// GYSK_FLAG_FLOW_TOPK_5MIN: the flush chain's level set takes the live slots' sets, up to NSLOTS x K keys (max_batch may be 1024)
+	if (cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) batch = std::max<size_t>(batch, (size_t)NSLOTS * TOPK_K + TOPK_K);
 	return std::max<size_t>(std::max<size_t>(std::max<size_t>((size_t)cfg.max_svcs + 1, cfg.max_tasks) + 1, batch), (size_t)cfg.max_trace_svcs + 1);
 }
 uint32_t sort_tiles(size_t nkeys) { return (uint32_t)((nkeys + SORT_TILE - 1) / SORT_TILE); }
@@ -618,6 +655,10 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_QUERY_LEVEL needs GYSK_FLAG_FLOW_QUERIES");
 	if ((cfg.flags & GYSK_FLAG_FLOW_RESP_HIST) && !(cfg.flags & GYSK_FLAG_FLOW_QUERIES))
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_RESP_HIST needs GYSK_FLAG_FLOW_QUERIES");
+	if ((cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) && !(cfg.flags & GYSK_FLAG_FLOW_TOPK))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_5MIN needs GYSK_FLAG_FLOW_TOPK");
+	if ((cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) && !(cfg.flags & (GYSK_FLAG_FLOW_LEVEL | GYSK_FLAG_FLOW_QUERY_LEVEL)))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_5MIN needs GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_FLOW_QUERY_LEVEL");
 
 	int ndev = 0;
 	cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -734,6 +775,16 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 			l.cap = (uint64_t)TOPK_K + cfg.max_batch;
 			A(dalloc(e, &l.keys, (size_t)l.cap, false)); A(dalloc(e, &l.n, 1)); A(dalloc(e, &l.ekeys, (size_t)tmp.flow_cap, false));
 			A(dalloc(e, &e->topk.open[w], (size_t)TOPK_SET_WORDS)); A(dalloc(e, &e->topk.last[w], (size_t)TOPK_SET_WORDS));
+		}
+		// GYSK_FLAG_FLOW_TOPK_5MIN: per held level its slot sets and level set, all empty with zero bounds; the flush chain's list
+		if (cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) {
+			Topk5min &t5 = e->topk5;
+			for (int w = 0; w < 2; ++w) {
+				if (!cms_held(cfg, TOPK5_LEVEL[w])) continue;
+				A(dalloc(e, &t5.slots[w], (size_t)NSLOTS * TOPK_SET_WORDS)); A(dalloc(e, &t5.level[w], (size_t)TOPK_SET_WORDS));
+			}
+			t5.list.cap = (uint64_t)NSLOTS * TOPK_K;
+			A(dalloc(e, &t5.list.keys, (size_t)t5.list.cap, false)); A(dalloc(e, &t5.list.n, 1)); A(dalloc(e, &t5.acc, 1));
 		}
 	}
 	st.svc_tbl.insert_fail = st.counters + CTR_INSERT_FAIL; st.task_tbl.insert_fail = nullptr;
@@ -1652,6 +1703,10 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->kernel_launches += launch_cms_level_roll(CMS_TABLES[r.open].live(e), r.ring(e), CMS_TABLES[r.level].live(e), cms_words(e->cfg, r.open),
 				e->st.levels, e->stream);
 	}
+	for (int w = 0; w < 2; ++w) {		// GYSK_FLAG_FLOW_TOPK_5MIN: each level set follows its ring, before the window sets swap
+		if (!e->topk5.level[w]) continue;
+		if (int rc = topk5_roll(e, w)) return rc;
+	}
 	for (int t : {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
 		if (!cms_held(e->cfg, t)) continue;
 		unsigned long long *&open = CMS_TABLES[t].live(e);
@@ -2092,12 +2147,23 @@ int gysk_query_flow_queries(gysk_engine *e, const uint64_t *keys, uint32_t n, in
 // GYSK_FLAG_FLOW_TOPK: the heaviest flows of the open or last window
 int gysk_topk_flows(gysk_engine *e, int last_window, uint32_t n, gysk_flow_est *out, uint32_t *nout)
 {
-	return topk_read(e, 0, last_window, false, n, out, nout, "topk_flows");
+	return topk_read(e, 0, last_window, false, false, n, out, nout, nullptr, "topk_flows");
 }
 
 int gysk_topk_flow_queries(gysk_engine *e, int last_window, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout)
 {
-	return topk_read(e, 1, last_window, false, n, reinterpret_cast<gysk_flow_est *>(out), nout, "topk_flow_queries");
+	return topk_read(e, 1, last_window, false, false, n, reinterpret_cast<gysk_flow_est *>(out), nout, nullptr, "topk_flow_queries");
+}
+
+// GYSK_FLAG_FLOW_TOPK_5MIN: the heaviest flows of the rolling 300-s levels, with the bound on the flows they leave out
+int gysk_topk_flows_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 0, 0, true, false, n, out, nout, bound, "topk_flows_5min");
+}
+
+int gysk_topk_flow_queries_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 1, 0, true, false, n, reinterpret_cast<gysk_flow_est *>(out), nout, bound, "topk_flow_queries_5min");
 }
 
 // GYSK_FLAG_FLOW_QUERY_LEVEL: the point query on the rolling 300-s level of the flow query tables

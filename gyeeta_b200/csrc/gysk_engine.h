@@ -253,6 +253,14 @@ constexpr int TOPK_TABLE[2] = {CMS_CUR, CMS_QRY_CUR}, TOPK_HALF[2] = {1, 0};
 // both sets of a rank in the merge slab, in whole SlabEntrys after the rest of its content
 constexpr uint32_t TOPK_SLAB_ENTRIES = (uint32_t)((2 * TOPK_SET_WORDS * sizeof(unsigned long long) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
 
+// GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without): per held level [w] (w as TopkSets; the level of CMS_RINGS[w]) the sets of
+// its NSLOTS ring slots ([NSLOTS][TOPK_SET_WORDS], word 1 each slot's bound B_s) and the level set L ([TOPK_SET_WORDS], word 1 B_L);
+// one candidate list of NSLOTS x K keys for the flush chain, and a word for its partial bound. Outside DevState and not per slot, as
+// TopkSets.
+struct Topk5min { unsigned long long *slots[2], *level[2]; TopkList list; unsigned long long *acc; };
+// the level table of each set (the scoring half is TOPK_HALF's)
+constexpr int TOPK5_LEVEL[2] = {CMS_5MIN, CMS_QRY_5MIN};
+
 // the cells of one count-min table
 inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
 
@@ -298,6 +306,10 @@ struct MergeState
 	bool			topk_done {false};
 	unsigned long long	*topk_buf {nullptr}, *topk_n {nullptr}, *topk_tiles {nullptr};
 	uint64_t		topk_cap {0};
+	// GYSK_FLAG_FLOW_TOPK_5MIN: the rank's level sets ride from slab entry topk5_off (TOPK_SLAB_ENTRIES); the merged sets of the last
+	// finished merge with their bounds ([2][TOPK_SET_WORDS]). They share the window sets' union buffers.
+	uint32_t		topk5_off {0};
+	unsigned long long	*topk5_final {nullptr};
 };
 
 } // namespace gysk
@@ -312,6 +324,7 @@ struct gysk_engine
 	gysk::FlowQueries	fq {};				// GYSK_FLAG_FLOW_QUERIES (every pointer nullptr without)
 	gysk::FlowRespHist	fr {};				// GYSK_FLAG_FLOW_RESP_HIST (every pointer nullptr without)
 	gysk::TopkSets		topk {};			// GYSK_FLAG_FLOW_TOPK (every pointer nullptr without)
+	gysk::Topk5min		topk5 {};			// GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
 	std::vector<void *>	hallocs;
@@ -449,8 +462,10 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
 // GYSK_FLAG_FLOW_TOPK: the first min(n, K) flows of heaviest-flow set `which` (0: connections, 1: flow queries), best first, with their
 // estimates on its table: the engine's open (last_window = 0) or last set, or merged, the last finished merge's set on the summed table.
-// Flows with a zero score are left out.
-int topk_read(gysk_engine *e, int which, int last_window, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout, const char *what);
+// level (GYSK_FLAG_FLOW_TOPK_5MIN): the 300-s level set instead, on the level (merged: the summed level), last_window ignored. Flows with
+// a zero score are left out; *bound (if not nullptr) = the set's word 1.
+int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout,
+		uint64_t *bound, const char *what);
 // the same on a flow response histogram table (CMS_RESP_*)
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what);
 

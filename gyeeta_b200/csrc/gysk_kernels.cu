@@ -2749,6 +2749,49 @@ int launch_topk_gather(const unsigned long long *sets, uint32_t world, size_t st
 	return 1;
 }
 
+// GYSK_FLAG_FLOW_TOPK_5MIN: one CTA per bit of mask, the set of a set bit appended to l as topk_gather_kernel does (a sibling, so that
+// the merge's gather keeps its code)
+__global__ void __launch_bounds__(256) topk_gather_mask_kernel(const unsigned long long *__restrict__ sets, size_t stride, uint32_t mask, TopkList l)
+{
+	if (!((mask >> blockIdx.x) & 1u)) return;
+	const unsigned long long *set = sets + blockIdx.x * stride;
+	const uint32_t m = (uint32_t)min(set[0], (unsigned long long)TOPK_K);
+	__shared__ unsigned long long base;
+	if (threadIdx.x == 0) base = atomicAdd(l.n, (unsigned long long)m);
+	__syncthreads();
+	for (uint32_t j = threadIdx.x; j < m; j += blockDim.x) l.keys[base + j] = set[2 + j];
+}
+
+int launch_topk_gather_mask(const unsigned long long *sets, size_t stride, uint32_t mask, const TopkList &l, bool reset, cudaStream_t s)
+{
+	if (reset) cudaMemsetAsync(l.n, 0, sizeof(unsigned long long), s);
+	if (!mask) return 0;
+	topk_gather_mask_kernel<<<32 - __builtin_clz(mask), 256, 0, s>>>(sets, stride, mask, l);
+	return 1;
+}
+
+// GYSK_FLAG_FLOW_TOPK_5MIN: the bound word of launch_topk_bound, one thread (a set's K-th key and at most world terms)
+__global__ void topk_bound_kernel(const unsigned long long *__restrict__ set, const unsigned long long *__restrict__ tbl, uint32_t depth,
+		uint32_t log2w, int half, const unsigned long long *terms, size_t stride, uint32_t nterms, uint32_t mask, int sum,
+		unsigned long long *out)
+{
+	unsigned long long thr = 0, t = 0;
+	if (set[0] >= TOPK_K) {
+		uint32_t lo, hi;
+		cms_point(tbl, depth, log2w, set[2 + TOPK_K - 1], lo, hi);
+		thr = half ? hi : lo;
+	}
+	for (uint32_t j = 0; j < nterms; ++j) if ((mask >> (j & 31u)) & 1u) t += terms[j * stride];
+	*out = sum ? thr + t : max(thr, t);
+}
+
+int launch_topk_bound(const unsigned long long *set, const unsigned long long *tbl, uint32_t depth, uint32_t log2w, int half,
+		const unsigned long long *terms, size_t stride, uint32_t nterms, uint32_t mask, bool sum, unsigned long long *out, cudaStream_t s)
+{
+	topk_bound_kernel<<<1, 1, 0, s>>>(set, tbl, depth, log2w, half, terms, stride, nterms, mask, sum ? 1 : 0, out);
+	return 1;
+}
+
 // per-task window of the three MTASK_HIST histograms: totals now minus totals at the previous flush (nothing on the ingest path).
 // With idle_secs, the process eviction (MCONN_HANDLER::cleanup_partha_unused_aggr_tasks, server/gy_mconnhdlr.cc:16492-16541: a MAGGR_TASK
 // whose last_tusec_ is older than 30 min goes): the thread of a live slot's first histogram stamps the slot with tsec when the window

@@ -175,7 +175,8 @@ static constexpr uint32_t CMS_LOG2W_MAX = 28;		// the widest count-min gysk_crea
 // pass, sweeping the batch flow table, the key its claimer stored in ekeys beside the entry. cap = K + max_batch: a record appends at most
 // once, directly or by claiming an entry. Every pointer nullptr: not held.
 struct TopkList { unsigned long long *keys, *n, *ekeys; unsigned long long cap; };
-// a heaviest-flow set: [TOPK_SET_WORDS] u64, word 0 its size, word 1 zero, then the K keys best first
+// a heaviest-flow set: [TOPK_SET_WORDS] u64, word 0 its size, word 1 zero (GYSK_FLAG_FLOW_TOPK_5MIN's sets: their bound), then the K
+// keys best first
 static constexpr uint32_t TOPK_K = GYSK_FLOW_TOPK_CAP, TOPK_SET_WORDS = TOPK_K + 2;
 // the held lists: [0] the connection table's, [1] the flow query table's
 struct FlowTopk { TopkList list[2]; };
@@ -275,6 +276,13 @@ int launch_topk_select(const SortTemp &tmp, const TopkList &l, uint64_t n_max, c
 		int half, unsigned long long *set, bool reseed, cudaStream_t s);
 // the merge's union into l (its count reset first): the keys of world sets, rank r's at sets + r * stride words
 int launch_topk_gather(const unsigned long long *sets, uint32_t world, size_t stride, const TopkList &l, cudaStream_t s);
+// GYSK_FLAG_FLOW_TOPK_5MIN: the keys of set j (at sets + j * stride words) appended to l for each bit j of mask (j < 32), l's count reset
+// first when reset is true
+int launch_topk_gather_mask(const unsigned long long *sets, size_t stride, uint32_t mask, const TopkList &l, bool reset, cudaStream_t s);
+// GYSK_FLAG_FLOW_TOPK_5MIN: a set's bound word. thr(set) is the score on tbl (half as launch_topk_select) of its K-th key when it holds K,
+// else 0; t the sum of terms[j * stride] over j < nterms with bit j % 32 of mask set. *out = sum ? thr + t : max(thr, t)
+int launch_topk_bound(const unsigned long long *set, const unsigned long long *tbl, uint32_t depth, uint32_t log2w, int half,
+		const unsigned long long *terms, size_t stride, uint32_t nterms, uint32_t mask, bool sum, unsigned long long *out, cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
 // bits outside [0, 64)), or n_max >= 2^30
 int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64_t n_max, int lo, int hi, int *which, cudaStream_t s);

@@ -879,7 +879,7 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// (re)allocate the arena
 	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
 	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel); dfree(e, mg.topn_slots); dfree(e, mg.topn_final); dfree(e, mg.lg.trace_final);
-	dfree(e, mg.topk_final); dfree(e, mg.topk_buf); dfree(e, mg.topk_n); dfree(e, mg.topk_tiles);
+	dfree(e, mg.topk_final); dfree(e, mg.topk_buf); dfree(e, mg.topk_n); dfree(e, mg.topk_tiles); dfree(e, mg.topk5_final);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
@@ -898,16 +898,19 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// GYSK_FLAG_MERGE_TOPN: the candidates after the digests, in whole SlabEntrys, so the slab stays one all-gather; GYSK_FLAG_MERGE_TRACES:
 	// the trace digests after them, packed as TraceSlabs in whole SlabEntrys
 	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
-	// GYSK_FLAG_FLOW_TOPK: the rank's last-window heaviest-flow sets after everything else
-	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK;
+	// GYSK_FLAG_FLOW_TOPK: the rank's last-window heaviest-flow sets after everything else; GYSK_FLAG_FLOW_TOPK_5MIN: its level sets
+	// and their bounds after those
+	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK, topk5 = e->cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN;
 	mg.trace_off = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
 	mg.topk_off = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
-	mg.slab_entries = mg.topk_off + (topk ? TOPK_SLAB_ENTRIES : 0);
+	mg.topk5_off = mg.topk_off + (topk ? TOPK_SLAB_ENTRIES : 0);
+	mg.slab_entries = mg.topk5_off + (topk5 ? TOPK_SLAB_ENTRIES : 0);
 	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
 	if (topk) {
 		if ((rc = dalloc(e, &mg.topk_final, 2 * (size_t)TOPK_SET_WORDS))) return rc;
 		if ((rc = dalloc(e, &mg.topk_n, 1))) return rc;
 	}
+	if (topk5 && (rc = dalloc(e, &mg.topk5_final, 2 * (size_t)TOPK_SET_WORDS))) return rc;
 	if (topn) {
 		if ((rc = dalloc(e, &mg.topn_slots, (size_t)TOPN_LISTS * TOPN_K))) return rc;
 		if ((rc = dalloc(e, &mg.topn_final, TopnLists::BYTES))) return rc;
@@ -1067,6 +1070,14 @@ int gysk_merge_prepare(gysk_engine *e)
 			else CU(e, cudaMemsetAsync(d, 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
 		}
 	}
+	if (mg.topk5_final) {		// GYSK_FLAG_FLOW_TOPK_5MIN: the level sets with their bounds (a level the engine does not hold: empty)
+		unsigned long long *dst = reinterpret_cast<unsigned long long *>(mg.lg.slab + mg.topk5_off);
+		for (int w = 0; w < 2; ++w) {
+			unsigned long long *d = dst + (size_t)w * TOPK_SET_WORDS;
+			if (e->topk5.level[w]) CU(e, cudaMemcpyAsync(d, e->topk5.level[w], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
+			else CU(e, cudaMemsetAsync(d, 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
+		}
+	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
 	return post_launch(e, "merge_prepare");
@@ -1139,6 +1150,19 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 					e->stream);
 			if (k < 0) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: heaviest-flow sort failed");
 			e->kernel_launches += k;
+		}
+		// GYSK_FLAG_FLOW_TOPK_5MIN: per held level the union of every rank's level set, the K best on the summed level, with
+		// B_G = max(thr(G), sum over ranks of B_L)
+		for (int w = 0; w < 2 && mg.topk5_final; ++w) {
+			unsigned long long *set = mg.topk5_final + (size_t)w * TOPK_SET_WORDS;
+			if (!e->topk5.level[w]) continue;
+			const unsigned long long *sets = reinterpret_cast<const unsigned long long *>(src + mg.topk5_off) + (size_t)w * TOPK_SET_WORDS;
+			const unsigned long long *tbl = mg.g_cms[TOPK5_LEVEL[w]];
+			e->kernel_launches += launch_topk_gather(sets, world, stride, l, e->stream);
+			const int k = launch_topk_select(t, l, need, tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, TOPK_HALF[w], set, false, e->stream);
+			if (k < 0) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: 300-s heaviest-flow sort failed");
+			e->kernel_launches += k + launch_topk_bound(set, tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, TOPK_HALF[w], sets + 1, stride, world, ~0u,
+					false, set + 1, e->stream);
 		}
 		mg.topk_done = true;
 	}
@@ -1437,12 +1461,23 @@ int gysk_merge_global(gysk_engine *e, void *comm)
 // GYSK_FLAG_FLOW_TOPK: the heaviest flows of the last finished merge
 int gysk_topk_flows_global(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout)
 {
-	return topk_read(e, 0, 1, true, n, out, nout, "topk_flows_global");
+	return topk_read(e, 0, 1, false, true, n, out, nout, nullptr, "topk_flows_global");
 }
 
 int gysk_topk_flow_queries_global(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout)
 {
-	return topk_read(e, 1, 1, true, n, reinterpret_cast<gysk_flow_est *>(out), nout, "topk_flow_queries_global");
+	return topk_read(e, 1, 1, false, true, n, reinterpret_cast<gysk_flow_est *>(out), nout, nullptr, "topk_flow_queries_global");
+}
+
+// GYSK_FLAG_FLOW_TOPK_5MIN: the heaviest flows of the summed 300-s levels of the last finished merge, with B_G
+int gysk_topk_flows_global_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 0, 0, true, true, n, out, nout, bound, "topk_flows_global_5min");
+}
+
+int gysk_topk_flow_queries_global_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 1, 0, true, true, n, reinterpret_cast<gysk_flow_est *>(out), nout, bound, "topk_flow_queries_global_5min");
 }
 
 int gysk_topn_global(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, gysk_svc_summary *rows, uint32_t *nout)

@@ -42,6 +42,7 @@ FLAG_FLOW_QUERIES = 128
 FLAG_FLOW_QUERY_LEVEL = 0x100
 FLAG_FLOW_RESP_HIST = 0x200
 FLAG_FLOW_TOPK = 0x400
+FLAG_FLOW_TOPK_5MIN = 0x800
 FLOW_TOPK_CAP = 4096
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
@@ -331,6 +332,10 @@ def load_library(path=None):
         "gysk_topk_flow_queries": (i32, [vp, i32, u32, vp, vp]),
         "gysk_topk_flows_global": (i32, [vp, u32, vp, vp]),
         "gysk_topk_flow_queries_global": (i32, [vp, u32, vp, vp]),
+        "gysk_topk_flows_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_topk_flow_queries_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_topk_flows_global_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_topk_flow_queries_global_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -397,7 +402,7 @@ class Engine:
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
                  max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False,
-                 flow_topk=False):
+                 flow_topk=False, flow_topk_5min=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -412,7 +417,8 @@ class Engine:
                     (FLAG_MERGE_STATES if merge_states else 0) | (FLAG_MERGE_CLUSTERS if merge_clusters else 0) | \
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
                     (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
-                    (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0)
+                    (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0) | \
+                    (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -742,6 +748,31 @@ class Engine:
     def topk_flow_queries_global(self, n=FLOW_TOPK_CAP):
         """gysk_topk_flow_queries_global: the n heaviest flows by queries over every rank, from the last finished merge"""
         return self._topk(self.L.gysk_topk_flow_queries_global, FLOW_QRY_EST_DTYPE, n)
+
+    def _topk_5min(self, fn, dtype, n):
+        """a 300-s heaviest-flow read fn(h, n, out, nout, bound): the rows, best first, and the bound on every flow left out"""
+        out = np.zeros(n, dtype=dtype)
+        k, b = C.c_uint32(), C.c_uint64()
+        self._chk(fn(self.h, n, _p(out), C.byref(k), C.byref(b)))
+        return out[: k.value], b.value
+
+    def topk_flows_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flows_5min: (rows, bound): the n heaviest flows by kbytes of the rolling 300-s connection level, with their
+        estimates, and B_L: every flow left out scores at most that over the 300 s (flow_topk_5min=True, flow_level=True)"""
+        return self._topk_5min(self.L.gysk_topk_flows_5min, FLOW_EST_DTYPE, n)
+
+    def topk_flow_queries_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_queries_5min: (rows, bound) of the rolling 300-s flow query level by queries (flow_topk_5min=True,
+        flow_query_level=True)"""
+        return self._topk_5min(self.L.gysk_topk_flow_queries_5min, FLOW_QRY_EST_DTYPE, n)
+
+    def topk_flows_global_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flows_global_5min: (rows, bound) over every rank's connection level, from the last finished merge"""
+        return self._topk_5min(self.L.gysk_topk_flows_global_5min, FLOW_EST_DTYPE, n)
+
+    def topk_flow_queries_global_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_queries_global_5min: (rows, bound) over every rank's flow query level, from the last finished merge"""
+        return self._topk_5min(self.L.gysk_topk_flow_queries_global_5min, FLOW_QRY_EST_DTYPE, n)
 
     def topn(self, metric, n=10, host_idx=-1):
         out = (TopnEntry * n)()

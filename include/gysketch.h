@@ -256,6 +256,12 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   below). Needs no other flag. Without it nothing is allocated, every other call answers
 						   as before and the four calls are GYSK_ERR_NOTSUP */
 #define GYSK_FLOW_TOPK_CAP		4096u	/* K: the flows each heaviest-flow set holds (fixed: gysk_config has no word for it) */
+#define GYSK_FLAG_FLOW_TOPK_5MIN	0x800u	/* the GYSK_FLOW_TOPK_CAP heaviest client flows of each held rolling 300-s flow level,
+						   with a bound on every flow they leave out (gysk_topk_flows_5min, "heaviest flows of the
+						   300-s levels" below), on each rank and across ranks. Needs GYSK_FLAG_FLOW_TOPK and
+						   GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_FLOW_QUERY_LEVEL: gysk_create refuses it without.
+						   Without it nothing is allocated, every other call answers as before and the four calls
+						   are GYSK_ERR_NOTSUP */
 
 typedef struct gysk_config
 {
@@ -756,11 +762,39 @@ int		gysk_query_flow_resp_global_5min(gysk_engine *e, const uint64_t *flow_keys,
  *   a zero score are left out, so *nout may be below n. gysk_topk_flow_queries: the same for the query table (GYSK_ERR_NOTSUP without
  *   GYSK_FLAG_FLOW_QUERIES). The _global pair: the merged lists of the last gysk_merge_finish, with their estimates on the summed tables
  *   (GYSK_ERR_INVAL before the first one). Every call is GYSK_ERR_NOTSUP without the flag.
- * Not covered: sets for the 300-s levels, a set scored by the response histograms, per-(service, client) pairs, a configurable K. */
+ * Not covered: a set scored by the response histograms, per-(service, client) pairs, a configurable K. */
 int		gysk_topk_flows(gysk_engine *e, int last_window, uint32_t n, gysk_flow_est *out, uint32_t *nout);
 int		gysk_topk_flow_queries(gysk_engine *e, int last_window, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout);
 int		gysk_topk_flows_global(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout);
 int		gysk_topk_flow_queries_global(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout);
+
+/* ---- heaviest flows of the 300-s levels (GYSK_FLAG_FLOW_TOPK_5MIN): the top talkers and requesters of the last five minutes ----
+ * A client that sends steadily for five minutes may never be among one window's K heaviest, yet be the heaviest of the five minutes.
+ * One set per held level: the connection level (GYSK_FLAG_FLOW_LEVEL), scored by its kbytes half, and the flow query level
+ * (GYSK_FLAG_FLOW_QUERY_LEVEL), scored by its queries half. A score is the level's point estimate (gysk_query_flows_5min /
+ * gysk_query_flow_queries_5min); the order is the window sets' (score descending, flow key ascending); K = GYSK_FLOW_TOPK_CAP.
+ * The rule follows the level's own ring: at every gysk_flush, once the closing window is in ring slot s = (tsec / 30) % 10, and before
+ * the window sets swap, per held level:
+ *   1. slot fold: if the flush cleared slot s, its set S_s and bound B_s are cleared first. S_s becomes the K best of S_s u W scored on
+ *      ring slot s, W the closing window's heaviest-flow set; B_s = max(thr(S_s), B_s + thr(W));
+ *   2. level set: L becomes the K best of the union of the live slots' sets scored on the level; B_L = max(thr(L), sum of the live B_s).
+ * thr(X) is the smallest score of X when it holds K flows, else 0. Before the first flush L is empty and B_L = 0; the open window is
+ * not in the level, so not in L either.
+ * Guarantee: if no cell half wraps, every flow that L does not hold has an exact 5-minute score of at most B_L; every flow whose exact
+ * score exceeds B_L is in L. (A flow outside W scores at most thr(W) in that window; a flow cut at a fold scores at most that fold's
+ * threshold; a slot's scores never fall within its epoch. DESIGN.md section 2 has the proof.) A steady client that no window ranks can
+ * leave B_L large: the bound says how much of the five minutes the list can have missed.
+ * Across ranks: gysk_merge_prepare carries each rank's L sets and B_L after the window sets in the t-digest slab (no logical map
+ * needed); gysk_merge_finish keeps the K best of the union of every rank's set scored on the summed levels, with B_G = max(thr(G), sum
+ * over ranks of B_L). Each rank's level is relative to its own last flush: gysk_merge_flush_range shows whether they closed the same one.
+ * gysk_topk_flows_5min / gysk_topk_flow_queries_5min: the first min(n, K) flows of L, best first, each row what the _5min point query
+ *   answers for its key; entries with a zero score are left out, so *nout may be below n. *bound (may be NULL) = B_L. GYSK_ERR_NOTSUP
+ *   without the flag or without the level the call reads. The _global pair: the same of the last gysk_merge_finish, each row what the
+ *   _global_5min point query answers, *bound = B_G (GYSK_ERR_INVAL before the first one). */
+int		gysk_topk_flows_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout, uint64_t *bound);
+int		gysk_topk_flow_queries_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound);
+int		gysk_topk_flows_global_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout, uint64_t *bound);
+int		gysk_topk_flow_queries_global_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound);
 
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
