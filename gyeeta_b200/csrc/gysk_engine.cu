@@ -75,17 +75,17 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, rr, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, e->topk.b_slow, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[2], e->stream));
 	// GYSK_FLAG_FLOW_TOPK: each held table's open set from its candidates, once all of the batch's increments are in the table. After the
-	// batch merge, whose sort buffers it takes.
-	for (int w = 0; w < 2; ++w) {
+	// batch merge, whose sort buffers it takes; GYSK_FLAG_FLOW_TOPK_SLOW's set last, in the same buffers.
+	for (int w = 0; w < TOPK_SETS; ++w) {
 		if (!e->topk.tk.list[w].keys) continue;
 		const int k = launch_topk_select(e->tmp, e->topk.tk.list[w], TOPK_K + n, CMS_TABLES[TOPK_TABLE[w]].live(e), e->cfg.cms_depth,
-				e->cfg.cms_log2_width, TOPK_HALF[w], e->topk.open[w], true, e->stream);
+				e->cfg.cms_log2_width, topk_score(e->topk, w), e->topk.open[w], true, e->stream);
 		if (k < 0) return fail(e, GYSK_ERR_INVAL, "heaviest-flow selection: no sort plan");
 		e->kernel_launches += k;
 	}
@@ -325,7 +325,17 @@ int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t
 	}, CopyRows<gysk_flow_est> {out});
 }
 
-int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout,
+// a row's score as its set ranks it: the half of a gysk_flow_est, the slow score of a gysk_flow_resp_est (saturated as resp_slow_score)
+static uint64_t topk_row_score(const gysk_engine *e, int which, const gysk_flow_est &r) { return TOPK_HALF[which] ? r.kbytes : r.count; }
+static uint64_t topk_row_score(const gysk_engine *e, int, const gysk_flow_resp_est &r)
+{
+	uint64_t s = 0;
+	for (uint32_t b = e->topk.b_slow; b < 15; ++b) s += r.counts[b];
+	return std::min<uint64_t>(s, 0xFFFFFFFFu);
+}
+
+template <typename Row>
+int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, Row *out, uint32_t *nout,
 		uint64_t *bound, const char *what)
 {
 	CHECK_ENGINE(e);
@@ -343,17 +353,23 @@ int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merge
 	const uint32_t m = (uint32_t)std::min<uint64_t>({keys[0], (uint64_t)n, (uint64_t)TOPK_K});
 	const int t = level ? TOPK5_LEVEL[which] : TOPK_TABLE[which] + (merged || last_window ? 1 : 0);	// merged: the summed table
 	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[t].live(e);
-	std::vector<gysk_flow_est> rows(m);
-	int rc = staged_read(e, keys.data() + 2, m, QCHUNK, sizeof(gysk_flow_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t k) {
-		return launch_query_flows(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, k, reinterpret_cast<gysk_flow_est *>(e->d_wstage), e->stream);
-	}, CopyRows<gysk_flow_est> {rows.data()});
+	std::vector<Row> rows(m);
+	int rc = staged_read(e, keys.data() + 2, m, QCHUNK, sizeof(Row), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t k) {
+		Row *d_out = reinterpret_cast<Row *>(e->d_wstage);
+		if constexpr (std::is_same<Row, gysk_flow_resp_est>::value)
+			return launch_query_flow_resp(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, k, d_out, e->stream);
+		else return launch_query_flows(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, k, d_out, e->stream);
+	}, CopyRows<Row> {rows.data()});
 	if (rc) return rc;
 	uint32_t k = 0;
-	for (const gysk_flow_est &r : rows) if (TOPK_HALF[which] ? r.kbytes : r.count) out[k++] = r;
+	for (const Row &r : rows) if (topk_row_score(e, which, r)) out[k++] = r;
 	*nout = k;
 	if (bound) *bound = keys[1];
 	return GYSK_OK;
 }
+template int topk_read<gysk_flow_est>(gysk_engine *, int, int, bool, bool, uint32_t, gysk_flow_est *, uint32_t *, uint64_t *, const char *);
+template int topk_read<gysk_flow_resp_est>(gysk_engine *, int, int, bool, bool, uint32_t, gysk_flow_resp_est *, uint32_t *, uint64_t *,
+		const char *);
 
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what)
 {
@@ -473,7 +489,7 @@ static int topk5_roll(gysk_engine *e, int w)
 	const Topk5min &t5 = e->topk5;
 	const CmsRingDesc &r = CMS_RINGS[w];
 	const uint32_t d = e->cfg.cms_depth, lw = e->cfg.cms_log2_width;
-	const int half = TOPK_HALF[w];
+	const int half = topk_score(e->topk, w);
 	unsigned long long *slot = t5.slots[w] + (size_t)lv.cur[0] * TOPK_SET_WORDS, *level = t5.level[w];
 	const unsigned long long *win = e->topk.open[w];		// W, still the open window's set
 	const unsigned long long *slot_tbl = r.ring(e) + (size_t)lv.cur[0] * cms_words(e->cfg, r.open), *level_tbl = CMS_TABLES[r.level].live(e);
@@ -659,6 +675,10 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_5MIN needs GYSK_FLAG_FLOW_TOPK");
 	if ((cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) && !(cfg.flags & (GYSK_FLAG_FLOW_LEVEL | GYSK_FLAG_FLOW_QUERY_LEVEL)))
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_5MIN needs GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_FLOW_QUERY_LEVEL");
+	if ((cfg.flags & GYSK_FLAG_FLOW_TOPK_SLOW) && !(cfg.flags & GYSK_FLAG_FLOW_TOPK))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_SLOW needs GYSK_FLAG_FLOW_TOPK");
+	if ((cfg.flags & GYSK_FLAG_FLOW_TOPK_SLOW) && !(cfg.flags & GYSK_FLAG_FLOW_RESP_HIST))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_SLOW needs GYSK_FLAG_FLOW_RESP_HIST");
 
 	int ndev = 0;
 	cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -768,19 +788,23 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
 		if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) A(dalloc(e, &e->fq.flow, (size_t)tmp.flow_cap));		// the query flow table, alike
 		if (cfg.flags & GYSK_FLAG_FLOW_RESP_HIST) A(dalloc(e, &e->fr.flow, (size_t)tmp.flow_cap));		// the response flow table, alike
-		// GYSK_FLAG_FLOW_TOPK: per held table its candidate list, the keys beside its batch flow table and its two sets, all empty
-		for (int w = 0; w < 2 && (cfg.flags & GYSK_FLAG_FLOW_TOPK); ++w) {
-			if (!cms_held(cfg, TOPK_TABLE[w])) continue;
+		// GYSK_FLAG_FLOW_TOPK: per held table its candidate list, the keys beside its batch flow table and its two sets, all empty.
+		// GYSK_FLAG_FLOW_TOPK_SLOW: the slow set's alike, without keys beside a flow table (a slow sample appends once per record, so
+		// cap = K + max_batch holds every one), at the default threshold.
+		e->topk.b_slow = TOPK_SLOW_DEFAULT_B;
+		for (int w = 0; w < TOPK_SETS && (cfg.flags & GYSK_FLAG_FLOW_TOPK); ++w) {
+			if (!cms_held(cfg, TOPK_TABLE[w]) || (w == 2 && !(cfg.flags & GYSK_FLAG_FLOW_TOPK_SLOW))) continue;
 			TopkList &l = e->topk.tk.list[w];
 			l.cap = (uint64_t)TOPK_K + cfg.max_batch;
-			A(dalloc(e, &l.keys, (size_t)l.cap, false)); A(dalloc(e, &l.n, 1)); A(dalloc(e, &l.ekeys, (size_t)tmp.flow_cap, false));
+			A(dalloc(e, &l.keys, (size_t)l.cap, false)); A(dalloc(e, &l.n, 1));
+			if (w < 2) A(dalloc(e, &l.ekeys, (size_t)tmp.flow_cap, false));
 			A(dalloc(e, &e->topk.open[w], (size_t)TOPK_SET_WORDS)); A(dalloc(e, &e->topk.last[w], (size_t)TOPK_SET_WORDS));
 		}
 		// GYSK_FLAG_FLOW_TOPK_5MIN: per held level its slot sets and level set, all empty with zero bounds; the flush chain's list
 		if (cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) {
 			Topk5min &t5 = e->topk5;
-			for (int w = 0; w < 2; ++w) {
-				if (!cms_held(cfg, TOPK5_LEVEL[w])) continue;
+			for (int w = 0; w < TOPK_SETS; ++w) {
+				if (!cms_held(cfg, TOPK5_LEVEL[w]) || !e->topk.open[w]) continue;
 				A(dalloc(e, &t5.slots[w], (size_t)NSLOTS * TOPK_SET_WORDS)); A(dalloc(e, &t5.level[w], (size_t)TOPK_SET_WORDS));
 			}
 			t5.list.cap = (uint64_t)NSLOTS * TOPK_K;
@@ -959,6 +983,7 @@ int gysk_ingest_device(gysk_engine *e, const gysk_event *d_events, uint64_t n)
 	CHECK_ENGINE(e);
 	if (!d_events && n) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Submit);					// keep arrival order
+	if (n) e->fed = true;
 	for (uint64_t off = 0; off < n; off += e->cfg.max_batch) {
 		const uint64_t m = std::min<uint64_t>(e->cfg.max_batch, n - off);
 		if (int rc = process_device_batch(e, d_events + off, m, nullptr)) return rc;
@@ -971,6 +996,7 @@ int gysk_ingest_pinned(gysk_engine *e, const gysk_event *pinned, uint64_t n)
 	CHECK_ENGINE(e);
 	if (!pinned && n) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Drain);
+	if (n) e->fed = true;
 	// zero copy on the host: the H2D copies read the caller's page-locked buffer directly, chunk by chunk into the two device
 	// event buffers; the copy of chunk c+1 is enqueued as soon as the ingest kernel of chunk c is, so the link never idles
 	return append_chunk(e, pinned, n);
@@ -1266,6 +1292,7 @@ int gysk_ingest_raw(gysk_engine *e, const uint8_t host_id[16], uint32_t host_idx
 	CHECK_ENGINE(e);
 	(void)host_id;
 	if (!events && n) return GYSK_ERR_INVAL;
+	if (n) e->fed = true;
 	ThreadStage *ts = get_stage(e);
 	if (!ts) return fail(e, GYSK_ERR_NOMEM, "thread stage");
 	std::lock_guard<std::mutex> tl(ts->m);
@@ -1295,6 +1322,7 @@ int gysk_ingest(gysk_engine *e, const uint8_t host_id[16], uint32_t host_idx, ui
 	CHECK_ENGINE(e);
 	(void)host_id;
 	if (!recs || !endptr || (const uint8_t *)endptr < (const uint8_t *)recs) return GYSK_ERR_INVAL;
+	if (nevents) e->fed = true;
 	ThreadStage *ts = get_stage(e);
 	if (!ts) return fail(e, GYSK_ERR_NOMEM, "thread stage");
 	std::lock_guard<std::mutex> tl(ts->m);
@@ -1655,6 +1683,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 {
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Submit);
+	e->fed = true;
 
 	if (int rc = auto_grow(e)) return rc;
 	if (int rc = roll_levels(e, tsec)) return rc;
@@ -1703,7 +1732,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->kernel_launches += launch_cms_level_roll(CMS_TABLES[r.open].live(e), r.ring(e), CMS_TABLES[r.level].live(e), cms_words(e->cfg, r.open),
 				e->st.levels, e->stream);
 	}
-	for (int w = 0; w < 2; ++w) {		// GYSK_FLAG_FLOW_TOPK_5MIN: each level set follows its ring, before the window sets swap
+	for (int w = 0; w < TOPK_SETS; ++w) {		// GYSK_FLAG_FLOW_TOPK_5MIN: each level set follows its ring, before the window sets swap
 		if (!e->topk5.level[w]) continue;
 		if (int rc = topk5_roll(e, w)) return rc;
 	}
@@ -1713,7 +1742,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		std::swap(open, CMS_TABLES[t + 1].live(e));
 		CU(e, cudaMemsetAsync(open, 0, sizeof(unsigned long long) * cms_words(e->cfg, t), e->stream));
 	}
-	for (int w = 0; w < 2; ++w) {		// GYSK_FLAG_FLOW_TOPK: each heaviest-flow set with its table, and no candidates yet
+	for (int w = 0; w < TOPK_SETS; ++w) {		// GYSK_FLAG_FLOW_TOPK: each heaviest-flow set with its table, and no candidates yet
 		if (!e->topk.open[w]) continue;
 		std::swap(e->topk.open[w], e->topk.last[w]);
 		CU(e, cudaMemsetAsync(e->topk.open[w], 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
@@ -2164,6 +2193,30 @@ int gysk_topk_flows_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_
 int gysk_topk_flow_queries_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound)
 {
 	return topk_read(e, 1, 0, true, false, n, reinterpret_cast<gysk_flow_est *>(out), nout, bound, "topk_flow_queries_5min");
+}
+
+// GYSK_FLAG_FLOW_TOPK_SLOW: the threshold of a slow sample, one of RESP_TIME_HASH's 13, before the engine sees its first event or flush
+int gysk_set_flow_slow(gysk_engine *e, uint32_t above_ms)
+{
+	CHECK_ENGINE(e);
+	if (!e->topk.open[2]) return GYSK_ERR_NOTSUP;
+	static constexpr uint32_t thr[13] = {1, 10, 30, 60, 100, 150, 200, 300, 450, 700, 1000, 3000, 15000};
+	const uint32_t *p = std::find(thr, thr + 13, above_ms);
+	if (p == thr + 13) return fail(e, GYSK_ERR_INVAL, "gysk_set_flow_slow: not a RESP_TIME_HASH threshold");
+	if (e->fed) return fail(e, GYSK_ERR_INVAL, "gysk_set_flow_slow: the engine has taken events or a flush");
+	e->topk.b_slow = 2u + (uint32_t)(p - thr);		// msec > thr[i] <=> bucket_resp_time(msec) >= i + 2
+	return GYSK_OK;
+}
+
+// GYSK_FLAG_FLOW_TOPK_SLOW: the flows with the most slow responses in the open or last window, and in the rolling 300-s level
+int gysk_topk_flow_slow(gysk_engine *e, int last_window, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout)
+{
+	return topk_read(e, 2, last_window, false, false, n, out, nout, nullptr, "topk_flow_slow");
+}
+
+int gysk_topk_flow_slow_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 2, 0, true, false, n, out, nout, bound, "topk_flow_slow_5min");
 }
 
 // GYSK_FLAG_FLOW_QUERY_LEVEL: the point query on the rolling 300-s level of the flow query tables

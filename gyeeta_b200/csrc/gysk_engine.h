@@ -245,21 +245,33 @@ constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(Sla
 enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, CMS_RESP_CUR, CMS_RESP_LAST, CMS_RESP_5MIN, NCMS };
 
 // GYSK_FLAG_FLOW_TOPK (every pointer nullptr without): the candidate lists and the open / last heaviest-flow sets ([TOPK_SET_WORDS]
-// each) of the connection table [0] and, with GYSK_FLAG_FLOW_QUERIES, the flow query table [1]. Outside DevState, so that the kernels
+// each) of the connection table [0] and, with GYSK_FLAG_FLOW_QUERIES, the flow query table [1]; with GYSK_FLAG_FLOW_TOPK_SLOW the slow
+// set of the response histogram table [2], b_slow its first slow bucket (gysk_set_flow_slow). Outside DevState, so that the kernels
 // without the flag keep their parameter layout; not per slot, so gysk_grow and eviction leave them.
-struct TopkSets { FlowTopk tk; unsigned long long *open[2], *last[2]; };
-// the count-min table of each set, and the half of its cells that scores (1: kbytes, the high half; 0: queries, the low half)
-constexpr int TOPK_TABLE[2] = {CMS_CUR, CMS_QRY_CUR}, TOPK_HALF[2] = {1, 0};
-// both sets of a rank in the merge slab, in whole SlabEntrys after the rest of its content
-constexpr uint32_t TOPK_SLAB_ENTRIES = (uint32_t)((2 * TOPK_SET_WORDS * sizeof(unsigned long long) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
+struct TopkSets { FlowTopk tk; unsigned long long *open[3], *last[3]; uint32_t b_slow; };
+constexpr int TOPK_SETS = 3;
+// the count-min table of each set, and the half of its cells that scores (1: kbytes, the high half; 0: queries, the low half; the slow
+// set's score is topk_score's)
+constexpr int TOPK_TABLE[TOPK_SETS] = {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR}, TOPK_HALF[2] = {1, 0};
+// the score of set w (launch_topk_select): TOPK_HALF[w], or the slow score from bucket b_slow
+inline int topk_score(const TopkSets &t, int w) { return w < 2 ? TOPK_HALF[w] : TOPK_SCORE_SLOW | (int)t.b_slow; }
+// GYSK_FLAG_FLOW_TOPK_SLOW's default threshold: a sample above 300 ms is slow (RESP_TIME_HASH bucket 9 and up)
+constexpr uint32_t TOPK_SLOW_DEFAULT_B = 9;
+// nsets sets of a rank in the merge slab, in whole SlabEntrys after the rest of its content
+constexpr uint32_t topk_slab_entries(uint32_t nsets)
+{
+	return (uint32_t)((nsets * TOPK_SET_WORDS * sizeof(unsigned long long) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry));
+}
+constexpr uint32_t TOPK_SLAB_ENTRIES = topk_slab_entries(2);
 
 // GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without): per held level [w] (w as TopkSets; the level of CMS_RINGS[w]) the sets of
 // its NSLOTS ring slots ([NSLOTS][TOPK_SET_WORDS], word 1 each slot's bound B_s) and the level set L ([TOPK_SET_WORDS], word 1 B_L);
 // one candidate list of NSLOTS x K keys for the flush chain, and a word for its partial bound. Outside DevState and not per slot, as
 // TopkSets.
-struct Topk5min { unsigned long long *slots[2], *level[2]; TopkList list; unsigned long long *acc; };
-// the level table of each set (the scoring half is TOPK_HALF's)
-constexpr int TOPK5_LEVEL[2] = {CMS_5MIN, CMS_QRY_5MIN};
+// [2]: GYSK_FLAG_FLOW_TOPK_SLOW's slow set of the response level (with GYSK_FLAG_FLOW_QUERY_LEVEL), scored as the window's.
+struct Topk5min { unsigned long long *slots[TOPK_SETS], *level[TOPK_SETS]; TopkList list; unsigned long long *acc; };
+// the level table of each set (the score is topk_score's)
+constexpr int TOPK5_LEVEL[TOPK_SETS] = {CMS_5MIN, CMS_QRY_5MIN, CMS_RESP_5MIN};
 
 // the cells of one count-min table
 inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
@@ -310,6 +322,9 @@ struct MergeState
 	// finished merge with their bounds ([2][TOPK_SET_WORDS]). They share the window sets' union buffers.
 	uint32_t		topk5_off {0};
 	unsigned long long	*topk5_final {nullptr};
+	// GYSK_FLAG_FLOW_TOPK_SLOW: the rank's last-window slow set and, with its 300-s level, L with B_L ride from slab entry topks_off
+	// (topk_slab_entries(1 or 2)); the merged ones land as set [2] of topk_final and topk5_final, which then hold three sets.
+	uint32_t		topks_off {0};
 };
 
 } // namespace gysk
@@ -325,6 +340,7 @@ struct gysk_engine
 	gysk::FlowRespHist	fr {};				// GYSK_FLAG_FLOW_RESP_HIST (every pointer nullptr without)
 	gysk::TopkSets		topk {};			// GYSK_FLAG_FLOW_TOPK (every pointer nullptr without)
 	gysk::Topk5min		topk5 {};			// GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without)
+	std::atomic<bool>	fed {false};			// an event was handed in or gysk_flush ran (gysk_set_flow_slow refuses after)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
 	std::vector<void *>	hallocs;
@@ -460,11 +476,13 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 // The count-min point queries of the flow query ABI calls on table t: the engine's own (the batch of the events handed in runs first) or,
 // merged, the last merge's sum over the ranks. GYSK_ERR_NOTSUP when the engine does not hold t; `what` names the call.
 int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_est *out, const char *what);
-// GYSK_FLAG_FLOW_TOPK: the first min(n, K) flows of heaviest-flow set `which` (0: connections, 1: flow queries), best first, with their
-// estimates on its table: the engine's open (last_window = 0) or last set, or merged, the last finished merge's set on the summed table.
-// level (GYSK_FLAG_FLOW_TOPK_5MIN): the 300-s level set instead, on the level (merged: the summed level), last_window ignored. Flows with
-// a zero score are left out; *bound (if not nullptr) = the set's word 1.
-int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, gysk_flow_est *out, uint32_t *nout,
+// GYSK_FLAG_FLOW_TOPK: the first min(n, K) flows of heaviest-flow set `which` (0: connections, 1: flow queries, 2: slow responses), best
+// first, with their estimates on its table: the engine's open (last_window = 0) or last set, or merged, the last finished merge's set on
+// the summed table. level (GYSK_FLAG_FLOW_TOPK_5MIN): the 300-s level set instead, on the level (merged: the summed level), last_window
+// ignored. Flows with a zero score are left out; *bound (if not nullptr) = the set's word 1. Row: gysk_flow_est for sets 0 and 1,
+// gysk_flow_resp_est for set 2.
+template <typename Row>
+int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, Row *out, uint32_t *nout,
 		uint64_t *bound, const char *what);
 // the same on a flow response histogram table (CMS_RESP_*)
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what);

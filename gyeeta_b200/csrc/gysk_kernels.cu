@@ -392,10 +392,12 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // response flow table fr (cells fr_cms past the probe limit).
 // TOPK (GYSK_FLAG_FLOW_TOPK): the record that claims an entry of the connection or query flow table stores its flow key beside the entry,
 // and a record on the direct path appends it to the table's candidates (tk).
-template <bool QRY, bool RH, bool TOPK, typename HotTable>
+// SLOW (GYSK_FLAG_FLOW_TOPK_SLOW, only with RH and TOPK): a response sample in bucket b >= b_slow appends its flow key to the slow set's
+// candidates tk.list[2], once per record (the selection's key sort removes the repeats).
+template <bool QRY, bool RH, bool TOPK, bool SLOW, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
 		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr,
-		unsigned long long *fr_cms, const FlowTopk &tk)
+		unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
@@ -427,6 +429,7 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 				rinc = resp_hist_inc(b);
 				rpos = table_hash(rkey) & fr.mask;
 				rk = ld_cg_hint_u64(&fr.ent[rpos].key, pol_last);
+				if (SLOW && b >= b_slow) topk_append(tk.list[2], fk);
 			}
 			cell = r.slot;
 			kb = (int)(r.value >> 10);
@@ -847,9 +850,10 @@ __device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &appl
 // RH (GYSK_FLAG_FLOW_RESP_HIST, only with QRY): the same once more with the response flow table fr and the response histogram cells fr_cms.
 // TOPK (GYSK_FLAG_FLOW_TOPK): the TCP pass keeps the flow keys of the connection and query records (drain_tcp_recs), and the TASK pass's
 // sweeps append the key beside each applied entry to that table's candidates tk.
-template <bool TASK, bool QRY, bool RH, bool TOPK>
+// SLOW (GYSK_FLAG_FLOW_TOPK_SLOW, TCP pass only): the TCP pass also keeps the flow key of each response sample in bucket b_slow or above.
+template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk)
+		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk, uint32_t b_slow)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
@@ -928,7 +932,8 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs<QRY, RH, TOPK>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms, tk);
+			drain_tcp_recs<QRY, RH, TOPK, SLOW>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms, tk,
+					b_slow);
 		}
 	}
 
@@ -2256,16 +2261,12 @@ __global__ void query_flows_kernel(const unsigned long long *__restrict__ tbl, u
 	out[i].flow_key = key; out[i].count = cnt; out[i].kbytes = kb;
 }
 
-// GYSK_FLAG_FLOW_RESP_HIST: per key and bucket the minimum over rows of the 8-word cells, then the response percentiles of those counts by
-// the rule of the service summaries' p95_5s_resp_ms (hist_percentile of RESP_TIME_HASH: GY_HISTOGRAM::get_percentiles), the full sum as the
-// total
-__global__ void query_flow_resp_kernel(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, const unsigned long long *__restrict__ keys,
-		uint32_t n, gysk_flow_resp_est *__restrict__ out)
+// GYSK_FLAG_FLOW_RESP_HIST: the point estimate of a flow key on a response histogram table, per bucket b the minimum over rows of its
+// count (mn[15], word 7's high half, ends 0). The one definition of a flow's bucket counts: the point query, and the slow score of
+// GYSK_FLAG_FLOW_TOPK_SLOW (resp_slow_score) read it.
+__device__ __forceinline__ void resp_point(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, unsigned long long key,
+		uint32_t (&mn)[16])
 {
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	const unsigned long long key = keys[i];
-	uint32_t mn[16];
 #pragma unroll
 	for (int b = 0; b < 16; ++b) mn[b] = 0xFFFFFFFFu;
 	for (uint32_t r = 0; r < depth; ++r) {
@@ -2277,6 +2278,32 @@ __global__ void query_flow_resp_kernel(const unsigned long long *__restrict__ tb
 			mn[4 * w + 2] = min(mn[4 * w + 2], (uint32_t)v.y); mn[4 * w + 3] = min(mn[4 * w + 3], (uint32_t)(v.y >> 32));
 		}
 	}
+}
+
+// GYSK_FLAG_FLOW_TOPK_SLOW: a flow's slow score S, the sum of its bucket counts from b_slow (2..14) on, saturated at 2^32 - 1 so that it
+// fits a rank key's 32 score bits and stays monotone in every count
+__device__ __forceinline__ uint32_t resp_slow_score(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, unsigned long long key,
+		uint32_t b_slow)
+{
+	uint32_t mn[16];
+	resp_point(tbl, depth, log2w, key, mn);
+	unsigned long long s = 0;
+#pragma unroll
+	for (uint32_t b = 0; b < 15; ++b) if (b >= b_slow) s += mn[b];
+	return (uint32_t)min(s, 0xFFFFFFFFull);
+}
+
+// GYSK_FLAG_FLOW_RESP_HIST: per key and bucket the minimum over rows of the 8-word cells, then the response percentiles of those counts by
+// the rule of the service summaries' p95_5s_resp_ms (hist_percentile of RESP_TIME_HASH: GY_HISTOGRAM::get_percentiles), the full sum as the
+// total
+__global__ void query_flow_resp_kernel(const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, const unsigned long long *__restrict__ keys,
+		uint32_t n, gysk_flow_resp_est *__restrict__ out)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const unsigned long long key = keys[i];
+	uint32_t mn[16];
+	resp_point(tbl, depth, log2w, key, mn);
 	uint64_t counts[15], total = 0;
 #pragma unroll
 	for (int b = 0; b < 15; ++b) { counts[b] = mn[b]; total += mn[b]; out[i].counts[b] = mn[b]; }
@@ -2420,38 +2447,45 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
-template <bool TASK, bool QRY, bool RH, bool TOPK>
+template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW>
 static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
+		cudaStream_t s)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
 		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK>, WARPS * 32, smem_max);
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW>, WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY, RH, TOPK><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq, fq_cms,
-			fr, fr_cms, tk);
+	drain_kernel<TASK, QRY, RH, TOPK, SLOW><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq,
+			fq_cms, fr, fr_cms, tk, b_slow);
 }
 
+// b_slow: GYSK_FLAG_FLOW_TOPK_SLOW's first slow bucket when tk.list[2] is held (RH only); the TASK pass is the TOPK one either way
 template <bool QRY, bool RH>
 static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, cudaStream_t s)
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
+		cudaStream_t s)
 {
 	if (tk.list[0].keys) {
-		launch_drain_pass<false, QRY, RH, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
-		launch_drain_pass<true, QRY, RH, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
+		if constexpr (RH) {
+			if (tk.list[2].keys) launch_drain_pass<false, QRY, RH, true, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, s);
+			else launch_drain_pass<false, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		}
+		else launch_drain_pass<false, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		launch_drain_pass<true, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
 	}
 	else {
-		launch_drain_pass<false, QRY, RH, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
-		launch_drain_pass<true, QRY, RH, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, s);
+		launch_drain_pass<false, QRY, RH, false, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		launch_drain_pass<true, QRY, RH, false, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
 	}
 	return 2;
 }
@@ -2461,8 +2495,8 @@ static int launch_drain_passes(const DevState &st, const FlowTable &ft, const So
 // batch's events (the flows are fewer than the connection records), up to what tmp holds, so that a small batch sweeps a small table.
 // With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size, and
 // with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too.
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, const RecRegions &rr,
-		uint64_t n_events, cudaStream_t s)
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
+		const RecRegions &rr, uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
@@ -2471,12 +2505,12 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable none {nullptr, 0u};
-	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, s);
+	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, 0, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable fqt {fq.flow, n - 1u};
-	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, s);
+	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
-	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, s);
+	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, s);
 }
 
 static void os_set_attrs(int dev)
@@ -2691,6 +2725,20 @@ __global__ void __launch_bounds__(256) topk_score_kernel(const unsigned long lon
 	}
 }
 
+// GYSK_FLAG_FLOW_TOPK_SLOW: the same rank keys scored by the slow score on a response histogram table (a sibling, so that
+// topk_score_kernel keeps its code)
+__global__ void __launch_bounds__(256) topk_slow_score_kernel(const unsigned long long *__restrict__ keys, const unsigned long long *__restrict__ d_n,
+		const unsigned long long *__restrict__ tbl, uint32_t depth, uint32_t log2w, uint32_t b_slow, unsigned long long *__restrict__ rank)
+{
+	const uint64_t n = *d_n;
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+		const unsigned long long k = keys[i];
+		unsigned long long r = i;
+		if (i == 0 || keys[i - 1] != k) r |= ((unsigned long long)resp_slow_score(tbl, depth, log2w, k, b_slow) << 32) | (1ull << 31);
+		rank[n - 1 - i] = r;
+	}
+}
+
 // the K best of the sorted rank keys into set (word 0 its size, then the keys, 0 past the size): the distinct keys are a suffix
 __global__ void __launch_bounds__(256) topk_pick_kernel(const unsigned long long *__restrict__ rank, const unsigned long long *__restrict__ d_n,
 		const unsigned long long *__restrict__ keys, unsigned long long *__restrict__ set)
@@ -2706,7 +2754,7 @@ __global__ void __launch_bounds__(256) topk_pick_kernel(const unsigned long long
 }
 
 int launch_topk_select(const SortTemp &tmp, const TopkList &l, uint64_t n_max, const unsigned long long *tbl, uint32_t depth, uint32_t log2w,
-		int half, unsigned long long *set, bool reseed, cudaStream_t s)
+		int score, unsigned long long *set, bool reseed, cudaStream_t s)
 {
 	// three buffers of at least n_max keys: the candidates, and tmp's two; the key sort ping-pongs between the first two, the rank sort
 	// between the two the sorted keys leave free
@@ -2719,7 +2767,8 @@ int launch_topk_select(const SortTemp &tmp, const TopkList &l, uint64_t n_max, c
 	const unsigned long long *sorted = buf[which];
 	t.keys_a = buf[which ^ 1]; t.keys_b = buf[2];
 	const uint32_t grid = std::min<uint32_t>(div_up(n_max, 256), (uint32_t)sm_count(current_device()) * 8u);
-	topk_score_kernel<<<grid ? grid : 1, 256, 0, s>>>(sorted, l.n, tbl, depth, log2w, half, t.keys_a);
+	if (score & TOPK_SCORE_SLOW) topk_slow_score_kernel<<<grid ? grid : 1, 256, 0, s>>>(sorted, l.n, tbl, depth, log2w, score & 0xFF, t.keys_a);
+	else topk_score_kernel<<<grid ? grid : 1, 256, 0, s>>>(sorted, l.n, tbl, depth, log2w, score, t.keys_a);
 	const unsigned long long *ranked[2] = {t.keys_a, t.keys_b};
 	const int n2 = launch_radix_sort(t, l.n, n_max, 31, 64, &which, s);
 	if (n2 < 0) return -1;
@@ -2785,10 +2834,23 @@ __global__ void topk_bound_kernel(const unsigned long long *__restrict__ set, co
 	*out = sum ? thr + t : max(thr, t);
 }
 
-int launch_topk_bound(const unsigned long long *set, const unsigned long long *tbl, uint32_t depth, uint32_t log2w, int half,
+// GYSK_FLAG_FLOW_TOPK_SLOW: the same with thr(set) the slow score on a response histogram table (a sibling, so that topk_bound_kernel
+// keeps its code)
+__global__ void topk_slow_bound_kernel(const unsigned long long *__restrict__ set, const unsigned long long *__restrict__ tbl, uint32_t depth,
+		uint32_t log2w, uint32_t b_slow, const unsigned long long *terms, size_t stride, uint32_t nterms, uint32_t mask, int sum,
+		unsigned long long *out)
+{
+	unsigned long long t = 0;
+	const unsigned long long thr = set[0] >= TOPK_K ? resp_slow_score(tbl, depth, log2w, set[2 + TOPK_K - 1], b_slow) : 0;
+	for (uint32_t j = 0; j < nterms; ++j) if ((mask >> (j & 31u)) & 1u) t += terms[j * stride];
+	*out = sum ? thr + t : max(thr, t);
+}
+
+int launch_topk_bound(const unsigned long long *set, const unsigned long long *tbl, uint32_t depth, uint32_t log2w, int score,
 		const unsigned long long *terms, size_t stride, uint32_t nterms, uint32_t mask, bool sum, unsigned long long *out, cudaStream_t s)
 {
-	topk_bound_kernel<<<1, 1, 0, s>>>(set, tbl, depth, log2w, half, terms, stride, nterms, mask, sum ? 1 : 0, out);
+	if (score & TOPK_SCORE_SLOW) topk_slow_bound_kernel<<<1, 1, 0, s>>>(set, tbl, depth, log2w, score & 0xFF, terms, stride, nterms, mask, sum ? 1 : 0, out);
+	else topk_bound_kernel<<<1, 1, 0, s>>>(set, tbl, depth, log2w, score, terms, stride, nterms, mask, sum ? 1 : 0, out);
 	return 1;
 }
 

@@ -178,8 +178,13 @@ struct TopkList { unsigned long long *keys, *n, *ekeys; unsigned long long cap; 
 // a heaviest-flow set: [TOPK_SET_WORDS] u64, word 0 its size, word 1 zero (GYSK_FLAG_FLOW_TOPK_5MIN's sets: their bound), then the K
 // keys best first
 static constexpr uint32_t TOPK_K = GYSK_FLOW_TOPK_CAP, TOPK_SET_WORDS = TOPK_K + 2;
-// the held lists: [0] the connection table's, [1] the flow query table's
-struct FlowTopk { TopkList list[2]; };
+// the held lists: [0] the connection table's, [1] the flow query table's, [2] GYSK_FLAG_FLOW_TOPK_SLOW's (the response histogram table's,
+// fed only by the TCP pass's slow samples: ekeys nullptr)
+struct FlowTopk { TopkList list[3]; };
+// a set's score (launch_topk_select, launch_topk_bound): 0 / 1 the low / high half of a one-word-cell table (query_flows_kernel's
+// estimate); TOPK_SCORE_SLOW | b_slow the slow score of a response histogram table, the sum of its bucket counts from b_slow on
+// (GYSK_FLAG_FLOW_TOPK_SLOW, resp_slow_score)
+static constexpr int TOPK_SCORE_SLOW = 0x100;
 
 struct SortTemp
 {
@@ -265,23 +270,23 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 		uint32_t key_slots, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
 // fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms;
-// tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the passes gather each held table's candidates
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, const RecRegions &rr,
-		uint64_t n_events, cudaStream_t s);
+// tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the passes gather each held table's candidates; tk.list[2].keys != nullptr
+// (GYSK_FLAG_FLOW_TOPK_SLOW, with fr.cur): the TCP pass gathers the flow key of each response sample in bucket b_slow or above
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
+		const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // GYSK_FLAG_FLOW_TOPK, after the batch merge (it takes tmp's sort buffers, of at least n_max keys): the *l.n candidates (n_max >= *l.n)
-// sorted by key in l.keys, the distinct ones scored on table tbl (half = 0: the low half, 1: the high half of a cell, the estimate of
-// query_flows_kernel) and the K best by (score descending, key ascending) written to set; then, unless reseed is false, set back into
-// l as the next batch's first candidates. -1: no sort plan
+// sorted by key in l.keys, the distinct ones scored on table tbl (score as TOPK_SCORE_SLOW says) and the K best by (score descending,
+// key ascending) written to set; then, unless reseed is false, set back into l as the next batch's first candidates. -1: no sort plan
 int launch_topk_select(const SortTemp &tmp, const TopkList &l, uint64_t n_max, const unsigned long long *tbl, uint32_t depth, uint32_t log2w,
-		int half, unsigned long long *set, bool reseed, cudaStream_t s);
+		int score, unsigned long long *set, bool reseed, cudaStream_t s);
 // the merge's union into l (its count reset first): the keys of world sets, rank r's at sets + r * stride words
 int launch_topk_gather(const unsigned long long *sets, uint32_t world, size_t stride, const TopkList &l, cudaStream_t s);
 // GYSK_FLAG_FLOW_TOPK_5MIN: the keys of set j (at sets + j * stride words) appended to l for each bit j of mask (j < 32), l's count reset
 // first when reset is true
 int launch_topk_gather_mask(const unsigned long long *sets, size_t stride, uint32_t mask, const TopkList &l, bool reset, cudaStream_t s);
-// GYSK_FLAG_FLOW_TOPK_5MIN: a set's bound word. thr(set) is the score on tbl (half as launch_topk_select) of its K-th key when it holds K,
-// else 0; t the sum of terms[j * stride] over j < nterms with bit j % 32 of mask set. *out = sum ? thr + t : max(thr, t)
-int launch_topk_bound(const unsigned long long *set, const unsigned long long *tbl, uint32_t depth, uint32_t log2w, int half,
+// GYSK_FLAG_FLOW_TOPK_5MIN: a set's bound word. thr(set) is the score on tbl (score as launch_topk_select) of its K-th key when it holds
+// K, else 0; t the sum of terms[j * stride] over j < nterms with bit j % 32 of mask set. *out = sum ? thr + t : max(thr, t)
+int launch_topk_bound(const unsigned long long *set, const unsigned long long *tbl, uint32_t depth, uint32_t log2w, int score,
 		const unsigned long long *terms, size_t stride, uint32_t nterms, uint32_t mask, bool sum, unsigned long long *out, cudaStream_t s);
 // sorts tmp.keys_a on key bits [lo, hi); *which = 1: the result is in keys_b. -1: no sort plan for the range (more than 8 passes, or
 // bits outside [0, 64)), or n_max >= 2^30

@@ -899,18 +899,21 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// the trace digests after them, packed as TraceSlabs in whole SlabEntrys
 	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
 	// GYSK_FLAG_FLOW_TOPK: the rank's last-window heaviest-flow sets after everything else; GYSK_FLAG_FLOW_TOPK_5MIN: its level sets
-	// and their bounds after those
+	// and their bounds after those; GYSK_FLAG_FLOW_TOPK_SLOW: its last-window slow set, and with the slow level set L (and B_L) after
+	// those. The merged slow sets are set [2] of topk_final / topk5_final.
 	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK, topk5 = e->cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN;
+	const uint32_t nslow = e->topk.open[2] ? (e->topk5.level[2] ? 2 : 1) : 0;
 	mg.trace_off = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
 	mg.topk_off = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
 	mg.topk5_off = mg.topk_off + (topk ? TOPK_SLAB_ENTRIES : 0);
-	mg.slab_entries = mg.topk5_off + (topk5 ? TOPK_SLAB_ENTRIES : 0);
+	mg.topks_off = mg.topk5_off + (topk5 ? TOPK_SLAB_ENTRIES : 0);
+	mg.slab_entries = mg.topks_off + (nslow ? topk_slab_entries(nslow) : 0);
 	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
 	if (topk) {
-		if ((rc = dalloc(e, &mg.topk_final, 2 * (size_t)TOPK_SET_WORDS))) return rc;
+		if ((rc = dalloc(e, &mg.topk_final, (nslow ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
 		if ((rc = dalloc(e, &mg.topk_n, 1))) return rc;
 	}
-	if (topk5 && (rc = dalloc(e, &mg.topk5_final, 2 * (size_t)TOPK_SET_WORDS))) return rc;
+	if (topk5 && (rc = dalloc(e, &mg.topk5_final, (nslow == 2 ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
 	if (topn) {
 		if ((rc = dalloc(e, &mg.topn_slots, (size_t)TOPN_LISTS * TOPN_K))) return rc;
 		if ((rc = dalloc(e, &mg.topn_final, TopnLists::BYTES))) return rc;
@@ -1078,6 +1081,12 @@ int gysk_merge_prepare(gysk_engine *e)
 			else CU(e, cudaMemsetAsync(d, 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
 		}
 	}
+	if (e->topk.open[2]) {		// GYSK_FLAG_FLOW_TOPK_SLOW: the last-window slow set, then with the slow level its L and B_L
+		unsigned long long *dst = reinterpret_cast<unsigned long long *>(mg.lg.slab + mg.topks_off);
+		CU(e, cudaMemcpyAsync(dst, e->topk.last[2], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
+		if (e->topk5.level[2])
+			CU(e, cudaMemcpyAsync(dst + TOPK_SET_WORDS, e->topk5.level[2], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
+	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
 	return post_launch(e, "merge_prepare");
@@ -1141,27 +1150,32 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 		t.tile_status = mg.topk_tiles; t.max_tiles = (uint32_t)((mg.topk_cap + SORT_TILE - 1) / SORT_TILE);
 		const TopkList l {mg.topk_buf, mg.topk_n, nullptr, mg.topk_cap};
 		const size_t stride = (size_t)mg.slab_entries * sizeof(SlabEntry) / sizeof(unsigned long long);
-		for (int w = 0; w < 2; ++w) {
+		// the rank's window set w in the slab (the slow set in its own region)
+		auto slab_set = [&](int w, bool level) {
+			const unsigned long long *base = reinterpret_cast<const unsigned long long *>(src + (w < 2 ? (level ? mg.topk5_off : mg.topk_off) : mg.topks_off));
+			return base + (size_t)(w < 2 ? w : level ? 1 : 0) * TOPK_SET_WORDS;
+		};
+		for (int w = 0; w < TOPK_SETS; ++w) {
 			unsigned long long *set = mg.topk_final + (size_t)w * TOPK_SET_WORDS;
 			if (!e->topk.last[w]) continue;
-			e->kernel_launches += launch_topk_gather(reinterpret_cast<const unsigned long long *>(src + mg.topk_off) + (size_t)w * TOPK_SET_WORDS, world,
-					stride, l, e->stream);
-			const int k = launch_topk_select(t, l, need, mg.g_cms[TOPK_TABLE[w] + 1], e->cfg.cms_depth, e->cfg.cms_log2_width, TOPK_HALF[w], set, false,
-					e->stream);
+			e->kernel_launches += launch_topk_gather(slab_set(w, false), world, stride, l, e->stream);
+			const int k = launch_topk_select(t, l, need, mg.g_cms[TOPK_TABLE[w] + 1], e->cfg.cms_depth, e->cfg.cms_log2_width, topk_score(e->topk, w), set,
+					false, e->stream);
 			if (k < 0) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: heaviest-flow sort failed");
 			e->kernel_launches += k;
 		}
 		// GYSK_FLAG_FLOW_TOPK_5MIN: per held level the union of every rank's level set, the K best on the summed level, with
 		// B_G = max(thr(G), sum over ranks of B_L)
-		for (int w = 0; w < 2 && mg.topk5_final; ++w) {
+		for (int w = 0; w < TOPK_SETS && mg.topk5_final; ++w) {
 			unsigned long long *set = mg.topk5_final + (size_t)w * TOPK_SET_WORDS;
 			if (!e->topk5.level[w]) continue;
-			const unsigned long long *sets = reinterpret_cast<const unsigned long long *>(src + mg.topk5_off) + (size_t)w * TOPK_SET_WORDS;
+			const unsigned long long *sets = slab_set(w, true);
 			const unsigned long long *tbl = mg.g_cms[TOPK5_LEVEL[w]];
+			const int score = topk_score(e->topk, w);
 			e->kernel_launches += launch_topk_gather(sets, world, stride, l, e->stream);
-			const int k = launch_topk_select(t, l, need, tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, TOPK_HALF[w], set, false, e->stream);
+			const int k = launch_topk_select(t, l, need, tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, score, set, false, e->stream);
 			if (k < 0) return fail(e, GYSK_ERR_INVAL, "gysk_merge_finish: 300-s heaviest-flow sort failed");
-			e->kernel_launches += k + launch_topk_bound(set, tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, TOPK_HALF[w], sets + 1, stride, world, ~0u,
+			e->kernel_launches += k + launch_topk_bound(set, tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, score, sets + 1, stride, world, ~0u,
 					false, set + 1, e->stream);
 		}
 		mg.topk_done = true;
@@ -1478,6 +1492,17 @@ int gysk_topk_flows_global_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, 
 int gysk_topk_flow_queries_global_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound)
 {
 	return topk_read(e, 1, 0, true, true, n, reinterpret_cast<gysk_flow_est *>(out), nout, bound, "topk_flow_queries_global_5min");
+}
+
+// GYSK_FLAG_FLOW_TOPK_SLOW: the flows with the most slow responses over every rank, from the last finished merge
+int gysk_topk_flow_slow_global(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout)
+{
+	return topk_read(e, 2, 1, false, true, n, out, nout, nullptr, "topk_flow_slow_global");
+}
+
+int gysk_topk_flow_slow_global_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 2, 0, true, true, n, out, nout, bound, "topk_flow_slow_global_5min");
 }
 
 int gysk_topn_global(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, gysk_svc_summary *rows, uint32_t *nout)

@@ -43,6 +43,7 @@ FLAG_FLOW_QUERY_LEVEL = 0x100
 FLAG_FLOW_RESP_HIST = 0x200
 FLAG_FLOW_TOPK = 0x400
 FLAG_FLOW_TOPK_5MIN = 0x800
+FLAG_FLOW_TOPK_SLOW = 0x1000
 FLOW_TOPK_CAP = 4096
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
@@ -336,6 +337,11 @@ def load_library(path=None):
         "gysk_topk_flow_queries_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_topk_flows_global_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_topk_flow_queries_global_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_set_flow_slow": (i32, [vp, u32]),
+        "gysk_topk_flow_slow": (i32, [vp, i32, u32, vp, vp]),
+        "gysk_topk_flow_slow_global": (i32, [vp, u32, vp, vp]),
+        "gysk_topk_flow_slow_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_topk_flow_slow_global_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -402,7 +408,7 @@ class Engine:
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
                  max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False,
-                 flow_topk=False, flow_topk_5min=False):
+                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -418,7 +424,7 @@ class Engine:
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
                     (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
                     (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0) | \
-                    (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0)
+                    (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0) | (FLAG_FLOW_TOPK_SLOW if flow_topk_slow else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -773,6 +779,29 @@ class Engine:
     def topk_flow_queries_global_5min(self, n=FLOW_TOPK_CAP):
         """gysk_topk_flow_queries_global_5min: (rows, bound) over every rank's flow query level, from the last finished merge"""
         return self._topk_5min(self.L.gysk_topk_flow_queries_global_5min, FLOW_QRY_EST_DTYPE, n)
+
+    def set_flow_slow(self, above_ms):
+        """gysk_set_flow_slow: a counted response sample above above_ms msec (one of the 13 RESP_TIME_HASH thresholds) is slow; before
+        the first event or flush (flow_topk_slow=True; the default is 300)"""
+        self._chk(self.L.gysk_set_flow_slow(self.h, above_ms))
+
+    def topk_flow_slow(self, n=FLOW_TOPK_CAP, last_window=False):
+        """gysk_topk_flow_slow: the n flows with the most slow responses of the open or last window, each row its
+        query_flow_resp row (flow_topk_slow=True)"""
+        return self._topk(self.L.gysk_topk_flow_slow, FLOW_RESP_EST_DTYPE, n, int(last_window))
+
+    def topk_flow_slow_global(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_slow_global: the n flows with the most slow responses over every rank, from the last finished merge"""
+        return self._topk(self.L.gysk_topk_flow_slow_global, FLOW_RESP_EST_DTYPE, n)
+
+    def topk_flow_slow_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_slow_5min: (rows, bound) of the rolling 300-s response level by slow responses (flow_topk_slow=True,
+        flow_topk_5min=True, flow_query_level=True)"""
+        return self._topk_5min(self.L.gysk_topk_flow_slow_5min, FLOW_RESP_EST_DTYPE, n)
+
+    def topk_flow_slow_global_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_slow_global_5min: (rows, bound) over every rank's response level, from the last finished merge"""
+        return self._topk_5min(self.L.gysk_topk_flow_slow_global_5min, FLOW_RESP_EST_DTYPE, n)
 
     def topn(self, metric, n=10, host_idx=-1):
         out = (TopnEntry * n)()

@@ -262,6 +262,12 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   GYSK_FLAG_FLOW_LEVEL or GYSK_FLAG_FLOW_QUERY_LEVEL: gysk_create refuses it without.
 						   Without it nothing is allocated, every other call answers as before and the four calls
 						   are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_FLOW_TOPK_SLOW	0x1000u	/* the GYSK_FLOW_TOPK_CAP client flows with the most slow responses of each window and,
+						   with GYSK_FLAG_FLOW_TOPK_5MIN and GYSK_FLAG_FLOW_QUERY_LEVEL, of the rolling 300-s
+						   level, on each rank and across ranks (gysk_topk_flow_slow, "flows with the most slow
+						   responses" below). Needs GYSK_FLAG_FLOW_TOPK and GYSK_FLAG_FLOW_RESP_HIST: gysk_create
+						   refuses it without. Without it nothing is allocated, every other call answers as before
+						   and the five calls are GYSK_ERR_NOTSUP */
 
 typedef struct gysk_config
 {
@@ -762,7 +768,7 @@ int		gysk_query_flow_resp_global_5min(gysk_engine *e, const uint64_t *flow_keys,
  *   a zero score are left out, so *nout may be below n. gysk_topk_flow_queries: the same for the query table (GYSK_ERR_NOTSUP without
  *   GYSK_FLAG_FLOW_QUERIES). The _global pair: the merged lists of the last gysk_merge_finish, with their estimates on the summed tables
  *   (GYSK_ERR_INVAL before the first one). Every call is GYSK_ERR_NOTSUP without the flag.
- * Not covered: a set scored by the response histograms, per-(service, client) pairs, a configurable K. */
+ * Not covered: per-(service, client) pairs, a configurable K. */
 int		gysk_topk_flows(gysk_engine *e, int last_window, uint32_t n, gysk_flow_est *out, uint32_t *nout);
 int		gysk_topk_flow_queries(gysk_engine *e, int last_window, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout);
 int		gysk_topk_flows_global(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout);
@@ -795,6 +801,46 @@ int		gysk_topk_flows_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32
 int		gysk_topk_flow_queries_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound);
 int		gysk_topk_flows_global_5min(gysk_engine *e, uint32_t n, gysk_flow_est *out, uint32_t *nout, uint64_t *bound);
 int		gysk_topk_flow_queries_global_5min(gysk_engine *e, uint32_t n, gysk_flow_qry_est *out, uint32_t *nout, uint64_t *bound);
+
+/* ---- flows with the most slow responses (GYSK_FLAG_FLOW_TOPK_SLOW): which clients get the slow answers ----
+ * The heaviest-flow sets rank by volume, so a client with few requests, many of them slow, is never listed there; the flow response
+ * histograms answer only for a key the caller has. These sets name the clients behind a bad p99.
+ * A counted response sample (one the flow response histograms count) is slow when its msec is above the threshold T, one of the 13
+ * RESP_TIME_HASH thresholds (1, 10, 30, 60, 100, 150, 200, 300, 450, 700, 1000, 3000, 15000): exactly when its bucket
+ * gysk_hist_bucket(GYSK_CLS_RESP_TIME, msec) >= b_slow = 2 + the index of T. T defaults to 300 ms (b_slow = 9), a choice of this
+ * library: the reference has no per-client rule. gysk_set_flow_slow sets it before the engine takes its first event or gysk_flush;
+ * every rank of a merge must use the same T, as with the flags (a set or slot folded under two thresholds has no guarantee).
+ * Score of a flow on a response table (open, last, ring slot, level or merged sum): S = sum over b >= b_slow of counts[b], the
+ * per-bucket minimum over rows that gysk_query_flow_resp returns, saturated at 2^32 - 1. S is never below the flow's exact slow count,
+ * never above the minimum over rows of the row sums, and never falls within a window, so the guarantees below are those of the sets
+ * above, word for word (DESIGN.md section 2).
+ * Window sets: one open and one last set of K = GYSK_FLOW_TOPK_CAP keys on the response tables. After each device batch the open set
+ * becomes the K best of C u B_slow by (score descending, flow key ascending), scored on the table after the batch; B_slow is the
+ * distinct flow keys with at least one slow counted sample in the batch (GYSK_EV_TRACE samples never enter). gysk_flush moves the open
+ * set to the last one. Guarantee: if no cell half wraps, a flow whose exact slow count exceeds the smallest score of a full set is in
+ * it; a window of at most K slow flows has every one of them. A flow with only fast samples is never listed.
+ * 300-s level (with GYSK_FLAG_FLOW_TOPK_5MIN and GYSK_FLAG_FLOW_QUERY_LEVEL): slot sets, L, B_s and B_L by the rule of the 300-s heaviest-
+ * flow sets above, on the response ring slots and level, scored by S; every flow outside L has an exact 5-minute slow count of at most B_L.
+ * Across ranks: gysk_merge_prepare carries the last-window slow set, and with the level L and B_L, after the other heaviest-flow sets
+ * in the t-digest slab; gysk_merge_finish keeps the K best of the union on the summed response tables, with B_G = max(thr(G), sum over
+ * ranks of B_L) for the level. A flow whose exact global slow count exceeds the sum of the ranks' thresholds is in the window union.
+ * Cost: a candidate list of K + max_batch keys (8 B each) and the sets; each batch appends one key per slow sample in the TCP drain pass,
+ * then sorts, scores (each candidate reads its depth 64-byte cells) and ranks the candidates after the other sets' selections, in the
+ * same sort buffers. Measured on one H100 80GB HBM3 at 700 W, bench workload (100 M-event batches, few slow samples): about 0.2 ms more
+ * in the TCP pass and 0.2 ms of selection per batch, gysk_merge_finish +0.15 ms, gysk_flush unchanged, device_bytes +1.07 GB (the list
+ * at max_batch = 2^27). DESIGN.md section 7 has the measurements.
+ * gysk_set_flow_slow: GYSK_ERR_NOTSUP without the flag; GYSK_ERR_INVAL when above_ms is not one of the 13 thresholds, or once the
+ *   engine has taken an event or a gysk_flush (the engine is left unchanged).
+ * gysk_topk_flow_slow: the first min(n, K) flows of the open (last_window = 0) or last set, best first, each row byte-equal to what
+ *   gysk_query_flow_resp(last_window) answers for its key (so score == sum of out.counts[b] from b_slow on, saturated); entries with a
+ *   zero score are left out, so *nout may be below n. gysk_topk_flow_slow_5min: the same of L with *bound (may be NULL) = B_L, rows as
+ *   gysk_query_flow_resp_5min (GYSK_ERR_NOTSUP without the level). The _global pair: the same of the last gysk_merge_finish, rows as
+ *   gysk_query_flow_resp_global(1) / _global_5min, *bound = B_G (GYSK_ERR_INVAL before the first one). */
+int		gysk_set_flow_slow(gysk_engine *e, uint32_t above_ms);
+int		gysk_topk_flow_slow(gysk_engine *e, int last_window, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout);
+int		gysk_topk_flow_slow_global(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout);
+int		gysk_topk_flow_slow_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound);
+int		gysk_topk_flow_slow_global_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound);
 
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
