@@ -161,6 +161,15 @@ __host__ __device__ __forceinline__ unsigned long long fmix64(unsigned long long
 	return h;
 }
 
+// the register index and rank of the mixed hash h at precision p; one h serves several precisions (GYSK_FLAG_CLIENT_LEVELS)
+__device__ __forceinline__ void hll_idx_rank_h(unsigned long long h, uint32_t p, uint32_t &idx, uint32_t &rank)
+{
+	const unsigned long long w = h << p;
+
+	idx = (uint32_t)(h >> (64 - p));
+	rank = w ? (uint32_t)__clzll((long long)w) + 1u : (64u - p + 1u);
+}
+__device__ __forceinline__ unsigned long long hll_hash2(uint32_t h1, uint32_t h2) { return fmix64(((unsigned long long)h2 << 32) | h1); }
 __device__ __forceinline__ void hll_idx_rank2(uint32_t h1, uint32_t h2, uint32_t p, uint32_t &idx, uint32_t &rank)
 {
 	const unsigned long long h = fmix64(((unsigned long long)h2 << 32) | h1);

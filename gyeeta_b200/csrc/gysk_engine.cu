@@ -71,11 +71,11 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	RecRegions rr;
-	const int li = launch_ingest(e->st, e->tmp, e->fq, e->topk.tk, d_ev, n, key_slots(e), rr, e->stream);
+	const int li = launch_ingest(e->st, e->tmp, e->fq, e->topk.tk, e->cl, d_ev, n, key_slots(e), rr, e->stream);
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, e->topk.b_slow, rr, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, e->topk.b_slow, e->cl, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
@@ -450,6 +450,10 @@ int launch_rows(gysk_engine *e, const unsigned long long *, const unsigned long 
 {
 	return launch_day_stats(e->st, d_slots, m, reinterpret_cast<gysk_listener_day_stats *>(e->d_wstage), e->stream);
 }
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_clients *)
+{
+	return launch_client_rows(e->st, e->cl, d_ids, d_slots, m, reinterpret_cast<gysk_svc_clients *>(e->d_wstage), e->stream);
+}
 // The rolling levels at the flush of tsec: the closing window goes to ring slot (tsec / width) % NSLOTS of each level, and a slot
 // still holding an older epoch is cleared first (LevelRing::fresh records it). Then the live slots, whose epochs lie in the level's
 // last NSLOTS: what every reader of the levels sums until the next flush. The count-min rings (CMS_RINGS) take level 0's decision as
@@ -515,12 +519,13 @@ static int topk5_roll(gysk_engine *e, int w)
 // Every device array indexed by service or process slot, with its elements per slot: f(pointer, elements per slot, kind). Svc arrays
 // hold max_svcs + 1 slots (slot max_svcs is the null slot), the level ring max_svcs rows in each of its NLEVELS x NSLOTS planes
 // (LevelRing::stride), Task arrays max_tasks slots. gysk_create allocates exactly these, gysk_grow moves them, slot_bytes sums them.
-// The process eviction's arrays exist only with task_idle_evict_secs (task_evict). The batch's segment arrays (Seg) are indexed by the
-// slot field of the sort keys: max_svcs + 1 entries, and one more per trace row (max_trace_svcs) beyond the null slot.
+// The process eviction's arrays exist only with task_idle_evict_secs (task_evict), the client register sets only with
+// GYSK_FLAG_CLIENT_LEVELS (clients; their ring in NSLOTS planes of ClientLevels::stride rows). The batch's segment arrays (Seg) are
+// indexed by the slot field of the sort keys: max_svcs + 1 entries, and one more per trace row (max_trace_svcs) beyond the null slot.
 enum class SlotKind { Svc, Ring, Task, Seg };
 
 template <typename F>
-void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, bool task_evict, F f)
+void each_slot_array(DevState &st, SortTemp &tmp, ClientLevels &cl, uint32_t hll_p, bool task_evict, bool clients, F f)
 {
 	f(st.slot_id, 1, SlotKind::Svc); f(st.slot_host, 1, SlotKind::Svc);
 	f(st.slot_first_seen, 1, SlotKind::Svc); f(st.slot_last_active, 1, SlotKind::Svc);
@@ -540,15 +545,20 @@ void each_slot_array(DevState &st, SortTemp &tmp, uint32_t hll_p, bool task_evic
 		f(st.task_last_active, 1, SlotKind::Task); f(st.task_evict_list, 1, SlotKind::Task); f(st.task_evict_ids, 1, SlotKind::Task);
 		f(st.task_tbl.free_slots, 1, SlotKind::Task);
 	}
+	if (clients) {
+		f(cl.open, CL_REGS, SlotKind::Svc); f(cl.last, CL_REGS, SlotKind::Svc);
+		f(cl.ring, (size_t)NSLOTS * CL_REGS, SlotKind::Ring); f(cl.level, CL_REGS, SlotKind::Svc);
+	}
 }
 
 // device bytes of one service slot (its ring rows included) and of one process slot: the sums of each_slot_array
-void slot_bytes(uint32_t hll_p, bool task_evict, uint64_t *svc, uint64_t *task)
+void slot_bytes(uint32_t hll_p, bool task_evict, bool clients, uint64_t *svc, uint64_t *task)
 {
 	DevState st {};
 	SortTemp tmp {};
+	ClientLevels cl {};
 	uint64_t b[4] = {0, 0, 0, 0};
-	each_slot_array(st, tmp, hll_p, task_evict, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
+	each_slot_array(st, tmp, cl, hll_p, task_evict, clients, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
 	*svc = b[(int)SlotKind::Svc] + b[(int)SlotKind::Ring] + b[(int)SlotKind::Seg];
 	*task = b[(int)SlotKind::Task];
 }
@@ -578,6 +588,7 @@ bool trace_fits(uint32_t max_svcs, uint32_t max_trace) { return !max_trace || (u
 SvcRows finish_rows(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
 CopyRows<gysk_task_summary> finish_rows(const gysk_engine *, gysk_task_summary *out) { return CopyRows<gysk_task_summary> {out}; }
 CopyRows<gysk_listener_day_stats> finish_rows(const gysk_engine *, gysk_listener_day_stats *out) { return CopyRows<gysk_listener_day_stats> {out}; }
+ClientRows finish_rows(const gysk_engine *, gysk_svc_clients *out) { return ClientRows {out}; }
 
 } // namespace
 
@@ -588,6 +599,15 @@ void gysk::SvcRows::operator()(const uint8_t *rows, uint32_t off, uint32_t m) co
 	for (uint32_t i = 0; i < m; ++i) {
 		out[off + i] = r[i];
 		out[off + i].distinct_clients = hll_finish(r[i].distinct_clients, hll_p);
+	}
+}
+void gysk::ClientRows::operator()(const uint8_t *rows, uint32_t off, uint32_t m) const
+{
+	const gysk_svc_clients *r = reinterpret_cast<const gysk_svc_clients *>(rows);
+	for (uint32_t i = 0; i < m; ++i) {
+		out[off + i] = r[i];
+		out[off + i].last_5s = hll_finish(r[i].last_5s, GYSK_HLL_WINDOW_P);
+		out[off + i].last_5min = hll_finish(r[i].last_5min, GYSK_HLL_WINDOW_P);
 	}
 }
 
@@ -717,9 +737,12 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &st.task_tbl.count, 1));
 	if (cfg.task_idle_evict_secs) A(dalloc(e, &st.task_tbl.free_n, 1));		// without it the process table has no free stack
 	SortTemp &tmp = e->tmp;
-	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) { if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs) * k); });
+	each_slot_array(st, tmp, e->cl, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, [&](auto *&p, size_t k, SlotKind kind) {
+		if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs) * k);
+	});
 	if (rc) return bail(rc);
 	st.levels.stride = cfg.max_svcs;
+	if (e->cl.open) e->cl.stride = cfg.max_svcs;
 	st.svc_tbl.slot_id = st.slot_id; st.svc_tbl.slot_host = st.slot_host;
 	st.task_tbl.slot_id = st.task_slot_id; st.task_tbl.slot_host = st.task_slot_host;
 	A(halloc(e, &e->h_evict, ns + 2));
@@ -1466,22 +1489,21 @@ int regrow(gysk_engine *e, T *&p, size_t old_n, size_t new_n)
 	return 0;
 }
 
-// The level ring [NLEVELS][NSLOTS][stride][16] at the stride new_ms: each of its NLEVELS x NSLOTS planes (stride rows, contiguous)
-// moves with one copy to the head of its new plane, the rows behind it zeroed. The source pitch is the ring's own stride, which an
-// earlier growth that stopped half way may already have raised.
-int regrow_ring(gysk_engine *e, uint32_t new_ms)
+// A ring [planes][stride][row] (the level ring: NLEVELS x NSLOTS planes of 16 cells a row; GYSK_FLAG_CLIENT_LEVELS' ring: NSLOTS planes
+// of CL_REGS registers) at the stride new_ms: each plane (stride rows, contiguous) moves with one copy to the head of its new plane, the
+// rows behind it zeroed. The source pitch is the ring's own stride, which an earlier growth that stopped half way may already have raised.
+template <typename T>
+int regrow_ring(gysk_engine *e, T *&ring, uint32_t &stride, size_t planes, size_t row, uint32_t new_ms)
 {
-	LevelRing &lv = e->st.levels;
-	if (lv.stride >= new_ms) return 0;
-	const size_t row = (size_t)HIST_CELLS * sizeof(HistCell), planes = (size_t)NLEVELS * NSLOTS;
-	HistCell *q = nullptr;
-	if (int rc = dalloc(e, &q, planes * new_ms * HIST_CELLS)) return rc;
+	if (stride >= new_ms) return 0;
+	T *q = nullptr;
+	if (int rc = dalloc(e, &q, planes * new_ms * row)) return rc;
 	for (size_t k = 0; k < planes; ++k)
-		CU(e, cudaMemcpyAsync(q + k * new_ms * HIST_CELLS, lv.ring + k * lv.stride * HIST_CELLS, lv.stride * row, cudaMemcpyDeviceToDevice, e->stream));
+		CU(e, cudaMemcpyAsync(q + k * new_ms * row, ring + k * stride * row, stride * row * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
-	dfree(e, lv.ring);
-	lv.ring = q;
-	lv.stride = new_ms;
+	dfree(e, ring);
+	ring = q;
+	stride = new_ms;
 	return 0;
 }
 
@@ -1494,6 +1516,7 @@ void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, siz
 	to.max_svcs = ms; to.max_tasks = mt;
 	DevState st {};
 	SortTemp tmp {};
+	ClientLevels cl {};
 	size_t a = 0, big = 0, n = 0;
 	auto move = [&](size_t elem, size_t old_n, size_t new_n) {
 		if (new_n <= old_n) return;
@@ -1501,7 +1524,7 @@ void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, siz
 		big = std::max(big, old_n * elem);
 		n++;
 	};
-	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, cl, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, [&](auto *&p, size_t k, SlotKind kind) {
 		move(k * sizeof(*p), slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs), slots_of(kind, ms, mt, cfg.max_trace_svcs));
 	});
 	if (cfg.max_trace_svcs) move(sizeof(uint32_t), (size_t)cfg.max_svcs + 1, (size_t)ms + 1);		// TraceTable::row_of
@@ -1540,9 +1563,13 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 	to.max_svcs = ms; to.max_tasks = mt;
 	int rc = 0;
 	// phase 1
-	each_slot_array(st, tmp, cfg.hll_p, cfg.task_idle_evict_secs, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, e->cl, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, [&](auto *&p, size_t k, SlotKind kind) {
 		if (rc) return;
-		if (kind == SlotKind::Ring) rc = regrow_ring(e, ms);
+		if (kind == SlotKind::Ring) {
+			if constexpr (std::is_same<std::remove_reference_t<decltype(*p)>, HistCell>::value)
+				rc = regrow_ring(e, p, st.levels.stride, (size_t)NLEVELS * NSLOTS, HIST_CELLS, ms);
+			else rc = regrow_ring(e, p, e->cl.stride, NSLOTS, CL_REGS, ms);
+		}
 		else rc = regrow(e, p, slots_of(kind, os, ot, cfg.max_trace_svcs) * k, slots_of(kind, ms, mt, cfg.max_trace_svcs) * k);
 		link_tables(st);
 	});
@@ -1675,7 +1702,7 @@ int gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *
 		c = *cfg;
 	}
 	if (c.hll_p < 4 || c.hll_p > 16) return GYSK_ERR_INVAL;
-	slot_bytes(c.hll_p, c.task_idle_evict_secs != 0, svc_slot_bytes, task_slot_bytes);
+	slot_bytes(c.hll_p, c.task_idle_evict_secs != 0, (c.flags & GYSK_FLAG_CLIENT_LEVELS) != 0, svc_slot_bytes, task_slot_bytes);
 	return GYSK_OK;
 }
 
@@ -1700,7 +1727,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->kernel_launches += launch_rebuild_table(e->st.task_tbl, e->cfg.max_tasks, e->stream);
 		e->task_tombstones = 0;
 	}
-	e->kernel_launches += launch_flush(e->st, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
+	e->kernel_launches += launch_flush(e->st, e->cl, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
 	e->kernel_launches += launch_task_flush(e->st, e->cfg.max_tasks, tsec, e->cfg.task_idle_evict_secs, e->d_tevict, e->stream);
 	if (e->st.trace.rows) {
 		// trace rows: the open window closes, the other half (the window before it) is cleared and opens
@@ -1731,6 +1758,13 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		if (!cms_held(e->cfg, r.level)) continue;
 		e->kernel_launches += launch_cms_level_roll(CMS_TABLES[r.open].live(e), r.ring(e), CMS_TABLES[r.level].live(e), cms_words(e->cfg, r.open),
 				e->st.levels, e->stream);
+	}
+	if (e->cl.open) {
+		// GYSK_FLAG_CLIENT_LEVELS (the evicted slots' sets were cleared by launch_flush): the closing window into the ring and the level over
+		// the capacity, then the window swap
+		e->kernel_launches += launch_client_roll(e->cl, e->cfg.max_svcs, e->st.levels, e->stream);
+		std::swap(e->cl.open, e->cl.last);
+		CU(e, cudaMemsetAsync(e->cl.open, 0, ((size_t)e->cfg.max_svcs + 1) * CL_REGS, e->stream));
 	}
 	for (int w = 0; w < TOPK_SETS; ++w) {		// GYSK_FLAG_FLOW_TOPK_5MIN: each level set follows its ring, before the window sets swap
 		if (!e->topk5.level[w]) continue;
@@ -2020,6 +2054,38 @@ int gysk_export_hll(gysk_engine *e, uint64_t id, uint8_t *regs)
 	if (rc) return rc;
 	if (!*reinterpret_cast<const int32_t *>(e->h_wstage)) return GYSK_ERR_NOENT;
 	memcpy(regs, e->h_wstage + HLL_STAGE_REGS, (size_t)1 << e->cfg.hll_p);
+	return GYSK_OK;
+}
+
+// GYSK_FLAG_CLIENT_LEVELS: the rows of n ids, and of the services of a window read, as of the last flush
+int gysk_query_svc_clients(gysk_engine *e, const uint64_t *ids, uint32_t n, gysk_svc_clients *out)
+{
+	CHECK_ENGINE(e);
+	if (!(e->cfg.flags & GYSK_FLAG_CLIENT_LEVELS)) return GYSK_ERR_NOTSUP;
+	return query_rows(e, ids, n, out, "client_rows");
+}
+
+int gysk_query_clients_window(gysk_engine *e, int32_t host_idx, uint32_t flags, gysk_svc_clients *out, uint32_t *hosts, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!(e->cfg.flags & GYSK_FLAG_CLIENT_LEVELS)) return GYSK_ERR_NOTSUP;
+	return window_rows(e, host_idx, flags, out, hosts, cap, n, "clients_window");
+}
+
+// the last-window or 300-s client registers of one id, with the contract of gysk_export_hll
+int gysk_export_hll_window(gysk_engine *e, uint64_t id, int which, uint8_t *regs)
+{
+	CHECK_ENGINE(e);
+	if (!regs || (which != GYSK_CLIENTS_LAST && which != GYSK_CLIENTS_5MIN)) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_CLIENT_LEVELS)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Submit);
+	int rc = stage_one(e, id, HLL_STAGE_REGS + CL_REGS, "gather_hll_window", [&](const unsigned long long *d_ids, uint32_t, uint32_t) {
+		return launch_gather_hll_window(e->st, which == GYSK_CLIENTS_LAST ? e->cl.last : e->cl.level, d_ids, reinterpret_cast<int32_t *>(e->d_wstage),
+				e->d_wstage + HLL_STAGE_REGS, e->stream);
+	});
+	if (rc) return rc;
+	if (!*reinterpret_cast<const int32_t *>(e->h_wstage)) return GYSK_ERR_NOENT;
+	memcpy(regs, e->h_wstage + HLL_STAGE_REGS, CL_REGS);
 	return GYSK_OK;
 }
 

@@ -325,6 +325,10 @@ struct MergeState
 	// GYSK_FLAG_FLOW_TOPK_SLOW: the rank's last-window slow set and, with its 300-s level, L with B_L ride from slab entry topks_off
 	// (topk_slab_entries(1 or 2)); the merged ones land as set [2] of topk_final and topk5_final, which then hold three sets.
 	uint32_t		topks_off {0};
+	// GYSK_FLAG_CLIENT_LEVELS: MAX [nl][2][CL_REGS] in the u8 MAX region after the all-time registers, each logical service's last-window
+	// and 300-s client sets (nullptr without)
+	uint8_t			*cl_hll {nullptr};
+	__host__ __device__ __forceinline__ uint8_t *cl_of(uint32_t l, int which) const { return cl_hll + ((size_t)l * 2 + which) * CL_REGS; }
 };
 
 } // namespace gysk
@@ -340,6 +344,7 @@ struct gysk_engine
 	gysk::FlowRespHist	fr {};				// GYSK_FLAG_FLOW_RESP_HIST (every pointer nullptr without)
 	gysk::TopkSets		topk {};			// GYSK_FLAG_FLOW_TOPK (every pointer nullptr without)
 	gysk::Topk5min		topk5 {};			// GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without)
+	gysk::ClientLevels	cl {};				// GYSK_FLAG_CLIENT_LEVELS (every pointer nullptr without)
 	std::atomic<bool>	fed {false};			// an event was handed in or gysk_flush ran (gysk_set_flow_slow refuses after)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
@@ -583,6 +588,7 @@ static_assert(HLL_STAGE_REGS + (1u << 16) <= STAGE_BYTES, "the stage holds the f
 static_assert(QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES && 64 * sizeof(gysk_topn_entry) <= STAGE_BYTES, "the stage holds the flow and top-N rows");
 static_assert(sizeof(SlabEntry) <= STAGE_BYTES, "the stage holds one merged digest");
 static_assert(sizeof(gysk_logical_state) == 80 && sizeof(gysk_logical_state) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS state rows");
+static_assert(sizeof(gysk_svc_clients) == 32 && sizeof(gysk_svc_clients) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS client rows");
 static_assert(sizeof(gysk_cluster_row) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS cluster rows");
 static_assert(sizeof(gysk_logical_trace) == 168 && sizeof(gysk_logical_trace) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS logical trace rows");
 static_assert(sizeof(TraceSlab) <= STAGE_BYTES, "the stage holds one merged trace digest");
@@ -625,5 +631,11 @@ struct SvcRows
 	void operator()(const uint8_t *rows, uint32_t off, uint32_t m) const;
 };
 struct RowsStay { void operator()(const uint8_t *, uint32_t, uint32_t) const {} };
+// client rows (GYSK_FLAG_CLIENT_LEVELS), whose two estimates the host finishes (hll_finish at GYSK_HLL_WINDOW_P)
+struct ClientRows
+{
+	gysk_svc_clients *out;
+	void operator()(const uint8_t *rows, uint32_t off, uint32_t m) const;
+};
 
 } // namespace gysk

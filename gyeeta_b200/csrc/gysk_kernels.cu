@@ -129,6 +129,22 @@ struct SvcSlotReset
 	}
 };
 struct TaskSlotReset { __device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const { task_slot_reset(st, slot, t, nt); } };
+// GYSK_FLAG_CLIENT_LEVELS: the service's reset and its 2 + NSLOTS + 1 client sets zeroed, so that a recycled slot starts from zero as its
+// all-time registers do
+struct SvcClientSlotReset
+{
+	ClientLevels cl;
+	__device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const
+	{
+		constexpr uint32_t Q = CL_REGS / 16;
+		for (uint32_t i = t; i < (3u + NSLOTS) * Q; i += nt) {
+			const uint32_t set = i / Q, q = i % Q;
+			uint8_t *base = set == 0 ? cl.open : set == 1 ? cl.last : set == 2 ? cl.level : cl.ring + (size_t)(set - 3) * cl.stride * CL_REGS;
+			reinterpret_cast<uint4 *>(base + (size_t)slot * CL_REGS)[q] = make_uint4(0, 0, 0, 0);
+		}
+		SvcSlotReset {}(st, slot, t, nt);
+	}
+};
 
 // service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state: one CTA per service slot, one thread per
 // process slot (grid-stride): gysk_create over every slot, gysk_grow over the new ones
@@ -394,15 +410,18 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // and a record on the direct path appends it to the table's candidates (tk).
 // SLOW (GYSK_FLAG_FLOW_TOPK_SLOW, only with RH and TOPK): a response sample in bucket b >= b_slow appends its flow key to the slow set's
 // candidates tk.list[2], once per record (the selection's key sort removes the repeats).
-template <bool QRY, bool RH, bool TOPK, bool SLOW, typename HotTable>
+// CL (GYSK_FLAG_CLIENT_LEVELS): a connection record also raises the open window's client register (cl_open, precision GYSK_HLL_WINDOW_P),
+// from the same mixed hash; its word is asked for beside the all-time one and taken with the same policy.
+template <bool QRY, bool RH, bool TOPK, bool SLOW, bool CL, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
 		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr,
-		unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow)
+		unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow, uint8_t *cl_open)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
 		bool qry = false;
 		uint32_t cell = 0, idx = 0, rank = 0, hw = 0, pos = 0, rpos = 0; int kb = 0;
+		uint32_t widx = 0, wrank = 0, ww = 0;
 		unsigned long long key = 0, inc = 0, k = 0, rkey = 0, rk = 0, rinc = 0, fk = 0;
 		if (act) {
 			const IngestRec r = ld_rec(q + i);
@@ -415,8 +434,14 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 			// the HLL register word and the flow table's first probe are asked for together and looked at after the cell update, which
 			// hides their latency (a stale register is harmless: the CAS re-validates)
 			if (!qry) {
-				hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
+				if (CL) {
+					const unsigned long long h = hll_hash2(h1, h2);
+					hll_idx_rank_h(h, st.hll_p, idx, rank);
+					hll_idx_rank_h(h, GYSK_HLL_WINDOW_P, widx, wrank);
+				}
+				else hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
 				hw = ld_na_hint_u32(reinterpret_cast<const uint32_t *>(st.hll + ((size_t)r.slot << st.hll_p)) + (idx >> 2), pol_hll);
+				if (CL) ww = ld_na_hint_u32(reinterpret_cast<const uint32_t *>(cl_open + (size_t)r.slot * CL_REGS) + (widx >> 2), pol_hll);
 			}
 			key = ((unsigned long long)h2 << 32) | h1;
 			// usec -> msec as the histogram takes it (ingest_kernel)
@@ -445,6 +470,7 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 			if (RH && qry) flow_add(st, fr, RespHistApply {st, fr_cms}, CTR_FLOWR_DIRECT, rkey, rpos, rk, rinc, pol_last);
 		}
 		if (act && !qry) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
+		if (CL && act && !qry) hll_raise(cl_open + (size_t)cell * CL_REGS, widx, wrank, ww);
 	}
 }
 
@@ -554,10 +580,16 @@ struct IngestShared
 // hot-row route, also joins the connection queue as a record {QRY_REC, usec, flow key} for the TCP drain pass.
 // TOPK: GYSK_FLAG_FLOW_TOPK (a separate instance too): the flow key of each ACTIVE record, which updates the count-min here, joins the
 // connection table's candidates tl.
-template <bool TRACE, bool QRY, bool TOPK>
+// ClOpen: GYSK_FLAG_CLIENT_LEVELS (a separate instance too) with one uint8_t * parameter, the open window's client registers, which each
+// ACTIVE record also raises. A pack, so that the instances without the flag keep their parameter list.
+__device__ __forceinline__ uint8_t *cl_open_of() { return nullptr; }
+__device__ __forceinline__ uint8_t *cl_open_of(uint8_t *p) { return p; }
+template <bool TRACE, bool QRY, bool TOPK, typename... ClOpen>
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
-		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, TopkList tl)
+		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, TopkList tl,
+		ClOpen... cl_open)
 {
+	constexpr bool CL = sizeof...(ClOpen) > 0;
 	constexpr int WARPS = IngestShape::WARPS, EPT = IngestShape::EPT, CHUNK = IngestShape::CHUNK, DH = IngestShared::DH;
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	IngestShared &S = *reinterpret_cast<IngestShared *>(smem_raw);
@@ -745,6 +777,10 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					if (TOPK) topk_append(tl, fk);
 					hll_idx_rank2(h1, h2, st.hll_p, idx, rank);
 					hll_update(st.hll + ((size_t)slot << st.hll_p), idx, rank);
+					if constexpr (CL) {		// ACTIVE records are few: the hash is mixed once more rather than kept across the all-time update
+						hll_idx_rank_h(hll_hash2(h1, h2), GYSK_HLL_WINDOW_P, idx, rank);
+						hll_update(cl_open_of(cl_open...) + (size_t)slot * CL_REGS, idx, rank);
+					}
 					red_add_u64(&st.slot_aux[slot].act_cur, inc);
 					atomicMax(&st.slot_aux[slot].rtt_cur, rb[k].z);		// non-negative floats order like their bit patterns
 					n_active++;
@@ -851,9 +887,10 @@ __device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &appl
 // TOPK (GYSK_FLAG_FLOW_TOPK): the TCP pass keeps the flow keys of the connection and query records (drain_tcp_recs), and the TASK pass's
 // sweeps append the key beside each applied entry to that table's candidates tk.
 // SLOW (GYSK_FLAG_FLOW_TOPK_SLOW, TCP pass only): the TCP pass also keeps the flow key of each response sample in bucket b_slow or above.
-template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW>
+// CL (GYSK_FLAG_CLIENT_LEVELS, TCP pass only): the TCP pass also raises the open window's client registers cl_open.
+template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk, uint32_t b_slow)
+		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk, uint32_t b_slow, uint8_t *cl_open)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
@@ -932,8 +969,8 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs<QRY, RH, TOPK, SLOW>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms, tk,
-					b_slow);
+			drain_tcp_recs<QRY, RH, TOPK, SLOW, CL>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms,
+					tk, b_slow, cl_open);
 		}
 	}
 
@@ -2228,14 +2265,20 @@ __global__ void __launch_bounds__(128) gather_tasks_kernel(DevState st, const un
 	for (int i = lane; i < 3 * HIST_CELLS; i += 32) (&out[q].h[0][0])[i] = st.task_hist[(size_t)r.slot * 3 * HIST_CELLS + i];
 }
 
-// gysk_export_hll: the registers of one id (ids[0]); every warp resolves the id itself
-__global__ void gather_hll_kernel(DevState st, const unsigned long long *__restrict__ ids, int32_t *found, uint8_t *__restrict__ out)
+// gysk_export_hll: the registers of one id (ids[0]); every warp resolves the id itself. With a Set parameter, set (gysk_export_hll_window,
+// GYSK_FLAG_CLIENT_LEVELS): the CL_REGS registers of the id's slot in that client set instead of its all-time ones. A pack, so that the
+// all-time instance keeps its parameter list.
+__device__ __forceinline__ const uint8_t *hll_regs_of(const DevState &st, int slot) { return st.hll + ((size_t)slot << st.hll_p); }
+__device__ __forceinline__ const uint8_t *hll_regs_of(const DevState &, int slot, const uint8_t *set) { return set + (size_t)slot * CL_REGS; }
+template <typename... Set>
+__global__ void gather_hll_kernel(DevState st, const unsigned long long *__restrict__ ids, int32_t *found, uint8_t *__restrict__ out, Set... set)
 {
 	const int slot = resolve_warp(st.svc_tbl, ids, nullptr, 0, threadIdx.x & 31).slot;
 	if (threadIdx.x == 0) *found = slot >= 0;
 	if (slot < 0) return;
-	const uint8_t *regs = st.hll + ((size_t)slot << st.hll_p);
-	for (uint32_t i = threadIdx.x; i < (1u << st.hll_p); i += blockDim.x) out[i] = regs[i];
+	const uint8_t *regs = hll_regs_of(st, slot, set...);
+	const uint32_t nregs = sizeof...(Set) ? CL_REGS : 1u << st.hll_p;
+	for (uint32_t i = threadIdx.x; i < nregs; i += blockDim.x) out[i] = regs[i];
 }
 
 // the point estimate of a flow key on a count-min of one u64 per cell: the minimum over rows of each half
@@ -2340,6 +2383,59 @@ __global__ void __launch_bounds__(256) cms_level_roll_kernel(const ulonglong2 *_
 	}
 }
 
+__device__ __forceinline__ uint4 vmax4(uint4 a, uint4 b) { return make_uint4(__vmaxu4(a.x, b.x), __vmaxu4(a.y, b.y), __vmaxu4(a.z, b.z), __vmaxu4(a.w, b.w)); }
+
+// GYSK_FLAG_CLIENT_LEVELS at a flush: one grid-stride pass over the registers of service slots [0, nslots) in 16-byte pieces. Ring slot
+// k takes the closing window's open set, max-merged into what it holds or, when the flush started a new epoch there, in its place
+// (which stands in for clearing the slot); the level becomes the registerwise maximum of the live slots, slot k's new content included:
+// the rule of cms_level_roll_kernel with max for +. nslots is the engine's capacity, which every client array holds; cl.stride is only
+// the ring planes' pitch (a growth that stopped half way may have raised it alone). The ring and the level are streamed (evict-first).
+__global__ void __launch_bounds__(256) client_roll_kernel(ClientLevels cl, uint32_t nslots, uint32_t k, uint32_t live, uint32_t fresh)
+{
+	constexpr uint32_t Q = CL_REGS / 16;
+	const uint64_t npiece = (uint64_t)nslots * Q, plane = (uint64_t)cl.stride * Q;
+	const uint4 *open = reinterpret_cast<const uint4 *>(cl.open);
+	uint4 *ring = reinterpret_cast<uint4 *>(cl.ring), *level = reinterpret_cast<uint4 *>(cl.level);
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < npiece; i += (uint64_t)gridDim.x * blockDim.x) {
+		uint4 r = open[i];
+		if (!fresh) r = vmax4(r, __ldcs(ring + k * plane + i));
+		__stcs(ring + k * plane + i, r);
+		uint4 a = make_uint4(0, 0, 0, 0);
+#pragma unroll
+		for (uint32_t j = 0; j < NSLOTS; ++j) {
+			if (!((live >> j) & 1u)) continue;
+			a = vmax4(a, j == k ? r : __ldcs(ring + j * plane + i));
+		}
+		__stcs(level + i, a);
+	}
+}
+
+// gysk_query_svc_clients / gysk_query_clients_window: one warp per service, by id (ids != nullptr: looked up, id 0 and unknown ids give
+// found = 0) or by slot (the window read): the register histograms of the last and the level sets, each estimate as hll_pending leaves it
+// (the host finishes it with hll_finish at GYSK_HLL_WINDOW_P)
+static constexpr int CL_WARPS = 4;
+__global__ void __launch_bounds__(CL_WARPS * 32) client_rows_kernel(DevState st, ClientLevels cl, const unsigned long long *__restrict__ ids,
+		const unsigned long long *__restrict__ slots, uint32_t n, gysk_svc_clients *__restrict__ out)
+{
+	__shared__ uint32_t hist[CL_WARPS][2][64];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t q = blockIdx.x * CL_WARPS + wid;
+
+	if (q >= n) return;
+	const Resolved s = resolve_warp(st.svc_tbl, ids, slots, q, lane);
+	gysk_svc_clients o;
+	memset(&o, 0, sizeof(o));
+	o.glob_id = s.id;
+	if (s.slot >= 0) {
+		hll_hist_warp(cl.last + (size_t)s.slot * CL_REGS, GYSK_HLL_WINDOW_P, hist[wid][0], lane);
+		hll_hist_warp(cl.level + (size_t)s.slot * CL_REGS, GYSK_HLL_WINDOW_P, hist[wid][1], lane);
+		o.found = 1;
+		o.last_5s = hll_pending(hist[wid][0], GYSK_HLL_WINDOW_P);
+		o.last_5min = hll_pending(hist[wid][1], GYSK_HLL_WINDOW_P);
+	}
+	if (lane == 0) out[q] = o;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------
@@ -2398,8 +2494,8 @@ static int plain_sort_plan(int lo, int hi, SortPlan &P)
 	return 0;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const gysk_event *d_ev, uint64_t n,
-		uint32_t key_slots, RecRegions &rr, cudaStream_t s)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, const gysk_event *d_ev,
+		uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
 	const int dev = current_device();
@@ -2413,13 +2509,19 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
 	static bool attr_set[MAX_DEVICES] = {};
 	using IngestFn = void (*)(DevState, const gysk_event *, uint64_t, unsigned long long *, uint32_t *, SortPlan, uint4 *, uint2 *, TopkList);
-	// [TRACE][QRY][TOPK]
+	using IngestClFn = void (*)(DevState, const gysk_event *, uint64_t, unsigned long long *, uint32_t *, SortPlan, uint4 *, uint2 *, TopkList, uint8_t *);
+	// [TRACE][QRY][TOPK]; fns_cl: the instances of GYSK_FLAG_CLIENT_LEVELS
 	static const IngestFn fns[2][2][2] = {
 		{{ingest_kernel<false, false, false>, ingest_kernel<false, false, true>}, {ingest_kernel<false, true, false>, ingest_kernel<false, true, true>}},
 		{{ingest_kernel<true, false, false>, ingest_kernel<true, false, true>}, {ingest_kernel<true, true, false>, ingest_kernel<true, true, true>}}};
-	// the instances of GYSK_FLAG_FLOW_TOPK only once an engine with it launches: setting a kernel's attribute loads it, which can wait for
-	// the work already on the device
-	static bool topk_attr_set[MAX_DEVICES] = {};
+	static const IngestClFn fns_cl[2][2][2] = {
+		{{ingest_kernel<false, false, false, uint8_t *>, ingest_kernel<false, false, true, uint8_t *>},
+		 {ingest_kernel<false, true, false, uint8_t *>, ingest_kernel<false, true, true, uint8_t *>}},
+		{{ingest_kernel<true, false, false, uint8_t *>, ingest_kernel<true, false, true, uint8_t *>},
+		 {ingest_kernel<true, true, false, uint8_t *>, ingest_kernel<true, true, true, uint8_t *>}}};
+	// the instances of GYSK_FLAG_FLOW_TOPK and GYSK_FLAG_CLIENT_LEVELS only once an engine with the flag launches: setting a kernel's
+	// attribute loads it, which can wait for the work already on the device
+	static bool topk_attr_set[MAX_DEVICES] = {}, cl_attr_set[MAX_DEVICES] = {};
 	const int topk = tk.list[0].keys ? 1 : 0;
 	if (!attr_set[dev]) {
 		for (const IngestFn f : {fns[0][0][0], fns[1][0][0], fns[0][1][0], fns[1][1][0]})
@@ -2431,6 +2533,11 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 			cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
 		topk_attr_set[dev] = true;
 	}
+	if (cl.open && !cl_attr_set[dev]) {
+		for (int i = 0; i < 8; ++i)
+			cudaFuncSetAttribute(fns_cl[i >> 2][(i >> 1) & 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		cl_attr_set[dev] = true;
+	}
 	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
 	const uint64_t full = (uint64_t)sm_count(dev) * IngestShape::MIN_CTAS;
 	const uint32_t grid = (uint32_t)(want < full ? want : full);
@@ -2440,54 +2547,65 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
 	// a counted response sample takes a connection-queue entry, as one connection event does: the regions hold one record per event
-	const IngestFn k = fns[st.trace.rows ? 1 : 0][fq.cur ? 1 : 0][topk];
-	k<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, tk.list[0]);
+	const int tr = st.trace.rows ? 1 : 0, qr = fq.cur ? 1 : 0;
+	if (cl.open) fns_cl[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
+			tk.list[0], cl.open);
+	else fns[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, tk.list[0]);
 	return 1;
 }
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
-template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW>
+template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL = false>
 static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		cudaStream_t s)
+		cudaStream_t s, uint8_t *cl_open = nullptr)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
 		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW>, WARPS * 32, smem_max);
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL>, WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY, RH, TOPK, SLOW><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq,
-			fq_cms, fr, fr_cms, tk, b_slow);
+	drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq,
+			fq_cms, fr, fr_cms, tk, b_slow, cl_open);
 }
 
-// b_slow: GYSK_FLAG_FLOW_TOPK_SLOW's first slow bucket when tk.list[2] is held (RH only); the TASK pass is the TOPK one either way
-template <bool QRY, bool RH>
-static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
+// b_slow: GYSK_FLAG_FLOW_TOPK_SLOW's first slow bucket when tk.list[2] is held (RH only); the TASK pass is the TOPK one either way.
+// cl_open (CL, GYSK_FLAG_CLIENT_LEVELS): the TCP pass's client registers; the TASK pass does not touch them.
+template <bool QRY, bool RH, bool CL>
+static int launch_drain_passes_t(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		cudaStream_t s)
+		uint8_t *cl_open, cudaStream_t s)
 {
 	if (tk.list[0].keys) {
 		if constexpr (RH) {
-			if (tk.list[2].keys) launch_drain_pass<false, QRY, RH, true, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, s);
-			else launch_drain_pass<false, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+			if (tk.list[2].keys) launch_drain_pass<false, QRY, RH, true, true, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, s, cl_open);
+			else launch_drain_pass<false, QRY, RH, true, false, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open);
 		}
-		else launch_drain_pass<false, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		else launch_drain_pass<false, QRY, RH, true, false, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open);
 		launch_drain_pass<true, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
 	}
 	else {
-		launch_drain_pass<false, QRY, RH, false, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		launch_drain_pass<false, QRY, RH, false, false, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open);
 		launch_drain_pass<true, QRY, RH, false, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
 	}
 	return 2;
+}
+template <bool QRY, bool RH>
+static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
+		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
+		uint8_t *cl_open, cudaStream_t s)
+{
+	if (cl_open) return launch_drain_passes_t<QRY, RH, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, cl_open, s);
+	return launch_drain_passes_t<QRY, RH, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, nullptr, s);
 }
 
 // the batch's queued connection records -> flow table, HLL, exact cells; then the flow table -> count-min and its process records ->
@@ -2496,7 +2614,7 @@ static int launch_drain_passes(const DevState &st, const FlowTable &ft, const So
 // With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size, and
 // with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too.
 int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
-		const RecRegions &rr, uint64_t n_events, cudaStream_t s)
+		const ClientLevels &cl, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
@@ -2505,12 +2623,12 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable none {nullptr, 0u};
-	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, 0, s);
+	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, 0, cl.open, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable fqt {fq.flow, n - 1u};
-	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, s);
+	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, cl.open, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
-	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, s);
+	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, cl.open, s);
 }
 
 static void os_set_attrs(int dev)
@@ -2892,14 +3010,16 @@ int launch_task_flush(const DevState &st, uint32_t max_tasks, uint32_t tsec, uin
 	return 2;
 }
 
-int launch_flush(const DevState &st, uint32_t nslots, uint32_t tsec, uint32_t idle_secs, cudaStream_t s)
+int launch_flush(const DevState &st, const ClientLevels &cl, uint32_t nslots, uint32_t tsec, uint32_t idle_secs, cudaStream_t s)
 {
 	if (!nslots) return 0;
 	cudaMemsetAsync(st.counters + CTR_NEVICT, 0, sizeof(unsigned long long), s);
 	flush_kernel<<<div_up((uint64_t)nslots * HIST_CELLS, 256), 256, 0, s>>>(st, nslots, tsec, idle_secs);
 	state_kernel<<<div_up(nslots, 128), 128, 0, s>>>(st, nslots, tsec);
 	if (!idle_secs) return 2;
-	evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL, nullptr,
+	if (cl.open) evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL,
+			nullptr, SvcClientSlotReset {cl});
+	else evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL, nullptr,
 			SvcSlotReset {});		// grid-stride over the (device-side) eviction list
 	return 3;
 }
@@ -2928,6 +3048,29 @@ int launch_gather_tasks(const DevState &st, const unsigned long long *d_ids, uin
 int launch_gather_hll(const DevState &st, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s)
 {
 	gather_hll_kernel<<<1, 256, 0, s>>>(st, d_ids, found, d_out);
+	return 1;
+}
+
+int launch_gather_hll_window(const DevState &st, const uint8_t *regs, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s)
+{
+	gather_hll_kernel<<<1, 256, 0, s>>>(st, d_ids, found, d_out, regs);
+	return 1;
+}
+
+int launch_client_rows(const DevState &st, const ClientLevels &cl, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n,
+		gysk_svc_clients *d_out, cudaStream_t s)
+{
+	if (!n) return 0;
+	client_rows_kernel<<<div_up(n, CL_WARPS), CL_WARPS * 32, 0, s>>>(st, cl, d_ids, d_slots, n, d_out);
+	return 1;
+}
+
+int launch_client_roll(const ClientLevels &cl, uint32_t nslots, const LevelRing &lv, cudaStream_t s)
+{
+	if (!nslots) return 0;
+	const uint64_t npiece = (uint64_t)nslots * (CL_REGS / 16);
+	client_roll_kernel<<<(uint32_t)std::min<uint64_t>(div_up(npiece, 256), (uint64_t)sm_count(current_device()) * 8), 256, 0, s>>>(cl, nslots,
+			lv.cur[0], lv.live[0], lv.fresh & 1u);
 	return 1;
 }
 

@@ -186,6 +186,13 @@ struct FlowTopk { TopkList list[3]; };
 // (GYSK_FLAG_FLOW_TOPK_SLOW, resp_slow_score)
 static constexpr int TOPK_SCORE_SLOW = 0x100;
 
+// GYSK_FLAG_CLIENT_LEVELS: per service slot register sets of CL_REGS one-byte registers (precision GYSK_HLL_WINDOW_P): the open window
+// and the last closed one ([max_svcs + 1][CL_REGS] each), the ring of NSLOTS 30-s slots ([NSLOTS][stride][CL_REGS], the level ring's
+// layout: stride = max_svcs, no row for the null slot) and the 300-s level, the registerwise maximum of the live slots ([max_svcs + 1]
+// [CL_REGS]). Outside DevState, so that the kernels without the flag keep their parameter layout. Every pointer nullptr: off.
+static constexpr uint32_t CL_REGS = 1u << GYSK_HLL_WINDOW_P;
+struct ClientLevels { uint8_t *open, *last, *ring, *level; uint32_t stride; };
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
@@ -266,14 +273,16 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 // key_slots: the values the slot field of a sort key takes (max_svcs, or max_svcs + 1 + trace rows with trace rows)
 // fq.cur != nullptr: the response samples are queued for the flow query table too (GYSK_FLAG_FLOW_QUERIES)
 // tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the flow keys of the ACTIVE records join the connection table's candidates
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const gysk_event *d_ev, uint64_t n,
-		uint32_t key_slots, RecRegions &rr, cudaStream_t s);
+// cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): the ACTIVE records raise the open window's client registers too
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, const gysk_event *d_ev,
+		uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
 // fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms;
 // tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the passes gather each held table's candidates; tk.list[2].keys != nullptr
-// (GYSK_FLAG_FLOW_TOPK_SLOW, with fr.cur): the TCP pass gathers the flow key of each response sample in bucket b_slow or above
+// (GYSK_FLAG_FLOW_TOPK_SLOW, with fr.cur): the TCP pass gathers the flow key of each response sample in bucket b_slow or above;
+// cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): each connection record raises the open window's client register beside the all-time one
 int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
-		const RecRegions &rr, uint64_t n_events, cudaStream_t s);
+		const ClientLevels &cl, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // GYSK_FLAG_FLOW_TOPK, after the batch merge (it takes tmp's sort buffers, of at least n_max keys): the *l.n candidates (n_max >= *l.n)
 // sorted by key in l.keys, the distinct ones scored on table tbl (score as TOPK_SCORE_SLOW says) and the K best by (score descending,
 // key ascending) written to set; then, unless reseed is false, set back into l as the next batch's first candidates. -1: no sort plan
@@ -305,7 +314,8 @@ int launch_topn_pick(const SortTemp &tmp, const unsigned long long *d_n, uint32_
 int launch_task_flush(const DevState &st, uint32_t max_tasks, uint32_t tsec, uint32_t idle_secs, unsigned long long *host_ids, cudaStream_t s);
 // the window roll into ring slot st.levels.cur of each level (cleared by the host when it starts a new epoch), the listener states,
 // the idle-service eviction
-int launch_flush(const DevState &st, uint32_t max_svcs, uint32_t tsec, uint32_t idle_secs, cudaStream_t s);
+// (GYSK_FLAG_CLIENT_LEVELS, cl.open != nullptr: an evicted slot's client sets are cleared with it)
+int launch_flush(const DevState &st, const ClientLevels &cl, uint32_t max_svcs, uint32_t tsec, uint32_t idle_secs, cudaStream_t s);
 // clears table t and re-inserts the ids t.slot_id holds in slots [0, nslots)
 int launch_rebuild_table(const IdTable &t, uint32_t nslots, cudaStream_t s);
 // the single-id exports: the raw state of n ids (id 0 and unknown ids: found = 0); the HLL registers of the id d_ids[0]
@@ -341,6 +351,15 @@ int launch_query_flow_resp(const unsigned long long *tbl, uint32_t depth, uint32
 // (replacing it when the slot is fresh), then level = the sum of the live slots (level 0's decision of lv)
 int launch_cms_level_roll(const unsigned long long *cur, unsigned long long *ring, unsigned long long *level, size_t cells, const LevelRing &lv,
 		cudaStream_t s);
+// GYSK_FLAG_CLIENT_LEVELS at the flush, after launch_flush and before the open / last swap: the open sets of slots [0, nslots) (the
+// capacity) max-merged into ring slot lv.cur[0] (in its place when the slot is fresh) and the level = the registerwise maximum of the
+// live slots (level 0's decision of lv)
+int launch_client_roll(const ClientLevels &cl, uint32_t nslots, const LevelRing &lv, cudaStream_t s);
+// the client rows (gysk_svc_clients) by id (d_ids) or by slot (d_slots); the estimates as hll_pending leaves them
+int launch_client_rows(const DevState &st, const ClientLevels &cl, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n,
+		gysk_svc_clients *d_out, cudaStream_t s);
+// the CL_REGS registers at regs + slot * CL_REGS of the id d_ids[0] (gysk_export_hll_window)
+int launch_gather_hll_window(const DevState &st, const uint8_t *regs, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s);
 // trace rows at gysk_flush: the half `open` (the one the flush opens) of rows [0, nrows) cleared
 int launch_trace_roll(const DevState &st, uint32_t open, uint32_t nrows, cudaStream_t s);
 // trace rows by id (d_ids) or by row (d_rows)

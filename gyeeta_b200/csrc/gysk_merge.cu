@@ -212,6 +212,21 @@ __global__ void fold_hll_kernel(DevState st, Members mb, LogicalArrays lg)
 	reinterpret_cast<uint32_t *>(lg.hll_of(l, st.hll_p))[w] = acc;
 }
 
+// GYSK_FLAG_CLIENT_LEVELS, one thread per (logical, set, 4 registers): per-byte max over the member services' last-window (set 0) and
+// 300-s (set 1) client registers, the HLL of the union of their clients
+__global__ void fold_clients_kernel(ClientLevels cl, Members mb, uint32_t nl, uint8_t *__restrict__ out)
+{
+	constexpr uint32_t words = CL_REGS / 4;
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= (uint64_t)nl * 2 * words) return;
+	const uint32_t l = (uint32_t)(i / (2 * words)), set = (uint32_t)(i / words) & 1u, w = (uint32_t)(i % words);
+	const uint8_t *src = set ? cl.level : cl.last;
+	uint32_t acc = 0;
+
+	mb.each(l, [&](uint32_t s) { acc = __vmaxu4(acc, reinterpret_cast<const uint32_t *>(src + (size_t)s * CL_REGS)[w]); });
+	reinterpret_cast<uint32_t *>(out)[i] = acc;
+}
+
 // GYSK_FLAG_MERGE_TRACES, one thread per (logical, word): words 0 .. LT_TD_COUNT sum the members' last closed trace windows (the half
 // par ^ 1 of the row a member slot holds; a slot without a row, or whose row is being taken, adds nothing), the LT_NTRACED thread counts
 // those rows and takes the three maxima.
@@ -415,6 +430,28 @@ __global__ void __launch_bounds__(LG_WARPS * 32) logical_summary_kernel(const in
 	summarize_warp(r, l >= 0 ? lids[l] : 0ull, hll_p, summ[wid], out + q, lane);
 }
 
+// GYSK_FLAG_CLIENT_LEVELS read side, one warp per row: the merged client sets (regs: [nl][2][CL_REGS]) of dense index lidx[q] as
+// client_rows_kernel reads a service's, logical id lids[l]; an index of -1 gives an all-zero row
+__global__ void __launch_bounds__(LG_WARPS * 32) logical_clients_kernel(const int32_t *__restrict__ lidx, uint32_t n, const uint8_t *__restrict__ regs,
+		const unsigned long long *__restrict__ lids, gysk_svc_clients *__restrict__ out)
+{
+	__shared__ uint32_t hist[LG_WARPS][2][64];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t q = blockIdx.x * LG_WARPS + wid;
+
+	if (q >= n) return;
+	const int32_t l = lidx[q];
+	gysk_svc_clients o;
+	memset(&o, 0, sizeof(o));
+	if (l >= 0) {
+		for (int set = 0; set < 2; ++set) hll_hist_warp(regs + ((size_t)l * 2 + set) * CL_REGS, GYSK_HLL_WINDOW_P, hist[wid][set], lane);
+		o.glob_id = lids[l]; o.found = 1;
+		o.last_5s = hll_pending(hist[wid][0], GYSK_HLL_WINDOW_P);
+		o.last_5min = hll_pending(hist[wid][1], GYSK_HLL_WINDOW_P);
+	}
+	if (lane == 0) out[q] = o;
+}
+
 // a logical service whose merged last window holds response samples or connection events (GYSK_WINDOW_ACTIVE_ONLY)
 __device__ __forceinline__ bool logical_active(const LogicalArrays &lg, uint32_t l)
 {
@@ -601,6 +638,12 @@ int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_cluster
 	cluster_row_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(lidx, m, e->mg.clusters.cl, e->mg.clusters.d_ids, reinterpret_cast<gysk_cluster_row *>(e->d_wstage));
 	return 1;
 }
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_clients *)
+{
+	logical_clients_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(lidx, m, e->mg.cl_hll, e->mg.d_logical_ids,
+			reinterpret_cast<gysk_svc_clients *>(e->d_wstage));
+	return 1;
+}
 int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical_trace *)
 {
 	logical_trace_kernel<<<div_up(m, 128), 128, 0, e->stream>>>(lidx, m, e->mg.lg, e->mg.d_logical_ids, reinterpret_cast<gysk_logical_trace *>(e->d_wstage));
@@ -610,14 +653,16 @@ SvcRows logical_finish(const gysk_engine *e, gysk_svc_summary *out) { return Svc
 CopyRows<gysk_logical_state> logical_finish(const gysk_engine *, gysk_logical_state *out) { return CopyRows<gysk_logical_state> {out}; }
 CopyRows<gysk_cluster_row> logical_finish(const gysk_engine *, gysk_cluster_row *out) { return CopyRows<gysk_cluster_row> {out}; }
 CopyRows<gysk_logical_trace> logical_finish(const gysk_engine *, gysk_logical_trace *out) { return CopyRows<gysk_logical_trace> {out}; }
+ClientRows logical_finish(const gysk_engine *, gysk_svc_clients *out) { return ClientRows {out}; }
 uint64_t &row_id(gysk_svc_summary &r) { return r.glob_id; }
 uint64_t &row_id(gysk_logical_state &r) { return r.logical_id; }
 uint64_t &row_id(gysk_cluster_row &r) { return r.cluster_id; }
 uint64_t &row_id(gysk_logical_trace &r) { return r.logical_id; }
+uint64_t &row_id(gysk_svc_clients &r) { return r.glob_id; }
 template <typename Row> constexpr uint32_t logical_flag()
 {
 	return std::is_same<Row, gysk_logical_state>::value ? GYSK_FLAG_MERGE_STATES : std::is_same<Row, gysk_cluster_row>::value ? GYSK_FLAG_MERGE_CLUSTERS :
-		std::is_same<Row, gysk_logical_trace>::value ? GYSK_FLAG_MERGE_TRACES : 0;
+		std::is_same<Row, gysk_logical_trace>::value ? GYSK_FLAG_MERGE_TRACES : std::is_same<Row, gysk_svc_clients>::value ? GYSK_FLAG_CLIENT_LEVELS : 0;
 }
 
 // gysk_query_logical / gysk_query_logical_states / gysk_query_cluster_states: the rows of n ids, in QCHUNK pieces, each row carrying its
@@ -853,6 +898,7 @@ int lay_out_arena(gysk_engine *e)
 		names.clear();
 		mg.off_maxu8 = off;
 		take(lg.hll, (size_t)nl << e->cfg.hll_p, "hll registers");
+		if (e->cfg.flags & GYSK_FLAG_CLIENT_LEVELS) take(mg.cl_hll, (size_t)nl * 2 * CL_REGS, "client registers");
 		mg.bytes_maxu8 = off - mg.off_maxu8;
 		mg.name_maxu8 = "max_u8: " + names;
 		return off;
@@ -1024,6 +1070,10 @@ int gysk_merge_prepare(gysk_engine *e)
 		}
 		fold_hist_kernel<<<div_up((uint64_t)nl * HIST_CELLS, 256), 256, 0, e->stream>>>(e->st, mg.members, mg.lg);
 		fold_hll_kernel<<<div_up((uint64_t)nl << (e->cfg.hll_p - 2), 256), 256, 0, e->stream>>>(e->st, mg.members, mg.lg);
+		if (mg.cl_hll) {		// GYSK_FLAG_CLIENT_LEVELS
+			fold_clients_kernel<<<div_up((uint64_t)nl * 2 * (CL_REGS / 4), 256), 256, 0, e->stream>>>(e->cl, mg.members, nl, mg.cl_hll);
+			e->kernel_launches++;
+		}
 		fold_td_kernel<<<std::min<uint32_t>(div_up(nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(e->st, mg.members, mg.lg);
 		e->kernel_launches += 3;
 		if (mg.lg.states) {		// GYSK_FLAG_MERGE_STATES
@@ -1354,6 +1404,29 @@ int gysk_export_logical_hll(gysk_engine *e, uint64_t logical_id, uint8_t *regs)
 	CU(e, cudaMemcpyAsync(e->h_wstage, mg.lg.hll_of((uint32_t)l, e->cfg.hll_p), nb, cudaMemcpyDeviceToHost, e->stream));
 	CU(e, cudaStreamSynchronize(e->stream));
 	memcpy(regs, e->h_wstage, nb);
+	return GYSK_OK;
+}
+
+// GYSK_FLAG_CLIENT_LEVELS: the merged client rows of n logical ids, and one logical service's merged client registers with the contract
+// of gysk_export_logical_hll
+int gysk_query_logical_clients(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_svc_clients *out)
+{
+	return logical_query_rows(e, logical_ids, n, out, "query_logical_clients");
+}
+
+int gysk_export_logical_hll_window(gysk_engine *e, uint64_t logical_id, int which, uint8_t *regs)
+{
+	CHECK_ENGINE(e);
+	if (!regs || (which != GYSK_CLIENTS_LAST && which != GYSK_CLIENTS_5MIN)) return GYSK_ERR_INVAL;
+	if (!(e->cfg.flags & GYSK_FLAG_CLIENT_LEVELS)) return GYSK_ERR_NOTSUP;
+	GYSK_ENTER(e, Drain);
+	MergeState &mg = e->mg;
+	if (!mg.finished) return fail(e, GYSK_ERR_INVAL, "gysk_export_logical_hll_window: no finished merge");
+	const int32_t l = logical_index(mg, logical_id);
+	if (l < 0) return GYSK_ERR_NOENT;
+	CU(e, cudaMemcpyAsync(e->h_wstage, mg.cl_of((uint32_t)l, which), CL_REGS, cudaMemcpyDeviceToHost, e->stream));
+	CU(e, cudaStreamSynchronize(e->stream));
+	memcpy(regs, e->h_wstage, CL_REGS);
 	return GYSK_OK;
 }
 

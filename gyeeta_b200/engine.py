@@ -44,6 +44,9 @@ FLAG_FLOW_RESP_HIST = 0x200
 FLAG_FLOW_TOPK = 0x400
 FLAG_FLOW_TOPK_5MIN = 0x800
 FLAG_FLOW_TOPK_SLOW = 0x1000
+FLAG_CLIENT_LEVELS = 0x2000
+HLL_WINDOW_P = 8
+CLIENTS_LAST, CLIENTS_5MIN = 0, 1
 FLOW_TOPK_CAP = 4096
 TOPN_TASK_CPU, TOPN_TASK_CPU_DELAY, TOPN_TASK_BLKIO_DELAY = range(3)
 TD_CAP = 256
@@ -156,6 +159,15 @@ class LogicalState(C.Structure):
 
 
 assert C.sizeof(LogicalState) == 80
+
+
+class SvcClients(C.Structure):
+    """gysk_svc_clients: distinct clients of a service (or logical service) in the last window and the rolling 300 s
+    (GYSK_FLAG_CLIENT_LEVELS)"""
+    _fields_ = [("glob_id", C.c_uint64), ("found", C.c_int32), ("pad", C.c_uint32), ("last_5s", C.c_double), ("last_5min", C.c_double)]
+
+
+assert C.sizeof(SvcClients) == 32
 
 
 class ClusterState(C.Structure):
@@ -342,6 +354,11 @@ def load_library(path=None):
         "gysk_topk_flow_slow_global": (i32, [vp, u32, vp, vp]),
         "gysk_topk_flow_slow_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_topk_flow_slow_global_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_query_svc_clients": (i32, [vp, vp, u32, vp]),
+        "gysk_query_clients_window": (i32, [vp, C.c_int32, u32, vp, vp, u32, vp]),
+        "gysk_export_hll_window": (i32, [vp, u64, i32, vp]),
+        "gysk_query_logical_clients": (i32, [vp, vp, u32, vp]),
+        "gysk_export_logical_hll_window": (i32, [vp, u64, i32, vp]),
         "gysk_nccl_unique_id": (i32, [vp]),
         "gysk_nccl_comm_init": (i32, [vp, vp, u32, u32]),
         "gysk_merge_global": (i32, [vp, vp]),
@@ -408,7 +425,7 @@ class Engine:
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
                  max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False,
-                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False):
+                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False, client_levels=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -424,7 +441,8 @@ class Engine:
                     (FLAG_MERGE_TOPN if merge_topn else 0) | (FLAG_FLOW_LEVEL if flow_level else 0) | (FLAG_MERGE_TRACES if merge_traces else 0) | \
                     (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
                     (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0) | \
-                    (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0) | (FLAG_FLOW_TOPK_SLOW if flow_topk_slow else 0)
+                    (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0) | (FLAG_FLOW_TOPK_SLOW if flow_topk_slow else 0) | \
+                    (FLAG_CLIENT_LEVELS if client_levels else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -862,6 +880,39 @@ class Engine:
     def export_hll(self, id_):
         return self._hll(self.L.gysk_export_hll, id_)
 
+    def query_svc_clients(self, ids):
+        """gysk_query_svc_clients: SvcClients rows of service ids as of the last flush (client_levels=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (SvcClients * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_svc_clients(self.h, _p(ids), len(ids), out))
+        return out[: len(ids)]
+
+    def query_clients_window(self, host_idx=-1, active_only=False, cap=None):
+        """gysk_query_clients_window: (SvcClients rows in the order of query_window_hosts, host_idx of each row, number of rows).
+        cap None = all rows (a count call first); 0 = the count only"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_clients_window(self.h, host_idx, flags, None, None, 0, C.byref(n)))
+            cap = n.value
+        out = (SvcClients * max(cap, 1))()
+        hosts = np.zeros(max(cap, 1), dtype=np.uint32)
+        self._chk(self.L.gysk_query_clients_window(self.h, host_idx, flags, out if cap else None, _p(hosts) if cap else None, cap, C.byref(n)))
+        k = min(cap, n.value)
+        return out[:k], hosts[:k].copy(), n.value
+
+    def export_hll_window(self, id_, which=CLIENTS_LAST):
+        """gysk_export_hll_window: the 256 client registers of CLIENTS_LAST or CLIENTS_5MIN, None for an unknown id"""
+        return self._hll_window(self.L.gysk_export_hll_window, id_, which)
+
+    def _hll_window(self, fn, id_, which):
+        regs = np.zeros(1 << HLL_WINDOW_P, dtype=np.uint8)
+        rc = fn(self.h, int(id_), which, _p(regs))
+        if rc == -2:
+            return None
+        self._chk(rc)
+        return regs
+
     def _hll(self, fn, id_):
         regs = np.zeros(1 << self.cfg.hll_p, dtype=np.uint8)
         rc = fn(self.h, int(id_), _p(regs))
@@ -998,6 +1049,17 @@ class Engine:
 
     def export_logical_hll(self, logical_id):
         return self._hll(self.L.gysk_export_logical_hll, logical_id)
+
+    def query_logical_clients(self, ids):
+        """gysk_query_logical_clients: SvcClients rows of logical ids from the last merge (client_levels=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = (SvcClients * max(len(ids), 1))()
+        self._chk(self.L.gysk_query_logical_clients(self.h, _p(ids), len(ids), out))
+        return out[: len(ids)]
+
+    def export_logical_hll_window(self, logical_id, which=CLIENTS_LAST):
+        """gysk_export_logical_hll_window: the merged 256 client registers of one logical service, None outside the map"""
+        return self._hll_window(self.L.gysk_export_logical_hll_window, logical_id, which)
 
     def query_logical_states(self, ids):
         """gysk_query_logical_states: LogicalState rows of logical ids from the last merge (merge_states=True)"""
