@@ -31,7 +31,7 @@ static constexpr int TD_CAP = 256;		// delta = 200 yields 200 ... 1.3 x 200 cent
 // so that the bin's exact msec sum (GY_HISTOGRAM::add_data adds usec / 1000 per sample) is (us - remainders) / 1000 and its mean
 // us / samples. Bin index = td_code(usec) + RESP_TIME_HASH bucket of its msec value: both terms are monotone in usec, so the
 // index is too and no bin straddles a histogram bucket. Two ways lead to the same numbers: the samples of most services travel as
-// sort keys and are summed per run of equal {slot, bin} (bins_merge_kernel, gysk_kernels.cu); a HOT service — one that brought at least
+// sort keys, sorted by slot and summed per bin of each service's segment (bins_merge_kernel, gysk_kernels.cu); a HOT service — one that brought at least
 // hot_min samples in an earlier batch — owns a dense row of such bins (DevState::hot_rows, L2-resident; layout below) and
 // every one of its samples is two 64-bit REDs into it, no key, no sort. The batch's merge kernel reads a row in order and zeroes it.
 struct alignas(16) Bin { unsigned long long cw; unsigned long long us; };

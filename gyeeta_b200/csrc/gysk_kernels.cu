@@ -7,7 +7,7 @@
 //   drain_kernel         the queued records, one launch per kind: TCP -> the flow's count-min increment summed in the batch flow table,
 //                        HLL register max, per-service exact cell; TASK -> the flow table into the count-min cells, then
 //                        MAGGR_TASK::set_local_task_state (3 histograms) server/gy_msocket.h:1009-1018
-//   os_pass_kernel       stable one-sweep LSD radix pass (RESP keys of a batch on {slot, bin}; the top-N rankings)
+//   os_pass_kernel       stable one-sweep LSD radix pass (RESP keys of a batch on their slot; the top-N rankings)
 //   segs_mark_kernel     sorted keys -> one segment per service, touched list (short segments), batch rows (long segments)
 //   long_sum_kernel      keys of the long segments -> per-bin samples and exact usec sums in their batch rows
 //   trace_keys_kernel    trace rows (max_trace_svcs): requests, usec sum / max, response buckets of each row from the tail of the sorted keys
@@ -34,17 +34,20 @@ namespace gysk {
 
 // RESP sort key = {slot : 24 | bin index : 10 | usec : 30}. Bin index = td_code(usec) + RESP_TIME_HASH bucket of usec / 1000: both
 // terms are monotone in usec, so the index is too and no bin straddles a histogram bucket (DESIGN.md §3). The radix passes sort on
-// the top 10 + slot bits only: the samples of one (service, bin) end up as one contiguous RUN, in no particular order inside it.
+// the slot bits only: the samples of one service end up as one contiguous SEGMENT, its bins in no particular order inside it
+// (bins_merge_kernel sums them per bin itself).
 static constexpr int KEY_GROUP_SHIFT = 30;				// key >> 30 = {slot, bin}
 static constexpr int KEY_SLOT_SHIFT = KEY_GROUP_SHIFT + TD_CODE_BITS;
 __device__ __forceinline__ uint32_t key_usec(unsigned long long k) { return (uint32_t)k & 0x3FFFFFFFu; }
 __device__ __forceinline__ uint32_t key_slot(unsigned long long k) { return (uint32_t)(k >> KEY_SLOT_SHIFT); }
 __device__ __forceinline__ uint32_t key_bin(unsigned long long k) { return (uint32_t)(k >> KEY_GROUP_SHIFT) & ((1u << TD_CODE_BITS) - 1u); }
+// the bin index of a response time, as the key carries it
+__device__ __forceinline__ uint32_t resp_bin(uint32_t usec) { return td_code(usec) + (uint32_t)bucket_resp_time((long long)(usec / 1000u)); }
 
-static constexpr int KEY_DIGIT_MAX = 8;				// widest digit of the RESP-key passes (key_sort_plan)
+static constexpr int KEY_DIGIT_MAX = 9;				// widest digit of the RESP-key passes (key_sort_plan)
 static constexpr int KEY_SLOT_BITS_MAX = 24;
 // passes of the longest RESP plan: ingest_kernel keeps this many digit histograms in shared memory
-static constexpr int KEY_PASSES_MAX = (TD_CODE_BITS + KEY_SLOT_BITS_MAX + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
+static constexpr int KEY_PASSES_MAX = (KEY_SLOT_BITS_MAX + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
 static_assert(KEY_PASSES_MAX <= OS_MAX_PASSES, "a RESP plan fits a SortPlan");
 // which bits of the key each pass of the radix sort takes as its digit, lowest first: pass p sorts on bits [shift[p], shift[p] + bits[p]).
 // key_sort_plan cuts the RESP keys, plain_sort_plan every other sort; ingest_kernel and os_hist_kernel fill the passes' histograms
@@ -756,7 +759,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					const uint32_t v = rb[k].x;
 					// the value bins of a RESP key (td_code + RESP_TIME_HASH bucket): the batch items are those of the service digest's path
 					if (tr_key) W.kq[nk + __popc(m_resp & lt)] = ((unsigned long long)(st.trace.base + (uint32_t)trow[k]) << KEY_SLOT_SHIFT) |
-							((unsigned long long)(td_code(v) + (uint32_t)bucket_resp_time((long long)(v / 1000u))) << KEY_GROUP_SHIFT) | v;
+							((unsigned long long)resp_bin(v) << KEY_GROUP_SHIFT) | v;
 					else if (trow[k] >= 0) {
 						// beyond the validity rule (rare): no key, the counters the key would have brought straight into the row
 						unsigned long long *w = st.trace.words(st.trace.par, (uint32_t)trow[k]);
@@ -982,7 +985,7 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 
 // ---------------------------------------------------------------------------------------------------
 // stable LSD radix sort of 64-bit keys on the bit range of a SortPlan, one digit of 6 to 9 bits per pass (a narrower last digit runs
-// in the 6-bit kernel), tile = SORT_TILE keys per CTA of 256 threads. It sorts every batch's RESP keys by {slot, bin}
+// in the 6-bit kernel), tile = SORT_TILE keys per CTA of 256 threads. It sorts every batch's RESP keys by slot
 // (launch_batch_merge) and, through launch_radix_sort, the window list by host, the top-N keys of services, processes and logical
 // services by score, and the group-by's keys by group.
 //
@@ -1363,9 +1366,13 @@ __device__ __forceinline__ void long_sum_chunk(const unsigned long long *__restr
 		red_add_u64(row + w + HOT_ROW_BINS, us);
 	};
 
-	// whole chunk inside one bin of a long segment (a popular bin of a big service): one RED pair for 128 samples
-	const uint32_t dfirst = __shfl_sync(0xffffffffu, dest(kk[0]), 0), dlast = __shfl_sync(0xffffffffu, dest(kk[LS_V - 1]), 31);
-	if (dfirst == dlast && dlast != ~0u) {
+	// whole chunk inside one bin of a long segment (a popular bin of a big service): one RED pair for 128 samples. The keys are sorted
+	// by slot only, so every key is checked against the chunk's first one
+	const uint32_t dfirst = __shfl_sync(0xffffffffu, dest(kk[0]), 0);
+	bool same = dfirst != ~0u;
+#pragma unroll
+	for (int t = 0; t < LS_V; ++t) same = same && dest(kk[t]) == dfirst;
+	if (__all_sync(0xffffffffu, same)) {
 		unsigned long long us = 0;
 		uint32_t rem = 0;
 #pragma unroll
@@ -1373,7 +1380,7 @@ __device__ __forceinline__ void long_sum_chunk(const unsigned long long *__restr
 		const unsigned long long gsum = (unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)us & 0xFFFFFu) +
 				((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(us >> 20)) << 20);	// us < 2^32: 20 + 12 bits, x 32 lanes fits
 		rem = __reduce_add_sync(0xffffffffu, rem);
-		if (lane == 0) red_bin(dlast, (unsigned long long)(32 * LS_V) | ((unsigned long long)rem << BIN_CNT_BITS), gsum);
+		if (lane == 0) red_bin(dfirst, (unsigned long long)(32 * LS_V) | ((unsigned long long)rem << BIN_CNT_BITS), gsum);
 		return;
 	}
 
@@ -1616,19 +1623,28 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 		bool staged = false;				// the batch items wait in the work area for warp_merge_compress_staged
 		if (t >= nrow) {
 			// a short segment, read straight from the sorted keys in blocks of 256: lane l holds keys [b0 + 8 l, b0 + 8 l + 8), four
-			// 16-byte loads, and the next block's loads go out before this one is scanned. A bin starts wherever the bin bits change.
-			// Each lane sums its own runs of equal bin; one segmented scan per block joins the runs that cross lanes (and the bin open
-			// from the block before), and the bin's last key leaves its totals {usec sum, samples | remainders | bin} in the bin's raw
-			// slot, j = the bins that start before it — the numbers a run of equal {slot, bin} adds up to. The raw slots of the items
-			// that fit the work area beside the old centroids lie there (the usec sum where the item's mean goes, W.src[na + j],
-			// the rest in W.pref[j], free until the merge), the others in items[j]. Then every lane takes every 32nd bin, as for a row.
+			// 16-byte loads, and the next block's loads go out before this one is summed. The keys arrive in slot order only, so each
+			// lane adds each of its samples to its bin's accumulator in the warp's work area with shared atomics of its own. (Joining
+			// the lanes of one bin first with match.any, then one set of atomics per bin, made the kernel 1.9 to 2.7 times slower on the
+			// bench workload, DESIGN.md §7.) Then the warp walks the bins in order, 32 per step, and packs every non-empty one
+			// {usec sum, samples | remainders | bin} at its item index j (j <= its bin: the walk overwrites only bins it has read),
+			// and every lane takes every 32nd item, as for a row.
 			nsamples = seg.end - seg.key0;
 			// a short segment's bin: samples <= LONG_SEG and remainders < 1000 x LONG_SEG fit below bit 54 of cw
 			constexpr int RAW_BIN_SHIFT = 54;
 			static_assert(BIN_CNT_BITS + 10 + 14 <= RAW_BIN_SHIFT && LONG_SEG <= (1 << 14), "cw of a short segment's bin below the bin bits");
-			const uint32_t room = (uint32_t)TD_SMEM_N - na;		// raw slots in the work area (na <= TD_CAP < TD_SMEM_N)
-			unsigned long long *raw_us = reinterpret_cast<unsigned long long *>(W.src + na), *raw_cw = W.pref;
-			ulonglong2 *raw = reinterpret_cast<ulonglong2 *>(items);
+			// every bin of the segment lies in [blo, bhi]: the bins of the service's batch extremes (ingest_kernel keeps them for every
+			// sample it makes a key of), every bin for a trace row's segment. Accumulator of bin b: 4 words at acc[4 (b - blo)],
+			// {sum of usec & 0x3FFFF < 2^31, sum of usec >> 18 < 2^25, samples, remainders < 2^23} — 32-bit shared atomics (native; a
+			// 64-bit one is a CAS loop) that cannot overflow over LONG_SEG samples. It aliases the start of the work area, which is free
+			// until the items are taken: the packed items fill [0, 16 nitems), below the staged means and weights (W.src, W.nxt). The
+			// merge writes over all of it, so each short segment zeroes its bins' accumulators first.
+			const uint32_t blo = trace ? 0u : resp_bin(sb.minv), nb = (trace ? (uint32_t)NBINS - 1u : resp_bin(sb.maxv)) - blo + 1u;
+			static_assert(sizeof(TdWorkT<TD_SMEM_N>) >= NBINS * 16 && offsetof(TdWorkT<TD_SMEM_N>, nxt) >= TD_SMEM_N * 16 &&
+					offsetof(TdWorkT<TD_SMEM_N>, src) >= TD_SMEM_N * 16, "the bin accumulators and packed items fit below the staged items");
+			uint32_t *const acc = reinterpret_cast<uint32_t *>(W.mean);
+			unsigned long long *const packed = reinterpret_cast<unsigned long long *>(W.mean);
+			for (uint32_t i = lane; i < 2u * nb; i += 32) reinterpret_cast<uint2 *>(acc)[i] = make_uint2(0u, 0u);
 			auto load8 = [&](uint32_t b0, unsigned long long (&k)[8]) {	// ~0ull: no key of the segment (never a key: bin <= 845)
 				const uint32_t i0 = b0 + (uint32_t)lane * 8u;
 				if (i0 >= seg.key0 && i0 + 8u <= seg.end) {
@@ -1643,85 +1659,51 @@ __global__ void __launch_bounds__(TD_WARPS * 32, TD_MERGE_CTAS_PER_SM) bins_merg
 					for (int u = 0; u < 8; ++u) k[u] = i0 + u >= seg.key0 && i0 + u < seg.end ? keys[i0 + u] : ~0ull;
 				}
 			};
-			auto rem_of = [](uint32_t v) { return v - (v / 1000u) * 1000u; };
-			uint32_t pbin = ~0u, ccnt = 0, crem = 0;	// bin of the key before the block, the totals of that bin so far
-			unsigned long long cus = 0;
 			const uint32_t a0 = seg.key0 & ~1u;		// even: every lane's keys start 16-byte aligned
 			unsigned long long kk[8], nk[8];
 			load8(a0, kk);
+			__syncwarp();
 			for (uint32_t b0 = a0; b0 < seg.end; b0 += 256) {
 				if (b0 + 256u < seg.end) load8(b0 + 256u, nk);
 				else {
 #pragma unroll
 					for (int u = 0; u < 8; ++u) nk[u] = ~0ull;
 				}
-				uint32_t bin[8];
-#pragma unroll
-				for (int u = 0; u < 8; ++u) bin[u] = kk[u] == ~0ull ? ~0u : key_bin(kk[u]);
-				const uint32_t nfirst = __shfl_sync(0xffffffffu, nk[0] == ~0ull ? ~0u : key_bin(nk[0]), 0);	// the key after the block
-				uint32_t prevb = __shfl_up_sync(0xffffffffu, bin[7], 1), nextb = __shfl_down_sync(0xffffffffu, bin[0], 1);
-				if (lane == 0) prevb = pbin;
-				if (lane == 31) nextb = nfirst;
-				// the lane's bin starts (hc) and the totals of its last run
-				uint32_t hc = 0, tc = 0, tr = 0;
-				unsigned long long tu = 0;
 #pragma unroll
 				for (int u = 0; u < 8; ++u) {
-					const bool valid = bin[u] != ~0u;
-					if (valid && bin[u] != (u ? bin[u - 1] : prevb)) { ++hc; tc = 0; tr = 0; tu = 0; }
-					const uint32_t v = key_usec(kk[u]);
-					if (valid) { ++tc; tr += rem_of(v); tu += v; }
-				}
-				// one scan over the lanes of {usec sum : 40 | bin starts} and {remainders : 18 | samples}: the sums of 256 samples
-				// fit every field. The segmented totals of a lane's last run start at the last lane with a bin start (h).
-				const unsigned long long X = tu | ((unsigned long long)hc << 40);
-				const uint32_t Y = tr | (tc << 18);
-				unsigned long long xi = X;
-				uint32_t yi = Y;
-#pragma unroll
-				for (int off = 1; off < 32; off <<= 1) {
-					const unsigned long long x = __shfl_up_sync(0xffffffffu, xi, off);
-					const uint32_t y = __shfl_up_sync(0xffffffffu, yi, off);
-					if (lane >= off) { xi += x; yi += y; }
-				}
-				const uint32_t hm = __ballot_sync(0xffffffffu, hc != 0);
-				const uint32_t upto = hm & (0xFFFFFFFFu >> (31 - lane));		// lanes <= this one with a bin start
-				const int h = upto ? 31 - __clz((int)upto) : 0;
-				const unsigned long long xs = xi - __shfl_sync(0xffffffffu, xi - X, h);
-				const uint32_t ys = yi - __shfl_sync(0xffffffffu, yi - Y, h);
-				unsigned long long su = xs & ((1ull << 40) - 1u);			// the bin open at the lane's last key, so far
-				uint32_t sc = ys >> 18, sr = ys & 0x3FFFFu;
-				if (!upto) { su += cus; sc += ccnt; sr += crem; }
-				// the bin open at the lane's first key (the lane before's, or the block before's at lane 0)
-				unsigned long long ru = __shfl_up_sync(0xffffffffu, su, 1);
-				uint32_t rc = __shfl_up_sync(0xffffffffu, sc, 1), rr = __shfl_up_sync(0xffffffffu, sr, 1);
-				if (lane == 0) { ru = cus; rc = ccnt; rr = crem; }
-				uint32_t j = nitems + (uint32_t)(xi >> 40) - hc - 1u;		// item of that bin
-#pragma unroll
-				for (int u = 0; u < 8; ++u) {
-					const bool valid = bin[u] != ~0u;
-					if (valid && bin[u] != (u ? bin[u - 1] : prevb)) { ++j; rc = 0; rr = 0; ru = 0; }
-					const uint32_t v = key_usec(kk[u]);
-					if (valid) { ++rc; rr += rem_of(v); ru += v; }
-					if (valid && bin[u] != (u < 7 ? bin[u + 1] : nextb)) {		// the bin's last key
-						const unsigned long long cwb = (unsigned long long)rc | ((unsigned long long)rr << BIN_CNT_BITS) |
-								((unsigned long long)bin[u] << RAW_BIN_SHIFT);
-						if (j < room) { raw_us[j] = ru; raw_cw[j] = cwb; }
-						else raw[j] = make_ulonglong2(ru, cwb);
-						binmax = max(binmax, rc);
+					if (kk[u] != ~0ull) {
+						const uint32_t v = key_usec(kk[u]);
+						uint32_t *const a = acc + 4u * (key_bin(kk[u]) - blo);
+						atomicAdd(a, v & 0x3FFFFu);
+						atomicAdd(a + 1, v >> 18);
+						atomicAdd(a + 2, 1u);
+						atomicAdd(a + 3, v - (v / 1000u) * 1000u);
 					}
 				}
-				cus = __shfl_sync(0xffffffffu, su, 31); ccnt = __shfl_sync(0xffffffffu, sc, 31); crem = __shfl_sync(0xffffffffu, sr, 31);
-				pbin = __shfl_sync(0xffffffffu, bin[7], 31);
-				nitems += (uint32_t)(__shfl_sync(0xffffffffu, xi, 31) >> 40);
 #pragma unroll
 				for (int u = 0; u < 8; ++u) kk[u] = nk[u];
 			}
-			staged = na + nitems <= (uint32_t)TD_SMEM_N;
 			__syncwarp();
+			for (uint32_t b0 = 0; b0 < nb; b0 += 32) {
+				const uint32_t i = b0 + lane;
+				uint2 us2 = make_uint2(0u, 0u), cr = make_uint2(0u, 0u);
+				if (i < nb) { us2 = reinterpret_cast<const uint2 *>(acc)[2u * i]; cr = reinterpret_cast<const uint2 *>(acc)[2u * i + 1u]; }
+				const bool ne = cr.x != 0u;
+				const uint32_t m = __ballot_sync(0xffffffffu, ne);
+				if (ne) {
+					const uint32_t j = nitems + __popc(m & lt);
+					packed[2u * j] = (unsigned long long)us2.x + ((unsigned long long)us2.y << 18);
+					packed[2u * j + 1u] = (unsigned long long)cr.x | ((unsigned long long)cr.y << BIN_CNT_BITS) |
+							((unsigned long long)(blo + i) << RAW_BIN_SHIFT);
+					binmax = max(binmax, cr.x);
+				}
+				nitems += __popc(m);
+				__syncwarp();
+			}
+			staged = na + nitems <= (uint32_t)TD_SMEM_N;
 			for (uint32_t j = lane; j < nitems; j += 32) {
-				const ulonglong2 r = j < room ? make_ulonglong2(raw_us[j], raw_cw[j]) : raw[j];
-				take_bin(j, r.y & ((1ull << RAW_BIN_SHIFT) - 1u), r.x, (uint32_t)(r.y >> RAW_BIN_SHIFT), staged);
+				const unsigned long long us = packed[2u * j], cw = packed[2u * j + 1u];
+				take_bin(j, cw & ((1ull << RAW_BIN_SHIFT) - 1u), us, (uint32_t)(cw >> RAW_BIN_SHIFT), staged);
 			}
 		}
 		else {
@@ -2462,17 +2444,18 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 	return 1;
 }
 
-// the radix passes of the RESP keys sort on {slot | bin} = key bits [30, 40 + slot bits): TD_CODE_BITS + slot bits significant
-// bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible (27 bits -> 7 7 7 6). Not 9 bits, even
-// where that would save a pass: a 9-bit pass has two look-back rows per thread and nine ballots per key.
-static int key_sort_plan(uint32_t max_svcs, SortPlan &P)
+// the radix passes of the RESP keys sort on the slot only = key bits [40, 40 + slot bits), where key_slots covers the services and
+// the trace pseudo-slots: the slot bits cut into the fewest digits of at most KEY_DIGIT_MAX bits, widths as even as possible
+// (17 bits -> 9 8). A 9-bit pass costs more per key than an 8-bit one (two look-back rows per thread, nine ballots per key), but a
+// pass's cost follows the bits it ranks, and a pass fewer saves one read and one write of every key.
+static int key_sort_plan(uint32_t key_slots, SortPlan &P)
 {
 	int slot_bits = 1;
-	while (slot_bits < KEY_SLOT_BITS_MAX && (1ull << slot_bits) < max_svcs) slot_bits++;
-	const int T = TD_CODE_BITS + slot_bits;
+	while (slot_bits < KEY_SLOT_BITS_MAX && (1ull << slot_bits) < key_slots) slot_bits++;
+	const int T = slot_bits;
 	P.np = (T + KEY_DIGIT_MAX - 1) / KEY_DIGIT_MAX;
 	if (P.np > KEY_PASSES_MAX) return -1;
-	int at = KEY_GROUP_SHIFT;
+	int at = KEY_SLOT_SHIFT;
 	for (int p = 0; p < P.np; ++p) { P.bits[p] = T / P.np + (p < T % P.np ? 1 : 0); P.shift[p] = at; at += P.bits[p]; }
 	return 0;
 }
@@ -2701,7 +2684,7 @@ int launch_radix_sort(const SortTemp &tmp, const unsigned long long *d_n, uint64
 	return 1 + launch_sort_passes(P, tmp, d_n, div_up(n_max, SORT_TILE), which, s);
 }
 
-// after the ingest kernel of a batch: sort its RESP keys by {slot, bin}, find every service's key segment, reduce the long ones into
+// after the ingest kernel of a batch: sort its RESP keys by slot, find every service's key segment, reduce the long ones into
 // batch rows and fold every touched service's bins into its window histogram and its digest. Nothing here needs a number from the
 // device on the host: the key count lives in st.counters[CTR_NKEYS], the digit histograms in tmp.os_ghist (both written by
 // ingest_kernel); grids are sized by n_events, the largest possible key count, and surplus CTAs leave at once.
