@@ -82,7 +82,8 @@ enum { CTR_IN = 0, CTR_DROPPED, CTR_RESP, CTR_TCP, CTR_TASK, CTR_FOREIGN, CTR_NK
 	CTR_NHOSTS /* host rows of the last gysk_query_host_listen */, CTR_TASK_NEVICT /* processes evicted by the last flush */,
 	CTR_FLOW_DIRECT /* connection records of the last batch whose count-min update bypassed the flow table */,
 	CTR_FLOWQ_DIRECT /* response samples of the last batch whose flow query update bypassed its flow table (GYSK_FLAG_FLOW_QUERIES) */,
-	CTR_FLOWR_DIRECT /* ... whose flow response histogram update bypassed its flow table (GYSK_FLAG_FLOW_RESP_HIST) */, CTR_MAX };
+	CTR_FLOWR_DIRECT /* ... whose flow response histogram update bypassed its flow table (GYSK_FLAG_FLOW_RESP_HIST) */,
+	CTR_FLOWE_DIRECT /* error samples of the last batch whose flow error update bypassed its flow table (GYSK_FLAG_FLOW_ERRORS) */, CTR_MAX };
 
 // ---------------------------------------------------------------------------------------------------
 // jhash: Bob Jenkins lookup2 in the form the reference uses (common/jhash.h:22-35,121-134); seed 0xceedfead

@@ -71,20 +71,20 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	RecRegions rr;
-	const int li = launch_ingest(e->st, e->tmp, e->fq, e->topk.tk, e->cl, d_ev, n, key_slots(e), rr, e->stream);
+	const int li = launch_ingest(e->st, e->tmp, e->fq, e->topk.tk, e->cl, e->fe.cur != nullptr, d_ev, n, key_slots(e), rr, e->stream);
 	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, e->topk.b_slow, e->cl, rr, n, e->stream);
+	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, e->topk.b_slow, e->cl, e->fe, rr, n, e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);
 	if (pe) CU(e, cudaEventRecord(pe[2], e->stream));
 	// GYSK_FLAG_FLOW_TOPK: each held table's open set from its candidates, once all of the batch's increments are in the table. After the
-	// batch merge, whose sort buffers it takes; GYSK_FLAG_FLOW_TOPK_SLOW's set last, in the same buffers.
+	// batch merge, whose sort buffers it takes; GYSK_FLAG_FLOW_TOPK_SLOW's and GYSK_FLAG_FLOW_ERRORS's sets last, in the same buffers.
 	for (int w = 0; w < TOPK_SETS; ++w) {
-		if (!e->topk.tk.list[w].keys) continue;
-		const int k = launch_topk_select(e->tmp, e->topk.tk.list[w], TOPK_K + n, CMS_TABLES[TOPK_TABLE[w]].live(e), e->cfg.cms_depth,
+		if (!topk_list(e, w).keys) continue;
+		const int k = launch_topk_select(e->tmp, topk_list(e, w), TOPK_K + n, CMS_TABLES[TOPK_TABLE[w]].live(e), e->cfg.cms_depth,
 				e->cfg.cms_log2_width, topk_score(e->topk, w), e->topk.open[w], true, e->stream);
 		if (k < 0) return fail(e, GYSK_ERR_INVAL, "heaviest-flow selection: no sort plan");
 		e->kernel_launches += k;
@@ -308,6 +308,9 @@ int tdigest_out(const TdHead &head, const Centroid *cent, double *means, uint64_
 
 static_assert(sizeof(gysk_flow_qry_est) == sizeof(gysk_flow_est) && offsetof(gysk_flow_qry_est, queries) == offsetof(gysk_flow_est, count) &&
 		offsetof(gysk_flow_qry_est, resp_ms) == offsetof(gysk_flow_est, kbytes), "a flow query row is read as a gysk_flow_est");
+static_assert(sizeof(gysk_flow_err_est) == 24 && offsetof(gysk_flow_err_est, queries) == 8 && offsetof(gysk_flow_err_est, ser_errors) == 16,
+		"gysk_flow_err_est: 24 bytes as documented");
+static_assert(2 * QCHUNK * sizeof(gysk_flow_est) <= STAGE_BYTES, "the stage holds a chunk of error rows and of query rows");
 static_assert(sizeof(gysk_flow_resp_est) == 96 && offsetof(gysk_flow_resp_est, counts) == 8 && offsetof(gysk_flow_resp_est, total) == 68 &&
 		offsetof(gysk_flow_resp_est, p25_ms) == 72 && offsetof(gysk_flow_resp_est, p99_ms) == 88, "gysk_flow_resp_est: 96 bytes as documented");
 
@@ -325,8 +328,37 @@ int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t
 	}, CopyRows<gysk_flow_est> {out});
 }
 
-// a row's score as its set ranks it: the half of a gysk_flow_est, the slow score of a gysk_flow_resp_est (saturated as resp_slow_score)
+// The rows of a flow error read (engine mutex held): per key the point estimate on error table terr and, for queries, on the flow query
+// table tqry of the same window. Both estimates of a piece land in the stage, the error rows first.
+static int err_rows(gysk_engine *e, const unsigned long long *terr, const unsigned long long *tqry, const uint64_t *keys, uint32_t n,
+		gysk_flow_err_est *out, const char *what)
+{
+	const uint32_t d = e->cfg.cms_depth, lw = e->cfg.cms_log2_width;
+	return staged_read(e, keys, n, QCHUNK, 2 * sizeof(gysk_flow_est), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t m) {
+		gysk_flow_est *rows = reinterpret_cast<gysk_flow_est *>(e->d_wstage);
+		return launch_query_flows(terr, d, lw, d_keys, m, rows, e->stream) + launch_query_flows(tqry, d, lw, d_keys, m, rows + m, e->stream);
+	}, [&](const uint8_t *stage, uint32_t off, uint32_t m) {
+		const gysk_flow_est *er = reinterpret_cast<const gysk_flow_est *>(stage), *qr = er + m;
+		for (uint32_t i = 0; i < m; ++i) out[off + i] = gysk_flow_err_est {er[i].flow_key, qr[i].count, er[i].count, er[i].kbytes, 0};
+	});
+}
+
+int query_cms_err(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_err_est *out, const char *what)
+{
+	CHECK_ENGINE(e);
+	if ((!keys || !out) && n) return GYSK_ERR_INVAL;
+	if (!cms_held(e->cfg, t)) return GYSK_ERR_NOTSUP;
+	Entry entry(e, merged ? Pending::Drain : Pending::Submit);
+	if (entry.rc) return entry.rc;
+	if (merged && !e->mg.prepared) return fail(e, GYSK_ERR_INVAL, ("gysk_" + std::string(what) + ": no merge").c_str());
+	const int tq = cms_err_queries(t);
+	return err_rows(e, merged ? e->mg.g_cms[t] : CMS_TABLES[t].live(e), merged ? e->mg.g_cms[tq] : CMS_TABLES[tq].live(e), keys, n, out, what);
+}
+
+// a row's score as its set ranks it: the half of a gysk_flow_est, the slow score of a gysk_flow_resp_est (saturated as resp_slow_score),
+// the server errors of a gysk_flow_err_est
 static uint64_t topk_row_score(const gysk_engine *e, int which, const gysk_flow_est &r) { return TOPK_HALF[which] ? r.kbytes : r.count; }
+static uint64_t topk_row_score(const gysk_engine *, int, const gysk_flow_err_est &r) { return r.ser_errors; }
 static uint64_t topk_row_score(const gysk_engine *e, int, const gysk_flow_resp_est &r)
 {
 	uint64_t s = 0;
@@ -354,7 +386,10 @@ int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merge
 	const int t = level ? TOPK5_LEVEL[which] : TOPK_TABLE[which] + (merged || last_window ? 1 : 0);	// merged: the summed table
 	const unsigned long long *tbl = merged ? e->mg.g_cms[t] : CMS_TABLES[t].live(e);
 	std::vector<Row> rows(m);
-	int rc = staged_read(e, keys.data() + 2, m, QCHUNK, sizeof(Row), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t k) {
+	int rc;
+	if constexpr (std::is_same<Row, gysk_flow_err_est>::value)
+		rc = err_rows(e, tbl, merged ? e->mg.g_cms[cms_err_queries(t)] : CMS_TABLES[cms_err_queries(t)].live(e), keys.data() + 2, m, rows.data(), what);
+	else rc = staged_read(e, keys.data() + 2, m, QCHUNK, sizeof(Row), what, [&](const unsigned long long *d_keys, uint32_t, uint32_t k) {
 		Row *d_out = reinterpret_cast<Row *>(e->d_wstage);
 		if constexpr (std::is_same<Row, gysk_flow_resp_est>::value)
 			return launch_query_flow_resp(tbl, e->cfg.cms_depth, e->cfg.cms_log2_width, d_keys, k, d_out, e->stream);
@@ -369,6 +404,8 @@ int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merge
 }
 template int topk_read<gysk_flow_est>(gysk_engine *, int, int, bool, bool, uint32_t, gysk_flow_est *, uint32_t *, uint64_t *, const char *);
 template int topk_read<gysk_flow_resp_est>(gysk_engine *, int, int, bool, bool, uint32_t, gysk_flow_resp_est *, uint32_t *, uint64_t *,
+		const char *);
+template int topk_read<gysk_flow_err_est>(gysk_engine *, int, int, bool, bool, uint32_t, gysk_flow_err_est *, uint32_t *, uint64_t *,
 		const char *);
 
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what)
@@ -699,6 +736,8 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_SLOW needs GYSK_FLAG_FLOW_TOPK");
 	if ((cfg.flags & GYSK_FLAG_FLOW_TOPK_SLOW) && !(cfg.flags & GYSK_FLAG_FLOW_RESP_HIST))
 		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_TOPK_SLOW needs GYSK_FLAG_FLOW_RESP_HIST");
+	if ((cfg.flags & GYSK_FLAG_FLOW_ERRORS) && !(cfg.flags & GYSK_FLAG_FLOW_QUERIES))
+		return fail(nullptr, GYSK_ERR_INVAL, "GYSK_FLAG_FLOW_ERRORS needs GYSK_FLAG_FLOW_QUERIES");
 
 	int ndev = 0;
 	cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -811,13 +850,14 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 		A(dalloc(e, &tmp.flow, (size_t)tmp.flow_cap));
 		if (cfg.flags & GYSK_FLAG_FLOW_QUERIES) A(dalloc(e, &e->fq.flow, (size_t)tmp.flow_cap));		// the query flow table, alike
 		if (cfg.flags & GYSK_FLAG_FLOW_RESP_HIST) A(dalloc(e, &e->fr.flow, (size_t)tmp.flow_cap));		// the response flow table, alike
+		if (cfg.flags & GYSK_FLAG_FLOW_ERRORS) A(dalloc(e, &e->fe.flow, (size_t)tmp.flow_cap));		// the error flow table, alike
 		// GYSK_FLAG_FLOW_TOPK: per held table its candidate list, the keys beside its batch flow table and its two sets, all empty.
 		// GYSK_FLAG_FLOW_TOPK_SLOW: the slow set's alike, without keys beside a flow table (a slow sample appends once per record, so
-		// cap = K + max_batch holds every one), at the default threshold.
+		// cap = K + max_batch holds every one), at the default threshold. GYSK_FLAG_FLOW_ERRORS: the server-error set's, as the slow set's.
 		e->topk.b_slow = TOPK_SLOW_DEFAULT_B;
 		for (int w = 0; w < TOPK_SETS && (cfg.flags & GYSK_FLAG_FLOW_TOPK); ++w) {
 			if (!cms_held(cfg, TOPK_TABLE[w]) || (w == 2 && !(cfg.flags & GYSK_FLAG_FLOW_TOPK_SLOW))) continue;
-			TopkList &l = e->topk.tk.list[w];
+			TopkList &l = topk_list(e, w);
 			l.cap = (uint64_t)TOPK_K + cfg.max_batch;
 			A(dalloc(e, &l.keys, (size_t)l.cap, false)); A(dalloc(e, &l.n, 1));
 			if (w < 2) A(dalloc(e, &l.ekeys, (size_t)tmp.flow_cap, false));
@@ -974,15 +1014,23 @@ int64_t gysk_last_batch_flow_resp_direct(gysk_engine *e)
 	return read_counter(e, CTR_FLOWR_DIRECT);
 }
 
-// diagnostic: entries of the flow table (and of the query and response flow tables, GYSK_FLAG_FLOW_QUERIES / GYSK_FLAG_FLOW_RESP_HIST)
-// that are not zero (a key or a sum left behind); 0 whenever no batch is in flight
+// diagnostic (GYSK_FLAG_FLOW_ERRORS): error samples of the last device batch whose flow error update bypassed the error flow table
+int64_t gysk_last_batch_flow_err_direct(gysk_engine *e)
+{
+	CHECK_ENGINE(e);
+	if (!cms_held(e->cfg, CMS_ERR_CUR)) return GYSK_ERR_NOTSUP;
+	return read_counter(e, CTR_FLOWE_DIRECT);
+}
+
+// diagnostic: entries of the flow table (and of the query, response and error flow tables, GYSK_FLAG_FLOW_QUERIES /
+// GYSK_FLAG_FLOW_RESP_HIST / GYSK_FLAG_FLOW_ERRORS) that are not zero (a key or a sum left behind); 0 whenever no batch is in flight
 int64_t gysk_flow_table_used(gysk_engine *e)
 {
 	CHECK_ENGINE(e);
 	GYSK_ENTER(e, Sync);
 	std::vector<FlowEnt> t(e->tmp.flow_cap);
 	int64_t used = 0;
-	for (const FlowEnt *tbl : {e->tmp.flow, e->fq.flow, e->fr.flow}) {
+	for (const FlowEnt *tbl : {e->tmp.flow, e->fq.flow, e->fr.flow, e->fe.flow}) {
 		if (!tbl) continue;
 		CU(e, cudaMemcpy(t.data(), tbl, t.size() * sizeof(FlowEnt), cudaMemcpyDeviceToHost));
 		used += (int64_t)std::count_if(t.begin(), t.end(), [](const FlowEnt &f) { return f.key || f.inc; });
@@ -1770,7 +1818,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		if (!e->topk5.level[w]) continue;
 		if (int rc = topk5_roll(e, w)) return rc;
 	}
-	for (int t : {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
+	for (int t : {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR, CMS_ERR_CUR}) {		// each windowed pair: the open window closes, a cleared one opens
 		if (!cms_held(e->cfg, t)) continue;
 		unsigned long long *&open = CMS_TABLES[t].live(e);
 		std::swap(open, CMS_TABLES[t + 1].live(e));
@@ -1780,7 +1828,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		if (!e->topk.open[w]) continue;
 		std::swap(e->topk.open[w], e->topk.last[w]);
 		CU(e, cudaMemsetAsync(e->topk.open[w], 0, sizeof(unsigned long long) * TOPK_SET_WORDS, e->stream));
-		CU(e, cudaMemsetAsync(e->topk.tk.list[w].n, 0, sizeof(unsigned long long), e->stream));
+		CU(e, cudaMemsetAsync(topk_list(e, w).n, 0, sizeof(unsigned long long), e->stream));
 	}
 	return post_launch(e, "flush");
 }
@@ -2400,6 +2448,38 @@ int gysk_query_flow_resp_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, 
 int gysk_export_cms_resp_5min(gysk_engine *e, uint64_t *words)
 {
 	return export_cms(e, CMS_RESP_5MIN, words);
+}
+
+// GYSK_FLAG_FLOW_ERRORS: the point query on the flow error tables (with the queries of the same window), their cells, the same on their
+// rolling 300-s level, and the flows with the most server errors
+int gysk_query_flow_errors(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_err_est *out)
+{
+	return query_cms_err(e, last_window ? CMS_ERR_LAST : CMS_ERR_CUR, false, keys, n, out, "query_flow_errors");
+}
+
+int gysk_query_flow_errors_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_err_est *out)
+{
+	return query_cms_err(e, CMS_ERR_5MIN, false, keys, n, out, "query_flow_errors_5min");
+}
+
+int gysk_export_cms_errors(gysk_engine *e, int last_window, uint64_t *cells)
+{
+	return export_cms(e, last_window ? CMS_ERR_LAST : CMS_ERR_CUR, cells);
+}
+
+int gysk_export_cms_errors_5min(gysk_engine *e, uint64_t *cells)
+{
+	return export_cms(e, CMS_ERR_5MIN, cells);
+}
+
+int gysk_topk_flow_errors(gysk_engine *e, int last_window, uint32_t n, gysk_flow_err_est *out, uint32_t *nout)
+{
+	return topk_read(e, 3, last_window, false, false, n, out, nout, nullptr, "topk_flow_errors");
+}
+
+int gysk_topk_flow_errors_5min(gysk_engine *e, uint32_t n, gysk_flow_err_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 3, 0, true, false, n, out, nout, bound, "topk_flow_errors_5min");
 }
 
 // ---- pure helpers ------------------------------------------------------------------------------------------------

@@ -242,19 +242,23 @@ constexpr uint32_t TOPN_SLAB_ENTRIES = (uint32_t)((TopnLists::BYTES + sizeof(Sla
 // which flag each one needs, its array in the merge arena, where the engine keeps it and its words per cell). Each windowed pair is an
 // open table and, right after it, the table of the window the last flush closed. A new table goes last, so that every engine without it
 // keeps its merge arena.
-enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, CMS_RESP_CUR, CMS_RESP_LAST, CMS_RESP_5MIN, NCMS };
+enum CmsTable { CMS_CUR, CMS_LAST, CMS_5MIN, CMS_QRY_CUR, CMS_QRY_LAST, CMS_QRY_5MIN, CMS_RESP_CUR, CMS_RESP_LAST, CMS_RESP_5MIN, CMS_ERR_CUR,
+	CMS_ERR_LAST, CMS_ERR_5MIN, NCMS };
+// the flow query table of the same window as flow error table t (gysk_flow_err_est.queries)
+constexpr int cms_err_queries(int t) { return t - CMS_ERR_CUR + CMS_QRY_CUR; }
 
 // GYSK_FLAG_FLOW_TOPK (every pointer nullptr without): the candidate lists and the open / last heaviest-flow sets ([TOPK_SET_WORDS]
 // each) of the connection table [0] and, with GYSK_FLAG_FLOW_QUERIES, the flow query table [1]; with GYSK_FLAG_FLOW_TOPK_SLOW the slow
-// set of the response histogram table [2], b_slow its first slow bucket (gysk_set_flow_slow). Outside DevState, so that the kernels
-// without the flag keep their parameter layout; not per slot, so gysk_grow and eviction leave them.
-struct TopkSets { FlowTopk tk; unsigned long long *open[3], *last[3]; uint32_t b_slow; };
-constexpr int TOPK_SETS = 3;
+// set of the response histogram table [2], b_slow its first slow bucket (gysk_set_flow_slow); with GYSK_FLAG_FLOW_ERRORS the server-error
+// set of the flow error table [3] (its candidates are FlowErrors::list, topk_list). Outside DevState, so that the kernels without the
+// flag keep their parameter layout; not per slot, so gysk_grow and eviction leave them.
+constexpr int TOPK_SETS = 4;
+struct TopkSets { FlowTopk tk; unsigned long long *open[TOPK_SETS], *last[TOPK_SETS]; uint32_t b_slow; };
 // the count-min table of each set, and the half of its cells that scores (1: kbytes, the high half; 0: queries, the low half; the slow
-// set's score is topk_score's)
-constexpr int TOPK_TABLE[TOPK_SETS] = {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR}, TOPK_HALF[2] = {1, 0};
+// set's score is topk_score's; 1: ser_errors, the high half)
+constexpr int TOPK_TABLE[TOPK_SETS] = {CMS_CUR, CMS_QRY_CUR, CMS_RESP_CUR, CMS_ERR_CUR}, TOPK_HALF[TOPK_SETS] = {1, 0, 0, 1};
 // the score of set w (launch_topk_select): TOPK_HALF[w], or the slow score from bucket b_slow
-inline int topk_score(const TopkSets &t, int w) { return w < 2 ? TOPK_HALF[w] : TOPK_SCORE_SLOW | (int)t.b_slow; }
+inline int topk_score(const TopkSets &t, int w) { return w != 2 ? TOPK_HALF[w] : TOPK_SCORE_SLOW | (int)t.b_slow; }
 // GYSK_FLAG_FLOW_TOPK_SLOW's default threshold: a sample above 300 ms is slow (RESP_TIME_HASH bucket 9 and up)
 constexpr uint32_t TOPK_SLOW_DEFAULT_B = 9;
 // nsets sets of a rank in the merge slab, in whole SlabEntrys after the rest of its content
@@ -268,10 +272,11 @@ constexpr uint32_t TOPK_SLAB_ENTRIES = topk_slab_entries(2);
 // its NSLOTS ring slots ([NSLOTS][TOPK_SET_WORDS], word 1 each slot's bound B_s) and the level set L ([TOPK_SET_WORDS], word 1 B_L);
 // one candidate list of NSLOTS x K keys for the flush chain, and a word for its partial bound. Outside DevState and not per slot, as
 // TopkSets.
-// [2]: GYSK_FLAG_FLOW_TOPK_SLOW's slow set of the response level (with GYSK_FLAG_FLOW_QUERY_LEVEL), scored as the window's.
+// [2]: GYSK_FLAG_FLOW_TOPK_SLOW's slow set of the response level (with GYSK_FLAG_FLOW_QUERY_LEVEL), scored as the window's; [3]:
+// GYSK_FLAG_FLOW_ERRORS's server-error set of the error level, alike.
 struct Topk5min { unsigned long long *slots[TOPK_SETS], *level[TOPK_SETS]; TopkList list; unsigned long long *acc; };
 // the level table of each set (the score is topk_score's)
-constexpr int TOPK5_LEVEL[TOPK_SETS] = {CMS_5MIN, CMS_QRY_5MIN, CMS_RESP_5MIN};
+constexpr int TOPK5_LEVEL[TOPK_SETS] = {CMS_5MIN, CMS_QRY_5MIN, CMS_RESP_5MIN, CMS_ERR_5MIN};
 
 // the cells of one count-min table
 inline size_t cms_cells(const gysk_config &cfg) { return (size_t)cfg.cms_depth << cfg.cms_log2_width; }
@@ -325,6 +330,10 @@ struct MergeState
 	// GYSK_FLAG_FLOW_TOPK_SLOW: the rank's last-window slow set and, with its 300-s level, L with B_L ride from slab entry topks_off
 	// (topk_slab_entries(1 or 2)); the merged ones land as set [2] of topk_final and topk5_final, which then hold three sets.
 	uint32_t		topks_off {0};
+	// GYSK_FLAG_FLOW_ERRORS with GYSK_FLAG_FLOW_TOPK: the rank's last-window server-error set and, with its 300-s level, L with B_L ride
+	// from slab entry topke_off, after the slow sets (topk_slab_entries(1 or 2)); the merged ones land as set [3] of topk_final and
+	// topk5_final, which then hold four sets.
+	uint32_t		topke_off {0};
 	// GYSK_FLAG_CLIENT_LEVELS: MAX [nl][2][CL_REGS] in the u8 MAX region after the all-time registers, each logical service's last-window
 	// and 300-s client sets (nullptr without)
 	uint8_t			*cl_hll {nullptr};
@@ -345,6 +354,7 @@ struct gysk_engine
 	gysk::TopkSets		topk {};			// GYSK_FLAG_FLOW_TOPK (every pointer nullptr without)
 	gysk::Topk5min		topk5 {};			// GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without)
 	gysk::ClientLevels	cl {};				// GYSK_FLAG_CLIENT_LEVELS (every pointer nullptr without)
+	gysk::FlowErrors	fe {};				// GYSK_FLAG_FLOW_ERRORS (every pointer nullptr without)
 	std::atomic<bool>	fed {false};			// an event was handed in or gysk_flush ran (gysk_set_flow_slow refuses after)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
@@ -443,6 +453,9 @@ inline const CmsTableDesc CMS_TABLES[NCMS] = {
 	{GYSK_FLAG_FLOW_RESP_HIST, "cms_resp_last", [](gysk_engine *e) -> unsigned long long *& { return e->fr.last; }, RESP_HIST_WORDS},
 	{GYSK_FLAG_FLOW_RESP_HIST | GYSK_FLAG_FLOW_QUERY_LEVEL, "cms_resp_5min", [](gysk_engine *e) -> unsigned long long *& { return e->fr.level; },
 			RESP_HIST_WORDS},
+	{GYSK_FLAG_FLOW_ERRORS, "cms_err_cur", [](gysk_engine *e) -> unsigned long long *& { return e->fe.cur; }, 1},
+	{GYSK_FLAG_FLOW_ERRORS, "cms_err_last", [](gysk_engine *e) -> unsigned long long *& { return e->fe.last; }, 1},
+	{GYSK_FLAG_FLOW_ERRORS | GYSK_FLAG_FLOW_QUERY_LEVEL, "cms_err_5min", [](gysk_engine *e) -> unsigned long long *& { return e->fe.level; }, 1},
 };
 inline bool cms_held(const gysk_config &cfg, int t) { return (cfg.flags & CMS_TABLES[t].flag) == CMS_TABLES[t].flag; }
 // the u64 words of count-min table t
@@ -460,7 +473,11 @@ inline const CmsRingDesc CMS_RINGS[] = {
 	{CMS_CUR, CMS_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->st.cms_ring; }},
 	{CMS_QRY_CUR, CMS_QRY_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->fq.ring; }},
 	{CMS_RESP_CUR, CMS_RESP_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->fr.ring; }},
+	{CMS_ERR_CUR, CMS_ERR_5MIN, [](gysk_engine *e) -> unsigned long long *& { return e->fe.ring; }},
 };
+
+// the candidate list of heaviest-flow set w: FlowTopk's, or for the server-error set FlowErrors'
+inline TopkList &topk_list(gysk_engine *e, int w) { return w < 3 ? e->topk.tk.list[w] : e->fe.list; }
 
 int fail(gysk_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess);
 int post_launch(gysk_engine *e, const char *what);
@@ -485,10 +502,12 @@ int query_cms(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t
 // first, with their estimates on its table: the engine's open (last_window = 0) or last set, or merged, the last finished merge's set on
 // the summed table. level (GYSK_FLAG_FLOW_TOPK_5MIN): the 300-s level set instead, on the level (merged: the summed level), last_window
 // ignored. Flows with a zero score are left out; *bound (if not nullptr) = the set's word 1. Row: gysk_flow_est for sets 0 and 1,
-// gysk_flow_resp_est for set 2.
+// gysk_flow_resp_est for set 2, gysk_flow_err_est for set 3 (server errors).
 template <typename Row>
 int topk_read(gysk_engine *e, int which, int last_window, bool level, bool merged, uint32_t n, Row *out, uint32_t *nout,
 		uint64_t *bound, const char *what);
+// the same on a flow error table (CMS_ERR_*), each row's queries from the flow query table of the same window
+int query_cms_err(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_err_est *out, const char *what);
 // the same on a flow response histogram table (CMS_RESP_*)
 int query_cms_resp(gysk_engine *e, int t, bool merged, const uint64_t *keys, uint32_t n, gysk_flow_resp_est *out, const char *what);
 

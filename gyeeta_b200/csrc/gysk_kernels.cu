@@ -415,10 +415,15 @@ __device__ __forceinline__ void flow_add(const DevState &st, const FlowTable &ft
 // candidates tk.list[2], once per record (the selection's key sort removes the repeats).
 // CL (GYSK_FLAG_CLIENT_LEVELS): a connection record also raises the open window's client register (cl_open, precision GYSK_HLL_WINDOW_P),
 // from the same mixed hash; its word is asked for beside the all-time one and taken with the same policy.
-template <bool QRY, bool RH, bool TOPK, bool SLOW, bool CL, typename HotTable>
+// ERR (GYSK_FLAG_FLOW_ERRORS, only with QRY): a response sample's value carries its error bits (QRY_CLI_ERR, QRY_SER_ERR), masked off
+// before its msec and bucket are taken; a sample with either bit adds {cli | ser << 32} to its flow's entry of the error flow table
+// ep.ft (cells ep.cms past the probe limit), under the query table's key, and one with the server-error bit appends its flow key to the
+// server-error set's candidates ep.list when they are held.
+struct ErrPass { FlowTable ft; unsigned long long *cms; TopkList list; };
+template <bool QRY, bool RH, bool TOPK, bool SLOW, bool CL, bool ERR, typename HotTable>
 __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTable &ft, HotTable &hot, const IngestRec *q, uint32_t m,
 		int lane, unsigned long long pol_hll, unsigned long long pol_last, const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr,
-		unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow, uint8_t *cl_open)
+		unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow, uint8_t *cl_open, const ErrPass &ep)
 {
 	for (uint32_t i = lane; i < ((m + 31u) & ~31u); i += 32) {
 		const bool act = i < m;
@@ -426,10 +431,13 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 		uint32_t cell = 0, idx = 0, rank = 0, hw = 0, pos = 0, rpos = 0; int kb = 0;
 		uint32_t widx = 0, wrank = 0, ww = 0;
 		unsigned long long key = 0, inc = 0, k = 0, rkey = 0, rk = 0, rinc = 0, fk = 0;
+		uint32_t eb = 0, epos = 0;
+		unsigned long long ek = 0;
 		if (act) {
-			const IngestRec r = ld_rec(q + i);
+			IngestRec r = ld_rec(q + i);
 			fk = r.flow_key;
 			qry = QRY && r.slot == QRY_REC;
+			if (ERR && qry) { eb = r.value >> 30; r.value &= QRY_USEC_MASK; }
 			FlowEnt *const tent = qry ? fq.ent : ft.ent;		// field by field: a selected reference would copy both tables to the stack
 			const uint32_t tmask = qry ? fq.mask : ft.mask;
 			uint32_t h1, h2;
@@ -459,6 +467,11 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 				rk = ld_cg_hint_u64(&fr.ent[rpos].key, pol_last);
 				if (SLOW && b >= b_slow) topk_append(tk.list[2], fk);
 			}
+			if (ERR && eb) {
+				epos = table_hash(key) & ep.ft.mask;
+				if (key) ek = ld_cg_hint_u64(&ep.ft.ent[epos].key, pol_last);
+				if (ep.list.keys && (eb & 2u)) topk_append(ep.list, fk);
+			}
 			cell = r.slot;
 			kb = (int)(r.value >> 10);
 		}
@@ -471,6 +484,8 @@ __device__ __forceinline__ void drain_tcp_recs(const DevState &st, const FlowTab
 			else if (qry) flow_add(st, fq, CmsApply {st, fq_cms}, CTR_FLOWQ_DIRECT, key, pos, k, inc, pol_last);
 			else flow_add(st, ft, CmsApply {st, st.cms_cur}, CTR_FLOW_DIRECT, key, pos, k, inc, pol_last);
 			if (RH && qry) flow_add(st, fr, RespHistApply {st, fr_cms}, CTR_FLOWR_DIRECT, rkey, rpos, rk, rinc, pol_last);
+			if (ERR && eb) flow_add(st, ep.ft, CmsApply {st, ep.cms}, CTR_FLOWE_DIRECT, key, epos, ek, (eb & 1u) | ((unsigned long long)(eb >> 1) << 32),
+					pol_last);
 		}
 		if (act && !qry) hll_raise(st.hll + ((size_t)cell << st.hll_p), idx, rank, hw);
 		if (CL && act && !qry) hll_raise(cl_open + (size_t)cell * CL_REGS, widx, wrank, ww);
@@ -583,11 +598,13 @@ struct IngestShared
 // hot-row route, also joins the connection queue as a record {QRY_REC, usec, flow key} for the TCP drain pass.
 // TOPK: GYSK_FLAG_FLOW_TOPK (a separate instance too): the flow key of each ACTIVE record, which updates the count-min here, joins the
 // connection table's candidates tl.
+// ERR: GYSK_FLAG_FLOW_ERRORS (a separate instance too, only with QRY): a queued response sample also carries its event's GYSK_EVF_CLI_ERROR
+// / GYSK_EVF_SER_ERROR bits in bits 30 / 31 of its value (QRY_CLI_ERR, QRY_SER_ERR).
 // ClOpen: GYSK_FLAG_CLIENT_LEVELS (a separate instance too) with one uint8_t * parameter, the open window's client registers, which each
 // ACTIVE record also raises. A pack, so that the instances without the flag keep their parameter list.
 __device__ __forceinline__ uint8_t *cl_open_of() { return nullptr; }
 __device__ __forceinline__ uint8_t *cl_open_of(uint8_t *p) { return p; }
-template <bool TRACE, bool QRY, bool TOPK, typename... ClOpen>
+template <bool TRACE, bool QRY, bool TOPK, bool ERR, typename... ClOpen>
 __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS) ingest_kernel(DevState st, const gysk_event *__restrict__ ev, uint64_t n,
 		unsigned long long *__restrict__ keys, uint32_t *__restrict__ ghist, SortPlan plan, uint4 *__restrict__ recq, uint2 *__restrict__ rec_cnt, TopkList tl,
 		ClOpen... cl_open)
@@ -751,7 +768,7 @@ __global__ void __launch_bounds__(IngestShape::WARPS * 32, IngestShape::MIN_CTAS
 					const uint32_t ef = rb[k].w >> 16;			// API_TRAN error flags: rare
 					if (ef & 3u) red_add_u64(&st.slot_aux[slot].err_cur, (unsigned long long)(ef & 1u) | ((unsigned long long)((ef >> 1) & 1u) << 32));
 					if (QRY) {
-						IngestRec r; r.slot = QRY_REC; r.value = v; r.flow_key = ((unsigned long long)ra[k].w << 32) | ra[k].z;
+						IngestRec r; r.slot = QRY_REC; r.value = ERR ? v | ((ef & 3u) << 30) : v; r.flow_key = ((unsigned long long)ra[k].w << 32) | ra[k].z;
 						W.tcp[ntcp + __popc(m_tcp & lt)] = r;
 					}
 				}
@@ -891,9 +908,13 @@ __device__ __forceinline__ void flow_sweep(const FlowTable &t, const Apply &appl
 // sweeps append the key beside each applied entry to that table's candidates tk.
 // SLOW (GYSK_FLAG_FLOW_TOPK_SLOW, TCP pass only): the TCP pass also keeps the flow key of each response sample in bucket b_slow or above.
 // CL (GYSK_FLAG_CLIENT_LEVELS, TCP pass only): the TCP pass also raises the open window's client registers cl_open.
-template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL>
+// ERR (GYSK_FLAG_FLOW_ERRORS, only with QRY): the TCP pass also sums the error samples in the error flow table ep.ft (drain_tcp_recs), and
+// the TASK pass applies that table to the error cells ep.cms after the others. A trailing parameter, so that the instances without the
+// flag keep their parameter layout.
+template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL, bool ERR>
 __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(DevState st, FlowTable ft, const uint4 *__restrict__ q, const uint2 *__restrict__ cnt,
-		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk, uint32_t b_slow, uint8_t *cl_open)
+		RecRegions rr, FlowTable fq, unsigned long long *fq_cms, FlowTable fr, unsigned long long *fr_cms, FlowTopk tk, uint32_t b_slow, uint8_t *cl_open,
+		ErrPass ep)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	using DrainHot = HotTableT<DrainShape<TASK>::HOT_BITS>;
@@ -901,11 +922,13 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		flow_sweep(ft, CmsApply {st, st.cms_cur}, TopkCapture {tk.list[0]});
 		if (QRY) flow_sweep(fq, CmsApply {st, fq_cms}, TopkCapture {tk.list[1]});
 		if (RH) flow_sweep(fr, RespHistApply {st, fr_cms});
+		if (ERR) flow_sweep(ep.ft, CmsApply {st, ep.cms});
 	}
 	else if (TASK) {
 		flow_sweep(ft, CmsApply {st, st.cms_cur});
 		if (QRY) flow_sweep(fq, CmsApply {st, fq_cms});
 		if (RH) flow_sweep(fr, RespHistApply {st, fr_cms});
+		if (ERR) flow_sweep(ep.ft, CmsApply {st, ep.cms});
 	}
 	const unsigned long long pol_hll = TASK ? 0 : l2_policy_evict_first(), pol_last = TASK ? 0 : l2_policy_evict_last();
 	extern __shared__ __align__(16) unsigned char drain_smem[];
@@ -972,8 +995,8 @@ __global__ void __launch_bounds__(DrainShape<TASK>::WARPS * 32) drain_kernel(Dev
 		for (uint32_t g = gbeg; g < gend; ++g) {
 			uint32_t off, m;
 			locate(g, off, m);
-			drain_tcp_recs<QRY, RH, TOPK, SLOW, CL>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr, fr_cms,
-					tk, b_slow, cl_open);
+			drain_tcp_recs<QRY, RH, TOPK, SLOW, CL, ERR>(st, ft, hot, recs + (unsigned long long)r * rr.cap + off, m, lane, pol_hll, pol_last, fq, fq_cms, fr,
+					fr_cms, tk, b_slow, cl_open, ep);
 		}
 	}
 
@@ -2477,8 +2500,8 @@ static int plain_sort_plan(int lo, int hi, SortPlan &P)
 	return 0;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, const gysk_event *d_ev,
-		uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, bool err,
+		const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
 	const int dev = current_device();
@@ -2495,16 +2518,23 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	using IngestClFn = void (*)(DevState, const gysk_event *, uint64_t, unsigned long long *, uint32_t *, SortPlan, uint4 *, uint2 *, TopkList, uint8_t *);
 	// [TRACE][QRY][TOPK]; fns_cl: the instances of GYSK_FLAG_CLIENT_LEVELS
 	static const IngestFn fns[2][2][2] = {
-		{{ingest_kernel<false, false, false>, ingest_kernel<false, false, true>}, {ingest_kernel<false, true, false>, ingest_kernel<false, true, true>}},
-		{{ingest_kernel<true, false, false>, ingest_kernel<true, false, true>}, {ingest_kernel<true, true, false>, ingest_kernel<true, true, true>}}};
+		{{ingest_kernel<false, false, false, false>, ingest_kernel<false, false, true, false>},
+		 {ingest_kernel<false, true, false, false>, ingest_kernel<false, true, true, false>}},
+		{{ingest_kernel<true, false, false, false>, ingest_kernel<true, false, true, false>},
+		 {ingest_kernel<true, true, false, false>, ingest_kernel<true, true, true, false>}}};
 	static const IngestClFn fns_cl[2][2][2] = {
-		{{ingest_kernel<false, false, false, uint8_t *>, ingest_kernel<false, false, true, uint8_t *>},
-		 {ingest_kernel<false, true, false, uint8_t *>, ingest_kernel<false, true, true, uint8_t *>}},
-		{{ingest_kernel<true, false, false, uint8_t *>, ingest_kernel<true, false, true, uint8_t *>},
-		 {ingest_kernel<true, true, false, uint8_t *>, ingest_kernel<true, true, true, uint8_t *>}}};
-	// the instances of GYSK_FLAG_FLOW_TOPK and GYSK_FLAG_CLIENT_LEVELS only once an engine with the flag launches: setting a kernel's
-	// attribute loads it, which can wait for the work already on the device
-	static bool topk_attr_set[MAX_DEVICES] = {}, cl_attr_set[MAX_DEVICES] = {};
+		{{ingest_kernel<false, false, false, false, uint8_t *>, ingest_kernel<false, false, true, false, uint8_t *>},
+		 {ingest_kernel<false, true, false, false, uint8_t *>, ingest_kernel<false, true, true, false, uint8_t *>}},
+		{{ingest_kernel<true, false, false, false, uint8_t *>, ingest_kernel<true, false, true, false, uint8_t *>},
+		 {ingest_kernel<true, true, false, false, uint8_t *>, ingest_kernel<true, true, true, false, uint8_t *>}}};
+	// GYSK_FLAG_FLOW_ERRORS (QRY only): [TRACE][TOPK], and with GYSK_FLAG_CLIENT_LEVELS
+	static const IngestFn fns_err[2][2] = {{ingest_kernel<false, true, false, true>, ingest_kernel<false, true, true, true>},
+					       {ingest_kernel<true, true, false, true>, ingest_kernel<true, true, true, true>}};
+	static const IngestClFn fns_err_cl[2][2] = {{ingest_kernel<false, true, false, true, uint8_t *>, ingest_kernel<false, true, true, true, uint8_t *>},
+						    {ingest_kernel<true, true, false, true, uint8_t *>, ingest_kernel<true, true, true, true, uint8_t *>}};
+	// the instances of GYSK_FLAG_FLOW_TOPK, GYSK_FLAG_CLIENT_LEVELS and GYSK_FLAG_FLOW_ERRORS only once an engine with the flag launches:
+	// setting a kernel's attribute loads it, which can wait for the work already on the device
+	static bool topk_attr_set[MAX_DEVICES] = {}, cl_attr_set[MAX_DEVICES] = {}, err_attr_set[MAX_DEVICES] = {};
 	const int topk = tk.list[0].keys ? 1 : 0;
 	if (!attr_set[dev]) {
 		for (const IngestFn f : {fns[0][0][0], fns[1][0][0], fns[0][1][0], fns[1][1][0]})
@@ -2521,6 +2551,13 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 			cudaFuncSetAttribute(fns_cl[i >> 2][(i >> 1) & 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
 		cl_attr_set[dev] = true;
 	}
+	if (err && !err_attr_set[dev]) {
+		for (int i = 0; i < 4; ++i) {
+			cudaFuncSetAttribute(fns_err[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+			cudaFuncSetAttribute(fns_err_cl[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+		}
+		err_attr_set[dev] = true;
+	}
 	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
 	const uint64_t full = (uint64_t)sm_count(dev) * IngestShape::MIN_CTAS;
 	const uint32_t grid = (uint32_t)(want < full ? want : full);
@@ -2531,7 +2568,11 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
 	// a counted response sample takes a connection-queue entry, as one connection event does: the regions hold one record per event
 	const int tr = st.trace.rows ? 1 : 0, qr = fq.cur ? 1 : 0;
-	if (cl.open) fns_cl[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
+	if (err && cl.open) fns_err_cl[tr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq,
+			tmp.rec_cnt, tk.list[0], cl.open);
+	else if (err) fns_err[tr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
+			tk.list[0]);
+	else if (cl.open) fns_cl[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
 			tk.list[0], cl.open);
 	else fns[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, tk.list[0]);
 	return 1;
@@ -2539,65 +2580,68 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 
 // one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
 // table + the region start table, whose largest size sets the occupancy
-template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL = false>
+template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL, bool ERR>
 static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		cudaStream_t s, uint8_t *cl_open = nullptr)
+		cudaStream_t s, uint8_t *cl_open, const ErrPass &ep)
 {
 	constexpr int WARPS = DrainShape<TASK>::WARPS;
 	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
 	static int per_sm[MAX_DEVICES] = {};
 	if (!per_sm[dev]) {
 		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
 		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL>, WARPS * 32, smem_max);
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR>, WARPS * 32, smem_max);
 		per_sm[dev] = b > 0 ? b : 1;
 	}
 	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
 	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
 	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr, fq,
-			fq_cms, fr, fr_cms, tk, b_slow, cl_open);
+	drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr,
+			fq, fq_cms, fr, fr_cms, tk, b_slow, cl_open, ep);
 }
 
 // b_slow: GYSK_FLAG_FLOW_TOPK_SLOW's first slow bucket when tk.list[2] is held (RH only); the TASK pass is the TOPK one either way.
 // cl_open (CL, GYSK_FLAG_CLIENT_LEVELS): the TCP pass's client registers; the TASK pass does not touch them.
-template <bool QRY, bool RH, bool CL>
+// ep (ERR, GYSK_FLAG_FLOW_ERRORS): the error flow table, cells and candidates (both passes).
+template <bool QRY, bool RH, bool CL, bool ERR>
 static int launch_drain_passes_t(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		uint8_t *cl_open, cudaStream_t s)
+		uint8_t *cl_open, const ErrPass &ep, cudaStream_t s)
 {
 	if (tk.list[0].keys) {
 		if constexpr (RH) {
-			if (tk.list[2].keys) launch_drain_pass<false, QRY, RH, true, true, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, s, cl_open);
-			else launch_drain_pass<false, QRY, RH, true, false, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open);
+			if (tk.list[2].keys) launch_drain_pass<false, QRY, RH, true, true, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, s, cl_open, ep);
+			else launch_drain_pass<false, QRY, RH, true, false, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open, ep);
 		}
-		else launch_drain_pass<false, QRY, RH, true, false, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open);
-		launch_drain_pass<true, QRY, RH, true, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		else launch_drain_pass<false, QRY, RH, true, false, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open, ep);
+		launch_drain_pass<true, QRY, RH, true, false, false, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, nullptr, ep);
 	}
 	else {
-		launch_drain_pass<false, QRY, RH, false, false, CL>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open);
-		launch_drain_pass<true, QRY, RH, false, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s);
+		launch_drain_pass<false, QRY, RH, false, false, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open, ep);
+		launch_drain_pass<true, QRY, RH, false, false, false, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, nullptr, ep);
 	}
 	return 2;
 }
-template <bool QRY, bool RH>
+template <bool QRY, bool RH, bool ERR = false>
 static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
 		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		uint8_t *cl_open, cudaStream_t s)
+		uint8_t *cl_open, cudaStream_t s, const ErrPass &ep = ErrPass {})
 {
-	if (cl_open) return launch_drain_passes_t<QRY, RH, true>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, cl_open, s);
-	return launch_drain_passes_t<QRY, RH, false>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, nullptr, s);
+	if (cl_open) return launch_drain_passes_t<QRY, RH, true, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, cl_open, ep, s);
+	return launch_drain_passes_t<QRY, RH, false, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, nullptr, ep, s);
 }
 
 // the batch's queued connection records -> flow table, HLL, exact cells; then the flow table -> count-min and its process records ->
 // process histograms. The TASK pass always runs: it leaves the flow table empty. The table takes the smallest power of two >= 2 x the
 // batch's events (the flows are fewer than the connection records), up to what tmp holds, so that a small batch sweeps a small table.
 // With GYSK_FLAG_FLOW_QUERIES (fq.cur) the queued response samples go the same way through a query flow table of the same size, and
-// with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too.
+// with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too. With GYSK_FLAG_FLOW_ERRORS (fe.cur) the error
+// samples go through an error flow table of that size as well: a batch whose samples all carry an error bit needs every entry the query
+// table needs (DESIGN.md section 7).
 int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
-		const ClientLevels &cl, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
+		const ClientLevels &cl, const FlowErrors &fe, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
 	const int dev = current_device();
@@ -2609,6 +2653,14 @@ int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, 0, cl.open, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
 	const FlowTable fqt {fq.flow, n - 1u};
+	if (fe.cur) {
+		cudaMemsetAsync(st.counters + CTR_FLOWE_DIRECT, 0, sizeof(unsigned long long), s);
+		const ErrPass ep {FlowTable {fe.flow, n - 1u}, fe.cur, fe.list};
+		if (fr.cur) cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
+		if (!fr.cur) return launch_drain_passes<true, false, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, cl.open, s, ep);
+		return launch_drain_passes<true, true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, cl.open,
+				s, ep);
+	}
 	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, cl.open, s);
 	cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
 	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, cl.open, s);

@@ -167,6 +167,7 @@ static constexpr uint32_t QRY_REC = 0xFFFFFFFFu;	// slot field of a queued respo
 // DevState as FlowQueries; every pointer nullptr: off. ring and level: with GYSK_FLAG_FLOW_QUERY_LEVEL too, the rolling 300-s level.
 struct FlowRespHist { unsigned long long *cur, *last; FlowEnt *flow; unsigned long long *ring, *level; };
 static constexpr uint32_t RESP_HIST_WORDS = 8;
+
 static constexpr uint32_t CMS_LOG2W_MAX = 28;		// the widest count-min gysk_create accepts (1 << 28 columns)
 
 // GYSK_FLAG_FLOW_TOPK: the candidates of one windowed table's heaviest-flow set in a batch. keys [0, *n) hold the open set (written at the
@@ -185,6 +186,16 @@ struct FlowTopk { TopkList list[3]; };
 // estimate); TOPK_SCORE_SLOW | b_slow the slow score of a response histogram table, the sum of its bucket counts from b_slow on
 // (GYSK_FLAG_FLOW_TOPK_SLOW, resp_slow_score)
 static constexpr int TOPK_SCORE_SLOW = 0x100;
+
+// GYSK_FLAG_FLOW_ERRORS: the count-min of the QRY_REC records that carry an error bit, cells {cli_errors | ser_errors << 32} with the
+// depth, width and row hashes of cms_cur, and the batch flow table the TCP pass sums them in (keyed as the query table's) before the TASK
+// pass applies it. ingest_kernel's ERR instances put the event's GYSK_EVF_CLI_ERROR / GYSK_EVF_SER_ERROR bits into bits 30 / 31 of the
+// record's value (a counted usec is below 1 000 001 000 < 2^30), and the drain passes' ERR instances mask them off. list: with
+// GYSK_FLAG_FLOW_TOPK the server-error set's candidates, fed by the TCP pass once per record with the server-error bit (ekeys nullptr).
+// Laid out and kept out of DevState and FlowTopk as FlowQueries, so that the kernels without the flag keep their parameter layout; every
+// pointer nullptr: off. ring and level: with GYSK_FLAG_FLOW_QUERY_LEVEL too, the rolling 300-s level.
+struct FlowErrors { unsigned long long *cur, *last; FlowEnt *flow; unsigned long long *ring, *level; TopkList list; };
+static constexpr uint32_t QRY_CLI_ERR = 1u << 30, QRY_SER_ERR = 1u << 31, QRY_USEC_MASK = QRY_CLI_ERR - 1u;
 
 // GYSK_FLAG_CLIENT_LEVELS: per service slot register sets of CL_REGS one-byte registers (precision GYSK_HLL_WINDOW_P): the open window
 // and the last closed one ([max_svcs + 1][CL_REGS] each), the ring of NSLOTS 30-s slots ([NSLOTS][stride][CL_REGS], the level ring's
@@ -274,15 +285,18 @@ int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_
 // fq.cur != nullptr: the response samples are queued for the flow query table too (GYSK_FLAG_FLOW_QUERIES)
 // tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the flow keys of the ACTIVE records join the connection table's candidates
 // cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): the ACTIVE records raise the open window's client registers too
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, const gysk_event *d_ev,
-		uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s);
+// err (GYSK_FLAG_FLOW_ERRORS, only with fq.cur): the queued response samples carry their error bits (QRY_CLI_ERR, QRY_SER_ERR)
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, bool err,
+		const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
 // fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms;
 // tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the passes gather each held table's candidates; tk.list[2].keys != nullptr
 // (GYSK_FLAG_FLOW_TOPK_SLOW, with fr.cur): the TCP pass gathers the flow key of each response sample in bucket b_slow or above;
-// cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): each connection record raises the open window's client register beside the all-time one
+// cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): each connection record raises the open window's client register beside the all-time one;
+// fe.cur != nullptr (GYSK_FLAG_FLOW_ERRORS, only with fq.cur): the error samples go to the flow error tables, and with fe.list.keys their
+// server-error flow keys to its candidates
 int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
-		const ClientLevels &cl, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
+		const ClientLevels &cl, const FlowErrors &fe, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // GYSK_FLAG_FLOW_TOPK, after the batch merge (it takes tmp's sort buffers, of at least n_max keys): the *l.n candidates (n_max >= *l.n)
 // sorted by key in l.keys, the distinct ones scored on table tbl (score as TOPK_SCORE_SLOW says) and the K best by (score descending,
 // key ascending) written to set; then, unless reseed is false, set back into l as the next batch's first candidates. -1: no sort plan

@@ -865,6 +865,7 @@ int lay_out_arena(gysk_engine *e)
 	// still three regions, three collectives. GYSK_FLAG_FLOW_QUERIES puts the two flow query tables after the count-min ones, and
 	// GYSK_FLAG_FLOW_QUERY_LEVEL their level after them, with the flush tsec pair. GYSK_FLAG_FLOW_RESP_HIST puts the flow response
 	// histograms (and with GYSK_FLAG_FLOW_QUERY_LEVEL their level) after all of them: 8 words a cell, summed like every other word.
+	// GYSK_FLAG_FLOW_ERRORS puts the flow error tables (and with GYSK_FLAG_FLOW_QUERY_LEVEL their level) after those.
 	// GYSK_FLAG_MERGE_TRACES puts its words at the end of the SUM region, its maxima at the end of the i64 MAX one, and needs the flush
 	// tsec pair too. Only the flags and the maps size the arena (never max_trace_svcs).
 	const bool levels = e->cfg.flags & GYSK_FLAG_MERGE_LEVELS, states = e->cfg.flags & GYSK_FLAG_MERGE_STATES, clusters = e->cfg.flags & GYSK_FLAG_MERGE_CLUSTERS;
@@ -946,20 +947,22 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	const bool topn = e->cfg.flags & GYSK_FLAG_MERGE_TOPN, traces = e->cfg.flags & GYSK_FLAG_MERGE_TRACES;
 	// GYSK_FLAG_FLOW_TOPK: the rank's last-window heaviest-flow sets after everything else; GYSK_FLAG_FLOW_TOPK_5MIN: its level sets
 	// and their bounds after those; GYSK_FLAG_FLOW_TOPK_SLOW: its last-window slow set, and with the slow level set L (and B_L) after
-	// those. The merged slow sets are set [2] of topk_final / topk5_final.
+	// those; GYSK_FLAG_FLOW_ERRORS: its last-window server-error set, and with its level L (and B_L), after the slow sets. The merged slow
+	// sets are set [2] of topk_final / topk5_final, the merged server-error sets set [3].
 	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK, topk5 = e->cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN;
-	const uint32_t nslow = e->topk.open[2] ? (e->topk5.level[2] ? 2 : 1) : 0;
+	const uint32_t nslow = e->topk.open[2] ? (e->topk5.level[2] ? 2 : 1) : 0, nerr = e->topk.open[3] ? (e->topk5.level[3] ? 2 : 1) : 0;
 	mg.trace_off = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
 	mg.topk_off = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
 	mg.topk5_off = mg.topk_off + (topk ? TOPK_SLAB_ENTRIES : 0);
 	mg.topks_off = mg.topk5_off + (topk5 ? TOPK_SLAB_ENTRIES : 0);
-	mg.slab_entries = mg.topks_off + (nslow ? topk_slab_entries(nslow) : 0);
+	mg.topke_off = mg.topks_off + (nslow ? topk_slab_entries(nslow) : 0);
+	mg.slab_entries = mg.topke_off + (nerr ? topk_slab_entries(nerr) : 0);
 	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
 	if (topk) {
-		if ((rc = dalloc(e, &mg.topk_final, (nslow ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
+		if ((rc = dalloc(e, &mg.topk_final, (nerr ? 4 : nslow ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
 		if ((rc = dalloc(e, &mg.topk_n, 1))) return rc;
 	}
-	if (topk5 && (rc = dalloc(e, &mg.topk5_final, (nslow == 2 ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
+	if (topk5 && (rc = dalloc(e, &mg.topk5_final, (nerr == 2 ? 4 : nslow == 2 ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
 	if (topn) {
 		if ((rc = dalloc(e, &mg.topn_slots, (size_t)TOPN_LISTS * TOPN_K))) return rc;
 		if ((rc = dalloc(e, &mg.topn_final, TopnLists::BYTES))) return rc;
@@ -1137,6 +1140,12 @@ int gysk_merge_prepare(gysk_engine *e)
 		if (e->topk5.level[2])
 			CU(e, cudaMemcpyAsync(dst + TOPK_SET_WORDS, e->topk5.level[2], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
 	}
+	if (e->topk.open[3]) {		// GYSK_FLAG_FLOW_ERRORS: the last-window server-error set, then with the error level its L and B_L
+		unsigned long long *dst = reinterpret_cast<unsigned long long *>(mg.lg.slab + mg.topke_off);
+		CU(e, cudaMemcpyAsync(dst, e->topk.last[3], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
+		if (e->topk5.level[3])
+			CU(e, cudaMemcpyAsync(dst + TOPK_SET_WORDS, e->topk5.level[3], sizeof(unsigned long long) * TOPK_SET_WORDS, cudaMemcpyDeviceToDevice, e->stream));
+	}
 	// no host sync: the caller enqueues the collectives on gysk_stream(e) (stream order) or calls gysk_sync() first
 	mg.prepared = true; mg.finished = false;
 	return post_launch(e, "merge_prepare");
@@ -1200,9 +1209,10 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 		t.tile_status = mg.topk_tiles; t.max_tiles = (uint32_t)((mg.topk_cap + SORT_TILE - 1) / SORT_TILE);
 		const TopkList l {mg.topk_buf, mg.topk_n, nullptr, mg.topk_cap};
 		const size_t stride = (size_t)mg.slab_entries * sizeof(SlabEntry) / sizeof(unsigned long long);
-		// the rank's window set w in the slab (the slow set in its own region)
+		// the rank's window set w in the slab (the slow and server-error sets each in their own region)
 		auto slab_set = [&](int w, bool level) {
-			const unsigned long long *base = reinterpret_cast<const unsigned long long *>(src + (w < 2 ? (level ? mg.topk5_off : mg.topk_off) : mg.topks_off));
+			const uint32_t off = w < 2 ? (level ? mg.topk5_off : mg.topk_off) : w == 2 ? mg.topks_off : mg.topke_off;
+			const unsigned long long *base = reinterpret_cast<const unsigned long long *>(src + off);
 			return base + (size_t)(w < 2 ? w : level ? 1 : 0) * TOPK_SET_WORDS;
 		};
 		for (int w = 0; w < TOPK_SETS; ++w) {
@@ -1480,6 +1490,17 @@ int gysk_query_flow_resp_global_5min(gysk_engine *e, const uint64_t *keys, uint3
 	return query_cms_resp(e, CMS_RESP_5MIN, true, keys, n, out, "query_flow_resp_global_5min");
 }
 
+// GYSK_FLAG_FLOW_ERRORS: the point query on the flow error tables (and their level) summed over the ranks, with the summed queries
+int gysk_query_flow_errors_global(gysk_engine *e, const uint64_t *keys, uint32_t n, int last_window, gysk_flow_err_est *out)
+{
+	return query_cms_err(e, last_window ? CMS_ERR_LAST : CMS_ERR_CUR, true, keys, n, out, "query_flow_errors_global");
+}
+
+int gysk_query_flow_errors_global_5min(gysk_engine *e, const uint64_t *keys, uint32_t n, gysk_flow_err_est *out)
+{
+	return query_cms_err(e, CMS_ERR_5MIN, true, keys, n, out, "query_flow_errors_global_5min");
+}
+
 #define NC(e, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return nccl_fail((e), #call, r__); } while (0)
 
 int gysk_nccl_unique_id(uint8_t out[GYSK_NCCL_UNIQUE_ID_BYTES])
@@ -1576,6 +1597,17 @@ int gysk_topk_flow_slow_global(gysk_engine *e, uint32_t n, gysk_flow_resp_est *o
 int gysk_topk_flow_slow_global_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound)
 {
 	return topk_read(e, 2, 0, true, true, n, out, nout, bound, "topk_flow_slow_global_5min");
+}
+
+// GYSK_FLAG_FLOW_ERRORS: the flows with the most server errors over every rank, from the last finished merge
+int gysk_topk_flow_errors_global(gysk_engine *e, uint32_t n, gysk_flow_err_est *out, uint32_t *nout)
+{
+	return topk_read(e, 3, 1, false, true, n, out, nout, nullptr, "topk_flow_errors_global");
+}
+
+int gysk_topk_flow_errors_global_5min(gysk_engine *e, uint32_t n, gysk_flow_err_est *out, uint32_t *nout, uint64_t *bound)
+{
+	return topk_read(e, 3, 0, true, true, n, out, nout, bound, "topk_flow_errors_global_5min");
 }
 
 int gysk_topn_global(gysk_engine *e, int metric, uint32_t n, gysk_topn_entry *out, gysk_svc_summary *rows, uint32_t *nout)

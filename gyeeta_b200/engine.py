@@ -16,6 +16,8 @@ FLOW_QRY_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("queries", "<u4"), ("resp_m
 FLOW_RESP_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("counts", "<u4", (15,)), ("total", "<u4"), ("p25_ms", "<i8"), ("p95_ms", "<i8"),
                                 ("p99_ms", "<i8")])                                                   # gysk_flow_resp_est
 RESP_HIST_WORDS = 8     # u64 words of one flow response histogram cell
+FLOW_ERR_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("queries", "<u4"), ("cli_errors", "<u4"), ("ser_errors", "<u4"),
+                               ("pad", "<u4")])                                                       # gysk_flow_err_est
 
 EV_CONNECT, EV_ACCEPT, EV_CLOSE_CLI, EV_CLOSE_SER, EV_RESP, EV_TASK, EV_ACTIVE = 1, 2, 3, 4, 5, 6, 7
 EVF_CLI_ERROR, EVF_SER_ERROR = 1, 2
@@ -45,6 +47,7 @@ FLAG_FLOW_TOPK = 0x400
 FLAG_FLOW_TOPK_5MIN = 0x800
 FLAG_FLOW_TOPK_SLOW = 0x1000
 FLAG_CLIENT_LEVELS = 0x2000
+FLAG_FLOW_ERRORS = 0x4000
 HLL_WINDOW_P = 8
 CLIENTS_LAST, CLIENTS_5MIN = 0, 1
 FLOW_TOPK_CAP = 4096
@@ -354,6 +357,17 @@ def load_library(path=None):
         "gysk_topk_flow_slow_global": (i32, [vp, u32, vp, vp]),
         "gysk_topk_flow_slow_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_topk_flow_slow_global_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_query_flow_errors": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_flow_errors_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_query_flow_errors_global": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_flow_errors_global_5min": (i32, [vp, vp, u32, vp]),
+        "gysk_export_cms_errors": (i32, [vp, i32, vp]),
+        "gysk_export_cms_errors_5min": (i32, [vp, vp]),
+        "gysk_last_batch_flow_err_direct": (C.c_int64, [vp]),
+        "gysk_topk_flow_errors": (i32, [vp, i32, u32, vp, vp]),
+        "gysk_topk_flow_errors_global": (i32, [vp, u32, vp, vp]),
+        "gysk_topk_flow_errors_5min": (i32, [vp, u32, vp, vp, vp]),
+        "gysk_topk_flow_errors_global_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_query_svc_clients": (i32, [vp, vp, u32, vp]),
         "gysk_query_clients_window": (i32, [vp, C.c_int32, u32, vp, vp, u32, vp]),
         "gysk_export_hll_window": (i32, [vp, u64, i32, vp]),
@@ -425,7 +439,7 @@ class Engine:
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
                  max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False,
-                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False, client_levels=False):
+                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False, client_levels=False, flow_errors=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -442,7 +456,7 @@ class Engine:
                     (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
                     (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0) | \
                     (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0) | (FLAG_FLOW_TOPK_SLOW if flow_topk_slow else 0) | \
-                    (FLAG_CLIENT_LEVELS if client_levels else 0)
+                    (FLAG_CLIENT_LEVELS if client_levels else 0) | (FLAG_FLOW_ERRORS if flow_errors else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -636,9 +650,13 @@ class Engine:
         """response samples of the last device batch whose flow response histogram update bypassed its flow table (flow_resp_hist=True)"""
         return self._counter(self.L.gysk_last_batch_flow_resp_direct)
 
+    def last_batch_flow_err_direct(self):
+        """error samples of the last device batch whose flow error update bypassed the error flow table (flow_errors=True)"""
+        return self._counter(self.L.gysk_last_batch_flow_err_direct)
+
     def flow_table_used(self):
         """non-zero entries of the batch flow tables (the query one too with flow_queries=True, the response one with
-        flow_resp_hist=True): 0 whenever no batch is in flight (diagnostic)"""
+        flow_resp_hist=True, the error one with flow_errors=True): 0 whenever no batch is in flight (diagnostic)"""
         n = self.L.gysk_flow_table_used(self.h)
         if n < 0:
             self._chk(int(n))
@@ -1174,6 +1192,50 @@ class Engine:
     def query_flow_resp_global_5min(self, keys):
         """gysk_query_flow_resp_global_5min: the point query on that level summed over the ranks by the last merge"""
         return self._point_query(self.L.gysk_query_flow_resp_global_5min, FLOW_RESP_EST_DTYPE, keys)
+
+    def query_flow_errors(self, keys, last_window=False):
+        """gysk_query_flow_errors: per flow key its queries (as query_flow_queries) and client / server errors, min over rows
+        (flow_errors=True)"""
+        return self._point_query(self.L.gysk_query_flow_errors, FLOW_ERR_EST_DTYPE, keys, int(last_window))
+
+    def export_cms_errors(self, last_window=False):
+        """gysk_export_cms_errors: the cells {cli_errors | ser_errors << 32} of the flow error table (flow_errors=True)"""
+        return self._export_cells(self.L.gysk_export_cms_errors, int(last_window))
+
+    def query_flow_errors_global(self, keys, last_window=False):
+        """gysk_query_flow_errors_global: the point query on the flow error and query tables summed over the ranks by the last merge"""
+        return self._point_query(self.L.gysk_query_flow_errors_global, FLOW_ERR_EST_DTYPE, keys, int(last_window))
+
+    def query_flow_errors_5min(self, keys):
+        """gysk_query_flow_errors_5min: the point query on the rolling 300-s level of the flow error tables
+        (flow_errors=True, flow_query_level=True)"""
+        return self._point_query(self.L.gysk_query_flow_errors_5min, FLOW_ERR_EST_DTYPE, keys)
+
+    def export_cms_errors_5min(self):
+        """gysk_export_cms_errors_5min: the cells of that level"""
+        return self._export_cells(self.L.gysk_export_cms_errors_5min)
+
+    def query_flow_errors_global_5min(self, keys):
+        """gysk_query_flow_errors_global_5min: the point query on that level summed over the ranks by the last merge"""
+        return self._point_query(self.L.gysk_query_flow_errors_global_5min, FLOW_ERR_EST_DTYPE, keys)
+
+    def topk_flow_errors(self, n=FLOW_TOPK_CAP, last_window=False):
+        """gysk_topk_flow_errors: the n flows with the most server errors of the open or last window, each row its
+        query_flow_errors row (flow_errors=True, flow_topk=True)"""
+        return self._topk(self.L.gysk_topk_flow_errors, FLOW_ERR_EST_DTYPE, n, int(last_window))
+
+    def topk_flow_errors_global(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_errors_global: the n flows with the most server errors over every rank, from the last finished merge"""
+        return self._topk(self.L.gysk_topk_flow_errors_global, FLOW_ERR_EST_DTYPE, n)
+
+    def topk_flow_errors_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_errors_5min: (rows, bound) of the rolling 300-s error level by server errors (flow_errors=True,
+        flow_topk_5min=True, flow_query_level=True)"""
+        return self._topk_5min(self.L.gysk_topk_flow_errors_5min, FLOW_ERR_EST_DTYPE, n)
+
+    def topk_flow_errors_global_5min(self, n=FLOW_TOPK_CAP):
+        """gysk_topk_flow_errors_global_5min: (rows, bound) over every rank's error level, from the last finished merge"""
+        return self._topk_5min(self.L.gysk_topk_flow_errors_global_5min, FLOW_ERR_EST_DTYPE, n)
 
     def export_cms_queries_5min(self):
         """gysk_export_cms_queries_5min: the cells of the rolling 300-s flow query level (flow_query_level=True)"""

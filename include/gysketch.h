@@ -272,6 +272,18 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   and merged across ranks (gysk_query_svc_clients, "distinct clients per window" below).
 						   Needs no other flag. Without it nothing is allocated, every other call answers as
 						   before and the five calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_FLOW_ERRORS		0x4000u	/* a count-min of each client flow's client and server errors beside the flow query
+						   tables, in the open and last window and with GYSK_FLAG_FLOW_QUERY_LEVEL the rolling
+						   300 s (gysk_query_flow_errors, "flow errors" below); with GYSK_FLAG_FLOW_TOPK also the
+						   flows with the most server errors; the merge step sums the tables and ranks the sets
+						   across ranks. Needs GYSK_FLAG_FLOW_QUERIES: gysk_create refuses it without; combines
+						   freely with every other flag. Costs 2 more tables of depth << log2_width cells (13 with
+						   the level), a fourth batch flow table and, with GYSK_FLAG_FLOW_TOPK, a candidate list
+						   of K + max_batch keys (device_bytes +1.24 GB at the bench's sizes). Measured on one H100
+						   80GB HBM3 at 700 W with the bench workload (100 M-event batches) at 1 % error samples:
+						   the TCP drain pass 6.57 -> 6.75 ms and the TASK pass 1.40 -> 1.58 ms per batch; at 100 %
+						   the TCP pass 17.2 ms. Without it nothing is allocated, every other call answers as
+						   before and the flow error calls are GYSK_ERR_NOTSUP */
 #define GYSK_HLL_WINDOW_P		8u	/* precision of the windowed client registers: 256 one-byte registers per set (fixed:
 						   gysk_config has no word for it) */
 
@@ -421,6 +433,16 @@ typedef struct gysk_flow_resp_est
 						   0, ...) on the same counts; -1 when the cut-off falls in bucket 0 (an empty histogram) */
 } gysk_flow_resp_est;
 
+/* a point query on the flow error tables (GYSK_FLAG_FLOW_ERRORS), 24 bytes */
+typedef struct gysk_flow_err_est
+{
+	uint64_t	flow_key;
+	uint32_t	queries;		/* the flow query tables' count for the same window (gysk_query_flow_queries) */
+	uint32_t	cli_errors;		/* min over rows of the client-error halves */
+	uint32_t	ser_errors;		/* min over rows of the server-error halves */
+	uint32_t	pad;
+} gysk_flow_err_est;
+
 typedef struct gysk_stats
 {
 	uint64_t	events_in;		/* events handed to the device */
@@ -474,6 +496,9 @@ int64_t		gysk_last_batch_flow_query_direct(gysk_engine *e);
 /* diagnostic (GYSK_FLAG_FLOW_RESP_HIST): response samples of the last device batch whose flow response histogram update did not go
  * through the batch's response flow table (its probe limit reached). Routing only. GYSK_ERR_NOTSUP without the flag. */
 int64_t		gysk_last_batch_flow_resp_direct(gysk_engine *e);
+/* diagnostic (GYSK_FLAG_FLOW_ERRORS): error samples of the last device batch whose flow error update did not go through the batch's
+ * error flow table (its probe limit reached). Routing only. GYSK_ERR_NOTSUP without the flag. */
+int64_t		gysk_last_batch_flow_err_direct(gysk_engine *e);
 
 /* ---- capacity: growing the service / process tables of a live engine ---- */
 /* Raise the service / process capacity of a live engine (either may equal the current value; neither may shrink, both <= 1 << 24).
@@ -847,6 +872,52 @@ int		gysk_topk_flow_slow(gysk_engine *e, int last_window, uint32_t n, gysk_flow_
 int		gysk_topk_flow_slow_global(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout);
 int		gysk_topk_flow_slow_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound);
 int		gysk_topk_flow_slow_global_5min(gysk_engine *e, uint32_t n, gysk_flow_resp_est *out, uint32_t *nout, uint64_t *bound);
+
+/* ---- flow errors (GYSK_FLAG_FLOW_ERRORS): which clients get the errors ----
+ * gysk_svc_summary.cli_errors / ser_errors count a service's errors, and ser_errors can turn a listener BAD, but no other answer names
+ * the clients that got them: the heaviest-flow sets rank by volume, the query tables count every request whatever its outcome, and a
+ * failing request is often fast. These tables count each client flow's errors.
+ * Counting rule: a response sample counts iff it counts in the flow query tables (gysk_query_flow_queries) and its event carries
+ * GYSK_EVF_CLI_ERROR and/or GYSK_EVF_SER_ERROR. It adds 1 to each half whose bit is set, exactly as the service's error counts take it.
+ * The key is the flow query tables' key, and the tables have their depth, width and row hashes, so a key lands in the same columns of
+ * every flow table family. Each cell is one u64 {cli_errors : low 32 | ser_errors : high 32}, summed mod 2^64. Hot-row and key routes
+ * count alike; GYSK_EV_TRACE events, samples beyond the validity rule, unknown ids and dropped events never count. Two limits follow
+ * from the routes: a GYSK_RAW_API_TRAN sample counts under the client port alone (as in the query tables), and the raw eBPF response
+ * events (GYSK_RAW_TCP_IPV4_RESP / _IPV6_RESP) carry no error bits, so they never count.
+ * Invariants: for every row the error halves of the open table sum to the open-window cli_errors / ser_errors of every service
+ * (mod 2^32); cell by cell each error half is at most the query half of the same flow query cell.
+ * Windows: the open table and the last closed one, by the count-min's flush rule; with GYSK_FLAG_FLOW_QUERY_LEVEL also the rolling 300-s
+ * level by the rule of gysk_query_flow_queries_5min.
+ * gysk_query_flow_errors: per key queries as gysk_query_flow_queries answers it for the same window, and each error half's minimum over
+ *   rows (a count-min estimate: never below the exact count). gysk_export_cms_errors: the open (last_window = 0) or last closed table,
+ *   depth << log2_width cells. The _global pair: the same on the tables summed over the ranks by the last merge (GYSK_ERR_INVAL before
+ *   gysk_merge_prepare). The _5min calls: the same on the level (GYSK_ERR_NOTSUP without GYSK_FLAG_FLOW_QUERY_LEVEL).
+ * Flows with the most server errors (with GYSK_FLAG_FLOW_TOPK; GYSK_ERR_NOTSUP without): one open and one last set of K =
+ *   GYSK_FLOW_TOPK_CAP keys on the error tables, scored by the ser_errors half, by the rule and guarantee of the heaviest-flow sets; the
+ *   candidates are the distinct flow keys with a server-error sample in the batch. A flow with no server error (a client-error-only
+ *   flow) is never listed. With GYSK_FLAG_FLOW_TOPK_5MIN and GYSK_FLAG_FLOW_QUERY_LEVEL the 300-s sets, L and B_L by the rule of the
+ *   heaviest flows of the 300-s levels, on the error ring and level. gysk_merge_prepare carries the last-window set, and with the level
+ *   L and B_L, after the slow sets in the t-digest slab; gysk_merge_finish keeps the K best of the union on the summed error tables, with
+ *   B_G = max(thr(G), sum over ranks of B_L).
+ * gysk_topk_flow_errors(_5min / _global / _global_5min): the first min(n, K) flows of the set, best first, each row byte-equal to what the
+ *   matching point query answers for its key; entries with zero ser_errors are left out, so *nout may be below n; *bound (may be NULL)
+ *   = B_L or B_G.
+ * Cost: each counted sample with an error bit adds a third batch flow-table update in the TCP drain pass, each server-error sample a
+ * candidate key, and the TASK pass sweeps one more table. Measured on one H100 80GB HBM3 at 700 W, bench workload (100 M-event batches,
+ * against GYSK_FLAG_FLOW_QUERIES and GYSK_FLAG_FLOW_TOPK alone): with no error samples the TASK pass +0.08 ms; at 1 % error samples the
+ * TCP pass 6.57 -> 6.75 ms, the TASK pass 1.40 -> 1.58 ms and the selection +0.3 ms per batch; at 100 % the TCP pass 6.6 -> 17.2 ms and the
+ * selection +4.9 ms; gysk_flush +0.02 ms, gysk_merge_prepare +0.06 ms, gysk_merge_finish up to +0.14 ms, device_bytes +1.24 GB (the
+ * candidate list at max_batch = 2^27). DESIGN.md section 7 has the measurements. */
+int		gysk_query_flow_errors(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_err_est *out);
+int		gysk_query_flow_errors_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_err_est *out);
+int		gysk_query_flow_errors_global(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, int last_window, gysk_flow_err_est *out);
+int		gysk_query_flow_errors_global_5min(gysk_engine *e, const uint64_t *flow_keys, uint32_t n, gysk_flow_err_est *out);
+int		gysk_export_cms_errors(gysk_engine *e, int last_window, uint64_t *cells /* depth << log2_width entries */);
+int		gysk_export_cms_errors_5min(gysk_engine *e, uint64_t *cells /* depth << log2_width entries */);
+int		gysk_topk_flow_errors(gysk_engine *e, int last_window, uint32_t n, gysk_flow_err_est *out, uint32_t *nout);
+int		gysk_topk_flow_errors_global(gysk_engine *e, uint32_t n, gysk_flow_err_est *out, uint32_t *nout);
+int		gysk_topk_flow_errors_5min(gysk_engine *e, uint32_t n, gysk_flow_err_est *out, uint32_t *nout, uint64_t *bound);
+int		gysk_topk_flow_errors_global_5min(gysk_engine *e, uint32_t n, gysk_flow_err_est *out, uint32_t *nout, uint64_t *bound);
 
 /* ---- distinct clients per window (GYSK_FLAG_CLIENT_LEVELS): how many clients a service has now ----
  * gysk_svc_summary.distinct_clients is an all-time estimate: its registers are never cleared, so it cannot show a new caller fleet, a
