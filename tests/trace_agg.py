@@ -97,10 +97,15 @@ class TraceOracle:
         self.orc = po.OracleEngine(max_svcs=max_windows, max_tasks=16, cms_log2_width=4, hll_p=4, td_compression=100)
         self.shadow = {}             # (glob_id, window number) -> oracle service id
         self.win_of = {}             # glob_id -> (number of its open window, of its last window)
+        self.nshadow = 0
         self.L = ge.load_library()
 
     def _shadow(self, id_, w):
-        return self.shadow.setdefault((id_, w), len(self.shadow) + 1)
+        # a new number for every pair: evict drops pairs, so the count of pairs held can repeat a number still in use
+        if (id_, w) not in self.shadow:
+            self.nshadow += 1
+            self.shadow[(id_, w)] = self.nshadow
+        return self.shadow[(id_, w)]
 
     def ingest(self, ev):
         """one device batch: its GYSK_EV_TRACE events, in order"""
