@@ -89,6 +89,12 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		if (k < 0) return fail(e, GYSK_ERR_INVAL, "heaviest-flow selection: no sort plan");
 		e->kernel_launches += k;
 	}
+	// GYSK_FLAG_SVC_TOP_CLIENTS: the batch's per-client sums into each service's open summary, last, in the same sort buffers
+	if (e->tc.open) {
+		const int k = launch_topc_batch(e->tmp, e->tc, rr, n, e->cfg.max_svcs, e->stream);
+		if (k < 0) return fail(e, GYSK_ERR_INVAL, "top-client summaries: no sort plan");
+		e->kernel_launches += k;
+	}
 	e->batches++;
 	return post_launch(e, "ingest batch");
 }
@@ -475,21 +481,26 @@ int stage_svc_raw(gysk_engine *e, uint64_t id)
 }
 
 // the two summary rows, by id (d_ids) or by slot (d_slots), into the stage
-int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_summary *)
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_summary *, int = 0)
 {
 	return launch_svc_summaries(e->st, d_ids, d_slots, m, reinterpret_cast<gysk_svc_summary *>(e->d_wstage), e->stream);
 }
-int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_task_summary *)
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_task_summary *, int = 0)
 {
 	return launch_task_summaries(e->st, d_ids, d_slots, m, reinterpret_cast<gysk_task_summary *>(e->d_wstage), e->stream);
 }
-int launch_rows(gysk_engine *e, const unsigned long long *, const unsigned long long *d_slots, uint32_t m, gysk_listener_day_stats *)
+int launch_rows(gysk_engine *e, const unsigned long long *, const unsigned long long *d_slots, uint32_t m, gysk_listener_day_stats *, int = 0)
 {
 	return launch_day_stats(e->st, d_slots, m, reinterpret_cast<gysk_listener_day_stats *>(e->d_wstage), e->stream);
 }
-int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_clients *)
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_clients *, int = 0)
 {
 	return launch_client_rows(e->st, e->cl, d_ids, d_slots, m, reinterpret_cast<gysk_svc_clients *>(e->d_wstage), e->stream);
+}
+// the rows of top-client summary `which` (GYSK_FLAG_SVC_TOP_CLIENTS)
+int launch_rows(gysk_engine *e, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t m, gysk_svc_top_clients *, int which)
+{
+	return launch_topc_rows(e->st, e->tc, which, d_ids, d_slots, m, reinterpret_cast<gysk_svc_top_clients *>(e->d_wstage), e->stream);
 }
 // The rolling levels at the flush of tsec: the closing window goes to ring slot (tsec / width) % NSLOTS of each level, and a slot
 // still holding an older epoch is cleared first (LevelRing::fresh records it). Then the live slots, whose epochs lie in the level's
@@ -557,12 +568,14 @@ static int topk5_roll(gysk_engine *e, int w)
 // hold max_svcs + 1 slots (slot max_svcs is the null slot), the level ring max_svcs rows in each of its NLEVELS x NSLOTS planes
 // (LevelRing::stride), Task arrays max_tasks slots. gysk_create allocates exactly these, gysk_grow moves them, slot_bytes sums them.
 // The process eviction's arrays exist only with task_idle_evict_secs (task_evict), the client register sets only with
-// GYSK_FLAG_CLIENT_LEVELS (clients; their ring in NSLOTS planes of ClientLevels::stride rows). The batch's segment arrays (Seg) are
+// GYSK_FLAG_CLIENT_LEVELS (clients; their ring in NSLOTS planes of ClientLevels::stride rows), the top-client summaries only with
+// GYSK_FLAG_SVC_TOP_CLIENTS (topc; their ring in NSLOTS planes of SvcTopClients::stride rows). The batch's segment arrays (Seg) are
 // indexed by the slot field of the sort keys: max_svcs + 1 entries, and one more per trace row (max_trace_svcs) beyond the null slot.
 enum class SlotKind { Svc, Ring, Task, Seg };
 
 template <typename F>
-void each_slot_array(DevState &st, SortTemp &tmp, ClientLevels &cl, uint32_t hll_p, bool task_evict, bool clients, F f)
+void each_slot_array(DevState &st, SortTemp &tmp, ClientLevels &cl, SvcTopClients &tc, uint32_t hll_p, bool task_evict, bool clients, bool topc,
+		F f)
 {
 	f(st.slot_id, 1, SlotKind::Svc); f(st.slot_host, 1, SlotKind::Svc);
 	f(st.slot_first_seen, 1, SlotKind::Svc); f(st.slot_last_active, 1, SlotKind::Svc);
@@ -586,16 +599,21 @@ void each_slot_array(DevState &st, SortTemp &tmp, ClientLevels &cl, uint32_t hll
 		f(cl.open, CL_REGS, SlotKind::Svc); f(cl.last, CL_REGS, SlotKind::Svc);
 		f(cl.ring, (size_t)NSLOTS * CL_REGS, SlotKind::Ring); f(cl.level, CL_REGS, SlotKind::Svc);
 	}
+	if (topc) {
+		f(tc.open, 1, SlotKind::Svc); f(tc.last, 1, SlotKind::Svc);
+		f(tc.ring, NSLOTS, SlotKind::Ring); f(tc.level, 1, SlotKind::Svc);
+	}
 }
 
 // device bytes of one service slot (its ring rows included) and of one process slot: the sums of each_slot_array
-void slot_bytes(uint32_t hll_p, bool task_evict, bool clients, uint64_t *svc, uint64_t *task)
+void slot_bytes(uint32_t hll_p, bool task_evict, bool clients, bool topc, uint64_t *svc, uint64_t *task)
 {
 	DevState st {};
 	SortTemp tmp {};
 	ClientLevels cl {};
+	SvcTopClients tc {};
 	uint64_t b[4] = {0, 0, 0, 0};
-	each_slot_array(st, tmp, cl, hll_p, task_evict, clients, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
+	each_slot_array(st, tmp, cl, tc, hll_p, task_evict, clients, topc, [&](auto *&p, size_t k, SlotKind kind) { b[(int)kind] += k * sizeof(*p); });
 	*svc = b[(int)SlotKind::Svc] + b[(int)SlotKind::Ring] + b[(int)SlotKind::Seg];
 	*task = b[(int)SlotKind::Task];
 }
@@ -626,6 +644,7 @@ SvcRows finish_rows(const gysk_engine *e, gysk_svc_summary *out) { return SvcRow
 CopyRows<gysk_task_summary> finish_rows(const gysk_engine *, gysk_task_summary *out) { return CopyRows<gysk_task_summary> {out}; }
 CopyRows<gysk_listener_day_stats> finish_rows(const gysk_engine *, gysk_listener_day_stats *out) { return CopyRows<gysk_listener_day_stats> {out}; }
 ClientRows finish_rows(const gysk_engine *, gysk_svc_clients *out) { return ClientRows {out}; }
+CopyRows<gysk_svc_top_clients> finish_rows(const gysk_engine *, gysk_svc_top_clients *out) { return CopyRows<gysk_svc_top_clients> {out}; }
 
 } // namespace
 
@@ -776,12 +795,14 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 	A(dalloc(e, &st.task_tbl.count, 1));
 	if (cfg.task_idle_evict_secs) A(dalloc(e, &st.task_tbl.free_n, 1));		// without it the process table has no free stack
 	SortTemp &tmp = e->tmp;
-	each_slot_array(st, tmp, e->cl, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, e->cl, e->tc, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS,
+			cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS, [&](auto *&p, size_t k, SlotKind kind) {
 		if (!rc) rc = dalloc(e, &p, slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs) * k);
 	});
 	if (rc) return bail(rc);
 	st.levels.stride = cfg.max_svcs;
 	if (e->cl.open) e->cl.stride = cfg.max_svcs;
+	if (e->tc.open) e->tc.stride = cfg.max_svcs;
 	st.svc_tbl.slot_id = st.slot_id; st.svc_tbl.slot_host = st.slot_host;
 	st.task_tbl.slot_id = st.task_slot_id; st.task_tbl.slot_host = st.task_slot_host;
 	A(halloc(e, &e->h_evict, ns + 2));
@@ -862,6 +883,16 @@ int gysk_create(const gysk_config *ucfg, gysk_engine **out)
 			A(dalloc(e, &l.keys, (size_t)l.cap, false)); A(dalloc(e, &l.n, 1));
 			if (w < 2) A(dalloc(e, &l.ekeys, (size_t)tmp.flow_cap, false));
 			A(dalloc(e, &e->topk.open[w], (size_t)TOPK_SET_WORDS)); A(dalloc(e, &e->topk.last[w], (size_t)TOPK_SET_WORDS));
+		}
+		// GYSK_FLAG_SVC_TOP_CLIENTS: the batch pair table (zero here, and the merge kernel leaves it so after every batch), at least twice
+		// the records a batch can bring, and the piece lists: a segment of len > TOPC_PIECE pairs takes fewer than 2 x len / TOPC_PIECE
+		if (cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS) {
+			SvcTopClients &tc = e->tc;
+			const uint32_t pcap = pow2_at_least(2ull * cfg.max_batch);
+			tc.pmask = pcap - 1;
+			A(dalloc(e, &tc.pkey, (size_t)pcap)); A(dalloc(e, &tc.pacc, (size_t)pcap)); A(dalloc(e, &tc.cnt, 3));
+			tc.pieces_cap = 2 * cfg.max_batch / TOPC_PIECE + 1;
+			A(dalloc(e, &tc.pieces, (size_t)tc.pieces_cap, false));
 		}
 		// GYSK_FLAG_FLOW_TOPK_5MIN: per held level its slot sets and level set, all empty with zero bounds; the flush chain's list
 		if (cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN) {
@@ -1565,6 +1596,7 @@ void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, siz
 	DevState st {};
 	SortTemp tmp {};
 	ClientLevels cl {};
+	SvcTopClients tc {};
 	size_t a = 0, big = 0, n = 0;
 	auto move = [&](size_t elem, size_t old_n, size_t new_n) {
 		if (new_n <= old_n) return;
@@ -1572,7 +1604,8 @@ void grow_bytes(const gysk_engine *e, uint32_t ms, uint32_t mt, size_t *add, siz
 		big = std::max(big, old_n * elem);
 		n++;
 	};
-	each_slot_array(st, tmp, cl, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, cl, tc, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS,
+			[&](auto *&p, size_t k, SlotKind kind) {
 		move(k * sizeof(*p), slots_of(kind, cfg.max_svcs, cfg.max_tasks, cfg.max_trace_svcs), slots_of(kind, ms, mt, cfg.max_trace_svcs));
 	});
 	if (cfg.max_trace_svcs) move(sizeof(uint32_t), (size_t)cfg.max_svcs + 1, (size_t)ms + 1);		// TraceTable::row_of
@@ -1611,11 +1644,13 @@ int grow_locked(gysk_engine *e, uint32_t ms, uint32_t mt)
 	to.max_svcs = ms; to.max_tasks = mt;
 	int rc = 0;
 	// phase 1
-	each_slot_array(st, tmp, e->cl, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS, [&](auto *&p, size_t k, SlotKind kind) {
+	each_slot_array(st, tmp, e->cl, e->tc, cfg.hll_p, cfg.task_idle_evict_secs, cfg.flags & GYSK_FLAG_CLIENT_LEVELS,
+			cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS, [&](auto *&p, size_t k, SlotKind kind) {
 		if (rc) return;
 		if (kind == SlotKind::Ring) {
-			if constexpr (std::is_same<std::remove_reference_t<decltype(*p)>, HistCell>::value)
-				rc = regrow_ring(e, p, st.levels.stride, (size_t)NLEVELS * NSLOTS, HIST_CELLS, ms);
+			using T = std::remove_reference_t<decltype(*p)>;
+			if constexpr (std::is_same<T, HistCell>::value) rc = regrow_ring(e, p, st.levels.stride, (size_t)NLEVELS * NSLOTS, HIST_CELLS, ms);
+			else if constexpr (std::is_same<T, TopcSet>::value) rc = regrow_ring(e, p, e->tc.stride, NSLOTS, 1, ms);
 			else rc = regrow_ring(e, p, e->cl.stride, NSLOTS, CL_REGS, ms);
 		}
 		else rc = regrow(e, p, slots_of(kind, os, ot, cfg.max_trace_svcs) * k, slots_of(kind, ms, mt, cfg.max_trace_svcs) * k);
@@ -1750,7 +1785,8 @@ int gysk_slot_bytes(const gysk_config *cfg, uint64_t *svc_slot_bytes, uint64_t *
 		c = *cfg;
 	}
 	if (c.hll_p < 4 || c.hll_p > 16) return GYSK_ERR_INVAL;
-	slot_bytes(c.hll_p, c.task_idle_evict_secs != 0, (c.flags & GYSK_FLAG_CLIENT_LEVELS) != 0, svc_slot_bytes, task_slot_bytes);
+	slot_bytes(c.hll_p, c.task_idle_evict_secs != 0, (c.flags & GYSK_FLAG_CLIENT_LEVELS) != 0, (c.flags & GYSK_FLAG_SVC_TOP_CLIENTS) != 0, svc_slot_bytes,
+			task_slot_bytes);
 	return GYSK_OK;
 }
 
@@ -1775,7 +1811,7 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->kernel_launches += launch_rebuild_table(e->st.task_tbl, e->cfg.max_tasks, e->stream);
 		e->task_tombstones = 0;
 	}
-	e->kernel_launches += launch_flush(e->st, e->cl, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
+	e->kernel_launches += launch_flush(e->st, e->cl, e->tc, e->cfg.max_svcs, tsec, e->cfg.idle_evict_secs, e->stream);
 	e->kernel_launches += launch_task_flush(e->st, e->cfg.max_tasks, tsec, e->cfg.task_idle_evict_secs, e->d_tevict, e->stream);
 	if (e->st.trace.rows) {
 		// trace rows: the open window closes, the other half (the window before it) is cleared and opens
@@ -1813,6 +1849,13 @@ int gysk_flush(gysk_engine *e, uint32_t tsec)
 		e->kernel_launches += launch_client_roll(e->cl, e->cfg.max_svcs, e->st.levels, e->stream);
 		std::swap(e->cl.open, e->cl.last);
 		CU(e, cudaMemsetAsync(e->cl.open, 0, ((size_t)e->cfg.max_svcs + 1) * CL_REGS, e->stream));
+	}
+	if (e->tc.open) {
+		// GYSK_FLAG_SVC_TOP_CLIENTS (the evicted slots' summaries were cleared by launch_flush): the closing window into the ring and the
+		// level over the capacity, then the window swap
+		e->kernel_launches += launch_topc_roll(e->tc, e->cfg.max_svcs, e->st.levels, e->stream);
+		std::swap(e->tc.open, e->tc.last);
+		CU(e, cudaMemsetAsync(e->tc.open, 0, ((size_t)e->cfg.max_svcs + 1) * sizeof(TopcSet), e->stream));
 	}
 	for (int w = 0; w < TOPK_SETS; ++w) {		// GYSK_FLAG_FLOW_TOPK_5MIN: each level set follows its ring, before the window sets swap
 		if (!e->topk5.level[w]) continue;
@@ -1923,21 +1966,22 @@ int window_list(gysk_engine *e, int is_task, int32_t host_idx, uint32_t flags, u
 	return 0;
 }
 
-// gysk_query_svcs / gysk_query_tasks: the rows of n ids, in QCHUNK pieces
+// gysk_query_svcs / gysk_query_tasks: the rows of n ids, in QCHUNK pieces (which: the summary of the top-client rows)
 template <typename Row>
-int query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out, const char *what)
+int query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out, const char *what, int which = 0)
 {
 	CHECK_ENGINE(e);
 	if ((!ids || !out) && n) return GYSK_ERR_INVAL;
 	GYSK_ENTER(e, Submit);
 	return staged_read(e, ids, n, QCHUNK, sizeof(Row), what,
-			[&](const unsigned long long *d_ids, uint32_t, uint32_t m) { return launch_rows(e, d_ids, nullptr, m, out); }, finish_rows(e, out));
+			[&](const unsigned long long *d_ids, uint32_t, uint32_t m) { return launch_rows(e, d_ids, nullptr, m, out, which); }, finish_rows(e, out));
 }
 
 // gysk_query_window_hosts / gysk_query_task_window: the slots of window_list, summarised in WIN_ROWS pieces; hosts (optional) from
 // the same snapshot
 template <typename Row>
-int window_rows(gysk_engine *e, int32_t host_idx, uint32_t flags, Row *out, uint32_t *hosts, uint32_t cap, uint32_t *n, const char *what)
+int window_rows(gysk_engine *e, int32_t host_idx, uint32_t flags, Row *out, uint32_t *hosts, uint32_t cap, uint32_t *n, const char *what,
+		int which = 0)
 {
 	CHECK_ENGINE(e);
 	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
@@ -1948,8 +1992,9 @@ int window_rows(gysk_engine *e, int32_t host_idx, uint32_t flags, Row *out, uint
 	int rc = window_list(e, std::is_same<Row, gysk_task_summary>::value, host_idx, flags, seen_before, cap, &total);
 	if (rc) return rc;
 	const uint32_t m = std::min(cap, total);
-	rc = staged_read<uint64_t>(e, nullptr, m, WIN_ROWS, sizeof(Row), what,
-			[&](const unsigned long long *, uint32_t off, uint32_t k) { return launch_rows(e, nullptr, e->tmp.keys_a + off, k, out); }, finish_rows(e, out));
+	rc = staged_read<uint64_t>(e, nullptr, m, (uint32_t)std::min<size_t>(WIN_ROWS, STAGE_BYTES / sizeof(Row)), sizeof(Row), what,
+			[&](const unsigned long long *, uint32_t off, uint32_t k) { return launch_rows(e, nullptr, e->tmp.keys_a + off, k, out, which); },
+			finish_rows(e, out));
 	if (rc) return rc;
 	// the within-host reorder of window_list leaves every position in its host's run
 	if (hosts) for (uint32_t i = 0; i < m; ++i) hosts[i] = (uint32_t)(e->win_keys[i] >> 32);
@@ -2118,6 +2163,24 @@ int gysk_query_clients_window(gysk_engine *e, int32_t host_idx, uint32_t flags, 
 	CHECK_ENGINE(e);
 	if (!(e->cfg.flags & GYSK_FLAG_CLIENT_LEVELS)) return GYSK_ERR_NOTSUP;
 	return window_rows(e, host_idx, flags, out, hosts, cap, n, "clients_window");
+}
+
+// GYSK_FLAG_SVC_TOP_CLIENTS: the rows of summary `which` of n ids, and of the services of a window read
+int gysk_query_svc_top_clients(gysk_engine *e, const uint64_t *ids, uint32_t n, int which, gysk_svc_top_clients *out)
+{
+	CHECK_ENGINE(e);
+	if (!(e->cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS)) return GYSK_ERR_NOTSUP;
+	if (which < GYSK_TOPC_OPEN || which > GYSK_TOPC_5MIN) return GYSK_ERR_INVAL;
+	return query_rows(e, ids, n, out, "top_client_rows", which);
+}
+
+int gysk_query_top_clients_window(gysk_engine *e, int32_t host_idx, uint32_t flags, int which, gysk_svc_top_clients *out, uint32_t *hosts, uint32_t cap,
+		uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!(e->cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS)) return GYSK_ERR_NOTSUP;
+	if (which < GYSK_TOPC_OPEN || which > GYSK_TOPC_5MIN) return GYSK_ERR_INVAL;
+	return window_rows(e, host_idx, flags, out, hosts, cap, n, "top_clients_window", which);
 }
 
 // the last-window or 300-s client registers of one id, with the contract of gysk_export_hll

@@ -355,6 +355,7 @@ struct gysk_engine
 	gysk::Topk5min		topk5 {};			// GYSK_FLAG_FLOW_TOPK_5MIN (every pointer nullptr without)
 	gysk::ClientLevels	cl {};				// GYSK_FLAG_CLIENT_LEVELS (every pointer nullptr without)
 	gysk::FlowErrors	fe {};				// GYSK_FLAG_FLOW_ERRORS (every pointer nullptr without)
+	gysk::SvcTopClients	tc {};				// GYSK_FLAG_SVC_TOP_CLIENTS (every pointer nullptr without)
 	std::atomic<bool>	fed {false};			// an event was handed in or gysk_flush ran (gysk_set_flow_slow refuses after)
 	std::vector<std::pair<void *, size_t>> dallocs;		// every device buffer and its bytes
 	size_t			dbytes {0};			// their sum (gysk_capacity_info's device_bytes)
@@ -609,6 +610,7 @@ static_assert(sizeof(SlabEntry) <= STAGE_BYTES, "the stage holds one merged dige
 static_assert(sizeof(gysk_logical_state) == 80 && sizeof(gysk_logical_state) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS state rows");
 static_assert(sizeof(gysk_svc_clients) == 32 && sizeof(gysk_svc_clients) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS client rows");
 static_assert(sizeof(gysk_cluster_row) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS cluster rows");
+static_assert(sizeof(gysk_svc_top_clients) == 280 && QCHUNK * sizeof(gysk_svc_top_clients) <= STAGE_BYTES, "the stage holds a chunk of top-client rows");
 static_assert(sizeof(gysk_logical_trace) == 168 && sizeof(gysk_logical_trace) <= sizeof(gysk_svc_summary), "the stage holds WIN_ROWS logical trace rows");
 static_assert(sizeof(TraceSlab) <= STAGE_BYTES, "the stage holds one merged trace digest");
 

@@ -148,6 +148,23 @@ struct SvcClientSlotReset
 		SvcSlotReset {}(st, slot, t, nt);
 	}
 };
+// GYSK_FLAG_SVC_TOP_CLIENTS: the reset of Inner and the slot's 3 + NSLOTS summaries zeroed
+template <typename Inner>
+struct SvcTopcSlotReset
+{
+	SvcTopClients tc;
+	Inner inner;
+	__device__ void operator()(const DevState &st, uint32_t slot, uint32_t t, uint32_t nt) const
+	{
+		constexpr uint32_t W = sizeof(TopcSet) / 8;
+		for (uint32_t i = t; i < (3u + NSLOTS) * W; i += nt) {
+			const uint32_t set = i / W, w = i % W;
+			TopcSet *base = set == 0 ? tc.open : set == 1 ? tc.last : set == 2 ? tc.level : tc.ring + (size_t)(set - 3) * tc.stride;
+			reinterpret_cast<unsigned long long *>(base + slot)[w] = 0ull;
+		}
+		inner(st, slot, t, nt);
+	}
+};
 
 // service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state: one CTA per service slot, one thread per
 // process slot (grid-stride): gysk_create over every slot, gysk_grow over the new ones
@@ -3045,14 +3062,19 @@ int launch_task_flush(const DevState &st, uint32_t max_tasks, uint32_t tsec, uin
 	return 2;
 }
 
-int launch_flush(const DevState &st, const ClientLevels &cl, uint32_t nslots, uint32_t tsec, uint32_t idle_secs, cudaStream_t s)
+int launch_flush(const DevState &st, const ClientLevels &cl, const SvcTopClients &tc, uint32_t nslots, uint32_t tsec, uint32_t idle_secs,
+		cudaStream_t s)
 {
 	if (!nslots) return 0;
 	cudaMemsetAsync(st.counters + CTR_NEVICT, 0, sizeof(unsigned long long), s);
 	flush_kernel<<<div_up((uint64_t)nslots * HIST_CELLS, 256), 256, 0, s>>>(st, nslots, tsec, idle_secs);
 	state_kernel<<<div_up(nslots, 128), 128, 0, s>>>(st, nslots, tsec);
 	if (!idle_secs) return 2;
-	if (cl.open) evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL,
+	if (tc.open && cl.open) evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT,
+			st.counters + CTR_EVICTED_TOTAL, nullptr, SvcTopcSlotReset<SvcClientSlotReset> {tc, SvcClientSlotReset {cl}});
+	else if (tc.open) evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT,
+			st.counters + CTR_EVICTED_TOTAL, nullptr, SvcTopcSlotReset<SvcSlotReset> {tc, SvcSlotReset {}});
+	else if (cl.open) evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL,
 			nullptr, SvcClientSlotReset {cl});
 	else evict_kernel<<<296, 256, 0, s>>>(st, st.svc_tbl, st.evict_list, st.evict_ids, st.counters + CTR_NEVICT, st.counters + CTR_EVICTED_TOTAL, nullptr,
 			SvcSlotReset {});		// grid-stride over the (device-side) eviction list
@@ -3319,6 +3341,307 @@ int launch_trace_list(const DevState &st, uint32_t nrows, int host_filter, uint3
 int launch_gather_trace(const DevState &st, const unsigned long long *d_id, int last_window, TraceRaw *d_out, cudaStream_t s)
 {
 	gather_trace_kernel<<<1, 32, 0, s>>>(st, d_id, last_window, d_out);
+	return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// GYSK_FLAG_SVC_TOP_CLIENTS: each service's heaviest clients by kbytes, weighted Misra-Gries in its mergeable form (DESIGN.md §2).
+// A batch: topc_pairs_kernel sums the connection records per (service, client) in the pair table, the claimed entries are sorted by
+// service, and each service's segment is merged into its open summary, a long segment in pieces of TOPC_PIECE pairs, one warp each,
+// whose K + 1 best the service's warp merges (the union's K + 1 best lie among them). A flush: topc_roll_kernel.
+// ---------------------------------------------------------------------------------------------------
+static constexpr int TOPC_WARPS = 4;
+
+// the merge's order: kbytes descending, then flow key ascending
+__device__ __forceinline__ bool topc_better(const TopcCand &a, const TopcCand &b) { return a.kb > b.kb || (a.kb == b.kb && a.key < b.key); }
+
+// The K + 1 best candidates offered so far, in order, in a warp's shared list l, n of them (warp-uniform). Every lane calls with one
+// candidate or none (valid false); the flow keys offered to one list are distinct. A round that beats nothing costs one ballot.
+__device__ __forceinline__ void topc_offer(TopcCand *l, uint32_t &n, const TopcCand &c, bool valid, int lane)
+{
+	constexpr uint32_t K1 = TOPC_K + 1;
+	const bool beat = valid && (n < K1 || topc_better(c, l[K1 - 1]));
+	const unsigned m = __ballot_sync(0xffffffffu, beat);
+	if (!m) return;
+	const TopcCand mine = (uint32_t)lane < n ? l[lane] : TopcCand {0ull, 0ull, 0ull};
+	uint32_t rl = (uint32_t)lane, rc = 0;		// ranks in the union of the list and this round's winners
+	for (unsigned b = m; b; b &= b - 1) {
+		const int j = __ffs(b) - 1;
+		const TopcCand o {__shfl_sync(0xffffffffu, c.key, j), __shfl_sync(0xffffffffu, c.kb, j), __shfl_sync(0xffffffffu, c.conns, j)};
+		if ((uint32_t)lane < n && topc_better(o, mine)) ++rl;
+		if (beat && j != lane && topc_better(o, c)) ++rc;
+	}
+	if (beat) for (uint32_t i = 0; i < n; ++i) rc += topc_better(l[i], c);
+	__syncwarp();
+	if ((uint32_t)lane < n && rl < K1) l[rl] = mine;
+	if (beat && rc < K1) l[rc] = c;
+	n = min(n + (uint32_t)__popc(m), K1);
+	__syncwarp();
+}
+
+// the merge's last steps from the K + 1 best groups l[0, n): c = the (K + 1)-th kbytes (0 with at most K groups), the groups above c
+// kept as kbytes - c, in order, saturated at 2^32 - 1, the rest of the entries zero; delta = delta_in + c
+__device__ __forceinline__ void topc_store(const TopcCand *l, uint32_t n, unsigned long long delta_in, TopcSet *out, int lane)
+{
+	const unsigned long long c = n > TOPC_K ? l[TOPC_K].kb : 0ull;
+	if ((uint32_t)lane < TOPC_K) {
+		gysk_topc_entry e {0ull, 0u, 0u};
+		if ((uint32_t)lane < n && l[lane].kb > c) {
+			e.flow_key = l[lane].key;
+			e.kbytes = (uint32_t)min(l[lane].kb - c, 0xFFFFFFFFull);
+			e.conns = (uint32_t)min(l[lane].conns, 0xFFFFFFFFull);
+		}
+		out->ent[lane] = e;
+	}
+	if (lane == 0) out->delta = delta_in + c;
+	__syncwarp();
+}
+
+// the held entries of summary s (a prefix: kbytes > 0) into buf[m ..]; returns m + their number
+__device__ __forceinline__ uint32_t topc_gather(const TopcSet *s, TopcCand *buf, uint32_t m, int lane)
+{
+	uint32_t kb = 0;
+	if ((uint32_t)lane < TOPC_K) {
+		const gysk_topc_entry e = s->ent[lane];
+		kb = e.kbytes;
+		if (kb) buf[m + lane] = TopcCand {e.flow_key, e.kbytes, e.conns};
+	}
+	const uint32_t k = (uint32_t)__popc(__ballot_sync(0xffffffffu, kb != 0));
+	__syncwarp();
+	return m + k;
+}
+
+__device__ __forceinline__ uint32_t topc_hash(uint32_t slot, unsigned long long fk)
+{
+	return table_hash(fk ^ ((unsigned long long)(slot + 1u) * 0xC2B2AE3D27D4EB4Full));
+}
+
+// one warp per record region (grid-stride): each connection record (every TCP record but the QRY_REC response samples, the records of
+// the service's exact cell) adds {kbytes, 1} to the entry of its (service, client) pair. The record that claims an entry with the 128-bit
+// CAS appends the sort key {slot : 32 | entry}. The table holds at least 2 x max_batch entries, so a probe always ends.
+__global__ void __launch_bounds__(256) topc_pairs_kernel(const uint4 *__restrict__ q, const uint2 *__restrict__ cnt, RecRegions rr, SvcTopClients tc,
+		unsigned long long *__restrict__ keys)
+{
+	const int lane = threadIdx.x & 31;
+	const IngestRec *recs = reinterpret_cast<const IngestRec *>(q);
+	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < rr.nwarps; r += (gridDim.x * blockDim.x) >> 5) {
+		const uint32_t m = cnt[r].x;
+		for (uint32_t i = lane; i < m; i += 32) {
+			const IngestRec rec = ld_rec(recs + (unsigned long long)r * rr.cap + i);
+			if (rec.slot == QRY_REC) continue;
+			const ulonglong2 want = make_ulonglong2(rec.flow_key, (unsigned long long)rec.slot + 1ull);
+			uint32_t pos = topc_hash(rec.slot, rec.flow_key) & tc.pmask;
+			for (;;) {
+				ulonglong2 k = __ldcg(tc.pkey + pos);
+				if (!k.y) {
+					k = atomicCAS(tc.pkey + pos, make_ulonglong2(0ull, 0ull), want);
+					if (!k.y) {
+						keys[atomicAdd(tc.cnt, 1ull)] = ((unsigned long long)rec.slot << 32) | pos;
+						break;
+					}
+				}
+				if (k.x == want.x && k.y == want.y) break;
+				pos = (pos + 1u) & tc.pmask;
+			}
+			atomicAdd(&tc.pacc[pos].x, (unsigned long long)(rec.value >> 10));
+			atomicAdd(&tc.pacc[pos].y, 1ull);
+		}
+	}
+}
+
+// one thread per sorted key: the first key of each service's run appends its segment {begin, end, slot, first piece}; a segment of more
+// than TOPC_PIECE pairs takes ceil(len / TOPC_PIECE) pieces
+__global__ void __launch_bounds__(256) topc_segs_kernel(const unsigned long long *__restrict__ keys, SvcTopClients tc, uint4 *__restrict__ segs)
+{
+	const uint32_t n = (uint32_t)tc.cnt[0], i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const uint32_t slot = (uint32_t)(keys[i] >> 32);
+	if (i && (uint32_t)(keys[i - 1] >> 32) == slot) return;
+	uint32_t lo = i + 1, hi = n;
+	while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if ((uint32_t)(keys[mid] >> 32) == slot) lo = mid + 1; else hi = mid; }
+	uint32_t base = 0;
+	if (lo - i > TOPC_PIECE) {
+		const uint32_t np = (lo - i + TOPC_PIECE - 1) / TOPC_PIECE;
+		base = (uint32_t)atomicAdd(tc.cnt + 2, (unsigned long long)np);
+		for (uint32_t j = 0; j < np; ++j) {
+			TopcPiece &p = tc.pieces[base + j];
+			p.beg = i + j * TOPC_PIECE; p.end = min(lo, i + (j + 1) * TOPC_PIECE); p.slot = slot;
+		}
+	}
+	segs[atomicAdd(tc.cnt + 1, 1ull)] = make_uint4(i, lo, slot, base);
+}
+
+// the pairs of sorted keys [beg, end), one service's, each with the old entry of the same client added (old[0, nold) in shared memory;
+// bit j of the returned mask for each old entry met), offered to the warp's list; each pair's entry emptied for the next batch
+__device__ __forceinline__ uint32_t topc_take_pairs(const SvcTopClients &tc, const unsigned long long *__restrict__ keys, uint32_t beg, uint32_t end,
+		const TopcCand *old, uint32_t nold, TopcCand *l, uint32_t &n, int lane)
+{
+	uint32_t matched = 0;
+	for (uint32_t i0 = beg; i0 < end; i0 += 32) {
+		const uint32_t i = i0 + (uint32_t)lane;
+		TopcCand c {0ull, 0ull, 0ull};
+		if (i < end) {
+			const uint32_t pos = (uint32_t)keys[i];
+			const ulonglong2 k = tc.pkey[pos], a = tc.pacc[pos];
+			tc.pkey[pos] = make_ulonglong2(0ull, 0ull); tc.pacc[pos] = make_ulonglong2(0ull, 0ull);
+			c = TopcCand {k.x, a.x, a.y};
+			for (uint32_t j = 0; j < nold; ++j) {
+				if (old[j].key != c.key) continue;
+				c.kb += old[j].kb; c.conns += old[j].conns; matched |= 1u << j;
+			}
+		}
+		topc_offer(l, n, c, c.kb != 0, lane);
+	}
+	return __reduce_or_sync(0xffffffffu, matched);
+}
+
+// one warp per piece of a long segment (grid-stride): its K + 1 best, and the old entries it met
+__global__ void __launch_bounds__(TOPC_WARPS * 32) topc_piece_kernel(const unsigned long long *__restrict__ keys, SvcTopClients tc)
+{
+	__shared__ TopcCand list[TOPC_WARPS][TOPC_K + 1], old[TOPC_WARPS][TOPC_K];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t np = (uint32_t)tc.cnt[2];
+	for (uint32_t p = blockIdx.x * TOPC_WARPS + wid; p < np; p += gridDim.x * TOPC_WARPS) {
+		TopcPiece &pc = tc.pieces[p];
+		const uint32_t nold = topc_gather(tc.open + pc.slot, old[wid], 0, lane);
+		uint32_t n = 0;
+		const uint32_t matched = topc_take_pairs(tc, keys, pc.beg, pc.end, old[wid], nold, list[wid], n, lane);
+		if ((uint32_t)lane < n) pc.c[lane] = list[wid][lane];
+		if (lane == 0) { pc.n = n; pc.matched = matched; }
+		__syncwarp();
+	}
+}
+
+// one warp per segment (grid-stride): the service's open summary merged with its batch sums, from the pairs themselves (a short segment)
+// or from its pieces' lists, then the old entries no pair met
+__global__ void __launch_bounds__(TOPC_WARPS * 32) topc_merge_kernel(const unsigned long long *__restrict__ keys, const uint4 *__restrict__ segs,
+		SvcTopClients tc)
+{
+	__shared__ TopcCand list[TOPC_WARPS][TOPC_K + 1], old[TOPC_WARPS][TOPC_K];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	const uint32_t ns = (uint32_t)tc.cnt[1];
+	for (uint32_t q = blockIdx.x * TOPC_WARPS + wid; q < ns; q += gridDim.x * TOPC_WARPS) {
+		const uint4 sg = segs[q];
+		TopcSet *set = tc.open + sg.z;
+		const unsigned long long delta = set->delta;
+		const uint32_t nold = topc_gather(set, old[wid], 0, lane);
+		uint32_t n = 0, matched = 0;
+		if (sg.y - sg.x <= TOPC_PIECE) matched = topc_take_pairs(tc, keys, sg.x, sg.y, old[wid], nold, list[wid], n, lane);
+		else {
+			const TopcPiece *pc = tc.pieces + sg.w, *pe = pc + (sg.y - sg.x + TOPC_PIECE - 1) / TOPC_PIECE;
+			for (; pc < pe; ++pc) {
+				const uint32_t pn = pc->n;
+				matched |= pc->matched;
+				TopcCand c {0ull, 0ull, 0ull};
+				if ((uint32_t)lane < pn) c = pc->c[lane];
+				topc_offer(list[wid], n, c, (uint32_t)lane < pn, lane);
+			}
+		}
+		const bool left = (uint32_t)lane < nold && !((matched >> lane) & 1u);
+		topc_offer(list[wid], n, left ? old[wid][lane] : TopcCand {0ull, 0ull, 0ull}, left, lane);
+		topc_store(list[wid], n, delta, set, lane);
+	}
+}
+
+// the groups of buf[0, m) by flow key (kbytes and conns summed, a group with 0 kbytes dropped) offered to the list
+__device__ __forceinline__ void topc_offer_groups(const TopcCand *buf, uint32_t m, TopcCand *l, uint32_t &n, int lane)
+{
+	for (uint32_t i0 = 0; i0 < m; i0 += 32) {
+		const uint32_t i = i0 + (uint32_t)lane;
+		TopcCand c {0ull, 0ull, 0ull};
+		bool first = i < m;
+		if (first) {
+			c = buf[i];
+			for (uint32_t j = 0; j < m; ++j) {
+				if (j == i || buf[j].key != c.key) continue;
+				if (j < i) { first = false; break; }
+				c.kb += buf[j].kb; c.conns += buf[j].conns;
+			}
+		}
+		topc_offer(l, n, c, first && c.kb != 0, lane);
+	}
+}
+
+// GYSK_FLAG_SVC_TOP_CLIENTS at a flush, one warp per service slot of [0, nslots) (grid-stride): ring slot k becomes the merge of the open
+// summary and what it holds (the open summary alone when the flush started a new epoch there), then the level the merge of the live
+// slots, slot k's new content included: the rule of client_roll_kernel with the summaries' merge for max
+__global__ void __launch_bounds__(TOPC_WARPS * 32) topc_roll_kernel(SvcTopClients tc, uint32_t nslots, uint32_t k, uint32_t live, uint32_t fresh)
+{
+	__shared__ TopcCand buf[TOPC_WARPS][NSLOTS * TOPC_K], list[TOPC_WARPS][TOPC_K + 1];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	for (uint32_t slot = blockIdx.x * TOPC_WARPS + wid; slot < nslots; slot += gridDim.x * TOPC_WARPS) {
+		const TopcSet *op = tc.open + slot;
+		TopcSet *rk = tc.ring + (size_t)k * tc.stride + slot;
+		unsigned long long delta = op->delta;
+		uint32_t m = topc_gather(op, buf[wid], 0, lane);
+		if (!fresh) { delta += rk->delta; m = topc_gather(rk, buf[wid], m, lane); }
+		uint32_t n = 0;
+		topc_offer_groups(buf[wid], m, list[wid], n, lane);
+		topc_store(list[wid], n, delta, rk, lane);
+		delta = 0; m = 0;
+		for (uint32_t j = 0; j < NSLOTS; ++j) {
+			if (!((live >> j) & 1u)) continue;
+			const TopcSet *sj = tc.ring + (size_t)j * tc.stride + slot;
+			delta += sj->delta;
+			m = topc_gather(sj, buf[wid], m, lane);
+		}
+		n = 0;
+		topc_offer_groups(buf[wid], m, list[wid], n, lane);
+		topc_store(list[wid], n, delta, tc.level + slot, lane);
+	}
+}
+
+// gysk_query_svc_top_clients / gysk_query_top_clients_window: one warp per row of summary array `sets`, by id (ids != nullptr: looked up,
+// id 0 and unknown ids give found = 0 and a zero row) or by slot (the window read)
+__global__ void __launch_bounds__(TOPC_WARPS * 32) topc_rows_kernel(DevState st, const TopcSet *__restrict__ sets, const unsigned long long *__restrict__ ids,
+		const unsigned long long *__restrict__ slots, uint32_t n, gysk_svc_top_clients *__restrict__ out)
+{
+	const int lane = threadIdx.x & 31;
+	const uint32_t q = blockIdx.x * TOPC_WARPS + (threadIdx.x >> 5);
+	if (q >= n) return;
+	const Resolved s = resolve_warp(st.svc_tbl, ids, slots, q, lane);
+	gysk_topc_entry e {0ull, 0u, 0u};
+	if (s.slot >= 0 && (uint32_t)lane < TOPC_K) e = sets[s.slot].ent[lane];
+	if ((uint32_t)lane < TOPC_K) out[q].entries[lane] = e;
+	const uint32_t held = (uint32_t)__popc(__ballot_sync(0xffffffffu, e.kbytes != 0));
+	if (lane == 0) {
+		out[q].glob_id = s.id; out[q].found = s.slot >= 0; out[q].n = held;
+		out[q].delta = s.slot >= 0 ? sets[s.slot].delta : 0ull;
+	}
+}
+
+int launch_topc_batch(const SortTemp &tmp, const SvcTopClients &tc, const RecRegions &rr, uint64_t n_events, uint32_t max_svcs, cudaStream_t s)
+{
+	if (!n_events) return 0;
+	const int nsm = sm_count(current_device());
+	cudaMemsetAsync(tc.cnt, 0, 3 * sizeof(unsigned long long), s);
+	topc_pairs_kernel<<<nsm * 8, 256, 0, s>>>(tmp.recq, tmp.rec_cnt, rr, tc, tmp.keys_a);
+	int slot_bits = 1;
+	while ((1ull << slot_bits) < max_svcs) ++slot_bits;
+	int which = 0;
+	const int sorted = launch_radix_sort(tmp, tc.cnt, n_events, 32, 32 + slot_bits, &which, s);
+	if (sorted < 0) return -1;
+	const unsigned long long *keys = which ? tmp.keys_b : tmp.keys_a;
+	topc_segs_kernel<<<div_up(n_events, 256), 256, 0, s>>>(keys, tc, tmp.segs);
+	topc_piece_kernel<<<nsm * 8, TOPC_WARPS * 32, 0, s>>>(keys, tc);
+	topc_merge_kernel<<<nsm * 16, TOPC_WARPS * 32, 0, s>>>(keys, tmp.segs, tc);
+	return 5 + sorted;
+}
+
+int launch_topc_roll(const SvcTopClients &tc, uint32_t nslots, const LevelRing &lv, cudaStream_t s)
+{
+	if (!nslots) return 0;
+	topc_roll_kernel<<<std::min<uint32_t>(div_up(nslots, TOPC_WARPS), (uint32_t)sm_count(current_device()) * 16u), TOPC_WARPS * 32, 0, s>>>(tc, nslots,
+			lv.cur[0], lv.live[0], lv.fresh & 1u);
+	return 1;
+}
+
+int launch_topc_rows(const DevState &st, const SvcTopClients &tc, int which, const unsigned long long *d_ids, const unsigned long long *d_slots,
+		uint32_t n, gysk_svc_top_clients *d_out, cudaStream_t s)
+{
+	if (!n) return 0;
+	const TopcSet *sets = which == GYSK_TOPC_OPEN ? tc.open : which == GYSK_TOPC_LAST ? tc.last : tc.level;
+	topc_rows_kernel<<<div_up(n, TOPC_WARPS), TOPC_WARPS * 32, 0, s>>>(st, sets, d_ids, d_slots, n, d_out);
 	return 1;
 }
 

@@ -204,6 +204,31 @@ static constexpr uint32_t QRY_CLI_ERR = 1u << 30, QRY_SER_ERR = 1u << 31, QRY_US
 static constexpr uint32_t CL_REGS = 1u << GYSK_HLL_WINDOW_P;
 struct ClientLevels { uint8_t *open, *last, *ring, *level; uint32_t stride; };
 
+// GYSK_FLAG_SVC_TOP_CLIENTS: per service slot summaries of TOPC_K entries (gysk_topc_entry, best first, zero past the held ones) and the
+// bound delta: the open window, the last closed one and the 300-s level ([max_svcs + 1] each), and the ring of NSLOTS 30-s slots
+// ([NSLOTS][stride], the client ring's layout). The batch scratch: the pair table of pmask + 1 entries keyed {flow_key, slot + 1} (hi 0:
+// empty) beside their sums {kbytes, conns}, zero between batches; the counters {pairs, segments, pieces}; the piece lists of the long
+// segments (TopcPiece, pieces_cap of them). Outside DevState, so that the kernels without the flag keep their parameter layout. Every
+// pointer nullptr: off.
+static constexpr uint32_t TOPC_K = GYSK_SVC_TOPC_K;
+static constexpr uint32_t TOPC_PIECE = 1024;		// pairs per piece: a longer segment is cut into pieces, one warp each
+struct TopcSet { gysk_topc_entry ent[TOPC_K]; unsigned long long delta; };
+static_assert(sizeof(TopcSet) == 264, "a summary is 16 entries and its bound");
+struct TopcCand { unsigned long long key, kb, conns; };
+// a piece of a long segment: its sorted keys [beg, end) of service slot, then the K + 1 best of its pairs (each with the old entry of its
+// client added) and the old entries it met (bit j: entry j)
+struct TopcPiece { TopcCand c[TOPC_K + 1]; uint32_t n, matched, beg, end, slot, pad; };
+struct SvcTopClients
+{
+	TopcSet			*open, *last, *ring, *level;
+	uint32_t		stride;
+	ulonglong2		*pkey, *pacc;
+	uint32_t		pmask;
+	unsigned long long	*cnt;
+	TopcPiece		*pieces;
+	uint32_t		pieces_cap;
+};
+
 struct SortTemp
 {
 	unsigned long long	*keys_a, *keys_b;	// [nkeys] RESP sort keys of the batch (also the top-N sort keys)
@@ -329,7 +354,9 @@ int launch_task_flush(const DevState &st, uint32_t max_tasks, uint32_t tsec, uin
 // the window roll into ring slot st.levels.cur of each level (cleared by the host when it starts a new epoch), the listener states,
 // the idle-service eviction
 // (GYSK_FLAG_CLIENT_LEVELS, cl.open != nullptr: an evicted slot's client sets are cleared with it)
-int launch_flush(const DevState &st, const ClientLevels &cl, uint32_t max_svcs, uint32_t tsec, uint32_t idle_secs, cudaStream_t s);
+// (GYSK_FLAG_SVC_TOP_CLIENTS, tc.open != nullptr: an evicted slot's summaries are cleared with it)
+int launch_flush(const DevState &st, const ClientLevels &cl, const SvcTopClients &tc, uint32_t max_svcs, uint32_t tsec, uint32_t idle_secs,
+		cudaStream_t s);
 // clears table t and re-inserts the ids t.slot_id holds in slots [0, nslots)
 int launch_rebuild_table(const IdTable &t, uint32_t nslots, cudaStream_t s);
 // the single-id exports: the raw state of n ids (id 0 and unknown ids: found = 0); the HLL registers of the id d_ids[0]
@@ -372,6 +399,17 @@ int launch_client_roll(const ClientLevels &cl, uint32_t nslots, const LevelRing 
 // the client rows (gysk_svc_clients) by id (d_ids) or by slot (d_slots); the estimates as hll_pending leaves them
 int launch_client_rows(const DevState &st, const ClientLevels &cl, const unsigned long long *d_ids, const unsigned long long *d_slots, uint32_t n,
 		gysk_svc_clients *d_out, cudaStream_t s);
+// GYSK_FLAG_SVC_TOP_CLIENTS after a batch's drain passes and top-K selections (it takes tmp's sort buffers and segment array): the
+// batch's exact per-(service, client) sums of the TCP regions' connection records, grouped by service and merged into each service's
+// open summary. -1: no sort plan
+// (rr: the regions of the batch's ingest launch)
+int launch_topc_batch(const SortTemp &tmp, const SvcTopClients &tc, const RecRegions &rr, uint64_t n_events, uint32_t max_svcs, cudaStream_t s);
+// GYSK_FLAG_SVC_TOP_CLIENTS at the flush, before the open / last swap: each open summary of slots [0, nslots) merged into ring slot
+// lv.cur[0] (in its place when the slot is fresh), then the level = the merge of the live slots (level 0's decision of lv)
+int launch_topc_roll(const SvcTopClients &tc, uint32_t nslots, const LevelRing &lv, cudaStream_t s);
+// the rows of summary `which` (GYSK_TOPC_*) by id (d_ids) or by slot (d_slots)
+int launch_topc_rows(const DevState &st, const SvcTopClients &tc, int which, const unsigned long long *d_ids, const unsigned long long *d_slots,
+		uint32_t n, gysk_svc_top_clients *d_out, cudaStream_t s);
 // the CL_REGS registers at regs + slot * CL_REGS of the id d_ids[0] (gysk_export_hll_window)
 int launch_gather_hll_window(const DevState &st, const uint8_t *regs, const unsigned long long *d_ids, int32_t *found, uint8_t *d_out, cudaStream_t s);
 // trace rows at gysk_flush: the half `open` (the one the flush opens) of rows [0, nrows) cleared

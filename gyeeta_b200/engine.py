@@ -16,6 +16,12 @@ FLOW_QRY_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("queries", "<u4"), ("resp_m
 FLOW_RESP_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("counts", "<u4", (15,)), ("total", "<u4"), ("p25_ms", "<i8"), ("p95_ms", "<i8"),
                                 ("p99_ms", "<i8")])                                                   # gysk_flow_resp_est
 RESP_HIST_WORDS = 8     # u64 words of one flow response histogram cell
+# gysk_svc_top_clients (GYSK_FLAG_SVC_TOP_CLIENTS): a service's heaviest clients, best first, and the bound delta
+TOPC_K = 16
+TOPC_ENTRY_DTYPE = np.dtype([("flow_key", "<u8"), ("kbytes", "<u4"), ("conns", "<u4")])
+SVC_TOP_CLIENTS_DTYPE = np.dtype([("glob_id", "<u8"), ("found", "<i4"), ("n", "<u4"), ("delta", "<u8"), ("entries", TOPC_ENTRY_DTYPE, (TOPC_K,))])
+assert SVC_TOP_CLIENTS_DTYPE.itemsize == 280
+TOPC_OPEN, TOPC_LAST, TOPC_5MIN = 0, 1, 2
 FLOW_ERR_EST_DTYPE = np.dtype([("flow_key", "<u8"), ("queries", "<u4"), ("cli_errors", "<u4"), ("ser_errors", "<u4"),
                                ("pad", "<u4")])                                                       # gysk_flow_err_est
 
@@ -48,6 +54,7 @@ FLAG_FLOW_TOPK_5MIN = 0x800
 FLAG_FLOW_TOPK_SLOW = 0x1000
 FLAG_CLIENT_LEVELS = 0x2000
 FLAG_FLOW_ERRORS = 0x4000
+FLAG_SVC_TOP_CLIENTS = 0x8000
 HLL_WINDOW_P = 8
 CLIENTS_LAST, CLIENTS_5MIN = 0, 1
 FLOW_TOPK_CAP = 4096
@@ -369,6 +376,8 @@ def load_library(path=None):
         "gysk_topk_flow_errors_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_topk_flow_errors_global_5min": (i32, [vp, u32, vp, vp, vp]),
         "gysk_query_svc_clients": (i32, [vp, vp, u32, vp]),
+        "gysk_query_svc_top_clients": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_top_clients_window": (i32, [vp, C.c_int32, u32, i32, vp, vp, u32, vp]),
         "gysk_query_clients_window": (i32, [vp, C.c_int32, u32, vp, vp, u32, vp]),
         "gysk_export_hll_window": (i32, [vp, u64, i32, vp]),
         "gysk_query_logical_clients": (i32, [vp, vp, u32, vp]),
@@ -439,7 +448,8 @@ class Engine:
                  td_compression=200, max_batch=1 << 20, auto_register=True, rank=0, world=1, stage_batch=0, idle_evict_secs=0,
                  merge_levels=False, merge_states=False, merge_clusters=False, merge_topn=False, flow_level=False, task_idle_evict_secs=0,
                  max_trace_svcs=0, merge_traces=False, flow_queries=False, flow_query_level=False, flow_resp_hist=False,
-                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False, client_levels=False, flow_errors=False):
+                 flow_topk=False, flow_topk_5min=False, flow_topk_slow=False, client_levels=False, flow_errors=False,
+                 svc_top_clients=False):
         self.L = load_library()
         cfg = Config()
         self.L.gysk_config_default(C.byref(cfg))
@@ -456,7 +466,8 @@ class Engine:
                     (FLAG_FLOW_QUERIES if flow_queries else 0) | (FLAG_FLOW_QUERY_LEVEL if flow_query_level else 0) | \
                     (FLAG_FLOW_RESP_HIST if flow_resp_hist else 0) | (FLAG_FLOW_TOPK if flow_topk else 0) | \
                     (FLAG_FLOW_TOPK_5MIN if flow_topk_5min else 0) | (FLAG_FLOW_TOPK_SLOW if flow_topk_slow else 0) | \
-                    (FLAG_CLIENT_LEVELS if client_levels else 0) | (FLAG_FLOW_ERRORS if flow_errors else 0)
+                    (FLAG_CLIENT_LEVELS if client_levels else 0) | (FLAG_FLOW_ERRORS if flow_errors else 0) | \
+                    (FLAG_SVC_TOP_CLIENTS if svc_top_clients else 0)
         cfg.rank, cfg.world = rank, world
         self.cfg = cfg
         self.h = C.c_void_p()
@@ -916,6 +927,29 @@ class Engine:
         out = (SvcClients * max(cap, 1))()
         hosts = np.zeros(max(cap, 1), dtype=np.uint32)
         self._chk(self.L.gysk_query_clients_window(self.h, host_idx, flags, out if cap else None, _p(hosts) if cap else None, cap, C.byref(n)))
+        k = min(cap, n.value)
+        return out[:k], hosts[:k].copy(), n.value
+
+    def query_svc_top_clients(self, ids, which=TOPC_LAST):
+        """gysk_query_svc_top_clients: SVC_TOP_CLIENTS_DTYPE rows of service ids, summary TOPC_OPEN, TOPC_LAST or TOPC_5MIN
+        (svc_top_clients=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = np.zeros(max(len(ids), 1), dtype=SVC_TOP_CLIENTS_DTYPE)
+        self._chk(self.L.gysk_query_svc_top_clients(self.h, _p(ids), len(ids), which, _p(out)))
+        return out[: len(ids)]
+
+    def query_top_clients_window(self, which=TOPC_LAST, host_idx=-1, active_only=False, cap=None):
+        """gysk_query_top_clients_window: (SVC_TOP_CLIENTS_DTYPE rows in the order of query_window_hosts, host_idx of each row, number
+        of rows). cap None = all rows (a count call first); 0 = the count only"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_top_clients_window(self.h, host_idx, flags, which, None, None, 0, C.byref(n)))
+            cap = n.value
+        out = np.zeros(max(cap, 1), dtype=SVC_TOP_CLIENTS_DTYPE)
+        hosts = np.zeros(max(cap, 1), dtype=np.uint32)
+        self._chk(self.L.gysk_query_top_clients_window(self.h, host_idx, flags, which, _p(out) if cap else None, _p(hosts) if cap else None, cap,
+                                                       C.byref(n)))
         k = min(cap, n.value)
         return out[:k], hosts[:k].copy(), n.value
 

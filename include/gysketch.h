@@ -284,6 +284,10 @@ typedef struct gysk_task24 { uint64_t aggr_task_id; uint32_t cpu_pct; uint32_t c
 						   the TCP drain pass 6.57 -> 6.75 ms and the TASK pass 1.40 -> 1.58 ms per batch; at 100 %
 						   the TCP pass 17.2 ms. Without it nothing is allocated, every other call answers as
 						   before and the flow error calls are GYSK_ERR_NOTSUP */
+#define GYSK_FLAG_SVC_TOP_CLIENTS	0x8000u	/* each service's GYSK_SVC_TOPC_K heaviest clients by kbytes, in the open window, the
+						   last one and the rolling 300 s, with a stated error bound (gysk_query_svc_top_clients,
+						   "each service's heaviest clients" below). Needs no other flag. Without it nothing is
+						   allocated, every other call answers as before and the two calls are GYSK_ERR_NOTSUP */
 #define GYSK_HLL_WINDOW_P		8u	/* precision of the windowed client registers: 256 one-byte registers per set (fixed:
 						   gysk_config has no word for it) */
 
@@ -965,6 +969,55 @@ int		gysk_query_clients_window(gysk_engine *e, int32_t host_idx, uint32_t flags,
 int		gysk_export_hll_window(gysk_engine *e, uint64_t glob_id, int which, uint8_t regs[256]);
 int		gysk_query_logical_clients(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_svc_clients *out);
 int		gysk_export_logical_hll_window(gysk_engine *e, uint64_t logical_id, int which, uint8_t regs[256]);
+
+/* ---- each service's heaviest clients (GYSK_FLAG_SVC_TOP_CLIENTS): who loads a listener ----
+ * The reference answers "who is loading this listener" from a per-listener map of client processes and their bytes, cleared every
+ * interval (connlistenmap_, written to activeconntbl). Here each service slot holds bounded summaries of K = GYSK_SVC_TOPC_K entries
+ * {flow_key, kbytes, conns} and one bound delta:
+ *  - what counts: exactly the records that feed the service's exact {count, kbytes} cell (nconns_5s / kbytes_5s): event32 CONNECT /
+ *    ACCEPT / CLOSE_CLI / CLOSE_SER, TCP24, raw IPv4 / IPv6 connection records and NOTIFY_TCP_CONN (flow_key = cli_task_aggr_id_).
+ *    Each adds conns += 1 and kbytes += bytes >> 10 to the pair (service, flow_key). Response samples, API_TRAN, trace events,
+ *    NOTIFY_ACTIVE_CONN_STATS, process records, unknown ids and dropped events never count;
+ *  - the rule is weighted Misra-Gries in its mergeable form (Agarwal et al., Mergeable Summaries, 2012). A merge of summaries, or of a
+ *    summary with exact per-client sums: group the union by flow_key and sum kbytes and conns, dropping a group with 0 kbytes; c = the
+ *    (K + 1)-th largest kbytes of the groups (0 with at most K groups); keep the groups with kbytes > c as kbytes - c with their conns;
+ *    delta = the sum of the inputs' deltas + c. Entries are ordered by kbytes descending, then flow_key ascending; kbytes and conns
+ *    saturate at 2^32 - 1. The result depends on neither record order nor route;
+ *  - guarantees, for every client f of the service over the records the summary covers (est = 0 for an unlisted client):
+ *    est(f) <= exact(f) <= est(f) + delta; sum(est) + (K + 1) x delta <= the service's kbytes over the same records; a service with at
+ *    most K clients of positive kbytes lists them all exactly with delta = 0; a listed client's conns is at most its exact count;
+ *  - after each device batch the open summary is merged with the batch's exact per-client sums. At gysk_flush the open summary is merged
+ *    into ring slot (tsec / 30) % 10 (it replaces a slot holding an older epoch), the 300-s level becomes the merge of the live ring
+ *    slots (the windows of p95_5min_resp_ms), and the open summary becomes the last one while a cleared one opens;
+ *  - an evicted service's summaries are cleared with its slot; gysk_grow keeps them.
+ * Cost: 13 summaries of 264 bytes per service slot (3 432 B; gysk_slot_bytes counts them), and a batch pair table of 32 bytes x
+ * next_pow2(2 x max_batch) entries plus the piece lists of the long segments (about 260 MiB at the default max_batch = 2^22; 8 GiB at 2^27).
+ * gysk_query_svc_top_clients: one row per id of the summary `which`; found = 0, n = 0 and zero entries for an unknown id. GYSK_TOPC_OPEN
+ *   answers as of the events handed in so far, the other two as of the last gysk_flush.
+ * gysk_query_top_clients_window: the rows of gysk_query_window_hosts' services, in its order, with its host filter,
+ *   GYSK_WINDOW_ACTIVE_ONLY and count / capacity rules; each row byte-equal to gysk_query_svc_top_clients' row of its id.
+ * Both are GYSK_ERR_NOTSUP without the flag and GYSK_ERR_INVAL for another `which`. K is fixed: gysk_config has no word for it. */
+#define GYSK_SVC_TOPC_K			16u
+#define GYSK_TOPC_OPEN			0	/* the open window */
+#define GYSK_TOPC_LAST			1	/* the window the last gysk_flush closed */
+#define GYSK_TOPC_5MIN			2	/* the rolling 300-s level */
+typedef struct gysk_topc_entry
+{
+	uint64_t	flow_key;		/* the client: the connection's flow key (NOTIFY_TCP_CONN: cli_task_aggr_id_) */
+	uint32_t	kbytes;			/* the estimate est(f), at most the client's exact kbytes */
+	uint32_t	conns;			/* records counted since the entry last entered the summary */
+} gysk_topc_entry;
+typedef struct gysk_svc_top_clients
+{
+	uint64_t	glob_id;
+	int32_t		found;
+	uint32_t	n;			/* entries held, best first; entries[n ..] are zero */
+	uint64_t	delta;			/* the bound: exact(f) <= est(f) + delta for every client */
+	gysk_topc_entry	entries[GYSK_SVC_TOPC_K];
+} gysk_svc_top_clients;
+int		gysk_query_svc_top_clients(gysk_engine *e, const uint64_t *ids, uint32_t n, int which, gysk_svc_top_clients *out);
+int		gysk_query_top_clients_window(gysk_engine *e, int32_t host_idx, uint32_t flags, int which, gysk_svc_top_clients *out, uint32_t *hosts,
+				uint32_t cap, uint32_t *n);
 
 /* ---- request traces (gysk_config.max_trace_svcs != 0): the trace view per service and 5-s window ----
  * madhava writes every API_TRAN as one row of tracereqtbl (handle_trace_requests, server/gy_mconnhdlr.cc:5883-6060) and the trace view
