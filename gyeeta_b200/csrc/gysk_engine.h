@@ -95,6 +95,10 @@ struct TraceSlab { TdHead head; Centroid cent[TRACE_TD_CAP]; };
 static_assert(sizeof(TraceSlab) == 1632 && sizeof(TraceSlab) % 16 == 0, "TraceSlab: 32-byte head, 100 centroids");
 // the trace digests of nl logical services in whole SlabEntrys, packed after the rank's digests and top-N candidates
 inline uint32_t trace_slab_entries(uint32_t nl) { return (uint32_t)(((size_t)nl * sizeof(TraceSlab) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry)); }
+// GYSK_FLAG_SVC_TOP_CLIENTS: the two summaries of nl logical services (TopcSet [nl][2]: GYSK_TOPC_LAST, GYSK_TOPC_5MIN) in whole
+// SlabEntrys, packed after the rest of a rank's slab
+static_assert(2 * sizeof(TopcSet) == 528 && sizeof(SlabEntry) == 4128, "a logical service's two summaries are 528 bytes of a 4128-byte entry");
+inline uint32_t topc_slab_entries(uint32_t nl) { return (uint32_t)(((size_t)nl * 2 * sizeof(TopcSet) + sizeof(SlabEntry) - 1) / sizeof(SlabEntry)); }
 // u64 SUM words of one logical service's merged trace window: the sums of gysk_trace_window in its order, then the members holding a row
 enum { LT_NREQ = 0, LT_NERR, LT_NCONNS, LT_SUM_US, LT_BYTES_IN, LT_BYTES_OUT, LT_BKT /* 8 words */, LT_TD_COUNT = LT_BKT + 8, LT_NTRACED,
 	LT_WORDS };
@@ -334,6 +338,10 @@ struct MergeState
 	// from slab entry topke_off, after the slow sets (topk_slab_entries(1 or 2)); the merged ones land as set [3] of topk_final and
 	// topk5_final, which then hold four sets.
 	uint32_t		topke_off {0};
+	// GYSK_FLAG_SVC_TOP_CLIENTS: the rank's per-logical summaries (fold_topc_kernel) ride from slab entry topc_off, after everything else
+	// (topc_slab_entries(nl)); the merged ones of the last finished merge, [nl][2] as in the slab (nullptr without)
+	uint32_t		topc_off {0};
+	TopcSet			*topc_final {nullptr};
 	// GYSK_FLAG_CLIENT_LEVELS: MAX [nl][2][CL_REGS] in the u8 MAX region after the all-time registers, each logical service's last-window
 	// and 300-s client sets (nullptr without)
 	uint8_t			*cl_hll {nullptr};

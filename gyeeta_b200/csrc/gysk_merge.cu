@@ -17,9 +17,11 @@
 //                          the flush tsec pair in the i64 MAX region (once when both are set); GYSK_FLAG_FLOW_QUERIES puts the
 //                          flow query tables cur/last after the count-min tables, GYSK_FLAG_FLOW_QUERY_LEVEL their level after
 //                          them with the flush tsec pair as GYSK_FLAG_FLOW_LEVEL; GYSK_FLAG_FLOW_RESP_HIST the flow response
-//                          histograms cur/last [, 5min] after those
+//                          histograms cur/last [, 5min] after those; GYSK_FLAG_SVC_TOP_CLIENTS appends each logical service's
+//                          heaviest-client summaries (its members' folded in map order) to the slab
 //   (caller)             all-reduce each region once, all-gather the slab        — NCCL via torch.distributed
 //   gysk_merge_finish      rank-ascending merge + compress of the gathered digests [, the global pick of the gathered top-N candidates]
+//                          [, the rank-ascending fold of the gathered top-client summaries]
 //   gysk_query_logical     same summary fields as gysk_query_svcs, for logical ids
 //   gysk_export_logical_hist / gysk_merge_flush_range   one merged histogram / the ranks' flush tsec range
 //   gysk_query_logical_states[_all]   the member listeners' state counts per logical service (GYSK_FLAG_MERGE_STATES)
@@ -31,6 +33,7 @@
 // (common/gy_statistics.h:625-650): integer sums are order independent => bit-exact at any GPU count.
 #include "gysk_engine.h"
 #include "gysk_summary.cuh"
+#include "gysk_topc.cuh"
 
 #include <climits>
 #include <dlfcn.h>
@@ -345,6 +348,75 @@ __global__ void __launch_bounds__(MG_WARPS * 32) finish_td_kernel(const SlabEntr
 	}
 }
 
+// GYSK_FLAG_SVC_TOP_CLIENTS: each logical service's two summaries (GYSK_TOPC_LAST, GYSK_TOPC_5MIN: [l][0], [l][1]) as sequential
+// folds acc = merge(acc, s) from the empty summary (DESIGN.md §2): its members in map order on each rank (fold_topc_kernel), then the
+// ranks' results in ascending rank order (finish_topc_kernel). Every step merges at most 2K entries, so one warp does it; the result
+// does not depend on the launch shape.
+static constexpr int TC_WARPS = 4;
+struct TopcScratch { TopcCand buf[2 * TOPC_K], list[TOPC_K + 1]; TopcSet acc; };
+
+// acc = the empty summary
+__device__ __forceinline__ void topc_clear(TopcSet *acc, int lane)
+{
+	if ((uint32_t)lane < TOPC_K) acc->ent[lane] = gysk_topc_entry {0ull, 0u, 0u};
+	if (lane == 0) acc->delta = 0ull;
+	__syncwarp();
+}
+
+// acc = merge(acc, s): the groups of both by flow key, c = the (K + 1)-th kbytes, the groups above c less c, delta = both deltas + c
+__device__ __forceinline__ void topc_fold(TopcScratch &S, const TopcSet *s, int lane)
+{
+	const unsigned long long delta = S.acc.delta + s->delta;
+	const uint32_t m = topc_gather(s, S.buf, topc_gather(&S.acc, S.buf, 0, lane), lane);
+	uint32_t n = 0;
+	topc_offer_groups(S.buf, m, S.list, n, lane);
+	topc_store(S.list, n, delta, &S.acc, lane);
+}
+
+__device__ __forceinline__ void topc_put(const TopcSet &acc, TopcSet *out, int lane)
+{
+	if ((uint32_t)lane < TOPC_K) out->ent[lane] = acc.ent[lane];
+	if (lane == 0) out->delta = acc.delta;
+	__syncwarp();
+}
+
+// one warp per logical service (grid-stride): its members' last-window and 300-s summaries folded in map order into out[l][0 / 1]; a
+// member without a slot here is skipped (the identity)
+__global__ void __launch_bounds__(TC_WARPS * 32) fold_topc_kernel(SvcTopClients tc, Members mb, uint32_t nl, TopcSet *__restrict__ out)
+{
+	__shared__ TopcScratch scratch[TC_WARPS];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	TopcScratch &S = scratch[wid];
+
+	for (uint32_t l = blockIdx.x * TC_WARPS + wid; l < nl; l += gridDim.x * TC_WARPS) {
+		for (int set = 0; set < 2; ++set) {
+			const TopcSet *src = set ? tc.level : tc.last;
+			topc_clear(&S.acc, lane);
+			mb.each(l, [&](uint32_t s) { topc_fold(S, src + s, lane); });
+			topc_put(S.acc, out + (size_t)l * 2 + set, lane);
+		}
+	}
+}
+
+// one warp per logical service (grid-stride): the ranks' summaries of the all-gathered slabs [world][stride] (rank r's from entry topc_off)
+// folded in ascending rank order into out[l][0 / 1]
+__global__ void __launch_bounds__(TC_WARPS * 32) finish_topc_kernel(const SlabEntry *__restrict__ gathered, uint32_t world, uint32_t stride,
+		uint32_t topc_off, uint32_t nl, TopcSet *__restrict__ out)
+{
+	__shared__ TopcScratch scratch[TC_WARPS];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	TopcScratch &S = scratch[wid];
+
+	for (uint32_t l = blockIdx.x * TC_WARPS + wid; l < nl; l += gridDim.x * TC_WARPS) {
+		for (int set = 0; set < 2; ++set) {
+			topc_clear(&S.acc, lane);
+			for (uint32_t r = 0; r < world; ++r)
+				topc_fold(S, reinterpret_cast<const TopcSet *>(gathered + (size_t)r * stride + topc_off) + (size_t)l * 2 + set, lane);
+			topc_put(S.acc, out + (size_t)l * 2 + set, lane);
+		}
+	}
+}
+
 // GYSK_FLAG_MERGE_TOPN, one CTA per list m, one thread per candidate of the gathered slabs (rank r's lists at gathered + r * stride + nl,
 // each best first). Candidates with a non-zero score are ordered by score descending, then rank ascending, then local order, so the place
 // of rank r's entry i is i plus, in every other rank's list, the entries with a greater score or an equal one on a lower rank (a binary
@@ -575,6 +647,26 @@ __global__ void logical_trace_kernel(const int32_t *__restrict__ lidx, uint32_t 
 	out[q] = o;
 }
 
+// GYSK_FLAG_SVC_TOP_CLIENTS read side, one warp per row: summary `set` (0: GYSK_TOPC_LAST, 1: GYSK_TOPC_5MIN) of dense index lidx[q] as
+// topc_rows_kernel reads a service's, logical id lids[l]; an index of -1 gives found = 0 and a zero row
+__global__ void __launch_bounds__(LG_WARPS * 32) logical_topc_kernel(const int32_t *__restrict__ lidx, uint32_t n, const TopcSet *__restrict__ sets,
+		int set, const unsigned long long *__restrict__ lids, gysk_svc_top_clients *__restrict__ out)
+{
+	const int lane = threadIdx.x & 31;
+	const uint32_t q = blockIdx.x * LG_WARPS + (threadIdx.x >> 5);
+	if (q >= n) return;
+	const int32_t l = lidx[q];
+	const TopcSet *s = l >= 0 ? sets + (size_t)l * 2 + set : nullptr;
+	gysk_topc_entry e {0ull, 0u, 0u};
+	if (s && (uint32_t)lane < TOPC_K) e = s->ent[lane];
+	if ((uint32_t)lane < TOPC_K) out[q].entries[lane] = e;
+	const uint32_t held = (uint32_t)__popc(__ballot_sync(0xffffffffu, e.kbytes != 0));
+	if (lane == 0) {
+		out[q].glob_id = s ? lids[l] : 0ull; out[q].found = s != nullptr; out[q].n = held;
+		out[q].delta = s ? s->delta : 0ull;
+	}
+}
+
 } // namespace gysk
 
 namespace {
@@ -622,31 +714,38 @@ void launch_select(gysk_engine *e, const gysk_logical_trace *, unsigned long lon
 // Per row type of the logical and cluster reads: the launch that makes the rows of the dense indices lidx[0 .. m) in the device stage
 // (an index of -1 gives the not-found row), the finish that copies them out, the field a by-id read stamps with the queried id, and the
 // engine flag the rows need.
-int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_summary *)
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_summary *, int = 0)
 {
 	logical_summary_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(lidx, m, e->cfg.hll_p, e->mg.lg, e->mg.d_logical_ids,
 			reinterpret_cast<gysk_svc_summary *>(e->d_wstage));
 	return 1;
 }
-int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical_state *)
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical_state *, int = 0)
 {
 	logical_state_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(lidx, m, e->mg.lg, e->mg.d_logical_ids, reinterpret_cast<gysk_logical_state *>(e->d_wstage));
 	return 1;
 }
-int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_cluster_row *)
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_cluster_row *, int = 0)
 {
 	cluster_row_kernel<<<div_up(m, 256), 256, 0, e->stream>>>(lidx, m, e->mg.clusters.cl, e->mg.clusters.d_ids, reinterpret_cast<gysk_cluster_row *>(e->d_wstage));
 	return 1;
 }
-int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_clients *)
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_clients *, int = 0)
 {
 	logical_clients_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(lidx, m, e->mg.cl_hll, e->mg.d_logical_ids,
 			reinterpret_cast<gysk_svc_clients *>(e->d_wstage));
 	return 1;
 }
-int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical_trace *)
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_logical_trace *, int = 0)
 {
 	logical_trace_kernel<<<div_up(m, 128), 128, 0, e->stream>>>(lidx, m, e->mg.lg, e->mg.d_logical_ids, reinterpret_cast<gysk_logical_trace *>(e->d_wstage));
+	return 1;
+}
+// (which: the summary of the top-client rows)
+int launch_logical(gysk_engine *e, const int32_t *lidx, uint32_t m, gysk_svc_top_clients *, int which)
+{
+	logical_topc_kernel<<<div_up(m, LG_WARPS), LG_WARPS * 32, 0, e->stream>>>(lidx, m, e->mg.topc_final, which == GYSK_TOPC_5MIN, e->mg.d_logical_ids,
+			reinterpret_cast<gysk_svc_top_clients *>(e->d_wstage));
 	return 1;
 }
 SvcRows logical_finish(const gysk_engine *e, gysk_svc_summary *out) { return SvcRows {e->cfg.hll_p, out}; }
@@ -654,21 +753,24 @@ CopyRows<gysk_logical_state> logical_finish(const gysk_engine *, gysk_logical_st
 CopyRows<gysk_cluster_row> logical_finish(const gysk_engine *, gysk_cluster_row *out) { return CopyRows<gysk_cluster_row> {out}; }
 CopyRows<gysk_logical_trace> logical_finish(const gysk_engine *, gysk_logical_trace *out) { return CopyRows<gysk_logical_trace> {out}; }
 ClientRows logical_finish(const gysk_engine *, gysk_svc_clients *out) { return ClientRows {out}; }
+CopyRows<gysk_svc_top_clients> logical_finish(const gysk_engine *, gysk_svc_top_clients *out) { return CopyRows<gysk_svc_top_clients> {out}; }
 uint64_t &row_id(gysk_svc_summary &r) { return r.glob_id; }
 uint64_t &row_id(gysk_logical_state &r) { return r.logical_id; }
 uint64_t &row_id(gysk_cluster_row &r) { return r.cluster_id; }
 uint64_t &row_id(gysk_logical_trace &r) { return r.logical_id; }
 uint64_t &row_id(gysk_svc_clients &r) { return r.glob_id; }
+uint64_t &row_id(gysk_svc_top_clients &r) { return r.glob_id; }
 template <typename Row> constexpr uint32_t logical_flag()
 {
 	return std::is_same<Row, gysk_logical_state>::value ? GYSK_FLAG_MERGE_STATES : std::is_same<Row, gysk_cluster_row>::value ? GYSK_FLAG_MERGE_CLUSTERS :
-		std::is_same<Row, gysk_logical_trace>::value ? GYSK_FLAG_MERGE_TRACES : std::is_same<Row, gysk_svc_clients>::value ? GYSK_FLAG_CLIENT_LEVELS : 0;
+		std::is_same<Row, gysk_logical_trace>::value ? GYSK_FLAG_MERGE_TRACES : std::is_same<Row, gysk_svc_clients>::value ? GYSK_FLAG_CLIENT_LEVELS :
+		std::is_same<Row, gysk_svc_top_clients>::value ? GYSK_FLAG_SVC_TOP_CLIENTS : 0;
 }
 
 // gysk_query_logical / gysk_query_logical_states / gysk_query_cluster_states: the rows of n ids, in QCHUNK pieces, each row carrying its
-// queried id
+// queried id (which: the summary of the top-client rows)
 template <typename Row>
-int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out, const char *what)
+int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out, const char *what, int which = 0)
 {
 	CHECK_ENGINE(e);
 	if ((!ids || !out) && n) return GYSK_ERR_INVAL;
@@ -682,7 +784,7 @@ int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out
 	for (uint32_t i = 0; i < n; ++i) lidx[i] = dense_index(*sp.index, ids[i]);
 	const auto rows = logical_finish(e, out);
 	return staged_read(e, lidx.data(), n, QCHUNK, sizeof(Row), what, [&](const unsigned long long *d_l, uint32_t, uint32_t m) {
-		return launch_logical(e, reinterpret_cast<const int32_t *>(d_l), m, out);
+		return launch_logical(e, reinterpret_cast<const int32_t *>(d_l), m, out, which);
 	}, [&](const uint8_t *h_rows, uint32_t off, uint32_t m) {
 		rows(h_rows, off, m);
 		for (uint32_t i = 0; i < m; ++i) row_id(out[off + i]) = ids[off + i];
@@ -690,9 +792,10 @@ int logical_query_rows(gysk_engine *e, const uint64_t *ids, uint32_t n, Row *out
 }
 
 // gysk_query_logical_all / gysk_query_logical_states_all / gysk_query_cluster_states_all: every row of the index space in ascending id
-// (the uploaded permutation, compacted on the device by logical_select_kernel under ACTIVE_ONLY), in WIN_ROWS pieces; *n = rows that match
+// (the uploaded permutation, compacted on the device by logical_select_kernel under ACTIVE_ONLY), in pieces of up to WIN_ROWS rows the
+// stage holds; *n = rows that match (which: the summary of the top-client rows)
 template <typename Row>
-int logical_all_rows(gysk_engine *e, uint32_t flags, Row *out, uint32_t cap, uint32_t *n, const char *what)
+int logical_all_rows(gysk_engine *e, uint32_t flags, Row *out, uint32_t cap, uint32_t *n, const char *what, int which = 0)
 {
 	CHECK_ENGINE(e);
 	if (!n || (!out && cap) || (flags & ~GYSK_WINDOW_ACTIVE_ONLY)) return GYSK_ERR_INVAL;
@@ -714,8 +817,8 @@ int logical_all_rows(gysk_engine *e, uint32_t flags, Row *out, uint32_t cap, uin
 		total = (uint32_t)cnt;
 		sel = sp.sel;
 	}
-	int rc = staged_read<uint64_t>(e, nullptr, std::min(cap, total), WIN_ROWS, sizeof(Row), what,
-			[&](const unsigned long long *, uint32_t off, uint32_t m) { return launch_logical(e, sel + off, m, out); }, logical_finish(e, out));
+	int rc = staged_read<uint64_t>(e, nullptr, std::min(cap, total), (uint32_t)std::min<size_t>(WIN_ROWS, STAGE_BYTES / sizeof(Row)), sizeof(Row), what,
+			[&](const unsigned long long *, uint32_t off, uint32_t m) { return launch_logical(e, sel + off, m, out, which); }, logical_finish(e, out));
 	if (rc) return rc;
 	*n = total;
 	return GYSK_OK;
@@ -926,7 +1029,7 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// (re)allocate the arena
 	dfree(e, mg.members.offs); dfree(e, mg.members.slots); dfree(e, mg.d_member_ids); dfree(e, mg.arena); dfree(e, mg.lg.slab); dfree(e, mg.lg.final_slab);
 	dfree(e, mg.d_logical_ids); dfree(e, mg.d_sorted); dfree(e, mg.d_sel); dfree(e, mg.topn_slots); dfree(e, mg.topn_final); dfree(e, mg.lg.trace_final);
-	dfree(e, mg.topk_final); dfree(e, mg.topk_buf); dfree(e, mg.topk_n); dfree(e, mg.topk_tiles); dfree(e, mg.topk5_final);
+	dfree(e, mg.topk_final); dfree(e, mg.topk_buf); dfree(e, mg.topk_n); dfree(e, mg.topk_tiles); dfree(e, mg.topk5_final); dfree(e, mg.topc_final);
 	{
 		std::vector<uint64_t> ids_keep(std::move(mg.logical_ids));
 		std::unordered_map<uint64_t, uint32_t> idx_keep(std::move(mg.index));
@@ -948,15 +1051,17 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 	// GYSK_FLAG_FLOW_TOPK: the rank's last-window heaviest-flow sets after everything else; GYSK_FLAG_FLOW_TOPK_5MIN: its level sets
 	// and their bounds after those; GYSK_FLAG_FLOW_TOPK_SLOW: its last-window slow set, and with the slow level set L (and B_L) after
 	// those; GYSK_FLAG_FLOW_ERRORS: its last-window server-error set, and with its level L (and B_L), after the slow sets. The merged slow
-	// sets are set [2] of topk_final / topk5_final, the merged server-error sets set [3].
-	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK, topk5 = e->cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN;
+	// sets are set [2] of topk_final / topk5_final, the merged server-error sets set [3]. GYSK_FLAG_SVC_TOP_CLIENTS: each logical service's
+	// two summaries after everything else.
+	const bool topk = e->cfg.flags & GYSK_FLAG_FLOW_TOPK, topk5 = e->cfg.flags & GYSK_FLAG_FLOW_TOPK_5MIN, topc = e->cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS;
 	const uint32_t nslow = e->topk.open[2] ? (e->topk5.level[2] ? 2 : 1) : 0, nerr = e->topk.open[3] ? (e->topk5.level[3] ? 2 : 1) : 0;
 	mg.trace_off = nl + (topn ? TOPN_SLAB_ENTRIES : 0);
 	mg.topk_off = mg.trace_off + (traces ? trace_slab_entries(nl) : 0);
 	mg.topk5_off = mg.topk_off + (topk ? TOPK_SLAB_ENTRIES : 0);
 	mg.topks_off = mg.topk5_off + (topk5 ? TOPK_SLAB_ENTRIES : 0);
 	mg.topke_off = mg.topks_off + (nslow ? topk_slab_entries(nslow) : 0);
-	mg.slab_entries = mg.topke_off + (nerr ? topk_slab_entries(nerr) : 0);
+	mg.topc_off = mg.topke_off + (nerr ? topk_slab_entries(nerr) : 0);
+	mg.slab_entries = mg.topc_off + (topc ? topc_slab_entries(nl) : 0);
 	if ((rc = dalloc(e, &lg.slab, mg.slab_entries ? mg.slab_entries : 1))) return rc;
 	if (topk) {
 		if ((rc = dalloc(e, &mg.topk_final, (nerr ? 4 : nslow ? 3 : 2) * (size_t)TOPK_SET_WORDS))) return rc;
@@ -972,6 +1077,7 @@ int set_logical_map(gysk_engine *e, const uint64_t *glob_ids, const uint64_t *lo
 		if ((rc = dalloc(e, &lg.trace_final, nl ? nl : 1))) return rc;
 	}
 	if ((rc = dalloc(e, &lg.final_slab, nl ? nl : 1))) return rc;
+	if (topc && (rc = dalloc(e, &mg.topc_final, nl ? 2 * (size_t)nl : 1))) return rc;
 	if ((rc = dalloc(e, &mg.members.offs, (size_t)nl + 1))) return rc;
 	if ((rc = dalloc(e, &mg.members.slots, (size_t)n + 1))) return rc;
 	mg.members.null_slot = e->cfg.max_svcs;
@@ -1087,6 +1193,11 @@ int gysk_merge_prepare(gysk_engine *e)
 			fold_traces_kernel<<<div_up((uint64_t)nl * LT_WORDS, 256), 256, 0, e->stream>>>(e->st, mg.members, mg.lg);
 			e->kernel_launches++;
 		}
+		if (mg.topc_final) {		// GYSK_FLAG_SVC_TOP_CLIENTS
+			fold_topc_kernel<<<std::min<uint32_t>(div_up(nl, TC_WARPS), 132 * 8), TC_WARPS * 32, 0, e->stream>>>(e->tc, mg.members, nl,
+					reinterpret_cast<TopcSet *>(mg.lg.slab + mg.topc_off));
+			e->kernel_launches++;
+		}
 	}
 	if (mg.lg.flush) {		// GYSK_FLAG_MERGE_LEVELS, a count-min level or GYSK_FLAG_MERGE_TRACES: also with no logical service, for the flush tsec pair
 		LogicalArrays lg = mg.lg;
@@ -1188,6 +1299,11 @@ int gysk_merge_finish(gysk_engine *e, const void *d_gathered, uint32_t world)
 	if (mg.lg.nl) {
 		finish_td_kernel<<<std::min<uint32_t>(div_up(mg.lg.nl, MG_WARPS), 132 * 8), MG_WARPS * 32, 0, e->stream>>>(src, world, mg.slab_entries, mg.lg,
 				e->st.td, mg.trace_off, e->st.trace.td);
+		e->kernel_launches++;
+	}
+	if (mg.topc_final && mg.lg.nl) {		// GYSK_FLAG_SVC_TOP_CLIENTS
+		finish_topc_kernel<<<std::min<uint32_t>(div_up(mg.lg.nl, TC_WARPS), 132 * 8), TC_WARPS * 32, 0, e->stream>>>(src, world, mg.slab_entries,
+				mg.topc_off, mg.lg.nl, mg.topc_final);
 		e->kernel_launches++;
 	}
 	if (mg.topn_final) {		// GYSK_FLAG_MERGE_TOPN
@@ -1422,6 +1538,24 @@ int gysk_export_logical_hll(gysk_engine *e, uint64_t logical_id, uint8_t *regs)
 int gysk_query_logical_clients(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, gysk_svc_clients *out)
 {
 	return logical_query_rows(e, logical_ids, n, out, "query_logical_clients");
+}
+
+// GYSK_FLAG_SVC_TOP_CLIENTS: summary `which` (GYSK_TOPC_LAST or GYSK_TOPC_5MIN) of n logical ids from the last finished merge, and of every
+// logical service in the order of gysk_query_logical_all
+int gysk_query_logical_top_clients(gysk_engine *e, const uint64_t *logical_ids, uint32_t n, int which, gysk_svc_top_clients *out)
+{
+	CHECK_ENGINE(e);
+	if (!(e->cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS)) return GYSK_ERR_NOTSUP;
+	if (which != GYSK_TOPC_LAST && which != GYSK_TOPC_5MIN) return GYSK_ERR_INVAL;
+	return logical_query_rows(e, logical_ids, n, out, "query_logical_top_clients", which);
+}
+
+int gysk_query_logical_top_clients_all(gysk_engine *e, uint32_t flags, int which, gysk_svc_top_clients *out, uint32_t cap, uint32_t *n)
+{
+	CHECK_ENGINE(e);
+	if (!(e->cfg.flags & GYSK_FLAG_SVC_TOP_CLIENTS)) return GYSK_ERR_NOTSUP;
+	if (which != GYSK_TOPC_LAST && which != GYSK_TOPC_5MIN) return GYSK_ERR_INVAL;
+	return logical_all_rows(e, flags, out, cap, n, "query_logical_top_clients_all", which);
 }
 
 int gysk_export_logical_hll_window(gysk_engine *e, uint64_t logical_id, int which, uint8_t *regs)

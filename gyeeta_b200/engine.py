@@ -378,6 +378,8 @@ def load_library(path=None):
         "gysk_query_svc_clients": (i32, [vp, vp, u32, vp]),
         "gysk_query_svc_top_clients": (i32, [vp, vp, u32, i32, vp]),
         "gysk_query_top_clients_window": (i32, [vp, C.c_int32, u32, i32, vp, vp, u32, vp]),
+        "gysk_query_logical_top_clients": (i32, [vp, vp, u32, i32, vp]),
+        "gysk_query_logical_top_clients_all": (i32, [vp, u32, i32, vp, u32, vp]),
         "gysk_query_clients_window": (i32, [vp, C.c_int32, u32, vp, vp, u32, vp]),
         "gysk_export_hll_window": (i32, [vp, u64, i32, vp]),
         "gysk_query_logical_clients": (i32, [vp, vp, u32, vp]),
@@ -1108,6 +1110,26 @@ class Engine:
         out = (SvcClients * max(len(ids), 1))()
         self._chk(self.L.gysk_query_logical_clients(self.h, _p(ids), len(ids), out))
         return out[: len(ids)]
+
+    def query_logical_top_clients(self, ids, which=TOPC_LAST):
+        """gysk_query_logical_top_clients: SVC_TOP_CLIENTS_DTYPE rows of logical ids from the last merge, summary TOPC_LAST or TOPC_5MIN
+        (svc_top_clients=True)"""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = np.zeros(max(len(ids), 1), dtype=SVC_TOP_CLIENTS_DTYPE)
+        self._chk(self.L.gysk_query_logical_top_clients(self.h, _p(ids), len(ids), which, _p(out)))
+        return out[: len(ids)]
+
+    def query_logical_top_clients_all(self, which=TOPC_LAST, active_only=False, cap=None):
+        """gysk_query_logical_top_clients_all: (SVC_TOP_CLIENTS_DTYPE rows in the order of query_logical_all, number of matching rows).
+        cap None = all rows (a count call first); 0 = the count only"""
+        flags = WINDOW_ACTIVE_ONLY if active_only else 0
+        n = C.c_uint32()
+        if cap is None:
+            self._chk(self.L.gysk_query_logical_top_clients_all(self.h, flags, which, None, 0, C.byref(n)))
+            cap = n.value
+        out = np.zeros(max(cap, 1), dtype=SVC_TOP_CLIENTS_DTYPE)
+        self._chk(self.L.gysk_query_logical_top_clients_all(self.h, flags, which, _p(out) if cap else None, cap, C.byref(n)))
+        return out[: min(cap, n.value)], n.value
 
     def export_logical_hll_window(self, logical_id, which=CLIENTS_LAST):
         """gysk_export_logical_hll_window: the merged 256 client registers of one logical service, None outside the map"""
