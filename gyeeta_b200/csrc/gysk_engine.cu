@@ -71,11 +71,14 @@ int process_device_batch(gysk_engine *e, const gysk_event *d_ev, uint64_t n, cud
 		CU(e, cudaEventRecord(pe[0], e->stream));
 	}
 	RecRegions rr;
-	const int li = launch_ingest(e->st, e->tmp, e->fq, e->topk.tk, e->cl, e->fe.cur != nullptr, d_ev, n, key_slots(e), rr, e->stream);
-	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no sort plan, or record regions beyond the record queue");
+	const FlowPass fp {e->fq, e->fr, e->topk.tk, e->topk.b_slow, e->cl, e->fe};
+	const int li = launch_ingest(e->st, e->tmp, fp, d_ev, n, key_slots(e), rr, e->stream);
+	if (li < 0) return fail(e, GYSK_ERR_INVAL, "ingest launch: no kernel for the flags, no sort plan, or record regions beyond the record queue");
 	e->kernel_launches += li;
 	if (consumed) CU(e, cudaEventRecord(consumed, e->stream));
-	e->kernel_launches += launch_drains(e->st, e->tmp, e->fq, e->fr, e->topk.tk, e->topk.b_slow, e->cl, e->fe, rr, n, e->stream);
+	const int ld = launch_drains(e->st, e->tmp, fp, rr, n, e->stream);
+	if (ld < 0) return fail(e, GYSK_ERR_INVAL, "drain launch: no kernel for the flags");
+	e->kernel_launches += ld;
 	if (pe) CU(e, cudaEventRecord(pe[1], e->stream));
 	// No number travels back to the host inside a batch: the list of touched services and its length stay in device memory.
 	e->kernel_launches += launch_batch_merge(e->st, e->tmp, n, key_slots(e), e->stream);

@@ -28,8 +28,10 @@
 #include <climits>
 #include <cmath>
 #include <algorithm>
+#include <array>
 #include <type_traits>
 #include <cstring>
+#include <utility>
 
 namespace gysk {
 
@@ -2518,10 +2520,45 @@ static int plain_sort_plan(int lo, int hi, SortPlan &P)
 	return 0;
 }
 
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, bool err,
-		const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s)
+// ingest_kernel and drain_kernel each keep their instances in one table indexed by the instance's feature bits, filled from an index
+// sequence. Each kernel's flag rules are stated once (ingest_reached, drain_reached): only the instances they reach are compiled, the
+// other entries launch nothing, and the launcher refuses a flag set outside the rules.
+
+// ingest_kernel's feature bits: TRACE (the engine has trace rows), then the FlowPass flags. ERR comes only with QRY: 24 instances.
+enum IngestBit { ING_TRACE = 1, ING_QRY = 2, ING_TOPK = 4, ING_ERR = 8, ING_CL = 16, ING_INSTANCES = 32 };
+static constexpr bool ingest_reached(int f) { return !(f & ING_ERR) || (f & ING_QRY); }
+
+// An instance's shared-memory attribute is set at its first launch on a device, so that an engine without a flag never loads that
+// flag's instances: setting the attribute loads the kernel, which can wait for the work already on the device.
+template <int F>
+static void launch_ingest_pass(const DevState &st, const SortTemp &tmp, const FlowPass &fp, const gysk_event *d_ev, uint64_t n, const SortPlan &plan,
+		uint32_t grid, int dev, cudaStream_t s)
+{
+	if constexpr (ingest_reached(F)) {
+		constexpr bool TRACE = F & ING_TRACE, QRY = F & ING_QRY, TOPK = F & ING_TOPK, ERR = F & ING_ERR, CL = F & ING_CL;
+		static bool attr_set[MAX_DEVICES] = {};
+		const auto launch = [&](auto kernel, auto... cl_open) {
+			if (!attr_set[dev]) {
+				cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
+				attr_set[dev] = true;
+			}
+			kernel<<<grid, IngestShape::WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
+					fp.tk.list[0], cl_open...);
+		};
+		if constexpr (CL) launch(ingest_kernel<TRACE, QRY, TOPK, ERR, uint8_t *>, fp.cl.open);
+		else launch(ingest_kernel<TRACE, QRY, TOPK, ERR>);
+	}
+}
+template <int... F>
+static constexpr auto ingest_passes(std::integer_sequence<int, F...>) { return std::array {launch_ingest_pass<F>...}; }
+
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowPass &fp, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
+		RecRegions &rr, cudaStream_t s)
 {
 	if (!n) return 0;
+	const int f = (st.trace.rows ? ING_TRACE : 0) | (fp.fq.cur ? ING_QRY : 0) | (fp.tk.list[0].keys ? ING_TOPK : 0) | (fp.fe.cur ? ING_ERR : 0) |
+			(fp.cl.open ? ING_CL : 0);
+	if (!ingest_reached(f)) return -1;
 	const int dev = current_device();
 	SortPlan plan {};
 	if (key_sort_plan(key_slots, plan) < 0) return -1;
@@ -2531,51 +2568,6 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	cudaMemsetAsync(st.counters + CTR_NKEYS, 0, sizeof(unsigned long long), s);
 	cudaMemsetAsync(tmp.os_ghist, 0, OS_GHIST_WORDS * sizeof(uint32_t), s);
 	constexpr int WARPS = IngestShape::WARPS, CHUNK = IngestShape::CHUNK;
-	static bool attr_set[MAX_DEVICES] = {};
-	using IngestFn = void (*)(DevState, const gysk_event *, uint64_t, unsigned long long *, uint32_t *, SortPlan, uint4 *, uint2 *, TopkList);
-	using IngestClFn = void (*)(DevState, const gysk_event *, uint64_t, unsigned long long *, uint32_t *, SortPlan, uint4 *, uint2 *, TopkList, uint8_t *);
-	// [TRACE][QRY][TOPK]; fns_cl: the instances of GYSK_FLAG_CLIENT_LEVELS
-	static const IngestFn fns[2][2][2] = {
-		{{ingest_kernel<false, false, false, false>, ingest_kernel<false, false, true, false>},
-		 {ingest_kernel<false, true, false, false>, ingest_kernel<false, true, true, false>}},
-		{{ingest_kernel<true, false, false, false>, ingest_kernel<true, false, true, false>},
-		 {ingest_kernel<true, true, false, false>, ingest_kernel<true, true, true, false>}}};
-	static const IngestClFn fns_cl[2][2][2] = {
-		{{ingest_kernel<false, false, false, false, uint8_t *>, ingest_kernel<false, false, true, false, uint8_t *>},
-		 {ingest_kernel<false, true, false, false, uint8_t *>, ingest_kernel<false, true, true, false, uint8_t *>}},
-		{{ingest_kernel<true, false, false, false, uint8_t *>, ingest_kernel<true, false, true, false, uint8_t *>},
-		 {ingest_kernel<true, true, false, false, uint8_t *>, ingest_kernel<true, true, true, false, uint8_t *>}}};
-	// GYSK_FLAG_FLOW_ERRORS (QRY only): [TRACE][TOPK], and with GYSK_FLAG_CLIENT_LEVELS
-	static const IngestFn fns_err[2][2] = {{ingest_kernel<false, true, false, true>, ingest_kernel<false, true, true, true>},
-					       {ingest_kernel<true, true, false, true>, ingest_kernel<true, true, true, true>}};
-	static const IngestClFn fns_err_cl[2][2] = {{ingest_kernel<false, true, false, true, uint8_t *>, ingest_kernel<false, true, true, true, uint8_t *>},
-						    {ingest_kernel<true, true, false, true, uint8_t *>, ingest_kernel<true, true, true, true, uint8_t *>}};
-	// the instances of GYSK_FLAG_FLOW_TOPK, GYSK_FLAG_CLIENT_LEVELS and GYSK_FLAG_FLOW_ERRORS only once an engine with the flag launches:
-	// setting a kernel's attribute loads it, which can wait for the work already on the device
-	static bool topk_attr_set[MAX_DEVICES] = {}, cl_attr_set[MAX_DEVICES] = {}, err_attr_set[MAX_DEVICES] = {};
-	const int topk = tk.list[0].keys ? 1 : 0;
-	if (!attr_set[dev]) {
-		for (const IngestFn f : {fns[0][0][0], fns[1][0][0], fns[0][1][0], fns[1][1][0]})
-			cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		attr_set[dev] = true;
-	}
-	if (topk && !topk_attr_set[dev]) {
-		for (const IngestFn f : {fns[0][0][1], fns[1][0][1], fns[0][1][1], fns[1][1][1]})
-			cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		topk_attr_set[dev] = true;
-	}
-	if (cl.open && !cl_attr_set[dev]) {
-		for (int i = 0; i < 8; ++i)
-			cudaFuncSetAttribute(fns_cl[i >> 2][(i >> 1) & 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		cl_attr_set[dev] = true;
-	}
-	if (err && !err_attr_set[dev]) {
-		for (int i = 0; i < 4; ++i) {
-			cudaFuncSetAttribute(fns_err[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-			cudaFuncSetAttribute(fns_err_cl[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IngestShared));
-		}
-		err_attr_set[dev] = true;
-	}
 	const uint64_t want = (n + (uint64_t)CHUNK * WARPS - 1) / ((uint64_t)CHUNK * WARPS);
 	const uint64_t full = (uint64_t)sm_count(dev) * IngestShape::MIN_CTAS;
 	const uint32_t grid = (uint32_t)(want < full ? want : full);
@@ -2585,71 +2577,52 @@ int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq
 	rr.cap = (nchunks + rr.nwarps - 1) / rr.nwarps * CHUNK;
 	if (rr.nwarps > tmp.rec_cnt_cap || (uint64_t)rr.nwarps * rr.cap > tmp.recq_cap) return -1;
 	// a counted response sample takes a connection-queue entry, as one connection event does: the regions hold one record per event
-	const int tr = st.trace.rows ? 1 : 0, qr = fq.cur ? 1 : 0;
-	if (err && cl.open) fns_err_cl[tr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq,
-			tmp.rec_cnt, tk.list[0], cl.open);
-	else if (err) fns_err[tr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
-			tk.list[0]);
-	else if (cl.open) fns_cl[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt,
-			tk.list[0], cl.open);
-	else fns[tr][qr][topk]<<<grid, WARPS * 32, sizeof(IngestShared), s>>>(st, d_ev, n, tmp.keys_a, tmp.os_ghist, plan, tmp.recq, tmp.rec_cnt, tk.list[0]);
+	static constexpr auto passes = ingest_passes(std::make_integer_sequence<int, ING_INSTANCES> {});
+	passes[f](st, tmp, fp, d_ev, n, plan, grid, dev, s);
 	return 1;
 }
 
-// one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
-// table + the region start table, whose largest size sets the occupancy
-template <bool TASK, bool QRY, bool RH, bool TOPK, bool SLOW, bool CL, bool ERR>
-static void launch_drain_pass(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		cudaStream_t s, uint8_t *cl_open, const ErrPass &ep)
+// drain_kernel's feature bits: TASK (the pass), then the FlowPass flags. RH and ERR come only with QRY, SLOW only with RH and TOPK, and
+// the TASK pass has neither SLOW nor CL: 24 TCP and 10 TASK instances.
+enum DrainBit { DR_TASK = 1, DR_QRY = 2, DR_RH = 4, DR_TOPK = 8, DR_SLOW = 16, DR_CL = 32, DR_ERR = 64, DR_INSTANCES = 128 };
+static constexpr bool drain_reached(int f)
 {
-	constexpr int WARPS = DrainShape<TASK>::WARPS;
-	constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
-	static int per_sm[MAX_DEVICES] = {};
-	if (!per_sm[dev]) {
-		const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
-		cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
-		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR>, WARPS * 32, smem_max);
-		per_sm[dev] = b > 0 ? b : 1;
-	}
-	const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
-	const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
-	const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
-	drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, ft, tmp.recq, tmp.rec_cnt, rr,
-			fq, fq_cms, fr, fr_cms, tk, b_slow, cl_open, ep);
+	if ((f & (DR_RH | DR_ERR)) && !(f & DR_QRY)) return false;
+	if ((f & DR_SLOW) && (f & (DR_RH | DR_TOPK)) != (DR_RH | DR_TOPK)) return false;
+	return !((f & DR_TASK) && (f & (DR_SLOW | DR_CL)));
 }
 
-// b_slow: GYSK_FLAG_FLOW_TOPK_SLOW's first slow bucket when tk.list[2] is held (RH only); the TASK pass is the TOPK one either way.
-// cl_open (CL, GYSK_FLAG_CLIENT_LEVELS): the TCP pass's client registers; the TASK pass does not touch them.
-// ep (ERR, GYSK_FLAG_FLOW_ERRORS): the error flow table, cells and candidates (both passes).
-template <bool QRY, bool RH, bool CL, bool ERR>
-static int launch_drain_passes_t(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		uint8_t *cl_open, const ErrPass &ep, cudaStream_t s)
+// one drain pass: as many CTAs as the SMs hold at once (at most one per 32 x WARPS events of the batch); shared memory = the hot
+// table + the region start table, whose largest size sets the occupancy. mask: the batch flow tables' entries - 1. A flag's parameters
+// go to the instances with its bit and zero to the others: b_slow (GYSK_FLAG_FLOW_TOPK_SLOW's first slow bucket) to the SLOW ones.
+template <int F>
+static void launch_drain_pass(const DevState &st, const SortTemp &tmp, const FlowPass &fp, const RecRegions &rr, uint64_t n_events, uint32_t mask,
+		int dev, cudaStream_t s)
 {
-	if (tk.list[0].keys) {
-		if constexpr (RH) {
-			if (tk.list[2].keys) launch_drain_pass<false, QRY, RH, true, true, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, s, cl_open, ep);
-			else launch_drain_pass<false, QRY, RH, true, false, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open, ep);
+	if constexpr (drain_reached(F)) {
+		constexpr bool TASK = F & DR_TASK, QRY = F & DR_QRY, RH = F & DR_RH, TOPK = F & DR_TOPK, SLOW = F & DR_SLOW, CL = F & DR_CL, ERR = F & DR_ERR;
+		constexpr int WARPS = DrainShape<TASK>::WARPS;
+		constexpr size_t HOT_BYTES = sizeof(HotTableT<DrainShape<TASK>::HOT_BITS>);
+		static int per_sm[MAX_DEVICES] = {};
+		if (!per_sm[dev]) {
+			const size_t smem_max = HOT_BYTES + ((size_t)tmp.rec_cnt_cap + 1) * sizeof(uint32_t);
+			cudaFuncSetAttribute(drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+			int b = 0;
+			cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR>, WARPS * 32, smem_max);
+			per_sm[dev] = b > 0 ? b : 1;
 		}
-		else launch_drain_pass<false, QRY, RH, true, false, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open, ep);
-		launch_drain_pass<true, QRY, RH, true, false, false, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, nullptr, ep);
+		const uint64_t want = (n_events + WARPS * 32 - 1) / (WARPS * 32);
+		const uint64_t full = (uint64_t)sm_count(dev) * per_sm[dev];
+		const size_t smem = HOT_BYTES + ((size_t)rr.nwarps + 1) * sizeof(uint32_t);
+		const FlowTable none {nullptr, 0u};
+		drain_kernel<TASK, QRY, RH, TOPK, SLOW, CL, ERR><<<(uint32_t)(want < full ? want : full), WARPS * 32, smem, s>>>(st, FlowTable {tmp.flow, mask},
+				tmp.recq, tmp.rec_cnt, rr, QRY ? FlowTable {fp.fq.flow, mask} : none, QRY ? fp.fq.cur : nullptr, RH ? FlowTable {fp.fr.flow, mask} : none,
+				RH ? fp.fr.cur : nullptr, fp.tk, SLOW ? fp.b_slow : 0u, CL ? fp.cl.open : nullptr,
+				ERR ? ErrPass {FlowTable {fp.fe.flow, mask}, fp.fe.cur, fp.fe.list} : ErrPass {});
 	}
-	else {
-		launch_drain_pass<false, QRY, RH, false, false, CL, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, cl_open, ep);
-		launch_drain_pass<true, QRY, RH, false, false, false, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, 0, s, nullptr, ep);
-	}
-	return 2;
 }
-template <bool QRY, bool RH, bool ERR = false>
-static int launch_drain_passes(const DevState &st, const FlowTable &ft, const SortTemp &tmp, const RecRegions &rr, uint64_t n_events, int dev,
-		const FlowTable &fq, unsigned long long *fq_cms, const FlowTable &fr, unsigned long long *fr_cms, const FlowTopk &tk, uint32_t b_slow,
-		uint8_t *cl_open, cudaStream_t s, const ErrPass &ep = ErrPass {})
-{
-	if (cl_open) return launch_drain_passes_t<QRY, RH, true, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, cl_open, ep, s);
-	return launch_drain_passes_t<QRY, RH, false, ERR>(st, ft, tmp, rr, n_events, dev, fq, fq_cms, fr, fr_cms, tk, b_slow, nullptr, ep, s);
-}
+template <int... F>
+static constexpr auto drain_passes(std::integer_sequence<int, F...>) { return std::array {launch_drain_pass<F>...}; }
 
 // the batch's queued connection records -> flow table, HLL, exact cells; then the flow table -> count-min and its process records ->
 // process histograms. The TASK pass always runs: it leaves the flow table empty. The table takes the smallest power of two >= 2 x the
@@ -2658,30 +2631,23 @@ static int launch_drain_passes(const DevState &st, const FlowTable &ft, const So
 // with GYSK_FLAG_FLOW_RESP_HIST (fr.cur) through a response flow table of that size too. With GYSK_FLAG_FLOW_ERRORS (fe.cur) the error
 // samples go through an error flow table of that size as well: a batch whose samples all carry an error bit needs every entry the query
 // table needs (DESIGN.md section 7).
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
-		const ClientLevels &cl, const FlowErrors &fe, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowPass &fp, const RecRegions &rr, uint64_t n_events, cudaStream_t s)
 {
 	if (!n_events) return 0;
+	const int tcp = (fp.fq.cur ? DR_QRY : 0) | (fp.fr.cur ? DR_RH : 0) | (fp.tk.list[0].keys ? DR_TOPK : 0) | (fp.tk.list[2].keys ? DR_SLOW : 0) |
+			(fp.cl.open ? DR_CL : 0) | (fp.fe.cur ? DR_ERR : 0);
+	if (!drain_reached(tcp)) return -1;
 	const int dev = current_device();
 	uint32_t n = 16;
 	while (n < tmp.flow_cap && n < 2 * n_events) n <<= 1;
-	const FlowTable ft {tmp.flow, n - 1u};
 	cudaMemsetAsync(st.counters + CTR_FLOW_DIRECT, 0, sizeof(unsigned long long), s);
-	const FlowTable none {nullptr, 0u};
-	if (!fq.cur) return launch_drain_passes<false, false>(st, ft, tmp, rr, n_events, dev, none, nullptr, none, nullptr, tk, 0, cl.open, s);
-	cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
-	const FlowTable fqt {fq.flow, n - 1u};
-	if (fe.cur) {
-		cudaMemsetAsync(st.counters + CTR_FLOWE_DIRECT, 0, sizeof(unsigned long long), s);
-		const ErrPass ep {FlowTable {fe.flow, n - 1u}, fe.cur, fe.list};
-		if (fr.cur) cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
-		if (!fr.cur) return launch_drain_passes<true, false, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, cl.open, s, ep);
-		return launch_drain_passes<true, true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, cl.open,
-				s, ep);
-	}
-	if (!fr.cur) return launch_drain_passes<true, false>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, none, nullptr, tk, 0, cl.open, s);
-	cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
-	return launch_drain_passes<true, true>(st, ft, tmp, rr, n_events, dev, fqt, fq.cur, FlowTable {fr.flow, n - 1u}, fr.cur, tk, b_slow, cl.open, s);
+	if (fp.fq.cur) cudaMemsetAsync(st.counters + CTR_FLOWQ_DIRECT, 0, sizeof(unsigned long long), s);
+	if (fp.fe.cur) cudaMemsetAsync(st.counters + CTR_FLOWE_DIRECT, 0, sizeof(unsigned long long), s);
+	if (fp.fr.cur) cudaMemsetAsync(st.counters + CTR_FLOWR_DIRECT, 0, sizeof(unsigned long long), s);
+	static constexpr auto passes = drain_passes(std::make_integer_sequence<int, DR_INSTANCES> {});
+	passes[tcp](st, tmp, fp, rr, n_events, n - 1u, dev, s);
+	passes[DR_TASK | (tcp & ~(DR_SLOW | DR_CL))](st, tmp, fp, rr, n_events, n - 1u, dev, s);
+	return 2;
 }
 
 static void os_set_attrs(int dev)

@@ -301,27 +301,30 @@ static constexpr int TD_MERGE_CTAS_PER_SM = 5, TD_MERGE_MAX_SMS = 192;	// bins_m
 // of bins_merge_kernel (DESIGN.md §4). Batch rows: min(max_svcs, ceil(max_batch / LONG_SEG)).
 static constexpr int LONG_SEG = 8192;
 
+// The opt-in flow state a batch's ingest and drain passes read, every pointer nullptr where its flag is off. Each flag's bit of the
+// ingest_kernel and drain_kernel instance follows from it:
+// fq.cur (GYSK_FLAG_FLOW_QUERIES, QRY): the response samples are queued for the flow query table too
+// fr.cur (GYSK_FLAG_FLOW_RESP_HIST, RH, only with fq.cur): the response samples also go to the flow response histograms
+// tk.list[0].keys (GYSK_FLAG_FLOW_TOPK, TOPK): the flow keys of the ACTIVE records join the connection table's candidates, and the
+// drain passes gather each held table's candidates
+// tk.list[2].keys (GYSK_FLAG_FLOW_TOPK_SLOW, SLOW, with fr.cur and tk.list[0].keys): the TCP pass gathers the flow key of each response
+// sample in bucket b_slow or above
+// cl.open (GYSK_FLAG_CLIENT_LEVELS, CL): the ACTIVE records and each connection record raise the open window's client registers too
+// fe.cur (GYSK_FLAG_FLOW_ERRORS, ERR, only with fq.cur): the queued response samples carry their error bits (QRY_CLI_ERR, QRY_SER_ERR),
+// the error samples go to the flow error tables, and with fe.list.keys their server-error flow keys to its candidates
+struct FlowPass { FlowQueries fq; FlowRespHist fr; FlowTopk tk; uint32_t b_slow; ClientLevels cl; FlowErrors fe; };
+
 // every launcher returns the number of kernel launches it issued
 // service slots [s_lo, s_hi) and process slots [t_lo, t_hi) in their just-created state (the arrays zeroed before)
 int launch_init_slots(const DevState &st, uint32_t s_lo, uint32_t s_hi, uint32_t t_lo, uint32_t t_hi, cudaStream_t s);
 int launch_register(const DevState &st, const unsigned long long *d_ids, uint32_t n, int is_task, cudaStream_t s);
-// -1: no sort plan for max_svcs, or the launch's record regions do not fit the buffers
+// -1: no ingest_kernel instance for fp's flags, no sort plan for max_svcs, or the launch's record regions do not fit the buffers
 // key_slots: the values the slot field of a sort key takes (max_svcs, or max_svcs + 1 + trace rows with trace rows)
-// fq.cur != nullptr: the response samples are queued for the flow query table too (GYSK_FLAG_FLOW_QUERIES)
-// tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the flow keys of the ACTIVE records join the connection table's candidates
-// cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): the ACTIVE records raise the open window's client registers too
-// err (GYSK_FLAG_FLOW_ERRORS, only with fq.cur): the queued response samples carry their error bits (QRY_CLI_ERR, QRY_SER_ERR)
-int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowTopk &tk, const ClientLevels &cl, bool err,
-		const gysk_event *d_ev, uint64_t n, uint32_t key_slots, RecRegions &rr, cudaStream_t s);
+int launch_ingest(const DevState &st, const SortTemp &tmp, const FlowPass &fp, const gysk_event *d_ev, uint64_t n, uint32_t key_slots,
+		RecRegions &rr, cudaStream_t s);
 int launch_batch_merge(const DevState &st, const SortTemp &tmp, uint64_t n_events, uint32_t key_slots, cudaStream_t s);
-// fr.cur != nullptr (GYSK_FLAG_FLOW_RESP_HIST, only with fq.cur): the response samples also go to the flow response histograms;
-// tk.list[0].keys != nullptr (GYSK_FLAG_FLOW_TOPK): the passes gather each held table's candidates; tk.list[2].keys != nullptr
-// (GYSK_FLAG_FLOW_TOPK_SLOW, with fr.cur): the TCP pass gathers the flow key of each response sample in bucket b_slow or above;
-// cl.open != nullptr (GYSK_FLAG_CLIENT_LEVELS): each connection record raises the open window's client register beside the all-time one;
-// fe.cur != nullptr (GYSK_FLAG_FLOW_ERRORS, only with fq.cur): the error samples go to the flow error tables, and with fe.list.keys their
-// server-error flow keys to its candidates
-int launch_drains(const DevState &st, const SortTemp &tmp, const FlowQueries &fq, const FlowRespHist &fr, const FlowTopk &tk, uint32_t b_slow,
-		const ClientLevels &cl, const FlowErrors &fe, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
+// the TCP and then the TASK drain pass over the records launch_ingest queued. -1: no drain_kernel instance for fp's flags
+int launch_drains(const DevState &st, const SortTemp &tmp, const FlowPass &fp, const RecRegions &rr, uint64_t n_events, cudaStream_t s);
 // GYSK_FLAG_FLOW_TOPK, after the batch merge (it takes tmp's sort buffers, of at least n_max keys): the *l.n candidates (n_max >= *l.n)
 // sorted by key in l.keys, the distinct ones scored on table tbl (score as TOPK_SCORE_SLOW says) and the K best by (score descending,
 // key ascending) written to set; then, unless reseed is false, set back into l as the next batch's first candidates. -1: no sort plan

@@ -1,7 +1,8 @@
 """The flag matrix is complete, on the CPU: the flag sets gysk_create accepts are the ones tests/all_flags.py's rule allows (the
 configuration check comes before any device is looked for), the GPU matrix of tests/test_gpu_flag_matrix.py reaches every TCP drain_kernel
-tuple and every ingest_kernel instance with trace rows on and off, and the instances it covers are the ones the dispatch tables of
-gysk_kernels.cu can launch. A new flag that adds kernel instances fails here until the matrix covers them."""
+tuple and every ingest_kernel instance with trace rows on and off, and the instances it covers are the ones the built library holds. Each
+kernel's dispatch table in gysk_kernels.cu compiles only the instances its flag rules reach, so the library's kernels are the launchable
+ones. A new flag that adds kernel instances fails here until the matrix covers them."""
 import inspect
 import os
 import re
@@ -14,75 +15,40 @@ from tests import all_flags as af
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INVAL, NODEV = -22, -19
 TINY = dict(max_svcs=16, max_tasks=16, cms_depth=1, cms_log2_width=4, hll_p=4, max_batch=1024)
+LIB = os.path.join(ROOT, "gyeeta_b200", "libgysketch.so")
 
 
 def _lib():
-    if not os.path.exists(os.path.join(ROOT, "gyeeta_b200", "libgysketch.so")):
+    if not os.path.exists(LIB):
         pytest.skip("library not built")
     return ge.load_library()
 
 
-def _src():
-    with open(os.path.join(ROOT, "gyeeta_b200", "csrc", "gysk_kernels.cu")) as f:
-        return f.read()
+def _kernels(pattern):
+    """the template arguments of every kernel instance the library holds whose mangled name matches pattern: the names its kernel
+    registration carries"""
+    _lib()
+    with open(LIB, "rb") as f:
+        return set(re.findall(pattern, f.read()))
 
 
-def _span(src, head):
-    """(start, end) of the brace block that follows the first match of head"""
-    m = re.search(head, src)
-    assert m, head
-    i = src.index("{", m.end())
-    depth = 0
-    for j in range(i, len(src)):
-        depth += {"{": 1, "}": -1}.get(src[j], 0)
-        if depth == 0:
-            return i + 1, j
-    raise AssertionError(head)
-
-
-def _body(src, head):
-    a, b = _span(src, head)
-    return src[a: b]
-
-
-def _bools(args):
-    return tuple(a.strip() == "true" for a in args.split(","))
+def _bools(mangled):
+    return tuple(b == b"1" for b in re.findall(rb"Lb([01])E", mangled))
 
 
 def ingest_instances():
-    """(TRACE, QRY, TOPK, ERR, CL) of every ingest_kernel instance launch_ingest's tables hold"""
-    body = _body(_src(), r"\bint launch_ingest\(")
-    out = set()
-    for args, cl_ in re.findall(r"ingest_kernel<((?:\s*(?:true|false)\s*,){3}\s*(?:true|false))\s*(,\s*uint8_t \*)?>", body):
-        out.add(_bools(args) + (bool(cl_),))
-    return out
+    """(TRACE, QRY, TOPK, ERR, CL) of every ingest_kernel instance in the library (CL: the one-pointer ClOpen pack)"""
+    return {_bools(args) + (bool(cl_),) for args, cl_ in _kernels(rb"_ZN4gysk13ingest_kernelI((?:Lb[01]E){4})J(Ph)?EEEv")}
+
+
+def drain_instances():
+    """(TASK, QRY, RH, TOPK, SLOW, CL, ERR) of every drain_kernel instance in the library"""
+    return {_bools(args) for args in _kernels(rb"_ZN4gysk12drain_kernelI((?:Lb[01]E){7})EEv")}
 
 
 def drain_tuples():
-    """(QRY, RH, TOPK, SLOW, CL, ERR) of every TCP drain_kernel pass launch_drains can reach, the dispatch evaluated from the sources:
-    each launch_drain_passes call of launch_drains (its QRY, RH and ERR), both values of CL (launch_drain_passes picks by cl_open), and
-    each TCP launch_drain_pass call of launch_drain_passes_t, those inside `if constexpr (RH)` only where RH holds"""
-    src = _src()
-    drains = _body(src, r"\bint launch_drains\(")
-    calls = [_bools(a) for a in re.findall(r"launch_drain_passes<([^>]*)>", drains)]
-    assert calls, "no launch_drain_passes call in launch_drains"
-    passes = _body(src, r"static int launch_drain_passes_t\(")
-    lo, hi = _span(passes, r"if constexpr \(RH\)")
-    tcp = [(m.group(1), lo <= m.start() < hi) for m in re.finditer(r"launch_drain_pass<false,\s*([^>]*)>", passes)]
-    assert any(r for _, r in tcp) and not all(r for _, r in tcp)
-    out = set()
-    for call in calls:
-        qry, rh = call[0], call[1]
-        err = call[2] if len(call) > 2 else False
-        for cl_ in (False, True):
-            env = {"QRY": qry, "RH": rh, "CL": cl_, "ERR": err, "true": True, "false": False}
-            for args, rh_only in tcp:
-                if rh_only and not rh:
-                    continue
-                vals = tuple(env[a.strip()] for a in args.split(","))
-                assert len(vals) == 6, args
-                out.add(vals)
-    return out
+    """(QRY, RH, TOPK, SLOW, CL, ERR) of every TCP drain_kernel instance in the library"""
+    return {t[1:] for t in drain_instances() if not t[0]}
 
 
 def test_accepted_flag_sets_are_the_rule():
@@ -103,7 +69,7 @@ def test_accepted_flag_sets_are_the_rule():
     assert accepted == want, [f for f in af.subsets() if (f in accepted) != (f in want)][:4]
 
 
-def test_dispatch_tables_hold_24_ingest_instances_and_24_tcp_drain_tuples():
+def test_library_holds_24_ingest_instances_and_24_tcp_and_10_task_drain_tuples():
     ing = ingest_instances()
     assert len(ing) == 24, sorted(ing)
     # every instance is one a flag set reaches: ERR only with QRY
@@ -112,9 +78,13 @@ def test_dispatch_tables_hold_24_ingest_instances_and_24_tcp_drain_tuples():
     tcp = drain_tuples()
     assert len(tcp) == 24, sorted(tcp)
     assert tcp == {af.drain_tuple(f) for f in af.subsets() if af.allowed(f)}
+    # the TASK pass runs beside each TCP pass with the same flags but SLOW and CL
+    task = {t[1:] for t in drain_instances() if t[0]}
+    assert len(task) == 10, sorted(task)
+    assert task == {(q, rh, tk, False, False, err) for q, rh, tk, _, _, err in tcp}
 
 
-def test_gpu_matrix_covers_every_instance():
+def test_gpu_matrix_covers_every_library_instance():
     cases = af.matrix()
     assert len(cases) == 48 and len({c[0] for c in cases}) == 48
     assert all(af.allowed(f) for _, f, _ in cases)
